@@ -3,7 +3,7 @@
 WebQSP-shape synthetic subgraphs, with the aggregation kernel's achieved HBM bandwidth (roofline) and the
 CPU oracle port timed beside it.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config cfg2] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config cfg2] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one batch: CSR batching of the fact list -> TypeLayer ->
@@ -14,6 +14,10 @@ pinned-host -> device copies, CSR batching, forward, ranking and the device -> h
 candidate lists, by wall clock between synchronizes.  Multi-GPU: one process per GPU, every rank runs its
 own B questions (weak scaling), no communication during the forward, one NCCL all-gather of the answer
 scores at the end of each step; time = max over ranks.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (pred_dist, loss, pred and the ranked
+candidate lists) as DIR/<name>.npy in float32 / float64.  Inputs and weights are seeded, so two builds run with the
+same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -35,9 +39,9 @@ METRIC = "questions/sec (GNN forward+score) on WebQSP-shape subgraphs; agg-kerne
 UNIT = "questions/s"
 WORKLOADS = {
     "cfg1": "single WebQSP question, ~2k-node/~6k-edge subgraph, 3-hop ReaRev fp32",
-    "cfg2": "batch=64 WebQSP-shape synthetic subgraphs (~2k nodes, 200-dim feat, 3 hops) on 1xB200",
+    "cfg2": "batch=64 WebQSP-shape synthetic subgraphs (~2k nodes, 200-dim feat, 3 hops) on 1xH100",
     "cfg3": "batch=256 CWQ-shape synthetic subgraphs (~10k nodes, ~40k edges, 4 hops)",
-    "cfg4": "batch=1024 WebQSP-shape subgraphs sharded across 8xB200 = 128 questions per GPU (weak scaling)",
+    "cfg4": "batch=1024 WebQSP-shape subgraphs sharded across 8xH100 = 128 questions per GPU (weak scaling)",
     "cfg5": "stress: 100k-node / 1M-edge synthetic subgraph, 400-dim feat, 3 hops",
     "d50": "batch=64 WebQSP-shape subgraphs at the PUBLISHED model shape (gnn/README.md:19: entity_dim 50, num_iter 3, "
            "num_ins 2, num_gnn 3)",
@@ -82,7 +86,29 @@ def parse():
                     help="0: dense-prior layers as aggregation kernel + GEMM instead of the fused layer kernel")
     ap.add_argument("--cuda-graph", type=int, default=1,
                     help="1: run the step through gnn_rag_b200.GraphedStep (CUDA-graph replay over static buffers)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32 / float64)")
     return ap.parse_args()
+
+
+DUMP_BUDGET = 64 << 20     # bytes of all dumped arrays together
+
+
+def dump_outputs(path, outs):
+    """Write {name: tensor} as float32 (floating outputs) / float64 (integer outputs: exact below 2^53) .npy files.
+    An array whose share of the budget is too small is reduced to a fixed, seeded sample of its rows (the row indices
+    go to <name>_rows.npy)."""
+    os.makedirs(path, exist_ok=True)
+    share = DUMP_BUDGET // max(len(outs), 1) // 2       # room for the row-index files too
+    for name, t in outs.items():
+        a = t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+        a = a.astype(np.float32 if a.dtype.kind == "f" else np.float64)
+        if a.nbytes > share and a.ndim >= 1:
+            keep = max(1, share // max(a.nbytes // a.shape[0], 1))
+            rows = np.sort(np.random.RandomState(0).choice(a.shape[0], keep, replace=False))
+            np.save(os.path.join(path, name + "_rows.npy"), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def model_args_for(c, use_cuda):
@@ -166,8 +192,8 @@ def init_state_dict_cpu(c):
 
 
 def run_reference(a):
-    """The reference's own CPU implementation of the path (the oracle port: /root/reference does not exist on the GPU
-    box and the reference is pure Python, so there is no oracle/_ref binary), all host threads, on this arm's config.
+    """The reference's own CPU implementation of the path (the oracle port oracle/kgqa_oracle.py: the reference is pure
+    Python, so there is no compiled reference binary), all host threads, on this arm's config.
     One step = forward + ranking of `sample` questions of the workload (the whole batch for cfg1 / cfg2 / cfg4)."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -289,26 +315,27 @@ def run_ours(a):
     dev_batch = tuple(
         (tuple(x.to(dev) if isinstance(x, torch.Tensor) else x for x in t) if isinstance(t, tuple)
          else (t.to(dev) if isinstance(t, torch.Tensor) else t)) for t in pinned)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
     eps = args["eps"]
 
     gs = G.GraphedStep(model, S.WEBQSP_NUM_ENTITY) if a.cuda_graph else None
 
     def step_eager(batch):
-        _loss, _pred, pred_dist, _ = model(batch)
+        loss, pred, pred_dist, _ = model(batch)
         cand = ops.rank_candidates(pred_dist, model.last_batch.local_entity,
                                    model.last_batch.query_entities, S.WEBQSP_NUM_ENTITY, eps)
         if world > 1:
             parallel.all_gather_scores(pred_dist, B * world)
-        return pred_dist, cand
+        return (loss, pred, pred_dist) + tuple(cand)
 
     def step(batch):
+        """-> (loss, pred, pred_dist, cand_idx, cand_count, cand_total): what a caller of the step receives"""
         if gs is None:
             return step_eager(batch)
         out = gs(batch)                     # copies the inputs into the static buffers, replays the graph
         if world > 1:
             parallel.all_gather_scores(out.pred_dist, B * world)
-        return out.pred_dist, out
+        return out.loss, out.pred, out.pred_dist, out.cand_idx, out.cand_count, out.cand_total
 
     def barrier():
         if world > 1:
@@ -367,15 +394,24 @@ def run_ours(a):
     evs = []
     barrier()
     wall0 = time.perf_counter()
+    last = None
     for _ in range(a.steps):
         flush.fill_(1)
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
-        step(dev_batch)
+        last = step(dev_batch)
         e.record()
         evs.append((s, e))
     barrier()
     wall = time.perf_counter() - wall0
+    if a.dump_outputs and rank == 0:
+        # before the e2e legs below: with --cuda-graph the outputs live in the graph's static buffers
+        loss, pred, pred_dist, cand_idx, cand_count, cand_total = last
+        ranked = cand_idx.long()
+        valid = torch.arange(ranked.shape[1], device=dev)[None, :] < cand_count.view(-1, 1).long()
+        ranked = torch.where(valid, ranked, torch.full_like(ranked, -1))     # slots past a question's count: -1
+        dump_outputs(a.dump_outputs, {"pred_dist": pred_dist, "loss": loss, "pred": pred, "cand_idx": ranked,
+                                      "cand_count": cand_count, "cand_total": cand_total})
     dev_ms = sum(s.elapsed_time(e) for s, e in evs)
     # clocks are sampled over the device-timed region only: nvidia-smi polling takes a driver lock and
     # perturbs the wall-clock e2e loop below (measured: 5.5 ms/step alone vs 8-19 ms with the sampler on)
@@ -465,8 +501,9 @@ def run_ours(a):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:  # noqa: BLE001
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "6650 GB/s (of fallback)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = ("MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks
+                else "3350 GB/s (H100 SXM data sheet, not reached)")
     per_step = len(agg) // max(agg_steps, 1)
     # layer 0 of every iteration sees the one-hot seed prior.  With the sparse-prior fast path (default) that layer
     # never reaches the aggregation kernel (K = D GEMM + frontier fix-up), so every timed launch is a dense-prior
@@ -478,14 +515,7 @@ def run_ours(a):
         dense = [ms for i, (ms, _) in enumerate(agg) if (i % per_step) % K != 0] if per_step else []
         seedl = [ms for i, (ms, _) in enumerate(agg) if (i % per_step) % K == 0] if per_step else []
     abytes = agg_algorithmic_bytes(B, N, F, D, I, R1, 2 if act_bf16 else 4)
-    traffic = None     # dram__bytes_read+write of the dense-prior launch from the committed ncu --set full capture
-    try:
-        import glob
-        tj = sorted(glob.glob(os.path.join(ROOT, "profiles", "*_traffic.json")))
-        if tj and a.config == "cfg2":
-            traffic = json.load(open(tj[-1])).get("agg_dense_traffic_bytes_per_launch")
-    except Exception:  # noqa: BLE001
-        pass
+    traffic = None     # measured DRAM bytes of the dense-prior launch: not measured
     dense_ms = float(np.mean(dense)) if dense else float("nan")
     achieved = abytes / (dense_ms * 1e-3) / 1e9
     agg_name = ("agg_abs_wsg_kernel (gr_aggregate_dual_abs)" if ops.AGG_ABS and D == 200 and ops.TC_LINEAR
@@ -505,13 +535,13 @@ def run_ours(a):
         g_ms = float(np.mean(ts))
         nprod = 1 if act_bf16 else 3                         # bf16 products per output (3 = fp32-class split)
         flops = nprod * 2.0 * gM * gN * gK
-        tf_peak = float(peaks.get("bf16_tflops", 1590.0))
+        tf_peak = float(peaks.get("bf16_tflops", 989.0))
         roofline_gemm = {"bound": "tensor", "kernel": "linear_tc_kernel (gr_linear_tc_planes, %d bf16 product%s)" % (
                              nprod, "s" if nprod > 1 else ""),
                          "shape": {"M": gM, "N": gN, "K": gK}, "achieved": flops / (g_ms * 1e-3) / 1e12,
                          "peak": tf_peak, "unit": "TFLOP/s", "frac": flops / (g_ms * 1e-3) / 1e12 / tf_peak,
                          "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst, of measured)" if "bf16_tflops" in peaks
-                         else "1590 TFLOP/s (of fallback)",
+                         else "989 TFLOP/s (H100 SXM data sheet, dense bf16, not reached)",
                          "avg_launch_ms": g_ms, "launches_per_step": len(ts) // max(agg_steps, 1),
                          "fp32_equivalent_tflops": 2.0 * gM * gN * gK / (g_ms * 1e-3) / 1e12}
     roofline_fused = None
@@ -519,10 +549,10 @@ def run_ours(a):
         f_ms = float(np.mean(fused_ms))
         Kd = (2 * I + 1) * D
         flops = 3 * 2.0 * B * N * D * Kd
-        tf_peak = float(peaks.get("bf16_tflops", 1590.0))
+        tf_peak = float(peaks.get("bf16_tflops", 989.0))
         # what the fused kernel has to move: both CSRs + prior, the relation tables, h planes in, h planes out
         fbytes = 2 * F * 8 + 2 * (B * N + 1) * 4 + B * N * 4 + 2 * R1 * D * 4 + B * I * D * 4 + 2 * B * N * D * 4
-        roofline_fused = {"bound": "tensor", "kernel": "fused_layer_kernel (gr_fused_layer: aggregation -> tcgen05 GEMM)",
+        roofline_fused = {"bound": "tensor", "kernel": "fused_layer_kernel (gr_fused_layer: aggregation -> wgmma GEMM)",
                           "achieved": flops / (f_ms * 1e-3) / 1e12, "peak": tf_peak, "unit": "TFLOP/s",
                           "frac": flops / (f_ms * 1e-3) / 1e12 / tf_peak, "avg_launch_ms": f_ms,
                           "launches_per_step": len(fused_ms) // max(a.steps, 1),

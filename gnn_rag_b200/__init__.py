@@ -1,4 +1,4 @@
-"""gnn_rag_b200 -- B200-native (sm_100a) implementation of GNN-RAG's GNN retrieval hot path.
+"""gnn_rag_b200 -- H100-native (sm_90a) implementation of GNN-RAG's GNN retrieval hot path.
 
 Public surface mirrors the reference (cmavro/GNN-RAG ``gnn/``):
     from gnn_rag_b200 import ReaRev, NSM, Evaluator

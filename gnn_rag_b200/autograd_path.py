@@ -79,7 +79,7 @@ HOST_CHECK = False      # tests only: let a CPU-resident model evaluate this res
 
 def _require_cuda(dev):
     if dev.type != "cuda" and not HOST_CHECK:
-        raise RuntimeError("gnn_rag_b200 runs on CUDA only: move the model to a B200 (model.cuda()); there is no CPU "
+        raise RuntimeError("gnn_rag_b200 runs on CUDA only: move the model to an H100 (model.cuda()); there is no CPU "
                            "path (training=True included)")
 
 

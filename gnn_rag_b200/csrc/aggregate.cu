@@ -54,7 +54,7 @@ struct AggParams {
   const float* ins;     // [B, I, D]
   float* out;               // fp32 output (may be null when the bf16 planes are requested)
   __nv_bfloat16* out_hi;    // optional split-bf16 planes (hi + lo ~= value to 2^-18): the A operand layout of
-  __nv_bfloat16* out_lo;    // the tcgen05 e2e GEMM (linear_tc.cu); same column indexing as `out`
+  __nv_bfloat16* out_lo;    // the wgmma e2e GEMM (linear_tc.cu); same column indexing as `out`
   int64_t ld_planes;
   float* possible;
   int64_t out_row_stride, out_col0, seg_stride_j, seg_stride_dir;
@@ -144,7 +144,7 @@ __device__ __forceinline__ float edge_coeff(const AggParams& p, const AggDir& d,
 
 // Two running sums per feature element, independent of the instruction:
 //   A = sum_e c_e * relu(v_e)     S = sum_e c_e * v_e       (=> sum_e c_e * relu(-v_e) = A - S)
-// accumulated with the packed fp32x2 FMA of sm_100 (FFMA2) when VEC is even.  If every v_e >= 0 the two
+// accumulated as fp32 pairs (ffma2) when VEC is even.  If every v_e >= 0 the two
 // chains execute bit-identical operations, so A - S is exactly 0 where the true value is 0.
 template <int VEC, int MODE>
 __device__ __forceinline__ void accumulate(float (&A)[VEC], float (&S)[VEC], const float (&v)[VEC], float c) {
@@ -153,11 +153,11 @@ __device__ __forceinline__ void accumulate(float (&A)[VEC], float (&S)[VEC], con
 #pragma unroll
     for (int k = 0; k < VEC; k += 2) {
       const float2 vv = make_float2(v[k], v[k + 1]);
-      float2 s2 = __ffma2_rn(cc, vv, make_float2(S[k], S[k + 1]));
+      float2 s2 = ffma2(cc, vv, make_float2(S[k], S[k + 1]));
       S[k] = s2.x; S[k + 1] = s2.y;
       if (MODE == MODE_MSG) {
         const float2 vp = make_float2(fmaxf(vv.x, 0.f), fmaxf(vv.y, 0.f));
-        float2 a2 = __ffma2_rn(cc, vp, make_float2(A[k], A[k + 1]));
+        float2 a2 = ffma2(cc, vp, make_float2(A[k], A[k + 1]));
         A[k] = a2.x; A[k + 1] = a2.y;
       }
     }
@@ -177,8 +177,8 @@ __device__ __forceinline__ void msg_epilogue(float (&y)[VEC], const float (&xp)[
   if constexpr (VEC % 2 == 0) {
 #pragma unroll
     for (int k = 0; k < VEC; k += 2) {
-      float2 r = __fmul2_rn(make_float2(xp[k], xp[k + 1]), make_float2(A[k], A[k + 1]));
-      r = __ffma2_rn(make_float2(xn[k], xn[k + 1]), make_float2(T[k], T[k + 1]), r);
+      float2 r = fmul2(make_float2(xp[k], xp[k + 1]), make_float2(A[k], A[k + 1]));
+      r = ffma2(make_float2(xn[k], xn[k + 1]), make_float2(T[k], T[k + 1]), r);
       y[k] = r.x; y[k + 1] = r.y;
     }
   } else {
@@ -467,7 +467,7 @@ __global__ void __launch_bounds__(kThreads, 2) agg_kernel(const AggParams p) {
             if constexpr (VEC % 2 == 0) {
 #pragma unroll
               for (int k = 0; k < VEC; k += 2) {
-                float2 t2 = __ffma2_rn(make_float2(S[ch][k], S[ch][k + 1]), make_float2(-1.f, -1.f),
+                float2 t2 = ffma2(make_float2(S[ch][k], S[ch][k + 1]), make_float2(-1.f, -1.f),
                                        make_float2(A[ch][k], A[ch][k + 1]));
                 T[k] = t2.x; T[k + 1] = t2.y;
               }

@@ -6,7 +6,7 @@
 // FFMA2s that do the work -- 14 % were FMNMX (relu of every gathered table element; 24 % of the stall samples) and
 // ~38 % were address / predicate / loop scaffolding.
 //
-//   * relu(v) = (v + |v|) / 2, and |.| is a free source modifier of FFMA2 on sm_100 (SASS: FFMA2 R, |R|.F32x2, ...).
+//   * relu(v) = (v + |v|) / 2, and |.| is a free source modifier of FFMA.
 //     The edge loop accumulates  S = sum c*v  and  Q = sum c*|v|  -- 8 FFMA2 per gathered edge and lane, no FMNMX --
 //     and the epilogue uses  sum c*relu(v) = (Q+S)/2,  sum c*relu(-v) = (Q-S)/2  (the 1/2 is folded into the staged
 //     relu(+-ins)).  If every v of a row is >= 0 the two chains execute bit-identical operations, so Q-S == 0 exactly
@@ -63,7 +63,7 @@ struct PnParams {
   int64_t ld, out_col0, Nt;
   int B, N, I, j0;
   int32_t* tile_counter;   // persistent kernel: dynamic tile scheduler (zeroed before the launch)
-  int64_t table_rows;      // rows of each padded relation table (R1): the gather4 tensor maps need the extent
+  int64_t table_rows;      // rows of each padded relation table (R1); > 0 enables the staged-row variant (agg_abs_ws 3)
 };
 
 __device__ __forceinline__ float4 ldg4(const char* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
@@ -71,21 +71,21 @@ __device__ __forceinline__ float4 zero4() { return make_float4(0.f, 0.f, 0.f, 0.
 
 __device__ __forceinline__ void fma4(float4& acc, float c, const float4& v) {          // acc += c * v
   const float2 cc = make_float2(c, c);
-  const float2 lo = __ffma2_rn(cc, make_float2(v.x, v.y), make_float2(acc.x, acc.y));
-  const float2 hi = __ffma2_rn(cc, make_float2(v.z, v.w), make_float2(acc.z, acc.w));
+  const float2 lo = ffma2(cc, make_float2(v.x, v.y), make_float2(acc.x, acc.y));
+  const float2 hi = ffma2(cc, make_float2(v.z, v.w), make_float2(acc.z, acc.w));
   acc = make_float4(lo.x, lo.y, hi.x, hi.y);
 }
 __device__ __forceinline__ void fma4_abs(float4& acc, float c, const float4& v) {      // acc += c * |v|
   const float2 cc = make_float2(c, c);
-  const float2 lo = __ffma2_rn(cc, make_float2(fabsf(v.x), fabsf(v.y)), make_float2(acc.x, acc.y));
-  const float2 hi = __ffma2_rn(cc, make_float2(fabsf(v.z), fabsf(v.w)), make_float2(acc.z, acc.w));
+  const float2 lo = ffma2(cc, make_float2(fabsf(v.x), fabsf(v.y)), make_float2(acc.x, acc.y));
+  const float2 hi = ffma2(cc, make_float2(fabsf(v.z), fabsf(v.w)), make_float2(acc.z, acc.w));
   acc = make_float4(lo.x, lo.y, hi.x, hi.y);
 }
 
 __device__ __forceinline__ float4 addsub4(const float4& q, const float4& s, float sign) {   // q + sign*s, packed
   const float2 ss = make_float2(sign, sign);
-  const float2 lo = __ffma2_rn(make_float2(s.x, s.y), ss, make_float2(q.x, q.y));
-  const float2 hi = __ffma2_rn(make_float2(s.z, s.w), ss, make_float2(q.z, q.w));
+  const float2 lo = ffma2(make_float2(s.x, s.y), ss, make_float2(q.x, q.y));
+  const float2 hi = ffma2(make_float2(s.z, s.w), ss, make_float2(q.z, q.w));
   return make_float4(lo.x, lo.y, hi.x, hi.y);
 }
 
@@ -93,10 +93,10 @@ __device__ __forceinline__ float4 addsub4(const float4& q, const float4& s, floa
 template <bool LO = true>
 __device__ __forceinline__ void emit4(__nv_bfloat16* ph, __nv_bfloat16* pl, bool pred, const float4& xp,
                                       const float4& xn, const float4& U, const float4& V) {
-  float2 y01 = __fmul2_rn(make_float2(xp.x, xp.y), make_float2(U.x, U.y));
-  float2 y23 = __fmul2_rn(make_float2(xp.z, xp.w), make_float2(U.z, U.w));
-  y01 = __ffma2_rn(make_float2(xn.x, xn.y), make_float2(V.x, V.y), y01);
-  y23 = __ffma2_rn(make_float2(xn.z, xn.w), make_float2(V.z, V.w), y23);
+  float2 y01 = fmul2(make_float2(xp.x, xp.y), make_float2(U.x, U.y));
+  float2 y23 = fmul2(make_float2(xp.z, xp.w), make_float2(U.z, U.w));
+  y01 = ffma2(make_float2(xn.x, xn.y), make_float2(V.x, V.y), y01);
+  y23 = ffma2(make_float2(xn.z, xn.w), make_float2(V.z, V.w), y23);
   const __nv_bfloat162 h01 = __floats2bfloat162_rn(y01.x, y01.y), h23 = __floats2bfloat162_rn(y23.x, y23.y);
   // bf16x2 -> float2 by hand: low half << 16, high half masked (2 ALU ops per pair; the library routine compiles to 4)
   const uint32_t u01 = *reinterpret_cast<const uint32_t*>(&h01), u23 = *reinterpret_cast<const uint32_t*>(&h23);
@@ -107,7 +107,7 @@ __device__ __forceinline__ void emit4(__nv_bfloat16* ph, __nv_bfloat16* pl, bool
     return;
   }
   const float2 m1 = make_float2(-1.f, -1.f);
-  const float2 r01 = __ffma2_rn(f01, m1, y01), r23 = __ffma2_rn(f23, m1, y23);   // y - hi, exact, packed
+  const float2 r01 = ffma2(f01, m1, y01), r23 = ffma2(f23, m1, y23);   // y - hi, exact, packed
   const __nv_bfloat162 l01 = __floats2bfloat162_rn(r01.x, r01.y);
   const __nv_bfloat162 l23 = __floats2bfloat162_rn(r23.x, r23.y);
   if (pred) {
@@ -489,38 +489,20 @@ __device__ __forceinline__ float lds1(uint32_t a) {
 constexpr int kG4Slots = 8;                 // slots per stage = two gather4 groups
 constexpr int kOobRow = 0x3fffffff;         // row coordinate outside any table: zero fill, no memory traffic
 
-typedef CUresult (*AggEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static bool make_table_tmap(CUtensorMap* m, const float* pn, int64_t rows, int cols) {
-  static AggEncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* q = nullptr;
-    cudaDriverEntryPointQueryResult r;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &r) == cudaSuccess &&
-        r == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<AggEncodeTiledFn>(q);
+// four table rows r0..r3 (`slot_bytes` of each) into consecutive slots at dst, completion counted on `bar`: one 1-D
+// bulk copy per row (16-byte aligned slots; a 2-D tensor copy would need 128-byte aligned destinations).  A row of
+// kOobRow (a slot past the unit's edges, never read) copies row 0.
+__device__ __forceinline__ void tma_gather4(uint32_t dst, const float* table, uint64_t* bar, int r0, int r1, int r2,
+                                            int r3, uint32_t slot_bytes) {
+  const int rows[4] = {r0, r1, r2, r3};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const char* src = reinterpret_cast<const char*>(table) + (size_t)(rows[i] == kOobRow ? 0 : rows[i]) * kPnRowBytes;
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                     dst + (uint32_t)i * slot_bytes),
+                 "l"(src), "r"(slot_bytes), "r"(smem_u32(bar))
+                 : "memory");
   }
-  if (!fn) return false;
-  cuuint64_t dims[2] = {(cuuint64_t)kPnCols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)kPnRowBytes};
-  cuuint32_t box[2] = {(cuuint32_t)cols, 1u};
-  cuuint32_t estr[2] = {1, 1};
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(pn), dims, strides, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const CUtensorMap* map, uint64_t* bar, int r0, int r1, int r2,
-                                            int r3) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(dst), "l"(map), "r"(smem_u32(bar)), "r"(0), "r"(r0), "r"(r1),
-      "r"(r2), "r"(r3)
-      : "memory");
 }
 
 template <int NI, int ROWS>
@@ -536,7 +518,7 @@ struct alignas(16) G5Buf {
 };
 
 // ---------------------------------------------------------------------------------------------------------
-// gather4 kernel with a deeper prefetch (gr_set_option("agg_abs_ws", 34)).
+// staged-row kernel with a deeper prefetch (gr_set_option("agg_abs_ws", 3)).
 // Three gather kernels with very different instruction counts (tma2 340, tma3 308, g4 303 per unit) all ran 157.5 us:
 // 1730 units per SM / 14 warps x 1.27 us.  With the copies of unit k + 1 issued when unit k starts, a unit cannot
 // take less than the latency of a TMA gather (issue -> bytes landed -> mbarrier flip -> waiter resumes), ~1.3 us here,
@@ -546,8 +528,7 @@ struct alignas(16) G5Buf {
 // ---------------------------------------------------------------------------------------------------------
 template <int NI, int DT, int SEGP, int KW, int RPW>
 __global__ void __launch_bounds__((KW + 2) * 32, 1)
-agg_abs_g5_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1,
-                  const PnParams p, int ntiles) {
+agg_abs_g5_kernel(const PnParams p, int ntiles) {
   static_assert(DT % 4 == 0 && DT > 128 && DT <= kPnCols, "two column chunks of 128");
   constexpr int ROWS = KW * RPW;
   constexpr int kSlot = DT * 4;
@@ -669,7 +650,8 @@ agg_abs_g5_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constan
             if (lane == 0) mbar_expect_tx(bar, (uint32_t)(ng * kGroup));
             if (lane < ng) {
               const int4 qd = pb.quad[pd][plr][lane];
-              tma_gather4(ring_s + (uint32_t)(((gh + lane) & 3) * kGroup), pd ? &map1 : &map0, bar, qd.x, qd.y, qd.z, qd.w);
+              tma_gather4(ring_s + (uint32_t)(((gh + lane) & 3) * kGroup), p.dir[pd].pn, bar, qd.x, qd.y, qd.z, qd.w,
+                          (uint32_t)kSlot);
             }
             gh = (gh + ng) & 3;
             gfree -= ng;
@@ -797,15 +779,10 @@ int launch_g4(const PnParams& p, cudaStream_t stream) {
   static bool done[64] = {};
   int rc = set_smem_once(kern, smem, done);
   if (rc != GR_OK) return rc;
-  CUtensorMap m0, m1;
-  if (!make_table_tmap(&m0, p.dir[0].pn, p.table_rows, 200) || !make_table_tmap(&m1, p.dir[1].pn, p.table_rows, 200)) {
-    set_error("gr_aggregate_dual_abs: cuTensorMapEncodeTiled failed for the padded relation table");
-    return GR_ERR_CUDA;
-  }
   GR_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), stream));
   const unsigned tiles = (unsigned)ceil_div(p.Nt, KW * RPW);
   const unsigned pgrid = std::min<unsigned>(tiles, (unsigned)sm_count());
-  kern<<<pgrid, (KW + 2) * 32, smem, stream>>>(m0, m1, p, (int)tiles);
+  kern<<<pgrid, (KW + 2) * 32, smem, stream>>>(p, (int)tiles);
   GR_CHECK_LAUNCH();
   return GR_OK;
 }

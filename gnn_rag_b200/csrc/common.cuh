@@ -1,4 +1,4 @@
-// Shared helpers for libgnnrag_b200.so (sm_100a only).
+// Shared helpers for libgnnrag_b200.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,7 +9,7 @@
 
 namespace gr {
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 void set_error(const char* fmt, ...);
 
@@ -36,7 +36,7 @@ void set_error(const char* fmt, ...);
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// number of SMs of the current device (148 on B200); cached
+// number of SMs of the current device (132 on H100 SXM); cached
 int sm_count();
 
 // true the first time it is called for (flag array, current device): kernel attributes such as the dynamic
@@ -47,6 +47,14 @@ inline bool first_use_on_device(bool (&done)[64]) {
   if (done[dev]) return false;
   done[dev] = true;
   return true;
+}
+
+// element-wise fp32x2 fma / mul, rounded to nearest like the scalar instructions they expand to
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }

@@ -5,7 +5,7 @@
 //
 // The unfused pair (aggregate_abs.cu -> linear_tc.cu) writes the 2*I neighbour segments of the layer-input matrix to
 // HBM (0.41 GB per layer at cfg2) and reads them straight back as the GEMM's A operand.  Here the neighbour k-blocks
-// never leave the SM: aggregation warps produce them directly into the UMMA shared-memory operand slots (K-major,
+// never leave the SM: aggregation warps produce them directly into the wgmma shared-memory operand slots (K-major,
 // SWIZZLE_64B, bf16 hi/lo planes -- the layout TMA would have written), only the h segment and W come from memory.
 //
 // Per 128-row tile the K dimension is walked in G column groups of 32; group g holds, in this order,
@@ -19,35 +19,31 @@
 //
 // Edge data: once per batch both CSRs are re-laid out slot-major per quad of 4 rows ("quad ELL",
 // fused_ell_build_kernel); the kernel's stagers move a tile's entries into shared memory with ONE bulk copy per
-// direction and turn {table offset, source node} into {table offset, c_f} there (weighted graphs: fused_coef_kernel).  (Staging the
-// CSR slices inside the kernel -- row pointers, src / rel gathers, prior gather, a search for each edge's row -- kept
-// one warp busy for 34 us per tile and bounded the kernel at 400 us; profiles/README.md has the sequence.)
+// direction and turn {table offset, source node} into {table offset, c_f} there (weighted graphs: fused_coef_kernel), so
+// no per-edge index arithmetic runs inside the fused kernel.
 //
-// Warp roles (768 threads, one CTA per SM, clusters of 2 share W by TMA multicast):
+// Warp roles (512 threads, one CTA per SM, clusters of 2 share W by TMA multicast):
 //   warp 0      TMA producer: W k-blocks into a 3-stage ring, the H block of every group into its operand slot (the
 //               next tile's h blocks are L2-prefetched a tile ahead)
-//   warp 1      MMA issuer (one thread): tcgen05.mma cta_group::1 kind::f16, 3 products per k-step
-//   warps 2, 3  stagers (warp 2 also allocates TMEM: 2 x 256 columns, the epilogue of tile i overlaps the mainloop of
-//               tile i+1): bulk copies of the tile's ELL entries + quad offsets, relu(+-ins)/2 of its <= 2 questions
+//   warps 2, 3  stagers: bulk copies of the tile's ELL entries + quad offsets, relu(+-ins)/2 of its <= 2 questions
 //               -> double-buffered tile descriptor
-//   warps 4-7   epilogue: tcgen05.ld -> bias + relu + score dot -> fp32 h / bf16 planes via TMA stores
-//   warps 8-23  aggregation: warp a owns tile rows 8a .. 8a+7 = two quads; a quarter-warp owns a row, lane = 4 columns of
-//               the 32-column group, so one warp-wide 16-byte load gathers one in-edge of each row of the quad (one
-//               128-byte table line per row); 8 such loads in flight per lane, no predicates (slots past a quad's
-//               block read a {0, 0} entry)
-// Registers: 768 x 80 at launch; setmaxnreg hands the control (56) and epilogue (72) warp groups' surplus to the four
-// aggregation warp groups (88).  Operand slots are dedicated: slot t < 2I is always written by the aggregation warps,
-// slot 2I always by TMA, so every slot barrier flips once per group and the parity is the group counter.
+//   warps 4-11  two consumer warpgroups, 64 tile rows each: wgmma.mma_async (m64n32k16 chunks, 3 products per k-step)
+//               with the fp32 accumulator in registers, then the epilogue: bias + relu + score dot -> fp32 h / bf16
+//               planes via TMA stores
+//   warps 12-15 aggregation: warp a owns tile rows 32a .. 32a+31 = eight quads; a quarter-warp owns a row, lane = 4
+//               columns of the 32-column group, so one warp-wide 16-byte load gathers one in-edge of each row of the
+//               quad (one 128-byte table line per row); 8 such loads in flight per lane, no predicates (slots past a
+//               quad's block read a {0, 0} entry)
+// Registers: 512 x 128 at launch; setmaxnreg shrinks the control (40) and aggregation (72) warpgroups and grows the
+// consumers (200), whose register accumulators (128 rows x n_pad fp32 per tile) take the place of tensor memory.
+// Operand slots are dedicated: slot t < 2I is always written by the aggregation warps, slot 2I always by TMA, so every
+// slot barrier flips once per group and the parity is the group counter.
 //
-// Measured (B200, cfg2: 128 000 rows, D = 200, I = 2): 259 us per layer against 287 us for the unfused pair (125 + 161).  Not faster than that because all three per-SM resources are near their limit at once:
-// tensor pipe 115 us of issue (3 products), the L1 / shared-memory SRAM (UMMA operand reads 2.0 MB + TMA writes 1.0 MB
-// + operand stores 0.45 MB + gathers 0.8 MB per tile; l1tex data pipe 68 %, MMA issue slows from 115 to 230 us when the
-// aggregation warps run), and the aggregation's L2 gather latency with only ~28 KB of L1 left beside 226 KB of shared
-// memory.  DESIGN.md 4.7 has the decomposition.
+// Performance on H100: not measured per kernel.
 #include <algorithm>
 #include <cstddef>
 
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 namespace gr {
 
@@ -67,17 +63,23 @@ namespace {
 using namespace tc;
 
 constexpr int BK = 32;                       // k-block width: 64-byte rows, SWIZZLE_64B
-constexpr int kAggWarps = 16;
-constexpr int kEpiWarps = 4;
-constexpr int kFirstEpi = 4, kFirstAgg = 8;
-constexpr int kThreads = (kFirstAgg + kAggWarps) * 32;      // 768
+constexpr int kAggWarps = 4;
+constexpr int kConsWarps = 8;                // two consumer warpgroups
+constexpr int kFirstCons = 4, kFirstAgg = 12;
+constexpr int kThreads = (kFirstAgg + kAggWarps) * 32;      // 512
+constexpr int kQuadsPerWarp = BM / 4 / kAggWarps;           // 8: an aggregation warp owns 32 tile rows
+constexpr int kMaxChunksFused = 7;           // register accumulator: n_pad <= 224 (= kXCols: D <= 224)
+// setmaxnreg budget: 512 x 128 at launch = 128 x 40 (control) + 256 x 200 (consumers) + 128 x 72 (aggregation)
+constexpr int kLaunchRegs = 128, kControlRegs = 40, kConsRegs = 200, kAggRegs = 72;
+static_assert(kControlRegs <= kLaunchRegs && kAggRegs <= kLaunchRegs && kConsRegs >= kLaunchRegs,
+              "setmaxnreg: control and aggregation warpgroups shrink (.dec), consumers grow (.inc)");
+static_assert(128 * (kControlRegs + kAggRegs) + 256 * kConsRegs <= kThreads * kLaunchRegs, "register budget");
 constexpr int kNW = 3;                       // W ring stages
 constexpr int kECap = 1024;                  // staged in-edges per direction per tile (mean 512 at cfg2); rest: slow path
 constexpr int kXCols = 224;                  // instruction columns kept per question: 7 groups of 32 (zero padded)
 constexpr int kPnRowBytes = 1024;            // padded relation table: 256 fp32 per row (gr_pad_table256)
 constexpr int kABytes = BM * BK * 2;         // one bf16 plane of an A slot: 8 KB
-constexpr int kOutBytes = BM * 16 * 4 + 2 * BM * 16 * 2;    // epilogue staging: fp32 8 KB + hi 4 KB + lo 4 KB
-constexpr int kAccStride = 256;
+constexpr int kOutBytes = 2 * kStageOutBytes;               // epilogue staging: 8 KB per consumer warpgroup
 
 struct FDir {
   const int32_t* rowptr;
@@ -140,7 +142,7 @@ struct alignas(16) ETile {
 template <int NI>
 constexpr size_t fused_smem_bytes(int n_pad) {
   return 1024 /*align slack*/ + (size_t)(2 * NI + 1) * 2 * kABytes + (size_t)kNW * 2 * n_pad * BK * 2 + kOutBytes +
-         2 * sizeof(ETile<NI>) + 64 * 8 + 16 + 2 * 256 * 4;
+         2 * sizeof(ETile<NI>) + 64 * 8 + 2 * 256 * 4;
 }
 
 // W [N, (2I+1)*D] fp32 -> hi/lo planes [N, G*T*32] in the kernel's K order (see the header comment)
@@ -367,10 +369,10 @@ struct Acc4 {                                   // S = sum c*v, Q = sum c*|v| fo
   __device__ __forceinline__ void clear() { s0 = s1 = q0 = q1 = make_float2(0.f, 0.f); }
   __device__ __forceinline__ void add(float c, const float4& v) {
     const float2 cc = make_float2(c, c);
-    s0 = __ffma2_rn(cc, make_float2(v.x, v.y), s0);
-    s1 = __ffma2_rn(cc, make_float2(v.z, v.w), s1);
-    q0 = __ffma2_rn(cc, make_float2(fabsf(v.x), fabsf(v.y)), q0);
-    q1 = __ffma2_rn(cc, make_float2(fabsf(v.z), fabsf(v.w)), q1);
+    s0 = ffma2(cc, make_float2(v.x, v.y), s0);
+    s1 = ffma2(cc, make_float2(v.z, v.w), s1);
+    q0 = ffma2(cc, make_float2(fabsf(v.x), fabsf(v.y)), q0);
+    q1 = ffma2(cc, make_float2(fabsf(v.z), fabsf(v.w)), q1);
   }
 };
 
@@ -380,15 +382,15 @@ __device__ __forceinline__ void emit_quad(uint32_t slot, const float4& xp, const
                                           const float2& U1, const float2& V0, const float2& V1) {
   const float2 xp0 = make_float2(xp.x, xp.y), xp1 = make_float2(xp.z, xp.w);
   const float2 xn0 = make_float2(xn.x, xn.y), xn1 = make_float2(xn.z, xn.w);
-  float2 y0 = __fmul2_rn(xp0, U0), y1 = __fmul2_rn(xp1, U1);
-  y0 = __ffma2_rn(xn0, V0, y0);
-  y1 = __ffma2_rn(xn1, V1, y1);
+  float2 y0 = fmul2(xp0, U0), y1 = fmul2(xp1, U1);
+  y0 = ffma2(xn0, V0, y0);
+  y1 = ffma2(xn1, V1, y1);
   const __nv_bfloat162 h0 = __floats2bfloat162_rn(y0.x, y0.y), h1 = __floats2bfloat162_rn(y1.x, y1.y);
   const uint32_t u0 = *reinterpret_cast<const uint32_t*>(&h0), u1 = *reinterpret_cast<const uint32_t*>(&h1);
   const float2 f0 = make_float2(__uint_as_float(u0 << 16), __uint_as_float(u0 & 0xffff0000u));
   const float2 f1 = make_float2(__uint_as_float(u1 << 16), __uint_as_float(u1 & 0xffff0000u));
   const float2 m1 = make_float2(-1.f, -1.f);
-  const float2 r0 = __ffma2_rn(f0, m1, y0), r1 = __ffma2_rn(f1, m1, y1);
+  const float2 r0 = ffma2(f0, m1, y0), r1 = ffma2(f1, m1, y1);
   const __nv_bfloat162 l0 = __floats2bfloat162_rn(r0.x, r0.y), l1 = __floats2bfloat162_rn(r1.x, r1.y);
   sts_u2(slot, u0, u1);
   sts_u2(slot + kABytes, *reinterpret_cast<const uint32_t*>(&l0), *reinterpret_cast<const uint32_t*>(&l1));
@@ -408,9 +410,9 @@ __device__ __forceinline__ void agg_pass(const ETile<NI>& et, const FParams& p, 
   const uint32_t rc_s = et_s + (uint32_t)d * kECap * 8u + (uint32_t)r * 8u;
   const uint32_t xs = et_s + (uint32_t)offsetof(ETile<NI>, x) + (uint32_t)((g * BK + 4 * c8) * 4);
   const float2 one = make_float2(1.f, 1.f), mone = make_float2(-1.f, -1.f);
-#pragma unroll
-  for (int qd = 0; qd < 2; ++qd) {
-    const int quad = wa * 2 + qd;
+#pragma unroll 1
+  for (int qd = 0; qd < kQuadsPerWarp; ++qd) {
+    const int quad = wa * kQuadsPerWarp + qd;
     const int lr = quad * 4 + r;
     if (quad * 4 >= nrows) break;                            // warp uniform
     Acc4 acc;
@@ -444,8 +446,8 @@ __device__ __forceinline__ void agg_pass(const ETile<NI>& et, const FParams& p, 
       }
     }
     if (lr < nrows) {
-      const float2 U0 = __ffma2_rn(acc.s0, one, acc.q0), V0 = __ffma2_rn(acc.s0, mone, acc.q0);
-      const float2 U1 = __ffma2_rn(acc.s1, one, acc.q1), V1 = __ffma2_rn(acc.s1, mone, acc.q1);
+      const float2 U0 = ffma2(acc.s0, one, acc.q0), V0 = ffma2(acc.s0, mone, acc.q0);
+      const float2 U1 = ffma2(acc.s1, one, acc.q1), V1 = ffma2(acc.s1, mone, acc.q1);
       const int q = lr >= lr_switch ? 1 : 0;
       const uint32_t off = (uint32_t)lr * 64u + ((uint32_t)((c8 >> 1) ^ ((lr >> 1) & 3)) << 4) + (uint32_t)(c8 & 1) * 8u;
 #pragma unroll
@@ -473,20 +475,17 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
   const int w_bytes = p.n_pad * BK * 2;
   uint8_t* a_slots = smem;                                        // [T] x {hi 8 KB, lo 8 KB}
   uint8_t* w_ring = a_slots + (size_t)T * 2 * kABytes;            // [kNW] x {W_hi, W_lo}
-  uint8_t* s_out = w_ring + (size_t)kNW * 2 * w_bytes;            // epilogue staging
+  uint8_t* s_out = w_ring + (size_t)kNW * 2 * w_bytes;            // epilogue staging: [2 consumer warpgroups]
   ETile<NI>* etile = reinterpret_cast<ETile<NI>*>(s_out + kOutBytes);
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(etile) + 2 * sizeof(ETile<NI>));
   uint64_t* wfull = bars;                 // [kNW]
   uint64_t* wempty = wfull + kNW;         // [kNW]
   uint64_t* afull = wempty + kNW;         // [T]
   uint64_t* aempty = afull + T;           // [T]
-  uint64_t* tmem_full = aempty + T;       // [2]
-  uint64_t* tmem_empty = tmem_full + 2;   // [2]
-  uint64_t* efull = tmem_empty + 2;       // [2]
+  uint64_t* efull = aempty + T;           // [2]
   uint64_t* eempty = efull + 2;           // [2]
   uint64_t* sbar = eempty + 2;            // [2] one per stager warp: its own bulk copies
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 64);
-  float* s_bias = reinterpret_cast<float*>(tmem_slot + 4);        // [256]
+  float* s_bias = reinterpret_cast<float*>(bars + 64);            // [256]
   float* s_ws = s_bias + 256;                                     // [256]
   for (int i = threadIdx.x; i < 256; i += kThreads) {
     s_bias[i] = (p.bias && i < p.N) ? p.bias[i] : 0.f;
@@ -499,32 +498,21 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
   constexpr uint16_t kMask = (uint16_t)((1u << CS) - 1);
   const int G = p.G;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kNW; ++s) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], CS); }
-    for (int t = 0; t < T; ++t) { mbar_init(&afull[t], t == T - 1 ? 1 : kAggWarps); mbar_init(&aempty[t], 1); }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], kEpiWarps);
-      mbar_init(&efull[a], 2); mbar_init(&eempty[a], kAggWarps); mbar_init(&sbar[a], 1);
-    }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kNW; ++s) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], kConsWarps * CS); }
+    for (int t = 0; t < T; ++t) { mbar_init(&afull[t], t == T - 1 ? 1 : kAggWarps); mbar_init(&aempty[t], kConsWarps); }
+    for (int a = 0; a < 2; ++a) { mbar_init(&efull[a], 2); mbar_init(&eempty[a], kAggWarps); mbar_init(&sbar[a], 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  } else if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(2u * kAccStride)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
   if (CS > 1) cluster_sync_all();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  // register file: 768 threads x 80 at launch = the CTA's pool; the control warpgroup (warps 0-3, -> 56) and the epilogue
-  // warpgroup (4-7, -> 72) hand back exactly what the four aggregation warpgroups take (-> 88: 16 gathers in flight per
-  // lane).  setmaxnreg.inc only draws on registers released inside the CTA: 128*56 + 128*72 + 512*88 = 768*80.
-  // (the instruction sits at the top of each role's branch: ptxas budgets the code it dominates)
-  if (warp < kFirstEpi) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+  // register file: kThreads x kLaunchRegs at launch = the CTA's pool; the control and aggregation warpgroups hand back
+  // what the two consumer warpgroups (register accumulators) take.  setmaxnreg.inc only draws on registers released
+  // inside the CTA.  (The instruction sits at the top of each role's branch: ptxas
+  // budgets the code it dominates.)
+  if (warp < kFirstCons) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kControlRegs));
     if (warp == 0) {
     // ===================== TMA producer =====================
     if (lane == 0) {
@@ -574,48 +562,7 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
       }
       pf.store(5, 2);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      Prof pf; pf.init(p.debug & 32);
-      const long long t_all = pf.t();
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.n_pad >> 3) << 17) |
-                             ((uint32_t)(BM >> 4) << 24);
-      uint32_t wphase = 0, grp = 0;
-      int ws = 0, it = 0;
-      for (int tg = cid; tg < ngroups; tg += ncluster, ++it) {
-        const int acc = it & 1;
-        { const long long t0 = pf.t(); mbar_wait_sleep(&tmem_empty[acc], ((it >> 1) & 1) ^ 1, 3); pf.add(3, t0); }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * kAccStride);
-        for (int g = 0; g < G; ++g, ++grp) {
-          const int ksteps = g == G - 1 ? p.ksteps_last : BK / UMMA_K;
-          for (int t = 0; t < T; ++t) {
-            const int sl = t == 0 ? T - 1 : t - 1;              // operand slot of block t (slot T-1 = the h block)
-            { const long long t0 = pf.t(); mbar_wait_sleep(&wfull[ws], wphase, 4); pf.add(0, t0); }
-            { const long long t0 = pf.t(); mbar_wait_sleep(&afull[sl], grp & 1, 10 + sl); pf.add(t == 0 ? 2 : 1, t0); }
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t sa = smem_u32(a_slots + (size_t)sl * 2 * kABytes);
-            const uint32_t sw = smem_u32(w_ring + (size_t)ws * 2 * w_bytes);
-            const uint64_t da_hi = make_smem_desc<BK>(sa), da_lo = make_smem_desc<BK>(sa + kABytes);
-            const uint64_t dw_hi = make_smem_desc<BK>(sw), dw_lo = make_smem_desc<BK>(sw + w_bytes);
-            for (int k = 0; k < ksteps; ++k) {
-              const uint64_t adv = (uint64_t)((k * UMMA_K * 2) >> 4);
-              umma_bf16(tmem_d, da_hi + adv, dw_hi + adv, idesc, (g | t | k) ? 1u : 0u);
-              umma_bf16(tmem_d, da_hi + adv, dw_lo + adv, idesc, 1u);
-              umma_bf16(tmem_d, da_lo + adv, dw_hi + adv, idesc, 1u);
-            }
-            if (CS == 1) umma_commit(&wempty[ws]); else umma_commit_mc(&wempty[ws], kMask);
-            umma_commit(&aempty[sl]);
-            if (++ws == kNW) { ws = 0; wphase ^= 1; }
-          }
-        }
-        umma_commit(&tmem_full[acc]);
-      }
-      pf.total(0, t_all);
-      pf.store(1, 4);
-    }
-  } else {
+  } else if (warp >= 2) {
     // ===================== edge stagers: warp 3 direction 0 (+ header, instructions), warp 2 direction 1 ==========
     Prof pf; pf.init((p.debug & 32) && warp == 3 && lane == 0);
     uint32_t own_uses = 0;
@@ -633,7 +580,7 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
   }
   } else if (warp >= kFirstAgg) {
     // ===================== aggregation warps =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 88;");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kAggRegs));   // kAggRegs < kLaunchRegs
     const int wa = warp - kFirstAgg;
     Prof pf; pf.init((p.debug & 32) && wa == 0 && lane == 0);
     const long long t_all = pf.t();
@@ -667,100 +614,70 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
     pf.total(7, t_all);
     pf.store(8, 3);
   } else {
-    // ===================== epilogue =====================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-    const int q = warp & 3;
-    const int row_in_tile = q * 32 + lane;
-    const bool relu = p.flags & GR_LINEAR_RELU;
-    const int nchunks = p.n_pad / 16;
-    float* s_c = reinterpret_cast<float*>(s_out) + row_in_tile * 16;
-    uint32_t* s_h = reinterpret_cast<uint32_t*>(s_out + BM * 16 * 4) + row_in_tile * 8;
-    uint32_t* s_l = reinterpret_cast<uint32_t*>(s_out + BM * 16 * 4 + BM * 16 * 2) + row_in_tile * 8;
-    const bool issuer = warp == kFirstEpi && lane == 0;
-    Prof pf; pf.init((p.debug & 32) && issuer);
+    // ===================== consumers: wgmma over the tile's k-blocks, then the epilogue =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsRegs));
+    const int cw = (warp - kFirstCons) >> 2, wq = warp & 3;     // consumer warpgroup (row half), warp inside it
+    const int nc = (p.n_pad + 31) / 32;
+    const bool tail16 = (p.n_pad & 31) != 0;
+    const EpiOut e{s_bias, s_ws, (p.flags & GR_LINEAR_RELU) != 0};
+    const int r = wq * 16 + (lane >> 2), cq = lane & 3;
+    uint8_t* stg = s_out + (size_t)cw * kStageOutBytes;
+    const bool issuer = wq == 0 && lane == 0;
+    Prof pf; pf.init((p.debug & 32) && cw == 0 && issuer);
     const long long t_all = pf.t();
-    int it = 0;
-    for (int tg = cid; tg < ngroups; tg += ncluster, ++it) {
+    uint32_t wphase = 0, grp = 0;
+    int ws = 0;
+    for (int tg = cid; tg < ngroups; tg += ncluster) {
       const int tile = tg * CS + crank;
-      const int acc = it & 1;
-      { const long long t0 = pf.t(); mbar_wait_sleep(&tmem_full[acc], (it >> 1) & 1, 7, 500); pf.add(0, t0); }
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int64_t row = (int64_t)tile * BM + row_in_tile;
-      const bool row_ok = row < p.M;
-      float dot = 0.f;
-      const uint32_t taddr = tmem_base + (uint32_t)(acc * kAccStride) + ((uint32_t)(q * 32) << 16);
-      for (int ch = (p.debug & 16) ? nchunks - 1 : 0; ch < nchunks; ++ch) {     // debug 16: last chunk only
-        const int c0 = ch * 16;
-        uint32_t r[16];
-        tmem_ld16(taddr + (uint32_t)c0, r);
-        if (ch == nchunks - 1) {
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        }
-        float v[16];
+      float acc[kMaxChunksFused][16];
 #pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const float4 b4 = *reinterpret_cast<const float4*>(s_bias + c0 + j);
-          const float4 w4 = *reinterpret_cast<const float4*>(s_ws + c0 + j);
-          float x0 = __uint_as_float(r[j]) + b4.x, x1 = __uint_as_float(r[j + 1]) + b4.y;
-          float x2 = __uint_as_float(r[j + 2]) + b4.z, x3 = __uint_as_float(r[j + 3]) + b4.w;
-          if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f); }
-          dot = fmaf(x0, w4.x, dot); dot = fmaf(x1, w4.y, dot);
-          dot = fmaf(x2, w4.z, dot); dot = fmaf(x3, w4.w, dot);
-          v[j] = x0; v[j + 1] = x1; v[j + 2] = x2; v[j + 3] = x3;
-        }
-        if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        named_bar_sync(1, kEpiWarps * 32);
-        if (p.C) {
+      for (int j = 0; j < kMaxChunksFused; ++j)
 #pragma unroll
-          for (int j = 0; j < 16; j += 4)
-            *reinterpret_cast<float4*>(s_c + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-        if (p.has_planes) {
-          uint32_t h[8], l[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            const __nv_bfloat162 h2 = __floats2bfloat162_rn(v[j], v[j + 1]);
-            const float2 hf = __bfloat1622float2(h2);
-            const __nv_bfloat162 l2 = __floats2bfloat162_rn(v[j] - hf.x, v[j + 1] - hf.y);
-            h[j / 2] = *reinterpret_cast<const uint32_t*>(&h2);
-            l[j / 2] = *reinterpret_cast<const uint32_t*>(&l2);
-          }
-          *reinterpret_cast<uint4*>(s_h) = make_uint4(h[0], h[1], h[2], h[3]);
-          *reinterpret_cast<uint4*>(s_h + 4) = make_uint4(h[4], h[5], h[6], h[7]);
-          *reinterpret_cast<uint4*>(s_l) = make_uint4(l[0], l[1], l[2], l[3]);
-          *reinterpret_cast<uint4*>(s_l + 4) = make_uint4(l[4], l[5], l[6], l[7]);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        named_bar_sync(1, kEpiWarps * 32);
-        if (issuer && !(p.debug & 4)) {
-          const int m0 = tile * BM;
-          if (p.C) tma_store_2d(&map_c, s_out, c0, m0);
-          if (p.has_planes) {
-            tma_store_2d(&map_c_hi, s_out + BM * 16 * 4, c0, m0);
-            tma_store_2d(&map_c_lo, s_out + BM * 16 * 4 + BM * 16 * 2, c0, m0);
-          }
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
+      int prev_ws = -1, prev_sl = -1;
+      for (int g = 0; g < G; ++g, ++grp) {
+        const int ksteps = g == G - 1 ? p.ksteps_last : BK / MMA_K;
+        for (int t = 0; t < T; ++t) {
+          const int sl = t == 0 ? T - 1 : t - 1;              // operand slot of block t (slot T-1 = the h block)
+          { const long long t0 = pf.t(); mbar_wait_sleep(&wfull[ws], wphase, 4); pf.add(0, t0); }
+          { const long long t0 = pf.t(); mbar_wait_sleep(&afull[sl], grp & 1, 10 + sl); pf.add(t == 0 ? 2 : 1, t0); }
+          const uint32_t sa = smem_u32(a_slots + (size_t)sl * 2 * kABytes) + (uint32_t)(cw * WG_M * BK * 2);
+          const uint32_t sw = smem_u32(w_ring + (size_t)ws * 2 * w_bytes);
+          mma_kblock<kMaxChunksFused, BK>(acc, make_smem_desc<BK>(sa), make_smem_desc<BK>(sa + kABytes),
+                                          make_smem_desc<BK>(sw), make_smem_desc<BK>(sw + w_bytes), ksteps, nc,
+                                          false, tail16);
+          wgmma_wait<1>();                                     // the previous k-block is done: free its W and A slots
+          if (prev_ws >= 0 && lane == 0) { release_slot<CS>(&wempty[prev_ws]); mbar_arrive(&aempty[prev_sl]); }
+          prev_ws = ws; prev_sl = sl;
+          if (++ws == kNW) { ws = 0; wphase ^= 1; }
         }
       }
-      if (p.dots && row_ok) {
-        p.dots[row] = dot;
-        p.dots[(int64_t)p.M + row] = 0.f;
+      wgmma_wait<0>();
+      if (prev_ws >= 0 && lane == 0) { release_slot<CS>(&wempty[prev_ws]); mbar_arrive(&aempty[prev_sl]); }
+
+      const int64_t row0 = (int64_t)tile * BM + cw * WG_M + r;
+      float dot0 = 0.f, dot1 = 0.f;
+      const bool store = !(p.debug & 4);
+#pragma unroll
+      for (int j = 0; j < kMaxChunksFused; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int c0 = 32 * j + 16 * h;
+          if (j >= nc || c0 >= p.n_pad) continue;
+          float v[8];
+          epi_values(acc[j], h, c0, cq, e, v, dot0, dot1);
+          epi_store_tma(v, stg, r, cq, issuer, 1 + cw, &map_c, &map_c_hi, &map_c_lo, store && p.C != nullptr,
+                        store && p.has_planes, c0, tile * BM + cw * WG_M);
+        }
       }
+      epi_dots(dot0, dot1, p.dots, row0, p.M, cq);
     }
     if (issuer) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    pf.total(14, t_all);
-    pf.store(13, 1);
+    pf.total(0, t_all);
+    pf.store(1, 4);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
   if (CS > 1) cluster_sync_all();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2u * kAccStride)
-                 : "memory");
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -881,12 +798,12 @@ FusedPlan plan_fused(int64_t Nq, int64_t D, int64_t pitch, int I, int64_t N_out)
   FusedPlan f{};
   f.n_pad = (int)((N_out + 15) / 16 * 16);
   f.G = (int)((pitch + BK - 1) / BK);
-  f.ksteps_last = (int)((pitch - (int64_t)(f.G - 1) * BK) / UMMA_K);
+  f.ksteps_last = (int)((pitch - (int64_t)(f.G - 1) * BK) / MMA_K);
   f.kp = (int64_t)f.G * (2 * I + 1) * BK;
   f.w_plane_bytes = align_up((size_t)N_out * f.kp * 2, 256);
   f.smem_bytes = I == 2 ? fused_smem_bytes<2>(f.n_pad) : fused_smem_bytes<1>(f.n_pad);
   f.ok = (I == 1 || I == 2) && Nq >= BM && D >= 8 && D <= pitch && pitch % 16 == 0 && (pitch + BK - 1) / BK * BK <= kXCols &&
-         N_out >= 8 && N_out <= 256 && f.smem_bytes <= 227 * 1024 && get_encode_fn() != nullptr;
+         N_out >= 8 && f.n_pad <= 32 * kMaxChunksFused && f.smem_bytes <= 227 * 1024 && get_encode_fn() != nullptr;
   return f;
 }
 
@@ -899,15 +816,16 @@ int launch_fused(const CUtensorMap& m_h_hi, const CUtensorMap& m_h_lo, const CUt
     GR_CHECK_CUDA(cudaFuncSetAttribute(fused_layer_kernel<NI, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        227 * 1024));
   }
-  // the setmaxnreg budget of the kernel (56 / 72 / 88) redistributes exactly 768 x 80 registers
+  // the setmaxnreg budget of the kernel redistributes exactly kThreads x kLaunchRegs registers
   static int num_regs = 0;
   if (num_regs == 0) {
     cudaFuncAttributes fa{};
     GR_CHECK_CUDA(cudaFuncGetAttributes(&fa, fused_layer_kernel<NI, CS>));
     num_regs = fa.numRegs;
   }
-  if (num_regs != 80) {
-    set_error("gr_fused_layer: kernel was compiled with %d registers per thread, the warp-group budget needs 80", num_regs);
+  if (num_regs != kLaunchRegs) {
+    set_error("gr_fused_layer: kernel was compiled with %d registers per thread, the warp-group budget needs %d",
+              num_regs, kLaunchRegs);
     return GR_ERR_UNSUPPORTED;
   }
   const int ngroups = (p.num_tiles + CS - 1) / CS;
@@ -1001,7 +919,7 @@ extern "C" int gr_fused_layer(const int32_t* rowptr_t, const int32_t* src_t, con
   FusedPlan f = plan_fused(N_nodes, D, seg_pitch, I, N_out);
   if (!f.ok) {
     set_error("gr_fused_layer: unsupported shape N=%d D=%d pitch=%lld I=%d N_out=%lld (need I <= 2, N >= 128, "
-              "pitch %% 16 == 0, pitch <= 256, N_out <= 256 and the stages must fit shared memory)",
+              "pitch %% 16 == 0, pitch <= 224, N_out <= 224 and the stages must fit shared memory)",
               N_nodes, D, (long long)seg_pitch, I, (long long)N_out);
     return GR_ERR_UNSUPPORTED;
   }

@@ -1,6 +1,6 @@
 // fp32 SIMT linear layer: C = act(A W^T + bias) (+ addend).  Exact-fp32 path of gr_linear: used for the
 // hoisted relation projection rel_linear_k(rel_features) (reference reasongnn.py:79,105 applies the same
-// Linear to F gathered rows), for small problems, and as the validator of the split-bf16 tcgen05 path
+// Linear to F gathered rows), for small problems, and as the validator of the split-bf16 wgmma path
 // (linear_tc.cu).  Classic 128x64x16 shared-memory tiling, 8x4 outputs per thread.
 #include "common.cuh"
 

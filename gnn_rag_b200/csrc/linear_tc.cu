@@ -1,20 +1,20 @@
-// Tensor-core linear layer for sm_100a:  C = act(A W^T + bias)  with fp32 in / fp32 out and fp32-class
-// accuracy, via the 3-product split-bf16 scheme on tcgen05:
+// Tensor-core linear layer for sm_90a:  C = act(A W^T + bias)  with fp32 in / fp32 out and fp32-class
+// accuracy, via the 3-product split-bf16 scheme on wgmma:
 //     x = hi + lo (hi = bf16(x), lo = bf16(x - hi));   A W^T ~= A_hi W_hi^T + A_hi W_lo^T + A_lo W_hi^T
-// (dropped term A_lo W_lo^T <= 2^-18 relative).  All three products accumulate into one fp32 TMEM
+// (dropped term A_lo W_lo^T <= 2^-18 relative).  All three products accumulate into one fp32 register
 // accumulator.  This is the `e2e_linear` of ReasonGNNLayer.forward / NSMBaseLayer.forward
 // (reference gnn/modules/kg_reasoning/reasongnn.py:163, nsm_gnn.py:63): a genuine dense contraction,
 // M = B*N node rows, K = (2*num_ins+1)*D, N = D.
 //
-// Kernel: one CTA per 128-row tile of A, full N (<= 256) per CTA.  Warp roles (canonical Blackwell
-// GEMM): warp 0 = TMA producer (cp.async.bulk.tensor, 128B-swizzled K-major tiles of the four bf16
-// planes), warp 1 = MMA issuer (single thread, tcgen05.mma.cta_group::1.kind::f16, UMMA 128 x Npad x 16,
-// 3 MMAs per K-step), warp 2 = TMEM allocator, warps 4-7 = epilogue (tcgen05.ld 32x32b, bias + relu,
-// stores).  smem ring of kStages {A_hi, A_lo, W_hi, W_lo} stages with full/empty mbarriers;
-// tcgen05.commit releases a stage and finally signals the epilogue.
+// Kernel: persistent, one 128-row tile of A at a time, full N (<= 256) per CTA.  Warpgroup 0 = TMA producer
+// (cp.async.bulk.tensor, swizzled K-major tiles of the four bf16 planes into a ring of `stages` slots with
+// full/empty mbarriers); warpgroups 1 and 2 = consumers, 64 rows each: wgmma.mma_async m64n32k16 / m64n16k16 from
+// shared memory (3 products per K step), fp32 accumulator in registers, then the epilogue (bias + relu + score dot,
+// fp32 and bf16 hi/lo plane outputs, staged TMA stores or direct stores).  Clusters of 2 CTAs share the W tiles by
+// TMA multicast.
 //
 // Roofline: tensor-pipe work 3 * 2*M*N*K flop; HBM traffic ~ 2 planes * M*K*2 B = M*K*4 B (same as fp32 A).
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 namespace gr {
 
@@ -26,10 +26,13 @@ int g_tc_tma_store = 1;    // gr_set_option("tc_tma_store", 0|1): staged TMA-sto
 namespace {
 
 using namespace tc;
-// k-block width BK (bf16 elements) is a template parameter: 64 (128-byte swizzle rows, 2-3 smem stages)
-// or 32 (64-byte swizzle rows, twice as many, finer stages -> more TMA requests in flight)
-constexpr int kThreads = 384;   // warps 0-3: TMA / MMA / TMEM alloc / idle; warps 4-11: epilogue (2 column halves)
-constexpr int kEpiWarps = 8;
+// k-block width BK (bf16 elements) is a template parameter: 64 (128-byte swizzle rows) or 32 (64-byte swizzle rows,
+// twice as many, finer stages -> more TMA requests in flight)
+constexpr int kThreads = 384;          // warpgroup 0: TMA producer; warpgroups 1, 2: consumers
+constexpr int kConsumerWarps = 8;
+// setmaxnreg budget: 384 threads x 168 registers at launch = 128 x 40 (producer) + 256 x 232 (consumers)
+constexpr int kLaunchRegs = 168, kProducerRegs = 40, kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= kThreads * kLaunchRegs, "register budget");
 
 // ---------------------------------------------------------------------------------------------------
 // fp32 -> (hi, lo) bf16 planes
@@ -95,20 +98,17 @@ struct TcParams {
   __nv_bfloat16* c_hi;      // optional bf16 hi/lo planes of the output (next layer's A operand)
   __nv_bfloat16* c_lo;
   int64_t ldc16;
-  const float* w_score;     // optional: score_func dot product (reasongnn.py:165), as two partial sums:
-  float* dots;              //   dots[half*M + m] = sum over this half's columns of out[m,n] * w_score[n]
-  int M, N, K, n_pad, stages, num_tiles;
+  const float* w_score;     // optional: score_func dot product (reasongnn.py:165): dots[m] = sum_n out[m,n] * w_score[n],
+  float* dots;              //   dots[M + m] = 0 (the [2, M] partial-dot layout callers sum)
+  int M, N, K, n_pad, n16, stages, num_tiles;
   uint32_t flags;
-  int tma_store;            // 1: epilogue stages 128x16 chunks in smem and writes them with TMA stores
+  int tma_store;            // 1: epilogue stages 64x16 chunks in smem and writes them with TMA stores
 };
 
-constexpr int kStageOutBytes = BM * 16 * 4 + 2 * BM * 16 * 2;   // per column-half: fp32 8 KB + hi 4 KB + lo 4 KB
-
-constexpr int kAccStride = 256;   // TMEM columns per accumulator buffer (two buffers -> 512 columns)
-
 // ---------------------------------------------------------------------------------------------------
-// the GEMM kernel: persistent over 128-row tiles; TMEM accumulators double-buffered so the epilogue of
-// tile i overlaps the TMA/MMA mainloop of tile i+1.
+// the GEMM kernel: persistent over 128-row tiles.  Warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 =
+// consumers: each issues wgmma for its 64 rows of the tile, holds the accumulator in registers and runs the epilogue.
+// The producer runs up to `stages` k-blocks ahead, so the next tile's loads overlap this tile's epilogue.
 // ---------------------------------------------------------------------------------------------------
 template <int CS, int BK>   // CS: CTAs per cluster sharing W tiles by multicast; BK: k-block width
 __global__ void __launch_bounds__(kThreads, 1)
@@ -117,24 +117,20 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
                  const __grid_constant__ CUtensorMap map_c, const __grid_constant__ CUtensorMap map_c_hi,
                  const __grid_constant__ CUtensorMap map_c_lo, const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages] x {A_hi 16K, A_lo 16K, W_hi n_pad*128, W_lo n_pad*128}, then barriers
+  // carve: [stages] x {A_hi, A_lo, W_hi, W_lo}, epilogue staging, barriers, bias / score weights
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int a_bytes = BM * BK * 2;            // 16384
-  const int w_bytes = p.n_pad * BK * 2;       // n_pad * 128
+  const int a_bytes = BM * BK * 2;
+  const int w_bytes = p.n_pad * BK * 2;
   // GR_LINEAR_BF16_SINGLE: bf16 activation storage -- one product A_hi W_hi, stages hold {A_hi, W_hi} only
   const bool single = (p.flags & GR_LINEAR_BF16_SINGLE) != 0;
   const int w_off = single ? a_bytes : 2 * a_bytes;          // W_hi tile inside a stage
   const int stage_bytes = single ? a_bytes + w_bytes : 2 * a_bytes + 2 * w_bytes;
-  // epilogue staging (TMA-store source, must be 128-byte aligned): right after the 1024-aligned stages
-  uint8_t* s_out = smem + (size_t)p.stages * stage_bytes;    // [2 halves] x {fp32 128x16, hi 128x16, lo 128x16}
+  uint8_t* s_out = smem + (size_t)p.stages * stage_bytes;    // [2 warpgroups] x kStageOutBytes (TMA-store source)
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_out + 2 * kStageOutBytes);
   uint64_t* full_bar = bars;                       // [stages]
   uint64_t* empty_bar = bars + p.stages;           // [stages]
-  uint64_t* tmem_full_bar = bars + 2 * p.stages;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-  float* s_bias = reinterpret_cast<float*>(tmem_slot + 4);   // [256] zero padded
-  float* s_ws = s_bias + 256;                                // [256] zero padded
+  float* s_bias = reinterpret_cast<float*>(bars + 2 * p.stages);   // [256] zero padded
+  float* s_ws = s_bias + 256;                                      // [256] zero padded
   for (int i = threadIdx.x; i < 256; i += kThreads) {
     s_bias[i] = (p.bias && i < p.N) ? p.bias[i] : 0.f;
     s_ws[i] = (p.w_score && i < p.N) ? p.w_score[i] : 0.f;
@@ -147,32 +143,20 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   const int ngroups = (p.num_tiles + CS - 1) / CS;       // tile groups: CS consecutive 128-row tiles
   constexpr uint16_t kMask = (uint16_t)((1u << CS) - 1);
 
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], CS);                      // every CTA of the cluster must release the slot
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], kEpiWarps);    // one arrive per epilogue warp
+      mbar_init(&empty_bar[s], kConsumerWarps * CS);     // every consumer warp of the cluster releases the slot
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  } else if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(2u * kAccStride)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
   if (CS > 1) cluster_sync_all();                        // all barriers of the cluster are initialised
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp == 0 && lane == 0) {
       uint32_t phase = 0;
       int s = 0;
       const int w_rows = p.n_pad / CS;                   // W rows this CTA fetches (and multicasts)
@@ -199,208 +183,100 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one thread) =====================
-    if (lane == 0) {
-      // instruction descriptor: D fp32, A/B bf16, both K-major, M = 128, N = n_pad
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.n_pad >> 3) << 17) |
-                             ((uint32_t)(BM >> 4) << 24);
-      uint32_t phase = 0;
-      int s = 0, it = 0;
-      for (int g = cid; g < ngroups; g += ncluster, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&tmem_empty_bar[acc], ((it >> 1) & 1) ^ 1);     // epilogue has drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * kAccStride);
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&full_bar[s], phase);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-          const uint64_t da_hi = make_smem_desc<BK>(sa), da_lo = make_smem_desc<BK>(sa + a_bytes);
-          const uint64_t dw_hi = make_smem_desc<BK>(sa + w_off);
-          const uint64_t dw_lo = make_smem_desc<BK>(sa + w_off + w_bytes);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t adv = (uint64_t)((k * UMMA_K * 2) >> 4);   // +32 B per K step inside the swizzle row
-            umma_bf16(tmem_d, da_hi + adv, dw_hi + adv, idesc, (kb | k) ? 1u : 0u);
-            if (!single) {
-              umma_bf16(tmem_d, da_hi + adv, dw_lo + adv, idesc, 1u);
-              umma_bf16(tmem_d, da_lo + adv, dw_hi + adv, idesc, 1u);
-            }
-          }
-          // free this smem stage (in every CTA of the cluster: their producers multicast into it)
-          if (CS == 1) umma_commit(&empty_bar[s]); else umma_commit_mc(&empty_bar[s], kMask);
-          if (++s == p.stages) { s = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full_bar[acc]);           // accumulator complete -> epilogue
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue: TMEM -> registers -> global =====================
-    // warp e = warp-4: TMEM lane quarter q = warp & 3 (hardware rule), column half = e >> 2
-    const int q = warp & 3, half = (warp - 4) >> 2;
-    const int row_in_tile = q * 32 + lane;
-    const bool relu = p.flags & GR_LINEAR_RELU;
-    const int nchunks = p.n_pad / 16;
-    const int ch_beg = half == 0 ? 0 : (nchunks + 1) / 2, ch_end = half == 0 ? (nchunks + 1) / 2 : nchunks;
-    const bool vec_ok = p.C && (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-    const bool vec16_ok = p.c_hi && (p.ldc16 % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.c_hi) & 7) == 0) &&
-                          ((reinterpret_cast<uintptr_t>(p.c_lo) & 7) == 0);
-    int it = 0;
-    for (int g = cid; g < ngroups; g += ncluster, ++it) {
+  } else {
+    // ===================== consumers: wgmma mainloop + epilogue =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    const int cw = (warp - 4) >> 2, wq = warp & 3;       // consumer warpgroup (row half), warp inside it
+    const int nc = (p.n_pad + 31) / 32;
+    const bool tail16 = (p.n_pad & 31) != 0;
+    const EpiOut e{s_bias, s_ws, (p.flags & GR_LINEAR_RELU) != 0};
+    const int r = wq * 16 + (lane >> 2), cq = lane & 3;
+    uint8_t* stg = s_out + (size_t)cw * kStageOutBytes;
+    const bool issuer = wq == 0 && lane == 0;
+    const bool vec_c = p.C && (p.ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+    const bool vec_h = p.c_hi && (p.ldc16 % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.c_hi) & 3) == 0) &&
+                       ((reinterpret_cast<uintptr_t>(p.c_lo) & 3) == 0);
+    uint32_t phase = 0;
+    int s = 0;
+    for (int g = cid; g < ngroups; g += ncluster) {
       const int tile = g * CS + crank;
-      const int acc = it & 1;
-      mbar_wait(&tmem_full_bar[acc], (it >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int64_t row = (int64_t)tile * BM + row_in_tile;
-      const bool row_ok = row < p.M;
-      float* crow = p.C ? p.C + row * p.ldc : nullptr;
-      __nv_bfloat16* hrow = p.c_hi ? p.c_hi + row * p.ldc16 : nullptr;
-      __nv_bfloat16* lrow = p.c_hi ? p.c_lo + row * p.ldc16 : nullptr;
-      float dot = 0.f;
-      const uint32_t taddr = tmem_base + (uint32_t)(acc * kAccStride) + ((uint32_t)(q * 32) << 16);
-      if (p.tma_store) {
-        // ---- staged epilogue: 128x16 chunk -> smem (dense rows) -> TMA store (clips rows >= M, cols >= N)
-        uint8_t* stg = s_out + (size_t)half * kStageOutBytes;
-        float* s_c = reinterpret_cast<float*>(stg) + row_in_tile * 16;
-        uint32_t* s_h = reinterpret_cast<uint32_t*>(stg + BM * 16 * 4) + row_in_tile * 8;
-        uint32_t* s_l = reinterpret_cast<uint32_t*>(stg + BM * 16 * 4 + BM * 16 * 2) + row_in_tile * 8;
-        const bool issuer = (warp == 4 + 4 * half) && lane == 0;
-        for (int ch = ch_beg; ch < ch_end; ++ch) {
-          const int c0 = ch * 16;
-          uint32_t r[16];
-          tmem_ld16(taddr + (uint32_t)c0, r);
-          if (ch == ch_end - 1) {        // last TMEM read of this tile: hand the accumulator back early
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-          }
-          float v[16];
+      float acc[kMaxChunks][16];
 #pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 b4 = *reinterpret_cast<const float4*>(s_bias + c0 + j);
-            const float4 w4 = *reinterpret_cast<const float4*>(s_ws + c0 + j);
-            float x0 = __uint_as_float(r[j]) + b4.x, x1 = __uint_as_float(r[j + 1]) + b4.y;
-            float x2 = __uint_as_float(r[j + 2]) + b4.z, x3 = __uint_as_float(r[j + 3]) + b4.w;
-            if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f); }
-            dot = fmaf(x0, w4.x, dot); dot = fmaf(x1, w4.y, dot);
-            dot = fmaf(x2, w4.z, dot); dot = fmaf(x3, w4.w, dot);
-            v[j] = x0; v[j + 1] = x1; v[j + 2] = x2; v[j + 3] = x3;
-          }
-          uint32_t h[8], l[8];
+      for (int j = 0; j < kMaxChunks; ++j)
 #pragma unroll
-          for (int j = 0; j < 16; j += 2) {
-            const __nv_bfloat162 h2 = __floats2bfloat162_rn(v[j], v[j + 1]);
-            const float2 hf = __bfloat1622float2(h2);
-            const __nv_bfloat162 l2 = __floats2bfloat162_rn(v[j] - hf.x, v[j + 1] - hf.y);
-            h[j / 2] = *reinterpret_cast<const uint32_t*>(&h2);
-            l[j / 2] = *reinterpret_cast<const uint32_t*>(&l2);
-          }
-          // the previous chunk's TMA stores must have finished READING the staging buffer
-          if (issuer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-          named_bar_sync(1 + half, 128);
-          if (p.C) {
-#pragma unroll
-            for (int j = 0; j < 16; j += 4)
-              *reinterpret_cast<float4*>(s_c + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-          }
-          if (p.c_hi) {
-            *reinterpret_cast<uint4*>(s_h) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4*>(s_h + 4) = make_uint4(h[4], h[5], h[6], h[7]);
-            *reinterpret_cast<uint4*>(s_l) = make_uint4(l[0], l[1], l[2], l[3]);
-            *reinterpret_cast<uint4*>(s_l + 4) = make_uint4(l[4], l[5], l[6], l[7]);
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          named_bar_sync(1 + half, 128);
-          if (issuer) {
-            const int m0 = tile * BM;
-            if (p.C) tma_store_2d(&map_c, stg, c0, m0);
-            if (p.c_hi) {
-              tma_store_2d(&map_c_hi, stg + BM * 16 * 4, c0, m0);
-              tma_store_2d(&map_c_lo, stg + BM * 16 * 4 + BM * 16 * 2, c0, m0);
-            }
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          }
-        }
-        if (p.dots && row_ok) p.dots[(int64_t)half * p.M + row] = dot;
-        continue;
+        for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full_bar[s], phase);
+        const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+        const uint32_t a_row = (uint32_t)(cw * WG_M * BK * 2);
+        mma_kblock<kMaxChunks, BK>(acc, make_smem_desc<BK>(sa + a_row), make_smem_desc<BK>(sa + a_bytes + a_row),
+                                   make_smem_desc<BK>(sa + w_off), make_smem_desc<BK>(sa + w_off + w_bytes),
+                                   BK / MMA_K, nc, single, tail16);
+        wgmma_wait<1>();                                 // the previous k-block's products are done: free its slot
+        if (prev >= 0 && lane == 0) release_slot<CS>(&empty_bar[prev]);
+        prev = s;
+        if (++s == p.stages) { s = 0; phase ^= 1; }
       }
-      for (int ch = ch_beg; ch < ch_end; ++ch) {
-        const int c0 = ch * 16;
-        uint32_t r[16];
-        tmem_ld16(taddr + (uint32_t)c0, r);
-        float v[16];
+      wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) release_slot<CS>(&empty_bar[prev]);
+
+      const int64_t row0 = (int64_t)tile * BM + cw * WG_M + r;
+      float dot0 = 0.f, dot1 = 0.f;
 #pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          // columns >= N: accumulator 0 (zero-filled W rows), bias 0, score weight 0 -> contribute 0
-          const float4 b4 = *reinterpret_cast<const float4*>(s_bias + c0 + j);
-          const float4 w4 = *reinterpret_cast<const float4*>(s_ws + c0 + j);
-          float x0 = __uint_as_float(r[j]) + b4.x, x1 = __uint_as_float(r[j + 1]) + b4.y;
-          float x2 = __uint_as_float(r[j + 2]) + b4.z, x3 = __uint_as_float(r[j + 3]) + b4.w;
-          if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f); }
-          dot = fmaf(x0, w4.x, dot); dot = fmaf(x1, w4.y, dot);
-          dot = fmaf(x2, w4.z, dot); dot = fmaf(x3, w4.w, dot);
-          v[j] = x0; v[j + 1] = x1; v[j + 2] = x2; v[j + 3] = x3;
-        }
-        if (row_ok) {
-          const bool full = c0 + 16 <= p.N;
-          if (crow) {
-            if (vec_ok && full) {
+      for (int j = 0; j < kMaxChunks; ++j) {
 #pragma unroll
-              for (int j = 0; j < 16; j += 4)
-                *reinterpret_cast<float4*>(crow + c0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (c0 + j < p.N) crow[c0 + j] = v[j];
-            }
+        for (int h = 0; h < 2; ++h) {
+          const int c0 = 32 * j + 16 * h;
+          if (j >= nc || c0 >= p.n_pad) continue;
+          float v[8];
+          epi_values(acc[j], h, c0, cq, e, v, dot0, dot1);
+          if (p.tma_store) {
+            epi_store_tma(v, stg, r, cq, issuer, 1 + cw, &map_c, &map_c_hi, &map_c_lo, p.C != nullptr,
+                          p.c_hi != nullptr, c0, tile * BM + cw * WG_M);
+            continue;
           }
-          if (hrow) {
-            uint32_t h[8], l[8];
 #pragma unroll
-            for (int j = 0; j < 16; j += 2) {
-              const __nv_bfloat162 h2 = __floats2bfloat162_rn(v[j], v[j + 1]);
-              const float2 hf = __bfloat1622float2(h2);
-              const __nv_bfloat162 l2 = __floats2bfloat162_rn(v[j] - hf.x, v[j + 1] - hf.y);
-              h[j / 2] = *reinterpret_cast<const uint32_t*>(&h2);
-              l[j / 2] = *reinterpret_cast<const uint32_t*>(&l2);
-            }
-            if (vec16_ok && full) {
+          for (int b = 0; b < 2; ++b) {
+            const int col = c0 + 8 * b + 2 * cq;
 #pragma unroll
-              for (int j = 0; j < 8; j += 2) {
-                *reinterpret_cast<uint2*>(hrow + c0 + 2 * j) = make_uint2(h[j], h[j + 1]);
-                *reinterpret_cast<uint2*>(lrow + c0 + 2 * j) = make_uint2(l[j], l[j + 1]);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (c0 + j < p.N) {
-                  const uint32_t hw = h[j / 2], lw = l[j / 2];
-                  reinterpret_cast<unsigned short*>(hrow)[c0 + j] = (unsigned short)((j & 1) ? (hw >> 16) : (hw & 0xFFFF));
-                  reinterpret_cast<unsigned short*>(lrow)[c0 + j] = (unsigned short)((j & 1) ? (lw >> 16) : (lw & 0xFFFF));
+            for (int hr = 0; hr < 2; ++hr) {
+              const int64_t row = row0 + 8 * hr;
+              if (row >= p.M) continue;
+              const float x0 = v[4 * b + 2 * hr], x1 = v[4 * b + 2 * hr + 1];
+              if (p.C) {
+                float* c = p.C + row * p.ldc + col;
+                if (vec_c && col + 1 < p.N) {
+                  *reinterpret_cast<float2*>(c) = make_float2(x0, x1);
+                } else {
+                  if (col < p.N) c[0] = x0;
+                  if (col + 1 < p.N) c[1] = x1;
                 }
+              }
+              if (p.c_hi) {
+                // the planes also receive the (exactly zero) columns N .. n16
+                uint32_t lo;
+                const uint32_t hi = split_hi_lo(x0, x1, lo);
+                unsigned short* ph = reinterpret_cast<unsigned short*>(p.c_hi + row * p.ldc16 + col);
+                unsigned short* pl = reinterpret_cast<unsigned short*>(p.c_lo + row * p.ldc16 + col);
+                if (vec_h && col + 1 < p.n16) {
+                  *reinterpret_cast<uint32_t*>(ph) = hi;
+                  *reinterpret_cast<uint32_t*>(pl) = lo;
+                } else {
+                  if (col < p.n16) { ph[0] = (unsigned short)(hi & 0xFFFF); pl[0] = (unsigned short)(lo & 0xFFFF); }
+                  if (col + 1 < p.n16) { ph[1] = (unsigned short)(hi >> 16); pl[1] = (unsigned short)(lo >> 16); }
+                }
+              }
             }
           }
         }
       }
-      if (p.dots && row_ok) p.dots[(int64_t)half * p.M + row] = dot;
-      // release the accumulator to the MMA warp
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
+      epi_dots(dot0, dot1, p.dots, row0, p.M, cq);
     }
-    if (p.tma_store && lane == 0 && (warp == 4 || warp == 8))
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // outstanding TMA stores complete
+    if (p.tma_store && issuer) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores complete
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
   if (CS > 1) cluster_sync_all();   // nobody exits while a peer may still multicast into / arrive on this CTA
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(2u * kAccStride)
-                 : "memory");
-  }
 }
 
 struct TcPlan {
@@ -418,17 +294,18 @@ TcPlan plan_tc(int64_t M, int64_t N, int64_t K, bool single = false) {
   t.n_pad = (int)((N + 15) / 16 * 16);
   const size_t stage = (single ? 1 : 2) * ((size_t)BM * BK * 2 + (size_t)t.n_pad * BK * 2);
   // 227 KB usable smem minus alignment slack, bias/score arrays, barriers and the epilogue staging buffers
-  int stages = (int)((227 * 1024 - 1024 - 2048 - 256 - 2 * kStageOutBytes) / stage);
+  int stages = (int)((227 * 1024 - 1024 - 2048 - 128 - 2 * kStageOutBytes) / stage);
   t.stages = stages > 8 ? 8 : stages;
   if (t.stages < 2) t.ok = false;
   t.bk = BK;
-  t.smem_bytes = (size_t)t.stages * stage + 1024 /*align slack*/ + (2 * t.stages + 4) * 8 + 16 + 2 * 256 * 4 + 2 * kStageOutBytes;
+  t.smem_bytes = (size_t)t.stages * stage + 1024 /*align slack*/ + 2 * t.stages * 8 + 2 * 256 * 4 + 2 * kStageOutBytes;
   t.a_plane_bytes = align_up((size_t)M * t.kp * 2, 256);
   t.w_plane_bytes = align_up((size_t)N * t.kp * 2, 256);
   t.total_bytes = 2 * t.a_plane_bytes + 2 * t.w_plane_bytes;
   t.w_only_bytes = 2 * t.w_plane_bytes;
   return t;
 }
+
 
 int split_launch(const float* A, int64_t lda, int64_t M, int64_t K, __nv_bfloat16* hi, __nv_bfloat16* lo,
                  int64_t ldo, cudaStream_t stream) {
@@ -450,6 +327,18 @@ int launch_tc_cs(const CUtensorMap& m_a_hi, const CUtensorMap& m_a_lo, const CUt
   if (first_use_on_device(attr_done)) {
     GR_CHECK_CUDA(cudaFuncSetAttribute(linear_tc_kernel<CS, BK>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  }
+  // setmaxnreg.inc only draws on registers the CTA was launched with: the budget needs exactly kLaunchRegs
+  static int num_regs = 0;
+  if (num_regs == 0) {
+    cudaFuncAttributes fa{};
+    GR_CHECK_CUDA(cudaFuncGetAttributes(&fa, linear_tc_kernel<CS, BK>));
+    num_regs = fa.numRegs;
+  }
+  if (num_regs != kLaunchRegs) {
+    set_error("gr_linear_tc: kernel was compiled with %d registers per thread, the warpgroup budget needs %d",
+              num_regs, kLaunchRegs);
+    return GR_ERR_UNSUPPORTED;
   }
   const int ngroups = (p.num_tiles + CS - 1) / CS;
   const int nclusters = std::max(1, std::min(ngroups, sm_count() / CS));
@@ -485,15 +374,15 @@ int launch_tc(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int64_t lda1
               "multiples of 8 elements)");
     return GR_ERR_CUDA;
   }
+  // the planes also receive the (exactly zero) columns N .. round16(N): whole 32-byte sectors per row
+  p.n16 = (int)std::min<int64_t>((p.N + 15) / 16 * 16, p.ldc16);
   // output tensor maps for the staged TMA-store epilogue (need 16-byte aligned bases and row pitches)
   CUtensorMap m_c, m_c_hi, m_c_lo;
   memset(&m_c, 0, sizeof(m_c)); memset(&m_c_hi, 0, sizeof(m_c_hi)); memset(&m_c_lo, 0, sizeof(m_c_lo));
   bool ok = g_tc_tma_store != 0;
   if (ok && p.C) ok = make_out_tmap(&m_c, p.C, p.M, p.N, p.ldc, 4);
-  // the planes also receive the (exactly zero) columns N .. round16(N): whole 32-byte sectors per row
-  const int64_t n16 = std::min<int64_t>((p.N + 15) / 16 * 16, p.ldc16);
-  if (ok && p.c_hi) ok = make_out_tmap(&m_c_hi, p.c_hi, p.M, n16, p.ldc16, 2) &&
-                         make_out_tmap(&m_c_lo, p.c_lo, p.M, n16, p.ldc16, 2);
+  if (ok && p.c_hi) ok = make_out_tmap(&m_c_hi, p.c_hi, p.M, p.n16, p.ldc16, 2) &&
+                         make_out_tmap(&m_c_lo, p.c_lo, p.M, p.n16, p.ldc16, 2);
   p.tma_store = ok ? 1 : 0;
   if (t.bk == 64) {
     if (cs == 2) return launch_tc_cs<2, 64>(m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, t, p, stream);

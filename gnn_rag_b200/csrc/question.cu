@@ -2,7 +2,7 @@
 //
 // These are the O(B*D^2) pieces between the graph layers: the instruction generator, the instruction reform
 // after every iteration and the evaluation loss / argmax.  In the reference each is a chain of 10-20 tiny torch
-// ops on [B, D] tensors; at B200 speeds the chain is pure launch latency (~230 launches per forward), so each
+// ops on [B, D] tensors; on a GPU the chain is pure launch latency (~230 launches per forward), so each
 // chain is one kernel here.
 //   gr_instructions   BaseInstruction.get_instruction x num_ins
 //                     (gnn/modules/question_encoding/base_encoder.py:73-114, lstm_encoder.py:38-45)
@@ -179,7 +179,7 @@ __global__ void __launch_bounds__(kQThreads) query_reform_kernel(const ReformPar
   __shared__ float s_val[kQThreads];
   __shared__ int s_woff[kQThreads / 32 + 1];
   // grid (B, S): CTA (b, s) owns output columns [d0, d1) of question b's new instructions (the seed pick is cheap and
-  // repeated by every slice); 4 x as many CTAs as questions: the one-CTA-per-question version occupied 64 of 148 SMs
+  // repeated by every slice); 4 x as many CTAs as questions: the one-CTA-per-question version left most SMs idle
   const int D = p.D, N = p.N, b = blockIdx.x, tid = threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
   const int dper = (D + gridDim.y - 1) / gridDim.y;

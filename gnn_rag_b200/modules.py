@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's ``gnn/modules`` for the retrieval hot path.
 
 Same class names, constructor arguments and parameter names as the reference so a reference
-``state_dict`` loads unchanged (SURVEY.md 8b), but the graph work runs in the hand-written sm_100a kernels
+``state_dict`` loads unchanged (SURVEY.md 8b), but the graph work runs in the hand-written sm_90a kernels
 behind the C ABI (ops.py) instead of ``index_select`` / ``Linear``-over-facts / ``torch.sparse.mm``:
 
   TypeLayer          gnn/modules/layer_init.py:8-65
@@ -276,7 +276,7 @@ class _GraphLayerBase(nn.Module):
     the aggregation kernel writes straight into its slot.  Two storage modes:
 
       planes (default): the matrix is kept as split-bf16 hi/lo planes (hi + lo = value to 2^-18), which is
-          the A-operand layout of the tcgen05 e2e GEMM; h additionally lives in fp32 ``h32`` [B*N, D].
+          the A-operand layout of the wgmma e2e GEMM; h additionally lives in fp32 ``h32`` [B*N, D].
       fp32: ping-pong fp32 buffers X[2] feeding the exact-fp32 SIMT linear (ops.TC_LINEAR = False)."""
 
     _plane_cache = {}     # (device, Nt, Kp) -> zero-initialised ping-pong planes, reused across forwards
@@ -288,7 +288,7 @@ class _GraphLayerBase(nn.Module):
         self.Kd = Kd
         if self.use_planes:
             # every segment ([h | nb_0 | nb_1 ...], D columns each) starts on a 32-byte sector: pitch = D rounded
-            # up to 16 bf16 columns (a 16-byte-misaligned segment start halves HBM write throughput on B200);
+            # up to 16 bf16 columns (a 32-byte-sector-aligned segment start keeps the plane writes whole sectors);
             # padding columns stay zero forever (nothing writes them), so the padded GEMM is exact
             self.Dp = (D + 15) // 16 * 16
             self.Kpad = Kd // D * self.Dp

@@ -1,5 +1,5 @@
 """Tensor-level wrappers over the C ABI (include/gnnrag_b200.h): torch CUDA tensors in, torch CUDA tensors
-out.  torch is used for device memory and streams only; every op below launches our own sm_100a kernels.
+out.  torch is used for device memory and streams only; every op below launches our own sm_90a kernels.
 All ops raise if handed a CPU tensor -- there is no CPU fallback on the product path."""
 import ctypes
 import weakref
@@ -190,11 +190,11 @@ def linear(A, W, bias=None, relu=False, out=None, addend=None, addend_rows=0, ex
     return out
 
 
-TC_LINEAR = True       # route the big e2e linears through the tcgen05 split-bf16 kernel (models use this)
+TC_LINEAR = True       # route the big e2e linears through the wgmma split-bf16 kernel (models use this)
 
 
 def linear_tc(A, W, bias=None, relu=False, out=None):
-    """Tensor-core (tcgen05, split-bf16 x3) version of :func:`linear` for 8 <= N <= 256."""
+    """Tensor-core (wgmma, split-bf16 x3) version of :func:`linear` for 8 <= N <= 256."""
     A, W = _cuda(A, torch.float32, "A"), _cuda(W, torch.float32, "W")
     M, K = A.shape
     N = W.shape[0]
@@ -213,7 +213,7 @@ def linear_tc(A, W, bias=None, relu=False, out=None):
 
 
 def rel_linear(A, W, bias=None, addend=None, addend_rows=0):
-    """Hoisted relation projection table = A W^T + b (+ pos_emb rows): tcgen05 split-bf16 path when enabled
+    """Hoisted relation projection table = A W^T + b (+ pos_emb rows): wgmma split-bf16 path when enabled
     (fp32-class accuracy, ~3x faster than the SIMT kernel at [6107 x 200 x 200]); the optional pos_emb addend
     keeps the exact SIMT kernel."""
     if TC_LINEAR and addend is None and 8 <= W.shape[0] <= 256 and W.shape[1] >= 8:
@@ -222,7 +222,7 @@ def rel_linear(A, W, bias=None, addend=None, addend_rows=0):
 
 
 def e2e_linear(A, W, bias, out):
-    """relu(A W^T + b) for the node-update GEMM: tcgen05 path when enabled and the shape fits."""
+    """relu(A W^T + b) for the node-update GEMM: wgmma path when enabled and the shape fits."""
     if TC_LINEAR and 8 <= W.shape[0] <= 256 and W.shape[1] >= 8:
         return linear_tc(A, W, bias, relu=True, out=out)
     return linear(A, W, bias, relu=True, out=out)
@@ -342,8 +342,8 @@ def aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, out_col0, seg_pitc
 
 
 FUSED_LAYER = True      # dense-prior ReaRev layers: aggregation fused into the e2e GEMM (csrc/fused_layer.cu)
-FUSED_MIN_ROWS = 148 * 128   # below one 128-row tile per SM the fused kernel's serial per-tile chain (35 dependent k-blocks)
-                             # loses to the two wide kernels (cfg1: 0.853 vs 0.836 ms per step)
+FUSED_MIN_ROWS = 132 * 128   # below one 128-row tile per SM the fused kernel's serial per-tile chain (35 dependent k-blocks)
+                             # loses to the two wide kernels
 
 
 def fused_layer_supported(N, D, seg_pitch, I, n_out):
@@ -489,13 +489,13 @@ def live_weight_workspaces():
     return [e[0] for e in _W_CACHE.values()] + [t for e in _P_CACHE.values() for t in e[:2]]
 
 
-TC_MAX_N = 256         # output columns of one tcgen05 GEMM launch (one TMEM accumulator buffer)
+TC_MAX_N = 256         # output columns of one wgmma GEMM launch (the register accumulator of a consumer warpgroup)
 TC_MAX_N_SPLIT = 512   # wider outputs are tiled over N: one launch per <= 256-column slice of W
 
 
 def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=None, dots=None, relu=True,
                      k_seg=0, k_seg_pitch=0, single_ok=False):
-    """tcgen05 split-bf16 GEMM whose A operand already lives in bf16 hi/lo planes [M, >=K].
+    """wgmma split-bf16 GEMM whose A operand already lives in bf16 hi/lo planes [M, >=K].
     ``single_ok``: this call may run as ONE bf16 product when ``ACT_BF16`` is on (the node-update GEMMs; the small
     relation-table GEMMs always keep the three-product fp32-class path).
     Writes any of: fp32 ``out`` [M,N]; ``out_planes`` (hi, lo) [M, >=N] (next layer's h columns);
@@ -572,7 +572,7 @@ def _tc_ok(n_out, k_in):
 
 def rel_features_from_embeddings(embs, W, bias):
     """relation_linear applied to the relation embedding table(s) (rearev.py:91-99 / nsm.py:97-104):
-    one tcgen05 GEMM per direction straight into the stacked planes (no fp32 round trip)."""
+    one wgmma GEMM per direction straight into the stacked planes (no fp32 round trip)."""
     R1, K = embs[0].shape
     D = W.shape[0]
     planes = _tc_ok(D, K) and _tc_ok(D, D)

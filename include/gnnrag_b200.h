@@ -1,5 +1,5 @@
 /*
- * gnnrag_b200.h -- C ABI of libgnnrag_b200.so: the B200 (sm_100a) implementation of GNN-RAG's GNN
+ * gnnrag_b200.h -- C ABI of libgnnrag_b200.so: the H100 (sm_90a) implementation of GNN-RAG's GNN
  * retrieval hot path (ReaRev / NSM multi-hop message passing + answer scoring + candidate ranking).
  *
  * The reference (cmavro/GNN-RAG) has no FFI; its boundary is the Python nn.Module contract that
@@ -54,8 +54,8 @@ typedef enum gr_status {
 int gr_abi_version(void);
 const char* gr_last_error(void);
 /* runtime switches: "agg_tma" (0|1: stage CSR slices with bulk TMA copies), "linear_tc" (0|1: split-bf16
- * tcgen05 GEMM for gr_linear when the shape allows), "tc_cluster" (1|2: CTAs per cluster that share the W
- * tiles of the tcgen05 GEMM through TMA multicast), "agg_abs_ws" (0|1: persistent warp-specialised build of the |v| aggregation
+ * wgmma GEMM for gr_linear when the shape allows), "tc_cluster" (1|2: CTAs per cluster that share the W
+ * tiles of the wgmma GEMM through TMA multicast), "agg_abs_ws" (0|1: persistent warp-specialised build of the |v| aggregation
  * kernel).  Process-wide; set before launching work. */
 int gr_set_option(const char* name, int64_t value);
 static inline int64_t gr_pad4(int64_t n) { return (n + 3) & ~(int64_t)3; }
@@ -98,8 +98,8 @@ int gr_linear(const float* A, int64_t lda, const float* W, int64_t ldw, const fl
               float* C, int64_t ldc, int64_t M, int64_t N, int64_t K, uint32_t flags, void* stream);
 
 /* Tensor-core variant of gr_linear for the big e2e_linear GEMMs (reasongnn.py:163, nsm_gnn.py:63):
- * fp32 in / fp32 out with fp32-class accuracy through the 3-product split-bf16 scheme on tcgen05
- * (x = hi + lo in bf16; A W^T ~= A_hi W_hi^T + A_hi W_lo^T + A_lo W_hi^T, fp32 accumulation in TMEM,
+ * fp32 in / fp32 out with fp32-class accuracy through the 3-product split-bf16 scheme on wgmma
+ * (x = hi + lo in bf16; A W^T ~= A_hi W_hi^T + A_hi W_lo^T + A_lo W_hi^T, fp32 accumulation in registers,
  * dropped term <= 2^-18 relative).  Persistent, TMA-fed 128 x N tiles over 32- or 64-column k-blocks ("tc_bk"),
  * W shared across a CTA pair by TMA multicast ("tc_cluster"), TMA-store epilogue ("tc_tma_store").  Requires
  * 8 <= N <= 256.  The workspace (256-byte aligned, gr_linear_tc_workspace_bytes) holds the bf16 planes.
@@ -113,7 +113,7 @@ int gr_linear_tc(const float* A, int64_t lda, const float* W, int64_t ldw, const
  * C_hi/C_lo (row stride ldc16) = the node-embedding columns of the NEXT layer's A operand; and
  * dots (float[2*M]): the score_func dot product (reasongnn.py:165) fused into the epilogue as two partial
  * sums over the lower / upper half of the output columns, dots[m] + dots[M+m] = sum_n C[m,n] * w_score[n]
- * (gr_masked_softmax adds them).  Persistent kernel, TMEM accumulators double-buffered (epilogue overlaps the next tile).
+ * (gr_masked_softmax adds them).  Persistent kernel, register accumulators (the producer loads the next tile during the epilogue).
  * Segmented K: when k_seg_pitch > k_seg > 0 the A planes hold K/k_seg_pitch segments of k_seg valid columns
  * at pitch k_seg_pitch (zero padding in between) while W is the dense [N, (K/k_seg_pitch)*k_seg] torch weight;
  * the W planes are built in the padded layout.  K is the padded length.
@@ -146,7 +146,7 @@ int gr_split_bf16(const float* A, int64_t lda, int64_t M, int64_t K, void* hi, v
  *     inverse  (head CSR, table_inv) -> columns out_col0 + (2j+1)*D
  * which is the concat order of ReasonGNNLayer.forward (reasongnn.py:150-161).  seg_pitch (0 = D) is the
  * column distance between consecutive segments: the bf16 planes use a pitch rounded up to 16 columns so that
- * every segment starts on a 32-byte sector (measured on B200: a 16-byte-misaligned segment start halves the
+ * every segment starts on a 32-byte sector (a 16-byte-misaligned segment start splits the
  * achievable write bandwidth, scripts/agg_probe.py).
  *
  * Split-bf16 planes (optional, gr_aggregate_dual / gr_type_layer): when out_hi/out_lo are non-NULL the
@@ -186,7 +186,7 @@ int gr_aggregate_dual(const int32_t* rowptr_t, const int32_t* src_t, const int32
 /* Specialised variant of gr_aggregate_dual for the hot shape (csrc/aggregate_abs.cu).  The hoisted relation table is
  * copied once per layer into a zero-padded 256-column layout (gr_pad_table256: table [rows, D] fp32, row stride ldt
  * -> out [rows][256] fp32, 16-byte aligned) so every lane of the gather is in-bounds, and the edge loop accumulates
- * sum c*v and sum c*|v| (|.| is a free FFMA2 source modifier on sm_100) instead of taking relu of every gathered
+ * sum c*v and sum c*|v| (|.| is a free FFMA source modifier) instead of taking relu of every gathered
  * element: sum c*relu(+-v) = (Q +- S)/2.  Output: the split-bf16 planes only.  This build specialises D = 200,
  * seg_pitch = 208, N >= 64 (gr_aggregate_dual_abs_supported); other shapes use gr_aggregate_dual.
  * Same reference lines: reasongnn.py:61-116. */
@@ -206,7 +206,7 @@ int gr_aggregate_dual_abs(const int32_t* rowptr_t, const int32_t* src_t, const i
 
 /* One dense-prior ReaRev layer as ONE kernel (csrc/fused_layer.cu): the aggregation of both directions and all
  * instructions (reason_layer / reason_layer_inv, reasongnn.py:61-116) is produced straight into the shared-memory
- * operand slots of the tcgen05 e2e GEMM (torch.cat + e2e_linear + relu, reasongnn.py:158-163; score_func dot :165), so
+ * operand slots of the wgmma e2e GEMM (torch.cat + e2e_linear + relu, reasongnn.py:158-163; score_func dot :165), so
  * the 2*I neighbour segments never reach HBM.  Replaces the pair gr_aggregate_dual_abs -> gr_linear_tc_planes.
  *   h_hi / h_lo    bf16 planes of the layer input h: [B*N, >= seg_pitch] with row stride ldh16 (only the first
  *                  seg_pitch columns are read; columns D .. seg_pitch-1 must be zero)
@@ -285,7 +285,7 @@ int gr_masked_softmax(const float* dots, const float* dots2, const float* b_scor
 
 /* ------------------------------------------------------------------------------------------------
  * Question-side updates, one CTA per question (csrc/question.cu).  In the reference each is a chain of 10-20
- * tiny torch ops on [B, D] tensors; fused here because at B200 speeds they are pure launch latency.
+ * tiny torch ops on [B, D] tensors; fused here because on a GPU they are pure launch latency.
  * Pointer arrays named *_host are HOST arrays of device pointers (one per instruction, <= 8).
  *
  * gr_instructions: LSTMInstruction.forward after the encoder (gnn/modules/question_encoding/

@@ -66,9 +66,11 @@ names = ["MMA loop total", "MMA wait W", "MMA wait aggregated operand", "MMA wai
 for label, bits in (("full", 32), ("no agg work", 33), ("no staging", 34), ("no agg, no staging", 35), ("bare (31)", 63)):
     ops.set_option("fused_debug", bits)
     flush.fill_(1); run(False); torch.cuda.synchronize()
-    buf = (ctypes.c_ulonglong * (148 * 16))()
-    _lib.check(_lib.load().gr_fused_profile_read(ctypes.cast(buf, ctypes.c_void_p), 148 * 16))
-    a = np.array(list(buf), dtype=np.float64).reshape(148, 16) / 1.965e3      # -> us at 1965 MHz
+    nsm = torch.cuda.get_device_properties(0).multi_processor_count
+    mhz = torch.cuda.get_device_properties(0).clock_rate / 1e3
+    buf = (ctypes.c_ulonglong * (nsm * 16))()
+    _lib.check(_lib.load().gr_fused_profile_read(ctypes.cast(buf, ctypes.c_void_p), nsm * 16))
+    a = np.array(list(buf), dtype=np.float64).reshape(nsm, 16) / mhz      # -> us at the SM clock
     print("--", label)
     print("   " + " | ".join("%s %.0f" % (n, a[:, i].mean()) for i, n in enumerate(names)))
 ops.set_option("fused_debug", 0)

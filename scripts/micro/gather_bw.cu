@@ -1,5 +1,5 @@
 // Micro-benchmark: how fast can 800-byte rows of a 12.5 MB table (L2 resident) be gathered at random by all SMs?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gather_bw gather_bw.cu && ./gather_bw
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_bw gather_bw.cu && ./gather_bw
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -100,7 +100,7 @@ int main() {
            cudaGetErrorString(cudaGetLastError()));
   };
   for (int wps : {16, 32, 48, 64}) {
-    const int threads = 256, blocks = 148 * wps / 8;
+    const int threads = 256, blocks = 132 * wps / 8;   // one wave on the 132 SMs of an H100 SXM
     char nm[64];
     snprintf(nm, 64, "ldg U=1 warps/SM=%d", wps); time([&] { gather_ldg<1><<<blocks, threads>>>(tab, rel, E, out); }, nm);
     snprintf(nm, 64, "ldg U=2 warps/SM=%d", wps); time([&] { gather_ldg<2><<<blocks, threads>>>(tab, rel, E, out); }, nm);

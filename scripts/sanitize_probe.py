@@ -1,5 +1,5 @@
 """Small D=200 ReaRev forward + ranking (every kernel of the hot path incl. the persistent aggregation kernel, the
-cluster LSTM, the frontier fix-up and the tcgen05 GEMM) -- run under compute-sanitizer:
+cluster LSTM, the frontier fix-up and the wgmma GEMM) -- run under compute-sanitizer:
     compute-sanitizer --tool memcheck  python scripts/sanitize_probe.py
     compute-sanitizer --tool racecheck python scripts/sanitize_probe.py"""
 import sys

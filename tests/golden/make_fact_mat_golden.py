@@ -10,7 +10,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
-from loader_fixture import CASES, FakeLoader  # noqa: E402
+from loader_fixture import CASES, FakeLoader, live_cases  # noqa: E402
 from oracle import ref_harness  # noqa: E402
 
 
@@ -28,4 +28,14 @@ if __name__ == "__main__":
         h, r, t, b, f, w, wr = fn(ld, ids, dropout)
         np.savez(os.path.join(HERE, "loader", "fact_mat_%s.npz" % name), heads=h, rels=r, tails=t, batch_ids=b, fact_ids=f,
                  weight_list=np.asarray(w, dtype=np.float64), weight_rel_list=np.asarray(wr, dtype=np.float64))
+        print(name, len(h), "facts")
+    # the larger states: compressed, indices as int32 (the tests compare values and dtype kinds)
+    for name, (kw, ids, dropout, seed) in live_cases().items():
+        ld = FakeLoader(**kw)
+        np.random.seed(seed)
+        h, r, t, b, f, w, wr = fn(ld, ids, dropout)
+        np.savez_compressed(os.path.join(HERE, "loader", "fact_mat_%s.npz" % name),
+                            **{k: np.asarray(v, dtype=np.int32) for k, v in
+                               dict(heads=h, rels=r, tails=t, batch_ids=b, fact_ids=f).items()},
+                            weight_list=np.asarray(w, dtype=np.float64), weight_rel_list=np.asarray(wr, dtype=np.float64))
         print(name, len(h), "facts")

@@ -1,5 +1,5 @@
 """Hot-shape goldens from the UNMODIFIED reference (cmavro/GNN-RAG @ /root/reference): entity_dim 200 with N >= 64 --
-the only shapes that reach the |v|-accumulating aggregation kernel, the K = 1040 tcgen05 GEMM and the frontier path --
+the only shapes that reach the |v|-accumulating aggregation kernel, the K = 1040 tensor-core GEMM and the frontier path --
 plus the FULL-SIZE cfg2 batch (B = 64, the configuration bench.py times) and the cfg5 stress graph.  Weights are
 ``synthetic.seeded_state_dict`` (rebuilt by the tests), so the files hold reference OUTPUTS only.  Build container only:
 

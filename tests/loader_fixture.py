@@ -34,3 +34,14 @@ CASES = {   # name -> (loader kwargs, sample_ids, fact_dropout, numpy seed)
     "empty_questions": (dict(seed=4, num_questions=5, max_local_entity=6, num_kb_relation=4, facts_hi=1),
                         [0, 1, 2, 3, 4], 0.5, 14),
 }
+
+
+def live_cases():
+    """Larger random loader states: name -> (loader kwargs, sample_ids, fact_dropout, numpy seed)."""
+    out = {}
+    for seed, (nq, nmax, nrel, lo, hi, dropout) in enumerate([(12, 300, 50, 100, 900, 0.0),
+                                                               (20, 500, 200, 0, 1500, 0.25)]):
+        kw = dict(seed=100 + seed, num_questions=nq, max_local_entity=nmax, num_kb_relation=nrel, facts_lo=lo,
+                  facts_hi=hi)
+        out["live%d" % seed] = (kw, list(np.random.RandomState(seed).permutation(nq)), dropout, 7 + seed)
+    return out

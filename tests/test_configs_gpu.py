@@ -291,14 +291,14 @@ def test_bf16_activation_storage_tracks_fp32():
 
 
 def test_entity_dim_400_runs_on_the_tensor_core_path():
-    """cfg5's feature width (D = 400 > 256 TMEM accumulator columns): the GEMM is tiled over the output columns (two
+    """cfg5's feature width (D = 400 > 256 accumulator columns per GEMM launch): the GEMM is tiled over the output columns (two
     launches per layer); same numbers as the exact-fp32 SIMT path within the split-bf16 bound."""
     c = dict(S.CONFIGS["cfg5"], B=2, N=300, E=1200, T=2)
     m, args = _model(c)
     b = S.make_batch(52, B=2, N=300, E=1200, with_weights=False, powerlaw=True)
     assert m.reasoning.__class__._alloc is not None
     _, _, d_tc, _ = m(b)
-    assert m.reasoning.use_planes                                  # the plane / tcgen05 data flow was taken
+    assert m.reasoning.use_planes                                  # the plane / tensor-core data flow was taken
     d_tc = d_tc.clone()
     ops.TC_LINEAR = False
     try:
@@ -308,5 +308,5 @@ def test_entity_dim_400_runs_on_the_tensor_core_path():
         ops.TC_LINEAR = True
     big = d_ref > 1e-12
     rel = ((d_tc - d_ref).abs()[big] / d_ref[big]).max().item()
-    print("D=400 tcgen05 (N-tiled) vs fp32 SIMT: max relative deviation %.2e" % rel)
+    print("D=400 wgmma (N-tiled) vs fp32 SIMT: max relative deviation %.2e" % rel)
     assert rel < 1e-3

@@ -1,4 +1,4 @@
-"""GPU: the fused layer kernel (csrc/fused_layer.cu: aggregation produced straight into the tcgen05 GEMM's operand
+"""GPU: the fused layer kernel (csrc/fused_layer.cu: aggregation produced straight into the wgmma GEMM's operand
 stages) against the unfused pair it replaces (gr_aggregate_dual_abs -> gr_linear_tc_planes), through the C ABI.
 The A operand is bit-identical by construction; the tensor core accumulates the k-blocks in a different order, so the
 outputs agree to fp32 rounding (checked at 2e-5 of the output scale, the existing plane tolerance) -- and against the

@@ -1,6 +1,6 @@
 """GPU parity at the HOT shapes against arrays produced by the unmodified reference (tests/golden/hot/*.npz, generator:
 tests/golden/make_golden_hot.py): entity_dim 200 with N >= 64 -- the |v|-accumulating aggregation kernel, the K = 1040
-tcgen05 GEMM and the sparse-prior / frontier path --, the full-size cfg2 batch bench.py times (B = 64) and the cfg5
+tensor-core GEMM and the sparse-prior / frontier path --, the full-size cfg2 batch bench.py times (B = 64) and the cfg5
 stress graph (D = 400).  Weights are rebuilt from synthetic.seeded_state_dict; the files hold reference outputs only."""
 import json
 import os

@@ -112,7 +112,7 @@ def test_linear_vs_torch(M, N, K):
 @pytest.mark.parametrize("M,N,K", [(300, 200, 1000), (1000, 200, 1000), (129, 64, 64), (4000, 50, 250),
                                    (257, 32, 160), (128, 256, 520), (5, 16, 8)])
 def test_linear_tc_split_bf16_vs_fp64(M, N, K):
-    """tcgen05 split-bf16 x3 GEMM: fp32-class accuracy (error ~1e-5 of the row scale), TMA OOB tails."""
+    """wgmma split-bf16 x3 GEMM: fp32-class accuracy (error ~1e-5 of the row scale), TMA OOB tails."""
     torch.manual_seed(1)
     big = torch.empty(M, K + 24, device=DEV).normal_()
     A = big[:, 8:8 + K] if (K % 4 == 0) else big[:, :K]         # strided row view (lda > K)
@@ -132,7 +132,7 @@ def test_linear_tc_split_bf16_vs_fp64(M, N, K):
 @pytest.mark.parametrize("bk", [32, 64])
 @pytest.mark.parametrize("cluster", [1, 2])
 def test_linear_tc_planes_cluster_variants(cluster, bk, tma_store):
-    """Planes-in GEMM (persistent, double-buffered TMEM) with and without W multicast across a CTA pair;
+    """Planes-in GEMM (persistent, register accumulators) with and without W multicast across a CTA pair;
     odd tile counts, fused score dots and plane outputs."""
     torch.manual_seed(2)
     ops.set_option("tc_cluster", cluster)

@@ -27,9 +27,9 @@
 //               next tile's h blocks are L2-prefetched a tile ahead)
 //   warps 2, 3  stagers: bulk copies of the tile's ELL entries + quad offsets, relu(+-ins)/2 of its <= 2 questions
 //               -> double-buffered tile descriptor
-//   warps 4-11  two consumer warpgroups, 64 tile rows each: wgmma.mma_async (m64n32k16 chunks, 3 products per k-step)
-//               with the fp32 accumulator in registers, then the epilogue: bias + relu + score dot -> fp32 h / bf16
-//               planes via TMA stores
+//   warps 4-11  two consumer warpgroups, 64 tile rows each: wgmma.mma_async (one full-width m64n{NP}k16 per product
+//               and k-step, 3 products) with the fp32 accumulator in registers, then the epilogue: bias + relu + score
+//               dot -> fp32 h / bf16 planes via TMA stores
 //   warps 12-15 aggregation: warp a owns tile rows 32a .. 32a+31 = eight quads; a quarter-warp owns a row, lane = 4
 //               columns of the 32-column group, so one warp-wide 16-byte load gathers one in-edge of each row of the
 //               quad (one 128-byte table line per row); 8 such loads in flight per lane, no predicates (slots past a
@@ -39,7 +39,10 @@
 // Operand slots are dedicated: slot t < 2I is always written by the aggregation warps, slot 2I always by TMA, so every
 // slot barrier flips once per group and the parity is the group counter.
 //
-// Performance on H100: not measured per kernel.
+// Registers: ptxas places a wgmma accumulator operand within the 128 registers per thread of the launch, so an
+// m64n208k16 (130 needed) does not compile here: accumulators wider than 128 columns are issued as 32-column
+// instructions, one straight-line batch per k-block.
+// Performance on one H100 SXM at 400 W, cfg2: 1.03 ms per dense layer (the unfused pair: 0.24 + 0.59 ms).
 #include <algorithm>
 #include <cstddef>
 
@@ -68,7 +71,6 @@ constexpr int kConsWarps = 8;                // two consumer warpgroups
 constexpr int kFirstCons = 4, kFirstAgg = 12;
 constexpr int kThreads = (kFirstAgg + kAggWarps) * 32;      // 512
 constexpr int kQuadsPerWarp = BM / 4 / kAggWarps;           // 8: an aggregation warp owns 32 tile rows
-constexpr int kMaxChunksFused = 7;           // register accumulator: n_pad <= 224 (= kXCols: D <= 224)
 // setmaxnreg budget: 512 x 128 at launch = 128 x 40 (control) + 256 x 200 (consumers) + 128 x 72 (aggregation)
 constexpr int kLaunchRegs = 128, kControlRegs = 40, kConsRegs = 200, kAggRegs = 72;
 static_assert(kControlRegs <= kLaunchRegs && kAggRegs <= kLaunchRegs && kConsRegs >= kLaunchRegs,
@@ -140,8 +142,8 @@ struct alignas(16) ETile {
 };
 
 template <int NI>
-constexpr size_t fused_smem_bytes(int n_pad) {
-  return 1024 /*align slack*/ + (size_t)(2 * NI + 1) * 2 * kABytes + (size_t)kNW * 2 * n_pad * BK * 2 + kOutBytes +
+constexpr size_t fused_smem_bytes(int np) {
+  return 1024 /*align slack*/ + (size_t)(2 * NI + 1) * 2 * kABytes + (size_t)kNW * 2 * np * BK * 2 + kOutBytes +
          2 * sizeof(ETile<NI>) + 64 * 8 + 2 * 256 * 4;
 }
 
@@ -463,7 +465,7 @@ __device__ __forceinline__ void agg_pass(const ETile<NI>& et, const FParams& p, 
 // ---------------------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------------------
-template <int NI, int CS>
+template <int NI, int NP, int CS>   // NP: accumulator width (W tile rows), n_pad rounded up to 64, 128, 208 or 224
 __global__ void __launch_bounds__(kThreads, 1)
 fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_constant__ CUtensorMap map_h_lo,
                    const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
@@ -472,7 +474,7 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
   constexpr int T = 2 * NI + 1;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int w_bytes = p.n_pad * BK * 2;
+  constexpr int w_bytes = NP * BK * 2;
   uint8_t* a_slots = smem;                                        // [T] x {hi 8 KB, lo 8 KB}
   uint8_t* w_ring = a_slots + (size_t)T * 2 * kABytes;            // [kNW] x {W_hi, W_lo}
   uint8_t* s_out = w_ring + (size_t)kNW * 2 * w_bytes;            // epilogue staging: [2 consumer warpgroups]
@@ -519,8 +521,8 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
       Prof pf; pf.init(p.debug & 32);
       uint32_t wphase = 0, grp = 0;
       int ws = 0;
-      const int w_rows = p.n_pad / CS;
-      const int w_slice = w_rows * BK * 2;
+      constexpr int w_rows = NP / CS;
+      constexpr int w_slice = w_rows * BK * 2;
       for (int tg = cid; tg < ngroups; tg += ncluster) {
         const int m0 = (tg * CS + crank) * BM;
         // the h planes come from HBM: pull the NEXT tile's blocks into L2 now, so that their TMA loads (issued only
@@ -617,8 +619,9 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
     // ===================== consumers: wgmma over the tile's k-blocks, then the epilogue =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsRegs));
     const int cw = (warp - kFirstCons) >> 2, wq = warp & 3;     // consumer warpgroup (row half), warp inside it
-    const int nc = (p.n_pad + 31) / 32;
-    const bool tail16 = (p.n_pad & 31) != 0;
+    // 512 threads launch with 128 registers each, and ptxas allocates every role within that (setmaxnreg only moves
+    // registers at run time): an accumulator operand wider than 128 columns does not fit one wgmma instruction
+    constexpr int kInstrCols = NP <= 128 ? NP : 32;
     const EpiOut e{s_bias, s_ws, (p.flags & GR_LINEAR_RELU) != 0};
     const int r = wq * 16 + (lane >> 2), cq = lane & 3;
     uint8_t* stg = s_out + (size_t)cw * kStageOutBytes;
@@ -629,23 +632,24 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
     int ws = 0;
     for (int tg = cid; tg < ngroups; tg += ncluster) {
       const int tile = tg * CS + crank;
-      float acc[kMaxChunksFused][16];
+      float acc[NP / 2];
 #pragma unroll
-      for (int j = 0; j < kMaxChunksFused; ++j)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
+      for (int i = 0; i < NP / 2; ++i) acc[i] = 0.f;
       int prev_ws = -1, prev_sl = -1;
       for (int g = 0; g < G; ++g, ++grp) {
-        const int ksteps = g == G - 1 ? p.ksteps_last : BK / MMA_K;
+        // the last column group of a 16-column-padded segment holds one k-step: its own straight-line batch
+        static_assert(BK / MMA_K == 2, "a k-block is one or two k-steps");
+        const bool half = g == G - 1 && p.ksteps_last == 1;
         for (int t = 0; t < T; ++t) {
           const int sl = t == 0 ? T - 1 : t - 1;              // operand slot of block t (slot T-1 = the h block)
           { const long long t0 = pf.t(); mbar_wait_sleep(&wfull[ws], wphase, 4); pf.add(0, t0); }
           { const long long t0 = pf.t(); mbar_wait_sleep(&afull[sl], grp & 1, 10 + sl); pf.add(t == 0 ? 2 : 1, t0); }
           const uint32_t sa = smem_u32(a_slots + (size_t)sl * 2 * kABytes) + (uint32_t)(cw * WG_M * BK * 2);
           const uint32_t sw = smem_u32(w_ring + (size_t)ws * 2 * w_bytes);
-          mma_kblock<kMaxChunksFused, BK>(acc, make_smem_desc<BK>(sa), make_smem_desc<BK>(sa + kABytes),
-                                          make_smem_desc<BK>(sw), make_smem_desc<BK>(sw + w_bytes), ksteps, nc,
-                                          false, tail16);
+          const uint64_t da_hi = make_smem_desc<BK>(sa), da_lo = make_smem_desc<BK>(sa + kABytes);
+          const uint64_t dw_hi = make_smem_desc<BK>(sw), dw_lo = make_smem_desc<BK>(sw + w_bytes);
+          if (half) mma_kblock<NP, BK, 1, false, kInstrCols>(acc, da_hi, da_lo, dw_hi, dw_lo);
+          else mma_kblock<NP, BK, 2, false, kInstrCols>(acc, da_hi, da_lo, dw_hi, dw_lo);
           wgmma_wait<1>();                                     // the previous k-block is done: free its W and A slots
           if (prev_ws >= 0 && lane == 0) { release_slot<CS>(&wempty[prev_ws]); mbar_arrive(&aempty[prev_sl]); }
           prev_ws = ws; prev_sl = sl;
@@ -659,16 +663,13 @@ fused_layer_kernel(const __grid_constant__ CUtensorMap map_h_hi, const __grid_co
       float dot0 = 0.f, dot1 = 0.f;
       const bool store = !(p.debug & 4);
 #pragma unroll
-      for (int j = 0; j < kMaxChunksFused; ++j) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int c0 = 32 * j + 16 * h;
-          if (j >= nc || c0 >= p.n_pad) continue;
-          float v[8];
-          epi_values(acc[j], h, c0, cq, e, v, dot0, dot1);
-          epi_store_tma(v, stg, r, cq, issuer, 1 + cw, &map_c, &map_c_hi, &map_c_lo, store && p.C != nullptr,
-                        store && p.has_planes, c0, tile * BM + cw * WG_M);
-        }
+      for (int q = 0; q < NP / 16; ++q) {
+        const int c0 = 16 * q;
+        if (c0 >= p.n_pad) continue;
+        float v[8];
+        epi_values(acc, q, cq, e, v, dot0, dot1);
+        epi_store_tma(v, stg, r, cq, issuer, 1 + cw, &map_c, &map_c_hi, &map_c_lo, store && p.C != nullptr,
+                      store && p.has_planes, c0, tile * BM + cw * WG_M);
       }
       epi_dots(dot0, dot1, p.dots, row0, p.M, cq);
     }
@@ -789,7 +790,7 @@ EllView ell_view(void* blob, const EllPlan& e) {
 
 struct FusedPlan {
   bool ok;
-  int n_pad, G, ksteps_last;
+  int n_pad, np, G, ksteps_last;   // np: instantiated accumulator width >= n_pad (W tile rows, zero filled beyond N)
   int64_t kp;                 // columns of the pre-formatted W planes
   size_t w_plane_bytes, smem_bytes;
 };
@@ -797,30 +798,31 @@ struct FusedPlan {
 FusedPlan plan_fused(int64_t Nq, int64_t D, int64_t pitch, int I, int64_t N_out) {
   FusedPlan f{};
   f.n_pad = (int)((N_out + 15) / 16 * 16);
+  f.np = f.n_pad <= 64 ? 64 : f.n_pad <= 128 ? 128 : f.n_pad <= 208 ? 208 : 224;
   f.G = (int)((pitch + BK - 1) / BK);
   f.ksteps_last = (int)((pitch - (int64_t)(f.G - 1) * BK) / MMA_K);
   f.kp = (int64_t)f.G * (2 * I + 1) * BK;
   f.w_plane_bytes = align_up((size_t)N_out * f.kp * 2, 256);
-  f.smem_bytes = I == 2 ? fused_smem_bytes<2>(f.n_pad) : fused_smem_bytes<1>(f.n_pad);
+  f.smem_bytes = I == 2 ? fused_smem_bytes<2>(f.np) : fused_smem_bytes<1>(f.np);
   f.ok = (I == 1 || I == 2) && Nq >= BM && D >= 8 && D <= pitch && pitch % 16 == 0 && (pitch + BK - 1) / BK * BK <= kXCols &&
-         N_out >= 8 && f.n_pad <= 32 * kMaxChunksFused && f.smem_bytes <= 227 * 1024 && get_encode_fn() != nullptr;
+         N_out >= 8 && f.n_pad <= 224 && f.smem_bytes <= 227 * 1024 && get_encode_fn() != nullptr;
   return f;
 }
 
-template <int NI, int CS>
+template <int NI, int NP, int CS>
 int launch_fused(const CUtensorMap& m_h_hi, const CUtensorMap& m_h_lo, const CUtensorMap& m_w_hi,
                  const CUtensorMap& m_w_lo, const CUtensorMap& m_c, const CUtensorMap& m_c_hi,
                  const CUtensorMap& m_c_lo, const FusedPlan& f, const FParams& p, cudaStream_t stream) {
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done)) {
-    GR_CHECK_CUDA(cudaFuncSetAttribute(fused_layer_kernel<NI, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    GR_CHECK_CUDA(cudaFuncSetAttribute(fused_layer_kernel<NI, NP, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        227 * 1024));
   }
   // the setmaxnreg budget of the kernel redistributes exactly kThreads x kLaunchRegs registers
   static int num_regs = 0;
   if (num_regs == 0) {
     cudaFuncAttributes fa{};
-    GR_CHECK_CUDA(cudaFuncGetAttributes(&fa, fused_layer_kernel<NI, CS>));
+    GR_CHECK_CUDA(cudaFuncGetAttributes(&fa, fused_layer_kernel<NI, NP, CS>));
     num_regs = fa.numRegs;
   }
   if (num_regs != kLaunchRegs) {
@@ -842,9 +844,20 @@ int launch_fused(const CUtensorMap& m_h_hi, const CUtensorMap& m_h_lo, const CUt
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  GR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fused_layer_kernel<NI, CS>, m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c, m_c_hi,
+  GR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fused_layer_kernel<NI, NP, CS>, m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c, m_c_hi,
                                    m_c_lo, p));
   return GR_OK;
+}
+
+template <int NP>
+int launch_fused_np(const CUtensorMap* const (&m)[7], int I, int cs, const FusedPlan& f, const FParams& p,
+                    cudaStream_t stream) {
+  if (I == 2) {
+    if (cs == 2) return launch_fused<2, NP, 2>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], f, p, stream);
+    return launch_fused<2, NP, 1>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], f, p, stream);
+  }
+  if (cs == 2) return launch_fused<1, NP, 2>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], f, p, stream);
+  return launch_fused<1, NP, 1>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], f, p, stream);
 }
 
 }  // namespace
@@ -957,12 +970,12 @@ extern "C" int gr_fused_layer(const int32_t* rowptr_t, const int32_t* src_t, con
   p.has_planes = C_hi ? 1 : 0;
   p.flags = flags;
   p.debug = g_fused_debug;
-  const int cs = ((f.n_pad / 2) % 8 == 0 && p.num_tiles >= 2) ? 2 : 1;
+  const int cs = ((f.np / 2) % 8 == 0 && p.num_tiles >= 2) ? 2 : 1;
   CUtensorMap m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo;
   // the h planes are exposed with seg_pitch columns only: the box of the last column group is zero filled beyond them
   if (!make_tmap(&m_h_hi, h_hi, M, seg_pitch, ldh16, BM, BK) || !make_tmap(&m_h_lo, h_lo, M, seg_pitch, ldh16, BM, BK) ||
-      !make_tmap(&m_w_hi, w_hi, N_out, f.kp, f.kp, f.n_pad / cs, BK) ||
-      !make_tmap(&m_w_lo, w_lo, N_out, f.kp, f.kp, f.n_pad / cs, BK)) {
+      !make_tmap(&m_w_hi, w_hi, N_out, f.kp, f.kp, f.np / cs, BK) ||
+      !make_tmap(&m_w_lo, w_lo, N_out, f.kp, f.kp, f.np / cs, BK)) {
     set_error("gr_fused_layer: cuTensorMapEncodeTiled failed (plane pointers must be 16-byte aligned)");
     return GR_ERR_CUDA;
   }
@@ -975,10 +988,11 @@ extern "C" int gr_fused_layer(const int32_t* rowptr_t, const int32_t* src_t, con
     set_error("gr_fused_layer: output pointers / pitches must be 16-byte aligned (TMA-store epilogue)");
     return GR_ERR_INVALID_ARG;
   }
-  if (I == 2) {
-    if (cs == 2) return launch_fused<2, 2>(m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, f, p, stream);
-    return launch_fused<2, 1>(m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, f, p, stream);
+  const CUtensorMap* m[7] = {&m_h_hi, &m_h_lo, &m_w_hi, &m_w_lo, &m_c, &m_c_hi, &m_c_lo};
+  switch (f.np) {
+    case 64: return launch_fused_np<64>(m, I, cs, f, p, stream);
+    case 128: return launch_fused_np<128>(m, I, cs, f, p, stream);
+    case 208: return launch_fused_np<208>(m, I, cs, f, p, stream);
+    default: return launch_fused_np<224>(m, I, cs, f, p, stream);
   }
-  if (cs == 2) return launch_fused<1, 2>(m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, f, p, stream);
-  return launch_fused<1, 1>(m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, f, p, stream);
 }

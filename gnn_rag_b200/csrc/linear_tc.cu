@@ -8,8 +8,9 @@
 //
 // Kernel: persistent, one 128-row tile of A at a time, full N (<= 256) per CTA.  Warpgroup 0 = TMA producer
 // (cp.async.bulk.tensor, swizzled K-major tiles of the four bf16 planes into a ring of `stages` slots with
-// full/empty mbarriers); warpgroups 1 and 2 = consumers, 64 rows each: wgmma.mma_async m64n32k16 / m64n16k16 from
-// shared memory (3 products per K step), fp32 accumulator in registers, then the epilogue (bias + relu + score dot,
+// full/empty mbarriers); warpgroups 1 and 2 = consumers, 64 rows each: one full-width wgmma.mma_async m64n{NP}k16
+// from shared memory per product and K step (NP = n_pad rounded up to an instantiated width: 64, 128, 208 or 256),
+// fp32 accumulator in registers, then the epilogue (bias + relu + score dot,
 // fp32 and bf16 hi/lo plane outputs, staged TMA stores or direct stores).  Clusters of 2 CTAs share the W tiles by
 // TMA multicast.
 //
@@ -100,7 +101,7 @@ struct TcParams {
   int64_t ldc16;
   const float* w_score;     // optional: score_func dot product (reasongnn.py:165): dots[m] = sum_n out[m,n] * w_score[n],
   float* dots;              //   dots[M + m] = 0 (the [2, M] partial-dot layout callers sum)
-  int M, N, K, n_pad, n16, stages, num_tiles;
+  int M, N, K, n_pad, n16, stages, num_tiles;   // n_pad = round16(N): the epilogue skips the columns beyond it
   uint32_t flags;
   int tma_store;            // 1: epilogue stages 64x16 chunks in smem and writes them with TMA stores
 };
@@ -110,7 +111,8 @@ struct TcParams {
 // consumers: each issues wgmma for its 64 rows of the tile, holds the accumulator in registers and runs the epilogue.
 // The producer runs up to `stages` k-blocks ahead, so the next tile's loads overlap this tile's epilogue.
 // ---------------------------------------------------------------------------------------------------
-template <int CS, int BK>   // CS: CTAs per cluster sharing W tiles by multicast; BK: k-block width
+// NP: accumulator width (W tile rows); CS: CTAs per cluster sharing W tiles by multicast; BK: k-block width
+template <int NP, int CS, int BK>
 __global__ void __launch_bounds__(kThreads, 1)
 linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                  const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
@@ -120,7 +122,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   // carve: [stages] x {A_hi, A_lo, W_hi, W_lo}, epilogue staging, barriers, bias / score weights
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int a_bytes = BM * BK * 2;
-  const int w_bytes = p.n_pad * BK * 2;
+  constexpr int w_bytes = NP * BK * 2;
   // GR_LINEAR_BF16_SINGLE: bf16 activation storage -- one product A_hi W_hi, stages hold {A_hi, W_hi} only
   const bool single = (p.flags & GR_LINEAR_BF16_SINGLE) != 0;
   const int w_off = single ? a_bytes : 2 * a_bytes;          // W_hi tile inside a stage
@@ -159,7 +161,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
     if (warp == 0 && lane == 0) {
       uint32_t phase = 0;
       int s = 0;
-      const int w_rows = p.n_pad / CS;                   // W rows this CTA fetches (and multicasts)
+      constexpr int w_rows = NP / CS;                    // W rows this CTA fetches (and multicasts)
       const int w_slice = w_rows * BK * 2;               // bytes
       for (int g = cid; g < ngroups; g += ncluster) {
         const int m0 = (g * CS + crank) * BM;            // may lie beyond M for the last group: zero-filled
@@ -187,8 +189,6 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
     // ===================== consumers: wgmma mainloop + epilogue =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
     const int cw = (warp - 4) >> 2, wq = warp & 3;       // consumer warpgroup (row half), warp inside it
-    const int nc = (p.n_pad + 31) / 32;
-    const bool tail16 = (p.n_pad & 31) != 0;
     const EpiOut e{s_bias, s_ws, (p.flags & GR_LINEAR_RELU) != 0};
     const int r = wq * 16 + (lane >> 2), cq = lane & 3;
     uint8_t* stg = s_out + (size_t)cw * kStageOutBytes;
@@ -200,19 +200,18 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
     int s = 0;
     for (int g = cid; g < ngroups; g += ncluster) {
       const int tile = g * CS + crank;
-      float acc[kMaxChunks][16];
+      float acc[NP / 2];
 #pragma unroll
-      for (int j = 0; j < kMaxChunks; ++j)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
+      for (int i = 0; i < NP / 2; ++i) acc[i] = 0.f;
       int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&full_bar[s], phase);
         const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
         const uint32_t a_row = (uint32_t)(cw * WG_M * BK * 2);
-        mma_kblock<kMaxChunks, BK>(acc, make_smem_desc<BK>(sa + a_row), make_smem_desc<BK>(sa + a_bytes + a_row),
-                                   make_smem_desc<BK>(sa + w_off), make_smem_desc<BK>(sa + w_off + w_bytes),
-                                   BK / MMA_K, nc, single, tail16);
+        const uint64_t da_hi = make_smem_desc<BK>(sa + a_row), da_lo = make_smem_desc<BK>(sa + a_bytes + a_row);
+        const uint64_t dw_hi = make_smem_desc<BK>(sa + w_off), dw_lo = make_smem_desc<BK>(sa + w_off + w_bytes);
+        if (single) mma_kblock<NP, BK, BK / MMA_K, true>(acc, da_hi, da_lo, dw_hi, dw_lo);
+        else mma_kblock<NP, BK, BK / MMA_K, false>(acc, da_hi, da_lo, dw_hi, dw_lo);
         wgmma_wait<1>();                                 // the previous k-block's products are done: free its slot
         if (prev >= 0 && lane == 0) release_slot<CS>(&empty_bar[prev]);
         prev = s;
@@ -224,48 +223,45 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
       const int64_t row0 = (int64_t)tile * BM + cw * WG_M + r;
       float dot0 = 0.f, dot1 = 0.f;
 #pragma unroll
-      for (int j = 0; j < kMaxChunks; ++j) {
+      for (int q = 0; q < NP / 16; ++q) {
+        const int c0 = 16 * q;
+        if (c0 >= p.n_pad) continue;
+        float v[8];
+        epi_values(acc, q, cq, e, v, dot0, dot1);
+        if (p.tma_store) {
+          epi_store_tma(v, stg, r, cq, issuer, 1 + cw, &map_c, &map_c_hi, &map_c_lo, p.C != nullptr,
+                        p.c_hi != nullptr, c0, tile * BM + cw * WG_M);
+          continue;
+        }
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int c0 = 32 * j + 16 * h;
-          if (j >= nc || c0 >= p.n_pad) continue;
-          float v[8];
-          epi_values(acc[j], h, c0, cq, e, v, dot0, dot1);
-          if (p.tma_store) {
-            epi_store_tma(v, stg, r, cq, issuer, 1 + cw, &map_c, &map_c_hi, &map_c_lo, p.C != nullptr,
-                          p.c_hi != nullptr, c0, tile * BM + cw * WG_M);
-            continue;
-          }
+        for (int b = 0; b < 2; ++b) {
+          const int col = c0 + 8 * b + 2 * cq;
 #pragma unroll
-          for (int b = 0; b < 2; ++b) {
-            const int col = c0 + 8 * b + 2 * cq;
-#pragma unroll
-            for (int hr = 0; hr < 2; ++hr) {
-              const int64_t row = row0 + 8 * hr;
-              if (row >= p.M) continue;
-              const float x0 = v[4 * b + 2 * hr], x1 = v[4 * b + 2 * hr + 1];
-              if (p.C) {
-                float* c = p.C + row * p.ldc + col;
-                if (vec_c && col + 1 < p.N) {
-                  *reinterpret_cast<float2*>(c) = make_float2(x0, x1);
-                } else {
-                  if (col < p.N) c[0] = x0;
-                  if (col + 1 < p.N) c[1] = x1;
-                }
+          for (int hr = 0; hr < 2; ++hr) {
+            const int64_t row = row0 + 8 * hr;
+            if (row >= p.M) continue;
+            const float x0 = v[4 * b + 2 * hr], x1 = v[4 * b + 2 * hr + 1];
+            if (p.C) {
+              float* c = p.C + row * p.ldc + col;
+              if (vec_c && col + 1 < p.N) {
+                *reinterpret_cast<float2*>(c) = make_float2(x0, x1);
+              } else {
+                if (col < p.N) c[0] = x0;
+                if (col + 1 < p.N) c[1] = x1;
               }
-              if (p.c_hi) {
-                // the planes also receive the (exactly zero) columns N .. n16
-                uint32_t lo;
-                const uint32_t hi = split_hi_lo(x0, x1, lo);
-                unsigned short* ph = reinterpret_cast<unsigned short*>(p.c_hi + row * p.ldc16 + col);
-                unsigned short* pl = reinterpret_cast<unsigned short*>(p.c_lo + row * p.ldc16 + col);
-                if (vec_h && col + 1 < p.n16) {
-                  *reinterpret_cast<uint32_t*>(ph) = hi;
-                  *reinterpret_cast<uint32_t*>(pl) = lo;
-                } else {
-                  if (col < p.n16) { ph[0] = (unsigned short)(hi & 0xFFFF); pl[0] = (unsigned short)(lo & 0xFFFF); }
-                  if (col + 1 < p.n16) { ph[1] = (unsigned short)(hi >> 16); pl[1] = (unsigned short)(lo >> 16); }
-                }
+            }
+            if (p.c_hi) {
+              // the planes also receive the (exactly zero) columns N .. n16
+              uint32_t lo;
+              const uint32_t hi = split_hi_lo(x0, x1, lo);
+              unsigned short* ph = reinterpret_cast<unsigned short*>(p.c_hi + row * p.ldc16 + col);
+              unsigned short* pl = reinterpret_cast<unsigned short*>(p.c_lo + row * p.ldc16 + col);
+              if (vec_h && col + 1 < p.n16) {
+                *reinterpret_cast<uint32_t*>(ph) = hi;
+                *reinterpret_cast<uint32_t*>(pl) = lo;
+              } else {
+                if (col < p.n16) { ph[0] = (unsigned short)(hi & 0xFFFF); pl[0] = (unsigned short)(lo & 0xFFFF); }
+                if (col + 1 < p.n16) { ph[1] = (unsigned short)(hi >> 16); pl[1] = (unsigned short)(lo >> 16); }
               }
             }
           }
@@ -281,7 +277,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
 
 struct TcPlan {
   int64_t kp;          // plane row stride (elements), multiple of 8
-  int n_pad, stages, bk;
+  int n_pad, np, stages, bk;   // np: instantiated accumulator width >= n_pad (W tile rows, zero filled beyond N)
   size_t a_plane_bytes, w_plane_bytes, total_bytes, w_only_bytes, smem_bytes;
   bool ok;
 };
@@ -292,7 +288,8 @@ TcPlan plan_tc(int64_t M, int64_t N, int64_t K, bool single = false) {
   t.ok = (N >= 8 && N <= 256 && K >= 8 && M >= 1);
   t.kp = (K + 7) / 8 * 8;
   t.n_pad = (int)((N + 15) / 16 * 16);
-  const size_t stage = (single ? 1 : 2) * ((size_t)BM * BK * 2 + (size_t)t.n_pad * BK * 2);
+  t.np = t.n_pad <= 64 ? 64 : t.n_pad <= 128 ? 128 : t.n_pad <= 208 ? 208 : 256;
+  const size_t stage = (single ? 1 : 2) * ((size_t)BM * BK * 2 + (size_t)t.np * BK * 2);
   // 227 KB usable smem minus alignment slack, bias/score arrays, barriers and the epilogue staging buffers
   int stages = (int)((227 * 1024 - 1024 - 2048 - 128 - 2 * kStageOutBytes) / stage);
   t.stages = stages > 8 ? 8 : stages;
@@ -319,20 +316,20 @@ int split_launch(const float* A, int64_t lda, int64_t M, int64_t K, __nv_bfloat1
   return GR_OK;
 }
 
-template <int CS, int BK>
+template <int NP, int CS, int BK>
 int launch_tc_cs(const CUtensorMap& m_a_hi, const CUtensorMap& m_a_lo, const CUtensorMap& m_w_hi,
                  const CUtensorMap& m_w_lo, const CUtensorMap& m_c, const CUtensorMap& m_c_hi,
                  const CUtensorMap& m_c_lo, const TcPlan& t, const TcParams& p, cudaStream_t stream) {
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done)) {
-    GR_CHECK_CUDA(cudaFuncSetAttribute(linear_tc_kernel<CS, BK>,
+    GR_CHECK_CUDA(cudaFuncSetAttribute(linear_tc_kernel<NP, CS, BK>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   }
   // setmaxnreg.inc only draws on registers the CTA was launched with: the budget needs exactly kLaunchRegs
   static int num_regs = 0;
   if (num_regs == 0) {
     cudaFuncAttributes fa{};
-    GR_CHECK_CUDA(cudaFuncGetAttributes(&fa, linear_tc_kernel<CS, BK>));
+    GR_CHECK_CUDA(cudaFuncGetAttributes(&fa, linear_tc_kernel<NP, CS, BK>));
     num_regs = fa.numRegs;
   }
   if (num_regs != kLaunchRegs) {
@@ -354,9 +351,19 @@ int launch_tc_cs(const CUtensorMap& m_a_hi, const CUtensorMap& m_a_lo, const CUt
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  GR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, linear_tc_kernel<CS, BK>, m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c, m_c_hi,
+  GR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, linear_tc_kernel<NP, CS, BK>, m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c, m_c_hi,
                                    m_c_lo, p));
   return GR_OK;
+}
+
+template <int NP>
+int launch_tc_np(const CUtensorMap* const (&m)[7], int cs, const TcPlan& t, const TcParams& p, cudaStream_t stream) {
+  if (t.bk == 64) {
+    if (cs == 2) return launch_tc_cs<NP, 2, 64>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], t, p, stream);
+    return launch_tc_cs<NP, 1, 64>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], t, p, stream);
+  }
+  if (cs == 2) return launch_tc_cs<NP, 2, 32>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], t, p, stream);
+  return launch_tc_cs<NP, 1, 32>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], t, p, stream);
 }
 
 int launch_tc(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int64_t lda16,
@@ -365,11 +372,11 @@ int launch_tc(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int64_t lda1
   p.n_pad = t.n_pad; p.stages = t.stages;
   p.num_tiles = (int)ceil_div(p.M, BM);
   // cluster multicast of W needs 8-row-aligned W slices and at least two tiles
-  int cs = (g_tc_cluster >= 2 && (t.n_pad / 2) % 8 == 0 && p.num_tiles >= 2) ? 2 : 1;
+  int cs = (g_tc_cluster >= 2 && (t.np / 2) % 8 == 0 && p.num_tiles >= 2) ? 2 : 1;
   CUtensorMap m_a_hi, m_a_lo, m_w_hi, m_w_lo;
   if (!make_tmap(&m_a_hi, a_hi, p.M, p.K, lda16, BM, t.bk) || !make_tmap(&m_a_lo, a_lo, p.M, p.K, lda16, BM, t.bk) ||
-      !make_tmap(&m_w_hi, w_hi, p.N, p.K, ldw16, t.n_pad / cs, t.bk) ||
-      !make_tmap(&m_w_lo, w_lo, p.N, p.K, ldw16, t.n_pad / cs, t.bk)) {
+      !make_tmap(&m_w_hi, w_hi, p.N, p.K, ldw16, t.np / cs, t.bk) ||
+      !make_tmap(&m_w_lo, w_lo, p.N, p.K, ldw16, t.np / cs, t.bk)) {
     set_error("gr_linear_tc: cuTensorMapEncodeTiled failed (pointers must be 16-byte aligned, row strides "
               "multiples of 8 elements)");
     return GR_ERR_CUDA;
@@ -384,12 +391,13 @@ int launch_tc(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int64_t lda1
   if (ok && p.c_hi) ok = make_out_tmap(&m_c_hi, p.c_hi, p.M, p.n16, p.ldc16, 2) &&
                          make_out_tmap(&m_c_lo, p.c_lo, p.M, p.n16, p.ldc16, 2);
   p.tma_store = ok ? 1 : 0;
-  if (t.bk == 64) {
-    if (cs == 2) return launch_tc_cs<2, 64>(m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, t, p, stream);
-    return launch_tc_cs<1, 64>(m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, t, p, stream);
+  const CUtensorMap* m[7] = {&m_a_hi, &m_a_lo, &m_w_hi, &m_w_lo, &m_c, &m_c_hi, &m_c_lo};
+  switch (t.np) {
+    case 64: return launch_tc_np<64>(m, cs, t, p, stream);
+    case 128: return launch_tc_np<128>(m, cs, t, p, stream);
+    case 208: return launch_tc_np<208>(m, cs, t, p, stream);
+    default: return launch_tc_np<256>(m, cs, t, p, stream);
   }
-  if (cs == 2) return launch_tc_cs<2, 32>(m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, t, p, stream);
-  return launch_tc_cs<1, 32>(m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c, m_c_hi, m_c_lo, t, p, stream);
 }
 
 }  // namespace

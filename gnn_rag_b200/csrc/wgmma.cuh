@@ -2,9 +2,11 @@
 // (linear_tc.cu, fused_layer.cu).  sm_90a.
 //
 // Both kernels run the same consumer: two warpgroups per CTA, warpgroup w owns rows 64w .. 64w+63 of a 128-row tile
-// and keeps its 64 x n_pad fp32 accumulator in registers as n_pad / 32 chunks of m64n32 (plus one m64n16 chunk when
-// n_pad % 32 == 16).  Operand tiles are K-major bf16, written by TMA (or by the fused kernel's aggregation warps) with
-// SWIZZLE_64B (BK = 32) or SWIZZLE_128B (BK = 64).
+// and keeps its 64 x NP fp32 accumulator in registers (NP / 2 per thread).  NP is the instantiated accumulator width
+// (64, 128, 208, 224 or 256): the output width n_pad rounds up to it, the W rows beyond N come from the TMA zero fill.
+// Every k-step issues ONE wgmma.mma_async.m64n{NP}k16 per product, and the k-steps of a k-block form one batch (one
+// fence, the products back to back, one commit).  Operand tiles are K-major bf16, written by TMA (or by the fused
+// kernel's aggregation warps) with SWIZZLE_64B (BK = 32) or SWIZZLE_128B (BK = 64).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -17,7 +19,6 @@ namespace tc {
 constexpr int BM = 128;          // rows per CTA tile: two consumer warpgroups of 64 rows
 constexpr int WG_M = 64;         // rows per consumer warpgroup (wgmma M)
 constexpr int MMA_K = 16;
-constexpr int kMaxChunks = 8;    // 32-column accumulator chunks: n_pad <= 256
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
@@ -172,91 +173,118 @@ __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 // keeps the compiler from moving accumulator accesses across the asynchronous wgmma window
-__device__ __forceinline__ void acc_fence(float (&d)[16]) {
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[64 x 32] += A[64 x 16] B[32 x 16]^T, bf16 operands from shared memory, fp32 accumulate
-__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b));
+// D[64 x N] += A[64 x 16] B[N x 16]^T, bf16 operands from shared memory, fp32 accumulate in d[OFF .. OFF + N/2 - 1]
+#define GR_ACC8(i) "+f"(d[OFF + (i)]), "+f"(d[OFF + (i) + 1]), "+f"(d[OFF + (i) + 2]), "+f"(d[OFF + (i) + 3]), \
+                   "+f"(d[OFF + (i) + 4]), "+f"(d[OFF + (i) + 5]), "+f"(d[OFF + (i) + 6]), "+f"(d[OFF + (i) + 7])
+#define GR_ACC32(i) GR_ACC8(i), GR_ACC8((i) + 8), GR_ACC8((i) + 16), GR_ACC8((i) + 24)
+#define GR_REGS8 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define GR_REGS16 GR_REGS8 ", %8, %9, %10, %11, %12, %13, %14, %15"
+#define GR_REGS32 GR_REGS16 ", %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define GR_REGS64 GR_REGS32 ", %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, " \
+                  "%49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define GR_REGS104 GR_REGS64 ", %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, " \
+                   "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, " \
+                   "%99, %100, %101, %102, %103"
+#define GR_REGS128 GR_REGS104 ", %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, " \
+                   "%117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+// REGS: the accumulator operands %0 .. %(N/2 - 1); the descriptors follow them as operands RA and RB
+#define GR_WGMMA(N, REGS, RA, RB, ...)                                                                   \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                          \
+               "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 {" REGS "}, %" #RA ", %" #RB  \
+               ", p, 1, 1, 0, 0;\n\t}"                                                                   \
+               : __VA_ARGS__                                                                             \
+               : "l"(a), "l"(b))
+template <int N, int OFF, int R>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[R], uint64_t a, uint64_t b) {
+  static_assert(OFF + N / 2 <= R, "accumulator range");
+  if constexpr (N == 16) {
+    GR_WGMMA(16, GR_REGS8, 8, 9, GR_ACC8(0));
+  } else if constexpr (N == 32) {
+    GR_WGMMA(32, GR_REGS16, 16, 17, GR_ACC8(0), GR_ACC8(8));
+  } else if constexpr (N == 64) {
+    GR_WGMMA(64, GR_REGS32, 32, 33, GR_ACC32(0));
+  } else if constexpr (N == 128) {
+    GR_WGMMA(128, GR_REGS64, 64, 65, GR_ACC32(0), GR_ACC32(32));
+  } else if constexpr (N == 208) {
+    GR_WGMMA(208, GR_REGS104, 104, 105, GR_ACC32(0), GR_ACC32(32), GR_ACC32(64), GR_ACC8(96));
+  } else {
+    static_assert(N == 256, "instruction widths: 16, 32, 64, 128, 208, 256");
+    GR_WGMMA(256, GR_REGS128, 128, 129, GR_ACC32(0), GR_ACC32(32), GR_ACC32(64), GR_ACC32(96));
+  }
 }
-// the same for a 16-column chunk: D[64 x 16] in d[0 .. 7]
-__device__ __forceinline__ void wgmma_n16(float (&d)[16], uint64_t a, uint64_t b) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b));
+#undef GR_WGMMA
+#undef GR_REGS128
+#undef GR_REGS104
+#undef GR_REGS64
+#undef GR_REGS32
+#undef GR_REGS16
+#undef GR_REGS8
+#undef GR_ACC32
+#undef GR_ACC8
+
+// one product over the NP accumulator columns: instructions of NI columns from column C0 on (the last one takes
+// what is left), W rows C0 .. of the tile with BK*2-byte rows
+template <int NP, int NI, int BK, int C0 = 0>
+__device__ __forceinline__ void wgmma_product(float (&acc)[NP / 2], uint64_t a, uint64_t b) {
+  constexpr int n = NP - C0 < NI ? NP - C0 : NI;
+  wgmma_bf16<n, C0 / 2>(acc, a, b + (uint64_t)((C0 * BK * 2) >> 4));
+  if constexpr (C0 + n < NP) wgmma_product<NP, NI, BK, C0 + n>(acc, a, b);
 }
 
-// One k-block of the 3-product split-bf16 contraction (or the single product A_hi W_hi) for one consumer warpgroup:
-// acc[j] += A[64 rows, ksteps*16] W[32j .. 32j+31, ksteps*16]^T for j < nc.  `da_*` / `dw_*` are descriptors of the
-// k-block's first column; the W tile holds n_pad rows of BK*2 bytes.  NC (template) sizes the register accumulator,
-// nc <= NC chunks are live, `tail16`: chunk nc - 1 has 16 columns.
-template <int NC, int BK>
-__device__ __forceinline__ void mma_kblock(float (&acc)[NC][16], uint64_t da_hi, uint64_t da_lo, uint64_t dw_hi,
-                                           uint64_t dw_lo, int ksteps, int nc, bool single, bool tail16) {
-  constexpr uint64_t kChunkAdv = (uint64_t)((32 * BK * 2) >> 4);     // 32 W rows
-#pragma unroll
-  for (int j = 0; j < NC; ++j) acc_fence(acc[j]);
+// One k-block of the 3-product split-bf16 contraction (or, SINGLE, the one product A_hi W_hi) for one consumer
+// warpgroup: acc += A[64 rows, KSTEPS*16] W[NP rows, KSTEPS*16]^T.  `da_*` / `dw_*` are descriptors of the k-block's
+// first column; the W tile holds NP rows of BK*2 bytes.  Each product is ONE m64n{NP}k16 instruction (NI = NP), or,
+// where the kernel's register budget cannot hold the accumulator as one instruction operand, NP / NI instructions of
+// NI columns (plus one for the rest).  KSTEPS and SINGLE are template parameters so that the batch is straight-line
+// code: a runtime condition between two wgmma instructions makes ptxas wait for the accumulator (C7519) and split
+// the batch.
+template <int NP, int BK, int KSTEPS, bool SINGLE, int NI = NP>
+__device__ __forceinline__ void mma_kblock(float (&acc)[NP / 2], uint64_t da_hi, uint64_t da_lo, uint64_t dw_hi,
+                                           uint64_t dw_lo) {
+  static_assert(KSTEPS >= 1 && KSTEPS <= BK / MMA_K, "k-steps of one k-block");
+  acc_fence(acc);
   wgmma_fence();
 #pragma unroll
-  for (int k = 0; k < BK / MMA_K; ++k) {
-    if (k < ksteps) {
-      const uint64_t adv = (uint64_t)((k * MMA_K * 2) >> 4);        // +32 B per K step inside the swizzle row
-#pragma unroll
-      for (int j = 0; j < NC; ++j) {
-        if (j >= nc) continue;
-        const uint64_t wh = dw_hi + j * kChunkAdv + adv, wl = dw_lo + j * kChunkAdv + adv;
-        if (j == nc - 1 && tail16) {
-          wgmma_n16(acc[j], da_hi + adv, wh);
-          if (!single) {
-            wgmma_n16(acc[j], da_hi + adv, wl);
-            wgmma_n16(acc[j], da_lo + adv, wh);
-          }
-        } else {
-          wgmma_n32(acc[j], da_hi + adv, wh);
-          if (!single) {
-            wgmma_n32(acc[j], da_hi + adv, wl);
-            wgmma_n32(acc[j], da_lo + adv, wh);
-          }
-        }
-      }
+  for (int k = 0; k < KSTEPS; ++k) {
+    const uint64_t adv = (uint64_t)((k * MMA_K * 2) >> 4);          // +32 B per K step inside the swizzle row
+    wgmma_product<NP, NI, BK>(acc, da_hi + adv, dw_hi + adv);
+    if (!SINGLE) {
+      wgmma_product<NP, NI, BK>(acc, da_hi + adv, dw_lo + adv);
+      wgmma_product<NP, NI, BK>(acc, da_lo + adv, dw_hi + adv);
     }
   }
   wgmma_commit();
-#pragma unroll
-  for (int j = 0; j < NC; ++j) acc_fence(acc[j]);
+  acc_fence(acc);
 }
 
-// Epilogue helpers.  Accumulator fragment of thread (warp w of the warpgroup, lane l), chunk j, element i:
-// row 16w + l/4 + 8*((i >> 1) & 1), column 32j + 8*(i >> 2) + 2*(l % 4) + (i & 1).
+// Epilogue helpers.  Accumulator fragment of thread (warp w of the warpgroup, lane l), element i of float[NP / 2]:
+// row 16w + l/4 + 8*((i >> 1) & 1), column 8*(i >> 2) + 2*(l % 4) + (i & 1) (m64nN is the concatenation of its
+// 8-column blocks), so the 16-column half q of the tile is elements 8q .. 8q+7.
 struct EpiOut {
   const float* bias;        // [256] in shared memory, zero padded
   const float* w_score;     // [256] in shared memory, zero padded
   bool relu;
 };
 
-// bias + relu + score dot of 16-column half `h` of chunk j: v[0..7] = columns (8*(2h) | 8*(2h+1)) + 2c + {0,1}, rows
-// r (v[0,1], v[4,5]) and r + 8 (v[2,3], v[6,7]); dot0 / dot1 accumulate the score dot of rows r / r + 8
-__device__ __forceinline__ void epi_values(const float (&a)[16], int h, int c0, int cq, const EpiOut& e, float (&v)[8],
+// bias + relu + score dot of 16-column half `q` (columns c0 = 16q .. 16q+15): v[0..7] = columns c0 + (0 | 8) + 2c +
+// {0,1}, rows r (v[0,1], v[4,5]) and r + 8 (v[2,3], v[6,7]); dot0 / dot1 accumulate the score dot of rows r / r + 8
+template <int R>
+__device__ __forceinline__ void epi_values(const float (&a)[R], int q, int cq, const EpiOut& e, float (&v)[8],
                                            float& dot0, float& dot1) {
 #pragma unroll
   for (int b = 0; b < 2; ++b) {
-    const int col = c0 + 8 * b + 2 * cq;
+    const int col = 16 * q + 8 * b + 2 * cq;
     const float2 bb = *reinterpret_cast<const float2*>(e.bias + col);
     const float2 ww = *reinterpret_cast<const float2*>(e.w_score + col);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      float x = a[8 * h + 4 * b + i] + ((i & 1) ? bb.y : bb.x);
+      float x = a[8 * q + 4 * b + i] + ((i & 1) ? bb.y : bb.x);
       if (e.relu) x = fmaxf(x, 0.f);
       v[4 * b + i] = x;
     }

@@ -85,6 +85,16 @@ SIGNATURES = {
     "gr_shortest_path_nodes": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_int,
                                        c_i32p, c_i32p, c_int, c_void_p, c_i32p, c_int, c_int,
                                        c_void_p, c_size, c_void_p]),
+    "gr_rule_adj_workspace_bytes": (c_size, [c_i64]),
+    "gr_rule_adj_build": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i64, c_i64,
+                                  c_i32p, c_i32p, c_i32p, c_i32p, c_void_p, c_size, c_void_p]),
+    "gr_rule_level_workspace_bytes": (c_size, [c_i64]),
+    "gr_rule_level_count": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_int, c_int, c_i32p, c_i32p,
+                                    c_i64, c_i32p, c_void_p, c_i32p, c_i32p, c_void_p, c_size, c_void_p]),
+    "gr_rule_level_emit": (c_int, [c_i32p, c_i32p, c_i32p, c_void_p, c_i64, c_i64, c_i32p, c_i32p, c_i32p,
+                                   c_void_p]),
+    "gr_rule_paths_write": (c_int, [c_void_p, c_void_p, c_i32p, c_i32p, c_void_p, c_void_p, c_int, c_i64, c_i32p,
+                                    c_void_p]),
 }
 
 _lib = None

@@ -60,4 +60,30 @@ __device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ int warp_id() { return threadIdx.x >> 5; }
 
+// Bitonic network with all comparators ascending (virtual +inf padding beyond n): sorts arbitrary n.  The whole
+// block calls it; `a` is shared or global memory.
+template <typename T>
+__device__ void bitonic_sort_block(T* a, int n) {
+  for (int k = 2; (k >> 1) < n; k <<= 1) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      int l = i ^ (k - 1);
+      if (l > i && l < n) {
+        T x = a[i], y = a[l];
+        if (x > y) { a[i] = y; a[l] = x; }
+      }
+    }
+    __syncthreads();
+    for (int j = k >> 2; j > 0; j >>= 1) {
+      for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        int l = i ^ j;
+        if (l > i && l < n) {
+          T x = a[i], y = a[l];
+          if (x > y) { a[i] = y; a[l] = x; }
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
 }  // namespace gr

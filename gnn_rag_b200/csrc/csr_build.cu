@@ -188,30 +188,6 @@ __global__ void sort_rows_small_kernel(const int32_t* __restrict__ rowptr_t,
     if (k < deg) fact[beg + k] = v[k];
 }
 
-// Bitonic network with all comparators ascending (virtual +inf padding beyond n): sorts arbitrary n.
-__device__ void bitonic_sort_block(int32_t* a, int n) {
-  for (int k = 2; (k >> 1) < n; k <<= 1) {
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-      int l = i ^ (k - 1);
-      if (l > i && l < n) {
-        int x = a[i], y = a[l];
-        if (x > y) { a[i] = y; a[l] = x; }
-      }
-    }
-    __syncthreads();
-    for (int j = k >> 2; j > 0; j >>= 1) {
-      for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        int l = i ^ j;
-        if (l > i && l < n) {
-          int x = a[i], y = a[l];
-          if (x > y) { a[i] = y; a[l] = x; }
-        }
-      }
-      __syncthreads();
-    }
-  }
-}
-
 __global__ void sort_rows_long_kernel(const int32_t* __restrict__ rowptr_t,
                                       const int32_t* __restrict__ rowptr_h,
                                       int32_t* __restrict__ fact_t, int32_t* __restrict__ fact_h,

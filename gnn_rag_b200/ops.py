@@ -4,6 +4,7 @@ All ops raise if handed a CPU tensor -- there is no CPU fallback on the product 
 import ctypes
 import weakref
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -790,11 +791,98 @@ def shortest_path_nodes(g, source_idx, source_cnt, target_idx, target_cnt, retur
     L = _L()
     nbytes = L.gr_paths_workspace_bytes(B, N, S, T)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    rc = L.gr_shortest_path_nodes(_p(g.rowptr_t), _p(g.src_t), _p(g.rowptr_h), _p(g.src_h),
-                                  _p(source_idx.contiguous()), _p(source_cnt.contiguous()), S,
-                                  _p(target_idx.contiguous()), _p(target_cnt.contiguous()), T,
-                                  _p(on_path), _p(pair_dist), B, N, _p(ws), nbytes, _stream())
+    with _OpTimer("paths"):
+        rc = L.gr_shortest_path_nodes(_p(g.rowptr_t), _p(g.src_t), _p(g.rowptr_h), _p(g.src_h),
+                                      _p(source_idx.contiguous()), _p(source_cnt.contiguous()), S,
+                                      _p(target_idx.contiguous()), _p(target_cnt.contiguous()), T,
+                                      _p(on_path), _p(pair_dist), B, N, _p(ws), nbytes, _stream())
     _lib.check(rc)
     if return_distances:
         return on_path, pair_dist, ws[: B * (S + T) * N * 4].view(torch.int32).view(B, S + T, N)
     return on_path, pair_dist
+
+
+class RuleAdjacency:
+    """Label-grouped undirected adjacency (gr_rule_adj_build): row u = [rowptr[u], rowptr[u] + len[u]) of nbr / lab,
+    sorted by (label, first fact) -- every label's neighbours form one segment in nx.Graph neighbour order."""
+
+    def __init__(self, rowptr, length, nbr, lab):
+        self.rowptr, self.len, self.nbr, self.lab = rowptr, length, nbr, lab
+
+
+def rule_adjacency(g):
+    """CsrGraph built with rels = per-triple label ids -> RuleAdjacency (global node ids, like the CSR)."""
+    Nt, F = g.B * g.N, g.F
+    dev = g.rowptr_t.device
+    i32 = dict(dtype=torch.int32, device=dev)
+    adj = RuleAdjacency(torch.empty(Nt + 1, **i32), torch.empty(Nt, **i32), torch.empty(max(2 * F, 1), **i32),
+                        torch.empty(max(2 * F, 1), **i32))
+    L = _L()
+    nbytes = L.gr_rule_adj_workspace_bytes(F)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    with _OpTimer("rule_paths"):
+        rc = L.gr_rule_adj_build(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(g.rowptr_h), _p(g.src_h),
+                                 _p(g.rel_h), _p(g.fact_h), Nt, F, _p(adj.rowptr), _p(adj.len), _p(adj.nbr),
+                                 _p(adj.lab), _p(ws), nbytes, _stream())
+    _lib.check(rc)
+    STATS.launches += 2
+    return adj
+
+
+def rule_walks(adj, start, rule_off, rule_len, rule_lab):
+    """All rule walks of J jobs (gr_rule_level_count / _emit per level, then gr_rule_paths_write).
+    Host numpy int32 inputs: start[J] (node id, -1 = not in the graph), rule_off[J] / rule_len[J] into rule_lab
+    (label ids, -1 = absent label).  Returns (paths, counts, elem_off): paths = int32 device tensor holding, for job j,
+    counts[j] rows of rule_len[j] + 1 node ids from elem_off[j] on (host int64 arrays)."""
+    with _OpTimer("rule_paths"):
+        return _rule_walks(adj, start, rule_off, rule_len, rule_lab)
+
+
+def _rule_walks(adj, start, rule_off, rule_len, rule_lab):
+    dev = adj.nbr.device
+    J = len(start)
+    start, rule_len = np.asarray(start, np.int32), np.asarray(rule_len, np.int32)
+    i32 = dict(dtype=torch.int32, device=dev)
+    keep = np.nonzero((rule_len == 0) | (start >= 0))[0]
+    node = torch.from_numpy(start[keep]).to(dev)
+    job = torch.from_numpy(keep.astype(np.int32)).to(dev)
+    d_off = torch.from_numpy(np.asarray(rule_off, np.int32)).to(dev)
+    d_len = torch.from_numpy(rule_len).to(dev)
+    d_lab = torch.from_numpy(np.append(np.asarray(rule_lab, np.int32), np.int32(-1))).to(dev)
+    res_begin = torch.zeros(max(J, 1), **i32)
+    res_count = torch.zeros(max(J, 1), **i32)
+    levels_node, levels_parent = [node], [torch.full_like(node, -1)]
+    L = _L()
+    for level in range(int(rule_len.max()) + 1 if J else 0):
+        n = node.numel()
+        seg = torch.empty(max(n, 1), **i32)
+        off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        nbytes = L.gr_rule_level_workspace_bytes(n)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _lib.check(L.gr_rule_level_count(_p(adj.rowptr), _p(adj.len), _p(adj.lab), _p(d_off), _p(d_len), _p(d_lab),
+                                         J, level, _p(node), _p(job), n, _p(seg), _p(off), _p(res_begin),
+                                         _p(res_count), _p(ws), nbytes, _stream()))
+        if level == rule_len.max():
+            break
+        total = int(off[n].item())              # the one read-back per level: the next level is allocated exactly
+        fits = total <= 0x7fffffff              # a level that int32 cannot index is refused by gr_rule_level_emit
+        nxt = [torch.empty(max(total if fits else 0, 1), **i32) for _ in range(3)]
+        _lib.check(L.gr_rule_level_emit(_p(adj.nbr), _p(job), _p(seg), _p(off), n, total, _p(nxt[0]), _p(nxt[1]),
+                                        _p(nxt[2]), _stream()))
+        node, job = nxt[0][:total], nxt[2][:total]
+        levels_node.append(node)
+        levels_parent.append(nxt[1][:total])
+    counts = res_count[:J].cpu().numpy().astype(np.int64)
+    path_off = np.zeros(J + 1, dtype=np.int64)
+    np.cumsum(counts, out=path_off[1:])
+    elems = counts * (rule_len.astype(np.int64) + 1)
+    elem_off = np.zeros(J + 1, dtype=np.int64)
+    np.cumsum(elems, out=elem_off[1:])
+    paths = torch.empty(max(int(elem_off[-1]), 1), **i32)
+    if path_off[-1] > 0:
+        lv_node = torch.tensor([t.data_ptr() for t in levels_node], dtype=torch.int64, device=dev)
+        lv_parent = torch.tensor([t.data_ptr() for t in levels_parent], dtype=torch.int64, device=dev)
+        d_path_off, d_elem_off = torch.from_numpy(path_off).to(dev), torch.from_numpy(elem_off).to(dev)
+        _lib.check(L.gr_rule_paths_write(_p(lv_node), _p(lv_parent), _p(d_len), _p(res_begin), _p(d_path_off),
+                                         _p(d_elem_off), J, int(path_off[-1]), _p(paths), _stream()))
+    return paths[: int(elem_off[-1])], counts, elem_off[:J]

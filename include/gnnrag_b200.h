@@ -355,6 +355,54 @@ int gr_shortest_path_nodes(const int32_t* rowptr_t, const int32_t* src_t,
                            uint8_t* on_path, int32_t* pair_dist, int B, int N,
                            void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Rule-guided reasoning paths (csrc/rule_paths.cu): bfs_with_rule over the undirected graph of build_graph
+ * (llm/src/utils/graph_utils.py:10-47) for many (start node, relation rule) jobs at once -- the calls
+ * PromptBuilder.apply_rules makes (llm/src/qa_prediction/build_qa_input.py:58-64).  Exact: every walk whose i-th edge
+ * label equals rule[i] (nodes may repeat), in the reference's FIFO order, never truncated.  Integer-only, bit-exact.
+ *
+ * gr_rule_adj_build: label-grouped adjacency from the two CSRs of gr_csr_build called with rels = per-triple LABEL ids
+ * (the stripped relation strings interned by the caller).  Row u lists each distinct neighbour once (nx.Graph),
+ * sorted by (label of the pair's LAST triple, the pair's FIRST triple), so the neighbours with one label form a
+ * contiguous segment in graph.neighbors(u) order.
+ *   adj_rowptr: int32[Nt+1] = rowptr_t + rowptr_h (row capacity); adj_len: int32[Nt] = entries used in each row;
+ *   adj_nbr, adj_lab: int32[2F].  Workspace: gr_rule_adj_workspace_bytes(F).
+ *
+ * Level expansion.  Jobs j < J: rule = rule_lab[job_rule_off[j] .. + job_rule_len[j]) (label ids; -1 = a label absent
+ * from the graph, which matches nothing).  The caller orders the jobs (apply_rules: source-major, rule-minor) and
+ * builds level 0 = one entry (node, job) per job, job ascending: node = the start node, or -1 for a start that is not
+ * in the graph (kept only when the rule is empty: the reference returns one empty path then).  Level l (l = 0, 1, ...):
+ *   gr_rule_level_count: for every entry, the length of its node's segment with label rule[l] (0 when the job's rule
+ *     is shorter), scanned in place into child_off: int64[n+1], child_off[n] = the next level's size (read it back
+ *     and allocate the next level).  seg_begin: int32[n].  Jobs whose rule length is l are finished: their entries
+ *     are their result paths, res_begin[j] / res_count[j] (int32[J]) receive that run of the level.  Workspace:
+ *     gr_rule_level_workspace_bytes(n).
+ *   gr_rule_level_emit: writes the next level, int32[total] each: child_node, child_parent (entry index in level l),
+ *     child_job; children of one entry are consecutive, in segment order.  A level of more than INT32_MAX entries is
+ *     refused with GR_ERR_UNSUPPORTED and the count in gr_last_error (never clamped).
+ * gr_rule_paths_write: after the last level; level_node / level_parent are DEVICE arrays of the per-level device
+ * pointers (level 0's parents are not read).  path_off: int64[J+1] exclusive sums of res_count; elem_off: int64[J]
+ * exclusive sums of res_count[j] * (job_rule_len[j] + 1).  Path k of job j is written to
+ * paths[elem_off[j] + k*(len+1) ...] as its len+1 node ids, start first; P = path_off[J].
+ */
+size_t gr_rule_adj_workspace_bytes(int64_t F);
+int gr_rule_adj_build(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t, const int32_t* fact_t,
+                      const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h, const int32_t* fact_h,
+                      int64_t Nt, int64_t F, int32_t* adj_rowptr, int32_t* adj_len, int32_t* adj_nbr,
+                      int32_t* adj_lab, void* workspace, size_t workspace_bytes, void* stream);
+size_t gr_rule_level_workspace_bytes(int64_t n);
+int gr_rule_level_count(const int32_t* adj_rowptr, const int32_t* adj_len, const int32_t* adj_lab,
+                        const int32_t* job_rule_off, const int32_t* job_rule_len, const int32_t* rule_lab, int J,
+                        int level, const int32_t* node, const int32_t* job, int64_t n, int32_t* seg_begin,
+                        int64_t* child_off, int32_t* res_begin, int32_t* res_count, void* workspace,
+                        size_t workspace_bytes, void* stream);
+int gr_rule_level_emit(const int32_t* adj_nbr, const int32_t* job, const int32_t* seg_begin, const int64_t* child_off,
+                       int64_t n, int64_t total, int32_t* child_node, int32_t* child_parent, int32_t* child_job,
+                       void* stream);
+int gr_rule_paths_write(const int32_t* const* level_node, const int32_t* const* level_parent,
+                        const int32_t* job_rule_len, const int32_t* res_begin, const int64_t* path_off,
+                        const int64_t* elem_off, int J, int64_t P, int32_t* paths, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

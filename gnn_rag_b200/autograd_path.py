@@ -99,7 +99,8 @@ class _AggregateFn(torch.autograd.Function):
     def backward(ctx, grad_out):
         from . import ops
         table, ins, prior = ctx.saved_tensors
-        gt, gi, gp = torch.zeros_like(table), torch.zeros_like(ins), torch.zeros_like(prior)
+        # the kernel accumulates into dense row-major buffers: zeros_like alone would keep a transposed input's strides
+        gt, gi, gp = (torch.zeros_like(t, memory_format=torch.contiguous_format) for t in (table, ins, prior))
         ops.aggregate_backward(ctx.graph, ctx.direction, prior, table.contiguous(), ins.contiguous(),
                                grad_out.contiguous(), gt, gi, gp, ctx.w)
         return gt, gi, gp, None, None, None

@@ -299,7 +299,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* b) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive1(uint64_t* b) { mbar_arrive(b); }
 __device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t parity) {
   uint32_t ok = 0;
   while (!ok) {
@@ -486,7 +485,6 @@ __device__ __forceinline__ float lds1(uint32_t a) {
   return v;
 }
 
-constexpr int kG4Slots = 8;                 // slots per stage = two gather4 groups
 constexpr int kOobRow = 0x3fffffff;         // row coordinate outside any table: zero fill, no memory traffic
 
 // four table rows r0..r3 (`slot_bytes` of each) into consecutive slots at dst, completion counted on `bar`: one 1-D

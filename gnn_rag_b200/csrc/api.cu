@@ -27,7 +27,6 @@ int sm_count() {
 }
 
 extern int g_opt_agg_tma;
-extern int g_opt_linear_tc;
 extern int g_tc_cluster;
 extern int g_tc_bk;
 extern int g_tc_tma_store;
@@ -48,7 +47,6 @@ extern "C" int gr_set_option(const char* name, int64_t value) {
   using namespace gr;
   GR_CHECK_ARG(name != nullptr, "null option name");
   if (!strcmp(name, "agg_tma")) { g_opt_agg_tma = (int)value; return GR_OK; }
-  if (!strcmp(name, "linear_tc")) { g_opt_linear_tc = (int)value; return GR_OK; }
   if (!strcmp(name, "tc_cluster")) { g_tc_cluster = (int)value; return GR_OK; }
   if (!strcmp(name, "tc_bk")) { g_tc_bk = (int)value; return GR_OK; }
   if (!strcmp(name, "tc_tma_store")) { g_tc_tma_store = (int)value; return GR_OK; }

@@ -19,7 +19,6 @@
 
 namespace gr {
 
-int g_opt_linear_tc = 0;   // gr_set_option("linear_tc", 0|1): route e2e linears through this kernel
 int g_tc_cluster = 2;      // gr_set_option("tc_cluster", 1|2): CTAs per cluster sharing W tiles by TMA multicast
 int g_tc_bk = 32;          // gr_set_option("tc_bk", 32|64): k-block width (64B / 128B swizzle)
 int g_tc_tma_store = 1;    // gr_set_option("tc_tma_store", 0|1): staged TMA-store epilogue vs direct per-row stores

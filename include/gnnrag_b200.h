@@ -53,10 +53,12 @@ typedef enum gr_status {
 
 int gr_abi_version(void);
 const char* gr_last_error(void);
-/* runtime switches: "agg_tma" (0|1: stage CSR slices with bulk TMA copies), "linear_tc" (0|1: split-bf16
- * wgmma GEMM for gr_linear when the shape allows), "tc_cluster" (1|2: CTAs per cluster that share the W
- * tiles of the wgmma GEMM through TMA multicast), "agg_abs_ws" (0|1: persistent warp-specialised build of the |v| aggregation
- * kernel).  Process-wide; set before launching work. */
+/* runtime switches: "agg_tma" (0|1: stage CSR slices with bulk TMA copies), "tc_cluster" (1|2: CTAs per cluster
+ * that share the W tiles of the wgmma GEMM through TMA multicast), "tc_bk" (32|64: k-block width of the wgmma GEMM),
+ * "tc_tma_store" (0|1: TMA-store epilogue of the wgmma GEMM where the outputs are 16-byte aligned), "agg_abs_ws"
+ * (0|1|2|3: build of the |v| aggregation kernel, see gr_aggregate_dual_abs), "fused_debug" (bits: timing decomposition
+ * of gr_fused_layer, see csrc/fused_layer.cu).  Process-wide; set before launching work.  Any other name returns
+ * GR_ERR_INVALID_ARG. */
 int gr_set_option(const char* name, int64_t value);
 static inline int64_t gr_pad4(int64_t n) { return (n + 3) & ~(int64_t)3; }
 

@@ -87,6 +87,7 @@ def test_argument_validation_returns_status_codes():
     rc = lib.gr_set_option(b"no_such_option", 1)
     assert rc == -1
     assert lib.gr_set_option(b"agg_tma", 0) == 0
+    assert lib.gr_set_option(b"linear_tc", 0) == -1 and b"unknown option" in lib.gr_last_error()   # never read: removed
     assert lib.gr_csr_build_workspace_bytes(1000, 100) > 0
     assert lib.gr_rank_workspace_bytes(4, 100) == 4 * 100 * 8
     with pytest.raises(_lib.GrError):

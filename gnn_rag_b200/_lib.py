@@ -63,6 +63,15 @@ SIGNATURES = {
                                     c_i64, c_i64, c_u32, c_void_p, c_size, c_void_p]),
     "gr_split_bf16": (c_int, [c_f32p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_i64, c_void_p]),
     "gr_masked_softmax": (c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_int, c_int, c_void_p]),
+    "gr_graft_stage_workspace_bytes": (c_size, [c_i64, c_i64]),
+    "gr_graft_stage": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p,
+                               c_int, c_int, c_i64, c_i64, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p,
+                               c_void_p, c_size, c_void_p]),
+    "gr_graft_attention": (c_int, [c_f32p, c_f32p, c_int, c_f32p, c_i64, c_i64, c_void_p, c_int, c_i64, c_int,
+                                   c_i32p, c_i32p, c_i32p, c_int, c_f32p, c_f32p, c_f32p, c_i32p, c_void_p]),
+    "gr_graft_aggregate": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_i64,
+                                   c_f32p, c_i64, c_f32p, c_dbl, c_f32p, c_i64, c_void_p, c_void_p, c_i64,
+                                   c_i64, c_i64, c_i64, c_f32p, c_f32p, c_int, c_int, c_int, c_void_p]),
     "gr_frontier_rows": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i64, c_i32p, c_i32p, c_void_p]),
     "gr_frontier_fixup": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p,
                                   c_f32p, c_f32p, c_f32p, c_void_p, c_void_p, c_i64, c_f32p, c_i64, c_f32p,

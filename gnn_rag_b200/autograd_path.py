@@ -314,3 +314,85 @@ def nsm_forward(model, batch):
     h1, f1 = eval_metric(model, pred_dist.detach(), answer_dist, seed_dist, local_entity)
     model.dist_history = dist_history
     return loss, pred, pred_dist, [h1.tolist(), f1.tolist()]
+
+
+def _graft_facts(graft, kb_fact_rel, B, N, dev):
+    """kb_adj_mat_graft -> (slot, head, tail) index vectors ordered by slot b*max_fact + f (build_adj_facts,
+    base_gnn.py:56-75: the head list (b, f, head) and the tail list (b, tail, f) paired by slot)."""
+    (e2f_b, e2f_f, e2f_e, _v0), (f2e_b, f2e_e, f2e_f, _v1) = graft
+
+    def idx(a):
+        if isinstance(a, torch.Tensor):
+            return a.to(device=dev, dtype=torch.int64)
+        return torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype=np.int64))).to(dev)
+    M = kb_fact_rel.shape[1]
+    kh, kt = idx(e2f_b) * M + idx(e2f_f), idx(f2e_b) * M + idx(f2e_f)
+    oh, ot = torch.argsort(kh), torch.argsort(kt)
+    slot = kh[oh]
+    if not torch.equal(slot, kt[ot]):
+        raise ValueError("kb_adj_mat_graft: the head and tail lists do not hold the same fact slots")
+    return slot, (idx(e2f_b) * N + idx(e2f_e))[oh], (idx(f2e_b) * N + idx(f2e_e))[ot]
+
+
+def graftnet_forward(model, batch):
+    """GraftNet forward with autograd (graftnet.py:135-183, graft_gnn.py:64-153) -> (loss, pred, pred_dist, [h1, f1]).
+    Per-fact messages are gathered and reduced with ``index_add_``; dropout sits where the reference applies it."""
+    (local_entity, query_entities, kb_adj_mat, graft, q_input, kb_fact_rel, seed_dist, _tb,
+     answer_dist) = batch[:9]
+    dev = model.word_embedding.weight.device
+    _require_cuda(dev)
+
+    def t(x, dtype):
+        x = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
+        return x.to(device=dev, dtype=dtype)
+    local_entity, q_input = t(local_entity, torch.int64), t(q_input, torch.int64)
+    seed_dist, answer_dist = t(seed_dist, torch.float32), t(answer_dist, torch.float32)
+    kb_fact_rel = t(kb_fact_rel, torch.int64)
+    B, N = local_entity.shape
+    Nt, D = B * N, model.entity_dim
+    layer = model.reasoning
+    drop = layer.linear_drop_train
+    rel = model.get_rel_feature_train()
+    if model.encode_type:
+        h = _type_layer(model.type_layer, _Facts(kb_adj_mat, dev, False, model.norm_rel), rel, Nt)
+    else:
+        h = model.entity_linear(model.entity_embedding(local_entity)).view(Nt, D)
+    enc = model.instruction
+    enc.encode_question_train(q_input)
+    qh, qnode, qmask = enc.query_hidden_emb, enc.query_node_emb, enc.query_mask_train
+    slot, head, tail = _graft_facts(graft, kb_fact_rel, B, N, dev)
+    # compute_attention (graft_gnn.py:64-87) over every slot
+    fact_emb = rel[kb_fact_rel]                                                   # [B, max_fact, D]
+    div = float(np.sqrt(D))
+    sim = torch.bmm(qh, fact_emb.transpose(1, 2)) / div
+    sim = F.softmax(sim + (1 - qmask.unsqueeze(2)) * VERY_NEG_NUMBER, dim=1)      # [B, Q, max_fact]
+    W = torch.sum(torch.bmm(sim.transpose(1, 2), qh) * fact_emb, dim=2) / div
+    W_tilde = torch.exp(W - torch.max(W, dim=1, keepdim=True)[0]).reshape(-1)[slot]
+    E = torch.clamp(torch.zeros(Nt, device=dev).index_add(0, head, W_tilde), min=1e-10)
+    mask = (local_entity != model.num_entity).float()
+    fact_rel = kb_fact_rel.reshape(-1)[slot]
+    d = seed_dist.reshape(-1)
+    query = qnode                                                                 # [B, 1, D]
+    dist_history, pagerank = [seed_dist], [seed_dist]
+    lam = layer.pagerank_lambda
+    for i in range(model.num_layer):
+        q2e = layer.lin("q2e_linear", i)(drop(query)).expand(B, N, D).reshape(Nt, D)
+        s = W_tilde * (d / E)[head]
+        v = F.relu(layer.lin("kb_self_linear", i)(rel)[fact_rel] + layer.lin("kb_head_linear", i)(drop(h))[head])
+        v = v * s.unsqueeze(1)
+        f2e = F.relu(layer.lin("kb_self_linear", i)(h) + torch.zeros(Nt, D, device=dev).index_add(
+            0, tail, layer.lin("kb_tail_linear", i)(drop(v))))
+        d = lam * torch.zeros(Nt, device=dev).index_add(0, tail, s) + (1 - lam) * d
+        x = torch.cat([h, q2e, layer.fact_scale * f2e], dim=1)
+        query = torch.bmm(d.view(B, 1, N), layer.lin("e2q_linear", i)(drop(x)).view(B, N, D))
+        h = F.relu(layer.lin("e2e_linear", i)(drop(x)))
+        logit = layer.score_func(drop(h)).view(B, N)
+        dist_history.append(F.softmax(logit + (1 - mask) * VERY_NEG_NUMBER, dim=1))
+        pagerank.append(d.view(B, N))
+    pred_dist = dist_history[-1]
+    case_valid = (torch.sum(answer_dist, dim=1, keepdim=True) > 0).float()
+    loss = model.calc_loss_label(logit, answer_dist, case_valid)
+    pred = torch.max(pred_dist, dim=1)[1]
+    h1, f1 = eval_metric(model, pred_dist.detach(), answer_dist, seed_dist, local_entity)
+    model.dist_history, model.pagerank_history = dist_history, pagerank
+    return loss, pred, pred_dist, [h1.tolist(), f1.tolist()]

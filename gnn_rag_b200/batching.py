@@ -97,3 +97,28 @@ def stage_batch(batch, device, num_rel_rows, normalized_gnn=False, norm_rel=Fals
         nbytes += 4 * F
     db.h2d_bytes = int(nbytes)
     return db
+
+
+def stage_graft_batch(batch, device, num_rel_rows, normalized_gnn=False, norm_rel=False):
+    """Copy one ``GraftSingleDataLoader.get_batch`` tuple (gnn/dataset_load_graft.py:113-149) to the device: the regular
+    CSRs of ``kb_adj_mat`` (the TypeLayer input) as :func:`stage_batch` builds them, plus the graft facts of
+    ``kb_adj_mat_graft`` paired by slot and ordered by (b, f) with their CSRs (``db.graft``, ops.GraftGraph)."""
+    if isinstance(batch, DeviceBatch):
+        return batch
+    (local_entity, query_entities, kb_adj_mat, kb_adj_mat_graft, q_input, kb_fact_rel, seed_dist, true_batch_id,
+     answer_dist) = batch[:9]
+    db = stage_batch((local_entity, query_entities, kb_adj_mat, q_input, seed_dist, true_batch_id, answer_dist),
+                     device, num_rel_rows, normalized_gnn, norm_rel)
+    (e2f_b, e2f_f, e2f_e, _v0), (f2e_b, f2e_e, f2e_f, _v1) = kb_adj_mat_graft
+
+    def idx(a):
+        if isinstance(a, torch.Tensor):
+            return a.to(device=device, dtype=torch.int64)
+        return _to_dev(np.asarray(a).astype(np.int64, copy=False), device)
+    rel = idx(kb_fact_rel)
+    if rel.dim() != 2:
+        rel = rel.view(db.B, -1)
+    db.graft = ops.graft_stage([idx(e2f_b), idx(e2f_f), idx(e2f_e)], [idx(f2e_b), idx(f2e_e), idx(f2e_f)], rel,
+                               db.B, db.N, num_rel_rows)
+    db.h2d_bytes += 8 * (rel.numel() + 3 * len(e2f_b) + 3 * len(f2e_b))
+    return db

@@ -1,0 +1,409 @@
+// GraftNet on the GPU: graft-tuple staging, query-conditioned fact attention and the per-layer PageRank aggregation.
+//
+// Reference: GraftLayer (gnn/modules/kg_reasoning/graft_gnn.py) on the batch of GraftSingleDataLoader.get_batch
+// (gnn/dataset_load_graft.py:70-149), with the sparse operators of BaseGNNLayer.build_adj_facts (base_gnn.py:56-75).
+//   gr_graft_stage      build_adj_facts: pairs the head list (b, f, head) and the tail list (b, tail, f) by fact slot
+//                       and orders the facts by (b, f), so gr_csr_build's stable CSRs list every row in slot order --
+//                       the order torch's CPU sparse bmm sums a row in.
+//   gr_graft_attention  compute_attention, graft_gnn.py:64-87: W per slot, W~ = exp(W - max_f W), E = max(sum, 1e-10).
+//   gr_graft_aggregate  reason_layer, graft_gnn.py:89-107 (the fact-side half): per tail row, in slot order,
+//                       s_f = W~_f * (d[head] / E[head]), v_f = relu(self_tab[r_f] + head_tab[head]) * s_f, and the
+//                       sums sum_f v_f, indeg, d' = lambda * sum_f s_f + (1 - lambda) * d.  No atomics: every output
+//                       row is owned by one warp, so results are bit-reproducible and do not depend on the loader's
+//                       permutation of the fact lists.
+#include <cub/device/device_scan.cuh>
+#include <cuda_bf16.h>
+
+#include <algorithm>
+
+#include "common.cuh"
+
+namespace gr {
+namespace {
+
+constexpr float kVeryNeg = -100000000000.0f;   // VERY_NEG_NUMBER, graft_gnn.py:11
+constexpr float kVerySmall = 1e-10f;           // VERY_SMALL_NUMBER, graft_gnn.py:10
+
+// status bits
+constexpr int kBadId = 1;         // batch / slot / node id out of range
+constexpr int kBadRel = 2;        // relation id out of range
+constexpr int kDupSlot = 4;       // a (b, f) slot listed twice in one list
+constexpr int kUnpaired = 8;      // a slot with a head but no tail or the reverse
+
+// ---- staging ------------------------------------------------------------------------------------------------------
+
+// One of the two graft lists -> dense per-slot node table (global node id, -1 = absent).
+__global__ void graft_scatter_kernel(const int64_t* __restrict__ bid, const int64_t* __restrict__ fid,
+                                     const int64_t* __restrict__ nid, int64_t F, int B, int N, int64_t max_fact,
+                                     int32_t* __restrict__ node_of, int32_t* __restrict__ status) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < F; i += stride) {
+    const int64_t b = bid[i], f = fid[i], e = nid[i];
+    if (b < 0 || b >= B || f < 0 || f >= max_fact || e < 0 || e >= N) {
+      atomicOr(status, kBadId);
+      continue;
+    }
+    const int32_t old = atomicExch(&node_of[b * max_fact + f], (int32_t)(b * N + e));
+    if (old != -1) atomicOr(status, kDupSlot);
+  }
+}
+
+__global__ void graft_flags_kernel(const int32_t* __restrict__ head_of, const int32_t* __restrict__ tail_of,
+                                   int64_t S, int32_t* __restrict__ flag, int32_t* __restrict__ status) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < S; s += stride) {
+    const bool h = head_of[s] >= 0, t = tail_of[s] >= 0;
+    if (h != t) atomicOr(status, kUnpaired);
+    flag[s] = (h && t) ? 1 : 0;
+  }
+}
+
+__global__ void graft_compact_kernel(const int32_t* __restrict__ head_of, const int32_t* __restrict__ tail_of,
+                                     const int32_t* __restrict__ flag, const int32_t* __restrict__ pos,
+                                     const int64_t* __restrict__ kb_fact_rel, int64_t S, int64_t R1, int64_t cap,
+                                     int32_t* __restrict__ heads, int32_t* __restrict__ rels,
+                                     int32_t* __restrict__ tails, int32_t* __restrict__ slot_of,
+                                     int32_t* __restrict__ nfacts, int32_t* __restrict__ status) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < S; s += stride) {
+    if (s == S - 1) *nfacts = (int32_t)min((int64_t)pos[s] + flag[s], cap);
+    if (!flag[s]) continue;
+    const int64_t p = pos[s];
+    if (p >= cap) continue;
+    int64_t r = kb_fact_rel[s];
+    if (r < 0 || r >= R1) {
+      atomicOr(status, kBadRel);
+      r = 0;
+    }
+    heads[p] = head_of[s];
+    tails[p] = tail_of[s];
+    rels[p] = (int32_t)r;
+    slot_of[p] = (int32_t)s;
+  }
+}
+
+struct StageWs {
+  size_t dense_bytes, scan_bytes, total;
+};
+
+StageWs stage_ws(int64_t S) {
+  StageWs w{};
+  w.dense_bytes = align_up((size_t)(S > 0 ? S : 1) * sizeof(int32_t), 256);
+  size_t tmp = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp, (const int32_t*)nullptr, (int32_t*)nullptr, (int)(S > 0 ? S : 1));
+  w.scan_bytes = align_up(tmp, 256);
+  w.total = 4 * w.dense_bytes + w.scan_bytes;
+  return w;
+}
+
+// ---- fact attention -----------------------------------------------------------------------------------------------
+
+template <int NC>
+__device__ __forceinline__ float warp_dot(const float (&x)[NC], const float* __restrict__ row, int D) {
+  const int lane = threadIdx.x & 31;
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    if (c < D) s = fmaf(x[k], __ldg(row + c), s);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  return s;
+}
+
+// One warp per fact slot (pads and dropped facts included: compute_attention runs over every slot, :71-81).
+// sim_q = <qh[b,q], rel[r]> / div + (1 - mask_q) * VERY_NEG;  a = softmax_q(sim);  W = <sum_q a_q qh[b,q], rel[r]> / div.
+template <int NC>
+__global__ void __launch_bounds__(256) graft_w_kernel(const float* __restrict__ qh, const float* __restrict__ qmask,
+                                                      int Q, const float* __restrict__ rel, int64_t ldr, int64_t R1,
+                                                      const int64_t* __restrict__ kb_fact_rel, int64_t S,
+                                                      int64_t max_fact, int D, float div, float* __restrict__ W,
+                                                      int32_t* __restrict__ status) {
+  const int lane = threadIdx.x & 31;
+  const int64_t s = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (s >= S) return;
+  const int64_t b = s / max_fact;
+  int64_t r = kb_fact_rel[s];
+  if (r < 0 || r >= R1) {
+    if (lane == 0) atomicOr(status, kBadRel);
+    r = 0;
+  }
+  float rv[NC];
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    rv[k] = c < D ? __ldg(rel + r * ldr + c) : 0.f;
+  }
+  const float* qb = qh + b * (int64_t)Q * D;
+  const float* mb = qmask + b * (int64_t)Q;
+  float mx = -INFINITY;
+  for (int q = 0; q < Q; ++q) {
+    const float sim = __fadd_rn(__fdiv_rn(warp_dot<NC>(rv, qb + (int64_t)q * D, D), div),
+                                __fmul_rn(1.0f - __ldg(mb + q), kVeryNeg));
+    mx = fmaxf(mx, sim);
+  }
+  float att[NC];
+#pragma unroll
+  for (int k = 0; k < NC; ++k) att[k] = 0.f;
+  float den = 0.f;
+  for (int q = 0; q < Q; ++q) {
+    const float* row = qb + (int64_t)q * D;
+    const float sim = __fadd_rn(__fdiv_rn(warp_dot<NC>(rv, row, D), div),
+                                __fmul_rn(1.0f - __ldg(mb + q), kVeryNeg));
+    const float e = expf(sim - mx);
+    den += e;
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D) att[k] = fmaf(e, __ldg(row + c), att[k]);
+    }
+  }
+  const float inv = 1.0f / den;
+#pragma unroll
+  for (int k = 0; k < NC; ++k) att[k] *= inv;
+  float w = 0.f;
+#pragma unroll
+  for (int k = 0; k < NC; ++k) w = fmaf(att[k], rv[k], w);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) w += __shfl_xor_sync(0xffffffffu, w, o);
+  if (lane == 0) W[s] = __fdiv_rn(w, div);
+}
+
+// One block per question: W~[b, f] = exp(W[b, f] - max_f W[b, f]) over every slot (graft_gnn.py:82-83).
+__global__ void __launch_bounds__(256) graft_wtilde_kernel(const float* __restrict__ W, int64_t max_fact,
+                                                           float* __restrict__ Wt) {
+  __shared__ float sm[32];
+  const float* w = W + blockIdx.x * max_fact;
+  float m = -INFINITY;
+  for (int64_t f = threadIdx.x; f < max_fact; f += blockDim.x) m = fmaxf(m, w[f]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float x = threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : -INFINITY;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, o));
+    if (threadIdx.x == 0) sm[0] = x;
+  }
+  __syncthreads();
+  m = sm[0];
+  for (int64_t f = threadIdx.x; f < max_fact; f += blockDim.x) Wt[blockIdx.x * max_fact + f] = expf(w[f] - m);
+}
+
+// E[n] = max(sum_{graft f: head_f = n} W~_f, 1e-10), summed in slot order over the head CSR (graft_gnn.py:84-85).
+__global__ void graft_e_kernel(const int32_t* __restrict__ rowptr_h, const int32_t* __restrict__ fact_h,
+                               const int32_t* __restrict__ slot_of, const float* __restrict__ Wt, int64_t Nt,
+                               float* __restrict__ E) {
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= Nt) return;
+  float s = 0.f;
+  for (int e = rowptr_h[n]; e < rowptr_h[n + 1]; ++e) s = __fadd_rn(s, Wt[slot_of[fact_h[e]]]);
+  E[n] = fmaxf(s, kVerySmall);
+}
+
+// ---- layer aggregation --------------------------------------------------------------------------------------------
+
+__device__ __forceinline__ void store_split(__nv_bfloat16* hi, __nv_bfloat16* lo, int64_t i, float y) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(y);
+  hi[i] = h;
+  lo[i] = __float2bfloat16_rn(y - __bfloat162float(h));
+}
+
+struct AggArgs {
+  const int32_t *rowptr, *src, *rel, *fact, *slot_of;
+  const float *Wt, *E, *prior, *self_tab, *head_tab, *q2e;
+  int64_t ld_self, ld_head;
+  float lam, one_minus_lam;
+  float* sum_out;
+  int64_t ld_sum;
+  __nv_bfloat16 *hi, *lo;
+  int64_t ld_planes, col_sum, col_indeg, col_q2e;
+  float *indeg_out, *prior_next;
+  int64_t Nt;
+  int N, D;
+};
+
+// One warp per destination (tail CSR) row; the lane owns columns lane + 32k.  Facts are visited in slot order.
+template <int NC>
+__global__ void __launch_bounds__(256) graft_aggregate_kernel(const AggArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int64_t n = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.Nt) return;
+  const int D = a.D;
+  float acc[NC];
+#pragma unroll
+  for (int k = 0; k < NC; ++k) acc[k] = 0.f;
+  float dsum = 0.f;
+  const int beg = a.rowptr[n], end = a.rowptr[n + 1];
+  for (int e = beg; e < end; ++e) {
+    const int h = __ldg(a.src + e);
+    const int r = __ldg(a.rel + e);
+    const int sl = __ldg(a.slot_of + __ldg(a.fact + e));
+    // e2f_softmax_normalized = W~ * (curr_dist / E)[head]   (graft_gnn.py:97)
+    const float s = __fmul_rn(__ldg(a.Wt + sl), __fdiv_rn(__ldg(a.prior + h), __ldg(a.E + h)));
+    dsum = __fadd_rn(dsum, s);
+    if (s == 0.f) continue;        // relu(x) * 0 == 0 for finite x: the fact adds nothing
+    const float* st = a.self_tab + (int64_t)r * a.ld_self;
+    const float* ht = a.head_tab + (int64_t)h * a.ld_head;
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D) {
+        const float x = fmaxf(__fadd_rn(__ldg(st + c), __ldg(ht + c)), 0.f);
+        acc[k] = __fadd_rn(acc[k], __fmul_rn(x, s));
+      }
+    }
+  }
+  const int64_t b = n / a.N;
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    if (c < D) {
+      if (a.sum_out) a.sum_out[n * a.ld_sum + c] = acc[k];
+      if (a.hi) {
+        store_split(a.hi, a.lo, n * a.ld_planes + a.col_sum + c, acc[k]);
+        if (a.q2e) store_split(a.hi, a.lo, n * a.ld_planes + a.col_q2e + c, __ldg(a.q2e + b * D + c));
+      }
+    }
+  }
+  if (lane == 0) {
+    const float deg = (float)(end - beg);
+    if (a.indeg_out) a.indeg_out[n] = deg;
+    if (a.hi) store_split(a.hi, a.lo, n * a.ld_planes + a.col_indeg, deg);
+    // next_curr_dist = lambda * next + (1 - lambda) * curr_dist   (graft_gnn.py:101-102)
+    a.prior_next[n] = __fadd_rn(__fmul_rn(a.lam, dsum), __fmul_rn(a.one_minus_lam, __ldg(a.prior + n)));
+  }
+}
+
+int nc_for(int D) { return D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16; }
+
+}  // namespace
+}  // namespace gr
+
+using namespace gr;
+
+extern "C" size_t gr_graft_stage_workspace_bytes(int64_t B, int64_t max_fact) {
+  return stage_ws(B * max_fact).total;
+}
+
+extern "C" int gr_graft_stage(const int64_t* e2f_b, const int64_t* e2f_f, const int64_t* e2f_e, int64_t F_e2f,
+                              const int64_t* f2e_b, const int64_t* f2e_e, const int64_t* f2e_f, int64_t F_f2e,
+                              const int64_t* kb_fact_rel, int B, int N, int64_t max_fact, int64_t R1, int32_t* heads,
+                              int32_t* rels, int32_t* tails, int32_t* slot_of, int32_t* nfacts, int32_t* status,
+                              void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && N > 0 && max_fact >= 0 && R1 > 0 && F_e2f >= 0 && F_f2e >= 0, "bad sizes");
+  GR_CHECK_ARG(nfacts && status && kb_fact_rel, "null pointer");
+  GR_CHECK_ARG((int64_t)B * N < 0x7fffffff && (int64_t)B * max_fact < 0x7fffffff, "B*N or B*max_fact exceeds int32");
+  GR_CHECK_ARG(F_e2f == 0 || (e2f_b && e2f_f && e2f_e && heads && rels && tails && slot_of), "null pointer");
+  GR_CHECK_ARG(F_f2e == 0 || (f2e_b && f2e_e && f2e_f), "null pointer");
+  const int64_t S = (int64_t)B * max_fact;
+  StageWs w = stage_ws(S);
+  if (workspace_bytes < w.total || !workspace) {
+    set_error("gr_graft_stage: workspace too small (%zu < %zu)", workspace_bytes, w.total);
+    return GR_ERR_WORKSPACE;
+  }
+  char* ws = reinterpret_cast<char*>(workspace);
+  int32_t* head_of = reinterpret_cast<int32_t*>(ws);
+  int32_t* tail_of = reinterpret_cast<int32_t*>(ws + w.dense_bytes);
+  int32_t* flag = reinterpret_cast<int32_t*>(ws + 2 * w.dense_bytes);
+  int32_t* pos = reinterpret_cast<int32_t*>(ws + 3 * w.dense_bytes);
+  void* tmp = ws + 4 * w.dense_bytes;
+  GR_CHECK_CUDA(cudaMemsetAsync(head_of, 0xff, 2 * w.dense_bytes, stream));
+  GR_CHECK_CUDA(cudaMemsetAsync(nfacts, 0, sizeof(int32_t), stream));
+  const int g1 = (int)std::min<int64_t>(ceil_div(std::max<int64_t>(std::max(F_e2f, F_f2e), 1), 256), 4096);
+  if (F_e2f > 0) {
+    graft_scatter_kernel<<<g1, 256, 0, stream>>>(e2f_b, e2f_f, e2f_e, F_e2f, B, N, max_fact, head_of, status);
+    GR_CHECK_LAUNCH();
+  }
+  if (S == 0) {           // no slots: every listed fact is out of range (reported by the scatter)
+    if (F_f2e > 0) {
+      graft_scatter_kernel<<<g1, 256, 0, stream>>>(f2e_b, f2e_f, f2e_e, F_f2e, B, N, max_fact, tail_of, status);
+      GR_CHECK_LAUNCH();
+    }
+    return GR_OK;
+  }
+  if (F_f2e > 0) {
+    graft_scatter_kernel<<<g1, 256, 0, stream>>>(f2e_b, f2e_f, f2e_e, F_f2e, B, N, max_fact, tail_of, status);
+    GR_CHECK_LAUNCH();
+  }
+  const int g2 = (int)std::min<int64_t>(ceil_div(S, 256), 8192);
+  graft_flags_kernel<<<g2, 256, 0, stream>>>(head_of, tail_of, S, flag, status);
+  GR_CHECK_LAUNCH();
+  size_t tmp_bytes = w.scan_bytes;
+  GR_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, pos, (int)S, stream));
+  graft_compact_kernel<<<g2, 256, 0, stream>>>(head_of, tail_of, flag, pos, kb_fact_rel, S, R1, F_e2f, heads, rels,
+                                               tails, slot_of, nfacts, status);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+extern "C" int gr_graft_attention(const float* qh, const float* qmask, int Q, const float* rel, int64_t ldr,
+                                  int64_t R1, const int64_t* kb_fact_rel, int B, int64_t max_fact, int D,
+                                  const int32_t* rowptr_h, const int32_t* fact_h, const int32_t* slot_of, int N,
+                                  float* W, float* Wt, float* E, int32_t* status, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512 && Q >= 0 && max_fact >= 0 && R1 > 0 && ldr >= D,
+               "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG(rowptr_h && E && status, "null pointer");
+  GR_CHECK_ARG(max_fact == 0 || (qh && qmask && rel && kb_fact_rel && W && Wt && fact_h && slot_of), "null pointer");
+  GR_CHECK_ARG(Q > 0 || max_fact == 0, "Q must be positive");
+  const int64_t S = (int64_t)B * max_fact, Nt = (int64_t)B * N;
+  if (S > 0) {
+    const float div = (float)sqrt((double)D);
+    const int grid = (int)ceil_div(S, 8);
+    switch (nc_for(D)) {
+      case 1: graft_w_kernel<1><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
+      case 2: graft_w_kernel<2><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
+      case 4: graft_w_kernel<4><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
+      case 8: graft_w_kernel<8><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
+      default: graft_w_kernel<16><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
+    }
+    GR_CHECK_LAUNCH();
+    graft_wtilde_kernel<<<B, 256, 0, stream>>>(W, max_fact, Wt);
+    GR_CHECK_LAUNCH();
+  }
+  graft_e_kernel<<<(int)ceil_div(Nt, 256), 256, 0, stream>>>(rowptr_h, fact_h, slot_of, Wt, Nt, E);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+extern "C" int gr_graft_aggregate(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                                  const int32_t* fact_t, const int32_t* slot_of, const float* Wt, const float* E,
+                                  const float* prior, const float* self_tab, int64_t ld_self, const float* head_tab,
+                                  int64_t ld_head, const float* q2e, double lambda, float* sum_out, int64_t ld_sum,
+                                  void* out_hi, void* out_lo, int64_t ld_planes, int64_t col_sum, int64_t col_indeg,
+                                  int64_t col_q2e, float* indeg_out, float* prior_next, int B, int N, int D,
+                                  void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512, "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG(rowptr_t && src_t && rel_t && fact_t && slot_of && Wt && E && prior && self_tab && head_tab &&
+                   prior_next, "null pointer");
+  GR_CHECK_ARG(ld_self >= D && ld_head >= D && (!sum_out || ld_sum >= D), "leading dimension smaller than D");
+  GR_CHECK_ARG(!out_hi || (out_lo && col_sum >= 0 && col_sum + D <= ld_planes && col_indeg >= 0 &&
+                           col_indeg < ld_planes && (!q2e || (col_q2e >= 0 && col_q2e + D <= ld_planes))),
+               "plane columns outside the row");
+  AggArgs a{};
+  a.rowptr = rowptr_t; a.src = src_t; a.rel = rel_t; a.fact = fact_t; a.slot_of = slot_of;
+  a.Wt = Wt; a.E = E; a.prior = prior; a.self_tab = self_tab; a.head_tab = head_tab; a.q2e = out_hi ? q2e : nullptr;
+  a.ld_self = ld_self; a.ld_head = ld_head;
+  a.lam = (float)lambda;                     // pagerank_lambda * x and (1 - pagerank_lambda) * y with the python
+  a.one_minus_lam = (float)(1.0 - lambda);   // double rounded once to fp32, as torch applies the scalars
+  a.sum_out = sum_out; a.ld_sum = ld_sum;
+  a.hi = reinterpret_cast<__nv_bfloat16*>(out_hi); a.lo = reinterpret_cast<__nv_bfloat16*>(out_lo);
+  a.ld_planes = ld_planes; a.col_sum = col_sum; a.col_indeg = col_indeg; a.col_q2e = col_q2e;
+  a.indeg_out = indeg_out; a.prior_next = prior_next;
+  a.Nt = (int64_t)B * N; a.N = N; a.D = D;
+  const int grid = (int)ceil_div(a.Nt, 8);
+  switch (nc_for(D)) {
+    case 1: graft_aggregate_kernel<1><<<grid, 256, 0, stream>>>(a); break;
+    case 2: graft_aggregate_kernel<2><<<grid, 256, 0, stream>>>(a); break;
+    case 4: graft_aggregate_kernel<4><<<grid, 256, 0, stream>>>(a); break;
+    case 8: graft_aggregate_kernel<8><<<grid, 256, 0, stream>>>(a); break;
+    default: graft_aggregate_kernel<16><<<grid, 256, 0, stream>>>(a); break;
+  }
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}

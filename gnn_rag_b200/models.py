@@ -7,6 +7,7 @@ gnn/train_model.py:236-252) and config keys (gnn/parsing.py) -- so the module dr
   BaseModel   gnn/models/base_model.py:10-297
   ReaRev      gnn/models/ReaRev/rearev.py:19-244
   NSM         gnn/models/NSM/nsm.py:19-254
+  GraftNet    gnn/models/GraftNet/graftnet.py:21-183
 
 ``model(batch)`` runs the hand-written CUDA path; ``model(batch, training=True)`` -- what ``Trainer_KBQA.train_epoch``
 calls (gnn/train_model.py:222) -- evaluates the same math with differentiable torch ops on the same parameters
@@ -19,8 +20,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import autograd_path, batching, ops
-from .modules import (AttnEncoder, BERTInstruction, Fusion, LSTMInstruction, NSMLayer, QueryReform, ReasonGNNLayer,
-                      TypeLayer)
+from .modules import (AttnEncoder, BERTInstruction, Fusion, GraftLayer, LSTMInstruction, NSMLayer, QueryReform,
+                      ReasonGNNLayer, TypeLayer)
 
 VERY_SMALL_NUMBER = 1e-10
 
@@ -341,4 +342,91 @@ class NSM(BaseModel):
             self.dist_history.append(dist)
         pred_dist = self.dist_history[-1]
         loss, pred = self._loss_and_pred(pred_dist, db.answer_dist)
+        return loss, pred, pred_dist, None
+
+
+class GraftNet(BaseModel):
+    """GraftNet (graftnet.py:21-183) on the 9-tuple of GraftSingleDataLoader.get_batch (10 with ``test=True``,
+    dataset_load_graft.py:113-149).  ``model(batch)`` runs the CUDA path (csrc/graft.cu + the wgmma GEMMs);
+    ``model(batch, training=True)`` the differentiable restatement of autograd_path.graftnet_forward."""
+
+    def __init__(self, args, num_entity, num_relation, num_word):
+        super().__init__(args, num_entity, num_relation, num_word)
+        D = self.entity_dim
+        self.num_layer = args["num_layer"]
+        self.loss_type = args["loss_type"]
+        self.model_name = args["model_name"].lower()
+        self.lm = args["lm"]
+        self.norm_rel = args["norm_rel"]
+        self.num_iter = self.num_layer
+        self.linear_dropout = args["linear_dropout"]
+        self.entity_linear = nn.Linear(self.ent_dim, D)
+        self.relation_linear1 = nn.Linear(self.rel_dim, D)
+        self.linear_drop = nn.Dropout(p=self.linear_dropout)
+        if self.encode_type:
+            self.type_layer = TypeLayer(D, D, self.linear_drop, self.device, self.norm_rel)
+        self.self_att_r = AttnEncoder(D)
+        self.reasoning = GraftLayer(args, num_entity, num_relation, D)
+        self.instruction = self._make_instruction(args)
+        if args["lm"] != "lstm":
+            self.relation_linear = nn.Linear(self.word_dim, D)    # graftnet.py:72 (unused in forward)
+        self.to(self.device)
+
+    def get_rel_feature_train(self):                               # graftnet.py:85-102
+        if self.rel_texts is None:
+            return self.relation_linear1(self.relation_embedding.weight)
+        if self.lm == "lstm":
+            raise NotImplementedError("relation texts with --lm lstm: the reference pools the relation states twice "
+                                      "and fails (graftnet.py:96-98)")
+        return self._rel_text_features(self.rel_features, self.rel_texts, self.self_att_r)
+
+    def get_rel_feature(self):
+        """fp32 relation features [R1, D]."""
+        if self.rel_texts is None:
+            lin = self.relation_linear1
+            return ops.rel_linear(self.relation_embedding.weight, lin.weight, lin.bias)
+        return self.get_rel_feature_train().contiguous()
+
+    def forward(self, batch, training=False):
+        """graftnet.py:135-183 -> (loss, pred, pred_dist, tp_list)."""
+        if training:
+            return autograd_path.graftnet_forward(self, batch)
+        with torch.no_grad():
+            return self._forward_infer(batch)
+
+    def _init_h(self, db, rel):                                    # graftnet.py:74-83
+        layer = self.reasoning
+        planes = layer.h_planes()
+        if self.encode_type:
+            self.type_layer(db.graph, ops.rel_features_from_tensors([rel]), layer.h32, planes)
+        else:
+            emb = self.entity_embedding(db.local_entity).view(db.B * db.N, -1).contiguous()
+            ops.linear(emb, self.entity_linear.weight, self.entity_linear.bias, out=layer.h32)
+            ops.split_bf16(layer.h32, planes[0], planes[1])
+
+    def _forward_infer(self, batch):
+        dev = self._check_ready()
+        db = batching.stage_graft_batch(batch, dev, self.num_relation + 1, self.normalized_gnn, self.norm_rel)
+        self.last_batch = db
+        enc = self.instruction
+        enc.encode_question(db.q_input)                            # graftnet.py:108-111 (the instructions are unused)
+        qh = enc.query_hidden_emb.contiguous()
+        qnode = enc.query_node_emb.reshape(db.B, -1)
+        rel = self.get_rel_feature()
+        layer = self.reasoning
+        layer.init_reason(db, rel, qh, enc.query_mask)
+        self._init_h(db, rel)
+        dist = db.seed_dist
+        self.dist_history = [dist]
+        self.pagerank_history = [dist]
+        query = qnode
+        for i in range(self.num_layer):                            # graftnet.py:163-165
+            score, dist, query = layer(dist, query, i, last=(i == self.num_layer - 1))
+            self.dist_history.append(score)
+            self.pagerank_history.append(dist)
+        pred_dist = self.dist_history[-1]
+        case_valid = (torch.sum(db.answer_dist, dim=1, keepdim=True) > 0).float()
+        loss = self.calc_loss_label(layer.logits(), db.answer_dist, case_valid)
+        pred = torch.max(pred_dist, dim=1)[1]
+        db.graft.check_status()
         return loss, pred, pred_dist, None

@@ -10,6 +10,7 @@ behind the C ABI (ops.py) instead of ``index_select`` / ``Linear``-over-facts / 
                      feeds the path, SURVEY.md 8a row 12)
   ReasonGNNLayer     gnn/modules/kg_reasoning/reasongnn.py:11-174
   NSMLayer           gnn/modules/kg_reasoning/nsm_gnn.py:14-112
+  GraftLayer         gnn/modules/kg_reasoning/graft_gnn.py:14-153
 """
 import torch
 import torch.nn as nn
@@ -90,6 +91,8 @@ class LSTMInstruction(nn.Module):
             self.num_ins = args["num_step"]
         elif "num_ins" in args:
             self.num_ins = args["num_ins"]
+        elif "num_layer" in args:                  # GraftNet's CLI args carry only num_layer
+            self.num_ins = args["num_layer"]
         else:
             self.num_ins = 1
         self.entity_dim = args["entity_dim"]
@@ -201,6 +204,8 @@ class BERTInstruction(nn.Module):
             self.num_ins = args["num_step"]
         elif "num_ins" in args:
             self.num_ins = args["num_ins"]
+        elif "num_layer" in args:                  # GraftNet's CLI args carry only num_layer
+            self.num_ins = args["num_layer"]
         else:
             self.num_ins = 1
         self.model = model
@@ -489,3 +494,124 @@ class NSMLayer(_GraphLayerBase):
                           out=self.X[self.cur], out_col0=D, seg_stride=D, w=w, possible=self.possible)
         mask = self.local_entity_mask * self.possible if self.reason_kb else self.local_entity_mask
         return self._e2e_and_score(getattr(self, "e2e_linear" + str(step)), mask, need_h32=False)
+
+
+class GraftLayer(nn.Module):
+    """GraftNet's reasoning layer (graft_gnn.py:14-153): query-conditioned fact attention once per forward, then per
+    layer a PageRank step over the graft facts and a node update.  Per layer i, on split-bf16 operand planes with five
+    D-column segments at pitch Dp, ``[sum_v | indeg | h | q2e | f2e]``:
+
+      head_tab = kb_head_i(h)                               GEMM over the h segment
+      gr_graft_aggregate                                    sum_v, indeg, q2e[b] -> planes; d' -> fp32
+      f2e = relu([sum_v | indeg | h] @ [W_tail | b_tail e_0 | W_self]^T + b_self)
+                                                            = relu(kb_self(h) + sum_f kb_tail(v_f)): the per-fact bias
+                                                              enters as indeg(n) * b_tail through the indeg column
+      query_emb = W_e2q (sum_n d' x) + (sum_n d') b_e2q     (not for the last layer: the reference never reads it)
+      h <- relu([h | q2e | f2e] @ [W_e2e[:, :2D] | fact_scale W_e2e[:, 2D:]]^T + b); score dot in the epilogue
+    """
+
+    K_SEGMENTS = 5
+    _plane_cache = {}
+
+    def __init__(self, args, num_entity, num_relation, entity_dim):
+        super().__init__()
+        self.num_entity, self.num_relation, self.entity_dim = num_entity, num_relation, entity_dim
+        self.num_layer = args["num_layer"]
+        self.pagerank_lambda = args["pagerank_lambda"]
+        self.fact_scale = args["fact_scale"]
+        self.k = 3
+        D = entity_dim
+        self.score_func = nn.Linear(D, 1)
+        for i in range(self.num_layer):
+            self.add_module("q2e_linear" + str(i), nn.Linear(D, D))
+            self.add_module("e2q_linear" + str(i), nn.Linear(self.k * D, D))
+            self.add_module("e2e_linear" + str(i), nn.Linear(self.k * D, D))
+            self.add_module("kb_head_linear" + str(i), nn.Linear(D, D))
+            self.add_module("kb_tail_linear" + str(i), nn.Linear(D, D))
+            self.add_module("kb_self_linear" + str(i), nn.Linear(D, D))
+        self.linear_drop_train = nn.Dropout(p=args.get("linear_dropout", 0.0))   # graft_gnn.py:32-33 (training path)
+
+    def lin(self, name, i):
+        return getattr(self, name + str(i))
+
+    def init_reason(self, db, rel, query_hidden_emb, query_mask):
+        """graft_gnn.py:45-61 + compute_attention (:64-87), which the reference runs at step 0.  ``rel``: fp32
+        relation features [R1, D]."""
+        D = self.entity_dim
+        if not (bool(ops.TC_LINEAR) and 8 <= D <= ops.TC_MAX_N_SPLIT):
+            raise NotImplementedError("GraftNet runs its GEMMs on the wgmma path: entity_dim must be in [8, %d]"
+                                      % ops.TC_MAX_N_SPLIT)
+        dev = db.local_entity.device
+        self.db, self.gg = db, db.graft
+        self.B, self.N = db.B, db.N
+        Nt = db.B * db.N
+        self.local_entity_mask = (db.local_entity != self.num_entity).float().view(-1)
+        self.Dp = (D + 15) // 16 * 16
+        Kp = (self.K_SEGMENTS * self.Dp + 63) // 64 * 64
+        key = (str(dev), Nt, Kp)
+        if key not in GraftLayer._plane_cache:
+            GraftLayer._plane_cache.clear()
+            GraftLayer._plane_cache[key] = [[torch.zeros(Nt, Kp, dtype=torch.bfloat16, device=dev) for _ in range(2)]
+                                            for _ in range(2)]
+        self.P = GraftLayer._plane_cache[key]
+        self.cur = 0
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.h32 = torch.empty(Nt, D, **f32)
+        self.f2e32 = torch.empty(Nt, D, **f32)
+        self.head_tab = torch.empty(Nt, D, **f32)
+        self.dots = torch.empty(2 * Nt, **f32)
+        self.self_tabs = [ops.rel_linear(rel, self.lin("kb_self_linear", i).weight, self.lin("kb_self_linear", i).bias)
+                          for i in range(self.num_layer)]
+        _w, self.W_tilde, self.E = ops.graft_attention(self.gg, query_hidden_emb, query_mask, rel)
+
+    def seg(self, planes, k, width=None):
+        c0 = k * self.Dp
+        c1 = c0 + (self.entity_dim if width is None else width)
+        return planes[0][:, c0:c1], planes[1][:, c0:c1]
+
+    def h_planes(self):
+        """Where the initial node embeddings go (the h segment of the current planes)."""
+        return self.seg(self.P[self.cur], 2)
+
+    def forward(self, dist, query_node, step, last):
+        """One layer (graft_gnn.py:111-153).  dist: PageRank prior [B, N]; query_node: [B, D] (query_node_emb at step
+        0, the previous layer's query_emb after).  Returns (score [B, N], next prior d' [B, N], query_emb or None)."""
+        D, Dp, B, N = self.entity_dim, self.Dp, self.B, self.N
+        hi, lo = self.P[self.cur]
+        e2e, e2q = self.lin("e2e_linear", step), self.lin("e2q_linear", step)
+        kh, kt, ks = self.lin("kb_head_linear", step), self.lin("kb_tail_linear", step), self.lin("kb_self_linear", step)
+        q2e_l = self.lin("q2e_linear", step)
+        ops.linear_tc_planes(hi[:, 2 * Dp:], lo[:, 2 * Dp:], Dp, kh.weight, kh.bias, out=self.head_tab, relu=False,
+                             k_seg=D, k_seg_pitch=Dp)
+        q2e = ops.linear(query_node.contiguous(), q2e_l.weight, q2e_l.bias)
+        d_next = ops.graft_aggregate(self.gg, self.W_tilde, self.E, dist, self.self_tabs[step], self.head_tab,
+                                     self.pagerank_lambda, q2e=q2e, planes=(hi, lo), col_sum=0, col_indeg=Dp,
+                                     col_q2e=3 * Dp)
+        W1 = torch.zeros(D, 3 * D, dtype=torch.float32, device=hi.device)
+        W1[:, :D] = kt.weight
+        W1[:, D] = kt.bias
+        W1[:, 2 * D:] = ks.weight
+        f2e_hi, f2e_lo = self.seg((hi, lo), 4, Dp)
+        ops.linear_tc_planes(hi, lo, 3 * Dp, W1, ks.bias, out=self.f2e32, out_planes=(f2e_hi, f2e_lo), relu=True,
+                             k_seg=D, k_seg_pitch=Dp)
+        query_emb = None
+        if not last:
+            # sum_n d'[n] x[n] with x = [h | q2e[b] | fact_scale f2e], from the layer-input h (graft_gnn.py:138-140)
+            mass = d_next.sum(dim=1, keepdim=True)
+            sx = torch.cat([ops.seed_retrieve(d_next, self.h32, B, N, D), mass * q2e,
+                            self.fact_scale * ops.seed_retrieve(d_next, self.f2e32, B, N, D)], dim=1)
+            query_emb = ops.linear(sx, e2q.weight, None)
+            query_emb += mass * e2q.bias
+        We = torch.cat([e2e.weight[:, :2 * D], self.fact_scale * e2e.weight[:, 2 * D:]], dim=1)
+        nhi, nlo = self.P[1 - self.cur]
+        ops.linear_tc_planes(hi[:, 2 * Dp:], lo[:, 2 * Dp:], 3 * Dp, We, e2e.bias, out=self.h32,
+                             out_planes=self.seg((nhi, nlo), 2), w_score=self.score_func.weight.view(-1),
+                             dots=self.dots, relu=True, k_seg=D, k_seg_pitch=Dp)
+        self.cur = 1 - self.cur
+        score = ops.masked_softmax(self.dots, self.score_func.bias, self.local_entity_mask, B, N)
+        return score, d_next, query_emb
+
+    def logits(self):
+        """score_func(h) of the last layer, unmasked [B, N] (the loss input, graft_gnn.py:144)."""
+        d = self.dots.view(2, -1)
+        return (d[0] + d[1] + self.score_func.bias).view(self.B, self.N)

@@ -886,3 +886,114 @@ def _rule_walks(adj, start, rule_off, rule_len, rule_lab):
         _lib.check(L.gr_rule_paths_write(_p(lv_node), _p(lv_parent), _p(d_len), _p(res_begin), _p(d_path_off),
                                          _p(d_elem_off), J, int(path_off[-1]), _p(paths), _stream()))
     return paths[: int(elem_off[-1])], counts, elem_off[:J]
+
+
+class GraftGraph:
+    """The graft facts of one batch (kb_adj_mat_graft, gnn/dataset_load_graft.py:70-102) staged on the device: facts
+    paired by slot and ordered by (b, f), their CSRs (``graph``: tail CSR = in-facts of every node, head CSR =
+    out-facts), ``slot_of`` = b*max_fact + f of each staged fact, and ``kb_fact_rel`` int64 [B, max_fact]."""
+
+    def __init__(self, B, N, max_fact, cap, device):
+        self.B, self.N, self.max_fact, self.cap = B, N, max_fact, cap
+        i32 = dict(dtype=torch.int32, device=device)
+        Fp = max(pad4(cap), 4)
+        self.heads, self.rels, self.tails, self.slot_of = (torch.empty(Fp, **i32) for _ in range(4))
+        self.nfacts = torch.zeros(1, **i32)
+        self.status = torch.zeros(1, **i32)
+        self.graph = None
+        self.kb_fact_rel = None
+
+    _MESSAGES = {1: "a batch, fact-slot or node id outside the batch", 2: "a relation id outside the relation table",
+                 4: "a fact slot listed twice", 8: "a fact slot with a head but no tail (or a tail but no head)"}
+
+    def check_status(self):
+        st = int(self.status.item())
+        if st:
+            why = "; ".join(m for bit, m in sorted(self._MESSAGES.items()) if st & bit)
+            raise RuntimeError("graft fact lists rejected: %s (offending entries were dropped or clamped)" % why)
+        self.graph.check_status()
+
+
+def _i64(x, name):
+    x = _cuda(x, torch.int64, name)
+    return x.contiguous()
+
+
+def graft_stage(e2f, f2e, kb_fact_rel, B, N, R1):
+    """e2f = (b, f, head), f2e = (b, tail, f): int64 CUDA tensors of kb_adj_mat_graft (the 1.0 values are not needed);
+    kb_fact_rel int64 [B, max_fact] -> GraftGraph (gr_graft_stage, then gr_csr_build over the staged facts)."""
+    e2f = [_i64(t, "e2f") for t in e2f]
+    f2e = [_i64(t, "f2e") for t in f2e]
+    kb_fact_rel = _i64(kb_fact_rel, "kb_fact_rel")
+    max_fact = kb_fact_rel.shape[1] if kb_fact_rel.dim() == 2 else 0
+    assert kb_fact_rel.shape[0] == B
+    F0, F1 = e2f[0].numel(), f2e[0].numel()
+    assert all(t.numel() == F0 for t in e2f) and all(t.numel() == F1 for t in f2e)
+    dev = kb_fact_rel.device
+    gg = GraftGraph(B, N, max_fact, F0, dev)
+    gg.kb_fact_rel = kb_fact_rel
+    L = _L()
+    nbytes = L.gr_graft_stage_workspace_bytes(B, max_fact)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    with _OpTimer("csr_build"):
+        rc = L.gr_graft_stage(_p(e2f[0]), _p(e2f[1]), _p(e2f[2]), F0, _p(f2e[0]), _p(f2e[1]), _p(f2e[2]), F1,
+                              _p(kb_fact_rel), B, N, max_fact, R1, _p(gg.heads), _p(gg.rels), _p(gg.tails),
+                              _p(gg.slot_of), _p(gg.nfacts), _p(gg.status), _p(ws), nbytes, _stream())
+    _lib.check(rc)
+    STATS.launches += 5
+    gg.graph = csr_build(gg.heads[:F0], gg.rels[:F0], gg.tails[:F0], B, N, R1, nfacts=gg.nfacts)
+    return gg
+
+
+def graft_attention(gg, qh, qmask, rel, out_w=False):
+    """Fact attention of GraftLayer.compute_attention (graft_gnn.py:64-87) -> (W or None, W~ [B, max_fact], E [B*N]).
+    qh [B,Q,D], qmask float [B,Q], rel [R1, D] (row view allowed)."""
+    qh = _cuda(qh, torch.float32, "qh").contiguous()
+    qmask = _cuda(qmask, torch.float32, "qmask").contiguous()
+    rel = _cuda(rel, torch.float32, "rel")
+    assert rel.stride(1) == 1
+    B, Q, D = qh.shape
+    dev = qh.device
+    S = B * gg.max_fact
+    W = torch.empty(max(S, 1), dtype=torch.float32, device=dev)
+    Wt = torch.empty(max(S, 1), dtype=torch.float32, device=dev)
+    E = torch.empty(B * gg.N, dtype=torch.float32, device=dev)
+    g = gg.graph
+    with _OpTimer("graft_attention"):
+        rc = _L().gr_graft_attention(_p(qh), _p(qmask), Q, _p(rel), rel.stride(0), rel.shape[0], _p(gg.kb_fact_rel),
+                                     B, gg.max_fact, D, _p(g.rowptr_h), _p(g.fact_h), _p(gg.slot_of), gg.N, _p(W),
+                                     _p(Wt), _p(E), _p(gg.status), _stream())
+    _lib.check(rc)
+    STATS.launches += 3 if S > 0 else 1
+    return (W[:S] if out_w else None), Wt[:S], E
+
+
+def graft_aggregate(gg, Wt, E, prior, self_tab, head_tab, lam, q2e=None, sum_out=None, planes=None, col_sum=0,
+                    col_indeg=0, col_q2e=0, indeg_out=None, prior_next=None):
+    """Fact side of one GraftLayer layer (graft_gnn.py:89-107, gr_graft_aggregate): returns prior_next [B, N] and
+    writes the per-row sum of v_f (fp32 ``sum_out`` and/or the split-bf16 ``planes`` at ``col_sum``), the in-degree and
+    the question vector ``q2e`` [B, D] into the planes."""
+    g = gg.graph
+    B, N = gg.B, gg.N
+    prior = _cuda(prior, torch.float32, "prior").contiguous()
+    self_tab = _cuda(self_tab, torch.float32, "self_tab")
+    head_tab = _cuda(head_tab, torch.float32, "head_tab")
+    D = self_tab.shape[1]
+    assert self_tab.stride(1) == 1 and head_tab.stride(1) == 1 and head_tab.shape[0] == B * N
+    if prior_next is None:
+        prior_next = torch.empty(B, N, dtype=torch.float32, device=prior.device)
+    if sum_out is not None:
+        assert sum_out.stride(1) == 1
+    if q2e is not None:
+        q2e = _cuda(q2e, torch.float32, "q2e").contiguous()
+    hi, lo = planes if planes is not None else (None, None)
+    with _AggTimer(("graft", 1)):
+        rc = _L().gr_graft_aggregate(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(gg.slot_of),
+                                     _p(Wt), _p(E), _p(prior), _p(self_tab), self_tab.stride(0), _p(head_tab),
+                                     head_tab.stride(0), _p(q2e), float(lam), _p(sum_out),
+                                     sum_out.stride(0) if sum_out is not None else 0, _p(hi), _p(lo),
+                                     hi.stride(0) if hi is not None else 0, col_sum, col_indeg, col_q2e,
+                                     _p(indeg_out), _p(prior_next), B, N, D, _stream())
+    _lib.check(rc)
+    STATS.launches += 1
+    return prior_next

@@ -132,7 +132,7 @@ def make_batch(seed, B, N, E, num_entity=WEBQSP_NUM_ENTITY, num_relation=WEBQSP_
     return out
 
 
-def model_args(model_name="ReaRev", entity_dim=200, num_iter=3, num_ins=2, num_gnn=3, num_step=3,
+def model_args(model_name="ReaRev", entity_dim=200, num_iter=3, num_ins=2, num_gnn=3, num_step=3, num_layer=3,
                data_folder="", use_cuda=False, **over):
     """The ``args`` dict the reference threads everywhere (gnn/parsing.py:13-125, main.py:33).
 
@@ -156,10 +156,79 @@ def model_args(model_name="ReaRev", entity_dim=200, num_iter=3, num_ins=2, num_g
     elif model_name == "NSM":
         args.update(num_step=num_step, reason_kb=False, lambda_constrain=0.0, lambda_back=0.0,
                     use_inverse_relation=False)
+    elif model_name == "GraftNet":                 # create_parser_graftnet, gnn/parsing.py:115-124; fact_scale :42
+        args.update(num_layer=num_layer, pagerank_lambda=0.8, loss_type="bce", use_inverse_relation=False,
+                    fact_scale=3)
     else:
         raise ValueError(model_name)
     args.update(over)
     return args
+
+
+def make_graft_batch(seed, B, N, E, num_entity=WEBQSP_NUM_ENTITY, num_relation=WEBQSP_NUM_RELATION,
+                     num_word=WEBQSP_NUM_WORD, fact_dropout=0.0, use_inverse_relation=False, test=False, **kw):
+    """One batch in the ``GraftSingleDataLoader.get_batch`` layout (gnn/dataset_load_graft.py:113-149):
+
+      [0] local_entity [1] query_entities [2] kb_adj_mat (as :func:`make_batch`, self-loops included)
+      [3] kb_adj_mat_graft = ((b, f, head, 1.0), (b, tail, f, 1.0))   the tuples only, no self-loops
+      [4] q_input [5] kb_fact_rel int64 [B, max_fact] [6] seed_dist [7] true_batch_id = None [8] answer_dist
+      ([9] answer_lists with ``test=True``)
+
+    The tuples of question b are the non-self-loop facts :func:`make_batch` draws for it.  As the loader does
+    (dataset_load_graft.py:27-102, dataset_load.py:265-291): max_fact = 2 * max_tuples + N; kb_fact_rel slots past the
+    tuples hold the pad relation ``num_relation`` (the last row of the [num_relation + 1, D] table); every question's
+    facts are permuted and only floor(n * (1 - fact_dropout)) of them kept.  With ``use_inverse_relation`` the relation
+    ids are drawn from the lower half, tuple i becomes graft facts 2i (head -> tail) and 2i+1 (tail -> head), and
+    kb_fact_rel[b, i] holds the INVERSE relation of tuple i -- the loader's own layout, which the model reads as is."""
+    base = make_batch(seed, B, N, E, num_entity=num_entity, num_relation=num_relation, num_word=num_word, test=test,
+                      **kw)
+    return graft_from_batch(base, seed, num_relation, fact_dropout, use_inverse_relation)
+
+
+def graft_from_batch(base, seed, num_relation, fact_dropout=0.0, use_inverse_relation=False):
+    """The graft tuple of :func:`make_graft_batch` around an existing ``make_batch`` tuple (its non-self-loop facts
+    are the tuples)."""
+    test = len(base) > 7
+    B, N = base[0].shape
+    local_entity, query_entities, kb, q_input, seed_dist, _tb, answer_dist = base[:7]
+    heads, rels, tails, bids, fids, wl, wrl = kb
+    loop = num_relation - 1
+    half = (num_relation - 1) // 2
+    rels = rels.copy()
+    if use_inverse_relation:
+        rels[rels != loop] %= half
+    kb = (heads, rels, tails, bids, fids, wl, wrl)
+    rs = np.random.RandomState(seed + 7919)
+    per_q = []
+    for b in range(B):
+        sel = np.nonzero((bids == b) & (rels != loop))[0]
+        per_q.append((heads[sel] - b * N, rels[sel], tails[sel] - b * N))
+    max_tuples = max([len(t[0]) for t in per_q] + [0])
+    max_fact = 2 * max_tuples + N
+    kb_fact_rel = np.full((B, max_fact), num_relation, dtype=np.int64)
+    lists = [[] for _ in range(6)]
+    for b, (h, r, t) in enumerate(per_q):
+        T = len(h)
+        if use_inverse_relation:
+            kb_fact_rel[b, :T] = r + half
+            e_head = np.stack([h, t], 1).reshape(-1)
+            e_tail = np.stack([t, h], 1).reshape(-1)
+            slots = np.arange(2 * T, dtype=np.int64)
+        else:
+            kb_fact_rel[b, :T] = r
+            e_head, e_tail, slots = h, t, np.arange(T, dtype=np.int64)
+        n = len(slots)
+        keep = rs.permutation(n)[: int(np.floor(n * (1 - fact_dropout)))]
+        for lst, arr in zip(lists, (np.full(len(keep), b, dtype=np.int64), slots[keep], e_head[keep],
+                                    np.full(len(keep), b, dtype=np.int64), e_tail[keep], slots[keep])):
+            lst.append(arr.astype(np.int64))
+    cat = [np.concatenate(x) if x else np.zeros(0, dtype=np.int64) for x in lists]
+    ones = np.ones(len(cat[0]))
+    graft = ((cat[0], cat[1], cat[2], ones), (cat[3], cat[4], cat[5], ones.copy()))
+    out = (local_entity, query_entities, kb, graft, q_input, kb_fact_rel, seed_dist, None, answer_dist)
+    if test:
+        out = out + (base[7],)
+    return out
 
 
 # Named workloads from BASELINE.json:configs / SURVEY.md §8

@@ -253,6 +253,54 @@ int gr_type_layer(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_
                   int B, int N, int D, int64_t F, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * GraftNet (csrc/graft.cu): GraftLayer, gnn/modules/kg_reasoning/graft_gnn.py, on the batch of
+ * GraftSingleDataLoader.get_batch (gnn/dataset_load_graft.py:113-149).
+ *
+ * gr_graft_stage: BaseGNNLayer.build_adj_facts (gnn/modules/kg_reasoning/base_gnn.py:56-75).  Input: the two lists
+ * of kb_adj_mat_graft as int64 device arrays -- head list (e2f_b, e2f_f, e2f_e) = (b, fact slot f, local head) and
+ * tail list (f2e_b, f2e_e, f2e_f) = (b, local tail, fact slot f) (dataset_load_graft.py:70-102) -- and kb_fact_rel
+ * int64 [B, max_fact].  Pairs head and tail by slot and writes the facts ordered by (b, f): heads / tails (global rows
+ * b*N + local), rels = kb_fact_rel[b, f], slot_of = b*max_fact + f, each int32 with capacity gr_pad4(F_e2f), and the
+ * count to nfacts (device int32[1]).  Feed them to gr_csr_build(F = F_e2f, nfacts): its stable CSRs then list every
+ * row in slot order, the order torch's sparse bmm sums a row in.  status (int32[1], OR-ed): 1 = batch / slot / node
+ * id out of range, 2 = relation id outside [0, R1), 4 = a slot listed twice, 8 = a slot with a head but no tail or the
+ * reverse.  Offending entries are dropped or clamped, never read out of bounds.
+ * Workspace: gr_graft_stage_workspace_bytes(B, max_fact).
+ *
+ * gr_graft_attention: GraftLayer.compute_attention (graft_gnn.py:64-87).  For EVERY slot (pads and dropped facts
+ * included) with r = kb_fact_rel[b, f]:
+ *     a_q = softmax_q(<qh[b,q], rel[r]>/sqrt(D) + (1 - qmask[b,q]) * -1e11),  W[b,f] = <sum_q a_q qh[b,q], rel[r]>/sqrt(D)
+ *     Wt[b,f] = exp(W[b,f] - max_f W[b,f]);   E[n] = max(sum_{graft f: head_f = n} Wt[f], 1e-10)  (head CSR, slot order)
+ * qh [B,Q,D], qmask float [B,Q], rel [R1, D] row stride ldr; W / Wt float [B*max_fact]; E float [B*N].
+ * rowptr_h / fact_h: the head CSR of gr_csr_build on the staged facts; slot_of from gr_graft_stage.  D <= 512.
+ *
+ * gr_graft_aggregate: the fact side of GraftLayer.reason_layer (graft_gnn.py:89-107) for one layer.  One destination
+ * row per tail-CSR row; its facts in slot order:
+ *     s_f = Wt[slot_f] * (prior[head_f] / E[head_f]),   v_f = relu(self_tab[r_f] + head_tab[head_f]) * s_f
+ *     sum[n] = sum_f v_f,   indeg[n] = number of facts,   prior_next[n] = lambda * sum_f s_f + (1 - lambda) * prior[n]
+ * self_tab = kb_self_linear_i(rel) [R1, D], head_tab = kb_head_linear_i(h) [B*N, D].  Outputs: prior_next (required);
+ * sum_out fp32 (optional); split-bf16 planes (optional, row stride ld_planes) with sum at columns col_sum.., indeg at
+ * column col_indeg and, when q2e [B, D] is given, the row's question vector q2e[b] at col_q2e.. -- the A operands of
+ * the f2e and e2e GEMMs; indeg_out fp32 [B*N] (optional).  No atomics: bit-reproducible.  D <= 512.
+ */
+size_t gr_graft_stage_workspace_bytes(int64_t B, int64_t max_fact);
+int gr_graft_stage(const int64_t* e2f_b, const int64_t* e2f_f, const int64_t* e2f_e, int64_t F_e2f,
+                   const int64_t* f2e_b, const int64_t* f2e_e, const int64_t* f2e_f, int64_t F_f2e,
+                   const int64_t* kb_fact_rel, int B, int N, int64_t max_fact, int64_t R1, int32_t* heads,
+                   int32_t* rels, int32_t* tails, int32_t* slot_of, int32_t* nfacts, int32_t* status,
+                   void* workspace, size_t workspace_bytes, void* stream);
+int gr_graft_attention(const float* qh, const float* qmask, int Q, const float* rel, int64_t ldr, int64_t R1,
+                       const int64_t* kb_fact_rel, int B, int64_t max_fact, int D, const int32_t* rowptr_h,
+                       const int32_t* fact_h, const int32_t* slot_of, int N, float* W, float* Wt, float* E,
+                       int32_t* status, void* stream);
+int gr_graft_aggregate(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t, const int32_t* fact_t,
+                       const int32_t* slot_of, const float* Wt, const float* E, const float* prior,
+                       const float* self_tab, int64_t ld_self, const float* head_tab, int64_t ld_head,
+                       const float* q2e, double lambda, float* sum_out, int64_t ld_sum, void* out_hi, void* out_lo,
+                       int64_t ld_planes, int64_t col_sum, int64_t col_indeg, int64_t col_q2e, float* indeg_out,
+                       float* prior_next, int B, int N, int D, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Sparse-prior fast path for one ReaRev layer (the first layer of every iteration sees the seed distribution,
  * rearev.py:208).  Rows none of whose in-edges carries prior mass get exactly zero neighbour messages, so
  * h_new = relu(W[:, :D] h + b) there (gr_linear_tc_planes with K = one segment).  gr_frontier_rows lists the

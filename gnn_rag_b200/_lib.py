@@ -66,7 +66,7 @@ SIGNATURES = {
     "gr_graft_stage_workspace_bytes": (c_size, [c_i64, c_i64]),
     "gr_graft_stage": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p,
                                c_int, c_int, c_i64, c_i64, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p,
-                               c_void_p, c_size, c_void_p]),
+                               c_i32p, c_void_p, c_size, c_void_p]),
     "gr_graft_attention": (c_int, [c_f32p, c_f32p, c_int, c_f32p, c_i64, c_i64, c_void_p, c_int, c_i64, c_int,
                                    c_i32p, c_i32p, c_i32p, c_int, c_f32p, c_f32p, c_f32p, c_i32p, c_void_p]),
     "gr_graft_aggregate": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_i64,

@@ -50,6 +50,17 @@ def pin_batch(batch):
             pin(ad.astype(np.float32)))
 
 
+def pin_graft_batch(batch):
+    """:func:`pin_batch` for a ``GraftSingleDataLoader.get_batch`` tuple: the kb part as there, the two graft lists and
+    ``kb_fact_rel`` as pinned int64 tensors."""
+    def pin(a, dtype=np.int64):
+        return torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype=dtype))).pin_memory()
+    le, qe, kb, qi, sd, tb, ad = pin_batch((batch[0], batch[1], batch[2], batch[4], batch[6], batch[7], batch[8]))
+    (hb, hf, he, hv), (tb_, te, tf, tv) = batch[3]
+    graft = ((pin(hb), pin(hf), pin(he), hv), (pin(tb_), pin(te), pin(tf), tv))
+    return (le, qe, kb, graft, qi, pin(batch[5]), sd, tb, ad) + tuple(batch[9:])
+
+
 def stage_batch(batch, device, num_rel_rows, normalized_gnn=False, norm_rel=False, nfacts=None):
     """Copy one ``get_batch`` tuple to the device and build its CSRs.  Returns DeviceBatch.
     ``nfacts``: optional int32[1] device tensor with the number of live facts when the fact arrays are fixed-capacity
@@ -99,16 +110,18 @@ def stage_batch(batch, device, num_rel_rows, normalized_gnn=False, norm_rel=Fals
     return db
 
 
-def stage_graft_batch(batch, device, num_rel_rows, normalized_gnn=False, norm_rel=False):
+def stage_graft_batch(batch, device, num_rel_rows, normalized_gnn=False, norm_rel=False, nfacts=None, graft_live=None):
     """Copy one ``GraftSingleDataLoader.get_batch`` tuple (gnn/dataset_load_graft.py:113-149) to the device: the regular
     CSRs of ``kb_adj_mat`` (the TypeLayer input) as :func:`stage_batch` builds them, plus the graft facts of
-    ``kb_adj_mat_graft`` paired by slot and ordered by (b, f) with their CSRs (``db.graft``, ops.GraftGraph)."""
+    ``kb_adj_mat_graft`` paired by slot and ordered by (b, f) with their CSRs (``db.graft``, ops.GraftGraph).
+    Fixed-capacity buffers (GraphedStep): ``nfacts`` int32[1] = live kb facts (see :func:`stage_batch`),
+    ``graft_live`` int32[2] = live entries of the graft head and tail lists (``ops.graft_stage(live=...)``)."""
     if isinstance(batch, DeviceBatch):
         return batch
     (local_entity, query_entities, kb_adj_mat, kb_adj_mat_graft, q_input, kb_fact_rel, seed_dist, true_batch_id,
      answer_dist) = batch[:9]
     db = stage_batch((local_entity, query_entities, kb_adj_mat, q_input, seed_dist, true_batch_id, answer_dist),
-                     device, num_rel_rows, normalized_gnn, norm_rel)
+                     device, num_rel_rows, normalized_gnn, norm_rel, nfacts=nfacts)
     (e2f_b, e2f_f, e2f_e, _v0), (f2e_b, f2e_e, f2e_f, _v1) = kb_adj_mat_graft
 
     def idx(a):
@@ -119,6 +132,6 @@ def stage_graft_batch(batch, device, num_rel_rows, normalized_gnn=False, norm_re
     if rel.dim() != 2:
         rel = rel.view(db.B, -1)
     db.graft = ops.graft_stage([idx(e2f_b), idx(e2f_f), idx(e2f_e)], [idx(f2e_b), idx(f2e_e), idx(f2e_f)], rel,
-                               db.B, db.N, num_rel_rows)
+                               db.B, db.N, num_rel_rows, live=graft_live)
     db.h2d_bytes += 8 * (rel.numel() + 3 * len(e2f_b) + 3 * len(f2e_b))
     return db

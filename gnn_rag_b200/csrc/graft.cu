@@ -32,10 +32,14 @@ constexpr int kUnpaired = 8;      // a slot with a head but no tail or the rever
 
 // ---- staging ------------------------------------------------------------------------------------------------------
 
-// One of the two graft lists -> dense per-slot node table (global node id, -1 = absent).
+// One of the two graft lists -> dense per-slot node table (global node id, -1 = absent).  ``live`` (optional device
+// int32): only the first min(F, *live) entries are read -- F is then the capacity of a fixed-shape buffer whose tail
+// holds whatever an earlier batch left there.
 __global__ void graft_scatter_kernel(const int64_t* __restrict__ bid, const int64_t* __restrict__ fid,
-                                     const int64_t* __restrict__ nid, int64_t F, int B, int N, int64_t max_fact,
-                                     int32_t* __restrict__ node_of, int32_t* __restrict__ status) {
+                                     const int64_t* __restrict__ nid, int64_t F, const int32_t* __restrict__ live,
+                                     int B, int N, int64_t max_fact, int32_t* __restrict__ node_of,
+                                     int32_t* __restrict__ status) {
+  if (live) F = min(F, (int64_t)max(*live, 0));
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < F; i += stride) {
     const int64_t b = bid[i], f = fid[i], e = nid[i];
@@ -292,7 +296,7 @@ extern "C" int gr_graft_stage(const int64_t* e2f_b, const int64_t* e2f_f, const 
                               const int64_t* f2e_b, const int64_t* f2e_e, const int64_t* f2e_f, int64_t F_f2e,
                               const int64_t* kb_fact_rel, int B, int N, int64_t max_fact, int64_t R1, int32_t* heads,
                               int32_t* rels, int32_t* tails, int32_t* slot_of, int32_t* nfacts, int32_t* status,
-                              void* workspace, size_t workspace_bytes, void* stream_) {
+                              const int32_t* live, void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   GR_CHECK_ARG(B > 0 && N > 0 && max_fact >= 0 && R1 > 0 && F_e2f >= 0 && F_f2e >= 0, "bad sizes");
   GR_CHECK_ARG(nfacts && status && kb_fact_rel, "null pointer");
@@ -313,20 +317,24 @@ extern "C" int gr_graft_stage(const int64_t* e2f_b, const int64_t* e2f_f, const 
   void* tmp = ws + 4 * w.dense_bytes;
   GR_CHECK_CUDA(cudaMemsetAsync(head_of, 0xff, 2 * w.dense_bytes, stream));
   GR_CHECK_CUDA(cudaMemsetAsync(nfacts, 0, sizeof(int32_t), stream));
+  // with live counts F_e2f / F_f2e are capacities: the launch shape depends on them only (fixed under graph capture)
   const int g1 = (int)std::min<int64_t>(ceil_div(std::max<int64_t>(std::max(F_e2f, F_f2e), 1), 256), 4096);
   if (F_e2f > 0) {
-    graft_scatter_kernel<<<g1, 256, 0, stream>>>(e2f_b, e2f_f, e2f_e, F_e2f, B, N, max_fact, head_of, status);
+    graft_scatter_kernel<<<g1, 256, 0, stream>>>(e2f_b, e2f_f, e2f_e, F_e2f, live, B, N, max_fact, head_of,
+                                                 status);
     GR_CHECK_LAUNCH();
   }
   if (S == 0) {           // no slots: every listed fact is out of range (reported by the scatter)
     if (F_f2e > 0) {
-      graft_scatter_kernel<<<g1, 256, 0, stream>>>(f2e_b, f2e_f, f2e_e, F_f2e, B, N, max_fact, tail_of, status);
+      graft_scatter_kernel<<<g1, 256, 0, stream>>>(f2e_b, f2e_f, f2e_e, F_f2e, live ? live + 1 : nullptr, B, N,
+                                                 max_fact, tail_of, status);
       GR_CHECK_LAUNCH();
     }
     return GR_OK;
   }
   if (F_f2e > 0) {
-    graft_scatter_kernel<<<g1, 256, 0, stream>>>(f2e_b, f2e_f, f2e_e, F_f2e, B, N, max_fact, tail_of, status);
+    graft_scatter_kernel<<<g1, 256, 0, stream>>>(f2e_b, f2e_f, f2e_e, F_f2e, live ? live + 1 : nullptr, B, N,
+                                                 max_fact, tail_of, status);
     GR_CHECK_LAUNCH();
   }
   const int g2 = (int)std::min<int64_t>(ceil_div(S, 256), 8192);

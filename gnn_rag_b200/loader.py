@@ -21,6 +21,15 @@ forward is invariant to the fact order up to fp32 summation order (SURVEY.md 7, 
 and with :func:`preconvert` (SURVEY.md 8f row 3: the per-question arrays flattened once at load time) the batch
 assembly is an offset concat.
 
+GraftNet's loader (``GraftSingleDataLoader``, gnn/dataset_load_graft.py) additionally calls
+``_build_fact_mat_maxfacts`` (:70-102) in every ``get_batch``: per question it re-parses the subgraph tuples
+(``create_kb_adj_mats_facts``, :27-68, a Python loop with dictionary lookups) and grows eight arrays by ``np.append``.
+:func:`build_fact_mat_maxfacts` is its drop-in -- same return values and dtypes, the same one ``permutation`` per
+question in order (so it interleaves with either ``_build_fact_mat`` under one seed), one concatenate per array, and
+the per-question triple taken from the loader's own ``create_kb_adj_mats_facts`` once per sample and cached:
+
+    loader.install_graft(GraftSingleDataLoader)    # monkeypatches _build_fact_mat_maxfacts
+
 Pure numpy on the host; nothing here touches the GPU.
 """
 import numpy as np
@@ -161,4 +170,53 @@ def install(loader, weights="lists", index_dtype=np.int64, shuffle=True):
     else:
         orig = loader._build_fact_mat
         loader._build_fact_mat = types.MethodType(patched, loader)
+    return orig
+
+
+def _graft_per_question(self, sample_id):
+    """``create_kb_adj_mats_facts(sample_id)`` of the loader itself, once per sample: the result is a pure function of
+    the loaded data, so it is cached on the instance (``_gr_graft``)."""
+    cache = self.__dict__.get("_gr_graft")
+    if cache is None:
+        cache = self._gr_graft = {}
+    ent = cache.get(sample_id)
+    if ent is None:
+        ((m00, m01, v0), (m10, m11, v1)), kb_fact_rel = self.create_kb_adj_mats_facts(sample_id)
+        assert len(v0) == len(v1)
+        ent = cache[sample_id] = (m00, m01, v0, m10, m11, v1, kb_fact_rel)
+    return ent
+
+
+def build_fact_mat_maxfacts(self, sample_ids, fact_dropout):
+    """-> ((mats0_batch, mats0_0, mats0_1, vals0), (mats1_batch, mats1_0, mats1_1, vals1)), kb_fact_rels,
+    gnn/dataset_load_graft.py:70-102, bit for bit (dtypes included) for the same ``np.random`` state."""
+    kb_fact_rels = np.full((len(sample_ids), self.max_facts), self.num_kb_relation, dtype=int)
+    # the reference grows each array from these empties by np.append: starting every concatenate from them gives the
+    # same dtype promotion
+    parts = [[np.array([], dtype=int)] for _ in range(3)] + [[np.array([], dtype=float)]] + \
+        [[np.array([], dtype=int)] for _ in range(3)] + [[np.array([], dtype=float)]]
+    for i, sample_id in enumerate(sample_ids):
+        m00, m01, v0, m10, m11, v1, kb_fact_rel = _graft_per_question(self, sample_id)
+        kb_fact_rels[i] = kb_fact_rel
+        num_fact = len(v0)
+        num_keep_fact = int(np.floor(num_fact * (1 - fact_dropout)))
+        mask_index = np.random.permutation(num_fact)[:num_keep_fact]      # same RNG stream as the reference (:90)
+        bcol = np.full(len(mask_index), i, dtype=int)
+        for lst, arr in zip(parts, (bcol, m00[mask_index], m01[mask_index], v0[mask_index],
+                                    bcol, m10[mask_index], m11[mask_index], v1[mask_index])):
+            lst.append(np.ravel(arr))
+    out = [np.concatenate(lst) for lst in parts]
+    return (tuple(out[:4]), tuple(out[4:])), kb_fact_rels
+
+
+def install_graft(loader):
+    """Monkeypatch ``_build_fact_mat_maxfacts`` on a reference graft loader class (or a single instance) with
+    :func:`build_fact_mat_maxfacts`.  Returns the original function so it can be restored."""
+    import types
+
+    orig = loader._build_fact_mat_maxfacts
+    if isinstance(loader, type):
+        loader._build_fact_mat_maxfacts = build_fact_mat_maxfacts
+    else:
+        loader._build_fact_mat_maxfacts = types.MethodType(build_fact_mat_maxfacts, loader)
     return orig

@@ -404,7 +404,9 @@ class GraftNet(BaseModel):
             ops.linear(emb, self.entity_linear.weight, self.entity_linear.bias, out=layer.h32)
             ops.split_bf16(layer.h32, planes[0], planes[1])
 
-    def _forward_infer(self, batch):
+    def _forward_infer(self, batch, check_status=True):
+        """``check_status=False``: skip the read-back of the staging status words (a host sync) -- for a caller that
+        reads ``db.graft.status`` / ``db.graph.status`` itself after the step (GraphedStep captures this forward)."""
         dev = self._check_ready()
         db = batching.stage_graft_batch(batch, dev, self.num_relation + 1, self.normalized_gnn, self.norm_rel)
         self.last_batch = db
@@ -428,5 +430,6 @@ class GraftNet(BaseModel):
         case_valid = (torch.sum(db.answer_dist, dim=1, keepdim=True) > 0).float()
         loss = self.calc_loss_label(layer.logits(), db.answer_dist, case_valid)
         pred = torch.max(pred_dist, dim=1)[1]
-        db.graft.check_status()
+        if check_status:
+            db.graft.check_status()
         return loss, pred, pred_dist, None

@@ -496,6 +496,13 @@ class NSMLayer(_GraphLayerBase):
         return self._e2e_and_score(getattr(self, "e2e_linear" + str(step)), mask, need_h32=False)
 
 
+def live_plane_buffers():
+    """Strong references to the operand planes the reasoning layers currently cache (held by GraphedStep entries: a
+    captured graph reads and writes them, and relies on their zero pad columns, after the cache has moved on)."""
+    return [t for cache in (_GraphLayerBase._plane_cache, GraftLayer._plane_cache) for sets in cache.values()
+            for pair in sets for t in pair]
+
+
 class GraftLayer(nn.Module):
     """GraftNet's reasoning layer (graft_gnn.py:14-153): query-conditioned fact attention once per forward, then per
     layer a PageRank step over the graft facts and a node update.  Per layer i, on split-bf16 operand planes with five

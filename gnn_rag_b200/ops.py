@@ -906,11 +906,15 @@ class GraftGraph:
     _MESSAGES = {1: "a batch, fact-slot or node id outside the batch", 2: "a relation id outside the relation table",
                  4: "a fact slot listed twice", 8: "a fact slot with a head but no tail (or a tail but no head)"}
 
-    def check_status(self):
-        st = int(self.status.item())
+    @classmethod
+    def raise_status(cls, st):
+        """Raise for a non-zero staging status word ``st`` (an int read back from ``status``)."""
         if st:
-            why = "; ".join(m for bit, m in sorted(self._MESSAGES.items()) if st & bit)
+            why = "; ".join(m for bit, m in sorted(cls._MESSAGES.items()) if st & bit)
             raise RuntimeError("graft fact lists rejected: %s (offending entries were dropped or clamped)" % why)
+
+    def check_status(self):
+        self.raise_status(int(self.status.item()))
         self.graph.check_status()
 
 
@@ -919,12 +923,17 @@ def _i64(x, name):
     return x.contiguous()
 
 
-def graft_stage(e2f, f2e, kb_fact_rel, B, N, R1):
+def graft_stage(e2f, f2e, kb_fact_rel, B, N, R1, live=None):
     """e2f = (b, f, head), f2e = (b, tail, f): int64 CUDA tensors of kb_adj_mat_graft (the 1.0 values are not needed);
-    kb_fact_rel int64 [B, max_fact] -> GraftGraph (gr_graft_stage, then gr_csr_build over the staged facts)."""
+    kb_fact_rel int64 [B, max_fact] -> GraftGraph (gr_graft_stage, then gr_csr_build over the staged facts).
+    ``live``: optional int32[2] device tensor with the live entries of the head and the tail list when the lists are
+    fixed-capacity buffers (GraphedStep); only those front parts are staged."""
     e2f = [_i64(t, "e2f") for t in e2f]
     f2e = [_i64(t, "f2e") for t in f2e]
     kb_fact_rel = _i64(kb_fact_rel, "kb_fact_rel")
+    if live is not None:
+        live = _cuda(live, torch.int32, "live")
+        assert live.numel() >= 2 and live.is_contiguous()
     max_fact = kb_fact_rel.shape[1] if kb_fact_rel.dim() == 2 else 0
     assert kb_fact_rel.shape[0] == B
     F0, F1 = e2f[0].numel(), f2e[0].numel()
@@ -938,7 +947,7 @@ def graft_stage(e2f, f2e, kb_fact_rel, B, N, R1):
     with _OpTimer("csr_build"):
         rc = L.gr_graft_stage(_p(e2f[0]), _p(e2f[1]), _p(e2f[2]), F0, _p(f2e[0]), _p(f2e[1]), _p(f2e[2]), F1,
                               _p(kb_fact_rel), B, N, max_fact, R1, _p(gg.heads), _p(gg.rels), _p(gg.tails),
-                              _p(gg.slot_of), _p(gg.nfacts), _p(gg.status), _p(ws), nbytes, _stream())
+                              _p(gg.slot_of), _p(gg.nfacts), _p(gg.status), _p(live), _p(ws), nbytes, _stream())
     _lib.check(rc)
     STATS.launches += 5
     gg.graph = csr_build(gg.heads[:F0], gg.rels[:F0], gg.tails[:F0], B, N, R1, nfacts=gg.nfacts)

@@ -38,6 +38,29 @@ def shard_batch(batch, rank, world):
     return out
 
 
+def shard_graft_batch(batch, rank, world):
+    """Slice a ``GraftSingleDataLoader.get_batch`` 9/10-tuple down to this rank's questions: the kb part as
+    :func:`shard_batch`; of both graft lists the entries of these questions, in their original order, with the
+    question id re-based (the fact slot f and the local node ids are per question already); ``kb_fact_rel``,
+    ``q_input``, the [B, N] arrays and ``answer_lists`` by rows."""
+    (local_entity, query_entities, kb, graft, q_input, kb_fact_rel, seed_dist, tb, answer_dist) = batch[:9]
+    B = local_entity.shape[0]
+    lo, hi = question_range(B, rank, world)
+    kb_part = shard_batch((local_entity, query_entities, kb, q_input, seed_dist, tb, answer_dist), rank, world)
+
+    def lists(lst, bcol):
+        b = np.asarray(lst[bcol])
+        sel = np.nonzero((b >= lo) & (b < hi))[0]
+        out = [np.asarray(a)[sel] for a in lst]
+        out[bcol] = out[bcol] - lo
+        return tuple(out)
+    graft2 = (lists(graft[0], 0), lists(graft[1], 0))
+    out = (kb_part[0], kb_part[1], kb_part[2], graft2, kb_part[3], kb_fact_rel[lo:hi], kb_part[4], tb, kb_part[6])
+    if len(batch) > 9:
+        out = out + (batch[9][lo:hi],)
+    return out
+
+
 def all_gather_scores(local_scores, B, group=None):
     """Gather per-rank ``[B_g, N]`` score blocks into the full ``[B, N]`` matrix on every rank (NCCL
     over NVLink on GPUs, gloo on CPU).  Ragged splits are padded to the largest block."""

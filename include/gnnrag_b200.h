@@ -265,7 +265,10 @@ int gr_type_layer(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_
  * row in slot order, the order torch's sparse bmm sums a row in.  status (int32[1], OR-ed): 1 = batch / slot / node
  * id out of range, 2 = relation id outside [0, R1), 4 = a slot listed twice, 8 = a slot with a head but no tail or the
  * reverse.  Offending entries are dropped or clamped, never read out of bounds.
- * Workspace: gr_graft_stage_workspace_bytes(B, max_fact).
+ * live (optional device int32[2], NULL = the whole lists): the live entries of the head list and of the tail list.
+ * F_e2f / F_f2e are then capacities of fixed-shape buffers and only the first min(F, live[k]) entries are read, so a
+ * stale capacity tail is never staged; the launch shape depends on the capacities only (CUDA-graph capture).
+ * Workspace: gr_graft_stage_workspace_bytes(B, max_fact) (depends on B * max_fact only).
  *
  * gr_graft_attention: GraftLayer.compute_attention (graft_gnn.py:64-87).  For EVERY slot (pads and dropped facts
  * included) with r = kb_fact_rel[b, f]:
@@ -288,7 +291,7 @@ int gr_graft_stage(const int64_t* e2f_b, const int64_t* e2f_f, const int64_t* e2
                    const int64_t* f2e_b, const int64_t* f2e_e, const int64_t* f2e_f, int64_t F_f2e,
                    const int64_t* kb_fact_rel, int B, int N, int64_t max_fact, int64_t R1, int32_t* heads,
                    int32_t* rels, int32_t* tails, int32_t* slot_of, int32_t* nfacts, int32_t* status,
-                   void* workspace, size_t workspace_bytes, void* stream);
+                   const int32_t* live, void* workspace, size_t workspace_bytes, void* stream);
 int gr_graft_attention(const float* qh, const float* qmask, int Q, const float* rel, int64_t ldr, int64_t R1,
                        const int64_t* kb_fact_rel, int B, int64_t max_fact, int D, const int32_t* rowptr_h,
                        const int32_t* fact_h, const int32_t* slot_of, int N, float* W, float* Wt, float* E,

@@ -1,11 +1,17 @@
 """GraftNet inference throughput on one GPU, per-kernel times, the aggregation's achieved bytes/s, the torch-CPU oracle
-on a bounded sample, and the GPU outputs against that oracle.
+on a bounded sample, the GPU outputs against that oracle, and the CUDA-graph serving leg.
 
     python scripts/graftnet_probe.py [--B 64] [--N 2000] [--E 6000] [--dims 50,200] [--steps 20] [--warmup 5]
-                                     [--cpu-questions 2] [--out results/graftnet_probe.json]
+                                     [--cpu-questions 2] [--graphed-only] [--out results/graftnet_probe.json]
 
 Device time comes from CUDA events around each forward; a 256 MB buffer is rewritten between steps so every step
-starts with a cold L2.  The card name and power limit are read in the same run (nvidia-smi query only)."""
+starts with a cold L2.  The card name and power limit are read in the same run (nvidia-smi query only).
+
+Graphed leg (``graphed`` per D): device ms per step of eager ``model(batch)`` + ``rank_candidates`` against
+``GraphedStep`` (static-buffer fill + replay), both from the same pinned batch, alternating, L2 flushed before each;
+end-to-end questions/s of ``submit`` / ``collect`` (two tickets in flight) over pageable-numpy batches whose fact
+counts differ (one ``max_fact``, as a loader's); and whether ``pred_dist`` and the candidate lists of the two paths are
+bit-identical."""
 import argparse
 import json
 import os
@@ -55,6 +61,8 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--cpu-questions", type=int, default=2)
+    ap.add_argument("--graphed-only", action="store_true", help="skip the per-kernel and CPU-oracle legs")
+    ap.add_argument("--e2e-steps", type=int, default=40)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     torch.cuda.set_device(0)
@@ -68,6 +76,10 @@ def main():
         args = S.model_args("GraftNet", entity_dim=D, num_layer=a.layers, word_dim=300, use_cuda=True)
         torch.manual_seed(0)
         m = G.GraftNet(dict(args), NUM_ENTITY, NUM_REL, NUM_WORD).cuda().eval()
+        if a.graphed_only:
+            res["dims"][D] = dict(graphed=graphed_leg(m, args, batch, flush, a))
+            print(json.dumps({D: res["dims"][D]}))
+            continue
         for _ in range(a.warmup):
             m(batch)
         times = []
@@ -107,12 +119,81 @@ def main():
                               aggregation_GBps=nbytes / (agg_ms * 1e-3) / 1e9 if agg_ms > 0 else None,
                               cpu_oracle_questions=k, cpu_oracle_s=cpu_s, cpu_oracle_questions_per_s=k / cpu_s,
                               pred_dist_rel_err_vs_oracle=err)
+        res["dims"][D]["graphed"] = graphed_leg(m, args, batch, flush, a)
         print(json.dumps({D: res["dims"][D]}))
     print(json.dumps(dict((k, v) for k, v in res.items() if k != "dims")))
     if a.out:
         os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
         with open(a.out, "w") as f:
             json.dump(res, f, indent=1)
+
+
+def _pad_max_fact(batch, width):
+    """kb_fact_rel padded to ``width`` slots with the pad relation (a loader's max_facts is one dataset constant)."""
+    kfr = batch[5]
+    wide = np.full((kfr.shape[0], width), NUM_REL, dtype=np.int64)
+    wide[:, :kfr.shape[1]] = kfr
+    return batch[:5] + (wide,) + batch[6:]
+
+
+def graphed_leg(m, args, batch, flush, a):
+    from gnn_rag_b200 import batching, evaluate
+    eps = args["eps"]
+    gs = G.GraphedStep(m, NUM_ENTITY)
+    pinned = batching.pin_graft_batch(batch)
+
+    def eager():
+        _l, _p, pd, _ = m(pinned)
+        ops.rank_candidates(pd, m.last_batch.local_entity, m.last_batch.query_entities, NUM_ENTITY, eps)
+
+    def graph():
+        gs(pinned)
+
+    for _ in range(a.warmup):
+        eager()
+        graph()
+    t = {"eager": [], "graphed": []}
+    for _ in range(a.steps):
+        for name, fn in (("eager", eager), ("graphed", graph)):
+            flush.add_(1.0)
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            fn()
+            e.record()
+            torch.cuda.synchronize()
+            t[name].append(s.elapsed_time(e))
+    out = dict((k + "_ms_per_step", float(np.median(v))) for k, v in t.items())
+    out.update((k + "_ms_min", float(np.min(v))) for k, v in t.items())
+    out["graphed_speedup"] = out["eager_ms_per_step"] / out["graphed_ms_per_step"]
+    # bit-for-bit: pred_dist and the candidate lists of the two paths on the same batch
+    _l, _p, pd_e, _ = m(batch)
+    ret_e, _ = evaluate.retrieve(pd_e, m.last_batch, NUM_ENTITY, eps)
+    pd_e = pd_e.clone()
+    o = gs(batch)
+    ret_g, _ = gs.retrieve(o)
+    out["pred_dist_bit_identical"] = bool(torch.equal(o.pred_dist, pd_e))
+    out["candidate_lists_identical"] = [r.ent.tolist() for r in ret_g] == [r.ent.tolist() for r in ret_e] and \
+        [r.prob.tolist() for r in ret_g] == [r.prob.tolist() for r in ret_e]
+    # end to end: pageable numpy batches with different fact counts, two tickets in flight
+    pool = [S.make_graft_batch(100 + i, a.B, a.N, a.E + d, num_entity=NUM_ENTITY, num_relation=NUM_REL,
+                               num_word=NUM_WORD, with_weights=False) for i, d in enumerate((0, -150, 120, -60))]
+    width = max(b[5].shape[1] for b in pool)
+    pool = [_pad_max_fact(b, width) for b in pool]
+    for b in pool:                     # capture / warm every bucket outside the timed window
+        gs.collect(gs.submit(b))
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    prev = None
+    for i in range(a.e2e_steps):
+        tk = gs.submit(pool[i % len(pool)])
+        if prev is not None:
+            gs.collect(prev)
+        prev = tk
+    gs.collect(prev)
+    wall = time.perf_counter() - t0
+    out.update(e2e_questions_per_s=a.B * a.e2e_steps / wall, e2e_steps=a.e2e_steps, e2e_graphs=len(gs._cache),
+               e2e_facts=[int(len(b[2][0])) for b in pool], e2e_graft_facts=[int(len(b[3][0][0])) for b in pool])
+    return out
 
 
 def _slice(batch, k):

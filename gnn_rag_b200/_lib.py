@@ -72,6 +72,16 @@ SIGNATURES = {
     "gr_graft_aggregate": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_i64,
                                    c_f32p, c_i64, c_f32p, c_dbl, c_f32p, c_i64, c_void_p, c_void_p, c_i64,
                                    c_i64, c_i64, c_i64, c_f32p, c_f32p, c_int, c_int, c_int, c_void_p]),
+    "gr_graft_dropout_mask": (c_int, [c_void_p, c_dbl, c_i64, c_int, c_void_p, c_void_p]),
+    "gr_graft_aggregate_train": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_f32p, c_i64,
+                                         c_void_p, c_dbl, c_f32p, c_i64, c_int, c_int, c_int, c_void_p]),
+    "gr_graft_aggregate_backward": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_f32p,
+                                            c_i64, c_void_p, c_dbl, c_f32p, c_i64, c_f32p, c_f32p, c_i64, c_f32p, c_i64,
+                                            c_int, c_int, c_int, c_void_p]),
+    "gr_graft_attention_backward": (c_int, [c_f32p, c_f32p, c_int, c_f32p, c_i64, c_i64, c_void_p, c_int, c_i64,
+                                            c_int, c_f32p, c_f32p, c_f32p, c_i64, c_void_p]),
+    "gr_type_layer_backward": (c_int, [c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_f32p, c_i64,
+                                       c_f32p, c_i64, c_int, c_int, c_int, c_i64, c_void_p]),
     "gr_frontier_rows": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i64, c_i32p, c_i32p, c_void_p]),
     "gr_frontier_fixup": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p,
                                   c_f32p, c_f32p, c_f32p, c_void_p, c_void_p, c_i64, c_f32p, c_i64, c_f32p,

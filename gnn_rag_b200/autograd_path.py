@@ -1,6 +1,6 @@
 """Differentiable forward for ``model(batch, training=True)`` (gnn/train_model.py:209-233).
 
-The inference path runs hand-written CUDA kernels without a backward; ``Trainer_KBQA.train_epoch`` needs
+The inference path runs hand-written CUDA kernels; ``Trainer_KBQA.train_epoch`` needs
 ``loss.backward()`` through the same parameters.  This module evaluates the same math with torch ops on the model's
 device (CUDA when the model lives there -- no CPU fallback is involved) so that autograd provides the gradients:
 
@@ -8,7 +8,10 @@ device (CUDA when the model lives there -- no CPU fallback is involved) so that 
   * messages are formed per fact (``relu(P[rel] * ins[batch]) * w^2 * prior[src]``) and reduced with ``index_add_``
     (deterministic order is not needed for training);
   * dropouts are applied where the reference applies them (``linear_drop`` before e2e / score / instruction linears,
-    ``lstm_drop`` on the word embeddings), active only under ``model.train()``.
+    ``lstm_drop`` on the word embeddings), active only under ``model.train()``;
+  * on CUDA with ``USE_KERNELS`` the aggregations, the TypeLayer and GraftNet's fact attention and fact messages run
+    in hand-written kernels with their own backward (the ``torch.autograd.Function``s below); the per-fact torch
+    restatement is the CPU reference under ``HOST_CHECK`` and the ``USE_KERNELS = False`` path.
 
 Reference: ReaRev.forward gnn/models/ReaRev/rearev.py:163-243, ReasonGNNLayer.forward gnn/modules/kg_reasoning/
 reasongnn.py:61-174, TypeLayer.forward gnn/modules/layer_init.py:25-62, BaseInstruction.get_instruction
@@ -54,8 +57,13 @@ def _scatter_rows(values, dst, rows):
     return out.index_add_(0, dst, values)
 
 
-def _type_layer(layer, facts, rel_features, Nt):
-    """layer_init.py:44-59: relu(sum over facts into tails + sum over facts into heads) of kb_self_linear(rel)."""
+def _type_layer(layer, facts, rel_features, Nt, graph=None):
+    """layer_init.py:44-59: relu(sum over facts into tails + sum over facts into heads) of kb_self_linear(rel).
+    With the batch's CsrGraph (kernel path) the sums and their backward run in gr_type_layer /
+    gr_type_layer_backward (_TypeLayerFn); otherwise per fact with index_add."""
+    if graph is not None:
+        wt, wh = (graph.wr_t, graph.wr_h) if layer.norm_rel else (None, None)
+        return _TypeLayerFn.apply(layer.kb_self_linear(rel_features), graph, wt, wh)
     fact_val = layer.kb_self_linear(rel_features)[facts.rels]
     if facts.wr is not None:
         fact_val = fact_val * facts.wr.unsqueeze(1)
@@ -106,12 +114,58 @@ class _AggregateFn(torch.autograd.Function):
         return gt, gi, gp, None, None, None
 
 
-def _kernel_graph(model, batch, device, D, I):
-    """CSR of the batch for the kernel path, or None (CPU tensors / shapes the backward kernel does not cover)."""
-    if not (USE_KERNELS and device.type == "cuda" and D <= 256 and I <= 4):
+class _TypeLayerFn(torch.autograd.Function):
+    """out = relu(sum_{tail CSR} w_e table[rel_e] + sum_{head CSR} w_e table[rel_e]) (TypeLayer, layer_init.py:46-57):
+    forward = gr_type_layer (csrc/aggregate.cu), backward = gr_type_layer_backward (csrc/aggregate_bwd.cu); saves the
+    [B*N, D] output for the relu mask."""
+
+    @staticmethod
+    def forward(ctx, table, graph, w_t, w_h):
+        from . import ops
+        out = torch.empty(graph.B * graph.N, table.shape[1], dtype=torch.float32, device=table.device)
+        ops.type_layer(graph, table.detach(), out, w_t, w_h)
+        ctx.save_for_backward(out)
+        ctx.graph, ctx.w, ctx.rows = graph, (w_t, w_h), table.shape[0]
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from . import ops
+        out, = ctx.saved_tensors
+        gt = torch.zeros(ctx.rows, out.shape[1], dtype=torch.float32, device=out.device)
+        ops.type_layer_backward(ctx.graph, grad_out.contiguous(), out, gt, *ctx.w)
+        return gt, None, None, None
+
+
+FACT_KERNEL_MAX_D = 512    # widths the TypeLayer / GraftNet training kernels cover; wider models keep the torch ops
+
+
+def _fact_kernels(device, D):
+    """True when the TypeLayer and GraftNet's fact-level work run in the training kernels: CUDA, ``USE_KERNELS`` and
+    D <= FACT_KERNEL_MAX_D (the per-fact torch ops otherwise, as before those kernels existed)."""
+    return bool(USE_KERNELS and device.type == "cuda" and D <= FACT_KERNEL_MAX_D)
+
+
+def _type_layer_graph(model, batch, device, D):
+    """The batch's CSR for the TypeLayer kernels, or None (no TypeLayer, or a shape / device they do not cover)."""
+    return _batch_graph(model, batch, device) if model.encode_type and _fact_kernels(device, D) else None
+
+
+def _batch_graph(model, batch, device):
+    """CSR of the batch for the kernel path (with the normalized_gnn / norm_rel weights the model uses), or None (CPU
+    tensors, or ``USE_KERNELS`` off)."""
+    if not (USE_KERNELS and device.type == "cuda"):
         return None
     from . import batching
-    return batching.stage_batch(batch, device, model.num_relation + 1, model.normalized_gnn, False).graph
+    return batching.stage_batch(batch, device, model.num_relation + 1, model.normalized_gnn, model.norm_rel).graph
+
+
+def _kernel_graph(model, batch, device, D, I, graph=None):
+    """CSR of the batch for the aggregation kernels, or None (CPU tensors / shapes the backward kernel does not cover).
+    ``graph``: the batch's CSR if it was already staged (for the TypeLayer)."""
+    if not (USE_KERNELS and device.type == "cuda" and D <= 256 and I <= 4):
+        return None
+    return graph if graph is not None else _batch_graph(model, batch, device)
 
 
 def _neighbours(table_f, table_i, ins, dist, facts, graph, Nt):
@@ -231,8 +285,9 @@ def rearev_forward(model, batch):
     Nt, D, I = B * N, model.entity_dim, model.num_ins
     layer = model.reasoning
     rel_f, rel_f_inv = model.get_rel_feature_train()
+    graph = _type_layer_graph(model, batch, local_entity.device, D)
     if model.encode_type:
-        h = _type_layer(model.type_layer, facts, rel_f, Nt)
+        h = _type_layer(model.type_layer, facts, rel_f, Nt, graph)
     else:
         h = model.entity_linear(model.entity_embedding(local_entity)).view(Nt, D)
     instructions = _instructions(model.instruction, q_input)           # [B, I, D]
@@ -250,7 +305,7 @@ def rearev_forward(model, batch):
         tables.append((tf, ti))
     dist_history = [seed_dist]
     dist = seed_dist
-    graph = _kernel_graph(model, batch, h.device, D, I)
+    graph = _kernel_graph(model, batch, h.device, D, I, graph)
     for _t in range(model.num_iter):
         dist = seed_dist
         ins = torch.stack(ins_list, dim=1)                                  # [B, I, D]
@@ -283,8 +338,9 @@ def nsm_forward(model, batch):
     Nt, D = B * N, model.entity_dim
     layer = model.reasoning
     rel_f = model.get_rel_feature_train()
+    graph = _type_layer_graph(model, batch, local_entity.device, D)
     if model.encode_type:
-        h = _type_layer(model.type_layer, facts, rel_f, Nt)
+        h = _type_layer(model.type_layer, facts, rel_f, Nt, graph)
     else:
         h = model.entity_linear(model.entity_embedding(local_entity)).view(Nt, D)
     instructions = _instructions(model.instruction, q_input)
@@ -292,7 +348,7 @@ def nsm_forward(model, batch):
     drop = layer.linear_drop_train
     dist = seed_dist
     dist_history = [dist]
-    graph = _kernel_graph(model, batch, h.device, D, 1)
+    graph = _kernel_graph(model, batch, h.device, D, 1, graph)
     for k in range(model.num_step):
         table = getattr(layer, "rel_linear" + str(k))(rel_f)
         pf = dist.reshape(-1)
@@ -334,9 +390,75 @@ def _graft_facts(graft, kb_fact_rel, B, N, dev):
     return slot, (idx(e2f_b) * N + idx(e2f_e))[oh], (idx(f2e_b) * N + idx(f2e_e))[ot]
 
 
+class _GraftAttentionFn(torch.autograd.Function):
+    """W [B, max_fact] of compute_attention (graft_gnn.py:64-87) for every slot: forward = gr_graft_attention,
+    backward = gr_graft_attention_backward (csrc/graft.cu), which recomputes the per-slot softmax."""
+
+    @staticmethod
+    def forward(ctx, qh, rel, qmask, gg):
+        from . import ops
+        W, _wt, _e = ops.graft_attention(gg, qh.detach(), qmask, rel.detach().contiguous(), out_w=True)
+        ctx.save_for_backward(qh, rel, qmask)
+        ctx.gg = gg
+        return W.view(gg.B, gg.max_fact)
+
+    @staticmethod
+    def backward(ctx, grad_W):
+        from . import ops
+        qh, rel, qmask = ctx.saved_tensors
+        gq = torch.zeros(qh.shape, dtype=torch.float32, device=qh.device)
+        gr = torch.zeros(rel.shape, dtype=torch.float32, device=rel.device)
+        ops.graft_attention_backward(ctx.gg, qh, qmask, rel.contiguous(), grad_W.reshape(-1), gq, gr)
+        return gq, gr, None, None
+
+
+class _GraftAggregateFn(torch.autograd.Function):
+    """sum_out[n] = sum_{f -> n} drop_f(relu(self_tab[r_f] + head_tab[head_f])) * s_f over the staged graft facts
+    (graft_gnn.py:103-107 before kb_tail_linear): forward = gr_graft_aggregate_train, backward =
+    gr_graft_aggregate_backward.  The dropout mask is recomputed from the saved seed, never stored."""
+
+    @staticmethod
+    def forward(ctx, self_tab, head_tab, s, gg, seed, p):
+        from . import ops
+        out = ops.graft_aggregate_train(gg, s.detach(), self_tab.detach().contiguous(), head_tab.detach().contiguous(),
+                                        seed, p)
+        ctx.save_for_backward(self_tab, head_tab, s, seed)
+        ctx.gg, ctx.p = gg, p
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from . import ops
+        self_tab, head_tab, s, seed = ctx.saved_tensors
+        gs = torch.zeros(s.shape, dtype=torch.float32, device=s.device)
+        gself = torch.zeros(self_tab.shape, dtype=torch.float32, device=s.device)
+        ghead = torch.zeros(head_tab.shape, dtype=torch.float32, device=s.device)
+        ops.graft_aggregate_backward(ctx.gg, s, self_tab.contiguous(), head_tab.contiguous(), grad_out.contiguous(),
+                                     gs, gself, ghead, seed, ctx.p)
+        return gself, ghead, gs, None, None, None
+
+
+def _graft_kernel_batch(model, batch, dev):
+    """Stage a graft batch for the kernel path (slot order, both graft CSRs, the kb CSRs with the norm_rel weights);
+    raises on malformed graft or kb fact lists with the messages of model(batch)."""
+    from . import batching
+    db = batching.stage_graft_batch(batch, dev, model.num_relation + 1, False, model.norm_rel)
+    db.graft.check_status()
+    db.graph.check_status()
+    return db
+
+
 def graftnet_forward(model, batch):
     """GraftNet forward with autograd (graftnet.py:135-183, graft_gnn.py:64-153) -> (loss, pred, pred_dist, [h1, f1]).
-    Per-fact messages are gathered and reduced with ``index_add_``; dropout sits where the reference applies it."""
+
+    Kernel path (CUDA, ``USE_KERNELS``, D <= FACT_KERNEL_MAX_D): the fact attention, the fact messages and the TypeLayer run in the kernels of
+    csrc/graft.cu and csrc/aggregate*.cu with their own backward (_GraftAttentionFn, _GraftAggregateFn, _TypeLayerFn),
+    so nothing of shape [facts, D] is formed or saved; kb_tail_linear is applied after the per-node sum (by linearity:
+    sum_f kb_tail(v_f) = kb_tail.weight @ sum_f v_f + indeg * kb_tail.bias).  The per-fact scalars (W~, E, s, d') stay
+    in torch autograd on [F] vectors.  The fact-message dropout is drawn in the kernels (Philox keyed by fact slot, one
+    seed per layer from torch's CUDA generator).
+    Otherwise (CPU under ``HOST_CHECK``, or ``USE_KERNELS`` off): per-fact messages are gathered and reduced with
+    ``index_add_``; dropout sits where the reference applies it."""
     (local_entity, query_entities, kb_adj_mat, graft, q_input, kb_fact_rel, seed_dist, _tb,
      answer_dist) = batch[:9]
     dev = model.word_embedding.weight.device
@@ -352,21 +474,31 @@ def graftnet_forward(model, batch):
     Nt, D = B * N, model.entity_dim
     layer = model.reasoning
     drop = layer.linear_drop_train
+    kernels = _fact_kernels(dev, D)
+    db = _graft_kernel_batch(model, batch, dev) if kernels else None
     rel = model.get_rel_feature_train()
-    if model.encode_type:
+    if model.encode_type and kernels:
+        h = _type_layer(model.type_layer, None, rel, Nt, db.graph)
+    elif model.encode_type:
         h = _type_layer(model.type_layer, _Facts(kb_adj_mat, dev, False, model.norm_rel), rel, Nt)
     else:
         h = model.entity_linear(model.entity_embedding(local_entity)).view(Nt, D)
     enc = model.instruction
     enc.encode_question_train(q_input)
     qh, qnode, qmask = enc.query_hidden_emb, enc.query_node_emb, enc.query_mask_train
-    slot, head, tail = _graft_facts(graft, kb_fact_rel, B, N, dev)
-    # compute_attention (graft_gnn.py:64-87) over every slot
-    fact_emb = rel[kb_fact_rel]                                                   # [B, max_fact, D]
-    div = float(np.sqrt(D))
-    sim = torch.bmm(qh, fact_emb.transpose(1, 2)) / div
-    sim = F.softmax(sim + (1 - qmask.unsqueeze(2)) * VERY_NEG_NUMBER, dim=1)      # [B, Q, max_fact]
-    W = torch.sum(torch.bmm(sim.transpose(1, 2), qh) * fact_emb, dim=2) / div
+    if kernels:
+        gg = db.graft
+        nf = int(gg.nfacts.item())
+        slot, head, tail = (t[:nf].long() for t in (gg.slot_of, gg.heads, gg.tails))
+        W = _GraftAttentionFn.apply(qh, rel, qmask.float(), gg)                  # [B, max_fact]
+    else:
+        slot, head, tail = _graft_facts(graft, kb_fact_rel, B, N, dev)
+        # compute_attention (graft_gnn.py:64-87) over every slot
+        fact_emb = rel[kb_fact_rel]                                               # [B, max_fact, D]
+        div = float(np.sqrt(D))
+        sim = torch.bmm(qh, fact_emb.transpose(1, 2)) / div
+        sim = F.softmax(sim + (1 - qmask.unsqueeze(2)) * VERY_NEG_NUMBER, dim=1)  # [B, Q, max_fact]
+        W = torch.sum(torch.bmm(sim.transpose(1, 2), qh) * fact_emb, dim=2) / div
     W_tilde = torch.exp(W - torch.max(W, dim=1, keepdim=True)[0]).reshape(-1)[slot]
     E = torch.clamp(torch.zeros(Nt, device=dev).index_add(0, head, W_tilde), min=1e-10)
     mask = (local_entity != model.num_entity).float()
@@ -375,13 +507,23 @@ def graftnet_forward(model, batch):
     query = qnode                                                                 # [B, 1, D]
     dist_history, pagerank = [seed_dist], [seed_dist]
     lam = layer.pagerank_lambda
+    if kernels:
+        indeg = torch.zeros(Nt, device=dev).index_add_(0, tail, torch.ones_like(W_tilde)).unsqueeze(1)
     for i in range(model.num_layer):
         q2e = layer.lin("q2e_linear", i)(drop(query)).expand(B, N, D).reshape(Nt, D)
         s = W_tilde * (d / E)[head]
-        v = F.relu(layer.lin("kb_self_linear", i)(rel)[fact_rel] + layer.lin("kb_head_linear", i)(drop(h))[head])
-        v = v * s.unsqueeze(1)
-        f2e = F.relu(layer.lin("kb_self_linear", i)(h) + torch.zeros(Nt, D, device=dev).index_add(
-            0, tail, layer.lin("kb_tail_linear", i)(drop(v))))
+        if kernels:
+            kt = layer.lin("kb_tail_linear", i)
+            p = float(drop.p) if drop.training else 0.0
+            seed = torch.randint(0, 2 ** 62, (1,), dtype=torch.int64, device=dev) if p > 0.0 else None
+            sum_v = _GraftAggregateFn.apply(layer.lin("kb_self_linear", i)(rel),
+                                            layer.lin("kb_head_linear", i)(drop(h)), s, gg, seed, p)
+            f2e = F.relu(layer.lin("kb_self_linear", i)(h) + F.linear(sum_v, kt.weight) + indeg * kt.bias)
+        else:
+            v = F.relu(layer.lin("kb_self_linear", i)(rel)[fact_rel] + layer.lin("kb_head_linear", i)(drop(h))[head])
+            v = v * s.unsqueeze(1)
+            f2e = F.relu(layer.lin("kb_self_linear", i)(h) + torch.zeros(Nt, D, device=dev).index_add(
+                0, tail, layer.lin("kb_tail_linear", i)(drop(v))))
         d = lam * torch.zeros(Nt, device=dev).index_add(0, tail, s) + (1 - lam) * d
         x = torch.cat([h, q2e, layer.fact_scale * f2e], dim=1)
         query = torch.bmm(d.view(B, 1, N), layer.lin("e2q_linear", i)(drop(x)).view(B, N, D))

@@ -154,3 +154,96 @@ extern "C" int gr_aggregate_backward(const int32_t* rowptr, const int32_t* src, 
   GR_CHECK_LAUNCH();
   return GR_OK;
 }
+
+// Backward of gr_type_layer (TypeLayer.forward, gnn/modules/layer_init.py:46-57):
+//     out[n] = relu( sum_{tail CSR of n} w_e table[rel_e] + sum_{head CSR of n} w_e table[rel_e] )
+//     grad_table[r] += sum_{tail CSR rows n} w_e Gm[n] + sum_{head CSR rows n} w_e Gm[n],   Gm = G * [out > 0]
+// One warp per row holds Gm[n] in registers and walks both of the row's CSR lists; runs of equal relations are merged
+// into one coefficient, then added to the R1 table rows with fp32 atomics (not bit-reproducible).
+namespace gr {
+namespace {
+
+template <int NC>
+__global__ void __launch_bounds__(kBwdThreads) type_bwd_kernel(const int32_t* __restrict__ rowptr_t,
+                                                               const int32_t* __restrict__ rel_t,
+                                                               const float* __restrict__ w_t,
+                                                               const int32_t* __restrict__ rowptr_h,
+                                                               const int32_t* __restrict__ rel_h,
+                                                               const float* __restrict__ w_h,
+                                                               const float* __restrict__ grad, int64_t ld_grad,
+                                                               const float* __restrict__ out, int64_t ld_out,
+                                                               float* __restrict__ gtable, int64_t ld_gt, int64_t Nt,
+                                                               int D) {
+  const int lane = threadIdx.x & 31;
+  const int64_t n = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= Nt) return;
+  const int bt = rowptr_t[n], et = rowptr_t[n + 1], bh = rowptr_h[n], eh = rowptr_h[n + 1];
+  if (bt == et && bh == eh) return;
+  float g[NC];
+  bool any = false;
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    g[k] = (c < D && __ldg(out + n * ld_out + c) > 0.f) ? __ldg(grad + n * ld_grad + c) : 0.f;
+    any |= g[k] != 0.f;
+  }
+  if (!__any_sync(0xffffffffu, any)) return;
+  int cur = -1;
+  float cw = 0.f;
+  auto flush = [&]() {
+    if (cur < 0 || cw == 0.f) return;
+    float* row = gtable + (int64_t)cur * ld_gt;
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D && g[k] != 0.f) atomicAdd(row + c, cw * g[k]);
+    }
+  };
+  for (int i = 0, len = (et - bt) + (eh - bh); i < len; ++i) {
+    const bool tail = i < et - bt;
+    const int e = tail ? bt + i : bh + (i - (et - bt));
+    const int r = __ldg((tail ? rel_t : rel_h) + e);
+    const float* w = tail ? w_t : w_h;
+    const float we = w ? __ldg(w + e) : 1.f;
+    if (r != cur) {
+      flush();
+      cur = r;
+      cw = 0.f;
+    }
+    cw += we;
+  }
+  flush();
+}
+
+}  // namespace
+}  // namespace gr
+
+extern "C" int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                                      const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
+                                      const float* grad_out, int64_t ld_grad, const float* out, int64_t ld_out,
+                                      float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F,
+                                      void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512 && F >= 0, "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG(rowptr_t && rowptr_h && grad_out && out && grad_table, "null pointer");
+  GR_CHECK_ARG(F == 0 || (rel_t && rel_h), "null edge arrays");
+  GR_CHECK_ARG(ld_grad >= D && ld_out >= D && ld_gtable >= D, "leading dimension smaller than D");
+  if (F == 0) return GR_OK;
+  const int64_t Nt = (int64_t)B * N;
+  const int grid = (int)ceil_div(Nt, kBwdThreads / 32);
+  const int nc = D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16;
+#define GR_LAUNCH(NC)                                                                                            \
+  type_bwd_kernel<NC><<<grid, kBwdThreads, 0, stream>>>(rowptr_t, rel_t, w_t, rowptr_h, rel_h, w_h, grad_out,     \
+                                                        ld_grad, out, ld_out, grad_table, ld_gtable, Nt, D)
+  switch (nc) {
+    case 1: GR_LAUNCH(1); break;
+    case 2: GR_LAUNCH(2); break;
+    case 4: GR_LAUNCH(4); break;
+    case 8: GR_LAUNCH(8); break;
+    default: GR_LAUNCH(16); break;
+  }
+#undef GR_LAUNCH
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}

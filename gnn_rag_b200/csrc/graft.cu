@@ -11,6 +11,9 @@
 //                       sums sum_f v_f, indeg, d' = lambda * sum_f s_f + (1 - lambda) * d.  No atomics: every output
 //                       row is owned by one warp, so results are bit-reproducible and do not depend on the loader's
 //                       permutation of the fact lists.
+// Training (model(batch, training=True)): gr_graft_aggregate_train / gr_graft_aggregate_backward (the fact messages
+// with kb_tail_linear moved after the per-node sum, in-kernel dropout keyed by fact slot), gr_graft_attention_backward
+// and gr_graft_dropout_mask.
 #include <cub/device/device_scan.cuh>
 #include <cuda_bf16.h>
 
@@ -283,6 +286,239 @@ __global__ void __launch_bounds__(256) graft_aggregate_kernel(const AggArgs a) {
 
 int nc_for(int D) { return D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16; }
 
+// ---- training: dropout, aggregation forward / backward, attention backward ----------------------------------------
+
+// Philox4x32-10 (Salmon et al., SC'11) with key = the 64-bit seed and counter = (slot lo, slot hi, column, 0); the
+// first output word decides.  Keyed by fact SLOT (b * max_fact + f), so the mask of a fact does not depend on where
+// the loader's permutation put it in the graft lists.
+__device__ __forceinline__ uint32_t philox_x0(uint64_t seed, uint64_t slot, uint32_t col) {
+  uint32_t c0 = (uint32_t)slot, c1 = (uint32_t)(slot >> 32), c2 = col, c3 = 0u;
+  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+    c0 = hi1 ^ c1 ^ k0;
+    c1 = lo1;
+    c2 = hi0 ^ c3 ^ k1;
+    c3 = lo0;
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c0;
+}
+
+// element (slot, col) survives dropout with probability 1 - p:  u = (x >> 8) * 2^-24 in [0, 1), keep iff u >= p
+__device__ __forceinline__ bool drop_keep(uint64_t seed, int64_t slot, int col, float p) {
+  return (float)(philox_x0(seed, (uint64_t)slot, (uint32_t)col) >> 8) * 5.9604644775390625e-8f >= p;
+}
+
+__global__ void graft_dropout_mask_kernel(const int64_t* __restrict__ seed, float p, int64_t S, int D,
+                                          uint8_t* __restrict__ mask) {
+  const uint64_t sd = p > 0.f ? (uint64_t)__ldg(seed) : 0;
+  const int64_t total = S * D, stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride)
+    mask[i] = p > 0.f ? (uint8_t)drop_keep(sd, i / D, (int)(i % D), p) : (uint8_t)1;
+}
+
+struct TrainArgs {
+  // forward: the tail CSR (src = head); backward: the head CSR (src = tail)
+  const int32_t *rowptr, *src, *rel, *fact, *slot_of;
+  const float *s, *self_tab, *head_tab;
+  int64_t ld_self, ld_head;
+  const int64_t* seed;      // NULL: no dropout
+  float p, scale;
+  float* sum_out;           // forward
+  int64_t ld_sum;
+  const float* grad;        // backward: dL/dsum_out
+  int64_t ld_grad;
+  float *grad_s, *grad_self, *grad_head;
+  int64_t ld_gself, ld_ghead;
+  int64_t Nt;
+  int D;
+};
+
+// sum_out[n] = sum_{f -> n} drop_f(relu(self_tab[r_f] + head_tab[head_f])) * s_f, one warp per tail-CSR row, slot order.
+template <int NC>
+__global__ void __launch_bounds__(256) graft_aggregate_train_kernel(const TrainArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int64_t n = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.Nt) return;
+  const int D = a.D;
+  const bool drop = a.seed != nullptr;
+  const uint64_t seed = drop ? (uint64_t)__ldg(a.seed) : 0;
+  float acc[NC];
+#pragma unroll
+  for (int k = 0; k < NC; ++k) acc[k] = 0.f;
+  const int beg = a.rowptr[n], end = a.rowptr[n + 1];
+  for (int e = beg; e < end; ++e) {
+    const int f = __ldg(a.fact + e);
+    const float s = __ldg(a.s + f);
+    if (s == 0.f) continue;        // the fact adds nothing (its relu term is finite)
+    const int h = __ldg(a.src + e), r = __ldg(a.rel + e);
+    const int64_t sl = __ldg(a.slot_of + f);
+    const float* st = a.self_tab + (int64_t)r * a.ld_self;
+    const float* ht = a.head_tab + (int64_t)h * a.ld_head;
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D) {
+        float v = __fmul_rn(fmaxf(__fadd_rn(__ldg(st + c), __ldg(ht + c)), 0.f), s);
+        if (drop) v = drop_keep(seed, sl, c, a.p) ? __fmul_rn(v, a.scale) : 0.f;
+        acc[k] = __fadd_rn(acc[k], v);
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    if (c < D) a.sum_out[n * a.ld_sum + c] = acc[k];
+  }
+}
+
+// Backward of graft_aggregate_train_kernel, one warp per HEAD-CSR row n (the out-facts of n).  With
+// g_f = G[tail_f] * mask_f / (1 - p) and a_f = self_tab[r_f] + head_tab[n]:
+//   grad_s[f] += <g_f, relu(a_f)>                 every fact, s_f = 0 included (lane 0, the fact is owned)
+//   grad_head[n] += sum_f g_f s_f [a_f > 0]       registers, one read-modify-write per row (the row is owned)
+//   grad_self[r_f] += g_f s_f [a_f > 0]           fp32 atomics into the R1 relation rows
+template <int NC>
+__global__ void __launch_bounds__(256) graft_aggregate_bwd_kernel(const TrainArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int64_t n = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.Nt) return;
+  const int beg = a.rowptr[n], end = a.rowptr[n + 1];
+  if (beg == end) return;
+  const int D = a.D;
+  const bool drop = a.seed != nullptr;
+  const uint64_t seed = drop ? (uint64_t)__ldg(a.seed) : 0;
+  float ht[NC], gh[NC];
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    ht[k] = c < D ? __ldg(a.head_tab + n * a.ld_head + c) : 0.f;
+    gh[k] = 0.f;
+  }
+  for (int e = beg; e < end; ++e) {
+    const int t = __ldg(a.src + e), r = __ldg(a.rel + e), f = __ldg(a.fact + e);
+    const int64_t sl = __ldg(a.slot_of + f);
+    const float s = __ldg(a.s + f);
+    const float* st = a.self_tab + (int64_t)r * a.ld_self;
+    const float* gt = a.grad + (int64_t)t * a.ld_grad;
+    float* gs_row = a.grad_self + (int64_t)r * a.ld_gself;
+    float gs = 0.f;
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D) {
+        const float x = __fadd_rn(__ldg(st + c), ht[k]);
+        float g = __ldg(gt + c);
+        if (drop) g = drop_keep(seed, sl, c, a.p) ? __fmul_rn(g, a.scale) : 0.f;
+        gs = fmaf(g, fmaxf(x, 0.f), gs);
+        if (s != 0.f && x > 0.f) {          // strict: relu'(0) = 0, as torch
+          const float v = __fmul_rn(g, s);
+          gh[k] = __fadd_rn(gh[k], v);
+          if (v != 0.f) atomicAdd(gs_row + c, v);
+        }
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) gs += __shfl_xor_sync(0xffffffffu, gs, o);
+    if (lane == 0) a.grad_s[f] += gs;
+  }
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    if (c < D) a.grad_head[n * a.ld_ghead + c] += gh[k];
+  }
+}
+
+constexpr int kSlotsPerBlock = 64;     // attention backward: 8 warps x 8 slots, all of one question
+
+// Backward of graft_w_kernel.  With z_q = <qh_q, rv>/div, a = softmax_q(z + mask) and W = sum_q a_q z_q:
+//   dW/dqh_q = c_q rv,   dW/drv = sum_q c_q qh_q,   c_q = a_q (1 + z_q - W) / div
+// One warp per slot recomputes the softmax (same operations as the forward); grad_rel goes out through fp32 atomics
+// by relation; grad_qh of the block's question is accumulated in shared memory (or, when Q*D does not fit, straight
+// into global memory) and flushed once per block.  Slots with grad_W == 0 contribute nothing and are skipped.
+template <int NC>
+__global__ void __launch_bounds__(256, 2) graft_w_bwd_kernel(const float* __restrict__ qh,
+                                                          const float* __restrict__ qmask, int Q,
+                                                          const float* __restrict__ rel, int64_t ldr, int64_t R1,
+                                                          const int64_t* __restrict__ kb_fact_rel, int64_t max_fact,
+                                                          int D, float div, const float* __restrict__ gW,
+                                                          float* __restrict__ grad_qh, float* __restrict__ grad_rel,
+                                                          int64_t ld_grel, bool smem_acc) {
+  extern __shared__ float sacc[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  const int64_t b = blockIdx.y;
+  const int64_t f0 = (int64_t)blockIdx.x * kSlotsPerBlock, f1 = min(f0 + kSlotsPerBlock, max_fact);
+  const int64_t QD = (int64_t)Q * D;
+  if (smem_acc) {
+    for (int64_t i = threadIdx.x; i < QD; i += blockDim.x) sacc[i] = 0.f;
+    __syncthreads();
+  }
+  float* acc = smem_acc ? sacc : grad_qh + b * QD;
+  const float* qb = qh + b * QD;
+  const float* mb = qmask + b * (int64_t)Q;
+  const float inv_div = __frcp_rn(div);
+  for (int64_t f = f0 + warp; f < f1; f += nwarps) {
+    const int64_t s = b * max_fact + f;
+    const float g = __ldg(gW + s);
+    if (g == 0.f) continue;
+    int64_t r = kb_fact_rel[s];
+    if (r < 0 || r >= R1) r = 0;           // as the forward (which reports it)
+    float rv[NC];
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      rv[k] = c < D ? __ldg(rel + r * ldr + c) : 0.f;
+    }
+    float mx = -INFINITY;
+    for (int q = 0; q < Q; ++q) {
+      const float sim = __fadd_rn(__fdiv_rn(warp_dot<NC>(rv, qb + (int64_t)q * D, D), div),
+                                  __fmul_rn(1.0f - __ldg(mb + q), kVeryNeg));
+      mx = fmaxf(mx, sim);
+    }
+    float den = 0.f, wz = 0.f;
+    for (int q = 0; q < Q; ++q) {
+      const float z = __fdiv_rn(warp_dot<NC>(rv, qb + (int64_t)q * D, D), div);
+      const float e = expf(__fadd_rn(z, __fmul_rn(1.0f - __ldg(mb + q), kVeryNeg)) - mx);
+      den += e;
+      wz = fmaf(e, z, wz);
+    }
+    const float inv = __frcp_rn(den), Wr = wz * inv, ginv = g * inv * inv_div;
+    float gr[NC];
+#pragma unroll
+    for (int k = 0; k < NC; ++k) gr[k] = 0.f;
+    for (int q = 0; q < Q; ++q) {
+      const float* row = qb + (int64_t)q * D;
+      const float z = __fdiv_rn(warp_dot<NC>(rv, row, D), div);
+      const float e = expf(__fadd_rn(z, __fmul_rn(1.0f - __ldg(mb + q), kVeryNeg)) - mx);
+      const float cq = e * ginv * (1.0f + z - Wr);
+      if (cq == 0.f) continue;             // warp-uniform: masked tokens (a_q = 0)
+#pragma unroll
+      for (int k = 0; k < NC; ++k) {
+        const int c = lane + 32 * k;
+        if (c < D) {
+          atomicAdd(acc + (int64_t)q * D + c, cq * rv[k]);
+          gr[k] = fmaf(cq, __ldg(row + c), gr[k]);
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D && gr[k] != 0.f) atomicAdd(grad_rel + r * ld_grel + c, gr[k]);
+    }
+  }
+  if (smem_acc) {
+    __syncthreads();
+    for (int64_t i = threadIdx.x; i < QD; i += blockDim.x) {
+      const float v = sacc[i];
+      if (v != 0.f) atomicAdd(grad_qh + b * QD + i, v);
+    }
+  }
+}
+
 }  // namespace
 }  // namespace gr
 
@@ -412,6 +648,118 @@ extern "C" int gr_graft_aggregate(const int32_t* rowptr_t, const int32_t* src_t,
     case 8: graft_aggregate_kernel<8><<<grid, 256, 0, stream>>>(a); break;
     default: graft_aggregate_kernel<16><<<grid, 256, 0, stream>>>(a); break;
   }
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+// ---- training entry points -----------------------------------------------------------------------------------------
+
+namespace {
+
+#define GR_NC_SWITCH(D, LAUNCH)         \
+  switch (nc_for(D)) {                  \
+    case 1: LAUNCH(1); break;           \
+    case 2: LAUNCH(2); break;           \
+    case 4: LAUNCH(4); break;           \
+    case 8: LAUNCH(8); break;           \
+    default: LAUNCH(16); break;         \
+  }
+
+// dropout arguments shared by the training entry points: p in [0, 1); p > 0 needs the seed, p == 0 ignores it
+int drop_args(const int64_t* seed, double p, TrainArgs& a) {
+  GR_CHECK_ARG(p >= 0.0 && p < 1.0, "dropout probability outside [0, 1)");
+  GR_CHECK_ARG(p == 0.0 || seed, "null seed with p > 0");
+  a.seed = p > 0.0 ? seed : nullptr;
+  a.p = (float)p;
+  a.scale = (float)(1.0 / (1.0 - p));
+  return GR_OK;
+}
+
+}  // namespace
+
+extern "C" int gr_graft_dropout_mask(const int64_t* seed, double p, int64_t S, int D, uint8_t* mask, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(S >= 0 && D > 0 && D <= 512, "bad sizes (need S >= 0, 0 < D <= 512)");
+  GR_CHECK_ARG(p >= 0.0 && p < 1.0, "dropout probability outside [0, 1)");
+  GR_CHECK_ARG(S == 0 || mask, "null pointer");
+  GR_CHECK_ARG(p == 0.0 || seed, "null seed with p > 0");
+  if (S == 0) return GR_OK;
+  const int grid = (int)std::min<int64_t>(ceil_div(S * D, 256), 8192);
+  graft_dropout_mask_kernel<<<grid, 256, 0, stream>>>(seed, (float)p, S, D, mask);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+extern "C" int gr_graft_aggregate_train(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                                        const int32_t* fact_t, const int32_t* slot_of, const float* s,
+                                        const float* self_tab, int64_t ld_self, const float* head_tab, int64_t ld_head,
+                                        const int64_t* seed, double p, float* sum_out, int64_t ld_sum, int B, int N,
+                                        int D, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512, "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG(rowptr_t && src_t && rel_t && fact_t && slot_of && s && self_tab && head_tab && sum_out,
+               "null pointer");
+  GR_CHECK_ARG(ld_self >= D && ld_head >= D && ld_sum >= D, "leading dimension smaller than D");
+  TrainArgs a{};
+  if (int rc = drop_args(seed, p, a)) return rc;
+  a.rowptr = rowptr_t; a.src = src_t; a.rel = rel_t; a.fact = fact_t; a.slot_of = slot_of;
+  a.s = s; a.self_tab = self_tab; a.head_tab = head_tab; a.ld_self = ld_self; a.ld_head = ld_head;
+  a.sum_out = sum_out; a.ld_sum = ld_sum;
+  a.Nt = (int64_t)B * N; a.D = D;
+  const int grid = (int)ceil_div(a.Nt, 8);
+#define GR_LAUNCH(NC) graft_aggregate_train_kernel<NC><<<grid, 256, 0, stream>>>(a)
+  GR_NC_SWITCH(D, GR_LAUNCH)
+#undef GR_LAUNCH
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+extern "C" int gr_graft_aggregate_backward(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                           const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                           const float* self_tab, int64_t ld_self, const float* head_tab,
+                                           int64_t ld_head, const int64_t* seed, double p, const float* grad_sum,
+                                           int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
+                                           float* grad_head, int64_t ld_ghead, int B, int N, int D, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512, "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG(rowptr_h && src_h && rel_h && fact_h && slot_of && s && self_tab && head_tab && grad_sum && grad_s &&
+                   grad_self && grad_head, "null pointer");
+  GR_CHECK_ARG(ld_self >= D && ld_head >= D && ld_grad >= D && ld_gself >= D && ld_ghead >= D,
+               "leading dimension smaller than D");
+  TrainArgs a{};
+  if (int rc = drop_args(seed, p, a)) return rc;
+  a.rowptr = rowptr_h; a.src = src_h; a.rel = rel_h; a.fact = fact_h; a.slot_of = slot_of;
+  a.s = s; a.self_tab = self_tab; a.head_tab = head_tab; a.ld_self = ld_self; a.ld_head = ld_head;
+  a.grad = grad_sum; a.ld_grad = ld_grad;
+  a.grad_s = grad_s; a.grad_self = grad_self; a.grad_head = grad_head; a.ld_gself = ld_gself; a.ld_ghead = ld_ghead;
+  a.Nt = (int64_t)B * N; a.D = D;
+  const int grid = (int)ceil_div(a.Nt, 8);
+#define GR_LAUNCH(NC) graft_aggregate_bwd_kernel<NC><<<grid, 256, 0, stream>>>(a)
+  GR_NC_SWITCH(D, GR_LAUNCH)
+#undef GR_LAUNCH
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+extern "C" int gr_graft_attention_backward(const float* qh, const float* qmask, int Q, const float* rel, int64_t ldr,
+                                           int64_t R1, const int64_t* kb_fact_rel, int B, int64_t max_fact, int D,
+                                           const float* grad_W, float* grad_qh, float* grad_rel, int64_t ld_grel,
+                                           void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && B <= 65535 && D > 0 && D <= 512 && Q > 0 && max_fact >= 0 && R1 > 0 && ldr >= D &&
+                   ld_grel >= D, "bad sizes (need 0 < D <= 512, 0 < B <= 65535, Q > 0)");
+  GR_CHECK_ARG(qh && qmask && rel && kb_fact_rel && grad_W && grad_qh && grad_rel, "null pointer");
+  if (max_fact == 0) return GR_OK;
+  const float div = (float)sqrt((double)D);
+  const size_t acc_bytes = (size_t)Q * D * sizeof(float);
+  const bool smem_acc = acc_bytes <= 48 * 1024;
+  const size_t smem = smem_acc ? acc_bytes : 0;
+  const dim3 grid((unsigned)ceil_div(max_fact, kSlotsPerBlock), (unsigned)B);
+#define GR_LAUNCH(NC)                                                                                          \
+  graft_w_bwd_kernel<NC><<<grid, 256, smem, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, max_fact, D, div, \
+                                                      grad_W, grad_qh, grad_rel, ld_grel, smem_acc)
+  GR_NC_SWITCH(D, GR_LAUNCH)
+#undef GR_LAUNCH
   GR_CHECK_LAUNCH();
   return GR_OK;
 }

@@ -1006,3 +1006,105 @@ def graft_aggregate(gg, Wt, E, prior, self_tab, head_tab, lam, q2e=None, sum_out
     _lib.check(rc)
     STATS.launches += 1
     return prior_next
+
+
+def _seed_p(seed, p):
+    """(seed pointer or None, p) of the dropout arguments: p == 0 takes the no-dropout path and ignores the seed."""
+    p = float(p)
+    if p == 0.0:
+        return None, 0.0
+    seed = _cuda(seed, torch.int64, "seed")
+    assert seed.numel() >= 1
+    return seed, p
+
+
+def graft_dropout_mask(seed, p, S, D):
+    """uint8 [S, D]: 1 where (slot, column) survives the fact-message dropout of :func:`graft_aggregate_train`
+    (same Philox keying, gr_graft_dropout_mask); all ones for p == 0."""
+    seed, p = _seed_p(seed, p)
+    dev = seed.device if seed is not None else torch.device("cuda")
+    mask = torch.empty(max(S, 1), D, dtype=torch.uint8, device=dev)
+    _lib.check(_L().gr_graft_dropout_mask(_p(seed), p, S, D, _p(mask), _stream()))
+    STATS.launches += 1 if S > 0 else 0
+    return mask[:S]
+
+
+def graft_aggregate_train(gg, s, self_tab, head_tab, seed=None, p=0.0, sum_out=None):
+    """Training forward of the fact messages (gr_graft_aggregate_train): sum_out [B*N, D] with
+    sum_out[n] = sum_{f -> n} drop_f(relu(self_tab[r_f] + head_tab[head_f])) * s_f.  ``s``: fp32 per staged fact;
+    ``seed``: device int64 [1] (read when p > 0)."""
+    g = gg.graph
+    self_tab = _cuda(self_tab, torch.float32, "self_tab")
+    head_tab = _cuda(head_tab, torch.float32, "head_tab")
+    s = _cuda(s, torch.float32, "s").contiguous()
+    D = self_tab.shape[1]
+    assert self_tab.stride(1) == 1 and head_tab.stride(1) == 1 and head_tab.shape[0] == gg.B * gg.N
+    seed, p = _seed_p(seed, p)
+    if sum_out is None:
+        sum_out = torch.empty(gg.B * gg.N, D, dtype=torch.float32, device=self_tab.device)
+    assert sum_out.stride(1) == 1
+    if s.numel() == 0:               # no staged facts (every question's subgraph empty): every row sums nothing
+        return sum_out.zero_()
+    with _AggTimer(("graft_train", 1)):
+        rc = _L().gr_graft_aggregate_train(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(gg.slot_of),
+                                           _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab), head_tab.stride(0),
+                                           _p(seed), p, _p(sum_out), sum_out.stride(0), gg.B, gg.N, D, _stream())
+    _lib.check(rc)
+    STATS.launches += 1
+    return sum_out
+
+
+def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_self, grad_head, seed=None, p=0.0):
+    """Accumulate the gradients of :func:`graft_aggregate_train` (same s, tables, seed and p) into grad_s [F],
+    grad_self [R1, D] and grad_head [B*N, D] (gr_graft_aggregate_backward, over the head CSR)."""
+    g = gg.graph
+    self_tab = _cuda(self_tab, torch.float32, "self_tab")
+    head_tab = _cuda(head_tab, torch.float32, "head_tab")
+    grad_sum = _cuda(grad_sum, torch.float32, "grad_sum")
+    s = _cuda(s, torch.float32, "s").contiguous()
+    D = self_tab.shape[1]
+    assert all(t.stride(1) == 1 for t in (self_tab, head_tab, grad_sum, grad_self, grad_head))
+    assert grad_s.is_contiguous() and grad_s.dtype == torch.float32
+    seed, p = _seed_p(seed, p)
+    if s.numel() == 0:               # no staged facts: nothing to add
+        return
+    with _OpTimer("aggregation_bwd"):
+        rc = _L().gr_graft_aggregate_backward(_p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h), _p(gg.slot_of),
+                                              _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab),
+                                              head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0),
+                                              _p(grad_s), _p(grad_self), grad_self.stride(0), _p(grad_head),
+                                              grad_head.stride(0), gg.B, gg.N, D, _stream())
+    _lib.check(rc)
+    STATS.launches += 1
+
+
+def graft_attention_backward(gg, qh, qmask, rel, grad_W, grad_qh, grad_rel):
+    """Accumulate dL/dqh [B, Q, D] and dL/drel [R1, D] of :func:`graft_attention`'s W given grad_W [B*max_fact]
+    (gr_graft_attention_backward)."""
+    qh = _cuda(qh, torch.float32, "qh").contiguous()
+    qmask = _cuda(qmask, torch.float32, "qmask").contiguous()
+    rel = _cuda(rel, torch.float32, "rel")
+    grad_W = _cuda(grad_W, torch.float32, "grad_W").contiguous()
+    assert rel.stride(1) == 1 and grad_rel.stride(1) == 1 and grad_qh.is_contiguous()
+    B, Q, D = qh.shape
+    with _OpTimer("graft_attention_bwd"):
+        rc = _L().gr_graft_attention_backward(_p(qh), _p(qmask), Q, _p(rel), rel.stride(0), rel.shape[0],
+                                              _p(gg.kb_fact_rel), B, gg.max_fact, D, _p(grad_W), _p(grad_qh),
+                                              _p(grad_rel), grad_rel.stride(0), _stream())
+    _lib.check(rc)
+    STATS.launches += 1 if gg.max_fact > 0 else 0
+
+
+def type_layer_backward(g, grad_out, out, grad_table, w_t=None, w_h=None):
+    """Accumulate dL/dtable [R1, D] of :func:`type_layer` given grad_out and the forward's fp32 ``out`` [B*N, D]
+    (gr_type_layer_backward)."""
+    grad_out = _cuda(grad_out, torch.float32, "grad_out")
+    out = _cuda(out, torch.float32, "out")
+    assert grad_out.stride(1) == 1 and out.stride(1) == 1 and grad_table.stride(1) == 1
+    D = out.shape[1]
+    with _OpTimer("type_layer_bwd"):
+        rc = _L().gr_type_layer_backward(_p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.rel_h), _p(w_h),
+                                         _p(grad_out), grad_out.stride(0), _p(out), out.stride(0), _p(grad_table),
+                                         grad_table.stride(0), g.B, g.N, D, g.F, _stream())
+    _lib.check(rc)
+    STATS.launches += 1

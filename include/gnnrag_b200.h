@@ -304,6 +304,58 @@ int gr_graft_aggregate(const int32_t* rowptr_t, const int32_t* src_t, const int3
                        float* prior_next, int B, int N, int D, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * GraftNet training (csrc/graft.cu; model(batch, training=True), gnn/train_model.py:222).  The per-fact scalars
+ * (W~, E, s_f, d') stay in torch autograd on [F] vectors; these kernels do the per-fact work of width D, so no [F, D]
+ * tensor exists.  Every gradient output is ACCUMULATED (+=, caller zeroes).  D <= 512.
+ *
+ * Dropout (linear_dropout on the fact messages, graft_gnn.py:105): element (slot, column) is kept iff
+ * u = (Philox4x32-10(key = *seed, counter = (slot lo, slot hi, column, 0))[0] >> 8) * 2^-24 >= p, and kept elements
+ * are scaled by 1/(1-p).  slot = b*max_fact + f (slot_of), so the mask does not depend on the loader's permutation of
+ * the graft lists.  seed: device int64[1]; p in [0, 1); p == 0 ignores the seed and computes without dropout.
+ *
+ * gr_graft_dropout_mask: mask[slot*D + c] = 1 if (slot, c) is kept, for slot < S (the same device function).
+ *
+ * gr_graft_aggregate_train: graft_gnn.py:89-107 (the fact messages, kb_tail_linear moved after the sum by
+ * linearity).  One warp per tail-CSR row n, facts in slot order:
+ *     sum_out[n] = sum_{f -> n} drop_f(relu(self_tab[r_f] + head_tab[head_f])) * s_f
+ * s: fp32 per staged fact (gr_graft_stage order); facts with s_f == 0 are skipped.  No atomics.
+ *
+ * gr_graft_aggregate_backward: given G = dL/dsum_out, g_f = G[tail_f] * mask_f/(1-p), a_f = self_tab[r_f] +
+ * head_tab[head_f]:
+ *     grad_s[f] += <g_f, relu(a_f)>  (every fact, s_f = 0 included)
+ *     grad_self[r] += sum_{f: r_f = r} g_f s_f [a_f > 0]      (fp32 atomics into the R1 rows)
+ *     grad_head[n] += sum_{f: head_f = n} g_f s_f [a_f > 0]   (one warp per head-CSR row, no atomics)
+ * Takes the HEAD CSR of the staged facts (rowptr_h, src_h = tails, rel_h, fact_h).
+ *
+ * gr_graft_attention_backward: graft_gnn.py:64-87.  Given grad_W [B*max_fact] (dL/dW of gr_graft_attention's W),
+ *     grad_qh[b, q] += sum_f c_{f,q} rel[r_f],   grad_rel[r] += sum_{f: r_f = r} sum_q c_{f,q} qh[b, q],
+ *     c_{f,q} = grad_W[f] a_{f,q} (1 + z_{f,q} - W_f) / sqrt(D),   z_{f,q} = <qh[b,q], rel[r_f]> / sqrt(D)
+ * with the softmax a recomputed per slot.  Slots with grad_W == 0 are skipped.  fp32 atomics.
+ *
+ * gr_type_layer_backward: TypeLayer.forward (layer_init.py:46-57) given G = dL/dout and gr_type_layer's fp32 output:
+ *     grad_table[r] += sum_{tail CSR} w_e (G * [out > 0])[n] + sum_{head CSR} w_e (G * [out > 0])[n]
+ * One warp per row, fp32 atomics into the R1 table rows.  Same CSRs and weights as the forward call.
+ */
+int gr_graft_dropout_mask(const int64_t* seed, double p, int64_t S, int D, uint8_t* mask, void* stream);
+int gr_graft_aggregate_train(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                             const int32_t* fact_t, const int32_t* slot_of, const float* s, const float* self_tab,
+                             int64_t ld_self, const float* head_tab, int64_t ld_head, const int64_t* seed, double p,
+                             float* sum_out, int64_t ld_sum, int B, int N, int D, void* stream);
+int gr_graft_aggregate_backward(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                const float* self_tab, int64_t ld_self, const float* head_tab, int64_t ld_head,
+                                const int64_t* seed, double p, const float* grad_sum, int64_t ld_grad, float* grad_s,
+                                float* grad_self, int64_t ld_gself, float* grad_head, int64_t ld_ghead, int B, int N,
+                                int D, void* stream);
+int gr_graft_attention_backward(const float* qh, const float* qmask, int Q, const float* rel, int64_t ldr,
+                                int64_t R1, const int64_t* kb_fact_rel, int B, int64_t max_fact, int D,
+                                const float* grad_W, float* grad_qh, float* grad_rel, int64_t ld_grel, void* stream);
+int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                           const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
+                           const float* grad_out, int64_t ld_grad, const float* out, int64_t ld_out,
+                           float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Sparse-prior fast path for one ReaRev layer (the first layer of every iteration sees the seed distribution,
  * rearev.py:208).  Rows none of whose in-edges carries prior mass get exactly zero neighbour messages, so
  * h_new = relu(W[:, :D] h + b) there (gr_linear_tc_planes with K = one segment).  gr_frontier_rows lists the

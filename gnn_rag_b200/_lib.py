@@ -82,6 +82,25 @@ SIGNATURES = {
                                             c_int, c_f32p, c_f32p, c_f32p, c_i64, c_void_p]),
     "gr_type_layer_backward": (c_int, [c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_f32p, c_i64,
                                        c_f32p, c_i64, c_int, c_int, c_int, c_i64, c_void_p]),
+    "gr_csr_row_of": (c_int, [c_i32p, c_i64, c_i32p, c_void_p]),
+    "gr_aggregate_backward_det_workspace_bytes": (c_size, [c_int, c_int, c_int, c_int, c_i64]),
+    "gr_aggregate_backward_det": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,
+                                          c_i64, c_i64, c_i64, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int,
+                                          c_i64, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i64, c_void_p, c_size,
+                                          c_void_p]),
+    "gr_type_layer_backward_det_workspace_bytes": (c_size, [c_i64, c_int]),
+    "gr_type_layer_backward_det": (c_int, [c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p,
+                                           c_i32p, c_f32p, c_i64, c_f32p, c_i64, c_f32p, c_i64, c_i64, c_int, c_i64,
+                                           c_void_p, c_size, c_void_p]),
+    "gr_graft_aggregate_backward_det_workspace_bytes": (c_size, [c_i64, c_int]),
+    "gr_graft_aggregate_backward_det": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64,
+                                                c_f32p, c_i64, c_void_p, c_dbl, c_f32p, c_i64, c_f32p, c_f32p, c_i64,
+                                                c_f32p, c_i64, c_int, c_int, c_int, c_i32p, c_i32p, c_i32p, c_i32p,
+                                                c_i32p, c_i64, c_i64, c_void_p, c_size, c_void_p]),
+    "gr_graft_attention_backward_det_workspace_bytes": (c_size, [c_int, c_i64, c_int, c_int]),
+    "gr_graft_attention_backward_det": (c_int, [c_f32p, c_f32p, c_int, c_f32p, c_i64, c_i64, c_void_p, c_int, c_i64,
+                                                c_int, c_f32p, c_f32p, c_f32p, c_i64, c_i32p, c_i32p, c_void_p,
+                                                c_size, c_void_p]),
     "gr_frontier_rows": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i64, c_i32p, c_i32p, c_void_p]),
     "gr_frontier_fixup": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p,
                                   c_f32p, c_f32p, c_f32p, c_void_p, c_void_p, c_i64, c_f32p, c_i64, c_f32p,

@@ -11,7 +11,10 @@ device (CUDA when the model lives there -- no CPU fallback is involved) so that 
     ``lstm_drop`` on the word embeddings), active only under ``model.train()``;
   * on CUDA with ``USE_KERNELS`` the aggregations, the TypeLayer and GraftNet's fact attention and fact messages run
     in hand-written kernels with their own backward (the ``torch.autograd.Function``s below); the per-fact torch
-    restatement is the CPU reference under ``HOST_CHECK`` and the ``USE_KERNELS = False`` path.
+    restatement is the CPU reference under ``HOST_CHECK`` and the ``USE_KERNELS = False`` path;
+  * under ``torch.use_deterministic_algorithms(True)`` (``warn_only`` included), read by each Function at forward,
+    those backward kernels are the fixed-order, atomic-free variants: every gradient they produce is a pure function
+    of the inputs.  The torch restatement's ``index_add`` is made deterministic by torch itself under the same flag.
 
 Reference: ReaRev.forward gnn/models/ReaRev/rearev.py:163-243, ReasonGNNLayer.forward gnn/modules/kg_reasoning/
 reasongnn.py:61-174, TypeLayer.forward gnn/modules/layer_init.py:25-62, BaseInstruction.get_instruction
@@ -101,6 +104,7 @@ class _AggregateFn(torch.autograd.Function):
         out = ops.aggregate(graph, direction, prior.detach(), table.detach(), ins.detach(), w=w)
         ctx.save_for_backward(table, ins, prior)
         ctx.graph, ctx.direction, ctx.w = graph, direction, w
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         return out
 
     @staticmethod
@@ -110,7 +114,7 @@ class _AggregateFn(torch.autograd.Function):
         # the kernel accumulates into dense row-major buffers: zeros_like alone would keep a transposed input's strides
         gt, gi, gp = (torch.zeros_like(t, memory_format=torch.contiguous_format) for t in (table, ins, prior))
         ops.aggregate_backward(ctx.graph, ctx.direction, prior, table.contiguous(), ins.contiguous(),
-                               grad_out.contiguous(), gt, gi, gp, ctx.w)
+                               grad_out.contiguous(), gt, gi, gp, ctx.w, deterministic=ctx.det)
         return gt, gi, gp, None, None, None
 
 
@@ -126,6 +130,7 @@ class _TypeLayerFn(torch.autograd.Function):
         ops.type_layer(graph, table.detach(), out, w_t, w_h)
         ctx.save_for_backward(out)
         ctx.graph, ctx.w, ctx.rows = graph, (w_t, w_h), table.shape[0]
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         return out
 
     @staticmethod
@@ -133,7 +138,7 @@ class _TypeLayerFn(torch.autograd.Function):
         from . import ops
         out, = ctx.saved_tensors
         gt = torch.zeros(ctx.rows, out.shape[1], dtype=torch.float32, device=out.device)
-        ops.type_layer_backward(ctx.graph, grad_out.contiguous(), out, gt, *ctx.w)
+        ops.type_layer_backward(ctx.graph, grad_out.contiguous(), out, gt, *ctx.w, deterministic=ctx.det)
         return gt, None, None, None
 
 
@@ -400,6 +405,7 @@ class _GraftAttentionFn(torch.autograd.Function):
         W, _wt, _e = ops.graft_attention(gg, qh.detach(), qmask, rel.detach().contiguous(), out_w=True)
         ctx.save_for_backward(qh, rel, qmask)
         ctx.gg = gg
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         return W.view(gg.B, gg.max_fact)
 
     @staticmethod
@@ -408,7 +414,8 @@ class _GraftAttentionFn(torch.autograd.Function):
         qh, rel, qmask = ctx.saved_tensors
         gq = torch.zeros(qh.shape, dtype=torch.float32, device=qh.device)
         gr = torch.zeros(rel.shape, dtype=torch.float32, device=rel.device)
-        ops.graft_attention_backward(ctx.gg, qh, qmask, rel.contiguous(), grad_W.reshape(-1), gq, gr)
+        ops.graft_attention_backward(ctx.gg, qh, qmask, rel.contiguous(), grad_W.reshape(-1), gq, gr,
+                                     deterministic=ctx.det)
         return gq, gr, None, None
 
 
@@ -424,6 +431,7 @@ class _GraftAggregateFn(torch.autograd.Function):
                                         seed, p)
         ctx.save_for_backward(self_tab, head_tab, s, seed)
         ctx.gg, ctx.p = gg, p
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         return out
 
     @staticmethod
@@ -434,7 +442,7 @@ class _GraftAggregateFn(torch.autograd.Function):
         gself = torch.zeros(self_tab.shape, dtype=torch.float32, device=s.device)
         ghead = torch.zeros(head_tab.shape, dtype=torch.float32, device=s.device)
         ops.graft_aggregate_backward(ctx.gg, s, self_tab.contiguous(), head_tab.contiguous(), grad_out.contiguous(),
-                                     gs, gself, ghead, seed, ctx.p)
+                                     gs, gself, ghead, seed, ctx.p, deterministic=ctx.det)
         return gself, ghead, gs, None, None, None
 
 

@@ -126,6 +126,257 @@ __global__ void __launch_bounds__(kBwdThreads) agg_bwd_kernel(const BwdParams p)
 }  // namespace
 }  // namespace gr
 
+// ---- deterministic variant (torch.use_deterministic_algorithms) ----------------------------------------------------
+// The same three gradients, each a sum whose order is fixed by the data (common.cuh, fixed-window segmented sums):
+//   dx_j[b]  windows of kRowWin destination rows walk the rows and their in-edges in CSR order; segment = question
+//   dp[s]    the row walk stores q_e = w_e^2 * dot_e per fact; one thread per source node then adds the q_e of its
+//            out-edges in the slot order of the OTHER destination CSR (which lists exactly the edges with that source)
+//   dP[r]    windows of kRelWin entries of the relation index (this CSR's slots sorted by (relation, slot)) gather
+//            G[n_e] and x_j[b_e] per edge; segment = relation
+// Inside every term __fmul_rn / __fadd_rn, so nothing is contracted: dot_e = butterfly over lanes of the lane sums
+// over (k, j) of g * (P * x), added in that order.
+namespace gr {
+namespace {
+
+constexpr int kRowWin = 32;   // destination rows per window of the dx pass
+constexpr int kRelWin = 64;   // relation-index entries per window of the dP / grad_table passes
+
+struct DetParams {
+  BwdParams p;
+  const int32_t *fact, *rowptr_o, *fact_o, *rix_ptr, *rix_slot, *row_of;
+  float* q;                 // [F] per-fact w^2 * dot, keyed by original fact id
+  float* part;              // segmented-sum partials (dx, then dP)
+  int64_t R1;
+};
+
+template <int NI>
+__global__ void __launch_bounds__(kBwdThreads) agg_bwd_det_rows_kernel(const DetParams d) {
+  const BwdParams& p = d.p;
+  const int lane = threadIdx.x & 31;
+  const int64_t win = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t a = win * kRowWin, bnd = min(p.Nt, a + kRowWin);
+  if (a >= p.Nt) return;
+  const int D = p.D, N = p.N;
+  const int64_t width = (int64_t)p.I * D;
+  auto seg_of = [N](int64_t n) { return n / N; };
+  float x[NI][kCPL], dx[NI][kCPL];
+  int64_t cur_b = -1;
+  bool first = true;
+  auto flush = [&]() {
+    const int slot = segwin_slot(a, bnd, p.Nt, cur_b, first, seg_of);
+#pragma unroll
+    for (int j = 0; j < NI; ++j)
+      segwin_store<kCPL>(dx[j], slot, d.part + (win * 2 + (slot > 0)) * width + j * D,
+                         p.gins + cur_b * width + (int64_t)j * D, D);
+    first = false;
+  };
+  for (int64_t n = a; n < bnd; ++n) {
+    const int64_t b = n / N;
+    if (b != cur_b) {
+      if (cur_b >= 0) flush();
+      cur_b = b;
+#pragma unroll
+      for (int j = 0; j < NI; ++j)
+#pragma unroll
+        for (int k = 0; k < kCPL; ++k) {
+          const int c = lane + 32 * k;
+          x[j][k] = c < D ? __ldg(p.ins + (b * p.I + j) * D + c) : 0.f;
+          dx[j][k] = 0.f;
+        }
+    }
+    const int beg = p.rowptr[n], end = p.rowptr[n + 1];
+    if (beg == end) continue;
+    float g[NI][kCPL];
+#pragma unroll
+    for (int j = 0; j < NI; ++j)
+#pragma unroll
+      for (int k = 0; k < kCPL; ++k) {
+        const int c = lane + 32 * k;
+        g[j][k] = c < D ? __ldg(p.gout + n * p.ld + p.col0 + (int64_t)j * p.seg + c) : 0.f;
+      }
+    for (int e = beg; e < end; ++e) {
+      const int s = p.src[e], r = p.rel[e];
+      const float w = p.w ? p.w[e] : 1.f;
+      const float w2 = __fmul_rn(w, w);
+      const float c_e = __fmul_rn(w2, p.prior[s]);
+      const float* prow = p.table + (int64_t)r * D;
+      float dot = 0.f;
+#pragma unroll
+      for (int k = 0; k < kCPL; ++k) {
+        const int c = lane + 32 * k;
+        if (c < D) {
+          const float pv = __ldg(prow + c);
+#pragma unroll
+          for (int j = 0; j < NI; ++j) {
+            const float pre = __fmul_rn(pv, x[j][k]);
+            if (pre > 0.f) {
+              dx[j][k] = __fadd_rn(dx[j][k], __fmul_rn(__fmul_rn(c_e, g[j][k]), pv));
+              dot = __fadd_rn(dot, __fmul_rn(g[j][k], pre));
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) dot = __fadd_rn(dot, __shfl_xor_sync(0xffffffffu, dot, o));
+      if (lane == 0) d.q[d.fact[e]] = __fmul_rn(w2, dot);
+    }
+  }
+  flush();
+}
+
+// dp[s] += sum of q over the out-edges of s, in the other CSR's slot order (one thread per node)
+__global__ void agg_bwd_det_prior_kernel(const int32_t* __restrict__ rowptr_o, const int32_t* __restrict__ fact_o,
+                                         const float* __restrict__ q, float* __restrict__ gprior, int64_t Nt) {
+  const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= Nt) return;
+  const int beg = rowptr_o[s], end = rowptr_o[s + 1];
+  if (beg == end) return;
+  float v = 0.f;
+  for (int e = beg; e < end; ++e) v = __fadd_rn(v, q[fact_o[e]]);
+  gprior[s] = __fadd_rn(gprior[s], v);
+}
+
+// dP[r] over the relation index: entry i -> CSR slot e = rix_slot[i] of relation rel[e], row row_of[e]
+template <int NI>
+__global__ void __launch_bounds__(kBwdThreads) agg_bwd_det_rel_kernel(const DetParams d) {
+  const BwdParams& p = d.p;
+  const int lane = threadIdx.x & 31;
+  const int64_t win = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t L = d.rix_ptr[d.R1];
+  const int64_t a = win * kRelWin, bnd = min(L, a + kRelWin);
+  if (a >= L) return;
+  const int D = p.D, N = p.N;
+  auto seg_of = [&](int64_t i) { return (int64_t)p.rel[d.rix_slot[i]]; };
+  float pv[kCPL], x[NI][kCPL], acc[kCPL];
+  int64_t cur_r = -1, cur_b = -1;
+  bool first = true;
+  auto flush = [&]() {
+    const int slot = segwin_slot(a, bnd, L, cur_r, first, seg_of);
+    segwin_store<kCPL>(acc, slot, d.part + (win * 2 + (slot > 0)) * D, p.gtable + cur_r * D, D);
+    first = false;
+  };
+  for (int64_t i = a; i < bnd; ++i) {
+    const int e = d.rix_slot[i];
+    const int64_t r = p.rel[e], n = d.row_of[e], b = n / N;
+    if (r != cur_r) {
+      if (cur_r >= 0) flush();
+      cur_r = r;
+#pragma unroll
+      for (int k = 0; k < kCPL; ++k) {
+        const int c = lane + 32 * k;
+        pv[k] = c < D ? __ldg(p.table + r * D + c) : 0.f;
+        acc[k] = 0.f;
+      }
+    }
+    if (b != cur_b) {
+      cur_b = b;
+#pragma unroll
+      for (int j = 0; j < NI; ++j)
+#pragma unroll
+        for (int k = 0; k < kCPL; ++k) {
+          const int c = lane + 32 * k;
+          x[j][k] = c < D ? __ldg(p.ins + (b * p.I + j) * D + c) : 0.f;
+        }
+    }
+    const float w = p.w ? p.w[e] : 1.f;
+    const float c_e = __fmul_rn(__fmul_rn(w, w), p.prior[p.src[e]]);
+#pragma unroll
+    for (int k = 0; k < kCPL; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D) {
+        float dp_c = 0.f;
+#pragma unroll
+        for (int j = 0; j < NI; ++j)
+          if (__fmul_rn(pv[k], x[j][k]) > 0.f)
+            dp_c = __fadd_rn(dp_c, __fmul_rn(__ldg(p.gout + n * p.ld + p.col0 + (int64_t)j * p.seg + c), x[j][k]));
+        acc[k] = __fadd_rn(acc[k], __fmul_rn(c_e, dp_c));
+      }
+    }
+  }
+  flush();
+}
+
+struct AggDetWs {
+  size_t q_bytes, part_bytes, total;
+};
+
+AggDetWs agg_det_ws(int64_t Nt, int D, int I, int64_t F) {
+  AggDetWs w;
+  w.q_bytes = align_up((size_t)(F > 0 ? F : 1) * sizeof(float), 256);
+  w.part_bytes = std::max(segwin_part_bytes(Nt, (int64_t)I * D, kRowWin), segwin_part_bytes(F, D, kRelWin));
+  w.total = w.q_bytes + w.part_bytes;
+  return w;
+}
+
+}  // namespace
+}  // namespace gr
+
+extern "C" size_t gr_aggregate_backward_det_workspace_bytes(int B, int N, int D, int I, int64_t F) {
+  if (B <= 0 || N <= 0 || D <= 0 || I <= 0 || F < 0) return 0;
+  return gr::agg_det_ws((int64_t)B * N, D, I, F).total;
+}
+
+extern "C" int gr_aggregate_backward_det(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
+                                         const int32_t* fact, const float* w, const float* prior, const float* table,
+                                         const float* ins, const float* grad_out, int64_t grad_row_stride,
+                                         int64_t grad_col0, int64_t seg_stride, float* grad_table, float* grad_ins,
+                                         float* grad_prior, int B, int N, int D, int I, int64_t F,
+                                         const int32_t* rowptr_o, const int32_t* fact_o, const int32_t* rix_ptr,
+                                         const int32_t* rix_slot, const int32_t* row_of, int64_t R1, void* workspace,
+                                         size_t workspace_bytes, void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(rowptr && prior && table && ins && grad_out && grad_table && grad_ins && grad_prior && rowptr_o &&
+                   rix_ptr, "null pointer");
+  GR_CHECK_ARG(F == 0 || (src && rel && fact && fact_o && rix_slot && row_of), "null edge arrays");
+  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 32 * kCPL && I > 0 && I <= 4 && F >= 0 && R1 > 0,
+               "need 0 < D <= 256 and 0 < I <= 4");
+  GR_CHECK_ARG(seg_stride >= D && grad_row_stride >= grad_col0 + (int64_t)(I - 1) * seg_stride + D,
+               "grad_out row stride / segment stride smaller than the rows it must hold");
+  if (F == 0) return GR_OK;
+  const int64_t Nt = (int64_t)B * N;
+  const AggDetWs ws = agg_det_ws(Nt, D, I, F);
+  if (!workspace || workspace_bytes < ws.total) {
+    set_error("gr_aggregate_backward_det: workspace too small (%zu < %zu)", workspace_bytes, ws.total);
+    return GR_ERR_WORKSPACE;
+  }
+  DetParams d{};
+  BwdParams& p = d.p;
+  p.rowptr = rowptr; p.src = src; p.rel = rel; p.w = w; p.prior = prior; p.table = table; p.ins = ins;
+  p.gout = grad_out; p.ld = grad_row_stride; p.col0 = grad_col0; p.seg = seg_stride;
+  p.gtable = grad_table; p.gins = grad_ins; p.gprior = grad_prior;
+  p.Nt = Nt; p.N = N; p.D = D; p.I = I;
+  d.fact = fact; d.rowptr_o = rowptr_o; d.fact_o = fact_o; d.rix_ptr = rix_ptr; d.rix_slot = rix_slot;
+  d.row_of = row_of; d.R1 = R1;
+  d.q = reinterpret_cast<float*>(workspace);
+  d.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws.q_bytes);
+  const int wpb = kBwdThreads / 32;
+  const int grid_rows = (int)ceil_div(ceil_div(Nt, kRowWin), wpb);
+  const int grid_rel = (int)ceil_div(ceil_div(F, kRelWin), wpb);
+  const int64_t width = (int64_t)I * D;
+#define GR_DET(NI)                                                                                \
+  agg_bwd_det_rows_kernel<NI><<<grid_rows, kBwdThreads, 0, stream>>>(d);                         \
+  GR_CHECK_LAUNCH();                                                                              \
+  segwin_combine_kernel<kRowWin><<<(int)ceil_div(B * width, 256), 256, 0, stream>>>(            \
+      d.part, width, nullptr, N, B, grad_ins, width);                                             \
+  GR_CHECK_LAUNCH();                                                                              \
+  agg_bwd_det_prior_kernel<<<(int)ceil_div(Nt, 256), 256, 0, stream>>>(rowptr_o, fact_o, d.q, grad_prior, Nt); \
+  GR_CHECK_LAUNCH();                                                                              \
+  agg_bwd_det_rel_kernel<NI><<<grid_rel, kBwdThreads, 0, stream>>>(d);                           \
+  GR_CHECK_LAUNCH();                                                                              \
+  segwin_combine_kernel<kRelWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(               \
+      d.part, D, rix_ptr, 0, R1, grad_table, D);
+  switch (I) {
+    case 1: { GR_DET(1) } break;
+    case 2: { GR_DET(2) } break;
+    case 3: { GR_DET(3) } break;
+    default: { GR_DET(4) } break;
+  }
+#undef GR_DET
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
 extern "C" int gr_aggregate_backward(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const float* w,
                                      const float* prior, const float* table, const float* ins, const float* grad_out,
                                      int64_t grad_row_stride, int64_t grad_col0, int64_t seg_stride, float* grad_table,
@@ -245,5 +496,113 @@ extern "C" int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* re
   }
 #undef GR_LAUNCH
   GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+// Deterministic variant of gr_type_layer_backward: two fixed-window segmented sums (common.cuh) over the relation
+// indexes of the tail CSR and then of the head CSR.  Entry i -> CSR slot e of relation rel[e], row n = row_of[e]:
+//     grad_table[r] = (grad_table[r] + sum_{tail-CSR slots of r} w_e Gm[n]) + sum_{head-CSR slots of r} w_e Gm[n]
+// each sum in slot order, each term __fmul_rn(w_e, Gm[n]).
+namespace gr {
+namespace {
+
+template <int NC>
+__global__ void __launch_bounds__(kBwdThreads) type_bwd_det_kernel(const int32_t* __restrict__ rix_ptr,
+                                                                   const int32_t* __restrict__ rix_slot,
+                                                                   const int32_t* __restrict__ rel,
+                                                                   const float* __restrict__ w,
+                                                                   const int32_t* __restrict__ row_of,
+                                                                   const float* __restrict__ grad, int64_t ld_grad,
+                                                                   const float* __restrict__ out, int64_t ld_out,
+                                                                   float* __restrict__ gtable, int64_t ld_gt,
+                                                                   float* __restrict__ part, int64_t R1, int D) {
+  const int lane = threadIdx.x & 31;
+  const int64_t win = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t L = rix_ptr[R1];
+  const int64_t a = win * kRelWin, bnd = min(L, a + kRelWin);
+  if (a >= L) return;
+  auto seg_of = [&](int64_t i) { return (int64_t)rel[rix_slot[i]]; };
+  float acc[NC];
+  int64_t cur = -1;
+  bool first = true;
+  auto flush = [&]() {
+    const int slot = segwin_slot(a, bnd, L, cur, first, seg_of);
+    segwin_store<NC>(acc, slot, part + (win * 2 + (slot > 0)) * D, gtable + cur * ld_gt, D);
+    first = false;
+  };
+  for (int64_t i = a; i < bnd; ++i) {
+    const int e = rix_slot[i];
+    const int64_t r = rel[e], n = row_of[e];
+    if (r != cur) {
+      if (cur >= 0) flush();
+      cur = r;
+#pragma unroll
+      for (int k = 0; k < NC; ++k) acc[k] = 0.f;
+    }
+    const float we = w ? __ldg(w + e) : 1.f;
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D) {
+        const float gm = __ldg(out + n * ld_out + c) > 0.f ? __ldg(grad + n * ld_grad + c) : 0.f;
+        acc[k] = __fadd_rn(acc[k], __fmul_rn(we, gm));
+      }
+    }
+  }
+  flush();
+}
+
+}  // namespace
+}  // namespace gr
+
+extern "C" size_t gr_type_layer_backward_det_workspace_bytes(int64_t F, int D) {
+  if (F < 0 || D <= 0) return 0;
+  return gr::segwin_part_bytes(F, D, gr::kRelWin);
+}
+
+extern "C" int gr_type_layer_backward_det(const int32_t* rel_t, const float* w_t, const int32_t* rix_ptr_t,
+                                          const int32_t* rix_slot_t, const int32_t* row_of_t, const int32_t* rel_h,
+                                          const float* w_h, const int32_t* rix_ptr_h, const int32_t* rix_slot_h,
+                                          const int32_t* row_of_h, const float* grad_out, int64_t ld_grad,
+                                          const float* out, int64_t ld_out, float* grad_table, int64_t ld_gtable,
+                                          int64_t R1, int D, int64_t F, void* workspace, size_t workspace_bytes,
+                                          void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(D > 0 && D <= 512 && F >= 0 && R1 > 0, "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG(rix_ptr_t && rix_ptr_h && grad_out && out && grad_table, "null pointer");
+  GR_CHECK_ARG(F == 0 || (rel_t && rix_slot_t && row_of_t && rel_h && rix_slot_h && row_of_h), "null edge arrays");
+  GR_CHECK_ARG(ld_grad >= D && ld_out >= D && ld_gtable >= D, "leading dimension smaller than D");
+  if (F == 0) return GR_OK;
+  const size_t need = segwin_part_bytes(F, D, kRelWin);
+  if (!workspace || workspace_bytes < need) {
+    set_error("gr_type_layer_backward_det: workspace too small (%zu < %zu)", workspace_bytes, need);
+    return GR_ERR_WORKSPACE;
+  }
+  float* part = reinterpret_cast<float*>(workspace);
+  const int grid = (int)ceil_div(ceil_div(F, kRelWin), kBwdThreads / 32);
+  const int nc = D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16;
+  for (int dir = 0; dir < 2; ++dir) {
+    const int32_t* rp = dir ? rix_ptr_h : rix_ptr_t;
+    const int32_t* sl = dir ? rix_slot_h : rix_slot_t;
+    const int32_t* rl = dir ? rel_h : rel_t;
+    const int32_t* ro = dir ? row_of_h : row_of_t;
+    const float* w = dir ? w_h : w_t;
+#define GR_LAUNCH(NC)                                                                                          \
+  type_bwd_det_kernel<NC><<<grid, kBwdThreads, 0, stream>>>(rp, sl, rl, w, ro, grad_out, ld_grad, out, ld_out, \
+                                                            grad_table, ld_gtable, part, R1, D)
+    switch (nc) {
+      case 1: GR_LAUNCH(1); break;
+      case 2: GR_LAUNCH(2); break;
+      case 4: GR_LAUNCH(4); break;
+      case 8: GR_LAUNCH(8); break;
+      default: GR_LAUNCH(16); break;
+    }
+#undef GR_LAUNCH
+    GR_CHECK_LAUNCH();
+    segwin_combine_kernel<kRelWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, rp, 0, R1, grad_table,
+                                                                                   ld_gtable);
+    GR_CHECK_LAUNCH();
+  }
   return GR_OK;
 }

@@ -86,4 +86,61 @@ __device__ void bitonic_sort_block(T* a, int n) {
   }
 }
 
+// ---- fixed-window segmented sums (the deterministic backward kernels) ---------------------------------------------
+// A list of L entries sorted by segment (relation, question) is cut into windows of W consecutive entries, W a
+// compile-time constant.  One warp per window adds each segment's entries in list order, starting from 0
+// (__fadd_rn, so the order written is the order computed).  A segment that lies inside one window is owned by it:
+// the warp adds its sum to the output row.  A segment that crosses a window edge leaves one partial per window it
+// touches, in `part` [windows][2][width]: slot 0 holds the partial of the window's first segment, slot 1 that of its
+// last; segwin_combine_kernel then sums those partials in window order and adds the total to the output row.  Every
+// output element is therefore  out + ((p_first + p_next) + ... + p_last)  with the windows fixed by the data and W
+// alone: no atomics, and nothing depends on the grid or on which block runs first.
+
+// where the partial of segment `seg` of window [a, b) goes: -1 = the window owns it (add to the output row), else
+// its slot in `part`.  `first`: seg is the window's first segment.
+template <typename SegOf>
+__device__ __forceinline__ int segwin_slot(int64_t a, int64_t b, int64_t L, int64_t seg, bool first, SegOf seg_of) {
+  const bool before = first && a > 0 && seg_of(a - 1) == seg;
+  const bool after = b < L && seg_of(b) == seg;
+  return (before || after) ? (first ? 0 : 1) : -1;
+}
+
+// store one warp's NC-columns-per-lane partial (column c = lane + 32 k, c < D): out_row += acc or part_row = acc
+template <int NC>
+__device__ __forceinline__ void segwin_store(const float (&acc)[NC], int slot, float* part_row, float* out_row,
+                                             int D) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    if (c < D) {
+      if (slot < 0) out_row[c] = __fadd_rn(out_row[c], acc[k]);
+      else part_row[c] = acc[k];
+    }
+  }
+}
+
+// one thread per (segment, column): segments that cross a window edge.  Segment s spans list entries
+// [seg_ptr[s], seg_ptr[s + 1]), or [s * seg_len, (s + 1) * seg_len) without seg_ptr.  out[s * ld_out + c] +=.
+template <int W>
+__global__ void segwin_combine_kernel(const float* __restrict__ part, int64_t width, const int32_t* __restrict__ seg_ptr,
+                                      int64_t seg_len, int64_t nseg, float* __restrict__ out, int64_t ld_out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nseg * width) return;
+  const int64_t s = i / width, c = i % width;
+  const int64_t beg = seg_ptr ? seg_ptr[s] : s * seg_len, end = seg_ptr ? seg_ptr[s + 1] : beg + seg_len;
+  if (end <= beg) return;
+  const int64_t ws = beg / W, we = (end - 1) / W;
+  if (ws == we) return;
+  float v = part[(ws * 2 + (beg == ws * W ? 0 : 1)) * width + c];
+#pragma unroll 8
+  for (int64_t w = ws + 1; w <= we; ++w) v = __fadd_rn(v, part[w * 2 * width + c]);
+  out[s * ld_out + c] = __fadd_rn(out[s * ld_out + c], v);
+}
+
+// bytes of `part` for a list of up to L entries and `width` floats per segment row
+static inline size_t segwin_part_bytes(int64_t L, int64_t width, int W) {
+  return align_up((size_t)2 * (size_t)ceil_div(L > 0 ? L : 1, W) * (size_t)width * sizeof(float), 256);
+}
+
 }  // namespace gr

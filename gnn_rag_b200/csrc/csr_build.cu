@@ -350,3 +350,25 @@ extern "C" int gr_gather_f32(const float* in, const int32_t* fact, float* out, i
   GR_CHECK_LAUNCH();
   return GR_OK;
 }
+
+namespace gr {
+namespace {
+
+__global__ void csr_row_of_kernel(const int32_t* __restrict__ rowptr, int64_t Nt, int32_t* __restrict__ row_of) {
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= Nt) return;
+  for (int e = rowptr[n], end = rowptr[n + 1]; e < end; ++e) row_of[e] = (int32_t)n;
+}
+
+}  // namespace
+}  // namespace gr
+
+extern "C" int gr_csr_row_of(const int32_t* rowptr, int64_t Nt, int32_t* row_of, void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(Nt > 0 && Nt < (int64_t)0x7fffffff, "need 0 < Nt < 2^31");
+  GR_CHECK_ARG(rowptr && row_of, "null pointer");
+  csr_row_of_kernel<<<(int)ceil_div(Nt, 256), 256, 0, stream>>>(rowptr, Nt, row_of);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}

@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(256) graft_aggregate_train_kernel(const TrainA
 //   grad_s[f] += <g_f, relu(a_f)>                 every fact, s_f = 0 included (lane 0, the fact is owned)
 //   grad_head[n] += sum_f g_f s_f [a_f > 0]       registers, one read-modify-write per row (the row is owned)
 //   grad_self[r_f] += g_f s_f [a_f > 0]           fp32 atomics into the R1 relation rows
-template <int NC>
+template <int NC, bool kSelfAtomics = true>
 __global__ void __launch_bounds__(256) graft_aggregate_bwd_kernel(const TrainArgs a) {
   const int lane = threadIdx.x & 31;
   const int64_t n = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -417,7 +417,7 @@ __global__ void __launch_bounds__(256) graft_aggregate_bwd_kernel(const TrainArg
         if (s != 0.f && x > 0.f) {          // strict: relu'(0) = 0, as torch
           const float v = __fmul_rn(g, s);
           gh[k] = __fadd_rn(gh[k], v);
-          if (v != 0.f) atomicAdd(gs_row + c, v);
+          if (kSelfAtomics && v != 0.f) atomicAdd(gs_row + c, v);
         }
       }
     }
@@ -517,6 +517,193 @@ __global__ void __launch_bounds__(256, 2) graft_w_bwd_kernel(const float* __rest
       if (v != 0.f) atomicAdd(grad_qh + b * QD + i, v);
     }
   }
+}
+
+// ---- deterministic backward (torch.use_deterministic_algorithms) --------------------------------------------------
+// grad_s and grad_head of graft_aggregate_bwd_kernel are already owned sums; only grad_self and the attention
+// gradients need a fixed order.  Both use the fixed-window segmented sums of common.cuh.
+
+constexpr int kFactWin = 64;   // relation-index entries per window (grad_self, grad_rel)
+
+// grad_self[r] += sum over the staged facts of relation r, in slot order, of  g_f s_f [a_f > 0]  (as the atomics of
+// graft_aggregate_bwd_kernel; g_f = G[tail_f] * mask_f / (1 - p), a_f = self_tab[r] + head_tab[head_f]).
+// Entry i of the relation index -> staged fact f = rix_fact[i].
+template <int NC>
+__global__ void __launch_bounds__(256) graft_self_det_kernel(const TrainArgs a, const int32_t* __restrict__ rix_ptr,
+                                                             const int32_t* __restrict__ rix_fact,
+                                                             const int32_t* __restrict__ heads,
+                                                             const int32_t* __restrict__ rels,
+                                                             const int32_t* __restrict__ tails,
+                                                             float* __restrict__ part, int64_t R1) {
+  const int lane = threadIdx.x & 31;
+  const int64_t win = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t L = rix_ptr[R1];
+  const int64_t lo = win * kFactWin, hi = min(L, lo + kFactWin);
+  if (lo >= L) return;
+  const int D = a.D;
+  const bool drop = a.seed != nullptr;
+  const uint64_t seed = drop ? (uint64_t)__ldg(a.seed) : 0;
+  auto seg_of = [&](int64_t i) { return (int64_t)rels[rix_fact[i]]; };
+  float st[NC], acc[NC];
+  int64_t cur = -1;
+  bool first = true;
+  auto flush = [&]() {
+    const int slot = segwin_slot(lo, hi, L, cur, first, seg_of);
+    segwin_store<NC>(acc, slot, part + (win * 2 + (slot > 0)) * D, a.grad_self + cur * a.ld_gself, D);
+    first = false;
+  };
+  for (int64_t i = lo; i < hi; ++i) {
+    const int f = rix_fact[i];
+    const int64_t r = rels[f];
+    if (r != cur) {
+      if (cur >= 0) flush();
+      cur = r;
+#pragma unroll
+      for (int k = 0; k < NC; ++k) {
+        const int c = lane + 32 * k;
+        st[k] = c < D ? __ldg(a.self_tab + r * a.ld_self + c) : 0.f;
+        acc[k] = 0.f;
+      }
+    }
+    const float s = __ldg(a.s + f);
+    if (s == 0.f) continue;
+    const int64_t h = heads[f], t = tails[f], sl = __ldg(a.slot_of + f);
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const int c = lane + 32 * k;
+      if (c < D && __fadd_rn(st[k], __ldg(a.head_tab + h * a.ld_head + c)) > 0.f) {
+        float g = __ldg(a.grad + t * a.ld_grad + c);
+        if (drop) g = drop_keep(seed, sl, c, a.p) ? __fmul_rn(g, a.scale) : 0.f;
+        acc[k] = __fadd_rn(acc[k], __fmul_rn(g, s));
+      }
+    }
+  }
+  flush();
+}
+
+// relation of slot s as the forward reads it (out-of-range ids are reported by the forward and read as row 0)
+__device__ __forceinline__ int64_t slot_rel(const int64_t* kb_fact_rel, int64_t s, int64_t R1) {
+  const int64_t r = kb_fact_rel[s];
+  return (r < 0 || r >= R1) ? 0 : r;
+}
+
+// c[s, q] = grad_W[s] a_{s,q} (1 + z_{s,q} - W_s) / div for every slot (0 where grad_W == 0 and for masked tokens),
+// one warp per slot, the operations of graft_w_bwd_kernel.
+template <int NC>
+__global__ void __launch_bounds__(256) graft_w_coef_kernel(const float* __restrict__ qh,
+                                                           const float* __restrict__ qmask, int Q,
+                                                           const float* __restrict__ rel, int64_t ldr, int64_t R1,
+                                                           const int64_t* __restrict__ kb_fact_rel, int64_t S,
+                                                           int64_t max_fact, int D, float div,
+                                                           const float* __restrict__ gW, float* __restrict__ coef) {
+  const int lane = threadIdx.x & 31;
+  const int64_t s = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (s >= S) return;
+  float* cs = coef + s * Q;
+  const float g = __ldg(gW + s);
+  if (g == 0.f) {
+    for (int q = lane; q < Q; q += 32) cs[q] = 0.f;
+    return;
+  }
+  const int64_t b = s / max_fact, r = slot_rel(kb_fact_rel, s, R1);
+  const float* qb = qh + b * (int64_t)Q * D;
+  const float* mb = qmask + b * (int64_t)Q;
+  float rv[NC];
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const int c = lane + 32 * k;
+    rv[k] = c < D ? __ldg(rel + r * ldr + c) : 0.f;
+  }
+  float mx = -INFINITY;
+#pragma unroll 1
+  for (int q = 0; q < Q; ++q) {
+    const float sim = __fadd_rn(__fdiv_rn(warp_dot<NC>(rv, qb + (int64_t)q * D, D), div),
+                                __fmul_rn(1.0f - __ldg(mb + q), kVeryNeg));
+    mx = fmaxf(mx, sim);
+  }
+  float den = 0.f, wz = 0.f;
+#pragma unroll 1
+  for (int q = 0; q < Q; ++q) {
+    const float z = __fdiv_rn(warp_dot<NC>(rv, qb + (int64_t)q * D, D), div);
+    const float e = expf(__fadd_rn(z, __fmul_rn(1.0f - __ldg(mb + q), kVeryNeg)) - mx);
+    den += e;
+    wz = fmaf(e, z, wz);
+  }
+  const float inv = __frcp_rn(den), Wr = wz * inv, ginv = g * inv * __frcp_rn(div);
+#pragma unroll 1
+  for (int q = 0; q < Q; ++q) {
+    const float z = __fdiv_rn(warp_dot<NC>(rv, qb + (int64_t)q * D, D), div);
+    const float e = expf(__fadd_rn(z, __fmul_rn(1.0f - __ldg(mb + q), kVeryNeg)) - mx);
+    if (lane == 0) cs[q] = e * ginv * (1.0f + z - Wr);
+  }
+}
+
+// grad_qh[b, q, c] += sum over the question's slots f, in slot order, of c[f, q] rel[r_f, c] (one thread per element)
+__global__ void graft_qh_det_kernel(const float* __restrict__ coef, int Q, const float* __restrict__ rel,
+                                    int64_t ldr, int64_t R1, const int64_t* __restrict__ kb_fact_rel, int B,
+                                    int64_t max_fact, int D, float* __restrict__ grad_qh) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)B * Q * D) return;
+  const int64_t c = i % D, q = (i / D) % Q, b = i / ((int64_t)Q * D);
+  float v = 0.f;
+  for (int64_t s = b * max_fact, e = s + max_fact; s < e; ++s) {
+    const float cq = coef[s * Q + q];
+    if (cq != 0.f) v = __fadd_rn(v, __fmul_rn(cq, __ldg(rel + slot_rel(kb_fact_rel, s, R1) * ldr + c)));
+  }
+  grad_qh[i] = __fadd_rn(grad_qh[i], v);
+}
+
+// grad_rel[r] += sum over the slots of relation r, in slot order, of sum_q c[s, q] qh[b_s, q] (q in order).
+// Entry i of the slot-level relation index -> slot rix_slot[i].
+template <int NC>
+__global__ void __launch_bounds__(256) graft_rel_det_kernel(const float* __restrict__ coef, int Q,
+                                                            const float* __restrict__ qh, int64_t R1,
+                                                            const int64_t* __restrict__ kb_fact_rel,
+                                                            int64_t max_fact, int D,
+                                                            const int32_t* __restrict__ rix_ptr,
+                                                            const int32_t* __restrict__ rix_slot,
+                                                            float* __restrict__ grad_rel, int64_t ld_grel,
+                                                            float* __restrict__ part) {
+  const int lane = threadIdx.x & 31;
+  const int64_t win = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t L = rix_ptr[R1];
+  const int64_t lo = win * kFactWin, hi = min(L, lo + kFactWin);
+  if (lo >= L) return;
+  auto seg_of = [&](int64_t i) { return slot_rel(kb_fact_rel, rix_slot[i], R1); };
+  float acc[NC];
+  int64_t cur = -1;
+  bool first = true;
+  auto flush = [&]() {
+    const int slot = segwin_slot(lo, hi, L, cur, first, seg_of);
+    segwin_store<NC>(acc, slot, part + (win * 2 + (slot > 0)) * D, grad_rel + cur * ld_grel, D);
+    first = false;
+  };
+  for (int64_t i = lo; i < hi; ++i) {
+    const int64_t s = rix_slot[i], r = slot_rel(kb_fact_rel, s, R1);
+    if (r != cur) {
+      if (cur >= 0) flush();
+      cur = r;
+#pragma unroll
+      for (int k = 0; k < NC; ++k) acc[k] = 0.f;
+    }
+    const float* qb = qh + (s / max_fact) * (int64_t)Q * D;
+    float t[NC];
+#pragma unroll
+    for (int k = 0; k < NC; ++k) t[k] = 0.f;
+#pragma unroll 1
+    for (int q = 0; q < Q; ++q) {
+      const float cq = coef[s * Q + q];
+      if (cq == 0.f) continue;           // warp-uniform
+#pragma unroll
+      for (int k = 0; k < NC; ++k) {
+        const int c = lane + 32 * k;
+        if (c < D) t[k] = __fadd_rn(t[k], __fmul_rn(cq, __ldg(qb + (int64_t)q * D + c)));
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < NC; ++k) acc[k] = __fadd_rn(acc[k], t[k]);
+  }
+  flush();
 }
 
 }  // namespace
@@ -760,6 +947,119 @@ extern "C" int gr_graft_attention_backward(const float* qh, const float* qmask, 
                                                       grad_W, grad_qh, grad_rel, ld_grel, smem_acc)
   GR_NC_SWITCH(D, GR_LAUNCH)
 #undef GR_LAUNCH
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+// ---- deterministic training entry points ---------------------------------------------------------------------------
+
+extern "C" size_t gr_graft_aggregate_backward_det_workspace_bytes(int64_t F, int D) {
+  if (F < 0 || D <= 0) return 0;
+  return segwin_part_bytes(F, D, kFactWin);
+}
+
+extern "C" int gr_graft_aggregate_backward_det(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                               const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                               const float* self_tab, int64_t ld_self, const float* head_tab,
+                                               int64_t ld_head, const int64_t* seed, double p, const float* grad_sum,
+                                               int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
+                                               float* grad_head, int64_t ld_ghead, int B, int N, int D,
+                                               const int32_t* heads, const int32_t* rels, const int32_t* tails,
+                                               const int32_t* rix_ptr, const int32_t* rix_fact, int64_t R1, int64_t F,
+                                               void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512 && R1 > 0 && F >= 0, "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG(rowptr_h && src_h && rel_h && fact_h && slot_of && s && self_tab && head_tab && grad_sum && grad_s &&
+                   grad_self && grad_head && heads && rels && tails && rix_ptr && rix_fact, "null pointer");
+  GR_CHECK_ARG(ld_self >= D && ld_head >= D && ld_grad >= D && ld_gself >= D && ld_ghead >= D,
+               "leading dimension smaller than D");
+  TrainArgs a{};
+  if (int rc = drop_args(seed, p, a)) return rc;
+  const size_t need = segwin_part_bytes(F, D, kFactWin);
+  if (!workspace || workspace_bytes < need) {
+    set_error("gr_graft_aggregate_backward_det: workspace too small (%zu < %zu)", workspace_bytes, need);
+    return GR_ERR_WORKSPACE;
+  }
+  a.rowptr = rowptr_h; a.src = src_h; a.rel = rel_h; a.fact = fact_h; a.slot_of = slot_of;
+  a.s = s; a.self_tab = self_tab; a.head_tab = head_tab; a.ld_self = ld_self; a.ld_head = ld_head;
+  a.grad = grad_sum; a.ld_grad = ld_grad;
+  a.grad_s = grad_s; a.grad_self = grad_self; a.grad_head = grad_head; a.ld_gself = ld_gself; a.ld_ghead = ld_ghead;
+  a.Nt = (int64_t)B * N; a.D = D;
+  const int grid = (int)ceil_div(a.Nt, 8);
+#define GR_LAUNCH(NC) graft_aggregate_bwd_kernel<NC, false><<<grid, 256, 0, stream>>>(a)
+  GR_NC_SWITCH(D, GR_LAUNCH)
+#undef GR_LAUNCH
+  GR_CHECK_LAUNCH();
+  if (F == 0) return GR_OK;
+  float* part = reinterpret_cast<float*>(workspace);
+  const int grid_w = (int)ceil_div(ceil_div(F, kFactWin), 8);
+#define GR_LAUNCH(NC) \
+  graft_self_det_kernel<NC><<<grid_w, 256, 0, stream>>>(a, rix_ptr, rix_fact, heads, rels, tails, part, R1)
+  GR_NC_SWITCH(D, GR_LAUNCH)
+#undef GR_LAUNCH
+  GR_CHECK_LAUNCH();
+  segwin_combine_kernel<kFactWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, rix_ptr, 0, R1, grad_self,
+                                                                                  ld_gself);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+namespace {
+struct AttnDetWs {
+  size_t coef_bytes, total;
+};
+AttnDetWs attn_det_ws(int64_t S, int Q, int D) {
+  AttnDetWs w;
+  w.coef_bytes = align_up((size_t)(S > 0 ? S : 1) * (size_t)Q * sizeof(float), 256);
+  w.total = w.coef_bytes + segwin_part_bytes(S, D, kFactWin);
+  return w;
+}
+}  // namespace
+
+extern "C" size_t gr_graft_attention_backward_det_workspace_bytes(int B, int64_t max_fact, int Q, int D) {
+  if (B <= 0 || max_fact < 0 || Q <= 0 || D <= 0) return 0;
+  return attn_det_ws((int64_t)B * max_fact, Q, D).total;
+}
+
+extern "C" int gr_graft_attention_backward_det(const float* qh, const float* qmask, int Q, const float* rel,
+                                               int64_t ldr, int64_t R1, const int64_t* kb_fact_rel, int B,
+                                               int64_t max_fact, int D, const float* grad_W, float* grad_qh,
+                                               float* grad_rel, int64_t ld_grel, const int32_t* rix_ptr,
+                                               const int32_t* rix_slot, void* workspace, size_t workspace_bytes,
+                                               void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(B > 0 && D > 0 && D <= 512 && Q > 0 && max_fact >= 0 && R1 > 0 && ldr >= D && ld_grel >= D,
+               "bad sizes (need 0 < D <= 512, Q > 0)");
+  GR_CHECK_ARG(qh && qmask && rel && kb_fact_rel && grad_W && grad_qh && grad_rel && rix_ptr, "null pointer");
+  GR_CHECK_ARG(max_fact == 0 || rix_slot, "null pointer");
+  const int64_t S = (int64_t)B * max_fact;
+  GR_CHECK_ARG(S < 0x7fffffff, "B*max_fact exceeds int32");
+  if (S == 0) return GR_OK;
+  const AttnDetWs ws = attn_det_ws(S, Q, D);
+  if (!workspace || workspace_bytes < ws.total) {
+    set_error("gr_graft_attention_backward_det: workspace too small (%zu < %zu)", workspace_bytes, ws.total);
+    return GR_ERR_WORKSPACE;
+  }
+  float* coef = reinterpret_cast<float*>(workspace);
+  float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws.coef_bytes);
+  const float div = (float)sqrt((double)D);
+#define GR_LAUNCH(NC)                                                                                            \
+  graft_w_coef_kernel<NC><<<(int)ceil_div(S, 8), 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S,   \
+                                                                   max_fact, D, div, grad_W, coef)
+  GR_NC_SWITCH(D, GR_LAUNCH)
+#undef GR_LAUNCH
+  GR_CHECK_LAUNCH();
+  graft_qh_det_kernel<<<(int)ceil_div((int64_t)B * Q * D, 256), 256, 0, stream>>>(coef, Q, rel, ldr, R1, kb_fact_rel,
+                                                                                  B, max_fact, D, grad_qh);
+  GR_CHECK_LAUNCH();
+#define GR_LAUNCH(NC)                                                                                        \
+  graft_rel_det_kernel<NC><<<(int)ceil_div(ceil_div(S, kFactWin), 8), 256, 0, stream>>>(                   \
+      coef, Q, qh, R1, kb_fact_rel, max_fact, D, rix_ptr, rix_slot, grad_rel, ld_grel, part)
+  GR_NC_SWITCH(D, GR_LAUNCH)
+#undef GR_LAUNCH
+  GR_CHECK_LAUNCH();
+  segwin_combine_kernel<kFactWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, rix_ptr, 0, R1, grad_rel,
+                                                                                  ld_grel);
   GR_CHECK_LAUNCH();
   return GR_OK;
 }

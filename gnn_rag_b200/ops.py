@@ -135,6 +135,8 @@ class CsrGraph:
         self.status = torch.zeros(1, **i32)
         self.w_t = self.w_h = None        # normalized_gnn edge weights (1/outdeg(head))
         self.wr_t = self.wr_h = None      # norm_rel edge weights (1/count(head, rel))
+        self.nfacts = None                # device int32[1] live fact count when F is a capacity
+        self.rel_index = {}               # direction -> relation index of that CSR (deterministic backward)
 
     def check_status(self):
         if int(self.status.item()) != 0:
@@ -161,7 +163,30 @@ def csr_build(heads, rels, tails, B, N, R1, nfacts=None):
                             _p(g.status), _p(nfacts), _p(ws), ws_bytes, _stream())
     _lib.check(rc)
     STATS.launches += 9 if F > 0 else 5     # memsets excluded: hist, 3x scan, place, 2x sort, fill (+gather)
+    g.nfacts = nfacts
     return g
+
+
+def _relation_index(keys, R1, nfacts=None):
+    """(rix_ptr int32 [R1+1], rix_slot): the positions of ``keys`` (a relation id per list entry, int32 or int64,
+    all in [0, R1)) grouped by relation, in increasing position inside each relation -- gr_csr_build keyed on the
+    relation.  The list order the deterministic backward kernels sum in."""
+    g = csr_build(keys, keys, keys, 1, R1, R1, nfacts=nfacts)
+    return g.rowptr_t, g.fact_t
+
+
+def csr_relation_index(g, direction):
+    """Relation index of one destination CSR of ``g`` ('fwd': tail CSR, 'inv': head CSR), built once and cached on
+    the graph: (rix_ptr [R1+1], rix_slot = that CSR's slots sorted by (relation, slot), row_of = the row of every
+    slot)."""
+    if direction not in g.rel_index:
+        rp, rel = (g.rowptr_t, g.rel_t) if direction == "fwd" else (g.rowptr_h, g.rel_h)
+        rix_ptr, rix_slot = _relation_index(rel[: g.F], g.R1, g.nfacts)
+        row_of = torch.empty(max(pad4(g.F), 4), dtype=torch.int32, device=rp.device)
+        _lib.check(_L().gr_csr_row_of(_p(rp), g.B * g.N, _p(row_of), _stream()))
+        STATS.launches += 1
+        g.rel_index[direction] = (rix_ptr, rix_slot, row_of)
+    return g.rel_index[direction]
 
 
 def gather_f32(values, fact):
@@ -256,9 +281,11 @@ def aggregate(g, direction, prior, table, ins, out=None, out_col0=0, seg_stride=
     return out
 
 
-def aggregate_backward(g, direction, prior, table, ins, grad_out, grad_table, grad_ins, grad_prior, w=None):
+def aggregate_backward(g, direction, prior, table, ins, grad_out, grad_table, grad_ins, grad_prior, w=None,
+                       deterministic=False):
     """Accumulate the gradients of :func:`aggregate` (same ``direction`` / CSR) into grad_table [R1,D], grad_ins
-    [B,I,D], grad_prior [B,N]; grad_out [B*N, I*D] contiguous rows (csrc/aggregate_bwd.cu)."""
+    [B,I,D], grad_prior [B,N]; grad_out [B*N, I*D] contiguous rows (csrc/aggregate_bwd.cu).  ``deterministic``:
+    the fixed-order kernels (gr_aggregate_backward_det) instead of the fp32 atomics."""
     prior = _cuda(prior, torch.float32, "prior").contiguous()
     table = _cuda(table, torch.float32, "table").contiguous()
     ins = _cuda(ins, torch.float32, "ins").contiguous()
@@ -266,6 +293,21 @@ def aggregate_backward(g, direction, prior, table, ins, grad_out, grad_table, gr
     B, I, D = ins.shape
     assert grad_out.stride(1) == 1 and grad_table.is_contiguous() and grad_ins.is_contiguous() and grad_prior.is_contiguous()
     rp, src, rel = (g.rowptr_t, g.src_t, g.rel_t) if direction == "fwd" else (g.rowptr_h, g.src_h, g.rel_h)
+    if deterministic:
+        assert grad_table.shape[0] >= g.R1
+        rix_ptr, rix_slot, row_of = csr_relation_index(g, direction)
+        fact, rp_o, fact_o = (g.fact_t, g.rowptr_h, g.fact_h) if direction == "fwd" else (g.fact_h, g.rowptr_t, g.fact_t)
+        L = _L()
+        nbytes = L.gr_aggregate_backward_det_workspace_bytes(B, g.N, D, I, g.F)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=prior.device)
+        with _OpTimer("aggregation_bwd_det"):
+            rc = L.gr_aggregate_backward_det(_p(rp), _p(src), _p(rel), _p(fact), _p(w), _p(prior), _p(table), _p(ins),
+                                             _p(grad_out), grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins),
+                                             _p(grad_prior), B, g.N, D, I, g.F, _p(rp_o), _p(fact_o), _p(rix_ptr),
+                                             _p(rix_slot), _p(row_of), g.R1, _p(ws), nbytes, _stream())
+        _lib.check(rc)
+        STATS.launches += 5 if g.F > 0 else 0
+        return
     with _OpTimer("aggregation_bwd"):
         rc = _L().gr_aggregate_backward(_p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table), _p(ins), _p(grad_out),
                                         grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins), _p(grad_prior),
@@ -902,6 +944,22 @@ class GraftGraph:
         self.status = torch.zeros(1, **i32)
         self.graph = None
         self.kb_fact_rel = None
+        self.rel_index = {}      # (kind, R1) -> relation index of the staged facts / of all slots (deterministic backward)
+
+    def fact_relation_index(self, R1):
+        """(rix_ptr, rix_fact): the staged facts grouped by relation, in slot order inside each relation."""
+        if ("facts", R1) not in self.rel_index:
+            self.rel_index[("facts", R1)] = _relation_index(self.rels[: self.cap], R1, self.nfacts)
+        return self.rel_index[("facts", R1)]
+
+    def slot_relation_index(self, R1):
+        """(rix_ptr, rix_slot): all B*max_fact slots grouped by relation (ids outside [0, R1) read as 0, as the
+        attention kernels read them), in slot order inside each relation."""
+        if ("slots", R1) not in self.rel_index:
+            r = self.kb_fact_rel.reshape(-1)
+            r = torch.where((r < 0) | (r >= R1), torch.zeros_like(r), r)
+            self.rel_index[("slots", R1)] = _relation_index(r, R1)
+        return self.rel_index[("slots", R1)]
 
     _MESSAGES = {1: "a batch, fact-slot or node id outside the batch", 2: "a relation id outside the relation table",
                  4: "a fact slot listed twice", 8: "a fact slot with a head but no tail (or a tail but no head)"}
@@ -1054,9 +1112,11 @@ def graft_aggregate_train(gg, s, self_tab, head_tab, seed=None, p=0.0, sum_out=N
     return sum_out
 
 
-def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_self, grad_head, seed=None, p=0.0):
+def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_self, grad_head, seed=None, p=0.0,
+                             deterministic=False):
     """Accumulate the gradients of :func:`graft_aggregate_train` (same s, tables, seed and p) into grad_s [F],
-    grad_self [R1, D] and grad_head [B*N, D] (gr_graft_aggregate_backward, over the head CSR)."""
+    grad_self [R1, D] and grad_head [B*N, D] (gr_graft_aggregate_backward, over the head CSR).  ``deterministic``:
+    grad_self in relation order instead of fp32 atomics (gr_graft_aggregate_backward_det)."""
     g = gg.graph
     self_tab = _cuda(self_tab, torch.float32, "self_tab")
     head_tab = _cuda(head_tab, torch.float32, "head_tab")
@@ -1068,6 +1128,22 @@ def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_s
     seed, p = _seed_p(seed, p)
     if s.numel() == 0:               # no staged facts: nothing to add
         return
+    if deterministic:
+        R1 = self_tab.shape[0]
+        rix_ptr, rix_fact = gg.fact_relation_index(R1)
+        L = _L()
+        nbytes = L.gr_graft_aggregate_backward_det_workspace_bytes(gg.cap, D)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=s.device)
+        with _OpTimer("aggregation_bwd_det"):
+            rc = L.gr_graft_aggregate_backward_det(
+                _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h), _p(gg.slot_of), _p(s), _p(self_tab),
+                self_tab.stride(0), _p(head_tab), head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0),
+                _p(grad_s), _p(grad_self), grad_self.stride(0), _p(grad_head), grad_head.stride(0), gg.B, gg.N, D,
+                _p(gg.heads), _p(gg.rels), _p(gg.tails), _p(rix_ptr), _p(rix_fact), R1, gg.cap, _p(ws), nbytes,
+                _stream())
+        _lib.check(rc)
+        STATS.launches += 3
+        return
     with _OpTimer("aggregation_bwd"):
         rc = _L().gr_graft_aggregate_backward(_p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h), _p(gg.slot_of),
                                               _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab),
@@ -1078,15 +1154,32 @@ def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_s
     STATS.launches += 1
 
 
-def graft_attention_backward(gg, qh, qmask, rel, grad_W, grad_qh, grad_rel):
+def graft_attention_backward(gg, qh, qmask, rel, grad_W, grad_qh, grad_rel, deterministic=False):
     """Accumulate dL/dqh [B, Q, D] and dL/drel [R1, D] of :func:`graft_attention`'s W given grad_W [B*max_fact]
-    (gr_graft_attention_backward)."""
+    (gr_graft_attention_backward).  ``deterministic``: per-slot coefficients, then fixed-order sums by question and
+    by relation (gr_graft_attention_backward_det)."""
     qh = _cuda(qh, torch.float32, "qh").contiguous()
     qmask = _cuda(qmask, torch.float32, "qmask").contiguous()
     rel = _cuda(rel, torch.float32, "rel")
     grad_W = _cuda(grad_W, torch.float32, "grad_W").contiguous()
     assert rel.stride(1) == 1 and grad_rel.stride(1) == 1 and grad_qh.is_contiguous()
     B, Q, D = qh.shape
+    if deterministic:
+        if gg.max_fact == 0:
+            return
+        R1 = rel.shape[0]
+        rix_ptr, rix_slot = gg.slot_relation_index(R1)
+        L = _L()
+        nbytes = L.gr_graft_attention_backward_det_workspace_bytes(B, gg.max_fact, Q, D)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=qh.device)
+        with _OpTimer("graft_attention_bwd_det"):
+            rc = L.gr_graft_attention_backward_det(_p(qh), _p(qmask), Q, _p(rel), rel.stride(0), R1,
+                                                   _p(gg.kb_fact_rel), B, gg.max_fact, D, _p(grad_W), _p(grad_qh),
+                                                   _p(grad_rel), grad_rel.stride(0), _p(rix_ptr), _p(rix_slot),
+                                                   _p(ws), nbytes, _stream())
+        _lib.check(rc)
+        STATS.launches += 4
+        return
     with _OpTimer("graft_attention_bwd"):
         rc = _L().gr_graft_attention_backward(_p(qh), _p(qmask), Q, _p(rel), rel.stride(0), rel.shape[0],
                                               _p(gg.kb_fact_rel), B, gg.max_fact, D, _p(grad_W), _p(grad_qh),
@@ -1095,13 +1188,29 @@ def graft_attention_backward(gg, qh, qmask, rel, grad_W, grad_qh, grad_rel):
     STATS.launches += 1 if gg.max_fact > 0 else 0
 
 
-def type_layer_backward(g, grad_out, out, grad_table, w_t=None, w_h=None):
+def type_layer_backward(g, grad_out, out, grad_table, w_t=None, w_h=None, deterministic=False):
     """Accumulate dL/dtable [R1, D] of :func:`type_layer` given grad_out and the forward's fp32 ``out`` [B*N, D]
-    (gr_type_layer_backward)."""
+    (gr_type_layer_backward).  ``deterministic``: relation-ordered sums instead of fp32 atomics
+    (gr_type_layer_backward_det)."""
     grad_out = _cuda(grad_out, torch.float32, "grad_out")
     out = _cuda(out, torch.float32, "out")
     assert grad_out.stride(1) == 1 and out.stride(1) == 1 and grad_table.stride(1) == 1
     D = out.shape[1]
+    if deterministic:
+        assert grad_table.shape[0] >= g.R1
+        ptr_t, slot_t, row_t = csr_relation_index(g, "fwd")
+        ptr_h, slot_h, row_h = csr_relation_index(g, "inv")
+        L = _L()
+        nbytes = L.gr_type_layer_backward_det_workspace_bytes(g.F, D)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
+        with _OpTimer("type_layer_bwd_det"):
+            rc = L.gr_type_layer_backward_det(_p(g.rel_t), _p(w_t), _p(ptr_t), _p(slot_t), _p(row_t), _p(g.rel_h),
+                                              _p(w_h), _p(ptr_h), _p(slot_h), _p(row_h), _p(grad_out),
+                                              grad_out.stride(0), _p(out), out.stride(0), _p(grad_table),
+                                              grad_table.stride(0), g.R1, D, g.F, _p(ws), nbytes, _stream())
+        _lib.check(rc)
+        STATS.launches += 4 if g.F > 0 else 0
+        return
     with _OpTimer("type_layer_bwd"):
         rc = _L().gr_type_layer_backward(_p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.rel_h), _p(w_h),
                                          _p(grad_out), grad_out.stride(0), _p(out), out.stride(0), _p(grad_table),

@@ -355,6 +355,62 @@ int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* rel_t, const 
                            const float* grad_out, int64_t ld_grad, const float* out, int64_t ld_out,
                            float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F, void* stream);
 
+/* Deterministic backward (torch.use_deterministic_algorithms): the gradients of the four entry points above, each
+ * output element a sum whose order is fixed by the data alone -- fact, slot and row ids and compile-time window sizes,
+ * never the grid, the SM count or block arrival.  No floating-point atomics; every term and sum is rounded with
+ * __fmul_rn / __fadd_rn.  Same accumulate-into-the-caller's-buffers convention as the atomic versions.
+ *
+ * The relation-keyed sums walk a relation index: gr_csr_build called with heads = rels = tails = the relation id of
+ * each list entry and Nt = num_rel_rows = R1, whose tail CSR (rix_ptr [R1+1], rix_slot) lists each relation's entries
+ * in increasing entry order.  row_of (gr_csr_row_of) maps a CSR slot to its row.  Partial sums go to `workspace`
+ * (size from the *_workspace_bytes helper, allocated by the caller): windows of 32 rows / 64 entries each add their
+ * entries in list order; sums that cross a window edge are then added in window order (csrc/common.cuh).
+ *
+ * gr_aggregate_backward_det: gr_aggregate_backward's arguments, plus fact (this CSR's slot -> fact id), the OTHER
+ *   destination CSR (rowptr_o, fact_o: it lists every source's out-edges in slot order) and this CSR's relation index
+ *   (rix_ptr, rix_slot over this CSR's slots, row_of).  dx per question over windows of 32 destination rows; dp[s] adds
+ *   q_e = w_e^2 <G[n_e], relu(P[r_e] x_j[b])> over the other CSR's row s; dP per relation over windows of 64 entries.
+ * gr_type_layer_backward_det: the relation indexes of both CSRs; grad_table[r] = (grad_table[r] + tail-CSR sum) +
+ *   head-CSR sum, each over the relation's slots in slot order.  No rowptr / B / N: the row comes from row_of.
+ * gr_graft_aggregate_backward_det: gr_graft_aggregate_backward's arguments, plus the staged facts (heads, rels, tails
+ *   of gr_graft_stage) and their relation index (rix_ptr, rix_fact over staged fact ids; F = the fact capacity).
+ *   grad_s and grad_head are the owned sums of the atomic version; grad_self per relation in slot order.
+ * gr_graft_attention_backward_det: a slot-level relation index over all B*max_fact slots (relation ids out of range
+ *   read as 0, as the forward does).  The coefficients c_{s,q} go to the workspace; grad_qh[b, q] sums the question's
+ *   slots in slot order, grad_rel[r] the relation's slots in slot order (each term summed over q in order).
+ */
+int gr_csr_row_of(const int32_t* rowptr, int64_t Nt, int32_t* row_of, void* stream);
+size_t gr_aggregate_backward_det_workspace_bytes(int B, int N, int D, int I, int64_t F);
+int gr_aggregate_backward_det(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const int32_t* fact,
+                              const float* w, const float* prior, const float* table, const float* ins,
+                              const float* grad_out, int64_t grad_row_stride, int64_t grad_col0, int64_t seg_stride,
+                              float* grad_table, float* grad_ins, float* grad_prior, int B, int N, int D, int I,
+                              int64_t F, const int32_t* rowptr_o, const int32_t* fact_o, const int32_t* rix_ptr,
+                              const int32_t* rix_slot, const int32_t* row_of, int64_t R1, void* workspace,
+                              size_t workspace_bytes, void* stream);
+size_t gr_type_layer_backward_det_workspace_bytes(int64_t F, int D);
+int gr_type_layer_backward_det(const int32_t* rel_t, const float* w_t, const int32_t* rix_ptr_t,
+                               const int32_t* rix_slot_t, const int32_t* row_of_t, const int32_t* rel_h,
+                               const float* w_h, const int32_t* rix_ptr_h, const int32_t* rix_slot_h,
+                               const int32_t* row_of_h, const float* grad_out, int64_t ld_grad, const float* out,
+                               int64_t ld_out, float* grad_table, int64_t ld_gtable, int64_t R1, int D, int64_t F,
+                               void* workspace, size_t workspace_bytes, void* stream);
+size_t gr_graft_aggregate_backward_det_workspace_bytes(int64_t F, int D);
+int gr_graft_aggregate_backward_det(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                    const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                    const float* self_tab, int64_t ld_self, const float* head_tab, int64_t ld_head,
+                                    const int64_t* seed, double p, const float* grad_sum, int64_t ld_grad,
+                                    float* grad_s, float* grad_self, int64_t ld_gself, float* grad_head,
+                                    int64_t ld_ghead, int B, int N, int D, const int32_t* heads, const int32_t* rels,
+                                    const int32_t* tails, const int32_t* rix_ptr, const int32_t* rix_fact, int64_t R1,
+                                    int64_t F, void* workspace, size_t workspace_bytes, void* stream);
+size_t gr_graft_attention_backward_det_workspace_bytes(int B, int64_t max_fact, int Q, int D);
+int gr_graft_attention_backward_det(const float* qh, const float* qmask, int Q, const float* rel, int64_t ldr,
+                                    int64_t R1, const int64_t* kb_fact_rel, int B, int64_t max_fact, int D,
+                                    const float* grad_W, float* grad_qh, float* grad_rel, int64_t ld_grel,
+                                    const int32_t* rix_ptr, const int32_t* rix_slot, void* workspace,
+                                    size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Sparse-prior fast path for one ReaRev layer (the first layer of every iteration sees the seed distribution,
  * rearev.py:208).  Rows none of whose in-edges carries prior mass get exactly zero neighbour messages, so

@@ -1,12 +1,17 @@
-"""GraftNet training step on one GPU: the kernel path of ``model(batch, training=True)`` (fact attention, fact messages
+"""Training step on one GPU, two paths alternating in one run.
+
+    python scripts/graftnet_train_probe.py [--model graftnet|rearev|nsm] [--compare torch|det] [--B 64] [--N 2000]
+                                           [--E 6000] [--dims 50,200] [--steps 10] [--warmup 2] [--dropout 0.2]
+                                           [--out results/train_probe.json]
+
+``--compare torch`` (GraftNet only): the kernel path of ``model(batch, training=True)`` (fact attention, fact messages
 and TypeLayer in csrc/graft.cu / csrc/aggregate_bwd.cu) against the per-fact torch path (``autograd_path.USE_KERNELS =
-False``), alternating in one run.
+False``).  ``--compare det``: the default backward kernels against the deterministic ones
+(``torch.use_deterministic_algorithms(True)``; CUBLAS_WORKSPACE_CONFIG is set before torch is imported), with the
+device time of every backward kernel class from CUDA events in one extra step per mode.
 
-    python scripts/graftnet_train_probe.py [--B 64] [--N 2000] [--E 6000] [--dims 50,200] [--steps 10] [--warmup 2]
-                                           [--dropout 0.2] [--out results/graftnet_train_probe.json]
-
-One step = forward + backward + Adam step from the loader's numpy tuple, as ``Trainer_KBQA.train_epoch`` runs it
-(gnn/train_model.py:219-231).  Step time: host clock between device synchronisations (the step reads metrics back to
+One step = forward + backward + clip_grad_norm_ + Adam step from the loader's numpy tuple, as
+``Trainer_KBQA.train_epoch`` runs it (gnn/train_model.py:219-231).  Step time: host clock between device synchronisations (the step reads metrics back to
 the host itself), median over ``--steps`` per path.  Peak memory: ``torch.cuda.max_memory_allocated`` over each path's
 steps, reset before them, and the same less what was allocated before the step (parameters, Adam state).  The card name
 and power limit are read in the same run (nvidia-smi query only)."""
@@ -18,12 +23,14 @@ import sys
 import time
 
 import numpy as np
-import torch
+
+os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")      # before cuBLAS starts: the deterministic mode needs it
+import torch  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import gnn_rag_b200 as G  # noqa: E402
-from gnn_rag_b200 import autograd_path, synthetic as S  # noqa: E402
+from gnn_rag_b200 import autograd_path, ops, synthetic as S  # noqa: E402
 
 NUM_ENTITY, NUM_REL, NUM_WORD = 100_000, 6106, 5000
 
@@ -43,12 +50,52 @@ def step(m, opt, batch):
     opt.zero_grad(set_to_none=True)
     loss = m(batch, training=True)[0]
     loss.backward()
+    torch.nn.utils.clip_grad_norm_([p for p in m.parameters() if p.requires_grad], 1.0)
     opt.step()
     return float(loss.detach())
 
 
+def set_mode(compare, mode):
+    if compare == "torch":
+        autograd_path.USE_KERNELS = mode
+    else:
+        torch.use_deterministic_algorithms(mode)
+
+
+def backward_kernel_ms(m, opt, batch):
+    """Device time (ms) per backward kernel class in one step, from the CUDA events ops records around each call."""
+    ops.STATS.reset()
+    ops.STATS.time_ops = True
+    try:
+        step(m, opt, batch)
+        torch.cuda.synchronize()
+    finally:
+        ops.STATS.time_ops = False
+    out = {}
+    for s, e, cls, _info in ops.STATS.op_events:
+        if "bwd" in cls:
+            out[cls] = out.get(cls, 0.0) + s.elapsed_time(e)
+    ops.STATS.reset()
+    return out
+
+
+def make_model(model, D, layers, dropout):
+    if model == "graftnet":
+        args = S.model_args("GraftNet", entity_dim=D, num_layer=layers, word_dim=300, use_cuda=True,
+                            linear_dropout=dropout)
+        return G.GraftNet(dict(args), NUM_ENTITY, NUM_REL, NUM_WORD)
+    if model == "rearev":
+        args = S.model_args("ReaRev", entity_dim=D, num_iter=3, num_ins=2, num_gnn=3, word_dim=300, use_cuda=True,
+                            linear_dropout=dropout)
+        return G.ReaRev(dict(args), NUM_ENTITY, NUM_REL, NUM_WORD)
+    args = S.model_args("NSM", entity_dim=D, num_step=3, word_dim=300, use_cuda=True, linear_dropout=dropout)
+    return G.NSM(dict(args), NUM_ENTITY, NUM_REL, NUM_WORD)
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", choices=["graftnet", "rearev", "nsm"], default="graftnet")
+    ap.add_argument("--compare", choices=["torch", "det"], default="torch")
     ap.add_argument("--B", type=int, default=64)
     ap.add_argument("--N", type=int, default=2000)
     ap.add_argument("--E", type=int, default=6000)
@@ -63,18 +110,23 @@ def main():
         raise SystemExit("graftnet_train_probe measures on a GPU; none is visible")
     torch.cuda.set_device(0)
     name, power = card()
-    res = dict(card=name, power_limit=power, B=a.B, N=a.N, E=a.E, layers=a.layers, linear_dropout=a.dropout, dims={})
-    batch = S.make_graft_batch(0, a.B, a.N, a.E, num_entity=NUM_ENTITY, num_relation=NUM_REL, num_word=NUM_WORD,
-                               with_weights=False, test=False)
-    res["graft_facts"] = int(len(batch[3][0][0]))
+    if a.compare == "torch" and a.model != "graftnet":
+        raise SystemExit("--compare torch is a GraftNet comparison")
+    res = dict(card=name, power_limit=power, model=a.model, compare=a.compare, B=a.B, N=a.N, E=a.E, layers=a.layers,
+               linear_dropout=a.dropout, dims={})
+    if a.model == "graftnet":
+        batch = S.make_graft_batch(0, a.B, a.N, a.E, num_entity=NUM_ENTITY, num_relation=NUM_REL, num_word=NUM_WORD,
+                                   with_weights=False, test=False)
+        res["graft_facts"] = int(len(batch[3][0][0]))
+        res["max_fact"] = int(batch[5].shape[1])
+    else:
+        batch = S.make_batch(0, a.B, a.N, a.E, num_entity=NUM_ENTITY, num_relation=NUM_REL, num_word=NUM_WORD,
+                             test=False)
     res["kb_facts"] = int(len(batch[2][0]))
-    res["max_fact"] = int(batch[5].shape[1])
-    paths = {"kernels": True, "torch": False}
+    paths = {"kernels": True, "torch": False} if a.compare == "torch" else {"default": False, "deterministic": True}
     for D in [int(x) for x in a.dims.split(",")]:
-        args = S.model_args("GraftNet", entity_dim=D, num_layer=a.layers, word_dim=300, use_cuda=True,
-                            linear_dropout=a.dropout)
         torch.manual_seed(0)
-        m = G.GraftNet(dict(args), NUM_ENTITY, NUM_REL, NUM_WORD).cuda().train()
+        m = make_model(a.model, D, a.layers, a.dropout).cuda().train()
         opt = torch.optim.Adam([p for p in m.parameters() if p.requires_grad], lr=1e-4)
         times = {k: [] for k in paths}
         peak = {k: 0 for k in paths}
@@ -82,12 +134,12 @@ def main():
         losses = {k: [] for k in paths}
         try:
             for k, mode in paths.items():          # warm-up (module loads, cuBLAS heuristics, Adam state)
-                autograd_path.USE_KERNELS = mode
+                set_mode(a.compare, mode)
                 for _ in range(a.warmup):
                     step(m, opt, batch)
             for _ in range(a.steps):
                 for k, mode in paths.items():      # alternate the two paths
-                    autograd_path.USE_KERNELS = mode
+                    set_mode(a.compare, mode)
                     torch.cuda.synchronize()
                     base = torch.cuda.memory_allocated()
                     torch.cuda.reset_peak_memory_stats()
@@ -98,15 +150,22 @@ def main():
                     mx = torch.cuda.max_memory_allocated()
                     peak[k] = max(peak[k], mx)
                     peak_step[k] = max(peak_step[k], mx - base)
+            kernel_ms = {}
+            for k, mode in paths.items():
+                set_mode(a.compare, mode)
+                kernel_ms[k] = backward_kernel_ms(m, opt, batch)
         finally:
             autograd_path.USE_KERNELS = True
+            torch.use_deterministic_algorithms(False)
         r = {}
         for k in paths:
             r[k] = dict(step_ms_median=float(np.median(times[k])), step_ms_min=float(np.min(times[k])),
                         step_ms_max=float(np.max(times[k])), peak_mem_gb=peak[k] / 1e9,
-                        peak_step_mem_gb=peak_step[k] / 1e9, loss_first=losses[k][0], loss_last=losses[k][-1])
-        r["speedup_median"] = r["torch"]["step_ms_median"] / r["kernels"]["step_ms_median"]
-        r["peak_step_mem_ratio_torch_over_kernels"] = peak_step["torch"] / max(peak_step["kernels"], 1)
+                        peak_step_mem_gb=peak_step[k] / 1e9, loss_first=losses[k][0], loss_last=losses[k][-1],
+                        backward_kernel_ms=kernel_ms[k])
+        slow, fast = list(paths)[1], list(paths)[0]
+        r["step_time_ratio_%s_over_%s" % (slow, fast)] = r[slow]["step_ms_median"] / r[fast]["step_ms_median"]
+        r["peak_step_mem_ratio_%s_over_%s" % (slow, fast)] = peak_step[slow] / max(peak_step[fast], 1)
         res["dims"][D] = r
         print(json.dumps({D: r}))
         del m, opt

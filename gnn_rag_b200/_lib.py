@@ -101,6 +101,33 @@ SIGNATURES = {
     "gr_graft_attention_backward_det": (c_int, [c_f32p, c_f32p, c_int, c_f32p, c_i64, c_i64, c_void_p, c_int, c_i64,
                                                 c_int, c_f32p, c_f32p, c_f32p, c_i64, c_i32p, c_i32p, c_void_p,
                                                 c_size, c_void_p]),
+    "gr_aggregate_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_void_p, c_i64, c_i64, c_i64,
+                                c_f32p, c_int, c_int, c_int, c_int, c_i64, c_u32, c_void_p]),
+    "gr_aggregate_backward_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_void_p, c_i64,
+                                         c_i64, c_i64, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_i64, c_u32,
+                                         c_void_p]),
+    "gr_aggregate_backward_det_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_void_p,
+                                             c_i64, c_i64, c_i64, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int,
+                                             c_i64, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i64, c_void_p, c_size,
+                                             c_u32, c_void_p]),
+    "gr_type_layer_ex": (c_int, [c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_f32p, c_f32p, c_void_p, c_i64,
+                                 c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_i64, c_u32, c_void_p]),
+    "gr_type_layer_backward_ex": (c_int, [c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_f32p, c_void_p, c_i64, c_void_p,
+                                          c_i64, c_f32p, c_i64, c_int, c_int, c_int, c_i64, c_u32, c_void_p]),
+    "gr_type_layer_backward_det_ex": (c_int, [c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p,
+                                              c_i32p, c_void_p, c_i64, c_void_p, c_i64, c_f32p, c_i64, c_i64, c_int,
+                                              c_i64, c_void_p, c_size, c_u32, c_void_p]),
+    "gr_graft_aggregate_train_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_void_p,
+                                            c_i64, c_void_p, c_dbl, c_void_p, c_i64, c_int, c_int, c_int, c_u32,
+                                            c_void_p]),
+    "gr_graft_aggregate_backward_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64,
+                                               c_void_p, c_i64, c_void_p, c_dbl, c_void_p, c_i64, c_f32p, c_f32p, c_i64,
+                                               c_void_p, c_i64, c_int, c_int, c_int, c_u32, c_void_p]),
+    "gr_graft_aggregate_backward_det_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64,
+                                                   c_void_p, c_i64, c_void_p, c_dbl, c_void_p, c_i64, c_f32p, c_f32p,
+                                                   c_i64, c_void_p, c_i64, c_int, c_int, c_int, c_i32p, c_i32p,
+                                                   c_i32p, c_i32p, c_i32p, c_i64, c_i64, c_void_p, c_size, c_u32,
+                                                   c_void_p]),
     "gr_frontier_rows": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i64, c_i32p, c_i32p, c_void_p]),
     "gr_frontier_fixup": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p,
                                   c_f32p, c_f32p, c_f32p, c_void_p, c_void_p, c_i64, c_f32p, c_i64, c_f32p,

@@ -14,7 +14,12 @@ device (CUDA when the model lives there -- no CPU fallback is involved) so that 
     restatement is the CPU reference under ``HOST_CHECK`` and the ``USE_KERNELS = False`` path;
   * under ``torch.use_deterministic_algorithms(True)`` (``warn_only`` included), read by each Function at forward,
     those backward kernels are the fixed-order, atomic-free variants: every gradient they produce is a pure function
-    of the inputs.  The torch restatement's ``index_add`` is made deterministic by torch itself under the same flag.
+    of the inputs.  The torch restatement's ``index_add`` is made deterministic by torch itself under the same flag;
+  * under ``torch.autocast("cuda", dtype=torch.bfloat16)``, read by each Function at forward as well, the kernels take
+    and produce their node-sized tensors ([B*N, D] outputs and gradients) in bf16: the same fp32 arithmetic, with each
+    stored value rounded to nearest even.  Their small operands (relation tables, instructions, priors, per-fact
+    scalars) are cast to fp32 inside the Functions.  Under fp16 autocast the Functions cast to fp32 and run the fp32
+    kernels.  The torch restatement accumulates its scatters in fp32.
 
 Reference: ReaRev.forward gnn/models/ReaRev/rearev.py:163-243, ReasonGNNLayer.forward gnn/modules/kg_reasoning/
 reasongnn.py:61-174, TypeLayer.forward gnn/modules/layer_init.py:25-62, BaseInstruction.get_instruction
@@ -56,8 +61,9 @@ class _Facts:
 
 
 def _scatter_rows(values, dst, rows):
-    out = torch.zeros(rows, values.shape[1], dtype=values.dtype, device=values.device)
-    return out.index_add_(0, dst, values)
+    """Row sums in fp32 (bf16 / fp16 values under autocast are widened; fp32 values are used as they are)."""
+    out = torch.zeros(rows, values.shape[1], dtype=torch.float32, device=values.device)
+    return out.index_add_(0, dst, values.float())
 
 
 def _type_layer(layer, facts, rel_features, Nt, graph=None):
@@ -88,6 +94,16 @@ HOST_CHECK = False      # tests only: let a CPU-resident model evaluate this res
                         # ``model(batch, training=True)`` on a CPU model raises, like the inference path.
 
 
+def _autocast_bf16():
+    """True under torch.autocast("cuda", dtype=torch.bfloat16): the training kernels then produce their node-sized
+    outputs in bf16.  Read by each Function at forward, like the deterministic flag."""
+    return torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
+
+
+def _node_dtype():
+    return torch.bfloat16 if _autocast_bf16() else torch.float32
+
+
 def _require_cuda(dev):
     if dev.type != "cuda" and not HOST_CHECK:
         raise RuntimeError("gnn_rag_b200 runs on CUDA only: move the model to an H100 (model.cuda()); there is no CPU "
@@ -96,12 +112,15 @@ def _require_cuda(dev):
 
 class _AggregateFn(torch.autograd.Function):
     """out[n, j, :] = sum_{e -> n} w_e^2 p[src_e] relu(table[rel_e] * ins[b, j]) for all instructions j of one direction:
-    forward = gr_aggregate (csrc/aggregate.cu), backward = gr_aggregate_backward (csrc/aggregate_bwd.cu)."""
+    forward = gr_aggregate (csrc/aggregate.cu), backward = gr_aggregate_backward (csrc/aggregate_bwd.cu).  The output
+    is bf16 under bf16 autocast; the backward reads grad_out in its own dtype."""
 
     @staticmethod
     def forward(ctx, table, ins, prior, graph, direction, w):
         from . import ops
-        out = ops.aggregate(graph, direction, prior.detach(), table.detach(), ins.detach(), w=w)
+        ctx.dtypes = (table.dtype, ins.dtype, prior.dtype)
+        table, ins, prior = table.detach().float(), ins.detach().float(), prior.detach().float()
+        out = ops.aggregate(graph, direction, prior, table, ins, w=w, dtype=_node_dtype())
         ctx.save_for_backward(table, ins, prior)
         ctx.graph, ctx.direction, ctx.w = graph, direction, w
         ctx.det = torch.are_deterministic_algorithms_enabled()
@@ -115,21 +134,21 @@ class _AggregateFn(torch.autograd.Function):
         gt, gi, gp = (torch.zeros_like(t, memory_format=torch.contiguous_format) for t in (table, ins, prior))
         ops.aggregate_backward(ctx.graph, ctx.direction, prior, table.contiguous(), ins.contiguous(),
                                grad_out.contiguous(), gt, gi, gp, ctx.w, deterministic=ctx.det)
-        return gt, gi, gp, None, None, None
+        return (*(g.to(dt) for g, dt in zip((gt, gi, gp), ctx.dtypes)), None, None, None)
 
 
 class _TypeLayerFn(torch.autograd.Function):
     """out = relu(sum_{tail CSR} w_e table[rel_e] + sum_{head CSR} w_e table[rel_e]) (TypeLayer, layer_init.py:46-57):
     forward = gr_type_layer (csrc/aggregate.cu), backward = gr_type_layer_backward (csrc/aggregate_bwd.cu); saves the
-    [B*N, D] output for the relu mask."""
+    [B*N, D] output (bf16 under bf16 autocast) for the relu mask."""
 
     @staticmethod
     def forward(ctx, table, graph, w_t, w_h):
         from . import ops
-        out = torch.empty(graph.B * graph.N, table.shape[1], dtype=torch.float32, device=table.device)
-        ops.type_layer(graph, table.detach(), out, w_t, w_h)
+        out = torch.empty(graph.B * graph.N, table.shape[1], dtype=_node_dtype(), device=table.device)
+        ops.type_layer(graph, table.detach().float(), out, w_t, w_h)
         ctx.save_for_backward(out)
-        ctx.graph, ctx.w, ctx.rows = graph, (w_t, w_h), table.shape[0]
+        ctx.graph, ctx.w, ctx.rows, ctx.dtype = graph, (w_t, w_h), table.shape[0], table.dtype
         ctx.det = torch.are_deterministic_algorithms_enabled()
         return out
 
@@ -137,9 +156,11 @@ class _TypeLayerFn(torch.autograd.Function):
     def backward(ctx, grad_out):
         from . import ops
         out, = ctx.saved_tensors
+        if grad_out.dtype != out.dtype:      # widening is exact: same gradients as with grad_out in out's dtype
+            out, grad_out = out.float(), grad_out.float()
         gt = torch.zeros(ctx.rows, out.shape[1], dtype=torch.float32, device=out.device)
         ops.type_layer_backward(ctx.graph, grad_out.contiguous(), out, gt, *ctx.w, deterministic=ctx.det)
-        return gt, None, None, None
+        return gt.to(ctx.dtype), None, None, None
 
 
 FACT_KERNEL_MAX_D = 512    # widths the TypeLayer / GraftNet training kernels cover; wider models keep the torch ops
@@ -402,7 +423,9 @@ class _GraftAttentionFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, qh, rel, qmask, gg):
         from . import ops
-        W, _wt, _e = ops.graft_attention(gg, qh.detach(), qmask, rel.detach().contiguous(), out_w=True)
+        ctx.dtypes = (qh.dtype, rel.dtype)
+        qh, rel, qmask = qh.detach().float(), rel.detach().float().contiguous(), qmask.float()
+        W, _wt, _e = ops.graft_attention(gg, qh, qmask, rel, out_w=True)
         ctx.save_for_backward(qh, rel, qmask)
         ctx.gg = gg
         ctx.det = torch.are_deterministic_algorithms_enabled()
@@ -414,21 +437,24 @@ class _GraftAttentionFn(torch.autograd.Function):
         qh, rel, qmask = ctx.saved_tensors
         gq = torch.zeros(qh.shape, dtype=torch.float32, device=qh.device)
         gr = torch.zeros(rel.shape, dtype=torch.float32, device=rel.device)
-        ops.graft_attention_backward(ctx.gg, qh, qmask, rel.contiguous(), grad_W.reshape(-1), gq, gr,
+        ops.graft_attention_backward(ctx.gg, qh, qmask, rel.contiguous(), grad_W.float().reshape(-1), gq, gr,
                                      deterministic=ctx.det)
-        return gq, gr, None, None
+        return gq.to(ctx.dtypes[0]), gr.to(ctx.dtypes[1]), None, None
 
 
 class _GraftAggregateFn(torch.autograd.Function):
     """sum_out[n] = sum_{f -> n} drop_f(relu(self_tab[r_f] + head_tab[head_f])) * s_f over the staged graft facts
     (graft_gnn.py:103-107 before kb_tail_linear): forward = gr_graft_aggregate_train, backward =
-    gr_graft_aggregate_backward.  The dropout mask is recomputed from the saved seed, never stored."""
+    gr_graft_aggregate_backward.  The dropout mask is recomputed from the saved seed, never stored.  Under bf16
+    autocast head_tab, sum_out and their gradients are bf16 (self_tab and s fp32)."""
 
     @staticmethod
     def forward(ctx, self_tab, head_tab, s, gg, seed, p):
         from . import ops
-        out = ops.graft_aggregate_train(gg, s.detach(), self_tab.detach().contiguous(), head_tab.detach().contiguous(),
-                                        seed, p)
+        ctx.dtypes = (self_tab.dtype, head_tab.dtype, s.dtype)
+        self_tab, s = self_tab.detach().float().contiguous(), s.detach().float()
+        head_tab = head_tab.detach().to(_node_dtype()).contiguous()
+        out = ops.graft_aggregate_train(gg, s, self_tab, head_tab, seed, p)
         ctx.save_for_backward(self_tab, head_tab, s, seed)
         ctx.gg, ctx.p = gg, p
         ctx.det = torch.are_deterministic_algorithms_enabled()
@@ -438,12 +464,14 @@ class _GraftAggregateFn(torch.autograd.Function):
     def backward(ctx, grad_out):
         from . import ops
         self_tab, head_tab, s, seed = ctx.saved_tensors
+        if grad_out.dtype != head_tab.dtype:     # widening is exact: same gradients as with grad_out in head_tab's dtype
+            head_tab, grad_out = head_tab.float(), grad_out.float()
         gs = torch.zeros(s.shape, dtype=torch.float32, device=s.device)
         gself = torch.zeros(self_tab.shape, dtype=torch.float32, device=s.device)
-        ghead = torch.zeros(head_tab.shape, dtype=torch.float32, device=s.device)
-        ops.graft_aggregate_backward(ctx.gg, s, self_tab.contiguous(), head_tab.contiguous(), grad_out.contiguous(),
-                                     gs, gself, ghead, seed, ctx.p, deterministic=ctx.det)
-        return gself, ghead, gs, None, None, None
+        ghead = torch.zeros(head_tab.shape, dtype=head_tab.dtype, device=s.device)
+        ops.graft_aggregate_backward(ctx.gg, s, self_tab, head_tab, grad_out.contiguous(), gs, gself, ghead, seed,
+                                     ctx.p, deterministic=ctx.det)
+        return (*(g.to(dt) for g, dt in zip((gself, ghead, gs), ctx.dtypes)), None, None, None)
 
 
 def _graft_kernel_batch(model, batch, dev):
@@ -531,7 +559,7 @@ def graftnet_forward(model, batch):
             v = F.relu(layer.lin("kb_self_linear", i)(rel)[fact_rel] + layer.lin("kb_head_linear", i)(drop(h))[head])
             v = v * s.unsqueeze(1)
             f2e = F.relu(layer.lin("kb_self_linear", i)(h) + torch.zeros(Nt, D, device=dev).index_add(
-                0, tail, layer.lin("kb_tail_linear", i)(drop(v))))
+                0, tail, layer.lin("kb_tail_linear", i)(drop(v)).float()))
         d = lam * torch.zeros(Nt, device=dev).index_add(0, tail, s) + (1 - lam) * d
         x = torch.cat([h, q2e, layer.fact_scale * f2e], dim=1)
         query = torch.bmm(d.view(B, 1, N), layer.lin("e2q_linear", i)(drop(x)).view(B, N, D))

@@ -60,6 +60,7 @@ struct AggParams {
   int64_t out_row_stride, out_col0, seg_stride_j, seg_stride_dir;
   int B, N, D, I, j0;   // this launch handles instructions j0 .. j0+NI-1
   int64_t Nt, Fpad;
+  __nv_bfloat16* out_bf;    // bf16 output instead of `out` (training under torch.autocast, GR_IO_BF16)
 };
 
 template <int VEC> struct Vec;
@@ -116,6 +117,20 @@ __device__ __forceinline__ SplitVec<VEC> split_vec(const float (&y)[VEC]) {
     r.l[0] = *reinterpret_cast<const unsigned short*>(&l);
   }
   return r;
+}
+
+// bf16 store of y rounded to nearest even (the packed conversions round each element like __float2bfloat16_rn)
+template <int VEC>
+__device__ __forceinline__ void st_bf16(__nv_bfloat16* p, const float (&y)[VEC]) {
+  if constexpr (VEC == 4) {
+    const __nv_bfloat162 a = __floats2bfloat162_rn(y[0], y[1]), b = __floats2bfloat162_rn(y[2], y[3]);
+    *reinterpret_cast<uint2*>(p) =
+        make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
+  } else if constexpr (VEC == 2) {
+    *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(y[0], y[1]);
+  } else {
+    *p = __float2bfloat16_rn(y[0]);
+  }
 }
 
 template <int VEC>
@@ -193,7 +208,8 @@ __device__ __forceinline__ void msg_epilogue(float (&y)[VEC], const float (&xp)[
 // both fixed every output-segment offset is an immediate, which removes the per-store address arithmetic the
 // generic kernel spends most of its issue slots on; the dual-direction ReaRev layout (segment 2j+d at column
 // (2j+d)*SEGP) is assumed when DT != 0.
-template <int VEC, int CH, int NI, int MODE, bool USE_TMA, bool PLANES, int DT, int SEGP>
+// OUT_BF16: the fp32 values of `out` are stored rounded to bf16 in p.out_bf (same row stride / column indexing).
+template <int VEC, int CH, int NI, int MODE, bool USE_TMA, bool PLANES, int DT, int SEGP, bool OUT_BF16 = false>
 __global__ void __launch_bounds__(kThreads, 2) agg_kernel(const AggParams p) {
   __shared__ int32_t s_rowptr[2][kRows + 1];
   __shared__ int2 s_rc[2][kEdgeCap];                       // {table byte offset rel*D*4, float_as_int(c)}
@@ -336,7 +352,8 @@ __global__ void __launch_bounds__(kThreads, 2) agg_kernel(const AggParams p) {
         for (int k = 0; k < VEC; ++k) xp[j][ch][k] = xn[j][ch][k] = 0.f;
 
     // per-lane base pointers of the tile (row 0, this lane's chunk-0 column)
-    float* const out_lane = PLANES ? nullptr : p.out + r0 * ld + p.out_col0 + col0 + j0off;
+    float* const out_lane = PLANES || OUT_BF16 ? nullptr : p.out + r0 * ld + p.out_col0 + col0 + j0off;
+    __nv_bfloat16* const bf_lane = OUT_BF16 ? p.out_bf + r0 * ld + p.out_col0 + col0 + j0off : nullptr;
     __nv_bfloat16* const hi_lane = PLANES ? p.out_hi + r0 * ld + p.out_col0 + col0 + j0off : nullptr;
     __nv_bfloat16* const lo_lane = PLANES ? p.out_lo + r0 * ld + p.out_col0 + col0 + j0off : nullptr;
 
@@ -367,13 +384,16 @@ __global__ void __launch_bounds__(kThreads, 2) agg_kernel(const AggParams p) {
         }
       }
       const int64_t rowoff = (int64_t)lr * ld;        // warp-uniform
-      float* const orow = PLANES ? nullptr : out_lane + rowoff;
+      float* const orow = PLANES || OUT_BF16 ? nullptr : out_lane + rowoff;
+      __nv_bfloat16* const brow = OUT_BF16 ? bf_lane + rowoff : nullptr;
       __nv_bfloat16* const hrow = PLANES ? hi_lane + rowoff : nullptr;
       __nv_bfloat16* const lrow = PLANES ? lo_lane + rowoff : nullptr;
       auto store = [&](int off, bool pred, const float (&y)[VEC]) {   // off: warp-uniform element offset
         if constexpr (PLANES) {
           const SplitVec<VEC> sv = split_vec<VEC>(y);
           if (pred) st_split<VEC>(hrow + off, lrow + off, sv);
+        } else if constexpr (OUT_BF16) {
+          if (pred) st_bf16<VEC>(brow + off, y);
         } else {
           if (pred) st_vec<VEC>(orow + off, y);
         }
@@ -388,7 +408,11 @@ __global__ void __launch_bounds__(kThreads, 2) agg_kernel(const AggParams p) {
           float z[VEC];
 #pragma unroll
           for (int k = 0; k < VEC; ++k) z[k] = 0.f;
-          if (pred) st_vec<VEC>(orow + off, z);
+          if constexpr (OUT_BF16) {
+            if (pred) st_bf16<VEC>(brow + off, z);
+          } else {
+            if (pred) st_vec<VEC>(orow + off, z);
+          }
         }
       };
       float tsum[CH][VEC];   // MODE_TYPE: sum over both directions
@@ -512,6 +536,12 @@ int launch_agg3(const AggParams& p, bool tma, cudaStream_t stream) {
       agg_kernel<VEC, CH, NI, MODE, false, false, DT, SEGP><<<grid, kThreads, 0, stream>>>(p);
     GR_CHECK_LAUNCH();
   }
+  if constexpr (DT == 0) {   // bf16 output: single-direction training calls only, never the DT-specialised layout
+    if (p.out_bf) {
+      agg_kernel<VEC, CH, NI, MODE, false, false, DT, SEGP, true><<<grid, kThreads, 0, stream>>>(p);
+      GR_CHECK_LAUNCH();
+    }
+  }
   if (p.out_hi) {   // split-bf16 planes (a second launch only if the caller asked for both formats)
     if (tma && DT == 0)
       agg_kernel<VEC, CH, NI, MODE, (DT == 0), true, DT, SEGP><<<grid, kThreads, 0, stream>>>(p);
@@ -546,7 +576,8 @@ int launch_agg(AggParams p, cudaStream_t stream) {
               p.seg_stride_j % v == 0 && p.seg_stride_dir % v == 0 &&
               (reinterpret_cast<size_t>(p.out) % a) == 0 && (reinterpret_cast<size_t>(p.ins) % a) == 0 &&
               p.ld_planes % v == 0 && (reinterpret_cast<size_t>(p.out_hi) % (a / 2)) == 0 &&
-              (reinterpret_cast<size_t>(p.out_lo) % (a / 2)) == 0;
+              (reinterpret_cast<size_t>(p.out_lo) % (a / 2)) == 0 &&
+              (reinterpret_cast<size_t>(p.out_bf) % (a / 2)) == 0;
     for (int d = 0; d < p.ndir; ++d) ok = ok && (reinterpret_cast<size_t>(p.dir[d].table) % a) == 0;
     return ok;
   };
@@ -631,23 +662,34 @@ extern "C" int gr_debug_store_probe(void* hi, void* lo, int64_t Nt, int64_t ld, 
   return GR_OK;
 }
 
-extern "C" int gr_aggregate(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
-                            const float* w, const float* prior, const float* table, const float* ins,
-                            float* out, int64_t out_row_stride, int64_t out_col0, int64_t seg_stride,
-                            float* possible, int B, int N, int D, int I, int64_t F, void* stream_) {
+extern "C" int gr_aggregate_ex(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const float* w,
+                               const float* prior, const float* table, const float* ins, void* out,
+                               int64_t out_row_stride, int64_t out_col0, int64_t seg_stride, float* possible, int B,
+                               int N, int D, int I, int64_t F, uint32_t io, void* stream_) {
   using namespace gr;
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
   GR_CHECK_ARG(rowptr && prior && table && ins && out, "null pointer");
   GR_CHECK_ARG(F == 0 || (src && rel), "null edge arrays");
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && I > 0, "B, N, D, I must be positive");
   AggParams p{};
   p.dir[0] = AggDir{rowptr, src, rel, w, table};
   p.ndir = 1;
-  p.prior = prior; p.ins = ins; p.out = out; p.possible = possible;
+  p.prior = prior; p.ins = ins; p.possible = possible;
+  if (io_bf16(io)) p.out_bf = static_cast<__nv_bfloat16*>(out);
+  else p.out = static_cast<float*>(out);
   p.out_row_stride = out_row_stride; p.out_col0 = out_col0;
   p.seg_stride_j = seg_stride; p.seg_stride_dir = 0;
   p.B = B; p.N = N; p.D = D; p.I = I; p.j0 = 0;
   p.Nt = (int64_t)B * N; p.Fpad = gr_pad4(F);
   return launch_agg<MODE_MSG>(p, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gr_aggregate(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
+                            const float* w, const float* prior, const float* table, const float* ins,
+                            float* out, int64_t out_row_stride, int64_t out_col0, int64_t seg_stride,
+                            float* possible, int B, int N, int D, int I, int64_t F, void* stream_) {
+  return gr_aggregate_ex(rowptr, src, rel, w, prior, table, ins, out, out_row_stride, out_col0, seg_stride, possible,
+                         B, N, D, I, F, 0u, stream_);
 }
 
 extern "C" int gr_aggregate_dual(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
@@ -679,12 +721,12 @@ extern "C" int gr_aggregate_dual(const int32_t* rowptr_t, const int32_t* src_t, 
   return launch_agg<MODE_MSG>(p, reinterpret_cast<cudaStream_t>(stream_));
 }
 
-extern "C" int gr_type_layer(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
-                             const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
-                             const float* table, float* out, int64_t out_row_stride, void* out_hi,
-                             void* out_lo, int64_t ld_planes, int B, int N, int D, int64_t F,
-                             void* stream_) {
+extern "C" int gr_type_layer_ex(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                                const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h, const float* table,
+                                void* out, int64_t out_row_stride, void* out_hi, void* out_lo, int64_t ld_planes,
+                                int B, int N, int D, int64_t F, uint32_t io, void* stream_) {
   using namespace gr;
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
   GR_CHECK_ARG(rowptr_t && rowptr_h && table, "null pointer");
   GR_CHECK_ARG(out || (out_hi && out_lo), "no output requested");
   GR_CHECK_ARG(F == 0 || (rel_t && rel_h), "null edge arrays");
@@ -693,7 +735,9 @@ extern "C" int gr_type_layer(const int32_t* rowptr_t, const int32_t* rel_t, cons
   p.dir[0] = AggDir{rowptr_t, nullptr, rel_t, w_t, table};
   p.dir[1] = AggDir{rowptr_h, nullptr, rel_h, w_h, table};
   p.ndir = 2;
-  p.prior = nullptr; p.ins = nullptr; p.out = out; p.possible = nullptr;
+  p.prior = nullptr; p.ins = nullptr; p.possible = nullptr;
+  if (io_bf16(io)) p.out_bf = static_cast<__nv_bfloat16*>(out);
+  else p.out = static_cast<float*>(out);
   p.out_hi = reinterpret_cast<__nv_bfloat16*>(out_hi); p.out_lo = reinterpret_cast<__nv_bfloat16*>(out_lo);
   p.ld_planes = out_hi ? ld_planes : 0;
   p.out_row_stride = out_row_stride; p.out_col0 = 0;
@@ -701,4 +745,13 @@ extern "C" int gr_type_layer(const int32_t* rowptr_t, const int32_t* rel_t, cons
   p.B = B; p.N = N; p.D = D; p.I = 1; p.j0 = 0;
   p.Nt = (int64_t)B * N; p.Fpad = gr_pad4(F);
   return launch_agg<MODE_TYPE>(p, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gr_type_layer(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                             const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
+                             const float* table, float* out, int64_t out_row_stride, void* out_hi,
+                             void* out_lo, int64_t ld_planes, int B, int N, int D, int64_t F,
+                             void* stream_) {
+  return gr_type_layer_ex(rowptr_t, rel_t, w_t, rowptr_h, rel_h, w_h, table, out, out_row_stride, out_hi, out_lo,
+                          ld_planes, B, N, D, F, 0u, stream_);
 }

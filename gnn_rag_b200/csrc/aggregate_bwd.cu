@@ -35,7 +35,7 @@ struct BwdParams {
   const float* prior;
   const float* table;     // [R1, D]
   const float* ins;       // [B, I, D]
-  const float* gout;      // [Nt, ld]: G[n, j, d] at n * ld + col0 + j * seg + d
+  const void* gout;       // [Nt, ld] fp32 or bf16: G[n, j, d] at n * ld + col0 + j * seg + d
   int64_t ld, col0, seg;
   float* gtable;          // [R1, D]   +=
   float* gins;            // [B, I, D] +=
@@ -44,8 +44,9 @@ struct BwdParams {
   int N, D, I;
 };
 
-template <int NI>
+template <int NI, typename TG>
 __global__ void __launch_bounds__(kBwdThreads) agg_bwd_kernel(const BwdParams p) {
+  const TG* gout = static_cast<const TG*>(p.gout);
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -87,7 +88,7 @@ __global__ void __launch_bounds__(kBwdThreads) agg_bwd_kernel(const BwdParams p)
 #pragma unroll
       for (int k = 0; k < kCPL; ++k) {
         const int c = lane + 32 * k;
-        g[j][k] = c < D ? __ldg(p.gout + n * p.ld + p.col0 + (int64_t)j * p.seg + c) : 0.f;
+        g[j][k] = c < D ? ldg_node(gout + n * p.ld + p.col0 + (int64_t)j * p.seg + c) : 0.f;
       }
     for (int e = beg; e < end; ++e) {
       const int s = p.src[e], r = p.rel[e];
@@ -149,9 +150,10 @@ struct DetParams {
   int64_t R1;
 };
 
-template <int NI>
+template <int NI, typename TG>
 __global__ void __launch_bounds__(kBwdThreads) agg_bwd_det_rows_kernel(const DetParams d) {
   const BwdParams& p = d.p;
+  const TG* gout = static_cast<const TG*>(p.gout);
   const int lane = threadIdx.x & 31;
   const int64_t win = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t a = win * kRowWin, bnd = min(p.Nt, a + kRowWin);
@@ -192,7 +194,7 @@ __global__ void __launch_bounds__(kBwdThreads) agg_bwd_det_rows_kernel(const Det
 #pragma unroll
       for (int k = 0; k < kCPL; ++k) {
         const int c = lane + 32 * k;
-        g[j][k] = c < D ? __ldg(p.gout + n * p.ld + p.col0 + (int64_t)j * p.seg + c) : 0.f;
+        g[j][k] = c < D ? ldg_node(gout + n * p.ld + p.col0 + (int64_t)j * p.seg + c) : 0.f;
       }
     for (int e = beg; e < end; ++e) {
       const int s = p.src[e], r = p.rel[e];
@@ -237,9 +239,10 @@ __global__ void agg_bwd_det_prior_kernel(const int32_t* __restrict__ rowptr_o, c
 }
 
 // dP[r] over the relation index: entry i -> CSR slot e = rix_slot[i] of relation rel[e], row row_of[e]
-template <int NI>
+template <int NI, typename TG>
 __global__ void __launch_bounds__(kBwdThreads) agg_bwd_det_rel_kernel(const DetParams d) {
   const BwdParams& p = d.p;
+  const TG* gout = static_cast<const TG*>(p.gout);
   const int lane = threadIdx.x & 31;
   const int64_t win = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t L = d.rix_ptr[d.R1];
@@ -288,7 +291,7 @@ __global__ void __launch_bounds__(kBwdThreads) agg_bwd_det_rel_kernel(const DetP
 #pragma unroll
         for (int j = 0; j < NI; ++j)
           if (__fmul_rn(pv[k], x[j][k]) > 0.f)
-            dp_c = __fadd_rn(dp_c, __fmul_rn(__ldg(p.gout + n * p.ld + p.col0 + (int64_t)j * p.seg + c), x[j][k]));
+            dp_c = __fadd_rn(dp_c, __fmul_rn(ldg_node(gout + n * p.ld + p.col0 + (int64_t)j * p.seg + c), x[j][k]));
         acc[k] = __fadd_rn(acc[k], __fmul_rn(c_e, dp_c));
       }
     }
@@ -316,16 +319,19 @@ extern "C" size_t gr_aggregate_backward_det_workspace_bytes(int B, int N, int D,
   return gr::agg_det_ws((int64_t)B * N, D, I, F).total;
 }
 
-extern "C" int gr_aggregate_backward_det(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
-                                         const int32_t* fact, const float* w, const float* prior, const float* table,
-                                         const float* ins, const float* grad_out, int64_t grad_row_stride,
-                                         int64_t grad_col0, int64_t seg_stride, float* grad_table, float* grad_ins,
-                                         float* grad_prior, int B, int N, int D, int I, int64_t F,
-                                         const int32_t* rowptr_o, const int32_t* fact_o, const int32_t* rix_ptr,
-                                         const int32_t* rix_slot, const int32_t* row_of, int64_t R1, void* workspace,
-                                         size_t workspace_bytes, void* stream_) {
+extern "C" int gr_aggregate_backward_det_ex(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
+                                            const int32_t* fact, const float* w, const float* prior,
+                                            const float* table, const float* ins, const void* grad_out,
+                                            int64_t grad_row_stride, int64_t grad_col0, int64_t seg_stride,
+                                            float* grad_table, float* grad_ins, float* grad_prior, int B, int N, int D,
+                                            int I, int64_t F, const int32_t* rowptr_o, const int32_t* fact_o,
+                                            const int32_t* rix_ptr, const int32_t* rix_slot, const int32_t* row_of,
+                                            int64_t R1, void* workspace, size_t workspace_bytes, uint32_t io,
+                                            void* stream_) {
   using namespace gr;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
+  const bool bf = io_bf16(io);
   GR_CHECK_ARG(rowptr && prior && table && ins && grad_out && grad_table && grad_ins && grad_prior && rowptr_o &&
                    rix_ptr, "null pointer");
   GR_CHECK_ARG(F == 0 || (src && rel && fact && fact_o && rix_slot && row_of), "null edge arrays");
@@ -355,14 +361,16 @@ extern "C" int gr_aggregate_backward_det(const int32_t* rowptr, const int32_t* s
   const int grid_rel = (int)ceil_div(ceil_div(F, kRelWin), wpb);
   const int64_t width = (int64_t)I * D;
 #define GR_DET(NI)                                                                                \
-  agg_bwd_det_rows_kernel<NI><<<grid_rows, kBwdThreads, 0, stream>>>(d);                         \
+  if (bf) agg_bwd_det_rows_kernel<NI, __nv_bfloat16><<<grid_rows, kBwdThreads, 0, stream>>>(d);  \
+  else agg_bwd_det_rows_kernel<NI, float><<<grid_rows, kBwdThreads, 0, stream>>>(d);             \
   GR_CHECK_LAUNCH();                                                                              \
   segwin_combine_kernel<kRowWin><<<(int)ceil_div(B * width, 256), 256, 0, stream>>>(            \
       d.part, width, nullptr, N, B, grad_ins, width);                                             \
   GR_CHECK_LAUNCH();                                                                              \
   agg_bwd_det_prior_kernel<<<(int)ceil_div(Nt, 256), 256, 0, stream>>>(rowptr_o, fact_o, d.q, grad_prior, Nt); \
   GR_CHECK_LAUNCH();                                                                              \
-  agg_bwd_det_rel_kernel<NI><<<grid_rel, kBwdThreads, 0, stream>>>(d);                           \
+  if (bf) agg_bwd_det_rel_kernel<NI, __nv_bfloat16><<<grid_rel, kBwdThreads, 0, stream>>>(d);    \
+  else agg_bwd_det_rel_kernel<NI, float><<<grid_rel, kBwdThreads, 0, stream>>>(d);               \
   GR_CHECK_LAUNCH();                                                                              \
   segwin_combine_kernel<kRelWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(               \
       d.part, D, rix_ptr, 0, R1, grad_table, D);
@@ -377,13 +385,27 @@ extern "C" int gr_aggregate_backward_det(const int32_t* rowptr, const int32_t* s
   return GR_OK;
 }
 
-extern "C" int gr_aggregate_backward(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const float* w,
-                                     const float* prior, const float* table, const float* ins, const float* grad_out,
-                                     int64_t grad_row_stride, int64_t grad_col0, int64_t seg_stride, float* grad_table,
-                                     float* grad_ins, float* grad_prior, int B, int N, int D, int I, int64_t F,
-                                     void* stream_) {
+extern "C" int gr_aggregate_backward_det(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
+                                         const int32_t* fact, const float* w, const float* prior, const float* table,
+                                         const float* ins, const float* grad_out, int64_t grad_row_stride,
+                                         int64_t grad_col0, int64_t seg_stride, float* grad_table, float* grad_ins,
+                                         float* grad_prior, int B, int N, int D, int I, int64_t F,
+                                         const int32_t* rowptr_o, const int32_t* fact_o, const int32_t* rix_ptr,
+                                         const int32_t* rix_slot, const int32_t* row_of, int64_t R1, void* workspace,
+                                         size_t workspace_bytes, void* stream_) {
+  return gr_aggregate_backward_det_ex(rowptr, src, rel, fact, w, prior, table, ins, grad_out, grad_row_stride,
+                                      grad_col0, seg_stride, grad_table, grad_ins, grad_prior, B, N, D, I, F, rowptr_o,
+                                      fact_o, rix_ptr, rix_slot, row_of, R1, workspace, workspace_bytes, 0u, stream_);
+}
+
+extern "C" int gr_aggregate_backward_ex(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
+                                        const float* w, const float* prior, const float* table, const float* ins,
+                                        const void* grad_out, int64_t grad_row_stride, int64_t grad_col0,
+                                        int64_t seg_stride, float* grad_table, float* grad_ins, float* grad_prior,
+                                        int B, int N, int D, int I, int64_t F, uint32_t io, void* stream_) {
   using namespace gr;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
   GR_CHECK_ARG(rowptr && prior && table && ins && grad_out && grad_table && grad_ins && grad_prior, "null pointer");
   GR_CHECK_ARG(F == 0 || (src && rel), "null edge arrays");
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 32 * kCPL && I > 0 && I <= 4, "need 0 < D <= 256 and 0 < I <= 4");
@@ -396,14 +418,27 @@ extern "C" int gr_aggregate_backward(const int32_t* rowptr, const int32_t* src, 
   p.gtable = grad_table; p.gins = grad_ins; p.gprior = grad_prior;
   p.Nt = (int64_t)B * N; p.N = N; p.D = D; p.I = I;
   const int grid = (int)std::min<int64_t>(ceil_div(p.Nt * 32, kBwdThreads), 16LL * sm_count());
+#define GR_LAUNCH(NI)                                                                   \
+  if (io_bf16(io)) agg_bwd_kernel<NI, __nv_bfloat16><<<grid, kBwdThreads, 0, stream>>>(p); \
+  else agg_bwd_kernel<NI, float><<<grid, kBwdThreads, 0, stream>>>(p);
   switch (I) {
-    case 1: agg_bwd_kernel<1><<<grid, kBwdThreads, 0, stream>>>(p); break;
-    case 2: agg_bwd_kernel<2><<<grid, kBwdThreads, 0, stream>>>(p); break;
-    case 3: agg_bwd_kernel<3><<<grid, kBwdThreads, 0, stream>>>(p); break;
-    default: agg_bwd_kernel<4><<<grid, kBwdThreads, 0, stream>>>(p); break;
+    case 1: GR_LAUNCH(1) break;
+    case 2: GR_LAUNCH(2) break;
+    case 3: GR_LAUNCH(3) break;
+    default: GR_LAUNCH(4) break;
   }
+#undef GR_LAUNCH
   GR_CHECK_LAUNCH();
   return GR_OK;
+}
+
+extern "C" int gr_aggregate_backward(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const float* w,
+                                     const float* prior, const float* table, const float* ins, const float* grad_out,
+                                     int64_t grad_row_stride, int64_t grad_col0, int64_t seg_stride, float* grad_table,
+                                     float* grad_ins, float* grad_prior, int B, int N, int D, int I, int64_t F,
+                                     void* stream_) {
+  return gr_aggregate_backward_ex(rowptr, src, rel, w, prior, table, ins, grad_out, grad_row_stride, grad_col0,
+                                  seg_stride, grad_table, grad_ins, grad_prior, B, N, D, I, F, 0u, stream_);
 }
 
 // Backward of gr_type_layer (TypeLayer.forward, gnn/modules/layer_init.py:46-57):
@@ -414,15 +449,15 @@ extern "C" int gr_aggregate_backward(const int32_t* rowptr, const int32_t* src, 
 namespace gr {
 namespace {
 
-template <int NC>
+template <int NC, typename T>
 __global__ void __launch_bounds__(kBwdThreads) type_bwd_kernel(const int32_t* __restrict__ rowptr_t,
                                                                const int32_t* __restrict__ rel_t,
                                                                const float* __restrict__ w_t,
                                                                const int32_t* __restrict__ rowptr_h,
                                                                const int32_t* __restrict__ rel_h,
                                                                const float* __restrict__ w_h,
-                                                               const float* __restrict__ grad, int64_t ld_grad,
-                                                               const float* __restrict__ out, int64_t ld_out,
+                                                               const T* __restrict__ grad, int64_t ld_grad,
+                                                               const T* __restrict__ out, int64_t ld_out,
                                                                float* __restrict__ gtable, int64_t ld_gt, int64_t Nt,
                                                                int D) {
   const int lane = threadIdx.x & 31;
@@ -435,7 +470,7 @@ __global__ void __launch_bounds__(kBwdThreads) type_bwd_kernel(const int32_t* __
 #pragma unroll
   for (int k = 0; k < NC; ++k) {
     const int c = lane + 32 * k;
-    g[k] = (c < D && __ldg(out + n * ld_out + c) > 0.f) ? __ldg(grad + n * ld_grad + c) : 0.f;
+    g[k] = (c < D && ldg_node(out + n * ld_out + c) > 0.f) ? ldg_node(grad + n * ld_grad + c) : 0.f;
     any |= g[k] != 0.f;
   }
   if (!__any_sync(0xffffffffu, any)) return;
@@ -469,13 +504,14 @@ __global__ void __launch_bounds__(kBwdThreads) type_bwd_kernel(const int32_t* __
 }  // namespace
 }  // namespace gr
 
-extern "C" int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
-                                      const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
-                                      const float* grad_out, int64_t ld_grad, const float* out, int64_t ld_out,
-                                      float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F,
-                                      void* stream_) {
+extern "C" int gr_type_layer_backward_ex(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                                         const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
+                                         const void* grad_out, int64_t ld_grad, const void* out, int64_t ld_out,
+                                         float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F,
+                                         uint32_t io, void* stream_) {
   using namespace gr;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512 && F >= 0, "bad sizes (need 0 < D <= 512)");
   GR_CHECK_ARG(rowptr_t && rowptr_h && grad_out && out && grad_table, "null pointer");
   GR_CHECK_ARG(F == 0 || (rel_t && rel_h), "null edge arrays");
@@ -484,19 +520,33 @@ extern "C" int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* re
   const int64_t Nt = (int64_t)B * N;
   const int grid = (int)ceil_div(Nt, kBwdThreads / 32);
   const int nc = D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16;
-#define GR_LAUNCH(NC)                                                                                            \
-  type_bwd_kernel<NC><<<grid, kBwdThreads, 0, stream>>>(rowptr_t, rel_t, w_t, rowptr_h, rel_h, w_h, grad_out,     \
-                                                        ld_grad, out, ld_out, grad_table, ld_gtable, Nt, D)
+#define GR_LAUNCH_T(NC, T)                                                                                       \
+  type_bwd_kernel<NC, T><<<grid, kBwdThreads, 0, stream>>>(rowptr_t, rel_t, w_t, rowptr_h, rel_h, w_h,            \
+                                                           static_cast<const T*>(grad_out), ld_grad,               \
+                                                           static_cast<const T*>(out), ld_out, grad_table,         \
+                                                           ld_gtable, Nt, D)
+#define GR_LAUNCH(NC) \
+  if (io_bf16(io)) GR_LAUNCH_T(NC, __nv_bfloat16); else GR_LAUNCH_T(NC, float);
   switch (nc) {
-    case 1: GR_LAUNCH(1); break;
-    case 2: GR_LAUNCH(2); break;
-    case 4: GR_LAUNCH(4); break;
-    case 8: GR_LAUNCH(8); break;
-    default: GR_LAUNCH(16); break;
+    case 1: GR_LAUNCH(1) break;
+    case 2: GR_LAUNCH(2) break;
+    case 4: GR_LAUNCH(4) break;
+    case 8: GR_LAUNCH(8) break;
+    default: GR_LAUNCH(16) break;
   }
 #undef GR_LAUNCH
+#undef GR_LAUNCH_T
   GR_CHECK_LAUNCH();
   return GR_OK;
+}
+
+extern "C" int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                                      const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
+                                      const float* grad_out, int64_t ld_grad, const float* out, int64_t ld_out,
+                                      float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F,
+                                      void* stream_) {
+  return gr_type_layer_backward_ex(rowptr_t, rel_t, w_t, rowptr_h, rel_h, w_h, grad_out, ld_grad, out, ld_out,
+                                   grad_table, ld_gtable, B, N, D, F, 0u, stream_);
 }
 
 // Deterministic variant of gr_type_layer_backward: two fixed-window segmented sums (common.cuh) over the relation
@@ -506,14 +556,14 @@ extern "C" int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* re
 namespace gr {
 namespace {
 
-template <int NC>
+template <int NC, typename T>
 __global__ void __launch_bounds__(kBwdThreads) type_bwd_det_kernel(const int32_t* __restrict__ rix_ptr,
                                                                    const int32_t* __restrict__ rix_slot,
                                                                    const int32_t* __restrict__ rel,
                                                                    const float* __restrict__ w,
                                                                    const int32_t* __restrict__ row_of,
-                                                                   const float* __restrict__ grad, int64_t ld_grad,
-                                                                   const float* __restrict__ out, int64_t ld_out,
+                                                                   const T* __restrict__ grad, int64_t ld_grad,
+                                                                   const T* __restrict__ out, int64_t ld_out,
                                                                    float* __restrict__ gtable, int64_t ld_gt,
                                                                    float* __restrict__ part, int64_t R1, int D) {
   const int lane = threadIdx.x & 31;
@@ -544,7 +594,7 @@ __global__ void __launch_bounds__(kBwdThreads) type_bwd_det_kernel(const int32_t
     for (int k = 0; k < NC; ++k) {
       const int c = lane + 32 * k;
       if (c < D) {
-        const float gm = __ldg(out + n * ld_out + c) > 0.f ? __ldg(grad + n * ld_grad + c) : 0.f;
+        const float gm = ldg_node(out + n * ld_out + c) > 0.f ? ldg_node(grad + n * ld_grad + c) : 0.f;
         acc[k] = __fadd_rn(acc[k], __fmul_rn(we, gm));
       }
     }
@@ -560,15 +610,16 @@ extern "C" size_t gr_type_layer_backward_det_workspace_bytes(int64_t F, int D) {
   return gr::segwin_part_bytes(F, D, gr::kRelWin);
 }
 
-extern "C" int gr_type_layer_backward_det(const int32_t* rel_t, const float* w_t, const int32_t* rix_ptr_t,
-                                          const int32_t* rix_slot_t, const int32_t* row_of_t, const int32_t* rel_h,
-                                          const float* w_h, const int32_t* rix_ptr_h, const int32_t* rix_slot_h,
-                                          const int32_t* row_of_h, const float* grad_out, int64_t ld_grad,
-                                          const float* out, int64_t ld_out, float* grad_table, int64_t ld_gtable,
-                                          int64_t R1, int D, int64_t F, void* workspace, size_t workspace_bytes,
-                                          void* stream_) {
+extern "C" int gr_type_layer_backward_det_ex(const int32_t* rel_t, const float* w_t, const int32_t* rix_ptr_t,
+                                             const int32_t* rix_slot_t, const int32_t* row_of_t, const int32_t* rel_h,
+                                             const float* w_h, const int32_t* rix_ptr_h, const int32_t* rix_slot_h,
+                                             const int32_t* row_of_h, const void* grad_out, int64_t ld_grad,
+                                             const void* out, int64_t ld_out, float* grad_table, int64_t ld_gtable,
+                                             int64_t R1, int D, int64_t F, void* workspace, size_t workspace_bytes,
+                                             uint32_t io, void* stream_) {
   using namespace gr;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
   GR_CHECK_ARG(D > 0 && D <= 512 && F >= 0 && R1 > 0, "bad sizes (need 0 < D <= 512)");
   GR_CHECK_ARG(rix_ptr_t && rix_ptr_h && grad_out && out && grad_table, "null pointer");
   GR_CHECK_ARG(F == 0 || (rel_t && rix_slot_t && row_of_t && rel_h && rix_slot_h && row_of_h), "null edge arrays");
@@ -588,21 +639,37 @@ extern "C" int gr_type_layer_backward_det(const int32_t* rel_t, const float* w_t
     const int32_t* rl = dir ? rel_h : rel_t;
     const int32_t* ro = dir ? row_of_h : row_of_t;
     const float* w = dir ? w_h : w_t;
-#define GR_LAUNCH(NC)                                                                                          \
-  type_bwd_det_kernel<NC><<<grid, kBwdThreads, 0, stream>>>(rp, sl, rl, w, ro, grad_out, ld_grad, out, ld_out, \
-                                                            grad_table, ld_gtable, part, R1, D)
+#define GR_LAUNCH_T(NC, T)                                                                                     \
+  type_bwd_det_kernel<NC, T><<<grid, kBwdThreads, 0, stream>>>(rp, sl, rl, w, ro, static_cast<const T*>(grad_out), \
+                                                               ld_grad, static_cast<const T*>(out), ld_out,         \
+                                                               grad_table, ld_gtable, part, R1, D)
+#define GR_LAUNCH(NC) \
+  if (io_bf16(io)) GR_LAUNCH_T(NC, __nv_bfloat16); else GR_LAUNCH_T(NC, float);
     switch (nc) {
-      case 1: GR_LAUNCH(1); break;
-      case 2: GR_LAUNCH(2); break;
-      case 4: GR_LAUNCH(4); break;
-      case 8: GR_LAUNCH(8); break;
-      default: GR_LAUNCH(16); break;
+      case 1: GR_LAUNCH(1) break;
+      case 2: GR_LAUNCH(2) break;
+      case 4: GR_LAUNCH(4) break;
+      case 8: GR_LAUNCH(8) break;
+      default: GR_LAUNCH(16) break;
     }
 #undef GR_LAUNCH
+#undef GR_LAUNCH_T
     GR_CHECK_LAUNCH();
     segwin_combine_kernel<kRelWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, rp, 0, R1, grad_table,
                                                                                    ld_gtable);
     GR_CHECK_LAUNCH();
   }
   return GR_OK;
+}
+
+extern "C" int gr_type_layer_backward_det(const int32_t* rel_t, const float* w_t, const int32_t* rix_ptr_t,
+                                          const int32_t* rix_slot_t, const int32_t* row_of_t, const int32_t* rel_h,
+                                          const float* w_h, const int32_t* rix_ptr_h, const int32_t* rix_slot_h,
+                                          const int32_t* row_of_h, const float* grad_out, int64_t ld_grad,
+                                          const float* out, int64_t ld_out, float* grad_table, int64_t ld_gtable,
+                                          int64_t R1, int D, int64_t F, void* workspace, size_t workspace_bytes,
+                                          void* stream_) {
+  return gr_type_layer_backward_det_ex(rel_t, w_t, rix_ptr_t, rix_slot_t, row_of_t, rel_h, w_h, rix_ptr_h, rix_slot_h,
+                                       row_of_h, grad_out, ld_grad, out, ld_out, grad_table, ld_gtable, R1, D, F,
+                                       workspace, workspace_bytes, 0u, stream_);
 }

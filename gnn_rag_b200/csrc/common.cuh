@@ -1,5 +1,6 @@
 // Shared helpers for libgnnrag_b200.so (sm_90a).
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -56,6 +57,19 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
 __device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
   return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
+
+// Node-sized training tensors ([B*N, D] outputs and their gradients) are fp32 or, under torch.autocast(bfloat16),
+// bf16 (GR_IO_BF16).  A bf16 load widens exactly and a bf16 store rounds the fp32 value to nearest even; the kernels
+// do the same fp32 operations in between for both types.
+__device__ __forceinline__ float ldg_node(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ldg_node(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+__device__ __forceinline__ float ld_node(const float* p) { return *p; }
+__device__ __forceinline__ float ld_node(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+__device__ __forceinline__ void st_node(float* p, float v) { *p = v; }
+__device__ __forceinline__ void st_node(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+
+// the io flags word of the *_ex entry points: only GR_IO_BF16 is defined
+static inline bool io_bf16(uint32_t io) { return (io & GR_IO_BF16) != 0; }
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ int warp_id() { return threadIdx.x >> 5; }

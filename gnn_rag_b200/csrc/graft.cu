@@ -324,22 +324,24 @@ __global__ void graft_dropout_mask_kernel(const int64_t* __restrict__ seed, floa
 struct TrainArgs {
   // forward: the tail CSR (src = head); backward: the head CSR (src = tail)
   const int32_t *rowptr, *src, *rel, *fact, *slot_of;
-  const float *s, *self_tab, *head_tab;
+  const float *s, *self_tab;
+  const void* head_tab;     // [B*N, D] fp32 or bf16 (the node-sized operands: head_tab, sum_out, grad, grad_head)
   int64_t ld_self, ld_head;
   const int64_t* seed;      // NULL: no dropout
   float p, scale;
-  float* sum_out;           // forward
+  void* sum_out;            // forward
   int64_t ld_sum;
-  const float* grad;        // backward: dL/dsum_out
+  const void* grad;         // backward: dL/dsum_out
   int64_t ld_grad;
-  float *grad_s, *grad_self, *grad_head;
+  float *grad_s, *grad_self;
+  void* grad_head;
   int64_t ld_gself, ld_ghead;
   int64_t Nt;
   int D;
 };
 
 // sum_out[n] = sum_{f -> n} drop_f(relu(self_tab[r_f] + head_tab[head_f])) * s_f, one warp per tail-CSR row, slot order.
-template <int NC>
+template <int NC, typename T>
 __global__ void __launch_bounds__(256) graft_aggregate_train_kernel(const TrainArgs a) {
   const int lane = threadIdx.x & 31;
   const int64_t n = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -358,12 +360,12 @@ __global__ void __launch_bounds__(256) graft_aggregate_train_kernel(const TrainA
     const int h = __ldg(a.src + e), r = __ldg(a.rel + e);
     const int64_t sl = __ldg(a.slot_of + f);
     const float* st = a.self_tab + (int64_t)r * a.ld_self;
-    const float* ht = a.head_tab + (int64_t)h * a.ld_head;
+    const T* ht = static_cast<const T*>(a.head_tab) + (int64_t)h * a.ld_head;
 #pragma unroll
     for (int k = 0; k < NC; ++k) {
       const int c = lane + 32 * k;
       if (c < D) {
-        float v = __fmul_rn(fmaxf(__fadd_rn(__ldg(st + c), __ldg(ht + c)), 0.f), s);
+        float v = __fmul_rn(fmaxf(__fadd_rn(__ldg(st + c), ldg_node(ht + c)), 0.f), s);
         if (drop) v = drop_keep(seed, sl, c, a.p) ? __fmul_rn(v, a.scale) : 0.f;
         acc[k] = __fadd_rn(acc[k], v);
       }
@@ -372,7 +374,7 @@ __global__ void __launch_bounds__(256) graft_aggregate_train_kernel(const TrainA
 #pragma unroll
   for (int k = 0; k < NC; ++k) {
     const int c = lane + 32 * k;
-    if (c < D) a.sum_out[n * a.ld_sum + c] = acc[k];
+    if (c < D) st_node(static_cast<T*>(a.sum_out) + n * a.ld_sum + c, acc[k]);
   }
 }
 
@@ -381,7 +383,7 @@ __global__ void __launch_bounds__(256) graft_aggregate_train_kernel(const TrainA
 //   grad_s[f] += <g_f, relu(a_f)>                 every fact, s_f = 0 included (lane 0, the fact is owned)
 //   grad_head[n] += sum_f g_f s_f [a_f > 0]       registers, one read-modify-write per row (the row is owned)
 //   grad_self[r_f] += g_f s_f [a_f > 0]           fp32 atomics into the R1 relation rows
-template <int NC, bool kSelfAtomics = true>
+template <int NC, bool kSelfAtomics, typename T>
 __global__ void __launch_bounds__(256) graft_aggregate_bwd_kernel(const TrainArgs a) {
   const int lane = threadIdx.x & 31;
   const int64_t n = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -395,7 +397,7 @@ __global__ void __launch_bounds__(256) graft_aggregate_bwd_kernel(const TrainArg
 #pragma unroll
   for (int k = 0; k < NC; ++k) {
     const int c = lane + 32 * k;
-    ht[k] = c < D ? __ldg(a.head_tab + n * a.ld_head + c) : 0.f;
+    ht[k] = c < D ? ldg_node(static_cast<const T*>(a.head_tab) + n * a.ld_head + c) : 0.f;
     gh[k] = 0.f;
   }
   for (int e = beg; e < end; ++e) {
@@ -403,7 +405,7 @@ __global__ void __launch_bounds__(256) graft_aggregate_bwd_kernel(const TrainArg
     const int64_t sl = __ldg(a.slot_of + f);
     const float s = __ldg(a.s + f);
     const float* st = a.self_tab + (int64_t)r * a.ld_self;
-    const float* gt = a.grad + (int64_t)t * a.ld_grad;
+    const T* gt = static_cast<const T*>(a.grad) + (int64_t)t * a.ld_grad;
     float* gs_row = a.grad_self + (int64_t)r * a.ld_gself;
     float gs = 0.f;
 #pragma unroll
@@ -411,7 +413,7 @@ __global__ void __launch_bounds__(256) graft_aggregate_bwd_kernel(const TrainArg
       const int c = lane + 32 * k;
       if (c < D) {
         const float x = __fadd_rn(__ldg(st + c), ht[k]);
-        float g = __ldg(gt + c);
+        float g = ldg_node(gt + c);
         if (drop) g = drop_keep(seed, sl, c, a.p) ? __fmul_rn(g, a.scale) : 0.f;
         gs = fmaf(g, fmaxf(x, 0.f), gs);
         if (s != 0.f && x > 0.f) {          // strict: relu'(0) = 0, as torch
@@ -428,7 +430,10 @@ __global__ void __launch_bounds__(256) graft_aggregate_bwd_kernel(const TrainArg
 #pragma unroll
   for (int k = 0; k < NC; ++k) {
     const int c = lane + 32 * k;
-    if (c < D) a.grad_head[n * a.ld_ghead + c] += gh[k];
+    if (c < D) {
+      T* q = static_cast<T*>(a.grad_head) + n * a.ld_ghead + c;
+      st_node(q, ld_node(q) + gh[k]);
+    }
   }
 }
 
@@ -528,7 +533,7 @@ constexpr int kFactWin = 64;   // relation-index entries per window (grad_self, 
 // grad_self[r] += sum over the staged facts of relation r, in slot order, of  g_f s_f [a_f > 0]  (as the atomics of
 // graft_aggregate_bwd_kernel; g_f = G[tail_f] * mask_f / (1 - p), a_f = self_tab[r] + head_tab[head_f]).
 // Entry i of the relation index -> staged fact f = rix_fact[i].
-template <int NC>
+template <int NC, typename T>
 __global__ void __launch_bounds__(256) graft_self_det_kernel(const TrainArgs a, const int32_t* __restrict__ rix_ptr,
                                                              const int32_t* __restrict__ rix_fact,
                                                              const int32_t* __restrict__ heads,
@@ -571,8 +576,8 @@ __global__ void __launch_bounds__(256) graft_self_det_kernel(const TrainArgs a, 
 #pragma unroll
     for (int k = 0; k < NC; ++k) {
       const int c = lane + 32 * k;
-      if (c < D && __fadd_rn(st[k], __ldg(a.head_tab + h * a.ld_head + c)) > 0.f) {
-        float g = __ldg(a.grad + t * a.ld_grad + c);
+      if (c < D && __fadd_rn(st[k], ldg_node(static_cast<const T*>(a.head_tab) + h * a.ld_head + c)) > 0.f) {
+        float g = ldg_node(static_cast<const T*>(a.grad) + t * a.ld_grad + c);
         if (drop) g = drop_keep(seed, sl, c, a.p) ? __fmul_rn(g, a.scale) : 0.f;
         acc[k] = __fadd_rn(acc[k], __fmul_rn(g, s));
       }
@@ -877,12 +882,13 @@ extern "C" int gr_graft_dropout_mask(const int64_t* seed, double p, int64_t S, i
   return GR_OK;
 }
 
-extern "C" int gr_graft_aggregate_train(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
-                                        const int32_t* fact_t, const int32_t* slot_of, const float* s,
-                                        const float* self_tab, int64_t ld_self, const float* head_tab, int64_t ld_head,
-                                        const int64_t* seed, double p, float* sum_out, int64_t ld_sum, int B, int N,
-                                        int D, void* stream_) {
+extern "C" int gr_graft_aggregate_train_ex(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                                           const int32_t* fact_t, const int32_t* slot_of, const float* s,
+                                           const float* self_tab, int64_t ld_self, const void* head_tab,
+                                           int64_t ld_head, const int64_t* seed, double p, void* sum_out,
+                                           int64_t ld_sum, int B, int N, int D, uint32_t io, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512, "bad sizes (need 0 < D <= 512)");
   GR_CHECK_ARG(rowptr_t && src_t && rel_t && fact_t && slot_of && s && self_tab && head_tab && sum_out,
                "null pointer");
@@ -894,20 +900,33 @@ extern "C" int gr_graft_aggregate_train(const int32_t* rowptr_t, const int32_t* 
   a.sum_out = sum_out; a.ld_sum = ld_sum;
   a.Nt = (int64_t)B * N; a.D = D;
   const int grid = (int)ceil_div(a.Nt, 8);
-#define GR_LAUNCH(NC) graft_aggregate_train_kernel<NC><<<grid, 256, 0, stream>>>(a)
+#define GR_LAUNCH(NC)                                                                 \
+  if (io_bf16(io)) graft_aggregate_train_kernel<NC, __nv_bfloat16><<<grid, 256, 0, stream>>>(a); \
+  else graft_aggregate_train_kernel<NC, float><<<grid, 256, 0, stream>>>(a)
   GR_NC_SWITCH(D, GR_LAUNCH)
 #undef GR_LAUNCH
   GR_CHECK_LAUNCH();
   return GR_OK;
 }
 
-extern "C" int gr_graft_aggregate_backward(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
-                                           const int32_t* fact_h, const int32_t* slot_of, const float* s,
-                                           const float* self_tab, int64_t ld_self, const float* head_tab,
-                                           int64_t ld_head, const int64_t* seed, double p, const float* grad_sum,
-                                           int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
-                                           float* grad_head, int64_t ld_ghead, int B, int N, int D, void* stream_) {
+extern "C" int gr_graft_aggregate_train(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                                        const int32_t* fact_t, const int32_t* slot_of, const float* s,
+                                        const float* self_tab, int64_t ld_self, const float* head_tab, int64_t ld_head,
+                                        const int64_t* seed, double p, float* sum_out, int64_t ld_sum, int B, int N,
+                                        int D, void* stream_) {
+  return gr_graft_aggregate_train_ex(rowptr_t, src_t, rel_t, fact_t, slot_of, s, self_tab, ld_self, head_tab, ld_head,
+                                     seed, p, sum_out, ld_sum, B, N, D, 0u, stream_);
+}
+
+extern "C" int gr_graft_aggregate_backward_ex(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                              const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                              const float* self_tab, int64_t ld_self, const void* head_tab,
+                                              int64_t ld_head, const int64_t* seed, double p, const void* grad_sum,
+                                              int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
+                                              void* grad_head, int64_t ld_ghead, int B, int N, int D, uint32_t io,
+                                              void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512, "bad sizes (need 0 < D <= 512)");
   GR_CHECK_ARG(rowptr_h && src_h && rel_h && fact_h && slot_of && s && self_tab && head_tab && grad_sum && grad_s &&
                    grad_self && grad_head, "null pointer");
@@ -921,11 +940,24 @@ extern "C" int gr_graft_aggregate_backward(const int32_t* rowptr_h, const int32_
   a.grad_s = grad_s; a.grad_self = grad_self; a.grad_head = grad_head; a.ld_gself = ld_gself; a.ld_ghead = ld_ghead;
   a.Nt = (int64_t)B * N; a.D = D;
   const int grid = (int)ceil_div(a.Nt, 8);
-#define GR_LAUNCH(NC) graft_aggregate_bwd_kernel<NC><<<grid, 256, 0, stream>>>(a)
+#define GR_LAUNCH(NC)                                                                    \
+  if (io_bf16(io)) graft_aggregate_bwd_kernel<NC, true, __nv_bfloat16><<<grid, 256, 0, stream>>>(a); \
+  else graft_aggregate_bwd_kernel<NC, true, float><<<grid, 256, 0, stream>>>(a)
   GR_NC_SWITCH(D, GR_LAUNCH)
 #undef GR_LAUNCH
   GR_CHECK_LAUNCH();
   return GR_OK;
+}
+
+extern "C" int gr_graft_aggregate_backward(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                           const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                           const float* self_tab, int64_t ld_self, const float* head_tab,
+                                           int64_t ld_head, const int64_t* seed, double p, const float* grad_sum,
+                                           int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
+                                           float* grad_head, int64_t ld_ghead, int B, int N, int D, void* stream_) {
+  return gr_graft_aggregate_backward_ex(rowptr_h, src_h, rel_h, fact_h, slot_of, s, self_tab, ld_self, head_tab,
+                                        ld_head, seed, p, grad_sum, ld_grad, grad_s, grad_self, ld_gself, grad_head,
+                                        ld_ghead, B, N, D, 0u, stream_);
 }
 
 extern "C" int gr_graft_attention_backward(const float* qh, const float* qmask, int Q, const float* rel, int64_t ldr,
@@ -958,16 +990,19 @@ extern "C" size_t gr_graft_aggregate_backward_det_workspace_bytes(int64_t F, int
   return segwin_part_bytes(F, D, kFactWin);
 }
 
-extern "C" int gr_graft_aggregate_backward_det(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
-                                               const int32_t* fact_h, const int32_t* slot_of, const float* s,
-                                               const float* self_tab, int64_t ld_self, const float* head_tab,
-                                               int64_t ld_head, const int64_t* seed, double p, const float* grad_sum,
-                                               int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
-                                               float* grad_head, int64_t ld_ghead, int B, int N, int D,
-                                               const int32_t* heads, const int32_t* rels, const int32_t* tails,
-                                               const int32_t* rix_ptr, const int32_t* rix_fact, int64_t R1, int64_t F,
-                                               void* workspace, size_t workspace_bytes, void* stream_) {
+extern "C" int gr_graft_aggregate_backward_det_ex(const int32_t* rowptr_h, const int32_t* src_h,
+                                                  const int32_t* rel_h, const int32_t* fact_h, const int32_t* slot_of,
+                                                  const float* s, const float* self_tab, int64_t ld_self,
+                                                  const void* head_tab, int64_t ld_head, const int64_t* seed, double p,
+                                                  const void* grad_sum, int64_t ld_grad, float* grad_s,
+                                                  float* grad_self, int64_t ld_gself, void* grad_head,
+                                                  int64_t ld_ghead, int B, int N, int D, const int32_t* heads,
+                                                  const int32_t* rels, const int32_t* tails, const int32_t* rix_ptr,
+                                                  const int32_t* rix_fact, int64_t R1, int64_t F, void* workspace,
+                                                  size_t workspace_bytes, uint32_t io, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
+  const bool bf = io_bf16(io);
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512 && R1 > 0 && F >= 0, "bad sizes (need 0 < D <= 512)");
   GR_CHECK_ARG(rowptr_h && src_h && rel_h && fact_h && slot_of && s && self_tab && head_tab && grad_sum && grad_s &&
                    grad_self && grad_head && heads && rels && tails && rix_ptr && rix_fact, "null pointer");
@@ -986,15 +1021,19 @@ extern "C" int gr_graft_aggregate_backward_det(const int32_t* rowptr_h, const in
   a.grad_s = grad_s; a.grad_self = grad_self; a.grad_head = grad_head; a.ld_gself = ld_gself; a.ld_ghead = ld_ghead;
   a.Nt = (int64_t)B * N; a.D = D;
   const int grid = (int)ceil_div(a.Nt, 8);
-#define GR_LAUNCH(NC) graft_aggregate_bwd_kernel<NC, false><<<grid, 256, 0, stream>>>(a)
+#define GR_LAUNCH(NC)                                                                        \
+  if (bf) graft_aggregate_bwd_kernel<NC, false, __nv_bfloat16><<<grid, 256, 0, stream>>>(a); \
+  else graft_aggregate_bwd_kernel<NC, false, float><<<grid, 256, 0, stream>>>(a)
   GR_NC_SWITCH(D, GR_LAUNCH)
 #undef GR_LAUNCH
   GR_CHECK_LAUNCH();
   if (F == 0) return GR_OK;
   float* part = reinterpret_cast<float*>(workspace);
   const int grid_w = (int)ceil_div(ceil_div(F, kFactWin), 8);
-#define GR_LAUNCH(NC) \
-  graft_self_det_kernel<NC><<<grid_w, 256, 0, stream>>>(a, rix_ptr, rix_fact, heads, rels, tails, part, R1)
+#define GR_LAUNCH(NC)                                                                                          \
+  if (bf) graft_self_det_kernel<NC, __nv_bfloat16><<<grid_w, 256, 0, stream>>>(a, rix_ptr, rix_fact, heads, rels, \
+                                                                               tails, part, R1);                \
+  else graft_self_det_kernel<NC, float><<<grid_w, 256, 0, stream>>>(a, rix_ptr, rix_fact, heads, rels, tails, part, R1)
   GR_NC_SWITCH(D, GR_LAUNCH)
 #undef GR_LAUNCH
   GR_CHECK_LAUNCH();
@@ -1002,6 +1041,21 @@ extern "C" int gr_graft_aggregate_backward_det(const int32_t* rowptr_h, const in
                                                                                   ld_gself);
   GR_CHECK_LAUNCH();
   return GR_OK;
+}
+
+extern "C" int gr_graft_aggregate_backward_det(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                               const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                               const float* self_tab, int64_t ld_self, const float* head_tab,
+                                               int64_t ld_head, const int64_t* seed, double p, const float* grad_sum,
+                                               int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
+                                               float* grad_head, int64_t ld_ghead, int B, int N, int D,
+                                               const int32_t* heads, const int32_t* rels, const int32_t* tails,
+                                               const int32_t* rix_ptr, const int32_t* rix_fact, int64_t R1, int64_t F,
+                                               void* workspace, size_t workspace_bytes, void* stream_) {
+  return gr_graft_aggregate_backward_det_ex(rowptr_h, src_h, rel_h, fact_h, slot_of, s, self_tab, ld_self, head_tab,
+                                            ld_head, seed, p, grad_sum, ld_grad, grad_s, grad_self, ld_gself,
+                                            grad_head, ld_ghead, B, N, D, heads, rels, tails, rix_ptr, rix_fact, R1, F,
+                                            workspace, workspace_bytes, 0u, stream_);
 }
 
 namespace {

@@ -26,6 +26,13 @@ from .modules import (AttnEncoder, BERTInstruction, Fusion, GraftLayer, LSTMInst
 VERY_SMALL_NUMBER = 1e-10
 
 
+def _no_autocast():
+    """Inference runs the project's fp32 kernels whatever torch.autocast says around it: an enabled autocast would
+    otherwise hand bf16 / fp16 activations from the torch-side GEMMs to kernels that take fp32, and the results must
+    not depend on it."""
+    return torch.autocast("cuda", enabled=False)
+
+
 class BaseModel(nn.Module):
     def __init__(self, args, num_entity, num_relation, num_word):
         super().__init__()
@@ -245,7 +252,7 @@ class ReaRev(BaseModel):
         :class:`batching.DeviceBatch`.  ``training=True``: differentiable torch path (autograd_path.py)."""
         if training:
             return autograd_path.rearev_forward(self, batch)
-        with torch.no_grad():
+        with torch.no_grad(), _no_autocast():
             return self._forward_infer(batch)
 
     def _forward_infer(self, batch):
@@ -323,7 +330,7 @@ class NSM(BaseModel):
         """nsm.py:179-254 (forward reasoning only).  ``training=True``: differentiable torch path."""
         if training:
             return autograd_path.nsm_forward(self, batch)
-        with torch.no_grad():
+        with torch.no_grad(), _no_autocast():
             return self._forward_infer(batch)
 
     def _forward_infer(self, batch):
@@ -391,7 +398,7 @@ class GraftNet(BaseModel):
         """graftnet.py:135-183 -> (loss, pred, pred_dist, tp_list)."""
         if training:
             return autograd_path.graftnet_forward(self, batch)
-        with torch.no_grad():
+        with torch.no_grad(), _no_autocast():
             return self._forward_infer(batch)
 
     def _init_h(self, db, rel):                                    # graftnet.py:74-83

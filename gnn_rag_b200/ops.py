@@ -107,6 +107,30 @@ def pad4(n):
     return (n + 3) & ~3
 
 
+IO_BF16 = 1     # GR_IO_BF16: the node-sized tensors of a training entry point are bf16 (include/gnnrag_b200.h)
+
+
+def _node_io(**tensors):
+    """io flags of the training entry points for their node-sized tensors (name -> tensor, None skipped): 0 when they
+    are torch.float32, IO_BF16 when they are torch.bfloat16 (training under torch.autocast).  Any other dtype, or a
+    mix of the two, is refused."""
+    ts = {k: _cuda(v, name=k) for k, v in tensors.items() if v is not None}
+    for k, t in ts.items():
+        if t.dtype not in (torch.float32, torch.bfloat16):
+            raise RuntimeError("%s must be torch.float32 or torch.bfloat16, got %s" % (k, t.dtype))
+    if len({t.dtype for t in ts.values()}) > 1:
+        raise RuntimeError("%s must share one dtype, got %s" % (", ".join(ts), ", ".join(str(t.dtype) for t in ts.values())))
+    return IO_BF16 if any(t.dtype == torch.bfloat16 for t in ts.values()) else 0
+
+
+def _call_io(L, name, io, *args):
+    """C entry point ``name`` (fp32 node-sized tensors) or, with io flags, its ``*_ex`` variant, which takes the flags
+    word before the stream (the last argument)."""
+    if not io:
+        return getattr(L, name)(*args)
+    return getattr(L, name + "_ex")(*args[:-1], io, args[-1])
+
+
 def set_option(name, value):
     _lib.check(_L().gr_set_option(name.encode(), int(value)))
 
@@ -255,9 +279,10 @@ def e2e_linear(A, W, bias, out):
 
 
 def aggregate(g, direction, prior, table, ins, out=None, out_col0=0, seg_stride=None, w=None,
-              possible=None):
+              possible=None, dtype=torch.float32):
     """One direction of the relation-typed aggregation.  direction: 'fwd' (tail CSR) | 'inv' (head CSR).
-    prior [B,N]; table [R1,D]; ins [B,I,D]; out [B*N, >= out_col0 + I*seg_stride] row-major view."""
+    prior [B,N]; table [R1,D]; ins [B,I,D]; out [B*N, >= out_col0 + I*seg_stride] row-major view, fp32 or bf16
+    (``dtype`` when ``out`` is None): bf16 holds the fp32 result rounded to nearest even."""
     prior = _cuda(prior, torch.float32, "prior").contiguous()
     table = _cuda(table, torch.float32, "table").contiguous()
     ins = _cuda(ins, torch.float32, "ins").contiguous()
@@ -266,16 +291,16 @@ def aggregate(g, direction, prior, table, ins, out=None, out_col0=0, seg_stride=
     if seg_stride is None:
         seg_stride = D
     if out is None:
-        out = torch.empty(B * N, I * seg_stride + out_col0, dtype=torch.float32, device=prior.device)
+        out = torch.empty(B * N, I * seg_stride + out_col0, dtype=dtype, device=prior.device)
+    io = _node_io(out=out)
     assert out.stride(1) == 1
     if direction == "fwd":
         rp, src, rel = g.rowptr_t, g.src_t, g.rel_t
     else:
         rp, src, rel = g.rowptr_h, g.src_h, g.rel_h
     with _AggTimer(("single", I)):
-        rc = _L().gr_aggregate(_p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table), _p(ins), _p(out),
-                               out.stride(0), out_col0, seg_stride, _p(possible), B, N, D, I, g.F,
-                               _stream())
+        rc = _call_io(_L(), "gr_aggregate", io, _p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table), _p(ins),
+                      _p(out), out.stride(0), out_col0, seg_stride, _p(possible), B, N, D, I, g.F, _stream())
     _lib.check(rc)
     STATS.launches += (I + 3) // 4
     return out
@@ -284,12 +309,12 @@ def aggregate(g, direction, prior, table, ins, out=None, out_col0=0, seg_stride=
 def aggregate_backward(g, direction, prior, table, ins, grad_out, grad_table, grad_ins, grad_prior, w=None,
                        deterministic=False):
     """Accumulate the gradients of :func:`aggregate` (same ``direction`` / CSR) into grad_table [R1,D], grad_ins
-    [B,I,D], grad_prior [B,N]; grad_out [B*N, I*D] contiguous rows (csrc/aggregate_bwd.cu).  ``deterministic``:
-    the fixed-order kernels (gr_aggregate_backward_det) instead of the fp32 atomics."""
+    [B,I,D], grad_prior [B,N]; grad_out [B*N, I*D] contiguous rows, fp32 or bf16 (csrc/aggregate_bwd.cu).
+    ``deterministic``: the fixed-order kernels (gr_aggregate_backward_det) instead of the fp32 atomics."""
     prior = _cuda(prior, torch.float32, "prior").contiguous()
     table = _cuda(table, torch.float32, "table").contiguous()
     ins = _cuda(ins, torch.float32, "ins").contiguous()
-    grad_out = _cuda(grad_out, torch.float32, "grad_out")
+    io = _node_io(grad_out=grad_out)
     B, I, D = ins.shape
     assert grad_out.stride(1) == 1 and grad_table.is_contiguous() and grad_ins.is_contiguous() and grad_prior.is_contiguous()
     rp, src, rel = (g.rowptr_t, g.src_t, g.rel_t) if direction == "fwd" else (g.rowptr_h, g.src_h, g.rel_h)
@@ -301,17 +326,17 @@ def aggregate_backward(g, direction, prior, table, ins, grad_out, grad_table, gr
         nbytes = L.gr_aggregate_backward_det_workspace_bytes(B, g.N, D, I, g.F)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=prior.device)
         with _OpTimer("aggregation_bwd_det"):
-            rc = L.gr_aggregate_backward_det(_p(rp), _p(src), _p(rel), _p(fact), _p(w), _p(prior), _p(table), _p(ins),
-                                             _p(grad_out), grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins),
-                                             _p(grad_prior), B, g.N, D, I, g.F, _p(rp_o), _p(fact_o), _p(rix_ptr),
-                                             _p(rix_slot), _p(row_of), g.R1, _p(ws), nbytes, _stream())
+            rc = _call_io(L, "gr_aggregate_backward_det", io, _p(rp), _p(src), _p(rel), _p(fact), _p(w), _p(prior),
+                          _p(table), _p(ins), _p(grad_out), grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins),
+                          _p(grad_prior), B, g.N, D, I, g.F, _p(rp_o), _p(fact_o), _p(rix_ptr), _p(rix_slot),
+                          _p(row_of), g.R1, _p(ws), nbytes, _stream())
         _lib.check(rc)
         STATS.launches += 5 if g.F > 0 else 0
         return
     with _OpTimer("aggregation_bwd"):
-        rc = _L().gr_aggregate_backward(_p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table), _p(ins), _p(grad_out),
-                                        grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins), _p(grad_prior),
-                                        B, g.N, D, I, g.F, _stream())
+        rc = _call_io(_L(), "gr_aggregate_backward", io, _p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table),
+                      _p(ins), _p(grad_out), grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins), _p(grad_prior),
+                      B, g.N, D, I, g.F, _stream())
     _lib.check(rc)
     STATS.launches += 1
 
@@ -443,16 +468,16 @@ def fused_layer(g, prior, pn_fwd, pn_inv, ins, h_planes, seg_pitch, W, bias, out
 
 def type_layer(g, table, out, w_t=None, w_h=None, planes=None):
     """out[:, :D] = relu(sum_tail w*table[rel] + sum_head w*table[rel]) (layer_init.py:46-57); optional
-    split-bf16 planes of the same values."""
+    split-bf16 planes of the same values.  ``out``: fp32, or bf16 (the fp32 values rounded to nearest even)."""
     table = _cuda(table, torch.float32, "table").contiguous()
     D = table.shape[1]
+    io = _node_io(out=out)
     assert out is None or out.stride(1) == 1
     hi, lo = planes if planes is not None else (None, None)
     with _OpTimer("type_layer"):
-        rc = _L().gr_type_layer(_p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.rel_h), _p(w_h),
-                                _p(table), _p(out), out.stride(0) if out is not None else 0,
-                                _p(hi), _p(lo), hi.stride(0) if hi is not None else 0,
-                                g.B, g.N, D, g.F, _stream())
+        rc = _call_io(_L(), "gr_type_layer", io, _p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.rel_h),
+                      _p(w_h), _p(table), _p(out), out.stride(0) if out is not None else 0,
+                      _p(hi), _p(lo), hi.stride(0) if hi is not None else 0, g.B, g.N, D, g.F, _stream())
     _lib.check(rc)
     STATS.launches += 1
     return out
@@ -1090,23 +1115,25 @@ def graft_dropout_mask(seed, p, S, D):
 def graft_aggregate_train(gg, s, self_tab, head_tab, seed=None, p=0.0, sum_out=None):
     """Training forward of the fact messages (gr_graft_aggregate_train): sum_out [B*N, D] with
     sum_out[n] = sum_{f -> n} drop_f(relu(self_tab[r_f] + head_tab[head_f])) * s_f.  ``s``: fp32 per staged fact;
-    ``seed``: device int64 [1] (read when p > 0)."""
+    ``seed``: device int64 [1] (read when p > 0).  head_tab and sum_out: both fp32 or both bf16 (sum_out, when not
+    given, takes head_tab's dtype; bf16 holds the fp32 sums rounded to nearest even)."""
     g = gg.graph
     self_tab = _cuda(self_tab, torch.float32, "self_tab")
-    head_tab = _cuda(head_tab, torch.float32, "head_tab")
+    head_tab = _cuda(head_tab, name="head_tab")
     s = _cuda(s, torch.float32, "s").contiguous()
     D = self_tab.shape[1]
     assert self_tab.stride(1) == 1 and head_tab.stride(1) == 1 and head_tab.shape[0] == gg.B * gg.N
     seed, p = _seed_p(seed, p)
     if sum_out is None:
-        sum_out = torch.empty(gg.B * gg.N, D, dtype=torch.float32, device=self_tab.device)
+        sum_out = torch.empty(gg.B * gg.N, D, dtype=head_tab.dtype, device=self_tab.device)
+    io = _node_io(head_tab=head_tab, sum_out=sum_out)
     assert sum_out.stride(1) == 1
     if s.numel() == 0:               # no staged facts (every question's subgraph empty): every row sums nothing
         return sum_out.zero_()
     with _AggTimer(("graft_train", 1)):
-        rc = _L().gr_graft_aggregate_train(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(gg.slot_of),
-                                           _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab), head_tab.stride(0),
-                                           _p(seed), p, _p(sum_out), sum_out.stride(0), gg.B, gg.N, D, _stream())
+        rc = _call_io(_L(), "gr_graft_aggregate_train", io, _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t),
+                      _p(gg.slot_of), _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab), head_tab.stride(0),
+                      _p(seed), p, _p(sum_out), sum_out.stride(0), gg.B, gg.N, D, _stream())
     _lib.check(rc)
     STATS.launches += 1
     return sum_out
@@ -1116,11 +1143,11 @@ def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_s
                              deterministic=False):
     """Accumulate the gradients of :func:`graft_aggregate_train` (same s, tables, seed and p) into grad_s [F],
     grad_self [R1, D] and grad_head [B*N, D] (gr_graft_aggregate_backward, over the head CSR).  ``deterministic``:
-    grad_self in relation order instead of fp32 atomics (gr_graft_aggregate_backward_det)."""
+    grad_self in relation order instead of fp32 atomics (gr_graft_aggregate_backward_det).  head_tab, grad_sum and
+    grad_head: all fp32 or all bf16 (grad_head is read, added to and stored rounded to nearest even)."""
     g = gg.graph
     self_tab = _cuda(self_tab, torch.float32, "self_tab")
-    head_tab = _cuda(head_tab, torch.float32, "head_tab")
-    grad_sum = _cuda(grad_sum, torch.float32, "grad_sum")
+    io = _node_io(head_tab=head_tab, grad_sum=grad_sum, grad_head=grad_head)
     s = _cuda(s, torch.float32, "s").contiguous()
     D = self_tab.shape[1]
     assert all(t.stride(1) == 1 for t in (self_tab, head_tab, grad_sum, grad_self, grad_head))
@@ -1135,9 +1162,9 @@ def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_s
         nbytes = L.gr_graft_aggregate_backward_det_workspace_bytes(gg.cap, D)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=s.device)
         with _OpTimer("aggregation_bwd_det"):
-            rc = L.gr_graft_aggregate_backward_det(
-                _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h), _p(gg.slot_of), _p(s), _p(self_tab),
-                self_tab.stride(0), _p(head_tab), head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0),
+            rc = _call_io(
+                L, "gr_graft_aggregate_backward_det", io, _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h),
+                _p(gg.slot_of), _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab), head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0),
                 _p(grad_s), _p(grad_self), grad_self.stride(0), _p(grad_head), grad_head.stride(0), gg.B, gg.N, D,
                 _p(gg.heads), _p(gg.rels), _p(gg.tails), _p(rix_ptr), _p(rix_fact), R1, gg.cap, _p(ws), nbytes,
                 _stream())
@@ -1145,11 +1172,10 @@ def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_s
         STATS.launches += 3
         return
     with _OpTimer("aggregation_bwd"):
-        rc = _L().gr_graft_aggregate_backward(_p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h), _p(gg.slot_of),
-                                              _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab),
-                                              head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0),
-                                              _p(grad_s), _p(grad_self), grad_self.stride(0), _p(grad_head),
-                                              grad_head.stride(0), gg.B, gg.N, D, _stream())
+        rc = _call_io(_L(), "gr_graft_aggregate_backward", io, _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h),
+                      _p(g.fact_h), _p(gg.slot_of), _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab),
+                      head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0), _p(grad_s), _p(grad_self),
+                      grad_self.stride(0), _p(grad_head), grad_head.stride(0), gg.B, gg.N, D, _stream())
     _lib.check(rc)
     STATS.launches += 1
 
@@ -1189,11 +1215,10 @@ def graft_attention_backward(gg, qh, qmask, rel, grad_W, grad_qh, grad_rel, dete
 
 
 def type_layer_backward(g, grad_out, out, grad_table, w_t=None, w_h=None, deterministic=False):
-    """Accumulate dL/dtable [R1, D] of :func:`type_layer` given grad_out and the forward's fp32 ``out`` [B*N, D]
-    (gr_type_layer_backward).  ``deterministic``: relation-ordered sums instead of fp32 atomics
+    """Accumulate dL/dtable [R1, D] of :func:`type_layer` given grad_out and the forward's ``out`` [B*N, D], both fp32
+    or both bf16 (gr_type_layer_backward).  ``deterministic``: relation-ordered sums instead of fp32 atomics
     (gr_type_layer_backward_det)."""
-    grad_out = _cuda(grad_out, torch.float32, "grad_out")
-    out = _cuda(out, torch.float32, "out")
+    io = _node_io(grad_out=grad_out, out=out)
     assert grad_out.stride(1) == 1 and out.stride(1) == 1 and grad_table.stride(1) == 1
     D = out.shape[1]
     if deterministic:
@@ -1204,16 +1229,16 @@ def type_layer_backward(g, grad_out, out, grad_table, w_t=None, w_h=None, determ
         nbytes = L.gr_type_layer_backward_det_workspace_bytes(g.F, D)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
         with _OpTimer("type_layer_bwd_det"):
-            rc = L.gr_type_layer_backward_det(_p(g.rel_t), _p(w_t), _p(ptr_t), _p(slot_t), _p(row_t), _p(g.rel_h),
-                                              _p(w_h), _p(ptr_h), _p(slot_h), _p(row_h), _p(grad_out),
-                                              grad_out.stride(0), _p(out), out.stride(0), _p(grad_table),
-                                              grad_table.stride(0), g.R1, D, g.F, _p(ws), nbytes, _stream())
+            rc = _call_io(L, "gr_type_layer_backward_det", io, _p(g.rel_t), _p(w_t), _p(ptr_t), _p(slot_t), _p(row_t),
+                          _p(g.rel_h), _p(w_h), _p(ptr_h), _p(slot_h), _p(row_h), _p(grad_out), grad_out.stride(0),
+                          _p(out), out.stride(0), _p(grad_table), grad_table.stride(0), g.R1, D, g.F, _p(ws), nbytes,
+                          _stream())
         _lib.check(rc)
         STATS.launches += 4 if g.F > 0 else 0
         return
     with _OpTimer("type_layer_bwd"):
-        rc = _L().gr_type_layer_backward(_p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.rel_h), _p(w_h),
-                                         _p(grad_out), grad_out.stride(0), _p(out), out.stride(0), _p(grad_table),
-                                         grad_table.stride(0), g.B, g.N, D, g.F, _stream())
+        rc = _call_io(_L(), "gr_type_layer_backward", io, _p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h),
+                      _p(g.rel_h), _p(w_h), _p(grad_out), grad_out.stride(0), _p(out), out.stride(0), _p(grad_table),
+                      grad_table.stride(0), g.B, g.N, D, g.F, _stream())
     _lib.check(rc)
     STATS.launches += 1

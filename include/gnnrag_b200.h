@@ -412,6 +412,74 @@ int gr_graft_attention_backward_det(const float* qh, const float* qmask, int Q, 
                                     size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Mixed-precision training (torch.autocast(bfloat16)): *_ex variants of the training entry points with an io flags
+ * word before the stream.  io = 0 is the entry point without the suffix.  io = GR_IO_BF16 makes the node-sized
+ * tensors ([B*N, D] rows) bf16; their pointers are then __nv_bfloat16 data with strides still counted in elements:
+ *   gr_aggregate_ex                  out
+ *   gr_aggregate_backward(_det)_ex   grad_out
+ *   gr_type_layer_ex                 out (the split-bf16 planes are unchanged)
+ *   gr_type_layer_backward(_det)_ex  grad_out and out (the forward's output, read for the relu mask)
+ *   gr_graft_aggregate_train_ex      head_tab, sum_out
+ *   gr_graft_aggregate_backward(_det)_ex  head_tab, grad_sum, grad_head (read, added to, stored: owned rows)
+ * Everything else keeps its fp32 type: relation tables, ins, priors, s, weights, every gradient accumulator and the
+ * workspaces, whose sizes (*_workspace_bytes) do not depend on io.
+ * Rounding contract: a bf16 load is widened to fp32 (exact), the kernel then does the fp32 kernel's operations in the
+ * same order, and a bf16 store is the round-to-nearest-even of the value the fp32 kernel would store.  So the forward
+ * and the deterministic backward in bf16 mode equal the fp32 call on the upcast inputs followed by a conversion to
+ * bf16, bit for bit; the atomic backward differs from it only by its summation order.  Shape limits are those of the
+ * fp32 entry points.  Other io bits are refused. */
+#define GR_IO_BF16 1u
+int gr_aggregate_ex(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const float* w, const float* prior,
+                    const float* table, const float* ins, void* out, int64_t out_row_stride, int64_t out_col0,
+                    int64_t seg_stride, float* possible, int B, int N, int D, int I, int64_t F, uint32_t io,
+                    void* stream);
+int gr_aggregate_backward_ex(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const float* w,
+                             const float* prior, const float* table, const float* ins, const void* grad_out,
+                             int64_t grad_row_stride, int64_t grad_col0, int64_t seg_stride, float* grad_table,
+                             float* grad_ins, float* grad_prior, int B, int N, int D, int I, int64_t F, uint32_t io,
+                             void* stream);
+int gr_aggregate_backward_det_ex(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const int32_t* fact,
+                                 const float* w, const float* prior, const float* table, const float* ins,
+                                 const void* grad_out, int64_t grad_row_stride, int64_t grad_col0, int64_t seg_stride,
+                                 float* grad_table, float* grad_ins, float* grad_prior, int B, int N, int D, int I,
+                                 int64_t F, const int32_t* rowptr_o, const int32_t* fact_o, const int32_t* rix_ptr,
+                                 const int32_t* rix_slot, const int32_t* row_of, int64_t R1, void* workspace,
+                                 size_t workspace_bytes, uint32_t io, void* stream);
+int gr_type_layer_ex(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t, const int32_t* rowptr_h,
+                     const int32_t* rel_h, const float* w_h, const float* table, void* out, int64_t out_row_stride,
+                     void* out_hi, void* out_lo, int64_t ld_planes, int B, int N, int D, int64_t F, uint32_t io,
+                     void* stream);
+int gr_type_layer_backward_ex(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                              const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h, const void* grad_out,
+                              int64_t ld_grad, const void* out, int64_t ld_out, float* grad_table, int64_t ld_gtable,
+                              int B, int N, int D, int64_t F, uint32_t io, void* stream);
+int gr_type_layer_backward_det_ex(const int32_t* rel_t, const float* w_t, const int32_t* rix_ptr_t,
+                                  const int32_t* rix_slot_t, const int32_t* row_of_t, const int32_t* rel_h,
+                                  const float* w_h, const int32_t* rix_ptr_h, const int32_t* rix_slot_h,
+                                  const int32_t* row_of_h, const void* grad_out, int64_t ld_grad, const void* out,
+                                  int64_t ld_out, float* grad_table, int64_t ld_gtable, int64_t R1, int D, int64_t F,
+                                  void* workspace, size_t workspace_bytes, uint32_t io, void* stream);
+int gr_graft_aggregate_train_ex(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                                const int32_t* fact_t, const int32_t* slot_of, const float* s, const float* self_tab,
+                                int64_t ld_self, const void* head_tab, int64_t ld_head, const int64_t* seed, double p,
+                                void* sum_out, int64_t ld_sum, int B, int N, int D, uint32_t io, void* stream);
+int gr_graft_aggregate_backward_ex(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                   const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                   const float* self_tab, int64_t ld_self, const void* head_tab, int64_t ld_head,
+                                   const int64_t* seed, double p, const void* grad_sum, int64_t ld_grad,
+                                   float* grad_s, float* grad_self, int64_t ld_gself, void* grad_head,
+                                   int64_t ld_ghead, int B, int N, int D, uint32_t io, void* stream);
+int gr_graft_aggregate_backward_det_ex(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                       const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                       const float* self_tab, int64_t ld_self, const void* head_tab, int64_t ld_head,
+                                       const int64_t* seed, double p, const void* grad_sum, int64_t ld_grad,
+                                       float* grad_s, float* grad_self, int64_t ld_gself, void* grad_head,
+                                       int64_t ld_ghead, int B, int N, int D, const int32_t* heads,
+                                       const int32_t* rels, const int32_t* tails, const int32_t* rix_ptr,
+                                       const int32_t* rix_fact, int64_t R1, int64_t F, void* workspace,
+                                       size_t workspace_bytes, uint32_t io, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Sparse-prior fast path for one ReaRev layer (the first layer of every iteration sees the seed distribution,
  * rearev.py:208).  Rows none of whose in-edges carries prior mass get exactly zero neighbour messages, so
  * h_new = relu(W[:, :D] h + b) there (gr_linear_tc_planes with K = one segment).  gr_frontier_rows lists the

@@ -379,6 +379,13 @@ extern "C" int gr_query_reform(const float* seed_info, const float* h, int64_t l
   p.B = B; p.N = N; p.D = D; p.I = I;
   const size_t smem = ((size_t)1 + 5 * (size_t)I) * D * sizeof(float);
   GR_CHECK_ARG(smem <= 48 * 1024, "num_ins x entity_dim too large for shared memory");
+  // the kernel's static seed list (s_list / s_val / s_woff, ~8 KB) comes on top of the dynamic area: without the
+  // opt-in, static + dynamic is capped at 48 KB and every admitted shape with (5I+1)*D > ~10200 fails to launch
+  static bool attr_done[64] = {};
+  if (first_use_on_device(attr_done)) {
+    GR_CHECK_CUDA(cudaFuncSetAttribute(query_reform_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       48 * 1024));
+  }
   const int slices = D >= 128 ? 4 : (D >= 64 ? 2 : 1);
   query_reform_kernel<<<dim3((unsigned)B, (unsigned)slices), kQThreads, smem, stream>>>(p);
   GR_CHECK_LAUNCH();

@@ -2,165 +2,52 @@
 missing the import fails loudly."""
 import ctypes
 import os
+import re
 
 from . import _build
 
-c_i32p = ctypes.c_void_p
-c_f32p = ctypes.c_void_p
-c_void_p = ctypes.c_void_p
-c_int = ctypes.c_int
-c_i64 = ctypes.c_int64
-c_u32 = ctypes.c_uint32
-c_size = ctypes.c_size_t
-c_dbl = ctypes.c_double
+HEADER = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "gnnrag_b200.h")
 
-# name -> (restype, argtypes); mirrors include/gnnrag_b200.h one to one
-SIGNATURES = {
-    "gr_abi_version": (c_int, []),
-    "gr_last_error": (ctypes.c_char_p, []),
-    "gr_set_option": (c_int, [ctypes.c_char_p, c_i64]),
-    "gr_csr_build_workspace_bytes": (c_size, [c_i64, c_i64]),
-    "gr_csr_build": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_i64, c_i64, c_i64,
-                             c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p,
-                             c_i32p, c_i32p, c_void_p, c_size, c_void_p]),
-    "gr_gather_f32": (c_int, [c_f32p, c_i32p, c_f32p, c_i64, c_void_p]),
-    "gr_linear": (c_int, [c_f32p, c_i64, c_f32p, c_i64, c_f32p, c_f32p, c_i64, c_i64, c_f32p, c_i64,
-                          c_i64, c_i64, c_i64, c_u32, c_void_p]),
-    "gr_linear_tc_workspace_bytes": (c_size, [c_i64, c_i64, c_i64]),
-    "gr_linear_tc": (c_int, [c_f32p, c_i64, c_f32p, c_i64, c_f32p, c_f32p, c_i64, c_i64, c_i64, c_i64,
-                             c_u32, c_void_p, c_size, c_void_p]),
-    "gr_aggregate": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_i64,
-                             c_i64, c_i64, c_f32p, c_int, c_int, c_int, c_int, c_i64, c_void_p]),
-    "gr_aggregate_backward": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_i64, c_i64,
-                                      c_i64, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_i64, c_void_p]),
-    "gr_aggregate_dual": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p,
-                                  c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_i64, c_i64, c_i64,
-                                  c_void_p, c_void_p, c_i64,
-                                  c_int, c_int, c_int, c_int, c_i64, c_void_p]),
-    "gr_pad_table256": (c_int, [c_f32p, c_i64, c_i64, c_int, c_f32p, c_void_p]),
-    "gr_aggregate_dual_abs_supported": (c_int, [c_int, c_int, c_i64, c_i64]),
-    "gr_aggregate_dual_abs": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p,
-                                     c_f32p, c_f32p, c_f32p, c_i64, c_f32p, c_void_p, c_void_p, c_i64, c_i64, c_i64,
-                                     c_int, c_int, c_int, c_int, c_i64, c_i32p, c_void_p]),
-    "gr_fused_profile_read": (c_int, [c_void_p, c_int]),
-    "gr_fused_layer_supported": (c_int, [c_i64, c_i64, c_i64, c_int, c_i64]),
-    "gr_fused_layer_workspace_bytes": (c_size, [c_i64, c_i64, c_int, c_i64]),
-    "gr_fused_layer": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p,
-                               c_f32p, c_f32p, c_f32p, c_f32p, c_void_p, c_void_p, c_i64, c_i64, c_f32p,
-                               c_i64, c_f32p, c_f32p, c_i64, c_void_p, c_void_p, c_i64, c_f32p, c_f32p,
-                               c_int, c_int, c_int, c_int, c_i64, c_i64, c_u32, c_void_p, c_size, c_void_p, c_size,
-                               c_void_p]),
-    "gr_fused_ell_bytes": (c_size, [c_int, c_int, c_i64]),
-    "gr_fused_ell_build": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p, c_int, c_int, c_i64,
-                                   c_void_p, c_size, c_void_p]),
-    "gr_debug_store_probe": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_int, c_int, c_int, c_void_p]),
-    "gr_type_layer": (c_int, [c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_i64,
-                              c_void_p, c_void_p, c_i64,
-                              c_int, c_int, c_int, c_i64, c_void_p]),
-    "gr_linear_tc_planes_workspace_bytes": (c_size, [c_i64, c_i64]),
-    "gr_linear_tc_planes": (c_int, [c_void_p, c_void_p, c_i64, c_f32p, c_i64, c_f32p, c_f32p, c_i64,
-                                    c_void_p, c_void_p, c_i64, c_f32p, c_f32p, c_i64, c_i64, c_i64,
-                                    c_i64, c_i64, c_u32, c_void_p, c_size, c_void_p]),
-    "gr_split_bf16": (c_int, [c_f32p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_i64, c_void_p]),
-    "gr_masked_softmax": (c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_int, c_int, c_void_p]),
-    "gr_graft_stage_workspace_bytes": (c_size, [c_i64, c_i64]),
-    "gr_graft_stage": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p,
-                               c_int, c_int, c_i64, c_i64, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p,
-                               c_i32p, c_void_p, c_size, c_void_p]),
-    "gr_graft_attention": (c_int, [c_f32p, c_f32p, c_int, c_f32p, c_i64, c_i64, c_void_p, c_int, c_i64, c_int,
-                                   c_i32p, c_i32p, c_i32p, c_int, c_f32p, c_f32p, c_f32p, c_i32p, c_void_p]),
-    "gr_graft_aggregate": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_i64,
-                                   c_f32p, c_i64, c_f32p, c_dbl, c_f32p, c_i64, c_void_p, c_void_p, c_i64,
-                                   c_i64, c_i64, c_i64, c_f32p, c_f32p, c_int, c_int, c_int, c_void_p]),
-    "gr_graft_dropout_mask": (c_int, [c_void_p, c_dbl, c_i64, c_int, c_void_p, c_void_p]),
-    "gr_graft_aggregate_train": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_f32p, c_i64,
-                                         c_void_p, c_dbl, c_f32p, c_i64, c_int, c_int, c_int, c_void_p]),
-    "gr_graft_aggregate_backward": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_f32p,
-                                            c_i64, c_void_p, c_dbl, c_f32p, c_i64, c_f32p, c_f32p, c_i64, c_f32p, c_i64,
-                                            c_int, c_int, c_int, c_void_p]),
-    "gr_graft_attention_backward": (c_int, [c_f32p, c_f32p, c_int, c_f32p, c_i64, c_i64, c_void_p, c_int, c_i64,
-                                            c_int, c_f32p, c_f32p, c_f32p, c_i64, c_void_p]),
-    "gr_type_layer_backward": (c_int, [c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_f32p, c_i64,
-                                       c_f32p, c_i64, c_int, c_int, c_int, c_i64, c_void_p]),
-    "gr_csr_row_of": (c_int, [c_i32p, c_i64, c_i32p, c_void_p]),
-    "gr_aggregate_backward_det_workspace_bytes": (c_size, [c_int, c_int, c_int, c_int, c_i64]),
-    "gr_aggregate_backward_det": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,
-                                          c_i64, c_i64, c_i64, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int,
-                                          c_i64, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i64, c_void_p, c_size,
-                                          c_void_p]),
-    "gr_type_layer_backward_det_workspace_bytes": (c_size, [c_i64, c_int]),
-    "gr_type_layer_backward_det": (c_int, [c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p,
-                                           c_i32p, c_f32p, c_i64, c_f32p, c_i64, c_f32p, c_i64, c_i64, c_int, c_i64,
-                                           c_void_p, c_size, c_void_p]),
-    "gr_graft_aggregate_backward_det_workspace_bytes": (c_size, [c_i64, c_int]),
-    "gr_graft_aggregate_backward_det": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64,
-                                                c_f32p, c_i64, c_void_p, c_dbl, c_f32p, c_i64, c_f32p, c_f32p, c_i64,
-                                                c_f32p, c_i64, c_int, c_int, c_int, c_i32p, c_i32p, c_i32p, c_i32p,
-                                                c_i32p, c_i64, c_i64, c_void_p, c_size, c_void_p]),
-    "gr_graft_attention_backward_det_workspace_bytes": (c_size, [c_int, c_i64, c_int, c_int]),
-    "gr_graft_attention_backward_det": (c_int, [c_f32p, c_f32p, c_int, c_f32p, c_i64, c_i64, c_void_p, c_int, c_i64,
-                                                c_int, c_f32p, c_f32p, c_f32p, c_i64, c_i32p, c_i32p, c_void_p,
-                                                c_size, c_void_p]),
-    "gr_aggregate_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_void_p, c_i64, c_i64, c_i64,
-                                c_f32p, c_int, c_int, c_int, c_int, c_i64, c_u32, c_void_p]),
-    "gr_aggregate_backward_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_void_p, c_i64,
-                                         c_i64, c_i64, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_i64, c_u32,
-                                         c_void_p]),
-    "gr_aggregate_backward_det_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_f32p, c_f32p, c_void_p,
-                                             c_i64, c_i64, c_i64, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int,
-                                             c_i64, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i64, c_void_p, c_size,
-                                             c_u32, c_void_p]),
-    "gr_type_layer_ex": (c_int, [c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_f32p, c_f32p, c_void_p, c_i64,
-                                 c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_i64, c_u32, c_void_p]),
-    "gr_type_layer_backward_ex": (c_int, [c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_f32p, c_void_p, c_i64, c_void_p,
-                                          c_i64, c_f32p, c_i64, c_int, c_int, c_int, c_i64, c_u32, c_void_p]),
-    "gr_type_layer_backward_det_ex": (c_int, [c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p,
-                                              c_i32p, c_void_p, c_i64, c_void_p, c_i64, c_f32p, c_i64, c_i64, c_int,
-                                              c_i64, c_void_p, c_size, c_u32, c_void_p]),
-    "gr_graft_aggregate_train_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64, c_void_p,
-                                            c_i64, c_void_p, c_dbl, c_void_p, c_i64, c_int, c_int, c_int, c_u32,
-                                            c_void_p]),
-    "gr_graft_aggregate_backward_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64,
-                                               c_void_p, c_i64, c_void_p, c_dbl, c_void_p, c_i64, c_f32p, c_f32p, c_i64,
-                                               c_void_p, c_i64, c_int, c_int, c_int, c_u32, c_void_p]),
-    "gr_graft_aggregate_backward_det_ex": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i64,
-                                                   c_void_p, c_i64, c_void_p, c_dbl, c_void_p, c_i64, c_f32p, c_f32p,
-                                                   c_i64, c_void_p, c_i64, c_int, c_int, c_int, c_i32p, c_i32p,
-                                                   c_i32p, c_i32p, c_i32p, c_i64, c_i64, c_void_p, c_size, c_u32,
-                                                   c_void_p]),
-    "gr_frontier_rows": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_i64, c_i32p, c_i32p, c_void_p]),
-    "gr_frontier_fixup": (c_int, [c_i32p, c_i32p, c_i32p, c_f32p, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p,
-                                  c_f32p, c_f32p, c_f32p, c_void_p, c_void_p, c_i64, c_f32p, c_i64, c_f32p,
-                                  c_f32p, c_void_p, c_void_p, c_i64, c_f32p, c_f32p, c_i32p, c_i32p,
-                                  c_int, c_int, c_int, c_int, c_void_p]),
-    "gr_score_softmax": (c_int, [c_f32p, c_i64, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p,
-                                 c_int, c_int, c_int, c_void_p]),
-    "gr_instructions": (c_int, [c_f32p, c_f32p, c_void_p, c_i64, c_void_p, c_void_p, c_f32p, c_f32p, c_f32p,
-                                c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_int, c_void_p]),
-    "gr_query_reform": (c_int, [c_f32p, c_f32p, c_i64, c_f32p, c_void_p, c_void_p, c_f32p, c_f32p,
-                                c_int, c_int, c_int, c_int, c_void_p]),
-    "gr_kl_loss_pred": (c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_void_p, c_int, c_int, c_void_p]),
-    "gr_lstm_max_hidden": (c_size, []),
-    "gr_lstm_forward": (c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_int, c_int, c_int, c_void_p]),
-    "gr_seed_retrieve": (c_int, [c_f32p, c_f32p, c_i64, c_f32p, c_int, c_int, c_int, c_void_p]),
-    "gr_rank_workspace_bytes": (c_size, [c_int, c_int]),
-    "gr_rank_candidates": (c_int, [c_f32p, c_void_p, c_f32p, c_i64, c_dbl, c_i32p, c_i32p, c_i32p,
-                                   c_int, c_int, c_void_p, c_size, c_void_p]),
-    "gr_paths_workspace_bytes": (c_size, [c_int, c_int, c_int, c_int]),
-    "gr_shortest_path_nodes": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_int,
-                                       c_i32p, c_i32p, c_int, c_void_p, c_i32p, c_int, c_int,
-                                       c_void_p, c_size, c_void_p]),
-    "gr_rule_adj_workspace_bytes": (c_size, [c_i64]),
-    "gr_rule_adj_build": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i64, c_i64,
-                                  c_i32p, c_i32p, c_i32p, c_i32p, c_void_p, c_size, c_void_p]),
-    "gr_rule_level_workspace_bytes": (c_size, [c_i64]),
-    "gr_rule_level_count": (c_int, [c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p, c_int, c_int, c_i32p, c_i32p,
-                                    c_i64, c_i32p, c_void_p, c_i32p, c_i32p, c_void_p, c_size, c_void_p]),
-    "gr_rule_level_emit": (c_int, [c_i32p, c_i32p, c_i32p, c_void_p, c_i64, c_i64, c_i32p, c_i32p, c_i32p,
-                                   c_void_p]),
-    "gr_rule_paths_write": (c_int, [c_void_p, c_void_p, c_i32p, c_i32p, c_void_p, c_void_p, c_int, c_i64, c_i32p,
-                                    c_void_p]),
+# C parameter / return type -> ctypes type; `const char*` binds as c_char_p and every other pointer as c_void_p
+_CTYPES = {
+    "int": ctypes.c_int,
+    "int64_t": ctypes.c_int64,
+    "uint32_t": ctypes.c_uint32,
+    "size_t": ctypes.c_size_t,
+    "double": ctypes.c_double,
 }
+
+
+def _ctype(decl, where):
+    """ctypes type of a declaration such as `const float* table` or `int64_t` (`where` names it in errors)."""
+    if "*" in decl:
+        base, _, rest = decl.partition("*")
+        if " ".join(base.split()) == "const char" and "*" not in rest:
+            return ctypes.c_char_p
+        return ctypes.c_void_p
+    words = decl.split()
+    for typ in (" ".join(words), " ".join(words[:-1])):   # without and with a parameter name
+        if typ in _CTYPES:
+            return _CTYPES[typ]
+    raise ImportError("%s: no ctypes binding for type %r" % (where, " ".join(words)))
+
+
+def parse_signatures(text):
+    """name -> (restype, argtypes) for every `ret gr_name(params);` prototype of a C header."""
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    text = re.sub(r"//[^\n]*", "", text)
+    sigs = {}
+    for m in re.finditer(r"((?:const\s+)?[A-Za-z_]\w*[\s*]+)\b(gr_\w+)\s*\(([^;{}()]*)\)\s*;", text):
+        ret, name, params = m.group(1), m.group(2), m.group(3).strip()
+        params = [] if params in ("", "void") else [p.strip() for p in params.split(",")]
+        sigs[name] = (_ctype(ret, "%s: return type" % name),
+                      [_ctype(p, "%s: parameter %d (%s)" % (name, i, p)) for i, p in enumerate(params)])
+    return sigs
+
+
+# name -> (restype, argtypes) of every entry point, read from include/gnnrag_b200.h
+with open(HEADER) as _f:
+    SIGNATURES = parse_signatures(_f.read())
 
 _lib = None
 

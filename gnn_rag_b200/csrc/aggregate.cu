@@ -587,31 +587,27 @@ int launch_agg(AggParams p, cudaStream_t stream) {
   for (int d = 0; d < p.ndir && tma; ++d)
     tma = (reinterpret_cast<size_t>(p.dir[d].src) % 16) == 0 &&
           (reinterpret_cast<size_t>(p.dir[d].rel) % 16) == 0;
-  if (MODE == MODE_TYPE) {
-#define GR_TYPE_CASE(V, C) if (vec == V && ch == C) return launch_agg2<V, C, 1, MODE_TYPE>(p, false, stream);
-    GR_TYPE_CASE(4, 1) GR_TYPE_CASE(4, 2) GR_TYPE_CASE(2, 1) GR_TYPE_CASE(2, 2) GR_TYPE_CASE(1, 1)
-    GR_TYPE_CASE(1, 2)
-#undef GR_TYPE_CASE
-    return GR_ERR_UNSUPPORTED;
+  // f(int_c<vec>{}, int_c<ch>{}): vec is 4, 2 or 1 and ch 1 or 2
+  auto with_vec_ch = [&](auto f) {
+    auto with_ch = [&](auto v) { return ch == 1 ? f(v, int_c<1>{}) : f(v, int_c<2>{}); };
+    return vec == 4 ? with_ch(int_c<4>{}) : vec == 2 ? with_ch(int_c<2>{}) : with_ch(int_c<1>{});
+  };
+  if constexpr (MODE == MODE_TYPE) {
+    return with_vec_ch([&](auto v, auto c) {
+      return launch_agg2<decltype(v)::value, decltype(c)::value, 1, MODE_TYPE>(p, false, stream);
+    });
+  } else {
+    for (int j0 = 0; j0 < p.I; j0 += 4) {   // instructions in groups of <= 4 (epilogue register budget)
+      p.j0 = j0;
+      const int rc = with_vec_ch([&](auto v, auto c) {
+        return with_ni(std::min(4, p.I - j0), [&](auto ni) {
+          return launch_agg2<decltype(v)::value, decltype(c)::value, decltype(ni)::value, MODE_MSG>(p, tma, stream);
+        });
+      });
+      if (rc != GR_OK) return rc;
+    }
+    return GR_OK;
   }
-  const int I = p.I;
-  for (int j0 = 0; j0 < I; j0 += 4) {   // instructions in groups of <= 4 (epilogue register budget)
-    p.j0 = j0;
-    int ni = std::min(4, I - j0);
-    int rc;
-#define GR_AGG_CASE(V, C, NI_)                                                       \
-  if (vec == V && ch == C && ni == NI_) rc = launch_agg2<V, C, NI_, MODE_MSG>(p, tma, stream); else
-    GR_AGG_CASE(4, 1, 1) GR_AGG_CASE(4, 1, 2) GR_AGG_CASE(4, 1, 3) GR_AGG_CASE(4, 1, 4)
-    GR_AGG_CASE(4, 2, 1) GR_AGG_CASE(4, 2, 2) GR_AGG_CASE(4, 2, 3) GR_AGG_CASE(4, 2, 4)
-    GR_AGG_CASE(2, 1, 1) GR_AGG_CASE(2, 1, 2) GR_AGG_CASE(2, 1, 3) GR_AGG_CASE(2, 1, 4)
-    GR_AGG_CASE(2, 2, 1) GR_AGG_CASE(2, 2, 2) GR_AGG_CASE(2, 2, 3) GR_AGG_CASE(2, 2, 4)
-    GR_AGG_CASE(1, 1, 1) GR_AGG_CASE(1, 1, 2) GR_AGG_CASE(1, 1, 3) GR_AGG_CASE(1, 1, 4)
-    GR_AGG_CASE(1, 2, 1) GR_AGG_CASE(1, 2, 2) GR_AGG_CASE(1, 2, 3) GR_AGG_CASE(1, 2, 4)
-    rc = GR_ERR_UNSUPPORTED;
-#undef GR_AGG_CASE
-    if (rc != GR_OK) return rc;
-  }
-  return GR_OK;
 }
 
 }  // namespace
@@ -667,7 +663,7 @@ extern "C" int gr_aggregate_ex(const int32_t* rowptr, const int32_t* src, const 
                                int64_t out_row_stride, int64_t out_col0, int64_t seg_stride, float* possible, int B,
                                int N, int D, int I, int64_t F, uint32_t io, void* stream_) {
   using namespace gr;
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
+  if (int rc = check_io(__func__, io)) return rc;
   GR_CHECK_ARG(rowptr && prior && table && ins && out, "null pointer");
   GR_CHECK_ARG(F == 0 || (src && rel), "null edge arrays");
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && I > 0, "B, N, D, I must be positive");
@@ -726,7 +722,7 @@ extern "C" int gr_type_layer_ex(const int32_t* rowptr_t, const int32_t* rel_t, c
                                 void* out, int64_t out_row_stride, void* out_hi, void* out_lo, int64_t ld_planes,
                                 int B, int N, int D, int64_t F, uint32_t io, void* stream_) {
   using namespace gr;
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
+  if (int rc = check_io(__func__, io)) return rc;
   GR_CHECK_ARG(rowptr_t && rowptr_h && table, "null pointer");
   GR_CHECK_ARG(out || (out_hi && out_lo), "no output requested");
   GR_CHECK_ARG(F == 0 || (rel_t && rel_h), "null edge arrays");

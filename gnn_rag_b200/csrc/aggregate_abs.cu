@@ -741,21 +741,11 @@ __global__ void pad_table_kernel(const float* __restrict__ table, int64_t ldt, i
 }
 
 
-// cudaFuncSetAttribute once per (kernel, device)
-template <class K>
-int set_smem_once(K kern, size_t smem, bool (&done)[64]) {
-  if (first_use_on_device(done))
-    GR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  return GR_OK;
-}
-
 template <int NI, int KW, int ROWS, int MINB, bool LO>
 int launch_wsg_lo(const PnParams& p, cudaStream_t stream) {
-  auto kern = agg_abs_wsg_kernel<NI, 200, 208, KW, ROWS, MINB, LO>;
+  constexpr auto kern = agg_abs_wsg_kernel<NI, 200, 208, KW, ROWS, MINB, LO>;
   const size_t smem = 2 * sizeof(HBuf<NI, ROWS>);
-  static bool done[64] = {};
-  int rc = set_smem_once(kern, smem, done);
-  if (rc != GR_OK) return rc;
+  if (int rc = opt_in_smem<kern>(__func__, (int)smem)) return rc;
   GR_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), stream));
   const unsigned tiles = (unsigned)ceil_div(p.Nt, ROWS);
   const unsigned pgrid = std::min<unsigned>(tiles, (unsigned)MINB * (unsigned)sm_count());
@@ -772,11 +762,9 @@ int launch_wsg(const PnParams& p, cudaStream_t stream) {
 
 template <int NI, int KW, int RPW>
 int launch_g4(const PnParams& p, cudaStream_t stream) {
-  auto kern = agg_abs_g5_kernel<NI, 200, 208, KW, RPW>;
+  constexpr auto kern = agg_abs_g5_kernel<NI, 200, 208, KW, RPW>;
   const size_t smem = 128 + (size_t)KW * 16 * 200 * 4 + 2 * sizeof(G5Buf<NI, KW * RPW>);
-  static bool done[64] = {};
-  int rc = set_smem_once(kern, smem, done);
-  if (rc != GR_OK) return rc;
+  if (int rc = opt_in_smem<kern>(__func__, (int)smem)) return rc;
   GR_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), stream));
   const unsigned tiles = (unsigned)ceil_div(p.Nt, KW * RPW);
   const unsigned pgrid = std::min<unsigned>(tiles, (unsigned)sm_count());

@@ -319,6 +319,80 @@ extern "C" size_t gr_aggregate_backward_det_workspace_bytes(int B, int N, int D,
   return gr::agg_det_ws((int64_t)B * N, D, I, F).total;
 }
 
+namespace gr {
+namespace {
+
+// gr_aggregate_backward_ex (det == false: fp32 atomics) and gr_aggregate_backward_det_ex (det == true: the fixed-order
+// kernels, which also take the arguments after F); `fn` is the entry point the argument checks report.
+int agg_backward(const char* fn, bool det, const int32_t* rowptr, const int32_t* src, const int32_t* rel,
+                 const int32_t* fact, const float* w, const float* prior, const float* table, const float* ins,
+                 const void* grad_out, int64_t grad_row_stride, int64_t grad_col0, int64_t seg_stride,
+                 float* grad_table, float* grad_ins, float* grad_prior, int B, int N, int D, int I, int64_t F,
+                 const int32_t* rowptr_o, const int32_t* fact_o, const int32_t* rix_ptr, const int32_t* rix_slot,
+                 const int32_t* row_of, int64_t R1, void* workspace, size_t workspace_bytes, uint32_t io,
+                 cudaStream_t stream) {
+  if (int rc = check_io(fn, io)) return rc;
+  GR_CHECK_ARG_AS(fn, rowptr && prior && table && ins && grad_out && grad_table && grad_ins && grad_prior &&
+                          (!det || (rowptr_o && rix_ptr)), "null pointer");
+  GR_CHECK_ARG_AS(fn, F == 0 || (src && rel && (!det || (fact && fact_o && rix_slot && row_of))), "null edge arrays");
+  GR_CHECK_ARG_AS(fn, B > 0 && N > 0 && D > 0 && D <= 32 * kCPL && I > 0 && I <= 4 && (!det || (F >= 0 && R1 > 0)),
+                  "need 0 < D <= 256 and 0 < I <= 4");
+  GR_CHECK_ARG_AS(fn, seg_stride >= D && grad_row_stride >= grad_col0 + (int64_t)(I - 1) * seg_stride + D,
+                  "grad_out row stride / segment stride smaller than the rows it must hold");
+  if (F == 0) return GR_OK;
+  const int64_t Nt = (int64_t)B * N;
+  DetParams d{};
+  BwdParams& p = d.p;
+  p.rowptr = rowptr; p.src = src; p.rel = rel; p.w = w; p.prior = prior; p.table = table; p.ins = ins;
+  p.gout = grad_out; p.ld = grad_row_stride; p.col0 = grad_col0; p.seg = seg_stride;
+  p.gtable = grad_table; p.gins = grad_ins; p.gprior = grad_prior;
+  p.Nt = Nt; p.N = N; p.D = D; p.I = I;
+  if (!det) {
+    const int grid = (int)std::min<int64_t>(ceil_div(p.Nt * 32, kBwdThreads), 16LL * sm_count());
+    with_ni(I, [&](auto ni) {
+      with_node_type(io, [&](auto t) {
+        agg_bwd_kernel<decltype(ni)::value, typename decltype(t)::type><<<grid, kBwdThreads, 0, stream>>>(p);
+      });
+    });
+    GR_CHECK_LAUNCH_AS(fn);
+    return GR_OK;
+  }
+  const AggDetWs ws = agg_det_ws(Nt, D, I, F);
+  if (int rc = check_workspace("gr_aggregate_backward_det", workspace, workspace_bytes, ws.total)) return rc;
+  d.fact = fact; d.rowptr_o = rowptr_o; d.fact_o = fact_o; d.rix_ptr = rix_ptr; d.rix_slot = rix_slot;
+  d.row_of = row_of; d.R1 = R1;
+  d.q = reinterpret_cast<float*>(workspace);
+  d.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws.q_bytes);
+  const int wpb = kBwdThreads / 32;
+  const int grid_rows = (int)ceil_div(ceil_div(Nt, kRowWin), wpb);
+  const int grid_rel = (int)ceil_div(ceil_div(F, kRelWin), wpb);
+  const int64_t width = (int64_t)I * D;
+  with_ni(I, [&](auto ni) {
+    with_node_type(io, [&](auto t) {
+      agg_bwd_det_rows_kernel<decltype(ni)::value, typename decltype(t)::type><<<grid_rows, kBwdThreads, 0, stream>>>(d);
+    });
+  });
+  GR_CHECK_LAUNCH_AS(fn);
+  segwin_combine_kernel<kRowWin><<<(int)ceil_div(B * width, 256), 256, 0, stream>>>(d.part, width, nullptr, N, B,
+                                                                                   grad_ins, width);
+  GR_CHECK_LAUNCH_AS(fn);
+  agg_bwd_det_prior_kernel<<<(int)ceil_div(Nt, 256), 256, 0, stream>>>(rowptr_o, fact_o, d.q, grad_prior, Nt);
+  GR_CHECK_LAUNCH_AS(fn);
+  with_ni(I, [&](auto ni) {
+    with_node_type(io, [&](auto t) {
+      agg_bwd_det_rel_kernel<decltype(ni)::value, typename decltype(t)::type><<<grid_rel, kBwdThreads, 0, stream>>>(d);
+    });
+  });
+  GR_CHECK_LAUNCH_AS(fn);
+  segwin_combine_kernel<kRelWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(d.part, D, rix_ptr, 0, R1,
+                                                                                 grad_table, D);
+  GR_CHECK_LAUNCH_AS(fn);
+  return GR_OK;
+}
+
+}  // namespace
+}  // namespace gr
+
 extern "C" int gr_aggregate_backward_det_ex(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
                                             const int32_t* fact, const float* w, const float* prior,
                                             const float* table, const float* ins, const void* grad_out,
@@ -328,61 +402,10 @@ extern "C" int gr_aggregate_backward_det_ex(const int32_t* rowptr, const int32_t
                                             const int32_t* rix_ptr, const int32_t* rix_slot, const int32_t* row_of,
                                             int64_t R1, void* workspace, size_t workspace_bytes, uint32_t io,
                                             void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
-  const bool bf = io_bf16(io);
-  GR_CHECK_ARG(rowptr && prior && table && ins && grad_out && grad_table && grad_ins && grad_prior && rowptr_o &&
-                   rix_ptr, "null pointer");
-  GR_CHECK_ARG(F == 0 || (src && rel && fact && fact_o && rix_slot && row_of), "null edge arrays");
-  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 32 * kCPL && I > 0 && I <= 4 && F >= 0 && R1 > 0,
-               "need 0 < D <= 256 and 0 < I <= 4");
-  GR_CHECK_ARG(seg_stride >= D && grad_row_stride >= grad_col0 + (int64_t)(I - 1) * seg_stride + D,
-               "grad_out row stride / segment stride smaller than the rows it must hold");
-  if (F == 0) return GR_OK;
-  const int64_t Nt = (int64_t)B * N;
-  const AggDetWs ws = agg_det_ws(Nt, D, I, F);
-  if (!workspace || workspace_bytes < ws.total) {
-    set_error("gr_aggregate_backward_det: workspace too small (%zu < %zu)", workspace_bytes, ws.total);
-    return GR_ERR_WORKSPACE;
-  }
-  DetParams d{};
-  BwdParams& p = d.p;
-  p.rowptr = rowptr; p.src = src; p.rel = rel; p.w = w; p.prior = prior; p.table = table; p.ins = ins;
-  p.gout = grad_out; p.ld = grad_row_stride; p.col0 = grad_col0; p.seg = seg_stride;
-  p.gtable = grad_table; p.gins = grad_ins; p.gprior = grad_prior;
-  p.Nt = Nt; p.N = N; p.D = D; p.I = I;
-  d.fact = fact; d.rowptr_o = rowptr_o; d.fact_o = fact_o; d.rix_ptr = rix_ptr; d.rix_slot = rix_slot;
-  d.row_of = row_of; d.R1 = R1;
-  d.q = reinterpret_cast<float*>(workspace);
-  d.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws.q_bytes);
-  const int wpb = kBwdThreads / 32;
-  const int grid_rows = (int)ceil_div(ceil_div(Nt, kRowWin), wpb);
-  const int grid_rel = (int)ceil_div(ceil_div(F, kRelWin), wpb);
-  const int64_t width = (int64_t)I * D;
-#define GR_DET(NI)                                                                                \
-  if (bf) agg_bwd_det_rows_kernel<NI, __nv_bfloat16><<<grid_rows, kBwdThreads, 0, stream>>>(d);  \
-  else agg_bwd_det_rows_kernel<NI, float><<<grid_rows, kBwdThreads, 0, stream>>>(d);             \
-  GR_CHECK_LAUNCH();                                                                              \
-  segwin_combine_kernel<kRowWin><<<(int)ceil_div(B * width, 256), 256, 0, stream>>>(            \
-      d.part, width, nullptr, N, B, grad_ins, width);                                             \
-  GR_CHECK_LAUNCH();                                                                              \
-  agg_bwd_det_prior_kernel<<<(int)ceil_div(Nt, 256), 256, 0, stream>>>(rowptr_o, fact_o, d.q, grad_prior, Nt); \
-  GR_CHECK_LAUNCH();                                                                              \
-  if (bf) agg_bwd_det_rel_kernel<NI, __nv_bfloat16><<<grid_rel, kBwdThreads, 0, stream>>>(d);    \
-  else agg_bwd_det_rel_kernel<NI, float><<<grid_rel, kBwdThreads, 0, stream>>>(d);               \
-  GR_CHECK_LAUNCH();                                                                              \
-  segwin_combine_kernel<kRelWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(               \
-      d.part, D, rix_ptr, 0, R1, grad_table, D);
-  switch (I) {
-    case 1: { GR_DET(1) } break;
-    case 2: { GR_DET(2) } break;
-    case 3: { GR_DET(3) } break;
-    default: { GR_DET(4) } break;
-  }
-#undef GR_DET
-  GR_CHECK_LAUNCH();
-  return GR_OK;
+  return gr::agg_backward(__func__, true, rowptr, src, rel, fact, w, prior, table, ins, grad_out, grad_row_stride,
+                          grad_col0, seg_stride, grad_table, grad_ins, grad_prior, B, N, D, I, F, rowptr_o, fact_o,
+                          rix_ptr, rix_slot, row_of, R1, workspace, workspace_bytes, io,
+                          reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int gr_aggregate_backward_det(const int32_t* rowptr, const int32_t* src, const int32_t* rel,
@@ -403,33 +426,9 @@ extern "C" int gr_aggregate_backward_ex(const int32_t* rowptr, const int32_t* sr
                                         const void* grad_out, int64_t grad_row_stride, int64_t grad_col0,
                                         int64_t seg_stride, float* grad_table, float* grad_ins, float* grad_prior,
                                         int B, int N, int D, int I, int64_t F, uint32_t io, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
-  GR_CHECK_ARG(rowptr && prior && table && ins && grad_out && grad_table && grad_ins && grad_prior, "null pointer");
-  GR_CHECK_ARG(F == 0 || (src && rel), "null edge arrays");
-  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 32 * kCPL && I > 0 && I <= 4, "need 0 < D <= 256 and 0 < I <= 4");
-  GR_CHECK_ARG(seg_stride >= D && grad_row_stride >= grad_col0 + (int64_t)(I - 1) * seg_stride + D,
-               "grad_out row stride / segment stride smaller than the rows it must hold");
-  if (F == 0) return GR_OK;
-  BwdParams p{};
-  p.rowptr = rowptr; p.src = src; p.rel = rel; p.w = w; p.prior = prior; p.table = table; p.ins = ins;
-  p.gout = grad_out; p.ld = grad_row_stride; p.col0 = grad_col0; p.seg = seg_stride;
-  p.gtable = grad_table; p.gins = grad_ins; p.gprior = grad_prior;
-  p.Nt = (int64_t)B * N; p.N = N; p.D = D; p.I = I;
-  const int grid = (int)std::min<int64_t>(ceil_div(p.Nt * 32, kBwdThreads), 16LL * sm_count());
-#define GR_LAUNCH(NI)                                                                   \
-  if (io_bf16(io)) agg_bwd_kernel<NI, __nv_bfloat16><<<grid, kBwdThreads, 0, stream>>>(p); \
-  else agg_bwd_kernel<NI, float><<<grid, kBwdThreads, 0, stream>>>(p);
-  switch (I) {
-    case 1: GR_LAUNCH(1) break;
-    case 2: GR_LAUNCH(2) break;
-    case 3: GR_LAUNCH(3) break;
-    default: GR_LAUNCH(4) break;
-  }
-#undef GR_LAUNCH
-  GR_CHECK_LAUNCH();
-  return GR_OK;
+  return gr::agg_backward(__func__, false, rowptr, src, rel, nullptr, w, prior, table, ins, grad_out, grad_row_stride,
+                          grad_col0, seg_stride, grad_table, grad_ins, grad_prior, B, N, D, I, F, nullptr, nullptr,
+                          nullptr, nullptr, nullptr, 0, nullptr, 0, io, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int gr_aggregate_backward(const int32_t* rowptr, const int32_t* src, const int32_t* rel, const float* w,
@@ -504,51 +503,6 @@ __global__ void __launch_bounds__(kBwdThreads) type_bwd_kernel(const int32_t* __
 }  // namespace
 }  // namespace gr
 
-extern "C" int gr_type_layer_backward_ex(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
-                                         const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
-                                         const void* grad_out, int64_t ld_grad, const void* out, int64_t ld_out,
-                                         float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F,
-                                         uint32_t io, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
-  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512 && F >= 0, "bad sizes (need 0 < D <= 512)");
-  GR_CHECK_ARG(rowptr_t && rowptr_h && grad_out && out && grad_table, "null pointer");
-  GR_CHECK_ARG(F == 0 || (rel_t && rel_h), "null edge arrays");
-  GR_CHECK_ARG(ld_grad >= D && ld_out >= D && ld_gtable >= D, "leading dimension smaller than D");
-  if (F == 0) return GR_OK;
-  const int64_t Nt = (int64_t)B * N;
-  const int grid = (int)ceil_div(Nt, kBwdThreads / 32);
-  const int nc = D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16;
-#define GR_LAUNCH_T(NC, T)                                                                                       \
-  type_bwd_kernel<NC, T><<<grid, kBwdThreads, 0, stream>>>(rowptr_t, rel_t, w_t, rowptr_h, rel_h, w_h,            \
-                                                           static_cast<const T*>(grad_out), ld_grad,               \
-                                                           static_cast<const T*>(out), ld_out, grad_table,         \
-                                                           ld_gtable, Nt, D)
-#define GR_LAUNCH(NC) \
-  if (io_bf16(io)) GR_LAUNCH_T(NC, __nv_bfloat16); else GR_LAUNCH_T(NC, float);
-  switch (nc) {
-    case 1: GR_LAUNCH(1) break;
-    case 2: GR_LAUNCH(2) break;
-    case 4: GR_LAUNCH(4) break;
-    case 8: GR_LAUNCH(8) break;
-    default: GR_LAUNCH(16) break;
-  }
-#undef GR_LAUNCH
-#undef GR_LAUNCH_T
-  GR_CHECK_LAUNCH();
-  return GR_OK;
-}
-
-extern "C" int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
-                                      const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
-                                      const float* grad_out, int64_t ld_grad, const float* out, int64_t ld_out,
-                                      float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F,
-                                      void* stream_) {
-  return gr_type_layer_backward_ex(rowptr_t, rel_t, w_t, rowptr_h, rel_h, w_h, grad_out, ld_grad, out, ld_out,
-                                   grad_table, ld_gtable, B, N, D, F, 0u, stream_);
-}
-
 // Deterministic variant of gr_type_layer_backward: two fixed-window segmented sums (common.cuh) over the relation
 // indexes of the tail CSR and then of the head CSR.  Entry i -> CSR slot e of relation rel[e], row n = row_of[e]:
 //     grad_table[r] = (grad_table[r] + sum_{tail-CSR slots of r} w_e Gm[n]) + sum_{head-CSR slots of r} w_e Gm[n]
@@ -602,8 +556,84 @@ __global__ void __launch_bounds__(kBwdThreads) type_bwd_det_kernel(const int32_t
   flush();
 }
 
+// one direction (tail / head CSR) of the TypeLayer's edges: the row pointers for the atomic kernel, the relation
+// index (rix_ptr / rix_slot / row_of) for the deterministic one
+struct TypeDir {
+  const int32_t *rowptr, *rel;
+  const float* w;
+  const int32_t *rix_ptr, *rix_slot, *row_of;
+};
+
+// gr_type_layer_backward_ex (det == false: B, N and the row pointers) and gr_type_layer_backward_det_ex (det == true:
+// R1, the relation indexes and the workspace); `fn` is the entry point the argument checks report.
+int type_layer_backward(const char* fn, bool det, const TypeDir& t, const TypeDir& h, const void* grad_out,
+                        int64_t ld_grad, const void* out, int64_t ld_out, float* grad_table, int64_t ld_gtable, int B,
+                        int N, int64_t R1, int D, int64_t F, void* workspace, size_t workspace_bytes, uint32_t io,
+                        cudaStream_t stream) {
+  if (int rc = check_io(fn, io)) return rc;
+  GR_CHECK_ARG_AS(fn, (det ? R1 > 0 : B > 0 && N > 0) && D > 0 && D <= 512 && F >= 0, "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG_AS(fn, (det ? t.rix_ptr && h.rix_ptr : t.rowptr && h.rowptr) && grad_out && out && grad_table,
+                  "null pointer");
+  GR_CHECK_ARG_AS(fn, F == 0 || (t.rel && h.rel && (!det || (t.rix_slot && t.row_of && h.rix_slot && h.row_of))),
+                  "null edge arrays");
+  GR_CHECK_ARG_AS(fn, ld_grad >= D && ld_out >= D && ld_gtable >= D, "leading dimension smaller than D");
+  if (F == 0) return GR_OK;
+  if (!det) {
+    const int64_t Nt = (int64_t)B * N;
+    const int grid = (int)ceil_div(Nt, kBwdThreads / 32);
+    with_nc(D, [&](auto nc) {
+      with_node_type(io, [&](auto tag) {
+        using T = typename decltype(tag)::type;
+        type_bwd_kernel<decltype(nc)::value, T><<<grid, kBwdThreads, 0, stream>>>(
+            t.rowptr, t.rel, t.w, h.rowptr, h.rel, h.w, static_cast<const T*>(grad_out), ld_grad,
+            static_cast<const T*>(out), ld_out, grad_table, ld_gtable, Nt, D);
+      });
+    });
+    GR_CHECK_LAUNCH_AS(fn);
+    return GR_OK;
+  }
+  const size_t need = segwin_part_bytes(F, D, kRelWin);
+  if (int rc = check_workspace("gr_type_layer_backward_det", workspace, workspace_bytes, need)) return rc;
+  float* part = reinterpret_cast<float*>(workspace);
+  const int grid = (int)ceil_div(ceil_div(F, kRelWin), kBwdThreads / 32);
+  for (const TypeDir* dir : {&t, &h}) {
+    with_nc(D, [&](auto nc) {
+      with_node_type(io, [&](auto tag) {
+        using T = typename decltype(tag)::type;
+        type_bwd_det_kernel<decltype(nc)::value, T><<<grid, kBwdThreads, 0, stream>>>(
+            dir->rix_ptr, dir->rix_slot, dir->rel, dir->w, dir->row_of, static_cast<const T*>(grad_out), ld_grad,
+            static_cast<const T*>(out), ld_out, grad_table, ld_gtable, part, R1, D);
+      });
+    });
+    GR_CHECK_LAUNCH_AS(fn);
+    segwin_combine_kernel<kRelWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, dir->rix_ptr, 0, R1,
+                                                                                   grad_table, ld_gtable);
+    GR_CHECK_LAUNCH_AS(fn);
+  }
+  return GR_OK;
+}
+
 }  // namespace
 }  // namespace gr
+
+extern "C" int gr_type_layer_backward_ex(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                                         const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
+                                         const void* grad_out, int64_t ld_grad, const void* out, int64_t ld_out,
+                                         float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F,
+                                         uint32_t io, void* stream_) {
+  return gr::type_layer_backward(__func__, false, {rowptr_t, rel_t, w_t}, {rowptr_h, rel_h, w_h}, grad_out, ld_grad,
+                                 out, ld_out, grad_table, ld_gtable, B, N, 0, D, F, nullptr, 0, io,
+                                 reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gr_type_layer_backward(const int32_t* rowptr_t, const int32_t* rel_t, const float* w_t,
+                                      const int32_t* rowptr_h, const int32_t* rel_h, const float* w_h,
+                                      const float* grad_out, int64_t ld_grad, const float* out, int64_t ld_out,
+                                      float* grad_table, int64_t ld_gtable, int B, int N, int D, int64_t F,
+                                      void* stream_) {
+  return gr_type_layer_backward_ex(rowptr_t, rel_t, w_t, rowptr_h, rel_h, w_h, grad_out, ld_grad, out, ld_out,
+                                   grad_table, ld_gtable, B, N, D, F, 0u, stream_);
+}
 
 extern "C" size_t gr_type_layer_backward_det_workspace_bytes(int64_t F, int D) {
   if (F < 0 || D <= 0) return 0;
@@ -617,49 +647,10 @@ extern "C" int gr_type_layer_backward_det_ex(const int32_t* rel_t, const float* 
                                              const void* out, int64_t ld_out, float* grad_table, int64_t ld_gtable,
                                              int64_t R1, int D, int64_t F, void* workspace, size_t workspace_bytes,
                                              uint32_t io, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
-  GR_CHECK_ARG(D > 0 && D <= 512 && F >= 0 && R1 > 0, "bad sizes (need 0 < D <= 512)");
-  GR_CHECK_ARG(rix_ptr_t && rix_ptr_h && grad_out && out && grad_table, "null pointer");
-  GR_CHECK_ARG(F == 0 || (rel_t && rix_slot_t && row_of_t && rel_h && rix_slot_h && row_of_h), "null edge arrays");
-  GR_CHECK_ARG(ld_grad >= D && ld_out >= D && ld_gtable >= D, "leading dimension smaller than D");
-  if (F == 0) return GR_OK;
-  const size_t need = segwin_part_bytes(F, D, kRelWin);
-  if (!workspace || workspace_bytes < need) {
-    set_error("gr_type_layer_backward_det: workspace too small (%zu < %zu)", workspace_bytes, need);
-    return GR_ERR_WORKSPACE;
-  }
-  float* part = reinterpret_cast<float*>(workspace);
-  const int grid = (int)ceil_div(ceil_div(F, kRelWin), kBwdThreads / 32);
-  const int nc = D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16;
-  for (int dir = 0; dir < 2; ++dir) {
-    const int32_t* rp = dir ? rix_ptr_h : rix_ptr_t;
-    const int32_t* sl = dir ? rix_slot_h : rix_slot_t;
-    const int32_t* rl = dir ? rel_h : rel_t;
-    const int32_t* ro = dir ? row_of_h : row_of_t;
-    const float* w = dir ? w_h : w_t;
-#define GR_LAUNCH_T(NC, T)                                                                                     \
-  type_bwd_det_kernel<NC, T><<<grid, kBwdThreads, 0, stream>>>(rp, sl, rl, w, ro, static_cast<const T*>(grad_out), \
-                                                               ld_grad, static_cast<const T*>(out), ld_out,         \
-                                                               grad_table, ld_gtable, part, R1, D)
-#define GR_LAUNCH(NC) \
-  if (io_bf16(io)) GR_LAUNCH_T(NC, __nv_bfloat16); else GR_LAUNCH_T(NC, float);
-    switch (nc) {
-      case 1: GR_LAUNCH(1) break;
-      case 2: GR_LAUNCH(2) break;
-      case 4: GR_LAUNCH(4) break;
-      case 8: GR_LAUNCH(8) break;
-      default: GR_LAUNCH(16) break;
-    }
-#undef GR_LAUNCH
-#undef GR_LAUNCH_T
-    GR_CHECK_LAUNCH();
-    segwin_combine_kernel<kRelWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, rp, 0, R1, grad_table,
-                                                                                   ld_gtable);
-    GR_CHECK_LAUNCH();
-  }
-  return GR_OK;
+  return gr::type_layer_backward(__func__, true, {nullptr, rel_t, w_t, rix_ptr_t, rix_slot_t, row_of_t},
+                                 {nullptr, rel_h, w_h, rix_ptr_h, rix_slot_h, row_of_h}, grad_out, ld_grad, out, ld_out,
+                                 grad_table, ld_gtable, 0, 0, R1, D, F, workspace, workspace_bytes, io,
+                                 reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int gr_type_layer_backward_det(const int32_t* rel_t, const float* w_t, const int32_t* rix_ptr_t,

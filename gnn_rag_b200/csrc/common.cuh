@@ -6,6 +6,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include "../../include/gnnrag_b200.h"
 
 namespace gr {
@@ -14,24 +16,29 @@ constexpr int kNumSMs = 132;  // H100 SXM
 
 void set_error(const char* fmt, ...);
 
-#define GR_CHECK_ARG(cond, msg)                                                     \
+// The checks report the function they are written in; the _AS forms report `name` instead, so that a launcher
+// shared by several entry points reports the entry point that called it.
+#define GR_CHECK_ARG_AS(name, cond, msg)                                            \
   do {                                                                              \
     if (!(cond)) {                                                                  \
-      gr::set_error("%s: invalid argument: %s", __func__, msg);                     \
+      gr::set_error("%s: invalid argument: %s", name, msg);                         \
       return GR_ERR_INVALID_ARG;                                                    \
     }                                                                               \
   } while (0)
+#define GR_CHECK_ARG(cond, msg) GR_CHECK_ARG_AS(__func__, cond, msg)
 
-#define GR_CHECK_CUDA(expr)                                                         \
+#define GR_CHECK_CUDA_AS(name, expr)                                                \
   do {                                                                              \
     cudaError_t _e = (expr);                                                        \
     if (_e != cudaSuccess) {                                                        \
-      gr::set_error("%s: CUDA error %s at %s:%d", __func__, cudaGetErrorString(_e), \
+      gr::set_error("%s: CUDA error %s at %s:%d", name, cudaGetErrorString(_e),     \
                     __FILE__, __LINE__);                                            \
       return GR_ERR_CUDA;                                                           \
     }                                                                               \
   } while (0)
+#define GR_CHECK_CUDA(expr) GR_CHECK_CUDA_AS(__func__, expr)
 
+#define GR_CHECK_LAUNCH_AS(name) GR_CHECK_CUDA_AS(name, cudaGetLastError())
 #define GR_CHECK_LAUNCH() GR_CHECK_CUDA(cudaGetLastError())
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
@@ -40,14 +47,26 @@ static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; 
 // number of SMs of the current device (132 on H100 SXM); cached
 int sm_count();
 
-// true the first time it is called for (flag array, current device): kernel attributes such as the dynamic
-// shared-memory opt-in are per device, a process may drive several
-inline bool first_use_on_device(bool (&done)[64]) {
+// Raises Kernel's dynamic shared-memory limit to `bytes` once per (Kernel, device): the attribute is per device and a
+// process may drive several.  Keyed on the kernel itself, not its type, so kernels with the same signature keep
+// separate flags.
+template <auto Kernel>
+int opt_in_smem(const char* fn, int bytes) {
+  static bool done[64] = {};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return true;
-  if (done[dev]) return false;
-  done[dev] = true;
-  return true;
+  if (cudaGetDevice(&dev) == cudaSuccess && dev >= 0 && dev < 64) {
+    if (done[dev]) return GR_OK;
+    done[dev] = true;
+  }
+  GR_CHECK_CUDA_AS(fn, cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  return GR_OK;
+}
+
+// GR_ERR_WORKSPACE unless `ws` is non-null and holds `need` bytes
+static inline int check_workspace(const char* fn, const void* ws, size_t have, size_t need) {
+  if (ws && have >= need) return GR_OK;
+  set_error("%s: workspace too small (%zu < %zu)", fn, have, need);
+  return GR_ERR_WORKSPACE;
 }
 
 // element-wise fp32x2 fma / mul, rounded to nearest like the scalar instructions they expand to
@@ -70,6 +89,53 @@ __device__ __forceinline__ void st_node(__nv_bfloat16* p, float v) { *p = __floa
 
 // the io flags word of the *_ex entry points: only GR_IO_BF16 is defined
 static inline bool io_bf16(uint32_t io) { return (io & GR_IO_BF16) != 0; }
+
+static inline int check_io(const char* fn, uint32_t io) {
+  GR_CHECK_ARG_AS(fn, (io & ~GR_IO_BF16) == 0, "unknown io flags");
+  return GR_OK;
+}
+
+// ---- host dispatch: a runtime value selects a template instance.  f receives it as a std::integral_constant (use
+// decltype(x)::value) or, in with_node_type, as a type_tag (use typename decltype(t)::type); the helper returns
+// what f returns.
+template <int V>
+using int_c = std::integral_constant<int, V>;
+template <typename T>
+struct type_tag {
+  using type = T;
+};
+
+// columns per lane of the warp-per-row kernels (column c = lane + 32 k, k < nc): D <= 512
+static inline int nc_for(int D) { return D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16; }
+
+template <typename F>
+auto with_nc(int D, F&& f) {
+  switch (nc_for(D)) {
+    case 1: return f(int_c<1>{});
+    case 2: return f(int_c<2>{});
+    case 4: return f(int_c<4>{});
+    case 8: return f(int_c<8>{});
+    default: return f(int_c<16>{});
+  }
+}
+
+// instructions per launch, 1..4 (anything above 4 takes 4)
+template <typename F>
+auto with_ni(int I, F&& f) {
+  switch (I) {
+    case 1: return f(int_c<1>{});
+    case 2: return f(int_c<2>{});
+    case 3: return f(int_c<3>{});
+    default: return f(int_c<4>{});
+  }
+}
+
+// element type of the node-sized tensors: float, or __nv_bfloat16 under GR_IO_BF16
+template <typename F>
+auto with_node_type(uint32_t io, F&& f) {
+  if (io_bf16(io)) return f(type_tag<__nv_bfloat16>{});
+  return f(type_tag<float>{});
+}
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ int warp_id() { return threadIdx.x >> 5; }

@@ -294,10 +294,7 @@ extern "C" int gr_csr_build(const void* heads, const void* rels, const void* tai
   GR_CHECK_ARG(rowptr_t && rowptr_h && status && workspace, "null output");
   GR_CHECK_ARG(F == 0 || (src_t && rel_t && fact_t && src_h && rel_h && fact_h), "null edge output");
   CsrWs w = carve(workspace, F, Nt);
-  if (workspace_bytes < w.bytes) {
-    set_error("gr_csr_build: workspace too small (%zu < %zu)", workspace_bytes, w.bytes);
-    return GR_ERR_WORKSPACE;
-  }
+  if (int rc = check_workspace(__func__, workspace, workspace_bytes, w.bytes)) return rc;
   int64_t n = Nt + 1;
   int nblocks = (int)ceil_div(n, kScanChunk);
   GR_CHECK_CUDA(cudaMemsetAsync(w.cur_t, 0, sizeof(int32_t) * n, stream));

@@ -270,13 +270,8 @@ extern "C" int gr_frontier_fixup(const int32_t* rowptr_t, const int32_t* src_t, 
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && I > 0 && ldw >= (2 * I + 1) * (int64_t)D, "bad shape");
   const size_t smem = (size_t)kFixRows * (2 * I + 1) * D * sizeof(float);
   GR_CHECK_ARG(smem <= 200 * 1024, "(2I+1)*D too large for the fix-up kernel's shared memory");
-  static bool attr_done[64] = {};
-  if (first_use_on_device(attr_done)) {
-    GR_CHECK_CUDA(cudaFuncSetAttribute(frontier_fixup_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)(200 * 1024)));
-    GR_CHECK_CUDA(cudaFuncSetAttribute(frontier_fixup_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)(200 * 1024)));
-  }
+  if (int rc = opt_in_smem<frontier_fixup_kernel<true>>(__func__, 200 * 1024)) return rc;
+  if (int rc = opt_in_smem<frontier_fixup_kernel<false>>(__func__, 200 * 1024)) return rc;
   FixParams p{};
   p.rp_t = rowptr_t; p.src_t = src_t; p.rel_t = rel_t; p.rp_h = rowptr_h; p.src_h = src_h; p.rel_h = rel_h;
   p.w_t = w_t; p.w_h = w_h; p.prior = prior; p.table_fwd = table_fwd; p.table_inv = table_inv; p.ins = ins;

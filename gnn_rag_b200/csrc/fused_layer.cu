@@ -813,40 +813,11 @@ template <int NI, int NP, int CS>
 int launch_fused(const CUtensorMap& m_h_hi, const CUtensorMap& m_h_lo, const CUtensorMap& m_w_hi,
                  const CUtensorMap& m_w_lo, const CUtensorMap& m_c, const CUtensorMap& m_c_hi,
                  const CUtensorMap& m_c_lo, const FusedPlan& f, const FParams& p, cudaStream_t stream) {
-  static bool attr_done[64] = {};
-  if (first_use_on_device(attr_done)) {
-    GR_CHECK_CUDA(cudaFuncSetAttribute(fused_layer_kernel<NI, NP, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       227 * 1024));
-  }
-  // the setmaxnreg budget of the kernel redistributes exactly kThreads x kLaunchRegs registers
-  static int num_regs = 0;
-  if (num_regs == 0) {
-    cudaFuncAttributes fa{};
-    GR_CHECK_CUDA(cudaFuncGetAttributes(&fa, fused_layer_kernel<NI, NP, CS>));
-    num_regs = fa.numRegs;
-  }
-  if (num_regs != kLaunchRegs) {
-    set_error("gr_fused_layer: kernel was compiled with %d registers per thread, the warp-group budget needs %d",
-              num_regs, kLaunchRegs);
-    return GR_ERR_UNSUPPORTED;
-  }
   const int ngroups = (p.num_tiles + CS - 1) / CS;
   const int nclusters = std::max(1, std::min(ngroups, sm_count() / CS));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(nclusters * CS));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = f.smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CS;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  GR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fused_layer_kernel<NI, NP, CS>, m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c, m_c_hi,
-                                   m_c_lo, p));
-  return GR_OK;
+  return launch_cluster<fused_layer_kernel<NI, NP, CS>>("gr_fused_layer", kLaunchRegs, CS, nclusters * CS, kThreads,
+                                                        f.smem_bytes, stream, m_h_hi, m_h_lo, m_w_hi, m_w_lo, m_c,
+                                                        m_c_hi, m_c_lo, p);
 }
 
 template <int NP>

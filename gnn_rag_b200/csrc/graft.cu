@@ -284,8 +284,6 @@ __global__ void __launch_bounds__(256) graft_aggregate_kernel(const AggArgs a) {
   }
 }
 
-int nc_for(int D) { return D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : 16; }
-
 // ---- training: dropout, aggregation forward / backward, attention backward ----------------------------------------
 
 // Philox4x32-10 (Salmon et al., SC'11) with key = the 64-bit seed and counter = (slot lo, slot hi, column, 0); the
@@ -733,10 +731,7 @@ extern "C" int gr_graft_stage(const int64_t* e2f_b, const int64_t* e2f_f, const 
   GR_CHECK_ARG(F_f2e == 0 || (f2e_b && f2e_e && f2e_f), "null pointer");
   const int64_t S = (int64_t)B * max_fact;
   StageWs w = stage_ws(S);
-  if (workspace_bytes < w.total || !workspace) {
-    set_error("gr_graft_stage: workspace too small (%zu < %zu)", workspace_bytes, w.total);
-    return GR_ERR_WORKSPACE;
-  }
+  if (int rc = check_workspace(__func__, workspace, workspace_bytes, w.total)) return rc;
   char* ws = reinterpret_cast<char*>(workspace);
   int32_t* head_of = reinterpret_cast<int32_t*>(ws);
   int32_t* tail_of = reinterpret_cast<int32_t*>(ws + w.dense_bytes);
@@ -790,13 +785,10 @@ extern "C" int gr_graft_attention(const float* qh, const float* qmask, int Q, co
   if (S > 0) {
     const float div = (float)sqrt((double)D);
     const int grid = (int)ceil_div(S, 8);
-    switch (nc_for(D)) {
-      case 1: graft_w_kernel<1><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
-      case 2: graft_w_kernel<2><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
-      case 4: graft_w_kernel<4><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
-      case 8: graft_w_kernel<8><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
-      default: graft_w_kernel<16><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, W, status); break;
-    }
+    with_nc(D, [&](auto nc) {
+      graft_w_kernel<decltype(nc)::value><<<grid, 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S,
+                                                                     max_fact, D, div, W, status);
+    });
     GR_CHECK_LAUNCH();
     graft_wtilde_kernel<<<B, 256, 0, stream>>>(W, max_fact, Wt);
     GR_CHECK_LAUNCH();
@@ -833,13 +825,7 @@ extern "C" int gr_graft_aggregate(const int32_t* rowptr_t, const int32_t* src_t,
   a.indeg_out = indeg_out; a.prior_next = prior_next;
   a.Nt = (int64_t)B * N; a.N = N; a.D = D;
   const int grid = (int)ceil_div(a.Nt, 8);
-  switch (nc_for(D)) {
-    case 1: graft_aggregate_kernel<1><<<grid, 256, 0, stream>>>(a); break;
-    case 2: graft_aggregate_kernel<2><<<grid, 256, 0, stream>>>(a); break;
-    case 4: graft_aggregate_kernel<4><<<grid, 256, 0, stream>>>(a); break;
-    case 8: graft_aggregate_kernel<8><<<grid, 256, 0, stream>>>(a); break;
-    default: graft_aggregate_kernel<16><<<grid, 256, 0, stream>>>(a); break;
-  }
+  with_nc(D, [&](auto nc) { graft_aggregate_kernel<decltype(nc)::value><<<grid, 256, 0, stream>>>(a); });
   GR_CHECK_LAUNCH();
   return GR_OK;
 }
@@ -847,15 +833,6 @@ extern "C" int gr_graft_aggregate(const int32_t* rowptr_t, const int32_t* src_t,
 // ---- training entry points -----------------------------------------------------------------------------------------
 
 namespace {
-
-#define GR_NC_SWITCH(D, LAUNCH)         \
-  switch (nc_for(D)) {                  \
-    case 1: LAUNCH(1); break;           \
-    case 2: LAUNCH(2); break;           \
-    case 4: LAUNCH(4); break;           \
-    case 8: LAUNCH(8); break;           \
-    default: LAUNCH(16); break;         \
-  }
 
 // dropout arguments shared by the training entry points: p in [0, 1); p > 0 needs the seed, p == 0 ignores it
 int drop_args(const int64_t* seed, double p, TrainArgs& a) {
@@ -888,7 +865,7 @@ extern "C" int gr_graft_aggregate_train_ex(const int32_t* rowptr_t, const int32_
                                            int64_t ld_head, const int64_t* seed, double p, void* sum_out,
                                            int64_t ld_sum, int B, int N, int D, uint32_t io, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
+  if (int rc = check_io(__func__, io)) return rc;
   GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512, "bad sizes (need 0 < D <= 512)");
   GR_CHECK_ARG(rowptr_t && src_t && rel_t && fact_t && slot_of && s && self_tab && head_tab && sum_out,
                "null pointer");
@@ -900,11 +877,11 @@ extern "C" int gr_graft_aggregate_train_ex(const int32_t* rowptr_t, const int32_
   a.sum_out = sum_out; a.ld_sum = ld_sum;
   a.Nt = (int64_t)B * N; a.D = D;
   const int grid = (int)ceil_div(a.Nt, 8);
-#define GR_LAUNCH(NC)                                                                 \
-  if (io_bf16(io)) graft_aggregate_train_kernel<NC, __nv_bfloat16><<<grid, 256, 0, stream>>>(a); \
-  else graft_aggregate_train_kernel<NC, float><<<grid, 256, 0, stream>>>(a)
-  GR_NC_SWITCH(D, GR_LAUNCH)
-#undef GR_LAUNCH
+  with_nc(D, [&](auto nc) {
+    with_node_type(io, [&](auto t) {
+      graft_aggregate_train_kernel<decltype(nc)::value, typename decltype(t)::type><<<grid, 256, 0, stream>>>(a);
+    });
+  });
   GR_CHECK_LAUNCH();
   return GR_OK;
 }
@@ -918,6 +895,73 @@ extern "C" int gr_graft_aggregate_train(const int32_t* rowptr_t, const int32_t* 
                                      seed, p, sum_out, ld_sum, B, N, D, 0u, stream_);
 }
 
+// ---- deterministic training entry points ---------------------------------------------------------------------------
+
+extern "C" size_t gr_graft_aggregate_backward_det_workspace_bytes(int64_t F, int D) {
+  if (F < 0 || D <= 0) return 0;
+  return segwin_part_bytes(F, D, kFactWin);
+}
+
+namespace {
+
+// gr_graft_aggregate_backward_ex (det == false: grad_self by fp32 atomics) and gr_graft_aggregate_backward_det_ex
+// (det == true: fixed-order grad_self, which also takes the arguments after D); `fn` is the entry point the argument
+// checks report.
+int graft_aggregate_backward(const char* fn, bool det, const int32_t* rowptr_h, const int32_t* src_h,
+                             const int32_t* rel_h, const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                             const float* self_tab, int64_t ld_self, const void* head_tab, int64_t ld_head,
+                             const int64_t* seed, double p, const void* grad_sum, int64_t ld_grad, float* grad_s,
+                             float* grad_self, int64_t ld_gself, void* grad_head, int64_t ld_ghead, int B, int N, int D,
+                             const int32_t* heads, const int32_t* rels, const int32_t* tails, const int32_t* rix_ptr,
+                             const int32_t* rix_fact, int64_t R1, int64_t F, void* workspace, size_t workspace_bytes,
+                             uint32_t io, cudaStream_t stream) {
+  if (int rc = check_io(fn, io)) return rc;
+  GR_CHECK_ARG_AS(fn, B > 0 && N > 0 && D > 0 && D <= 512 && (!det || (R1 > 0 && F >= 0)),
+                  "bad sizes (need 0 < D <= 512)");
+  GR_CHECK_ARG_AS(fn, rowptr_h && src_h && rel_h && fact_h && slot_of && s && self_tab && head_tab && grad_sum &&
+                          grad_s && grad_self && grad_head && (!det || (heads && rels && tails && rix_ptr && rix_fact)),
+                  "null pointer");
+  GR_CHECK_ARG_AS(fn, ld_self >= D && ld_head >= D && ld_grad >= D && ld_gself >= D && ld_ghead >= D,
+                  "leading dimension smaller than D");
+  TrainArgs a{};
+  if (int rc = drop_args(seed, p, a)) return rc;
+  const size_t need = det ? segwin_part_bytes(F, D, kFactWin) : 0;
+  if (det) {
+    if (int rc = check_workspace("gr_graft_aggregate_backward_det", workspace, workspace_bytes, need)) return rc;
+  }
+  a.rowptr = rowptr_h; a.src = src_h; a.rel = rel_h; a.fact = fact_h; a.slot_of = slot_of;
+  a.s = s; a.self_tab = self_tab; a.head_tab = head_tab; a.ld_self = ld_self; a.ld_head = ld_head;
+  a.grad = grad_sum; a.ld_grad = ld_grad;
+  a.grad_s = grad_s; a.grad_self = grad_self; a.grad_head = grad_head; a.ld_gself = ld_gself; a.ld_ghead = ld_ghead;
+  a.Nt = (int64_t)B * N; a.D = D;
+  const int grid = (int)ceil_div(a.Nt, 8);
+  with_nc(D, [&](auto nc) {
+    with_node_type(io, [&](auto t) {
+      constexpr int NC = decltype(nc)::value;
+      using T = typename decltype(t)::type;
+      if (det) graft_aggregate_bwd_kernel<NC, false, T><<<grid, 256, 0, stream>>>(a);
+      else graft_aggregate_bwd_kernel<NC, true, T><<<grid, 256, 0, stream>>>(a);
+    });
+  });
+  GR_CHECK_LAUNCH_AS(fn);
+  if (!det || F == 0) return GR_OK;
+  float* part = reinterpret_cast<float*>(workspace);
+  const int grid_w = (int)ceil_div(ceil_div(F, kFactWin), 8);
+  with_nc(D, [&](auto nc) {
+    with_node_type(io, [&](auto t) {
+      graft_self_det_kernel<decltype(nc)::value, typename decltype(t)::type><<<grid_w, 256, 0, stream>>>(
+          a, rix_ptr, rix_fact, heads, rels, tails, part, R1);
+    });
+  });
+  GR_CHECK_LAUNCH_AS(fn);
+  segwin_combine_kernel<kFactWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, rix_ptr, 0, R1, grad_self,
+                                                                                  ld_gself);
+  GR_CHECK_LAUNCH_AS(fn);
+  return GR_OK;
+}
+
+}  // namespace
+
 extern "C" int gr_graft_aggregate_backward_ex(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
                                               const int32_t* fact_h, const int32_t* slot_of, const float* s,
                                               const float* self_tab, int64_t ld_self, const void* head_tab,
@@ -925,28 +969,10 @@ extern "C" int gr_graft_aggregate_backward_ex(const int32_t* rowptr_h, const int
                                               int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
                                               void* grad_head, int64_t ld_ghead, int B, int N, int D, uint32_t io,
                                               void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
-  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512, "bad sizes (need 0 < D <= 512)");
-  GR_CHECK_ARG(rowptr_h && src_h && rel_h && fact_h && slot_of && s && self_tab && head_tab && grad_sum && grad_s &&
-                   grad_self && grad_head, "null pointer");
-  GR_CHECK_ARG(ld_self >= D && ld_head >= D && ld_grad >= D && ld_gself >= D && ld_ghead >= D,
-               "leading dimension smaller than D");
-  TrainArgs a{};
-  if (int rc = drop_args(seed, p, a)) return rc;
-  a.rowptr = rowptr_h; a.src = src_h; a.rel = rel_h; a.fact = fact_h; a.slot_of = slot_of;
-  a.s = s; a.self_tab = self_tab; a.head_tab = head_tab; a.ld_self = ld_self; a.ld_head = ld_head;
-  a.grad = grad_sum; a.ld_grad = ld_grad;
-  a.grad_s = grad_s; a.grad_self = grad_self; a.grad_head = grad_head; a.ld_gself = ld_gself; a.ld_ghead = ld_ghead;
-  a.Nt = (int64_t)B * N; a.D = D;
-  const int grid = (int)ceil_div(a.Nt, 8);
-#define GR_LAUNCH(NC)                                                                    \
-  if (io_bf16(io)) graft_aggregate_bwd_kernel<NC, true, __nv_bfloat16><<<grid, 256, 0, stream>>>(a); \
-  else graft_aggregate_bwd_kernel<NC, true, float><<<grid, 256, 0, stream>>>(a)
-  GR_NC_SWITCH(D, GR_LAUNCH)
-#undef GR_LAUNCH
-  GR_CHECK_LAUNCH();
-  return GR_OK;
+  return graft_aggregate_backward(__func__, false, rowptr_h, src_h, rel_h, fact_h, slot_of, s, self_tab, ld_self,
+                                  head_tab, ld_head, seed, p, grad_sum, ld_grad, grad_s, grad_self, ld_gself,
+                                  grad_head, ld_ghead, B, N, D, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0,
+                                  nullptr, 0, io, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int gr_graft_aggregate_backward(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
@@ -958,6 +984,37 @@ extern "C" int gr_graft_aggregate_backward(const int32_t* rowptr_h, const int32_
   return gr_graft_aggregate_backward_ex(rowptr_h, src_h, rel_h, fact_h, slot_of, s, self_tab, ld_self, head_tab,
                                         ld_head, seed, p, grad_sum, ld_grad, grad_s, grad_self, ld_gself, grad_head,
                                         ld_ghead, B, N, D, 0u, stream_);
+}
+
+extern "C" int gr_graft_aggregate_backward_det_ex(const int32_t* rowptr_h, const int32_t* src_h,
+                                                  const int32_t* rel_h, const int32_t* fact_h, const int32_t* slot_of,
+                                                  const float* s, const float* self_tab, int64_t ld_self,
+                                                  const void* head_tab, int64_t ld_head, const int64_t* seed, double p,
+                                                  const void* grad_sum, int64_t ld_grad, float* grad_s,
+                                                  float* grad_self, int64_t ld_gself, void* grad_head,
+                                                  int64_t ld_ghead, int B, int N, int D, const int32_t* heads,
+                                                  const int32_t* rels, const int32_t* tails, const int32_t* rix_ptr,
+                                                  const int32_t* rix_fact, int64_t R1, int64_t F, void* workspace,
+                                                  size_t workspace_bytes, uint32_t io, void* stream_) {
+  return graft_aggregate_backward(__func__, true, rowptr_h, src_h, rel_h, fact_h, slot_of, s, self_tab, ld_self,
+                                  head_tab, ld_head, seed, p, grad_sum, ld_grad, grad_s, grad_self, ld_gself,
+                                  grad_head, ld_ghead, B, N, D, heads, rels, tails, rix_ptr, rix_fact, R1, F,
+                                  workspace, workspace_bytes, io, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gr_graft_aggregate_backward_det(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                                               const int32_t* fact_h, const int32_t* slot_of, const float* s,
+                                               const float* self_tab, int64_t ld_self, const float* head_tab,
+                                               int64_t ld_head, const int64_t* seed, double p, const float* grad_sum,
+                                               int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
+                                               float* grad_head, int64_t ld_ghead, int B, int N, int D,
+                                               const int32_t* heads, const int32_t* rels, const int32_t* tails,
+                                               const int32_t* rix_ptr, const int32_t* rix_fact, int64_t R1, int64_t F,
+                                               void* workspace, size_t workspace_bytes, void* stream_) {
+  return gr_graft_aggregate_backward_det_ex(rowptr_h, src_h, rel_h, fact_h, slot_of, s, self_tab, ld_self, head_tab,
+                                            ld_head, seed, p, grad_sum, ld_grad, grad_s, grad_self, ld_gself,
+                                            grad_head, ld_ghead, B, N, D, heads, rels, tails, rix_ptr, rix_fact, R1, F,
+                                            workspace, workspace_bytes, 0u, stream_);
 }
 
 extern "C" int gr_graft_attention_backward(const float* qh, const float* qmask, int Q, const float* rel, int64_t ldr,
@@ -974,88 +1031,13 @@ extern "C" int gr_graft_attention_backward(const float* qh, const float* qmask, 
   const bool smem_acc = acc_bytes <= 48 * 1024;
   const size_t smem = smem_acc ? acc_bytes : 0;
   const dim3 grid((unsigned)ceil_div(max_fact, kSlotsPerBlock), (unsigned)B);
-#define GR_LAUNCH(NC)                                                                                          \
-  graft_w_bwd_kernel<NC><<<grid, 256, smem, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, max_fact, D, div, \
-                                                      grad_W, grad_qh, grad_rel, ld_grel, smem_acc)
-  GR_NC_SWITCH(D, GR_LAUNCH)
-#undef GR_LAUNCH
+  with_nc(D, [&](auto nc) {
+    graft_w_bwd_kernel<decltype(nc)::value><<<grid, 256, smem, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel,
+                                                                          max_fact, D, div, grad_W, grad_qh, grad_rel,
+                                                                          ld_grel, smem_acc);
+  });
   GR_CHECK_LAUNCH();
   return GR_OK;
-}
-
-// ---- deterministic training entry points ---------------------------------------------------------------------------
-
-extern "C" size_t gr_graft_aggregate_backward_det_workspace_bytes(int64_t F, int D) {
-  if (F < 0 || D <= 0) return 0;
-  return segwin_part_bytes(F, D, kFactWin);
-}
-
-extern "C" int gr_graft_aggregate_backward_det_ex(const int32_t* rowptr_h, const int32_t* src_h,
-                                                  const int32_t* rel_h, const int32_t* fact_h, const int32_t* slot_of,
-                                                  const float* s, const float* self_tab, int64_t ld_self,
-                                                  const void* head_tab, int64_t ld_head, const int64_t* seed, double p,
-                                                  const void* grad_sum, int64_t ld_grad, float* grad_s,
-                                                  float* grad_self, int64_t ld_gself, void* grad_head,
-                                                  int64_t ld_ghead, int B, int N, int D, const int32_t* heads,
-                                                  const int32_t* rels, const int32_t* tails, const int32_t* rix_ptr,
-                                                  const int32_t* rix_fact, int64_t R1, int64_t F, void* workspace,
-                                                  size_t workspace_bytes, uint32_t io, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG((io & ~GR_IO_BF16) == 0, "unknown io flags");
-  const bool bf = io_bf16(io);
-  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= 512 && R1 > 0 && F >= 0, "bad sizes (need 0 < D <= 512)");
-  GR_CHECK_ARG(rowptr_h && src_h && rel_h && fact_h && slot_of && s && self_tab && head_tab && grad_sum && grad_s &&
-                   grad_self && grad_head && heads && rels && tails && rix_ptr && rix_fact, "null pointer");
-  GR_CHECK_ARG(ld_self >= D && ld_head >= D && ld_grad >= D && ld_gself >= D && ld_ghead >= D,
-               "leading dimension smaller than D");
-  TrainArgs a{};
-  if (int rc = drop_args(seed, p, a)) return rc;
-  const size_t need = segwin_part_bytes(F, D, kFactWin);
-  if (!workspace || workspace_bytes < need) {
-    set_error("gr_graft_aggregate_backward_det: workspace too small (%zu < %zu)", workspace_bytes, need);
-    return GR_ERR_WORKSPACE;
-  }
-  a.rowptr = rowptr_h; a.src = src_h; a.rel = rel_h; a.fact = fact_h; a.slot_of = slot_of;
-  a.s = s; a.self_tab = self_tab; a.head_tab = head_tab; a.ld_self = ld_self; a.ld_head = ld_head;
-  a.grad = grad_sum; a.ld_grad = ld_grad;
-  a.grad_s = grad_s; a.grad_self = grad_self; a.grad_head = grad_head; a.ld_gself = ld_gself; a.ld_ghead = ld_ghead;
-  a.Nt = (int64_t)B * N; a.D = D;
-  const int grid = (int)ceil_div(a.Nt, 8);
-#define GR_LAUNCH(NC)                                                                        \
-  if (bf) graft_aggregate_bwd_kernel<NC, false, __nv_bfloat16><<<grid, 256, 0, stream>>>(a); \
-  else graft_aggregate_bwd_kernel<NC, false, float><<<grid, 256, 0, stream>>>(a)
-  GR_NC_SWITCH(D, GR_LAUNCH)
-#undef GR_LAUNCH
-  GR_CHECK_LAUNCH();
-  if (F == 0) return GR_OK;
-  float* part = reinterpret_cast<float*>(workspace);
-  const int grid_w = (int)ceil_div(ceil_div(F, kFactWin), 8);
-#define GR_LAUNCH(NC)                                                                                          \
-  if (bf) graft_self_det_kernel<NC, __nv_bfloat16><<<grid_w, 256, 0, stream>>>(a, rix_ptr, rix_fact, heads, rels, \
-                                                                               tails, part, R1);                \
-  else graft_self_det_kernel<NC, float><<<grid_w, 256, 0, stream>>>(a, rix_ptr, rix_fact, heads, rels, tails, part, R1)
-  GR_NC_SWITCH(D, GR_LAUNCH)
-#undef GR_LAUNCH
-  GR_CHECK_LAUNCH();
-  segwin_combine_kernel<kFactWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, rix_ptr, 0, R1, grad_self,
-                                                                                  ld_gself);
-  GR_CHECK_LAUNCH();
-  return GR_OK;
-}
-
-extern "C" int gr_graft_aggregate_backward_det(const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
-                                               const int32_t* fact_h, const int32_t* slot_of, const float* s,
-                                               const float* self_tab, int64_t ld_self, const float* head_tab,
-                                               int64_t ld_head, const int64_t* seed, double p, const float* grad_sum,
-                                               int64_t ld_grad, float* grad_s, float* grad_self, int64_t ld_gself,
-                                               float* grad_head, int64_t ld_ghead, int B, int N, int D,
-                                               const int32_t* heads, const int32_t* rels, const int32_t* tails,
-                                               const int32_t* rix_ptr, const int32_t* rix_fact, int64_t R1, int64_t F,
-                                               void* workspace, size_t workspace_bytes, void* stream_) {
-  return gr_graft_aggregate_backward_det_ex(rowptr_h, src_h, rel_h, fact_h, slot_of, s, self_tab, ld_self, head_tab,
-                                            ld_head, seed, p, grad_sum, ld_grad, grad_s, grad_self, ld_gself,
-                                            grad_head, ld_ghead, B, N, D, heads, rels, tails, rix_ptr, rix_fact, R1, F,
-                                            workspace, workspace_bytes, 0u, stream_);
 }
 
 namespace {
@@ -1090,27 +1072,22 @@ extern "C" int gr_graft_attention_backward_det(const float* qh, const float* qma
   GR_CHECK_ARG(S < 0x7fffffff, "B*max_fact exceeds int32");
   if (S == 0) return GR_OK;
   const AttnDetWs ws = attn_det_ws(S, Q, D);
-  if (!workspace || workspace_bytes < ws.total) {
-    set_error("gr_graft_attention_backward_det: workspace too small (%zu < %zu)", workspace_bytes, ws.total);
-    return GR_ERR_WORKSPACE;
-  }
+  if (int rc = check_workspace(__func__, workspace, workspace_bytes, ws.total)) return rc;
   float* coef = reinterpret_cast<float*>(workspace);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws.coef_bytes);
   const float div = (float)sqrt((double)D);
-#define GR_LAUNCH(NC)                                                                                            \
-  graft_w_coef_kernel<NC><<<(int)ceil_div(S, 8), 256, 0, stream>>>(qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S,   \
-                                                                   max_fact, D, div, grad_W, coef)
-  GR_NC_SWITCH(D, GR_LAUNCH)
-#undef GR_LAUNCH
+  with_nc(D, [&](auto nc) {
+    graft_w_coef_kernel<decltype(nc)::value><<<(int)ceil_div(S, 8), 256, 0, stream>>>(
+        qh, qmask, Q, rel, ldr, R1, kb_fact_rel, S, max_fact, D, div, grad_W, coef);
+  });
   GR_CHECK_LAUNCH();
   graft_qh_det_kernel<<<(int)ceil_div((int64_t)B * Q * D, 256), 256, 0, stream>>>(coef, Q, rel, ldr, R1, kb_fact_rel,
                                                                                   B, max_fact, D, grad_qh);
   GR_CHECK_LAUNCH();
-#define GR_LAUNCH(NC)                                                                                        \
-  graft_rel_det_kernel<NC><<<(int)ceil_div(ceil_div(S, kFactWin), 8), 256, 0, stream>>>(                   \
-      coef, Q, qh, R1, kb_fact_rel, max_fact, D, rix_ptr, rix_slot, grad_rel, ld_grel, part)
-  GR_NC_SWITCH(D, GR_LAUNCH)
-#undef GR_LAUNCH
+  with_nc(D, [&](auto nc) {
+    graft_rel_det_kernel<decltype(nc)::value><<<(int)ceil_div(ceil_div(S, kFactWin), 8), 256, 0, stream>>>(
+        coef, Q, qh, R1, kb_fact_rel, max_fact, D, rix_ptr, rix_slot, grad_rel, ld_grel, part);
+  });
   GR_CHECK_LAUNCH();
   segwin_combine_kernel<kFactWin><<<(int)ceil_div(R1 * D, 256), 256, 0, stream>>>(part, D, rix_ptr, 0, R1, grad_rel,
                                                                                   ld_grel);

@@ -319,40 +319,11 @@ template <int NP, int CS, int BK>
 int launch_tc_cs(const CUtensorMap& m_a_hi, const CUtensorMap& m_a_lo, const CUtensorMap& m_w_hi,
                  const CUtensorMap& m_w_lo, const CUtensorMap& m_c, const CUtensorMap& m_c_hi,
                  const CUtensorMap& m_c_lo, const TcPlan& t, const TcParams& p, cudaStream_t stream) {
-  static bool attr_done[64] = {};
-  if (first_use_on_device(attr_done)) {
-    GR_CHECK_CUDA(cudaFuncSetAttribute(linear_tc_kernel<NP, CS, BK>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-  }
-  // setmaxnreg.inc only draws on registers the CTA was launched with: the budget needs exactly kLaunchRegs
-  static int num_regs = 0;
-  if (num_regs == 0) {
-    cudaFuncAttributes fa{};
-    GR_CHECK_CUDA(cudaFuncGetAttributes(&fa, linear_tc_kernel<NP, CS, BK>));
-    num_regs = fa.numRegs;
-  }
-  if (num_regs != kLaunchRegs) {
-    set_error("gr_linear_tc: kernel was compiled with %d registers per thread, the warpgroup budget needs %d",
-              num_regs, kLaunchRegs);
-    return GR_ERR_UNSUPPORTED;
-  }
   const int ngroups = (p.num_tiles + CS - 1) / CS;
   const int nclusters = std::max(1, std::min(ngroups, sm_count() / CS));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(nclusters * CS));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = t.smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CS;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  GR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, linear_tc_kernel<NP, CS, BK>, m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c, m_c_hi,
-                                   m_c_lo, p));
-  return GR_OK;
+  return launch_cluster<linear_tc_kernel<NP, CS, BK>>("gr_linear_tc", kLaunchRegs, CS, nclusters * CS, kThreads,
+                                                      t.smem_bytes, stream, m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c,
+                                                      m_c_hi, m_c_lo, p);
 }
 
 template <int NP>
@@ -441,10 +412,7 @@ extern "C" int gr_linear_tc(const float* A, int64_t lda, const float* W, int64_t
               (long long)M, (long long)N, (long long)K);
     return GR_ERR_UNSUPPORTED;
   }
-  if (workspace_bytes < t.total_bytes) {
-    set_error("gr_linear_tc: workspace too small (%zu < %zu)", workspace_bytes, t.total_bytes);
-    return GR_ERR_WORKSPACE;
-  }
+  if (int rc = check_workspace(__func__, workspace, workspace_bytes, t.total_bytes)) return rc;
   if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) {
     set_error("gr_linear_tc: workspace must be 256-byte aligned");
     return GR_ERR_INVALID_ARG;

@@ -351,11 +351,7 @@ extern "C" int gr_instructions(const float* hidden, const float* qnode, const in
   p.B = B; p.Q = Q; p.D = D; p.I = I;
   const size_t smem = ((size_t)Q * D + (size_t)(I + 7) * D + 2 * (size_t)Q) * sizeof(float);
   GR_CHECK_ARG(smem <= 200 * 1024, "question length x entity_dim too large for shared memory");
-  static bool attr_done[64] = {};
-  if (first_use_on_device(attr_done)) {
-    GR_CHECK_CUDA(cudaFuncSetAttribute(instructions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       200 * 1024));
-  }
+  if (int rc = opt_in_smem<instructions_kernel>(__func__, 200 * 1024)) return rc;
   instructions_kernel<<<B, kQThreads, smem, stream>>>(p);
   GR_CHECK_LAUNCH();
   return GR_OK;
@@ -381,11 +377,7 @@ extern "C" int gr_query_reform(const float* seed_info, const float* h, int64_t l
   GR_CHECK_ARG(smem <= 48 * 1024, "num_ins x entity_dim too large for shared memory");
   // the kernel's static seed list (s_list / s_val / s_woff, ~8 KB) comes on top of the dynamic area: without the
   // opt-in, static + dynamic is capped at 48 KB and every admitted shape with (5I+1)*D > ~10200 fails to launch
-  static bool attr_done[64] = {};
-  if (first_use_on_device(attr_done)) {
-    GR_CHECK_CUDA(cudaFuncSetAttribute(query_reform_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       48 * 1024));
-  }
+  if (int rc = opt_in_smem<query_reform_kernel>(__func__, 48 * 1024)) return rc;
   const int slices = D >= 128 ? 4 : (D >= 64 ? 2 : 1);
   query_reform_kernel<<<dim3((unsigned)B, (unsigned)slices), kQThreads, smem, stream>>>(p);
   GR_CHECK_LAUNCH();
@@ -525,10 +517,7 @@ extern "C" int gr_lstm_forward(const float* gates_x, const float* W_hh, const fl
   GR_CHECK_ARG(B > 0 && Q > 0 && D > 0 && D <= 256, "bad shape (hidden size <= 256)");
   const int U = (D + kLstmCluster - 1) / kLstmCluster;
   const size_t smem = ((size_t)4 * U * (D | 1) + 8 + (size_t)2 * D * kLstmQB + (size_t)4 * U * kLstmQB) * sizeof(float);
-  static bool attr_done[64] = {};
-  if (first_use_on_device(attr_done)) {
-    GR_CHECK_CUDA(cudaFuncSetAttribute(lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  }
+  if (int rc = opt_in_smem<lstm_kernel>(__func__, 200 * 1024)) return rc;
   GR_CHECK_ARG(smem <= 200 * 1024, "hidden size too large for shared memory");
   const int clusters = (B + kLstmQB - 1) / kLstmQB;
   lstm_kernel<<<clusters * kLstmCluster, kLstmThreads, smem, stream>>>(gates_x, W_hh, b_hh, hidden, B, Q, D);

@@ -330,10 +330,7 @@ extern "C" int gr_rule_adj_build(const int32_t* rowptr_t, const int32_t* src_t, 
   GR_CHECK_ARG(rowptr_t && rowptr_h && adj_rowptr && adj_len, "null pointer");
   GR_CHECK_ARG(F == 0 || (src_t && rel_t && fact_t && src_h && rel_h && fact_h && adj_nbr && adj_lab),
                "null edge array");
-  if (!workspace || workspace_bytes < gr_rule_adj_workspace_bytes(F)) {
-    set_error("gr_rule_adj_build: workspace too small (%zu < %zu)", workspace_bytes, gr_rule_adj_workspace_bytes(F));
-    return GR_ERR_WORKSPACE;
-  }
+  if (int rc = check_workspace(__func__, workspace, workspace_bytes, gr_rule_adj_workspace_bytes(F))) return rc;
   Csr2 g{rowptr_t, src_t, rel_t, fact_t, rowptr_h, src_h, rel_h, fact_h};
   adj_small_kernel<<<(unsigned)ceil_div(Nt, kThreads), kThreads, 0, stream>>>(g, Nt, adj_rowptr, adj_len, adj_nbr,
                                                                              adj_lab);
@@ -364,11 +361,7 @@ extern "C" int gr_rule_level_count(const int32_t* adj_rowptr, const int32_t* adj
   GR_CHECK_ARG(adj_rowptr && adj_len && child_off && res_begin && res_count, "null pointer");
   GR_CHECK_ARG(J == 0 || (job_rule_off && job_rule_len), "null job array");
   GR_CHECK_ARG(n == 0 || (node && job && seg_begin), "null frontier array");
-  if (!workspace || workspace_bytes < gr_rule_level_workspace_bytes(n)) {
-    set_error("gr_rule_level_count: workspace too small (%zu < %zu)", workspace_bytes,
-              gr_rule_level_workspace_bytes(n));
-    return GR_ERR_WORKSPACE;
-  }
+  if (int rc = check_workspace(__func__, workspace, workspace_bytes, gr_rule_level_workspace_bytes(n))) return rc;
   Jobs jobs{job_rule_off, job_rule_len, rule_lab, J};
   count_kernel<<<grid_for(n + 1, kThreads), kThreads, 0, stream>>>(adj_rowptr, adj_len, adj_lab, jobs, level, node,
                                                                    job, n, seg_begin, child_off);

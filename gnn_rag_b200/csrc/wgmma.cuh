@@ -352,5 +352,40 @@ __device__ __forceinline__ void epi_dots(float dot0, float dot1, float* dots, in
   }
 }
 
+// Launches a warp-specialised kernel as `grid` CTAs of `threads` threads in clusters of `cs` along x.  The kernel is
+// opted in to 227 KB of dynamic shared memory once per device, and refused unless it was compiled with exactly
+// `launch_regs` registers per thread: setmaxnreg only redistributes the registers the CTA was launched with, so the
+// warpgroups' budgets add up to exactly threads x launch_regs.  Errors are reported as `fn`.
+template <auto Kernel, typename... Args>
+int launch_cluster(const char* fn, int launch_regs, int cs, int grid, int threads, size_t smem, cudaStream_t stream,
+                   const Args&... args) {
+  if (int rc = opt_in_smem<Kernel>(fn, 227 * 1024)) return rc;
+  static int num_regs = 0;   // one per Kernel
+  if (num_regs == 0) {
+    cudaFuncAttributes fa{};
+    GR_CHECK_CUDA_AS(fn, cudaFuncGetAttributes(&fa, Kernel));
+    num_regs = fa.numRegs;
+  }
+  if (num_regs != launch_regs) {
+    set_error("%s: kernel was compiled with %d registers per thread, the warpgroup budget needs %d", fn, num_regs,
+              launch_regs);
+    return GR_ERR_UNSUPPORTED;
+  }
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3((unsigned)threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cs;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  GR_CHECK_CUDA_AS(fn, cudaLaunchKernelEx(&cfg, Kernel, args...));
+  return GR_OK;
+}
+
 }  // namespace tc
 }  // namespace gr

@@ -12,6 +12,9 @@ device (CUDA when the model lives there -- no CPU fallback is involved) so that 
   * on CUDA with ``USE_KERNELS`` the aggregations, the TypeLayer and GraftNet's fact attention and fact messages run
     in hand-written kernels with their own backward (the ``torch.autograd.Function``s below); the per-fact torch
     restatement is the CPU reference under ``HOST_CHECK`` and the ``USE_KERNELS = False`` path;
+  * on CUDA with ``USE_KERNELS``, at the shapes the forward kernels admit, the instruction steps (ReaRev, NSM) and
+    ReaRev's query reform run in the question-side kernels with their own backward (_InstructionsFn, _QueryReformFn);
+    the instruction dropout is drawn in the kernel from a seed of torch's CUDA generator;
   * under ``torch.use_deterministic_algorithms(True)`` (``warn_only`` included), read by each Function at forward,
     those backward kernels are the fixed-order, atomic-free variants: every gradient they produce is a pure function
     of the inputs.  The torch restatement's ``index_add`` is made deterministic by torch itself under the same flag;
@@ -212,10 +215,131 @@ def _neighbours(table_f, table_i, ins, dist, facts, graph, Nt):
     return torch.stack(reps, dim=1)
 
 
+INS_MAX_SMEM = 200 * 1024      # gr_instructions: (Q D + (I + 7) D + 2 Q) floats of shared memory
+REFORM_MAX_SMEM = 48 * 1024    # gr_query_reform: (5 I + 1) D floats
+
+
+def _instruction_kernels(device, Q, D, I):
+    """True when the instruction steps run in gr_instructions_train / gr_instructions_backward: CUDA, ``USE_KERNELS``
+    and a shape gr_instructions admits."""
+    return bool(USE_KERNELS and device.type == "cuda" and I <= 8 and (Q * D + (I + 7) * D + 2 * Q) * 4 <= INS_MAX_SMEM)
+
+
+def _reform_kernels(device, D, I):
+    """True when the query reform runs in gr_query_reform_ex / gr_query_reform_backward: CUDA, ``USE_KERNELS`` and a
+    shape gr_query_reform admits."""
+    return bool(USE_KERNELS and device.type == "cuda" and I <= 8 and D <= 1024 and (5 * I + 1) * D * 4 <= REFORM_MAX_SMEM)
+
+
+def _weight_grads(G, X):
+    """(G^T X, column sums of G) over the rows of the per-question operands: one GEMM per weight, fp32 outside
+    autocast.  Deterministic under use_deterministic_algorithms (torch's cuBLAS path and reductions)."""
+    with torch.autocast("cuda", enabled=False):
+        G2 = G.reshape(-1, G.shape[-1])
+        return G2.t() @ X.reshape(G2.shape[0], -1), G2.sum(0)
+
+
+class _InstructionsFn(torch.autograd.Function):
+    """All num_ins steps of get_instruction (base_encoder.py:73-114) with the reference's three linear_drop sites:
+    forward = gr_instructions_train, backward = gr_instructions_backward (csrc/question.cu), which redraws the Philox
+    mask from the saved seed.  The kernels write the per-question gradient operands; each weight gradient is one torch
+    GEMM over them.  The question tensors are not node-sized: under autocast everything here is fp32, and each
+    gradient is returned in its input's dtype.  Inputs after the data: wca, bca, Wcq, bcq, then (W_i, b_i) of every
+    question_linear_i."""
+
+    @staticmethod
+    def forward(ctx, hidden, qnode, qtext, pad_id, seed, p, wca, bca, Wcq, bcq, *wq):
+        from . import ops
+        ctx.dtypes = (hidden.dtype, qnode.dtype) + tuple(t.dtype for t in (wca, bca, Wcq, bcq) + wq)
+        hidden, qnode = hidden.detach().float().contiguous(), qnode.detach().float().contiguous()
+        wts = [t.detach().float().contiguous() for t in (wca, bca, Wcq, bcq) + wq]
+        Wq, bq = wts[4::2], wts[5::2]
+        out, attn = ops.instructions_train(hidden, qnode, qtext, pad_id, Wq, bq, wts[2], wts[3], wts[0], wts[1],
+                                           seed, p)
+        ctx.save_for_backward(hidden, qnode, qtext, seed, out, attn, *wts)
+        ctx.pad_id, ctx.p = pad_id, p
+        ctx.det = torch.are_deterministic_algorithms_enabled()
+        ctx.amp = _autocast_bf16()
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from . import ops
+        hidden, qnode, qtext, seed, out, attn, *wts = ctx.saved_tensors
+        wca, bca, Wcq, bcq = wts[:4]
+        Wq, bq = wts[4::2], wts[5::2]
+        gh, gqn, Gq, Xq, Gcq, Xcq, Gca, Xca = ops.instructions_backward(
+            hidden, qnode, qtext, ctx.pad_id, Wq, bq, Wcq, bcq, wca, bca, seed, ctx.p, out, attn, grad_out.float())
+        gwca, gbca = _weight_grads(Gca.unsqueeze(-1), Xca)       # rows (b, i, q)
+        gWcq, gbcq = _weight_grads(Gcq, Xcq)                     # rows (b, i)
+        gq = []
+        for i in range(len(Wq)):
+            gq.extend(_weight_grads(Gq[:, i], Xq[:, i]))          # rows b
+        grads = [gh, gqn, gwca.view(wca.shape), gbca.view(bca.shape), gWcq, gbcq] + gq
+        dts = ctx.dtypes
+        return (grads[0].to(dts[0]), grads[1].to(dts[1]), None, None, None, None,
+                *(g.to(dt) for g, dt in zip(grads[2:], dts[2:])))
+
+
+def _instructions_kernel(enc, hidden, qnode, q_input):
+    """The instruction steps through _InstructionsFn; the dropout seed is one int64 from torch's CUDA generator,
+    drawn on the device (no host sync), when the encoder's linear_drop is active."""
+    drop = enc.linear_drop
+    p = float(drop.p) if drop.training else 0.0
+    seed = torch.randint(0, 2 ** 62, (1,), dtype=torch.int64, device=hidden.device) if p > 0.0 else None
+    lins = [getattr(enc, "question_linear" + str(i)) for i in range(enc.num_ins)]
+    wq = [t for lin in lins for t in (lin.weight, lin.bias)]
+    return _InstructionsFn.apply(hidden, qnode.reshape(qnode.shape[0], -1), q_input, enc.pad_val, seed, p,
+                                 enc.ca_linear.weight, enc.ca_linear.bias, enc.cq_linear.weight, enc.cq_linear.bias,
+                                 *wq)
+
+
+class _QueryReformFn(torch.autograd.Function):
+    """QueryReform + Fusion for every instruction (query_update.py:6-44, rearev.py:214-221): forward =
+    gr_query_reform_ex (one seed retrieve serves all I reforms), backward = gr_query_reform_backward, which adds the
+    seed-row gradient into a zero [B*N, D] grad_h in h's dtype (only the seed rows are written).  h is read in its own
+    dtype (bf16 under bf16 autocast); everything else is fp32.  Inputs after the data: (Wr_j, Wg_j) of every reform."""
+
+    @staticmethod
+    def forward(ctx, seed_info, h, ins, B, N, *wts):
+        from . import ops
+        ctx.dtypes = (h.dtype, ins.dtype) + tuple(t.dtype for t in wts)
+        h = h.detach()
+        if h.dtype not in (torch.float32, torch.bfloat16):
+            h = h.float()
+        ins = ins.detach().float().contiguous()
+        wts = [t.detach().float().contiguous() for t in wts]
+        out = ops.query_reform_train(seed_info, h, ins, wts[0::2], wts[1::2], B, N)
+        ctx.save_for_backward(seed_info, h, ins, *wts)
+        ctx.BN = (B, N)
+        ctx.det = torch.are_deterministic_algorithms_enabled()
+        ctx.amp = _autocast_bf16()
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from . import ops
+        seed_info, h, ins, *wts = ctx.saved_tensors
+        B, N = ctx.BN
+        grad_h = torch.zeros(h.shape, dtype=h.dtype, device=h.device)
+        gins, Gr, Gg, Z = ops.query_reform_backward(seed_info, h, ins, wts[0::2], wts[1::2], B, N, grad_out.float(),
+                                                    grad_h)
+        gw = []
+        for j in range(len(wts) // 2):
+            gw.append(_weight_grads(Gr[:, j], Z[:, j])[0])
+            gw.append(_weight_grads(Gg[:, j], Z[:, j])[0])
+        dts = ctx.dtypes
+        return (None, grad_h.to(dts[0]), gins.to(dts[1]), None, None, *(g.to(dt) for g, dt in zip(gw, dts[2:])))
+
+
 def _instructions(enc, q_input):
-    """base_encoder.py:73-114 on top of encode_question; returns [B, num_ins, D]."""
+    """base_encoder.py:73-114 on top of encode_question; returns [B, num_ins, D].  The steps run in the question-side
+    kernels (_InstructionsFn) on CUDA with ``USE_KERNELS`` at the shapes gr_instructions admits; otherwise as torch ops
+    below."""
     enc.encode_question_train(q_input)
     hidden, qnode, qmask = enc.query_hidden_emb, enc.query_node_emb, enc.query_mask_train
+    if _instruction_kernels(hidden.device, hidden.shape[1], hidden.shape[2], enc.num_ins):
+        return _instructions_kernel(enc, hidden, qnode, q_input)
     drop = enc.linear_drop
     rel_ins = torch.zeros(q_input.size(0), enc.entity_dim, device=q_input.device)
     out = []
@@ -332,6 +456,9 @@ def rearev_forward(model, batch):
     dist_history = [seed_dist]
     dist = seed_dist
     graph = _kernel_graph(model, batch, h.device, D, I, graph)
+    reform_kernels = _reform_kernels(h.device, D, I)
+    fusion_w = [w for j in range(I) for w in (getattr(model, "reform" + str(j)).fusion.r.weight,
+                                               getattr(model, "reform" + str(j)).fusion.g.weight)]
     for _t in range(model.num_iter):
         dist = seed_dist
         ins = torch.stack(ins_list, dim=1)                                  # [B, I, D]
@@ -342,6 +469,10 @@ def rearev_forward(model, batch):
             score = layer.score_func(drop(h)).view(B, N) + (1 - mask) * VERY_NEG_NUMBER
             dist = F.softmax(score, dim=1)
         dist_history.append(dist)
+        if reform_kernels:                                                # one seed retrieve for all I reforms
+            new = _QueryReformFn.apply(query_entities, h, torch.stack(ins_list, dim=1), B, N, *fusion_w)
+            ins_list = [new[:, j] for j in range(I)]
+            continue
         hB = h.view(B, N, D)
         new = []
         for j in range(I):

@@ -137,6 +137,31 @@ auto with_node_type(uint32_t io, F&& f) {
   return f(type_tag<float>{});
 }
 
+// ---- in-kernel dropout ----------------------------------------------------------------------------------------------
+// Philox4x32-10 (Salmon et al., SC'11) with key = the 64-bit seed and counter (c0, c1, c2, c3); returns the first output
+// word.  A kernel's dropout keys each element by its own counter layout (documented at its entry point).
+__device__ __forceinline__ uint32_t philox4x32_10_x0(uint64_t seed, uint32_t c0, uint32_t c1, uint32_t c2,
+                                                     uint32_t c3) {
+  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+    c0 = hi1 ^ c1 ^ k0;
+    c1 = lo1;
+    c2 = hi0 ^ c3 ^ k1;
+    c3 = lo0;
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c0;
+}
+
+// an element survives dropout with probability 1 - p:  u = (x >> 8) * 2^-24 in [0, 1), kept iff u >= p
+__device__ __forceinline__ bool philox_keep(uint32_t x, float p) {
+  return (float)(x >> 8) * 5.9604644775390625e-8f >= p;
+}
+
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ int warp_id() { return threadIdx.x >> 5; }
 

@@ -286,29 +286,11 @@ __global__ void __launch_bounds__(256) graft_aggregate_kernel(const AggArgs a) {
 
 // ---- training: dropout, aggregation forward / backward, attention backward ----------------------------------------
 
-// Philox4x32-10 (Salmon et al., SC'11) with key = the 64-bit seed and counter = (slot lo, slot hi, column, 0); the
-// first output word decides.  Keyed by fact SLOT (b * max_fact + f), so the mask of a fact does not depend on where
-// the loader's permutation put it in the graft lists.
-__device__ __forceinline__ uint32_t philox_x0(uint64_t seed, uint64_t slot, uint32_t col) {
-  uint32_t c0 = (uint32_t)slot, c1 = (uint32_t)(slot >> 32), c2 = col, c3 = 0u;
-  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
-#pragma unroll
-  for (int i = 0; i < 10; ++i) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-    c0 = hi1 ^ c1 ^ k0;
-    c1 = lo1;
-    c2 = hi0 ^ c3 ^ k1;
-    c3 = lo0;
-    k0 += 0x9E3779B9u;
-    k1 += 0xBB67AE85u;
-  }
-  return c0;
-}
-
-// element (slot, col) survives dropout with probability 1 - p:  u = (x >> 8) * 2^-24 in [0, 1), keep iff u >= p
+// Philox4x32-10 (common.cuh) with counter = (slot lo, slot hi, column, 0).  Keyed by fact SLOT (b * max_fact + f), so
+// the mask of a fact does not depend on where the loader's permutation put it in the graft lists.
 __device__ __forceinline__ bool drop_keep(uint64_t seed, int64_t slot, int col, float p) {
-  return (float)(philox_x0(seed, (uint64_t)slot, (uint32_t)col) >> 8) * 5.9604644775390625e-8f >= p;
+  return philox_keep(philox4x32_10_x0(seed, (uint32_t)(uint64_t)slot, (uint32_t)((uint64_t)slot >> 32), (uint32_t)col, 0u),
+                     p);
 }
 
 __global__ void graft_dropout_mask_kernel(const int64_t* __restrict__ seed, float p, int64_t S, int D,

@@ -12,6 +12,8 @@
 //                     (gnn/models/base_model.py:186-215, gnn/models/ReaRev/rearev.py:156-160,228-232)
 #include <math.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace gr {
@@ -85,12 +87,30 @@ struct InsParams {
   float* out;               // [B, I, D]
   float* attn_out;          // optional [B, I, Q]
   int B, Q, D, I;
+  const int64_t* seed;      // training dropout (kDrop): device int64[1]
+  float p, scale;           // drop probability and 1 / (1 - p)
 };
 
+// The three linear_drop sites of get_instruction (base_encoder.py:85-98) at step i: 0 = qnode before
+// question_linear_i (column c < D), 1 = [ri, q_i, q_i - ri, q_i * ri] before cq_linear (c < 4D), 2 = cq * hidden[q]
+// before ca_linear (token q, c < D).  Counter = (question, 4 * step + site, token (0 for sites 0 / 1), column).
+enum { kSiteQnode = 0, kSiteCq = 1, kSiteCa = 2 };
+
+__device__ __forceinline__ bool ins_keep(uint64_t seed, float p, int b, int i, int site, int q, int c) {
+  return philox_keep(philox4x32_10_x0(seed, (uint32_t)b, (uint32_t)(4 * i + site), (uint32_t)q, (uint32_t)c), p);
+}
+
+// v dropped at one site: v * scale if kept, else 0
+__device__ __forceinline__ float ins_drop(float v, bool keep, float scale) { return keep ? __fmul_rn(v, scale) : 0.f; }
+
+// kDrop = false: gr_instructions (eval) and gr_instructions_train with p = 0.  kDrop = true: the three dropout sites;
+// q_i is then formed per step from that step's dropped qnode (same GEMV rows, same dot order).
+template <bool kDrop>
 __global__ void __launch_bounds__(kQThreads) instructions_kernel(const InsParams p) {
   extern __shared__ __align__(16) float smq[];
   const int D = p.D, Q = p.Q, I = p.I, b = blockIdx.x, tid = threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
+  const uint64_t seed = kDrop ? (uint64_t)__ldg(p.seed) : 0;
   float* s_hid = smq;                    // [Q][D]
   float* s_qn = s_hid + (size_t)Q * D;   // [D]
   float* s_qi = s_qn + D;                // [I][D]
@@ -106,20 +126,33 @@ __global__ void __launch_bounds__(kQThreads) instructions_kernel(const InsParams
   }
   for (int q = tid; q < Q; q += blockDim.x) s_mask[q] = p.qtext[(int64_t)b * Q + q] != p.pad ? 1.f : 0.f;
   __syncthreads();
-  {
+  if constexpr (!kDrop) {
     GemvGroup grp[kMaxIns];                               // q_i = question_linear_i(qnode) for every i at once
     for (int i = 0; i < I; ++i) grp[i] = GemvGroup{p.Wq[i], p.bq[i], s_qn, s_qi + (size_t)i * D};
     block_gemv(grp, I, D, D, D);
+    __syncthreads();
   }
-  __syncthreads();
   for (int i = 0; i < I; ++i) {
     const float* qi = s_qi + (size_t)i * D;
+    if constexpr (kDrop) {                                // q_i = question_linear_i(drop(qnode)), s_z as scratch
+      for (int d = tid; d < D; d += blockDim.x)
+        s_z[d] = ins_drop(s_qn[d], ins_keep(seed, p.p, b, i, kSiteQnode, 0, d), p.scale);
+      __syncthreads();
+      GemvGroup grp[1] = {GemvGroup{p.Wq[i], p.bq[i], s_z, s_qi + (size_t)i * D}};
+      block_gemv(grp, 1, D, D, D);
+      __syncthreads();
+    }
     for (int d = tid; d < D; d += blockDim.x) {           // cat(ri, q_i, q_i - ri, q_i * ri)
       const float r = s_ri[d], q = qi[d];
-      s_z[d] = r;
-      s_z[D + d] = q;
-      s_z[2 * D + d] = q - r;
-      s_z[3 * D + d] = q * r;
+      float z[4] = {r, q, q - r, q * r};
+      if constexpr (kDrop) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) z[k] = ins_drop(z[k], ins_keep(seed, p.p, b, i, kSiteCq, 0, k * D + d), p.scale);
+      }
+      s_z[d] = z[0];
+      s_z[D + d] = z[1];
+      s_z[2 * D + d] = z[2];
+      s_z[3 * D + d] = z[3];
     }
     __syncthreads();
     {
@@ -129,7 +162,11 @@ __global__ void __launch_bounds__(kQThreads) instructions_kernel(const InsParams
     __syncthreads();
     for (int q = warp; q < Q; q += nw) {                   // ca[q] = ca_linear(cq * hidden[q])
       float s = 0.f;
-      for (int d = lane; d < D; d += 32) s = fmaf(__ldg(p.wca + d), s_cq[d] * s_hid[(size_t)q * D + d], s);
+      for (int d = lane; d < D; d += 32) {
+        float e = s_cq[d] * s_hid[(size_t)q * D + d];
+        if constexpr (kDrop) e = ins_drop(e, ins_keep(seed, p.p, b, i, kSiteCa, q, d), p.scale);
+        s = fmaf(__ldg(p.wca + d), e, s);
+      }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
       if (lane == 0) s_ca[q] = (s + p.bca[0]) + (1.f - s_mask[q]) * kVeryNegQ;
@@ -161,9 +198,182 @@ __global__ void __launch_bounds__(kQThreads) instructions_kernel(const InsParams
   }
 }
 
+struct InsBwdParams {
+  InsParams f;              // the forward's inputs (out / attn_out unused), seed, p, scale
+  const float* ri;          // [B, I, D] the forward's instructions
+  const float* attn;        // [B, I, Q] the forward's attention
+  const float* grad_out;    // [B, I, D]
+  float* grad_hidden;       // [B, Q, D]
+  float* grad_qnode;        // [B, D]
+  float *g_q, *x_q;         // [B, I, D]: question_linear_i pre-activation gradient and its (dropped) input
+  float *g_cq, *x_cq;       // [B, I, D], [B, I, 4D]: cq_linear
+  float *g_ca, *x_ca;       // [B, I, Q], [B, I, Q, D]: ca_linear (the masked logit's gradient)
+};
+
+// y[k] = sum_n W[n * ldw + k] * x[n] for k < K, n in order: one thread per output column (coalesced across k)
+__device__ __forceinline__ void block_gemv_t(const float* __restrict__ W, int64_t ldw, const float* x, float* y,
+                                             int N, int K) {
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    float s = 0.f;
+    for (int n = 0; n < N; ++n) s = fmaf(__ldg(W + (int64_t)n * ldw + k), x[n], s);
+    y[k] = s;
+  }
+}
+
+// gr_instructions_backward: one CTA per question walks the steps in reverse.  Step i is recomputed from the saved
+// inputs, the forward's ri[i-1] and attention and the seed (the mask is redrawn, never stored), with the forward
+// kernel's operations, so the recomputed q_i, cq and dropped operands are the forward's bits.  Every output element is
+// owned by this CTA and written by one thread per step, in a fixed order: no atomics.
+template <bool kDrop>
+__global__ void __launch_bounds__(kQThreads) instructions_bwd_kernel(const InsBwdParams a) {
+  extern __shared__ __align__(16) float smq[];
+  const InsParams& p = a.f;
+  const int D = p.D, Q = p.Q, I = p.I, b = blockIdx.x, tid = threadIdx.x;
+  const int lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
+  const uint64_t seed = kDrop ? (uint64_t)__ldg(p.seed) : 0;
+  float* s_hid = smq;                    // [Q][D]
+  float* s_qn = s_hid + (size_t)Q * D;   // [D]
+  float* s_q = s_qn + D;                 // [D]   q_i
+  float* s_cq = s_q + D;                 // [D]   cq, then its gradient
+  float* s_gr = s_cq + D;                // [D]   gradient of ri[i]
+  float* s_g4 = s_gr + D;                // [4D]  gradient of the dropped cq_linear input, then of q_i (first D)
+  float* s_gca = s_g4 + 4 * D;           // [Q]   dattn, then the logit gradient (pads: attn = 0, so 0)
+  const int64_t bq = (int64_t)b * Q * D;
+  for (int i = tid; i < Q * D; i += blockDim.x) {
+    s_hid[i] = p.hidden[bq + i];
+    a.grad_hidden[bq + i] = 0.f;
+  }
+  for (int d = tid; d < D; d += blockDim.x) {
+    s_qn[d] = p.qnode[(int64_t)b * D + d];
+    s_gr[d] = a.grad_out[((int64_t)b * I + I - 1) * D + d];
+    a.grad_qnode[(int64_t)b * D + d] = 0.f;
+  }
+  __syncthreads();
+  for (int i = I - 1; i >= 0; --i) {
+    const int64_t bi = (int64_t)b * I + i;
+    const float* ri_prev = i > 0 ? a.ri + (bi - 1) * D : nullptr;   // ri[-1] = 0
+    float* xq = a.x_q + bi * D;
+    float* xcq = a.x_cq + bi * 4 * D;
+    const float* at = a.attn + bi * Q;
+    // ---- recompute q_i and cq of step i (the forward's operations) ----
+    for (int d = tid; d < D; d += blockDim.x)
+      xq[d] = kDrop ? ins_drop(s_qn[d], ins_keep(seed, p.p, b, i, kSiteQnode, 0, d), p.scale) : s_qn[d];
+    __syncthreads();
+    {
+      GemvGroup grp[1] = {GemvGroup{p.Wq[i], p.bq[i], xq, s_q}};
+      block_gemv(grp, 1, D, D, D);
+    }
+    __syncthreads();
+    for (int d = tid; d < D; d += blockDim.x) {
+      const float r = ri_prev ? ri_prev[d] : 0.f, q = s_q[d];
+      float z[4] = {r, q, q - r, q * r};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        if (kDrop) z[k] = ins_drop(z[k], ins_keep(seed, p.p, b, i, kSiteCq, 0, k * D + d), p.scale);
+        xcq[k * D + d] = z[k];
+      }
+    }
+    __syncthreads();
+    {
+      GemvGroup grp[1] = {GemvGroup{p.Wcq, p.bcq, xcq, s_cq}};
+      block_gemv(grp, 1, 4 * D, D, 4 * D);
+    }
+    // ---- ri[i] = sum_q attn[q] hidden[q]:  dattn[q] = <hidden[q], g_ri> ----
+    for (int q = warp; q < Q; q += nw) {
+      float s = 0.f;
+      for (int d = lane; d < D; d += 32) s = fmaf(s_hid[(size_t)q * D + d], s_gr[d], s);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) s_gca[q] = s;
+    }
+    __syncthreads();
+    // ---- softmax: g_ca[q] = attn[q] (dattn[q] - sum_q' attn[q'] dattn[q']), q' in order ----
+    if (warp == 0) {
+      float s = 0.f;
+      for (int q = lane; q < Q; q += 32) s = fmaf(__ldg(at + q), s_gca[q], s);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      for (int q = lane; q < Q; q += 32) {
+        const float g = __ldg(at + q) * (s_gca[q] - s);
+        s_gca[q] = g;
+        a.g_ca[bi * Q + q] = g;
+      }
+    }
+    __syncthreads();
+    // ---- ca[q] = <wca, drop(cq * hidden[q])> + bca:  one thread per column d walks the tokens in order ----
+    for (int d = tid; d < D; d += blockDim.x) {
+      const float cq = s_cq[d], w = __ldg(p.wca + d), gr = s_gr[d];
+      float gcq = 0.f;
+      for (int q = 0; q < Q; ++q) {
+        const float h = s_hid[(size_t)q * D + d];
+        float e = cq * h, ge = s_gca[q] * w;
+        if (kDrop) {
+          const bool keep = ins_keep(seed, p.p, b, i, kSiteCa, q, d);
+          e = ins_drop(e, keep, p.scale);
+          ge = ins_drop(ge, keep, p.scale);
+        }
+        a.x_ca[(bi * Q + q) * D + d] = e;
+        float* gh = a.grad_hidden + bq + (int64_t)q * D + d;
+        *gh = *gh + fmaf(ge, cq, __ldg(at + q) * gr);
+        gcq = fmaf(ge, h, gcq);
+      }
+      s_cq[d] = gcq;                                      // cq is dead in this column from here on
+      a.g_cq[bi * D + d] = gcq;
+    }
+    __syncthreads();
+    // ---- cq = Wcq drop(z) + bcq:  g_z = drop'(Wcq^T g_cq) ----
+    block_gemv_t(p.Wcq, 4 * D, s_cq, s_g4, D, 4 * D);
+    __syncthreads();
+    for (int d = tid; d < D; d += blockDim.x) {
+      float gz[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        gz[k] = s_g4[k * D + d];
+        if (kDrop) gz[k] = ins_drop(gz[k], ins_keep(seed, p.p, b, i, kSiteCq, 0, k * D + d), p.scale);
+      }
+      const float r = ri_prev ? ri_prev[d] : 0.f, q = s_q[d];
+      const float gq = fmaf(gz[3], r, gz[1] + gz[2]);     // z = [ri, q, q - ri, q * ri]
+      const float gri = fmaf(gz[3], q, gz[0] - gz[2]);
+      s_g4[d] = gq;                                       // this thread's own columns only
+      a.g_q[bi * D + d] = gq;
+      s_gr[d] = i > 0 ? a.grad_out[(bi - 1) * D + d] + gri : 0.f;
+    }
+    __syncthreads();
+    // ---- q_i = Wq_i drop(qnode) + bq_i:  grad_qnode += drop'(Wq_i^T g_q) ----
+    for (int k = tid; k < D; k += blockDim.x) {
+      float s = 0.f;
+      for (int n = 0; n < D; ++n) s = fmaf(__ldg(p.Wq[i] + (int64_t)n * D + k), s_g4[n], s);
+      if (kDrop) s = ins_drop(s, ins_keep(seed, p.p, b, i, kSiteQnode, 0, k), p.scale);
+      a.grad_qnode[(int64_t)b * D + k] += s;
+    }
+    __syncthreads();
+  }
+}
+
+// the dropout masks of gr_instructions_train: one thread per element of the three sites
+__global__ void instructions_dropout_mask_kernel(const int64_t* __restrict__ seed, float p, int B, int Q, int D, int I,
+                                                 uint8_t* __restrict__ m_q, uint8_t* __restrict__ m_cq,
+                                                 uint8_t* __restrict__ m_ca) {
+  const uint64_t sd = (uint64_t)__ldg(seed);
+  const int64_t nq = (int64_t)B * I * D, ncq = 4 * nq, nca = (int64_t)Q * nq;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < nq + ncq + nca; t += stride) {
+    if (t < nq) {
+      const int64_t bi = t / D;
+      m_q[t] = ins_keep(sd, p, (int)(bi / I), (int)(bi % I), kSiteQnode, 0, (int)(t % D));
+    } else if (t < nq + ncq) {
+      const int64_t u = t - nq, bi = u / (4 * D);
+      m_cq[u] = ins_keep(sd, p, (int)(bi / I), (int)(bi % I), kSiteCq, 0, (int)(u % (4 * D)));
+    } else {
+      const int64_t u = t - nq - ncq, biq = u / D, bi = biq / Q;
+      m_ca[u] = ins_keep(sd, p, (int)(bi / I), (int)(bi % I), kSiteCa, (int)(biq % Q), (int)(u % D));
+    }
+  }
+}
+
 struct ReformParams {
   const float* seed;        // [B, N] seed weights (query_entities)
-  const float* h;           // [B*N, ldh] node embeddings
+  const void* h;            // [B*N, ldh] node embeddings, fp32 or (GR_IO_BF16) bf16
   int64_t ldh;
   const float* ins_in;      // [B, I, D]
   const float* Wr[kMaxIns]; // reform_j.fusion.r.weight [D, 3D]
@@ -173,15 +383,60 @@ struct ReformParams {
   int B, N, D, I;
 };
 
+// The non-zero seeds of one question in index order, a block-wide walk: chunks of blockDim.x nodes are compacted into
+// (s_list, s_val) and f(cnt) is called by every thread after each chunk, with the chunk's cnt seeds in index order.
+struct SeedList {
+  int list[kQThreads];
+  float val[kQThreads];
+  int woff[kQThreads / 32 + 1];
+};
+
+template <typename F>
+__device__ __forceinline__ void for_each_seed_chunk(const float* sd, int N, SeedList& sl, F&& f) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
+  for (int base = 0; base < N; base += blockDim.x) {
+    const int n = base + tid;
+    const float v = n < N ? sd[n] : 0.f;
+    const bool nz = v != 0.f;
+    const unsigned bal = __ballot_sync(0xffffffffu, nz);
+    if (lane == 0) sl.woff[warp + 1] = __popc(bal);
+    __syncthreads();
+    if (tid == 0) {
+      sl.woff[0] = 0;
+      for (int i = 0; i < nw; ++i) sl.woff[i + 1] += sl.woff[i];
+    }
+    __syncthreads();
+    if (nz) {
+      const int pos = sl.woff[warp] + __popc(bal & ((1u << lane) - 1));
+      sl.list[pos] = n;
+      sl.val[pos] = v;
+    }
+    __syncthreads();
+    f(sl.woff[nw]);
+    __syncthreads();
+  }
+}
+
+// seed_retrieve = seed_info[b] @ h[b] (query_update.py:40) for column tid < D, seeds in index order
+template <typename T>
+__device__ __forceinline__ float seed_retrieve_col(const float* sd, const T* h, int64_t ldh, int b, int N, int D,
+                                                   SeedList& sl) {
+  const int tid = threadIdx.x;
+  float acc = 0.f;             // thread d owns column d (D <= 1024)
+  for_each_seed_chunk(sd, N, sl, [&](int cnt) {
+    if (tid < D)
+      for (int i = 0; i < cnt; ++i) acc = fmaf(sl.val[i], ldg_node(h + ((int64_t)b * N + sl.list[i]) * ldh + tid), acc);
+  });
+  return acc;
+}
+
+template <typename T>
 __global__ void __launch_bounds__(kQThreads) query_reform_kernel(const ReformParams p) {
   extern __shared__ __align__(16) float smq[];
-  __shared__ int s_list[kQThreads];
-  __shared__ float s_val[kQThreads];
-  __shared__ int s_woff[kQThreads / 32 + 1];
+  __shared__ SeedList sl;
   // grid (B, S): CTA (b, s) owns output columns [d0, d1) of question b's new instructions (the seed pick is cheap and
   // repeated by every slice); 4 x as many CTAs as questions: the one-CTA-per-question version left most SMs idle
   const int D = p.D, N = p.N, b = blockIdx.x, tid = threadIdx.x;
-  const int lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
   const int dper = (D + gridDim.y - 1) / gridDim.y;
   const int d0 = min(D, (int)blockIdx.y * dper), d1 = min(D, d0 + dper);
   float* s_y = smq;            // [D]        seed_retrieve
@@ -189,31 +444,7 @@ __global__ void __launch_bounds__(kQThreads) query_reform_kernel(const ReformPar
   float* s_g = s_z + (size_t)p.I * 3 * D;   // [I][D]
   float* s_r = s_g + (size_t)p.I * D;       // [I][D]
   // ---- seed_retrieve = seed_info[b] @ h[b]  (query_update.py:40); seeds visited in index order ----
-  const float* sd = p.seed + (int64_t)b * N;
-  float acc = 0.f;             // thread d owns column d (D <= 1024)
-  for (int base = 0; base < N; base += blockDim.x) {
-    const int n = base + tid;
-    const float v = n < N ? sd[n] : 0.f;
-    const bool nz = v != 0.f;
-    const unsigned bal = __ballot_sync(0xffffffffu, nz);
-    if (lane == 0) s_woff[warp + 1] = __popc(bal);
-    __syncthreads();
-    if (tid == 0) {
-      s_woff[0] = 0;
-      for (int i = 0; i < nw; ++i) s_woff[i + 1] += s_woff[i];
-    }
-    __syncthreads();
-    if (nz) {
-      const int pos = s_woff[warp] + __popc(bal & ((1u << lane) - 1));
-      s_list[pos] = n;
-      s_val[pos] = v;
-    }
-    __syncthreads();
-    const int cnt = s_woff[nw];
-    if (tid < D)
-      for (int i = 0; i < cnt; ++i) acc = fmaf(s_val[i], p.h[((int64_t)b * N + s_list[i]) * p.ldh + tid], acc);
-    __syncthreads();
-  }
+  const float acc = seed_retrieve_col(p.seed + (int64_t)b * N, static_cast<const T*>(p.h), p.ldh, b, N, D, sl);
   if (tid < D) {
     s_y[tid] = acc;
     if (p.seed_out && blockIdx.y == 0) p.seed_out[(int64_t)b * D + tid] = acc;
@@ -244,6 +475,99 @@ __global__ void __launch_bounds__(kQThreads) query_reform_kernel(const ReformPar
     const float g = 1.f / (1.f + expf(-s_g[(size_t)j * D + d]));
     p.ins_out[((int64_t)b * p.I + j) * D + d] = g * s_r[(size_t)j * D + d] + (1.f - g) * s_z[(size_t)j * 3 * D + d];
   }
+}
+
+struct ReformBwdParams {
+  ReformParams f;           // the forward's inputs (ins_out / seed_out unused)
+  const float* grad_out;    // [B, I, D]
+  float* grad_ins;          // [B, I, D]
+  void* grad_h;             // [B*N, ldg] in h's type: the seed rows are added to, nothing else is touched
+  int64_t ldg;
+  float *g_r, *g_g;         // [B, I, D] pre-activation gradients of fusion.r / fusion.g
+  float* x_z;               // [B, I, 3D] their input z = [x, y, x - y]
+};
+
+// gr_query_reform_backward: one CTA per question recomputes y, z, g and r with the forward's operations (the same
+// seed walk and GEMV rows), then
+//   g_r = G g,  g_g = G (r - x) g (1 - g),  g_z = Wr^T g_r + Wg^T g_g   (each transposed GEMV over n in order),
+//   grad_x = (G (1 - g) + g_z[x]) + g_z[x - y],   g_y = sum_j (g_z[y] - g_z[x - y]) in j order,
+//   grad_h[seed n] = fma(s_n, g_y, grad_h[seed n]) over the forward's seed list.
+template <typename T>
+__global__ void __launch_bounds__(kQThreads) query_reform_bwd_kernel(const ReformBwdParams a) {
+  extern __shared__ __align__(16) float smq[];
+  __shared__ SeedList sl;
+  const ReformParams& p = a.f;
+  const int D = p.D, N = p.N, I = p.I, b = blockIdx.x, tid = threadIdx.x;
+  float* s_y = smq;                         // [D]      y, then g_y
+  float* s_z = s_y + D;                     // [I][3D]  z, then g_z
+  float* s_g = s_z + (size_t)I * 3 * D;     // [I][D]   G z, then g_g
+  float* s_r = s_g + (size_t)I * D;         // [I][D]   R z, then g_r
+  const float* sd = p.seed + (int64_t)b * N;
+  const float acc = seed_retrieve_col(sd, static_cast<const T*>(p.h), p.ldh, b, N, D, sl);
+  if (tid < D) s_y[tid] = acc;
+  __syncthreads();
+  for (int i = tid; i < I * D; i += blockDim.x) {
+    const int j = i / D, d = i - j * D;
+    const float xv = p.ins_in[((int64_t)b * I + j) * D + d], yv = s_y[d];
+    float* z = s_z + (size_t)j * 3 * D;
+    float* xz = a.x_z + ((int64_t)b * I + j) * 3 * D;
+    z[d] = xz[d] = xv;
+    z[D + d] = xz[D + d] = yv;
+    z[2 * D + d] = xz[2 * D + d] = xv - yv;
+  }
+  __syncthreads();
+  {
+    GemvGroup grp[2 * kMaxIns];
+    for (int j = 0; j < I; ++j) {
+      grp[2 * j] = GemvGroup{p.Wg[j], nullptr, s_z + (size_t)j * 3 * D, s_g + (size_t)j * D};
+      grp[2 * j + 1] = GemvGroup{p.Wr[j], nullptr, s_z + (size_t)j * 3 * D, s_r + (size_t)j * D};
+    }
+    block_gemv(grp, 2 * I, 3 * D, D, 3 * D);
+  }
+  __syncthreads();
+  for (int i = tid; i < I * D; i += blockDim.x) {   // out = g r + (1 - g) x
+    const int j = i / D, d = i - j * D;
+    const int64_t o = ((int64_t)b * I + j) * D + d;
+    const float G = a.grad_out[o];
+    const float g = 1.f / (1.f + expf(-s_g[i])), r = s_r[i], x = s_z[(size_t)j * 3 * D + d];
+    const float gr = G * g, gg = G * (r - x) * (g * (1.f - g));
+    s_r[i] = gr;
+    s_g[i] = gg;
+    a.g_r[o] = gr;
+    a.g_g[o] = gg;
+    a.grad_ins[o] = G * (1.f - g);
+  }
+  __syncthreads();
+  for (int i = tid; i < I * 3 * D; i += blockDim.x) {   // g_z = Wr^T g_r + Wg^T g_g  (z is in x_z from here on)
+    const int j = i / (3 * D), k = i - j * 3 * D;
+    float sr = 0.f, sg = 0.f;
+    for (int n = 0; n < D; ++n) {
+      sr = fmaf(__ldg(p.Wr[j] + (int64_t)n * 3 * D + k), s_r[(size_t)j * D + n], sr);
+      sg = fmaf(__ldg(p.Wg[j] + (int64_t)n * 3 * D + k), s_g[(size_t)j * D + n], sg);
+    }
+    s_z[i] = sr + sg;
+  }
+  __syncthreads();
+  for (int i = tid; i < I * D; i += blockDim.x) {
+    const int j = i / D, d = i - j * D;
+    const float* gz = s_z + (size_t)j * 3 * D;
+    const int64_t o = ((int64_t)b * I + j) * D + d;
+    a.grad_ins[o] = (a.grad_ins[o] + gz[d]) + gz[2 * D + d];
+  }
+  for (int d = tid; d < D; d += blockDim.x) {
+    float gy = 0.f;
+    for (int j = 0; j < I; ++j) gy += s_z[(size_t)j * 3 * D + D + d] - s_z[(size_t)j * 3 * D + 2 * D + d];
+    s_y[d] = gy;
+  }
+  __syncthreads();
+  T* gh = static_cast<T*>(a.grad_h);
+  for_each_seed_chunk(sd, N, sl, [&](int cnt) {
+    for (int i = 0; i < cnt; ++i)
+      for (int d = tid; d < D; d += blockDim.x) {
+        T* e = gh + ((int64_t)b * N + sl.list[i]) * a.ldg + d;
+        st_node(e, fmaf(sl.val[i], s_y[d], ld_node(e)));
+      }
+  });
 }
 
 __device__ __forceinline__ float block_sum(float v, float* sm) {
@@ -331,57 +655,218 @@ __global__ void loss_finalize_kernel(const float* __restrict__ loss_q, float* __
 }  // namespace
 }  // namespace gr
 
+namespace gr {
+namespace {
+
+// InsParams of the three instruction entry points: the forward's inputs and the dropout (p in [0, 1); p = 0 ignores
+// the seed).  Admits exactly the shapes of gr_instructions: I <= 8 and (Q D + (I + 7) D + 2 Q) floats <= 200 KB.
+int ins_params(const char* fn, InsParams& p, const float* hidden, const float* qnode, const int64_t* qtext,
+               int64_t pad_id, const float* const* Wq_host, const float* const* bq_host, const float* Wcq,
+               const float* bcq, const float* wca, const float* bca, const int64_t* seed, double drop, int B, int Q,
+               int D, int I, size_t* smem) {
+  GR_CHECK_ARG_AS(fn, hidden && qnode && qtext && Wq_host && bq_host && Wcq && bcq && wca && bca, "null pointer");
+  GR_CHECK_ARG_AS(fn, B > 0 && Q > 0 && D > 0 && I > 0 && I <= kMaxIns, "bad shape (num_ins <= 8)");
+  GR_CHECK_ARG_AS(fn, drop >= 0.0 && drop < 1.0, "dropout probability outside [0, 1)");
+  GR_CHECK_ARG_AS(fn, drop == 0.0 || seed, "null seed with p > 0");
+  p.hidden = hidden; p.qnode = qnode; p.qtext = qtext; p.pad = pad_id;
+  for (int i = 0; i < I; ++i) {
+    GR_CHECK_ARG_AS(fn, Wq_host[i] && bq_host[i], "null question_linear pointer");
+    p.Wq[i] = Wq_host[i];
+    p.bq[i] = bq_host[i];
+  }
+  p.Wcq = Wcq; p.bcq = bcq; p.wca = wca; p.bca = bca;
+  p.B = B; p.Q = Q; p.D = D; p.I = I;
+  p.seed = drop > 0.0 ? seed : nullptr;
+  p.p = (float)drop;
+  p.scale = (float)(1.0 / (1.0 - drop));
+  *smem = ((size_t)Q * D + (size_t)(I + 7) * D + 2 * (size_t)Q) * sizeof(float);
+  GR_CHECK_ARG_AS(fn, *smem <= 200 * 1024, "question length x entity_dim too large for shared memory");
+  return GR_OK;
+}
+
+int launch_instructions(const char* fn, const InsParams& p, size_t smem, cudaStream_t stream) {
+  auto go = [&](auto drop) -> int {
+    constexpr bool kDrop = decltype(drop)::value;
+    if (int rc = opt_in_smem<instructions_kernel<kDrop>>(fn, 200 * 1024)) return rc;
+    instructions_kernel<kDrop><<<p.B, kQThreads, smem, stream>>>(p);
+    GR_CHECK_LAUNCH_AS(fn);
+    return GR_OK;
+  };
+  return p.p > 0.f ? go(std::true_type{}) : go(std::false_type{});
+}
+
+// the backward keeps Q D + 8 D + Q floats in shared memory: never more than the forward's Q D + (I + 7) D + 2 Q
+int launch_instructions_bwd(const char* fn, const InsBwdParams& a, cudaStream_t stream) {
+  const InsParams& p = a.f;
+  const size_t smem = ((size_t)p.Q * p.D + 8 * (size_t)p.D + (size_t)p.Q) * sizeof(float);
+  auto go = [&](auto drop) -> int {
+    constexpr bool kDrop = decltype(drop)::value;
+    if (int rc = opt_in_smem<instructions_bwd_kernel<kDrop>>(fn, 200 * 1024)) return rc;
+    instructions_bwd_kernel<kDrop><<<p.B, kQThreads, smem, stream>>>(a);
+    GR_CHECK_LAUNCH_AS(fn);
+    return GR_OK;
+  };
+  return p.p > 0.f ? go(std::true_type{}) : go(std::false_type{});
+}
+
+// ReformParams of the reform entry points.  Admits exactly the shapes of gr_query_reform: D <= 1024, I <= 8 and
+// (5I + 1) D floats <= 48 KB.
+int reform_params(const char* fn, ReformParams& p, const float* seed_info, const void* h, int64_t ldh,
+                  const float* ins_in, const float* const* Wr_host, const float* const* Wg_host, int B, int N, int D,
+                  int I, uint32_t io, size_t* smem) {
+  if (int rc = check_io(fn, io)) return rc;
+  GR_CHECK_ARG_AS(fn, seed_info && h && ins_in && Wr_host && Wg_host, "null pointer");
+  GR_CHECK_ARG_AS(fn, B > 0 && N > 0 && D > 0 && D <= kQThreads && ldh >= D && I > 0 && I <= kMaxIns,
+                  "bad shape (D <= 1024, num_ins <= 8)");
+  p.seed = seed_info; p.h = h; p.ldh = ldh; p.ins_in = ins_in;
+  for (int j = 0; j < I; ++j) {
+    GR_CHECK_ARG_AS(fn, Wr_host[j] && Wg_host[j], "null fusion weight pointer");
+    p.Wr[j] = Wr_host[j];
+    p.Wg[j] = Wg_host[j];
+  }
+  p.B = B; p.N = N; p.D = D; p.I = I;
+  *smem = ((size_t)1 + 5 * (size_t)I) * D * sizeof(float);
+  GR_CHECK_ARG_AS(fn, *smem <= 48 * 1024, "num_ins x entity_dim too large for shared memory");
+  return GR_OK;
+}
+
+// The kernels' static seed list (SeedList, ~8 KB) comes on top of the dynamic area: without the opt-in, static +
+// dynamic is capped at 48 KB and every admitted shape with (5I+1)*D > ~10200 fails to launch.
+int launch_query_reform(const char* fn, const ReformParams& p, size_t smem, uint32_t io, cudaStream_t stream) {
+  const int slices = p.D >= 128 ? 4 : (p.D >= 64 ? 2 : 1);
+  return with_node_type(io, [&](auto t) -> int {
+    using T = typename decltype(t)::type;
+    if (int rc = opt_in_smem<query_reform_kernel<T>>(fn, 48 * 1024)) return rc;
+    query_reform_kernel<T><<<dim3((unsigned)p.B, (unsigned)slices), kQThreads, smem, stream>>>(p);
+    GR_CHECK_LAUNCH_AS(fn);
+    return GR_OK;
+  });
+}
+
+int launch_query_reform_bwd(const char* fn, const ReformBwdParams& a, size_t smem, uint32_t io, cudaStream_t stream) {
+  return with_node_type(io, [&](auto t) -> int {
+    using T = typename decltype(t)::type;
+    if (int rc = opt_in_smem<query_reform_bwd_kernel<T>>(fn, 48 * 1024)) return rc;
+    query_reform_bwd_kernel<T><<<a.f.B, kQThreads, smem, stream>>>(a);
+    GR_CHECK_LAUNCH_AS(fn);
+    return GR_OK;
+  });
+}
+
+}  // namespace
+}  // namespace gr
+
 extern "C" int gr_instructions(const float* hidden, const float* qnode, const int64_t* qtext, int64_t pad_id,
                                const float* const* Wq_host, const float* const* bq_host, const float* Wcq,
                                const float* bcq, const float* wca, const float* bca, float* out,
                                float* attn_out, int B, int Q, int D, int I, void* stream_) {
   using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(hidden && qnode && qtext && Wq_host && bq_host && Wcq && bcq && wca && bca && out,
-               "null pointer");
-  GR_CHECK_ARG(B > 0 && Q > 0 && D > 0 && I > 0 && I <= kMaxIns, "bad shape (num_ins <= 8)");
   InsParams p{};
-  p.hidden = hidden; p.qnode = qnode; p.qtext = qtext; p.pad = pad_id;
-  for (int i = 0; i < I; ++i) {
-    GR_CHECK_ARG(Wq_host[i] && bq_host[i], "null question_linear pointer");
-    p.Wq[i] = Wq_host[i];
-    p.bq[i] = bq_host[i];
-  }
-  p.Wcq = Wcq; p.bcq = bcq; p.wca = wca; p.bca = bca; p.out = out; p.attn_out = attn_out;
-  p.B = B; p.Q = Q; p.D = D; p.I = I;
-  const size_t smem = ((size_t)Q * D + (size_t)(I + 7) * D + 2 * (size_t)Q) * sizeof(float);
-  GR_CHECK_ARG(smem <= 200 * 1024, "question length x entity_dim too large for shared memory");
-  if (int rc = opt_in_smem<instructions_kernel>(__func__, 200 * 1024)) return rc;
-  instructions_kernel<<<B, kQThreads, smem, stream>>>(p);
+  size_t smem = 0;
+  if (int rc = ins_params(__func__, p, hidden, qnode, qtext, pad_id, Wq_host, bq_host, Wcq, bcq, wca, bca, nullptr,
+                          0.0, B, Q, D, I, &smem))
+    return rc;
+  GR_CHECK_ARG(out, "null pointer");
+  p.out = out; p.attn_out = attn_out;
+  return launch_instructions(__func__, p, smem, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gr_instructions_train(const float* hidden, const float* qnode, const int64_t* qtext, int64_t pad_id,
+                                     const float* const* Wq_host, const float* const* bq_host, const float* Wcq,
+                                     const float* bcq, const float* wca, const float* bca, const int64_t* seed,
+                                     double p_drop, float* out, float* attn_out, int B, int Q, int D, int I,
+                                     void* stream_) {
+  using namespace gr;
+  InsParams p{};
+  size_t smem = 0;
+  if (int rc = ins_params(__func__, p, hidden, qnode, qtext, pad_id, Wq_host, bq_host, Wcq, bcq, wca, bca, seed,
+                          p_drop, B, Q, D, I, &smem))
+    return rc;
+  GR_CHECK_ARG(out && attn_out, "null pointer");
+  p.out = out; p.attn_out = attn_out;
+  return launch_instructions(__func__, p, smem, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gr_instructions_backward(const float* hidden, const float* qnode, const int64_t* qtext, int64_t pad_id,
+                                        const float* const* Wq_host, const float* const* bq_host, const float* Wcq,
+                                        const float* bcq, const float* wca, const float* bca, const int64_t* seed,
+                                        double p_drop, const float* ri, const float* attn, const float* grad_out,
+                                        float* grad_hidden, float* grad_qnode, float* g_q, float* x_q, float* g_cq,
+                                        float* x_cq, float* g_ca, float* x_ca, int B, int Q, int D, int I,
+                                        void* stream_) {
+  using namespace gr;
+  InsBwdParams a{};
+  size_t smem = 0;
+  if (int rc = ins_params(__func__, a.f, hidden, qnode, qtext, pad_id, Wq_host, bq_host, Wcq, bcq, wca, bca, seed,
+                          p_drop, B, Q, D, I, &smem))
+    return rc;
+  GR_CHECK_ARG(ri && attn && grad_out && grad_hidden && grad_qnode && g_q && x_q && g_cq && x_cq && g_ca && x_ca,
+               "null pointer");
+  a.ri = ri; a.attn = attn; a.grad_out = grad_out; a.grad_hidden = grad_hidden; a.grad_qnode = grad_qnode;
+  a.g_q = g_q; a.x_q = x_q; a.g_cq = g_cq; a.x_cq = x_cq; a.g_ca = g_ca; a.x_ca = x_ca;
+  return launch_instructions_bwd(__func__, a, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gr_instructions_dropout_mask(const int64_t* seed, double p, int B, int Q, int D, int I, uint8_t* mask_q,
+                                            uint8_t* mask_cq, uint8_t* mask_ca, void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(seed && mask_q && mask_cq && mask_ca, "null pointer");
+  GR_CHECK_ARG(B > 0 && Q > 0 && D > 0 && I > 0 && I <= kMaxIns, "bad shape (num_ins <= 8)");
+  GR_CHECK_ARG(p > 0.0 && p < 1.0, "dropout probability outside (0, 1)");
+  const int64_t total = (int64_t)B * I * D * (5 + (int64_t)Q);
+  const int grid = (int)std::min<int64_t>(ceil_div(total, 256), 8192);
+  instructions_dropout_mask_kernel<<<grid, 256, 0, stream>>>(seed, (float)p, B, Q, D, I, mask_q, mask_cq, mask_ca);
   GR_CHECK_LAUNCH();
   return GR_OK;
 }
 
+namespace gr {
+namespace {
+
+// gr_query_reform and gr_query_reform_ex; errors name the entry point `fn`
+int query_reform_entry(const char* fn, const float* seed_info, const void* h, int64_t ldh, const float* ins_in,
+                       const float* const* Wr_host, const float* const* Wg_host, float* ins_out, float* seed_out,
+                       int B, int N, int D, int I, uint32_t io, void* stream_) {
+  ReformParams p{};
+  size_t smem = 0;
+  if (int rc = reform_params(fn, p, seed_info, h, ldh, ins_in, Wr_host, Wg_host, B, N, D, I, io, &smem)) return rc;
+  GR_CHECK_ARG_AS(fn, ins_out, "null pointer");
+  p.ins_out = ins_out; p.seed_out = seed_out;
+  return launch_query_reform(fn, p, smem, io, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+}  // namespace
+}  // namespace gr
+
 extern "C" int gr_query_reform(const float* seed_info, const float* h, int64_t ldh, const float* ins_in,
                                const float* const* Wr_host, const float* const* Wg_host, float* ins_out,
                                float* seed_out, int B, int N, int D, int I, void* stream_) {
+  return gr::query_reform_entry(__func__, seed_info, h, ldh, ins_in, Wr_host, Wg_host, ins_out, seed_out, B, N, D, I,
+                                0u, stream_);
+}
+
+extern "C" int gr_query_reform_ex(const float* seed_info, const void* h, int64_t ldh, const float* ins_in,
+                                  const float* const* Wr_host, const float* const* Wg_host, float* ins_out,
+                                  float* seed_out, int B, int N, int D, int I, uint32_t io, void* stream_) {
+  return gr::query_reform_entry(__func__, seed_info, h, ldh, ins_in, Wr_host, Wg_host, ins_out, seed_out, B, N, D, I,
+                                io, stream_);
+}
+
+extern "C" int gr_query_reform_backward(const float* seed_info, const void* h, int64_t ldh, const float* ins_in,
+                                        const float* const* Wr_host, const float* const* Wg_host,
+                                        const float* grad_out, float* grad_ins, void* grad_h, int64_t ldg, float* g_r,
+                                        float* g_g, float* x_z, int B, int N, int D, int I, uint32_t io,
+                                        void* stream_) {
   using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(seed_info && h && ins_in && Wr_host && Wg_host && ins_out, "null pointer");
-  GR_CHECK_ARG(B > 0 && N > 0 && D > 0 && D <= kQThreads && ldh >= D && I > 0 && I <= kMaxIns,
-               "bad shape (D <= 1024, num_ins <= 8)");
-  ReformParams p{};
-  p.seed = seed_info; p.h = h; p.ldh = ldh; p.ins_in = ins_in; p.ins_out = ins_out; p.seed_out = seed_out;
-  for (int j = 0; j < I; ++j) {
-    GR_CHECK_ARG(Wr_host[j] && Wg_host[j], "null fusion weight pointer");
-    p.Wr[j] = Wr_host[j];
-    p.Wg[j] = Wg_host[j];
-  }
-  p.B = B; p.N = N; p.D = D; p.I = I;
-  const size_t smem = ((size_t)1 + 5 * (size_t)I) * D * sizeof(float);
-  GR_CHECK_ARG(smem <= 48 * 1024, "num_ins x entity_dim too large for shared memory");
-  // the kernel's static seed list (s_list / s_val / s_woff, ~8 KB) comes on top of the dynamic area: without the
-  // opt-in, static + dynamic is capped at 48 KB and every admitted shape with (5I+1)*D > ~10200 fails to launch
-  if (int rc = opt_in_smem<query_reform_kernel>(__func__, 48 * 1024)) return rc;
-  const int slices = D >= 128 ? 4 : (D >= 64 ? 2 : 1);
-  query_reform_kernel<<<dim3((unsigned)B, (unsigned)slices), kQThreads, smem, stream>>>(p);
-  GR_CHECK_LAUNCH();
-  return GR_OK;
+  ReformBwdParams a{};
+  size_t smem = 0;
+  if (int rc = reform_params(__func__, a.f, seed_info, h, ldh, ins_in, Wr_host, Wg_host, B, N, D, I, io, &smem))
+    return rc;
+  GR_CHECK_ARG(grad_out && grad_ins && grad_h && g_r && g_g && x_z, "null pointer");
+  GR_CHECK_ARG(ldg >= D, "bad grad_h row stride");
+  a.grad_out = grad_out; a.grad_ins = grad_ins; a.grad_h = grad_h; a.ldg = ldg; a.g_r = g_r; a.g_g = g_g; a.x_z = x_z;
+  return launch_query_reform_bwd(__func__, a, smem, io, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int gr_kl_loss_pred(const float* dist, const float* teacher, float* loss_q, float* loss,

@@ -810,6 +810,105 @@ def query_reform(seed_info, h, ins, Wr, Wg, B, N):
     return out
 
 
+def _ins_args(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca):
+    hidden = _cuda(hidden, torch.float32, "hidden").contiguous()
+    qnode = _cuda(qnode, torch.float32, "qnode").contiguous()
+    qtext = _cuda(qtext, torch.int64, "qtext").contiguous()
+    wca = wca.reshape(-1).contiguous()
+    return (hidden, qnode, qtext, [_p(hidden), _p(qnode), _p(qtext), int(pad_id), _ptr_array(Wq), _ptr_array(bq),
+                                   _p(Wcq.contiguous()), _p(bcq), _p(wca), _p(bca)])
+
+
+def instructions_train(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca, seed=None, p=0.0):
+    """Training forward of :func:`instructions` with the three linear_drop sites drawn in the kernel
+    (gr_instructions_train).  ``seed``: device int64 [1] (read when p > 0).  Returns (ins [B, I, D], attn [B, I, Q])."""
+    hidden, _qn, _qt, args = _ins_args(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca)
+    seed, p = _seed_p(seed, p)
+    B, Q, D = hidden.shape
+    I = len(Wq)
+    out = torch.empty(B, I, D, dtype=torch.float32, device=hidden.device)
+    attn = torch.empty(B, I, Q, dtype=torch.float32, device=hidden.device)
+    with _OpTimer("question_train"):
+        rc = _L().gr_instructions_train(*args, _p(seed), p, _p(out), _p(attn), B, Q, D, I, _stream())
+    _lib.check(rc)
+    STATS.launches += 1
+    return out, attn
+
+
+def instructions_dropout_mask(seed, p, B, Q, D, I):
+    """uint8 masks (1 = kept) of :func:`instructions_train`'s three dropout sites for 0 < p < 1:
+    (qnode [B, I, D], cq_linear input [B, I, 4D], ca_linear input [B, I, Q, D])."""
+    seed = _cuda(seed, torch.int64, "seed")
+    m = [torch.empty(s, dtype=torch.uint8, device=seed.device) for s in ((B, I, D), (B, I, 4 * D), (B, I, Q, D))]
+    _lib.check(_L().gr_instructions_dropout_mask(_p(seed), float(p), B, Q, D, I, *(_p(t) for t in m), _stream()))
+    STATS.launches += 1
+    return m
+
+
+def instructions_backward(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca, seed, p, ri, attn, grad_out):
+    """Backward of :func:`instructions_train` (same inputs, seed and p; its outputs ri and attn) given
+    grad_out = dL/dri [B, I, D] (gr_instructions_backward).  Returns grad_hidden [B, Q, D], grad_qnode [B, D] and the
+    weight-gradient operands (g_q, x_q [B, I, D]; g_cq [B, I, D], x_cq [B, I, 4D]; g_ca [B, I, Q], x_ca [B, I, Q, D])."""
+    hidden, _qn, _qt, args = _ins_args(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca)
+    seed, p = _seed_p(seed, p)
+    B, Q, D = hidden.shape
+    I = len(Wq)
+    ri = _cuda(ri, torch.float32, "ri").contiguous()
+    attn = _cuda(attn, torch.float32, "attn").contiguous()
+    grad_out = _cuda(grad_out, torch.float32, "grad_out").contiguous()
+    e = lambda *s: torch.empty(s, dtype=torch.float32, device=hidden.device)   # noqa: E731
+    outs = [e(B, Q, D), e(B, D), e(B, I, D), e(B, I, D), e(B, I, D), e(B, I, 4 * D), e(B, I, Q), e(B, I, Q, D)]
+    with _OpTimer("question_train"):
+        rc = _L().gr_instructions_backward(*args, _p(seed), p, _p(ri), _p(attn), _p(grad_out), *(_p(t) for t in outs),
+                                           B, Q, D, I, _stream())
+    _lib.check(rc)
+    STATS.launches += 1
+    return outs
+
+
+def _reform_h(h):
+    h = _cuda(h, name="h")
+    assert h.stride(1) == 1 and h.dtype in (torch.float32, torch.bfloat16), (h.stride(), h.dtype)
+    return h, IO_BF16 if h.dtype == torch.bfloat16 else 0
+
+
+def query_reform_train(seed_info, h, ins, Wr, Wg, B, N):
+    """:func:`query_reform` reading h in its own dtype (fp32, or bf16 under autocast: gr_query_reform_ex)."""
+    seed_info = _cuda(seed_info, torch.float32, "seed_info").contiguous()
+    ins = _cuda(ins, torch.float32, "ins").contiguous()
+    h, io = _reform_h(h)
+    _, I, D = ins.shape
+    out = torch.empty_like(ins)
+    with _OpTimer("question_train"):
+        rc = _L().gr_query_reform_ex(_p(seed_info), _p(h), h.stride(0), _p(ins), _ptr_array(Wr), _ptr_array(Wg),
+                                     _p(out), None, B, N, D, I, io, _stream())
+    _lib.check(rc)
+    STATS.launches += 1
+    return out
+
+
+def query_reform_backward(seed_info, h, ins, Wr, Wg, B, N, grad_out, grad_h):
+    """Backward of :func:`query_reform_train` (gr_query_reform_backward): adds s_n dL/dy to the seed rows of grad_h
+    ([B*N, D], h's dtype; no other row is touched) and returns grad_ins [B, I, D] and the weight-gradient operands
+    g_r, g_g [B, I, D] and z [B, I, 3D]."""
+    seed_info = _cuda(seed_info, torch.float32, "seed_info").contiguous()
+    ins = _cuda(ins, torch.float32, "ins").contiguous()
+    h, io = _reform_h(h)
+    grad_out = _cuda(grad_out, torch.float32, "grad_out").contiguous()
+    assert grad_h.dtype == h.dtype and grad_h.stride(1) == 1 and grad_h.shape[0] == B * N
+    _, I, D = ins.shape
+    e = lambda *s: torch.empty(s, dtype=torch.float32, device=ins.device)   # noqa: E731
+    outs = [e(B, I, D), e(B, I, D), e(B, I, D), e(B, I, 3 * D)]
+    with _OpTimer("question_train"):
+        rc = _L().gr_query_reform_backward(_p(seed_info), _p(h), h.stride(0), _p(ins), _ptr_array(Wr), _ptr_array(Wg),
+                                           _p(grad_out), _p(outs[0]), _p(grad_h), grad_h.stride(0), *(_p(t) for t in
+                                                                                                    outs[1:]),
+                                           B, N, D, I, io, _stream())
+    _lib.check(rc)
+    STATS.launches += 1
+    return outs
+
+
 def kl_loss_pred(dist, teacher):
     """-> (loss 0-dim fp32, pred int64[B]) : calc_loss_label('kl') with case_valid, and argmax (base_model.py:186)."""
     dist = _cuda(dist, torch.float32, "dist").contiguous()

@@ -533,6 +533,52 @@ int gr_instructions(const float* hidden, const float* qnode, const int64_t* qtex
 int gr_query_reform(const float* seed_info, const float* h, int64_t ldh, const float* ins_in,
                     const float* const* Wr_host, const float* const* Wg_host, float* ins_out,
                     float* seed_out, int B, int N, int D, int I, void* stream);
+/* gr_query_reform_ex: gr_query_reform with an io flags word (see the *_ex entry points): GR_IO_BF16 makes h bf16
+ * (widened on load; everything else fp32).  io = 0 is gr_query_reform. */
+int gr_query_reform_ex(const float* seed_info, const void* h, int64_t ldh, const float* ins_in,
+                       const float* const* Wr_host, const float* const* Wg_host, float* ins_out, float* seed_out,
+                       int B, int N, int D, int I, uint32_t io, void* stream);
+
+/* Question-side training (model(batch, training=True), gnn/train_model.py:222).  Same shapes as the forward entry
+ * points above (gr_instructions: I <= 8 and (Q D + (I+7) D + 2 Q) * 4 bytes <= 200 KB; gr_query_reform: D <= 1024,
+ * I <= 8 and (5I+1) D * 4 bytes <= 48 KB).  One CTA per question in every backward; each output element is owned by
+ * one question and written in a fixed order: no atomics, bit-reproducible.  The weight gradients are left to the
+ * caller as one GEMM per weight over the per-question operands written here (G = the pre-activation gradient, X =
+ * the layer's dropped input): grad_W = G^T X over the rows (b, i) (ca_linear: rows (b, i, q)), grad_b = column sums.
+ *
+ * gr_instructions_train: gr_instructions with the three linear_drop sites of get_instruction (base_encoder.py:85-98)
+ * drawn in the kernel.  Element (question b, step i, site s, token q, column c) is kept iff
+ * u = (Philox4x32-10(key = *seed, counter = (b, 4 i + s, q, c))[0] >> 8) * 2^-24 >= p, and kept elements are scaled
+ * by 1/(1-p).  Sites: s = 0 qnode before question_linear_i (q = 0, c < D); s = 1 [ri, q_i, q_i - ri, q_i * ri]
+ * before cq_linear (q = 0, c < 4D); s = 2 cq * hidden[q] before ca_linear (c < D).  seed: device int64[1]; p in
+ * [0, 1); p == 0 ignores the seed and runs gr_instructions' kernel (the same bits).  attn_out [B,I,Q] is required:
+ * the backward reads it.
+ * gr_instructions_dropout_mask: the masks of the three sites (1 = kept) for 0 < p < 1: mask_q [B,I,D],
+ * mask_cq [B,I,4D], mask_ca [B,I,Q,D] (the same device function).
+ * gr_instructions_backward: the forward's inputs, seed and p, its outputs ri [B,I,D] and attn [B,I,Q], and
+ * grad_out = dL/dri [B,I,D].  Writes (overwrites) grad_hidden [B,Q,D], grad_qnode [B,D] and the operands g_q, x_q
+ * [B,I,D] (question_linear_i), g_cq [B,I,D], x_cq [B,I,4D] (cq_linear), g_ca [B,I,Q], x_ca [B,I,Q,D] (ca_linear).
+ * The mask is redrawn from the seed, never stored.
+ * gr_query_reform_backward: the forward's inputs (h fp32, or bf16 with GR_IO_BF16) and grad_out = dL/dins_out
+ * [B,I,D].  Writes grad_ins [B,I,D] and the operands g_r, g_g [B,I,D] (fusion.r / fusion.g) and x_z [B,I,3D]
+ * (their input z = [x, y, x - y]); adds s_n * dL/dy to each seed row n of grad_h (row stride ldg, h's type), seeds
+ * in index order as in the forward.  No other row of grad_h is read or written. */
+int gr_instructions_train(const float* hidden, const float* qnode, const int64_t* qtext, int64_t pad_id,
+                          const float* const* Wq_host, const float* const* bq_host, const float* Wcq,
+                          const float* bcq, const float* wca, const float* bca, const int64_t* seed, double p,
+                          float* out, float* attn_out, int B, int Q, int D, int I, void* stream);
+int gr_instructions_dropout_mask(const int64_t* seed, double p, int B, int Q, int D, int I, uint8_t* mask_q,
+                                 uint8_t* mask_cq, uint8_t* mask_ca, void* stream);
+int gr_instructions_backward(const float* hidden, const float* qnode, const int64_t* qtext, int64_t pad_id,
+                             const float* const* Wq_host, const float* const* bq_host, const float* Wcq,
+                             const float* bcq, const float* wca, const float* bca, const int64_t* seed, double p,
+                             const float* ri, const float* attn, const float* grad_out, float* grad_hidden,
+                             float* grad_qnode, float* g_q, float* x_q, float* g_cq, float* x_cq, float* g_ca,
+                             float* x_ca, int B, int Q, int D, int I, void* stream);
+int gr_query_reform_backward(const float* seed_info, const void* h, int64_t ldh, const float* ins_in,
+                             const float* const* Wr_host, const float* const* Wg_host, const float* grad_out,
+                             float* grad_ins, void* grad_h, int64_t ldg, float* g_r, float* g_g, float* x_z, int B,
+                             int N, int D, int I, uint32_t io, void* stream);
 /* gr_kl_loss_pred: BaseModel.calc_loss_label with loss_type "kl" (gnn/models/base_model.py:186-215,
  * rearev.py:156-160,228-232) and pred = argmax_n dist[b,n] (lowest index on ties):
  * loss = sum_b valid_b * sum_n kl_div(log(dist+1e-8), teacher/len_b) / B.  loss_q: float[B] scratch/output. */

@@ -34,6 +34,8 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from . import ops
+
 VERY_NEG_NUMBER = -100000000000
 
 
@@ -120,7 +122,6 @@ class _AggregateFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, ins, prior, graph, direction, w):
-        from . import ops
         ctx.dtypes = (table.dtype, ins.dtype, prior.dtype)
         table, ins, prior = table.detach().float(), ins.detach().float(), prior.detach().float()
         out = ops.aggregate(graph, direction, prior, table, ins, w=w, dtype=_node_dtype())
@@ -131,7 +132,6 @@ class _AggregateFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
-        from . import ops
         table, ins, prior = ctx.saved_tensors
         # the kernel accumulates into dense row-major buffers: zeros_like alone would keep a transposed input's strides
         gt, gi, gp = (torch.zeros_like(t, memory_format=torch.contiguous_format) for t in (table, ins, prior))
@@ -147,7 +147,6 @@ class _TypeLayerFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, table, graph, w_t, w_h):
-        from . import ops
         out = torch.empty(graph.B * graph.N, table.shape[1], dtype=_node_dtype(), device=table.device)
         ops.type_layer(graph, table.detach().float(), out, w_t, w_h)
         ctx.save_for_backward(out)
@@ -157,7 +156,6 @@ class _TypeLayerFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
-        from . import ops
         out, = ctx.saved_tensors
         if grad_out.dtype != out.dtype:      # widening is exact: same gradients as with grad_out in out's dtype
             out, grad_out = out.float(), grad_out.float()
@@ -166,13 +164,10 @@ class _TypeLayerFn(torch.autograd.Function):
         return gt.to(ctx.dtype), None, None, None
 
 
-FACT_KERNEL_MAX_D = 512    # widths the TypeLayer / GraftNet training kernels cover; wider models keep the torch ops
-
-
 def _fact_kernels(device, D):
     """True when the TypeLayer and GraftNet's fact-level work run in the training kernels: CUDA, ``USE_KERNELS`` and
-    D <= FACT_KERNEL_MAX_D (the per-fact torch ops otherwise, as before those kernels existed)."""
-    return bool(USE_KERNELS and device.type == "cuda" and D <= FACT_KERNEL_MAX_D)
+    a width they admit (:func:`ops.fact_train_ok`); the per-fact torch ops otherwise."""
+    return bool(USE_KERNELS and device.type == "cuda" and ops.fact_train_ok(D))
 
 
 def _type_layer_graph(model, batch, device, D):
@@ -190,9 +185,9 @@ def _batch_graph(model, batch, device):
 
 
 def _kernel_graph(model, batch, device, D, I, graph=None):
-    """CSR of the batch for the aggregation kernels, or None (CPU tensors / shapes the backward kernel does not cover).
-    ``graph``: the batch's CSR if it was already staged (for the TypeLayer)."""
-    if not (USE_KERNELS and device.type == "cuda" and D <= 256 and I <= 4):
+    """CSR of the batch for the aggregation kernels, or None (CPU tensors / shapes the backward kernel does not admit,
+    :func:`ops.aggregate_backward_ok`).  ``graph``: the batch's CSR if it was already staged (for the TypeLayer)."""
+    if not (USE_KERNELS and device.type == "cuda" and ops.aggregate_backward_ok(D, I)):
         return None
     return graph if graph is not None else _batch_graph(model, batch, device)
 
@@ -215,20 +210,16 @@ def _neighbours(table_f, table_i, ins, dist, facts, graph, Nt):
     return torch.stack(reps, dim=1)
 
 
-INS_MAX_SMEM = 200 * 1024      # gr_instructions: (Q D + (I + 7) D + 2 Q) floats of shared memory
-REFORM_MAX_SMEM = 48 * 1024    # gr_query_reform: (5 I + 1) D floats
-
-
 def _instruction_kernels(device, Q, D, I):
     """True when the instruction steps run in gr_instructions_train / gr_instructions_backward: CUDA, ``USE_KERNELS``
-    and a shape gr_instructions admits."""
-    return bool(USE_KERNELS and device.type == "cuda" and I <= 8 and (Q * D + (I + 7) * D + 2 * Q) * 4 <= INS_MAX_SMEM)
+    and a shape gr_instructions admits (:func:`ops.instructions_ok`)."""
+    return bool(USE_KERNELS and device.type == "cuda" and ops.instructions_ok(Q, D, I))
 
 
 def _reform_kernels(device, D, I):
-    """True when the query reform runs in gr_query_reform_ex / gr_query_reform_backward: CUDA, ``USE_KERNELS`` and a
-    shape gr_query_reform admits."""
-    return bool(USE_KERNELS and device.type == "cuda" and I <= 8 and D <= 1024 and (5 * I + 1) * D * 4 <= REFORM_MAX_SMEM)
+    """True when the query reform runs in gr_query_reform(_ex) / gr_query_reform_backward: CUDA, ``USE_KERNELS`` and
+    a shape gr_query_reform admits (:func:`ops.query_reform_ok`)."""
+    return bool(USE_KERNELS and device.type == "cuda" and ops.query_reform_ok(D, I))
 
 
 def _weight_grads(G, X):
@@ -249,7 +240,6 @@ class _InstructionsFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, hidden, qnode, qtext, pad_id, seed, p, wca, bca, Wcq, bcq, *wq):
-        from . import ops
         ctx.dtypes = (hidden.dtype, qnode.dtype) + tuple(t.dtype for t in (wca, bca, Wcq, bcq) + wq)
         hidden, qnode = hidden.detach().float().contiguous(), qnode.detach().float().contiguous()
         wts = [t.detach().float().contiguous() for t in (wca, bca, Wcq, bcq) + wq]
@@ -258,13 +248,10 @@ class _InstructionsFn(torch.autograd.Function):
                                            seed, p)
         ctx.save_for_backward(hidden, qnode, qtext, seed, out, attn, *wts)
         ctx.pad_id, ctx.p = pad_id, p
-        ctx.det = torch.are_deterministic_algorithms_enabled()
-        ctx.amp = _autocast_bf16()
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        from . import ops
         hidden, qnode, qtext, seed, out, attn, *wts = ctx.saved_tensors
         wca, bca, Wcq, bcq = wts[:4]
         Wq, bq = wts[4::2], wts[5::2]
@@ -296,29 +283,25 @@ def _instructions_kernel(enc, hidden, qnode, q_input):
 
 class _QueryReformFn(torch.autograd.Function):
     """QueryReform + Fusion for every instruction (query_update.py:6-44, rearev.py:214-221): forward =
-    gr_query_reform_ex (one seed retrieve serves all I reforms), backward = gr_query_reform_backward, which adds the
+    gr_query_reform(_ex) (one seed retrieve serves all I reforms), backward = gr_query_reform_backward, which adds the
     seed-row gradient into a zero [B*N, D] grad_h in h's dtype (only the seed rows are written).  h is read in its own
     dtype (bf16 under bf16 autocast); everything else is fp32.  Inputs after the data: (Wr_j, Wg_j) of every reform."""
 
     @staticmethod
     def forward(ctx, seed_info, h, ins, B, N, *wts):
-        from . import ops
         ctx.dtypes = (h.dtype, ins.dtype) + tuple(t.dtype for t in wts)
         h = h.detach()
         if h.dtype not in (torch.float32, torch.bfloat16):
             h = h.float()
         ins = ins.detach().float().contiguous()
         wts = [t.detach().float().contiguous() for t in wts]
-        out = ops.query_reform_train(seed_info, h, ins, wts[0::2], wts[1::2], B, N)
+        out = ops.query_reform(seed_info, h, ins, wts[0::2], wts[1::2], B, N, op="question_train")
         ctx.save_for_backward(seed_info, h, ins, *wts)
         ctx.BN = (B, N)
-        ctx.det = torch.are_deterministic_algorithms_enabled()
-        ctx.amp = _autocast_bf16()
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        from . import ops
         seed_info, h, ins, *wts = ctx.saved_tensors
         B, N = ctx.BN
         grad_h = torch.zeros(h.shape, dtype=h.dtype, device=h.device)
@@ -386,7 +369,6 @@ def eval_metric(model, pred_dist, answer_dist, seed_dist, local_entity):
     if bool(h1.any()):
         seeds = (seed_dist > 0).float()
         if pred_dist.is_cuda:
-            from . import ops
             cand_idx, cand_count, _ = ops.rank_candidates(pred_dist.contiguous(), local_entity, seeds,
                                                           model.num_entity, model.eps)
         else:
@@ -553,7 +535,6 @@ class _GraftAttentionFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, qh, rel, qmask, gg):
-        from . import ops
         ctx.dtypes = (qh.dtype, rel.dtype)
         qh, rel, qmask = qh.detach().float(), rel.detach().float().contiguous(), qmask.float()
         W, _wt, _e = ops.graft_attention(gg, qh, qmask, rel, out_w=True)
@@ -564,7 +545,6 @@ class _GraftAttentionFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_W):
-        from . import ops
         qh, rel, qmask = ctx.saved_tensors
         gq = torch.zeros(qh.shape, dtype=torch.float32, device=qh.device)
         gr = torch.zeros(rel.shape, dtype=torch.float32, device=rel.device)
@@ -581,7 +561,6 @@ class _GraftAggregateFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, self_tab, head_tab, s, gg, seed, p):
-        from . import ops
         ctx.dtypes = (self_tab.dtype, head_tab.dtype, s.dtype)
         self_tab, s = self_tab.detach().float().contiguous(), s.detach().float()
         head_tab = head_tab.detach().to(_node_dtype()).contiguous()
@@ -593,7 +572,6 @@ class _GraftAggregateFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
-        from . import ops
         self_tab, head_tab, s, seed = ctx.saved_tensors
         if grad_out.dtype != head_tab.dtype:     # widening is exact: same gradients as with grad_out in head_tab's dtype
             head_tab, grad_out = head_tab.float(), grad_out.float()
@@ -618,7 +596,7 @@ def _graft_kernel_batch(model, batch, dev):
 def graftnet_forward(model, batch):
     """GraftNet forward with autograd (graftnet.py:135-183, graft_gnn.py:64-153) -> (loss, pred, pred_dist, [h1, f1]).
 
-    Kernel path (CUDA, ``USE_KERNELS``, D <= FACT_KERNEL_MAX_D): the fact attention, the fact messages and the TypeLayer run in the kernels of
+    Kernel path (CUDA, ``USE_KERNELS``, ``ops.fact_train_ok(D)``): the fact attention, the fact messages and the TypeLayer run in the kernels of
     csrc/graft.cu and csrc/aggregate*.cu with their own backward (_GraftAttentionFn, _GraftAggregateFn, _TypeLayerFn),
     so nothing of shape [facts, D] is formed or saved; kb_tail_linear is applied after the per-node sum (by linearity:
     sum_f kb_tail(v_f) = kb_tail.weight @ sum_f v_f + indeg * kb_tail.bias).  The per-fact scalars (W~, E, s, d') stay

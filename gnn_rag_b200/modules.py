@@ -123,7 +123,7 @@ class LSTMInstruction(nn.Module):
         emb = self.word_embedding(query_text)
         Bq = query_text.size(0)
         enc = self.node_encoder
-        if emb.is_cuda and self.entity_dim <= ops.LSTM_MAX_HIDDEN:
+        if emb.is_cuda and ops.lstm_ok(self.entity_dim):
             # input projection for all tokens at once (one GEMM), recurrence in one cluster kernel
             gx = F.linear(emb, enc.weight_ih_l0, enc.bias_ih_l0)
             hidden = ops.lstm_forward(gx, enc.weight_hh_l0, enc.bias_hh_l0)
@@ -288,7 +288,7 @@ class _GraphLayerBase(nn.Module):
 
     def _alloc(self, Nt, Kd, device):
         D = self.entity_dim
-        self.use_planes = bool(ops.TC_LINEAR) and 8 <= D <= ops.TC_MAX_N_SPLIT
+        self.use_planes = ops.tc_planes_ok(D, D)
         self.cur = 0
         self.Kd = Kd
         if self.use_planes:
@@ -545,7 +545,7 @@ class GraftLayer(nn.Module):
         """graft_gnn.py:45-61 + compute_attention (:64-87), which the reference runs at step 0.  ``rel``: fp32
         relation features [R1, D]."""
         D = self.entity_dim
-        if not (bool(ops.TC_LINEAR) and 8 <= D <= ops.TC_MAX_N_SPLIT):
+        if not ops.tc_planes_ok(D, D):
             raise NotImplementedError("GraftNet runs its GEMMs on the wgmma path: entity_dim must be in [8, %d]"
                                       % ops.TC_MAX_N_SPLIT)
         dev = db.local_entity.device

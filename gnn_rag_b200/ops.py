@@ -1,7 +1,11 @@
 """Tensor-level wrappers over the C ABI (include/gnnrag_b200.h): torch CUDA tensors in, torch CUDA tensors
 out.  torch is used for device memory and streams only; every op below launches our own sm_90a kernels.
-All ops raise if handed a CPU tensor -- there is no CPU fallback on the product path."""
+All ops raise if handed a CPU tensor -- there is no CPU fallback on the product path.
+
+Each kernel's shape rule (``*_ok``) sits next to its wrapper: the training path asks it to choose between a kernel and
+its torch restatement, and tests/test_entry_refusals_host.py holds it to the entry point's own refusals."""
 import ctypes
+import functools
 import weakref
 
 import numpy as np
@@ -40,43 +44,32 @@ class _Stats:
 STATS = _Stats()
 
 
-class _AggTimer:
-    def __init__(self, tag):
-        self.tag = tag
+class _Timer:
+    """CUDA events (on the launching stream) around one wrapper call: into ``STATS.op_events`` as op class ``op`` with
+    ``info`` when ``STATS.time_ops`` is on.  An aggregation tag ``agg`` makes the class "aggregation" with the tag as
+    info, and also goes into ``STATS.agg_events`` when ``STATS.time_agg`` is on.  Neither given: untimed."""
+
+    def __init__(self, op=None, info=None, agg=None):
+        if agg is not None:
+            op, info = "aggregation", agg
+        self.op, self.info, self.agg = op, info, agg
 
     def __enter__(self):
-        if STATS.time_agg or STATS.time_ops:
+        self.to_ops = self.op is not None and STATS.time_ops
+        self.to_agg = self.agg is not None and STATS.time_agg
+        if self.to_ops or self.to_agg:
             self.s = torch.cuda.Event(enable_timing=True)
             self.e = torch.cuda.Event(enable_timing=True)
             self.s.record()
         return self
 
     def __exit__(self, *a):
-        if STATS.time_agg or STATS.time_ops:
+        if self.to_ops or self.to_agg:
             self.e.record()
-            if STATS.time_agg:
-                STATS.agg_events.append((self.s, self.e, self.tag))
-            if STATS.time_ops:
-                STATS.op_events.append((self.s, self.e, "aggregation", self.tag))
-
-
-class _OpTimer:
-    """CUDA events (on the launching stream) around one wrapper call when ``STATS.time_ops`` is on."""
-
-    def __init__(self, cls, info=None):
-        self.cls, self.info = cls, info
-
-    def __enter__(self):
-        if STATS.time_ops:
-            self.s = torch.cuda.Event(enable_timing=True)
-            self.e = torch.cuda.Event(enable_timing=True)
-            self.s.record()
-        return self
-
-    def __exit__(self, *a):
-        if STATS.time_ops:
-            self.e.record()
-            STATS.op_events.append((self.s, self.e, self.cls, self.info))
+            if self.to_agg:
+                STATS.agg_events.append((self.s, self.e, self.agg))
+            if self.to_ops:
+                STATS.op_events.append((self.s, self.e, self.op, self.info))
 
 
 def _L():
@@ -85,6 +78,27 @@ def _L():
 
 def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _launch(name, *args, io=0, launches=1, op=None, info=None, agg=None):
+    """Call C entry point ``name`` with ``args`` and the current stream; with io flags its ``*_ex`` form, which takes
+    the flags before the stream.  Timed as :class:`_Timer` says (``op``, ``info``, ``agg``); raises on any refusal and
+    adds ``launches`` to ``STATS.launches``."""
+    fn = getattr(_L(), name + "_ex" if io else name)
+    args = (*args, io, _stream()) if io else (*args, _stream())
+    if (op is None and agg is None) or not (STATS.time_ops or STATS.time_agg):     # untimed: no per-call timer object
+        rc = fn(*args)
+    else:
+        with _Timer(op, info, agg):
+            rc = fn(*args)
+    _lib.check(rc)
+    STATS.launches += launches
+
+
+def _workspace(device, sizer, *sizes):
+    """(workspace, nbytes): an uninitialised device buffer of the bytes the size entry point ``sizer`` asks for."""
+    nbytes = getattr(_L(), sizer)(*sizes)
+    return torch.empty(nbytes, dtype=torch.uint8, device=device), nbytes
 
 
 def _p(t):
@@ -123,14 +137,6 @@ def _node_io(**tensors):
     return IO_BF16 if any(t.dtype == torch.bfloat16 for t in ts.values()) else 0
 
 
-def _call_io(L, name, io, *args):
-    """C entry point ``name`` (fp32 node-sized tensors) or, with io flags, its ``*_ex`` variant, which takes the flags
-    word before the stream (the last argument)."""
-    if not io:
-        return getattr(L, name)(*args)
-    return getattr(L, name + "_ex")(*args[:-1], io, args[-1])
-
-
 def set_option(name, value):
     _lib.check(_L().gr_set_option(name.encode(), int(value)))
 
@@ -162,6 +168,12 @@ class CsrGraph:
         self.nfacts = None                # device int32[1] live fact count when F is a capacity
         self.rel_index = {}               # direction -> relation index of that CSR (deterministic backward)
 
+    def csr(self, direction):
+        """(rowptr, src, rel, fact) of one destination CSR: 'fwd' = the tail CSR, 'inv' = the head CSR."""
+        if direction == "fwd":
+            return self.rowptr_t, self.src_t, self.rel_t, self.fact_t
+        return self.rowptr_h, self.src_h, self.rel_h, self.fact_h
+
     def check_status(self):
         if int(self.status.item()) != 0:
             raise RuntimeError("fact list contains node/relation ids outside the batch (clamped)")
@@ -176,17 +188,13 @@ def csr_build(heads, rels, tails, B, N, R1, nfacts=None):
         raise RuntimeError("fact arrays must share dtype int64 or int32")
     F = heads.numel()
     g = CsrGraph(B, N, F, R1, heads.device)
-    L = _L()
-    ws_bytes = L.gr_csr_build_workspace_bytes(F, B * N)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=heads.device)
-    with _OpTimer("csr_build"):
-        rc = L.gr_csr_build(_p(heads.contiguous()), _p(rels.contiguous()), _p(tails.contiguous()),
-                            heads.element_size(), F, B * N, R1,
-                            _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t),
-                            _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h),
-                            _p(g.status), _p(nfacts), _p(ws), ws_bytes, _stream())
-    _lib.check(rc)
-    STATS.launches += 9 if F > 0 else 5     # memsets excluded: hist, 3x scan, place, 2x sort, fill (+gather)
+    ws, ws_bytes = _workspace(heads.device, "gr_csr_build_workspace_bytes", F, B * N)
+    # memsets excluded: hist, 3x scan, place, 2x sort, fill (+gather)
+    _launch("gr_csr_build", _p(heads.contiguous()), _p(rels.contiguous()), _p(tails.contiguous()),
+            heads.element_size(), F, B * N, R1,
+            _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t),
+            _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h),
+            _p(g.status), _p(nfacts), _p(ws), ws_bytes, launches=9 if F > 0 else 5, op="csr_build")
     g.nfacts = nfacts
     return g
 
@@ -204,11 +212,10 @@ def csr_relation_index(g, direction):
     the graph: (rix_ptr [R1+1], rix_slot = that CSR's slots sorted by (relation, slot), row_of = the row of every
     slot)."""
     if direction not in g.rel_index:
-        rp, rel = (g.rowptr_t, g.rel_t) if direction == "fwd" else (g.rowptr_h, g.rel_h)
+        rp, _src, rel, _fact = g.csr(direction)
         rix_ptr, rix_slot = _relation_index(rel[: g.F], g.R1, g.nfacts)
         row_of = torch.empty(max(pad4(g.F), 4), dtype=torch.int32, device=rp.device)
-        _lib.check(_L().gr_csr_row_of(_p(rp), g.B * g.N, _p(row_of), _stream()))
-        STATS.launches += 1
+        _launch("gr_csr_row_of", _p(rp), g.B * g.N, _p(row_of))
         g.rel_index[direction] = (rix_ptr, rix_slot, row_of)
     return g.rel_index[direction]
 
@@ -217,8 +224,7 @@ def gather_f32(values, fact):
     values = _cuda(values, torch.float32, "values")
     F = values.numel()
     out = torch.empty(max(pad4(F), 4), dtype=torch.float32, device=values.device)
-    _lib.check(_L().gr_gather_f32(_p(values), _p(fact), _p(out), F, _stream()))
-    STATS.launches += 1
+    _launch("gr_gather_f32", _p(values), _p(fact), _p(out), F)
     return out
 
 
@@ -232,19 +238,29 @@ def linear(A, W, bias=None, relu=False, out=None, addend=None, addend_rows=0, ex
         out = torch.empty(M, N, dtype=torch.float32, device=A.device)
     assert out.shape == (M, N) and out.stride(1) == 1
     flags = (LINEAR_RELU if relu else 0) | (LINEAR_EXACT_FP32 if exact else 0)
-    rc = _L().gr_linear(_p(A), A.stride(0), _p(W), W.stride(0), _p(bias), _p(addend),
-                        addend.stride(0) if addend is not None else 0, addend_rows,
-                        _p(out), out.stride(0), M, N, K, flags, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_linear", _p(A), A.stride(0), _p(W), W.stride(0), _p(bias), _p(addend),
+            addend.stride(0) if addend is not None else 0, addend_rows, _p(out), out.stride(0), M, N, K, flags)
     return out
 
 
 TC_LINEAR = True       # route the big e2e linears through the wgmma split-bf16 kernel (models use this)
+TC_MAX_N = 256         # output columns of one wgmma GEMM launch (the register accumulator of a consumer warpgroup)
+TC_MAX_N_SPLIT = 512   # wider outputs are tiled over N: one launch per <= 256-column slice of W
+
+
+def tc_linear_ok(N, K):
+    """True when ``TC_LINEAR`` is on and gr_linear_tc admits an [N, K] weight: 8 <= N <= 256, K >= 8."""
+    return bool(TC_LINEAR) and 8 <= N <= TC_MAX_N and K >= 8
+
+
+def tc_planes_ok(N, K):
+    """True when ``TC_LINEAR`` is on and :func:`linear_tc_planes` takes an [N, K] weight: 8 <= N <= 512 (wider than
+    256 through column slices), K >= 8."""
+    return bool(TC_LINEAR) and 8 <= N <= TC_MAX_N_SPLIT and K >= 8
 
 
 def linear_tc(A, W, bias=None, relu=False, out=None):
-    """Tensor-core (wgmma, split-bf16 x3) version of :func:`linear` for 8 <= N <= 256."""
+    """Tensor-core (wgmma, split-bf16 x3) version of :func:`linear` for the shapes :func:`tc_linear_ok` admits."""
     A, W = _cuda(A, torch.float32, "A"), _cuda(W, torch.float32, "W")
     M, K = A.shape
     N = W.shape[0]
@@ -252,13 +268,9 @@ def linear_tc(A, W, bias=None, relu=False, out=None):
     if out is None:
         out = torch.empty(M, N, dtype=torch.float32, device=A.device)
     assert out.shape == (M, N) and out.stride(1) == 1
-    L = _L()
-    nbytes = L.gr_linear_tc_workspace_bytes(M, N, K)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=A.device)
-    rc = L.gr_linear_tc(_p(A), A.stride(0), _p(W), W.stride(0), _p(bias), _p(out), out.stride(0),
-                        M, N, K, LINEAR_RELU if relu else 0, _p(ws), nbytes, _stream())
-    _lib.check(rc)
-    STATS.launches += 3
+    ws, nbytes = _workspace(A.device, "gr_linear_tc_workspace_bytes", M, N, K)
+    _launch("gr_linear_tc", _p(A), A.stride(0), _p(W), W.stride(0), _p(bias), _p(out), out.stride(0),
+            M, N, K, LINEAR_RELU if relu else 0, _p(ws), nbytes, launches=3)
     return out
 
 
@@ -266,14 +278,14 @@ def rel_linear(A, W, bias=None, addend=None, addend_rows=0):
     """Hoisted relation projection table = A W^T + b (+ pos_emb rows): wgmma split-bf16 path when enabled
     (fp32-class accuracy, ~3x faster than the SIMT kernel at [6107 x 200 x 200]); the optional pos_emb addend
     keeps the exact SIMT kernel."""
-    if TC_LINEAR and addend is None and 8 <= W.shape[0] <= 256 and W.shape[1] >= 8:
+    if addend is None and tc_linear_ok(*W.shape):
         return linear_tc(A, W, bias, relu=False)
     return linear(A, W, bias, addend=addend, addend_rows=addend_rows)
 
 
 def e2e_linear(A, W, bias, out):
     """relu(A W^T + b) for the node-update GEMM: wgmma path when enabled and the shape fits."""
-    if TC_LINEAR and 8 <= W.shape[0] <= 256 and W.shape[1] >= 8:
+    if tc_linear_ok(*W.shape):
         return linear_tc(A, W, bias, relu=True, out=out)
     return linear(A, W, bias, relu=True, out=out)
 
@@ -294,16 +306,16 @@ def aggregate(g, direction, prior, table, ins, out=None, out_col0=0, seg_stride=
         out = torch.empty(B * N, I * seg_stride + out_col0, dtype=dtype, device=prior.device)
     io = _node_io(out=out)
     assert out.stride(1) == 1
-    if direction == "fwd":
-        rp, src, rel = g.rowptr_t, g.src_t, g.rel_t
-    else:
-        rp, src, rel = g.rowptr_h, g.src_h, g.rel_h
-    with _AggTimer(("single", I)):
-        rc = _call_io(_L(), "gr_aggregate", io, _p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table), _p(ins),
-                      _p(out), out.stride(0), out_col0, seg_stride, _p(possible), B, N, D, I, g.F, _stream())
-    _lib.check(rc)
-    STATS.launches += (I + 3) // 4
+    rp, src, rel, _fact = g.csr(direction)
+    _launch("gr_aggregate", _p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table), _p(ins), _p(out), out.stride(0),
+            out_col0, seg_stride, _p(possible), B, N, D, I, g.F, io=io, launches=(I + 3) // 4, agg=("single", I))
     return out
+
+
+def aggregate_backward_ok(D, I):
+    """True when gr_aggregate_backward (and its _det form) admits width D and I instructions: 0 < D <= 256,
+    0 < I <= 4."""
+    return 0 < D <= 256 and 0 < I <= 4
 
 
 def aggregate_backward(g, direction, prior, table, ins, grad_out, grad_table, grad_ins, grad_prior, w=None,
@@ -317,28 +329,20 @@ def aggregate_backward(g, direction, prior, table, ins, grad_out, grad_table, gr
     io = _node_io(grad_out=grad_out)
     B, I, D = ins.shape
     assert grad_out.stride(1) == 1 and grad_table.is_contiguous() and grad_ins.is_contiguous() and grad_prior.is_contiguous()
-    rp, src, rel = (g.rowptr_t, g.src_t, g.rel_t) if direction == "fwd" else (g.rowptr_h, g.src_h, g.rel_h)
+    rp, src, rel, fact = g.csr(direction)
     if deterministic:
         assert grad_table.shape[0] >= g.R1
         rix_ptr, rix_slot, row_of = csr_relation_index(g, direction)
-        fact, rp_o, fact_o = (g.fact_t, g.rowptr_h, g.fact_h) if direction == "fwd" else (g.fact_h, g.rowptr_t, g.fact_t)
-        L = _L()
-        nbytes = L.gr_aggregate_backward_det_workspace_bytes(B, g.N, D, I, g.F)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=prior.device)
-        with _OpTimer("aggregation_bwd_det"):
-            rc = _call_io(L, "gr_aggregate_backward_det", io, _p(rp), _p(src), _p(rel), _p(fact), _p(w), _p(prior),
-                          _p(table), _p(ins), _p(grad_out), grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins),
-                          _p(grad_prior), B, g.N, D, I, g.F, _p(rp_o), _p(fact_o), _p(rix_ptr), _p(rix_slot),
-                          _p(row_of), g.R1, _p(ws), nbytes, _stream())
-        _lib.check(rc)
-        STATS.launches += 5 if g.F > 0 else 0
+        rp_o, _src, _rel, fact_o = g.csr("inv" if direction == "fwd" else "fwd")
+        ws, nbytes = _workspace(prior.device, "gr_aggregate_backward_det_workspace_bytes", B, g.N, D, I, g.F)
+        _launch("gr_aggregate_backward_det", _p(rp), _p(src), _p(rel), _p(fact), _p(w), _p(prior), _p(table), _p(ins),
+                _p(grad_out), grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins), _p(grad_prior), B, g.N, D, I,
+                g.F, _p(rp_o), _p(fact_o), _p(rix_ptr), _p(rix_slot), _p(row_of), g.R1, _p(ws), nbytes, io=io,
+                launches=5 if g.F > 0 else 0, op="aggregation_bwd_det")
         return
-    with _OpTimer("aggregation_bwd"):
-        rc = _call_io(_L(), "gr_aggregate_backward", io, _p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table),
-                      _p(ins), _p(grad_out), grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins), _p(grad_prior),
-                      B, g.N, D, I, g.F, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_aggregate_backward", _p(rp), _p(src), _p(rel), _p(w), _p(prior), _p(table), _p(ins), _p(grad_out),
+            grad_out.stride(0), 0, D, _p(grad_table), _p(grad_ins), _p(grad_prior), B, g.N, D, I, g.F, io=io,
+            op="aggregation_bwd")
 
 
 def aggregate_dual(g, prior, table_fwd, table_inv, ins, out, out_col0, w_t=None, w_h=None, planes=None,
@@ -352,15 +356,12 @@ def aggregate_dual(g, prior, table_fwd, table_inv, ins, out, out_col0, w_t=None,
     assert table_fwd.is_contiguous() and table_inv.is_contiguous()
     assert out is None or out.stride(1) == 1
     hi, lo = planes if planes is not None else (None, None)
-    with _AggTimer(("dual", I)):
-        rc = _L().gr_aggregate_dual(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
-                                    _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h),
-                                    _p(prior), _p(table_fwd), _p(table_inv), _p(ins), _p(out),
-                                    out.stride(0) if out is not None else 0, out_col0, seg_pitch,
-                                    _p(hi), _p(lo), hi.stride(0) if hi is not None else 0,
-                                    B, g.N, D, I, g.F, _stream())
-    _lib.check(rc)
-    STATS.launches += (I + 3) // 4
+    _launch("gr_aggregate_dual", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
+            _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h),
+            _p(prior), _p(table_fwd), _p(table_inv), _p(ins), _p(out),
+            out.stride(0) if out is not None else 0, out_col0, seg_pitch,
+            _p(hi), _p(lo), hi.stride(0) if hi is not None else 0,
+            B, g.N, D, I, g.F, launches=(I + 3) // 4, agg=("dual", I))
     return out
 
 
@@ -374,9 +375,7 @@ def pad_table256(table):
     rows, D = table.shape
     assert table.stride(1) == 1
     pn = torch.empty(rows, 256, dtype=torch.float32, device=table.device)
-    with _OpTimer("table_prep"):
-        _lib.check(_L().gr_pad_table256(_p(table), table.stride(0), rows, D, _p(pn), _stream()))
-    STATS.launches += 1
+    _launch("gr_pad_table256", _p(table), table.stride(0), rows, D, _p(pn), op="table_prep")
     return pn
 
 
@@ -399,14 +398,10 @@ def aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, out_col0, seg_pitc
     dev = prior.device
     if dev not in _TILE_COUNTER:
         _TILE_COUNTER[dev] = torch.zeros(1, dtype=torch.int32, device=dev)
-    with _AggTimer(("dual", I)):
-        rc = _L().gr_aggregate_dual_abs(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
-                                       _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h),
-                                       _p(prior), _p(pn_fwd), _p(pn_inv), pn_fwd.shape[0], _p(ins), _p(hi), _p(lo),
-                                       hi.stride(0),
-                                       out_col0, seg_pitch, B, g.N, D, I, g.F, _p(_TILE_COUNTER[dev]), _stream())
-    _lib.check(rc)
-    STATS.launches += (I + 3) // 4
+    _launch("gr_aggregate_dual_abs", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
+            _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h),
+            _p(prior), _p(pn_fwd), _p(pn_inv), pn_fwd.shape[0], _p(ins), _p(hi), _p(lo), hi.stride(0),
+            out_col0, seg_pitch, B, g.N, D, I, g.F, _p(_TILE_COUNTER[dev]), launches=(I + 3) // 4, agg=("dual", I))
 
 
 FUSED_LAYER = True      # dense-prior ReaRev layers: aggregation fused into the e2e GEMM (csrc/fused_layer.cu)
@@ -424,14 +419,9 @@ def fused_ell(g, w_t=None, w_h=None):
     key = "_ell_w" if w_t is not None else "_ell"
     ell = getattr(g, key, None)
     if ell is None:
-        L = _L()
-        nbytes = L.gr_fused_ell_bytes(g.B, g.N, g.F)
-        ell = torch.empty(nbytes, dtype=torch.uint8, device=g.rowptr_t.device)
-        with _OpTimer("csr_build"):
-            _lib.check(L.gr_fused_ell_build(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
-                                            _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h),
-                                            g.B, g.N, g.F, _p(ell), nbytes, _stream()))
-        STATS.launches += 1
+        ell, nbytes = _workspace(g.rowptr_t.device, "gr_fused_ell_bytes", g.B, g.N, g.F)
+        _launch("gr_fused_ell_build", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
+                _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h), g.B, g.N, g.F, _p(ell), nbytes, op="csr_build")
         setattr(g, key, ell)
     return ell
 
@@ -448,21 +438,19 @@ def fused_layer(g, prior, pn_fwd, pn_inv, ins, h_planes, seg_pitch, W, bias, out
     n_out = W.shape[0]
     assert pn_fwd.is_contiguous() and pn_inv.is_contiguous() and hi.stride(0) == lo.stride(0)
     assert W.stride(1) == 1 and W.shape[1] == (2 * I + 1) * D
-    L = _L()
-    nbytes = L.gr_fused_layer_workspace_bytes(D, seg_pitch, I, n_out)
+    nbytes = _L().gr_fused_layer_workspace_bytes(D, seg_pitch, I, n_out)
     ws, presplit = _weight_ws(W, n_out, W.shape[1], "fused", seg_pitch, nbytes)
     ell = fused_ell(g, w_t, w_h)
     chi, clo = out_planes if out_planes is not None else (None, None)
     flags = (LINEAR_RELU if relu else 0) | (LINEAR_W_PRESPLIT if presplit else 0)
-    with _OpTimer("fused_layer"):
-        rc = L.gr_fused_layer(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
-                              _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h),
-                              _p(prior), _p(pn_fwd), _p(pn_inv), _p(ins), _p(hi), _p(lo), hi.stride(0), seg_pitch,
-                              _p(W), W.stride(0), _p(bias), _p(out), out.stride(0) if out is not None else 0,
-                              _p(chi), _p(clo), chi.stride(0) if chi is not None else 0, _p(w_score), _p(dots),
-                              B, g.N, D, I, n_out, g.F, flags, _p(ws), ws.numel(), _p(ell), ell.numel(), _stream())
-    _lib.check(rc)
-    STATS.launches += 2 if (w_t is not None or w_h is not None) else 1     # weighted graphs: + the coefficient pass
+    _launch("gr_fused_layer", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
+            _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h),
+            _p(prior), _p(pn_fwd), _p(pn_inv), _p(ins), _p(hi), _p(lo), hi.stride(0), seg_pitch,
+            _p(W), W.stride(0), _p(bias), _p(out), out.stride(0) if out is not None else 0,
+            _p(chi), _p(clo), chi.stride(0) if chi is not None else 0, _p(w_score), _p(dots),
+            B, g.N, D, I, n_out, g.F, flags, _p(ws), ws.numel(), _p(ell), ell.numel(),
+            launches=2 if (w_t is not None or w_h is not None) else 1,     # weighted graphs: + the coefficient pass
+            op="fused_layer")
     return out
 
 
@@ -474,12 +462,9 @@ def type_layer(g, table, out, w_t=None, w_h=None, planes=None):
     io = _node_io(out=out)
     assert out is None or out.stride(1) == 1
     hi, lo = planes if planes is not None else (None, None)
-    with _OpTimer("type_layer"):
-        rc = _call_io(_L(), "gr_type_layer", io, _p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.rel_h),
-                      _p(w_h), _p(table), _p(out), out.stride(0) if out is not None else 0,
-                      _p(hi), _p(lo), hi.stride(0) if hi is not None else 0, g.B, g.N, D, g.F, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_type_layer", _p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.rel_h), _p(w_h), _p(table),
+            _p(out), out.stride(0) if out is not None else 0, _p(hi), _p(lo), hi.stride(0) if hi is not None else 0,
+            g.B, g.N, D, g.F, io=io, op="type_layer")
     return out
 
 
@@ -488,82 +473,78 @@ def split_bf16(A, hi, lo):
     A = _cuda(A, torch.float32, "A")
     M, K = A.shape
     assert A.stride(1) == 1 and hi.stride(1) == 1 and hi.stride(0) == lo.stride(0)
-    _lib.check(_L().gr_split_bf16(_p(A), A.stride(0), M, K, _p(hi), _p(lo), hi.stride(0), _stream()))
-    STATS.launches += 1
+    _launch("gr_split_bf16", _p(A), A.stride(0), M, K, _p(hi), _p(lo), hi.stride(0))
 
 
-WEIGHT_CACHE = True    # keep the bf16 hi/lo split of a weight matrix until its tensor version changes
-_W_CACHE = {}          # (ptr, ldw, N, K, k_seg, pitch) -> [workspace, version, weakref(base tensor)]
-_P_CACHE = {}          # ptr -> [hi, lo, version, weakref(tensor)]
+WEIGHT_CACHE = True    # keep pre-formatted weights (bf16 hi/lo splits) until their tensor version changes
+_CACHE = {}            # key -> [buffers (tuple of tensors), owner version, weakref(owner tensor)]
 
 
 def _base(t):
     return t._base if t._base is not None else t
 
 
-def _weight_ws(W, N, K, k_seg, k_seg_pitch, nbytes):
-    """Workspace holding W's split planes + whether it is still valid (weight pre-formatting: the conversion
-    runs once per weight VERSION, so an in-place update / load_state_dict re-splits on the next call)."""
+def _cached(key, owner, fits, make):
+    """(buffers, current): device buffers pre-formatted from tensor ``owner`` (conversion runs once per VERSION, so an
+    in-place update / load_state_dict re-formats on the next call).  The entry of ``key`` is reused while it belongs
+    to the same ``owner`` object and ``fits(buffers)``; ``current`` says whether it still holds owner's ``_version``
+    (False: the caller rewrites the buffers).  Otherwise ``make()`` gives new buffers.  While a CUDA graph is being
+    captured nothing is inserted or refreshed: a stale or missing entry gets new buffers the cache does not keep."""
     capturing = torch.cuda.is_current_stream_capturing()
-    key = (W.data_ptr(), W.stride(0), N, K, k_seg, k_seg_pitch)
-    ent = _W_CACHE.get(key) if WEIGHT_CACHE else None
-    if ent is not None and ent[2]() is _base(W) and ent[0].numel() >= nbytes:
-        if ent[1] == W._version:
+    ent = _CACHE.get(key) if WEIGHT_CACHE else None
+    if ent is not None and ent[2]() is owner and fits(ent[0]):
+        if ent[1] == owner._version:
             return ent[0], True
         if not capturing:
-            ent[1] = W._version
-            return ent[0], False          # same buffer, re-split
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=W.device)
+            ent[1] = owner._version
+            return ent[0], False          # same buffers, re-formatted by the caller
+    buffers = make()
     if WEIGHT_CACHE and not capturing:
-        if len(_W_CACHE) > 512:          # models that were dropped: release the workspaces of dead weights
-            for k in [k for k, e in _W_CACHE.items() if e[2]() is None]:
-                del _W_CACHE[k]
-        _W_CACHE[key] = [ws, W._version, weakref.ref(_base(W))]
-    return ws, False
+        if len(_CACHE) > 512:            # models that were dropped: release the buffers of dead tensors
+            for k in [k for k, e in _CACHE.items() if e[2]() is None]:
+                del _CACHE[k]
+        _CACHE[key] = [buffers, owner._version, weakref.ref(owner)]
+    return buffers, False
+
+
+def _weight_ws(W, N, K, k_seg, k_seg_pitch, nbytes):
+    """Workspace holding W's split planes + whether it is still valid (weight pre-formatting)."""
+    (ws,), presplit = _cached(("ws", W.data_ptr(), W.stride(0), N, K, k_seg, k_seg_pitch), _base(W),
+                              lambda b: b[0].numel() >= nbytes,
+                              lambda: (torch.empty(nbytes, dtype=torch.uint8, device=W.device),))
+    return ws, presplit
 
 
 def param_planes(P):
     """bf16 hi/lo planes [M, round_up(K, 64)] of a parameter matrix used as a GEMM A operand (relation embedding
     tables), cached per tensor version like the weight split."""
     M, K = P.shape
-    capturing = torch.cuda.is_current_stream_capturing()
-    ent = _P_CACHE.get(P.data_ptr()) if WEIGHT_CACHE else None
-    if ent is not None and ent[3]() is P and ent[0].shape[0] == M and ent[2] == P._version:
-        return ent[0], ent[1]
-    if ent is not None and ent[3]() is P and ent[0].shape[0] == M and not capturing:
-        hi, lo = ent[0], ent[1]
-        ent[2] = P._version
-    else:
-        Kp = (K + 63) // 64 * 64
-        hi = torch.zeros(M, Kp, dtype=torch.bfloat16, device=P.device)
-        lo = torch.zeros(M, Kp, dtype=torch.bfloat16, device=P.device)
-        if WEIGHT_CACHE and not capturing:
-            _P_CACHE[P.data_ptr()] = [hi, lo, P._version, weakref.ref(P)]
-    split_bf16(P.detach(), hi, lo)
+    Kp = (K + 63) // 64 * 64
+    (hi, lo), current = _cached(("planes", P.data_ptr()), P, lambda b: b[0].shape[0] == M,
+                                lambda: tuple(torch.zeros(M, Kp, dtype=torch.bfloat16, device=P.device)
+                                              for _ in range(2)))
+    if not current:
+        split_bf16(P.detach(), hi, lo)
     return hi, lo
 
 
 def clear_weight_cache():
     """Drop the cached pre-formatted weights.  Captured CUDA graphs keep their own references to the workspaces they
     read (:func:`live_weight_workspaces`), so clearing the cache never frees memory a graph replay still uses.
-    Note: the caches are validated by ``tensor._version``; in-place writes through ``.data`` (``p.data.copy_``,
+    Note: the cache is validated by ``tensor._version``; in-place writes through ``.data`` (``p.data.copy_``,
     ``p.data.mul_``) do not bump it -- call this function after such updates."""
-    _W_CACHE.clear()
-    _P_CACHE.clear()
+    _CACHE.clear()
 
 
 def live_weight_workspaces():
     """Strong references to every cached pre-formatted weight buffer (held by GraphedStep entries)."""
-    return [e[0] for e in _W_CACHE.values()] + [t for e in _P_CACHE.values() for t in e[:2]]
-
-
-TC_MAX_N = 256         # output columns of one wgmma GEMM launch (the register accumulator of a consumer warpgroup)
-TC_MAX_N_SPLIT = 512   # wider outputs are tiled over N: one launch per <= 256-column slice of W
+    return [t for e in _CACHE.values() for t in e[0]]
 
 
 def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=None, dots=None, relu=True,
                      k_seg=0, k_seg_pitch=0, single_ok=False):
-    """wgmma split-bf16 GEMM whose A operand already lives in bf16 hi/lo planes [M, >=K].
+    """wgmma split-bf16 GEMM whose A operand already lives in bf16 hi/lo planes [M, >=K] (shapes:
+    :func:`tc_planes_ok`).
     ``single_ok``: this call may run as ONE bf16 product when ``ACT_BF16`` is on (the node-update GEMMs; the small
     relation-table GEMMs always keep the three-product fp32-class path).
     Writes any of: fp32 ``out`` [M,N]; ``out_planes`` (hi, lo) [M, >=N] (next layer's h columns);
@@ -594,20 +575,16 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
     else:
         assert W.shape[1] == K
     assert W.stride(1) == 1
-    L = _L()
-    nbytes = L.gr_linear_tc_planes_workspace_bytes(N, K)
+    nbytes = _L().gr_linear_tc_planes_workspace_bytes(N, K)
     ws, presplit = _weight_ws(W, N, K, k_seg, k_seg_pitch, nbytes)
     chi, clo = out_planes if out_planes is not None else (None, None)
     flags = (LINEAR_RELU if relu else 0) | (LINEAR_W_PRESPLIT if presplit else 0) | \
         (LINEAR_BF16_SINGLE if (ACT_BF16 and single_ok) else 0)
-    with _OpTimer("gemm_tc", (M, N, K)):
-        rc = L.gr_linear_tc_planes(_p(a_hi), _p(a_lo), a_hi.stride(0), _p(W), W.stride(0), _p(bias),
-                                   _p(out), out.stride(0) if out is not None else 0,
-                                   _p(chi), _p(clo), chi.stride(0) if chi is not None else 0,
-                                   _p(w_score), _p(dots), M, N, K, k_seg, k_seg_pitch,
-                                   flags, _p(ws), nbytes, _stream())
-    _lib.check(rc)
-    STATS.launches += 1 if presplit else 2
+    _launch("gr_linear_tc_planes", _p(a_hi), _p(a_lo), a_hi.stride(0), _p(W), W.stride(0), _p(bias),
+            _p(out), out.stride(0) if out is not None else 0,
+            _p(chi), _p(clo), chi.stride(0) if chi is not None else 0,
+            _p(w_score), _p(dots), M, N, K, k_seg, k_seg_pitch, flags, _p(ws), nbytes,
+            launches=1 if presplit else 2, op="gemm_tc", info=(M, N, K))
     return out
 
 
@@ -634,16 +611,12 @@ class RelFeatures:
         return slice(d * self.R1, (d + 1) * self.R1)
 
 
-def _tc_ok(n_out, k_in):
-    return bool(TC_LINEAR) and 8 <= n_out <= TC_MAX_N_SPLIT and k_in >= 8
-
-
 def rel_features_from_embeddings(embs, W, bias):
     """relation_linear applied to the relation embedding table(s) (rearev.py:91-99 / nsm.py:97-104):
     one wgmma GEMM per direction straight into the stacked planes (no fp32 round trip)."""
     R1, K = embs[0].shape
     D = W.shape[0]
-    planes = _tc_ok(D, K) and _tc_ok(D, D)
+    planes = tc_planes_ok(D, K) and tc_planes_ok(D, D)
     rf = RelFeatures(R1, D, len(embs), W.device, planes)
     for d, E in enumerate(embs):
         if planes:
@@ -657,7 +630,7 @@ def rel_features_from_embeddings(embs, W, bias):
 def rel_features_from_tensors(feats):
     """Relation features computed elsewhere in fp32 (relation-text encoder, rearev.py:100-111)."""
     R1, D = feats[0].shape
-    planes = _tc_ok(D, D)
+    planes = tc_planes_ok(D, D)
     rf = RelFeatures(R1, D, len(feats), feats[0].device, planes)
     for d, f in enumerate(feats):
         if planes:
@@ -692,10 +665,8 @@ SPARSE_PRIOR_FASTPATH = True   # first layer of every ReaRev iteration (seed pri
 def frontier_rows(g, prior, rows, count):
     """rows/count <- destination rows with at least one in-edge (either direction) from a node with prior != 0."""
     prior = _cuda(prior, torch.float32, "prior").contiguous()
-    with _OpTimer("frontier"):
-        _lib.check(_L().gr_frontier_rows(_p(g.rowptr_t), _p(g.src_t), _p(g.rowptr_h), _p(g.src_h), _p(prior),
-                                         g.B * g.N, _p(rows), _p(count), _stream()))
-    STATS.launches += 1
+    _launch("gr_frontier_rows", _p(g.rowptr_t), _p(g.src_t), _p(g.rowptr_h), _p(g.src_h), _p(prior), g.B * g.N,
+            _p(rows), _p(count), op="frontier")
 
 
 def frontier_fixup(g, prior, table_fwd, table_inv, ins, cur_planes, W, bias, w_score, nxt_planes, h32, dots,
@@ -707,14 +678,10 @@ def frontier_fixup(g, prior, table_fwd, table_inv, ins, cur_planes, W, bias, w_s
     chi, clo = cur_planes
     nhi, nlo = nxt_planes
     assert W.stride(1) == 1 and table_fwd.is_contiguous() and table_inv.is_contiguous()
-    with _OpTimer("frontier"):
-        rc = _L().gr_frontier_fixup(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.src_h),
-                                    _p(g.rel_h), _p(w_h), _p(prior), _p(table_fwd), _p(table_inv), _p(ins),
-                                    _p(chi), _p(clo), chi.stride(0), _p(W), W.stride(0), _p(bias), _p(w_score),
-                                    _p(nhi), _p(nlo), nhi.stride(0), _p(h32), _p(dots), _p(rows), _p(count),
-                                    B, g.N, D, I, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_frontier_fixup", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.src_h),
+            _p(g.rel_h), _p(w_h), _p(prior), _p(table_fwd), _p(table_inv), _p(ins),
+            _p(chi), _p(clo), chi.stride(0), _p(W), W.stride(0), _p(bias), _p(w_score),
+            _p(nhi), _p(nlo), nhi.stride(0), _p(h32), _p(dots), _p(rows), _p(count), B, g.N, D, I, op="frontier")
 
 
 def masked_softmax(dots, b_score, mask, B, N):
@@ -722,10 +689,8 @@ def masked_softmax(dots, b_score, mask, B, N):
     ``dots`` = the [2, B*N] partial score dots of :func:`linear_tc_planes`."""
     dist = torch.empty(B, N, dtype=torch.float32, device=dots.device)
     d = dots.view(2, -1)
-    with _OpTimer("softmax"):
-        _lib.check(_L().gr_masked_softmax(_p(d[0]), _p(d[1]), _p(b_score), _p(mask.contiguous()), _p(dist), B, N,
-                                          _stream()))
-    STATS.launches += 1
+    _launch("gr_masked_softmax", _p(d[0]), _p(d[1]), _p(b_score), _p(mask.contiguous()), _p(dist), B, N,
+            op="softmax")
     return dist
 
 
@@ -735,10 +700,8 @@ def score_softmax(h, w_score, b_score, mask, B, N, logits_out=None):
     D = w_score.numel()
     assert h.stride(1) == 1
     dist = torch.empty(B, N, dtype=torch.float32, device=h.device)
-    rc = _L().gr_score_softmax(_p(h), h.stride(0), _p(w_score.contiguous()), _p(b_score),
-                               _p(mask.contiguous()), _p(dist), _p(logits_out), B, N, D, _stream())
-    _lib.check(rc)
-    STATS.launches += 2
+    _launch("gr_score_softmax", _p(h), h.stride(0), _p(w_score.contiguous()), _p(b_score),
+            _p(mask.contiguous()), _p(dist), _p(logits_out), B, N, D, launches=2)
     return dist
 
 
@@ -746,8 +709,7 @@ def seed_retrieve(seed_info, h, B, N, D):
     seed_info = _cuda(seed_info, torch.float32, "seed_info").contiguous()
     out = torch.empty(B, D, dtype=torch.float32, device=h.device)
     assert h.stride(1) == 1
-    _lib.check(_L().gr_seed_retrieve(_p(seed_info), _p(h), h.stride(0), _p(out), B, N, D, _stream()))
-    STATS.launches += 1
+    _launch("gr_seed_retrieve", _p(seed_info), _p(h), h.stride(0), _p(out), B, N, D)
     return out
 
 
@@ -758,56 +720,10 @@ def _ptr_array(tensors):
     return (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
 
 
-def instructions(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca):
-    """All ``num_ins`` instruction vectors of one question batch in one launch (base_encoder.py:73-114).
-    hidden [B,Q,D], qnode [B,D], qtext int64 [B,Q]; Wq/bq: lists of question_linear_i weight/bias.
-    Returns ins [B, I, D]."""
-    hidden = _cuda(hidden, torch.float32, "hidden").contiguous()
-    qnode = _cuda(qnode, torch.float32, "qnode").contiguous()
-    qtext = _cuda(qtext, torch.int64, "qtext").contiguous()
-    B, Q, D = hidden.shape
-    I = len(Wq)
-    out = torch.empty(B, I, D, dtype=torch.float32, device=hidden.device)
-    with _OpTimer("question_side"):
-        rc = _L().gr_instructions(_p(hidden), _p(qnode), _p(qtext), int(pad_id), _ptr_array(Wq), _ptr_array(bq),
-                                  _p(Wcq.contiguous()), _p(bcq), _p(wca.contiguous()), _p(bca), _p(out), None,
-                                  B, Q, D, I, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
-    return out
-
-
-LSTM_MAX_HIDDEN = 256
-
-
-def lstm_forward(gates_x, W_hh, b_hh):
-    """hidden [B,Q,D] of a one-layer LSTM with zero initial state, given gates_x = x W_ih^T + b_ih [B,Q,4D]
-    (lstm_encoder.py:27-36); one launch for the whole sequence."""
-    gates_x = _cuda(gates_x, torch.float32, "gates_x").contiguous()
-    B, Q, G = gates_x.shape
-    D = G // 4
-    assert W_hh.shape == (4 * D, D) and W_hh.is_contiguous()
-    hidden = torch.empty(B, Q, D, dtype=torch.float32, device=gates_x.device)
-    with _OpTimer("question_side"):
-        _lib.check(_L().gr_lstm_forward(_p(gates_x), _p(W_hh), _p(b_hh), _p(hidden), B, Q, D, _stream()))
-    STATS.launches += 1
-    return hidden
-
-
-def query_reform(seed_info, h, ins, Wr, Wg, B, N):
-    """ins_new[b,j] = Fusion_j(ins[b,j], seed_info[b] @ h[b]) for every instruction (query_update.py:6-44)."""
-    seed_info = _cuda(seed_info, torch.float32, "seed_info").contiguous()
-    ins = _cuda(ins, torch.float32, "ins").contiguous()
-    h = _cuda(h, torch.float32, "h")
-    assert h.stride(1) == 1
-    _, I, D = ins.shape
-    out = torch.empty_like(ins)
-    with _OpTimer("query_reform"):
-        rc = _L().gr_query_reform(_p(seed_info), _p(h), h.stride(0), _p(ins), _ptr_array(Wr), _ptr_array(Wg),
-                                  _p(out), None, B, N, D, I, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
-    return out
+def instructions_ok(Q, D, I):
+    """True when gr_instructions (and its _train / _backward forms) admits Q tokens of width D and I instructions:
+    I <= 8 and (Q D + (I + 7) D + 2 Q) floats of shared memory <= 200 KB."""
+    return I <= 8 and (Q * D + (I + 7) * D + 2 * Q) * 4 <= 200 * 1024
 
 
 def _ins_args(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca):
@@ -819,6 +735,66 @@ def _ins_args(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca):
                                    _p(Wcq.contiguous()), _p(bcq), _p(wca), _p(bca)])
 
 
+def instructions(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca):
+    """All ``num_ins`` instruction vectors of one question batch in one launch (base_encoder.py:73-114).
+    hidden [B,Q,D], qnode [B,D], qtext int64 [B,Q]; Wq/bq: lists of question_linear_i weight/bias.
+    Returns ins [B, I, D]."""
+    hidden, _qn, _qt, args = _ins_args(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca)
+    B, Q, D = hidden.shape
+    I = len(Wq)
+    out = torch.empty(B, I, D, dtype=torch.float32, device=hidden.device)
+    _launch("gr_instructions", *args, _p(out), None, B, Q, D, I, op="question_side")
+    return out
+
+
+@functools.lru_cache(maxsize=None)
+def _lstm_max_hidden():
+    return int(_L().gr_lstm_max_hidden())
+
+
+def lstm_ok(D):
+    """True when gr_lstm_forward admits hidden size D: D <= gr_lstm_max_hidden()."""
+    return D <= _lstm_max_hidden()
+
+
+def lstm_forward(gates_x, W_hh, b_hh):
+    """hidden [B,Q,D] of a one-layer LSTM with zero initial state, given gates_x = x W_ih^T + b_ih [B,Q,4D]
+    (lstm_encoder.py:27-36); one launch for the whole sequence."""
+    gates_x = _cuda(gates_x, torch.float32, "gates_x").contiguous()
+    B, Q, G = gates_x.shape
+    D = G // 4
+    assert W_hh.shape == (4 * D, D) and W_hh.is_contiguous()
+    hidden = torch.empty(B, Q, D, dtype=torch.float32, device=gates_x.device)
+    _launch("gr_lstm_forward", _p(gates_x), _p(W_hh), _p(b_hh), _p(hidden), B, Q, D, op="question_side")
+    return hidden
+
+
+def query_reform_ok(D, I):
+    """True when gr_query_reform (and its _ex / _backward forms) admits width D and I instructions: D <= 1024, I <= 8
+    and (5 I + 1) D floats of shared memory <= 48 KB."""
+    return D <= 1024 and I <= 8 and (5 * I + 1) * D * 4 <= 48 * 1024
+
+
+def _reform_h(h):
+    h = _cuda(h, name="h")
+    assert h.stride(1) == 1 and h.dtype in (torch.float32, torch.bfloat16), (h.stride(), h.dtype)
+    return h, IO_BF16 if h.dtype == torch.bfloat16 else 0
+
+
+def query_reform(seed_info, h, ins, Wr, Wg, B, N, op="query_reform"):
+    """ins_new[b,j] = Fusion_j(ins[b,j], seed_info[b] @ h[b]) for every instruction (query_update.py:6-44).  h is
+    read in its own dtype: fp32, or bf16 under autocast (gr_query_reform_ex).  ``op``: the op class the call is
+    timed under."""
+    seed_info = _cuda(seed_info, torch.float32, "seed_info").contiguous()
+    ins = _cuda(ins, torch.float32, "ins").contiguous()
+    h, io = _reform_h(h)
+    _, I, D = ins.shape
+    out = torch.empty_like(ins)
+    _launch("gr_query_reform", _p(seed_info), _p(h), h.stride(0), _p(ins), _ptr_array(Wr), _ptr_array(Wg),
+            _p(out), None, B, N, D, I, io=io, op=op)
+    return out
+
+
 def instructions_train(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca, seed=None, p=0.0):
     """Training forward of :func:`instructions` with the three linear_drop sites drawn in the kernel
     (gr_instructions_train).  ``seed``: device int64 [1] (read when p > 0).  Returns (ins [B, I, D], attn [B, I, Q])."""
@@ -828,10 +804,7 @@ def instructions_train(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, bca,
     I = len(Wq)
     out = torch.empty(B, I, D, dtype=torch.float32, device=hidden.device)
     attn = torch.empty(B, I, Q, dtype=torch.float32, device=hidden.device)
-    with _OpTimer("question_train"):
-        rc = _L().gr_instructions_train(*args, _p(seed), p, _p(out), _p(attn), B, Q, D, I, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_instructions_train", *args, _p(seed), p, _p(out), _p(attn), B, Q, D, I, op="question_train")
     return out, attn
 
 
@@ -840,8 +813,7 @@ def instructions_dropout_mask(seed, p, B, Q, D, I):
     (qnode [B, I, D], cq_linear input [B, I, 4D], ca_linear input [B, I, Q, D])."""
     seed = _cuda(seed, torch.int64, "seed")
     m = [torch.empty(s, dtype=torch.uint8, device=seed.device) for s in ((B, I, D), (B, I, 4 * D), (B, I, Q, D))]
-    _lib.check(_L().gr_instructions_dropout_mask(_p(seed), float(p), B, Q, D, I, *(_p(t) for t in m), _stream()))
-    STATS.launches += 1
+    _launch("gr_instructions_dropout_mask", _p(seed), float(p), B, Q, D, I, *(_p(t) for t in m))
     return m
 
 
@@ -858,37 +830,13 @@ def instructions_backward(hidden, qnode, qtext, pad_id, Wq, bq, Wcq, bcq, wca, b
     grad_out = _cuda(grad_out, torch.float32, "grad_out").contiguous()
     e = lambda *s: torch.empty(s, dtype=torch.float32, device=hidden.device)   # noqa: E731
     outs = [e(B, Q, D), e(B, D), e(B, I, D), e(B, I, D), e(B, I, D), e(B, I, 4 * D), e(B, I, Q), e(B, I, Q, D)]
-    with _OpTimer("question_train"):
-        rc = _L().gr_instructions_backward(*args, _p(seed), p, _p(ri), _p(attn), _p(grad_out), *(_p(t) for t in outs),
-                                           B, Q, D, I, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_instructions_backward", *args, _p(seed), p, _p(ri), _p(attn), _p(grad_out), *(_p(t) for t in outs),
+            B, Q, D, I, op="question_train")
     return outs
 
 
-def _reform_h(h):
-    h = _cuda(h, name="h")
-    assert h.stride(1) == 1 and h.dtype in (torch.float32, torch.bfloat16), (h.stride(), h.dtype)
-    return h, IO_BF16 if h.dtype == torch.bfloat16 else 0
-
-
-def query_reform_train(seed_info, h, ins, Wr, Wg, B, N):
-    """:func:`query_reform` reading h in its own dtype (fp32, or bf16 under autocast: gr_query_reform_ex)."""
-    seed_info = _cuda(seed_info, torch.float32, "seed_info").contiguous()
-    ins = _cuda(ins, torch.float32, "ins").contiguous()
-    h, io = _reform_h(h)
-    _, I, D = ins.shape
-    out = torch.empty_like(ins)
-    with _OpTimer("question_train"):
-        rc = _L().gr_query_reform_ex(_p(seed_info), _p(h), h.stride(0), _p(ins), _ptr_array(Wr), _ptr_array(Wg),
-                                     _p(out), None, B, N, D, I, io, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
-    return out
-
-
 def query_reform_backward(seed_info, h, ins, Wr, Wg, B, N, grad_out, grad_h):
-    """Backward of :func:`query_reform_train` (gr_query_reform_backward): adds s_n dL/dy to the seed rows of grad_h
+    """Backward of :func:`query_reform` (gr_query_reform_backward): adds s_n dL/dy to the seed rows of grad_h
     ([B*N, D], h's dtype; no other row is touched) and returns grad_ins [B, I, D] and the weight-gradient operands
     g_r, g_g [B, I, D] and z [B, I, 3D]."""
     seed_info = _cuda(seed_info, torch.float32, "seed_info").contiguous()
@@ -899,13 +847,9 @@ def query_reform_backward(seed_info, h, ins, Wr, Wg, B, N, grad_out, grad_h):
     _, I, D = ins.shape
     e = lambda *s: torch.empty(s, dtype=torch.float32, device=ins.device)   # noqa: E731
     outs = [e(B, I, D), e(B, I, D), e(B, I, D), e(B, I, 3 * D)]
-    with _OpTimer("question_train"):
-        rc = _L().gr_query_reform_backward(_p(seed_info), _p(h), h.stride(0), _p(ins), _ptr_array(Wr), _ptr_array(Wg),
-                                           _p(grad_out), _p(outs[0]), _p(grad_h), grad_h.stride(0), *(_p(t) for t in
-                                                                                                    outs[1:]),
-                                           B, N, D, I, io, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_query_reform_backward", _p(seed_info), _p(h), h.stride(0), _p(ins), _ptr_array(Wr), _ptr_array(Wg),
+            _p(grad_out), _p(outs[0]), _p(grad_h), grad_h.stride(0), *(_p(t) for t in outs[1:]), B, N, D, I, io,
+            op="question_train")
     return outs
 
 
@@ -917,9 +861,8 @@ def kl_loss_pred(dist, teacher):
     loss_q = torch.empty(B, dtype=torch.float32, device=dist.device)
     loss = torch.empty((), dtype=torch.float32, device=dist.device)
     pred = torch.empty(B, dtype=torch.int64, device=dist.device)
-    with _OpTimer("loss_rank"):
-        _lib.check(_L().gr_kl_loss_pred(_p(dist), _p(teacher), _p(loss_q), _p(loss), _p(pred), B, N, _stream()))
-    STATS.launches += 2
+    _launch("gr_kl_loss_pred", _p(dist), _p(teacher), _p(loss_q), _p(loss), _p(pred), B, N, launches=2,
+            op="loss_rank")
     return loss, pred
 
 
@@ -933,15 +876,9 @@ def rank_candidates(dist, local_entity, query_entities, pad_id, eps):
     cand_idx = torch.empty(B, N, dtype=torch.int32, device=dev)
     cand_count = torch.empty(B, dtype=torch.int32, device=dev)
     cand_total = torch.empty(B, dtype=torch.int32, device=dev)
-    L = _L()
-    nbytes = L.gr_rank_workspace_bytes(B, N)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    with _OpTimer("loss_rank"):
-        rc = L.gr_rank_candidates(_p(dist), _p(local_entity), _p(query_entities), int(pad_id), float(eps),
-                                  _p(cand_idx), _p(cand_count), _p(cand_total), B, N, _p(ws), nbytes,
-                                  _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    ws, nbytes = _workspace(dev, "gr_rank_workspace_bytes", B, N)
+    _launch("gr_rank_candidates", _p(dist), _p(local_entity), _p(query_entities), int(pad_id), float(eps),
+            _p(cand_idx), _p(cand_count), _p(cand_total), B, N, _p(ws), nbytes, op="loss_rank")
     return cand_idx, cand_count, cand_total
 
 
@@ -954,15 +891,11 @@ def shortest_path_nodes(g, source_idx, source_cnt, target_idx, target_cnt, retur
     dev = source_idx.device
     on_path = torch.empty(B, N, dtype=torch.uint8, device=dev)
     pair_dist = torch.empty(B, S, T, dtype=torch.int32, device=dev)
-    L = _L()
-    nbytes = L.gr_paths_workspace_bytes(B, N, S, T)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    with _OpTimer("paths"):
-        rc = L.gr_shortest_path_nodes(_p(g.rowptr_t), _p(g.src_t), _p(g.rowptr_h), _p(g.src_h),
-                                      _p(source_idx.contiguous()), _p(source_cnt.contiguous()), S,
-                                      _p(target_idx.contiguous()), _p(target_cnt.contiguous()), T,
-                                      _p(on_path), _p(pair_dist), B, N, _p(ws), nbytes, _stream())
-    _lib.check(rc)
+    ws, nbytes = _workspace(dev, "gr_paths_workspace_bytes", B, N, S, T)
+    _launch("gr_shortest_path_nodes", _p(g.rowptr_t), _p(g.src_t), _p(g.rowptr_h), _p(g.src_h),
+            _p(source_idx.contiguous()), _p(source_cnt.contiguous()), S,
+            _p(target_idx.contiguous()), _p(target_cnt.contiguous()), T,
+            _p(on_path), _p(pair_dist), B, N, _p(ws), nbytes, launches=0, op="paths")
     if return_distances:
         return on_path, pair_dist, ws[: B * (S + T) * N * 4].view(torch.int32).view(B, S + T, N)
     return on_path, pair_dist
@@ -983,15 +916,10 @@ def rule_adjacency(g):
     i32 = dict(dtype=torch.int32, device=dev)
     adj = RuleAdjacency(torch.empty(Nt + 1, **i32), torch.empty(Nt, **i32), torch.empty(max(2 * F, 1), **i32),
                         torch.empty(max(2 * F, 1), **i32))
-    L = _L()
-    nbytes = L.gr_rule_adj_workspace_bytes(F)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    with _OpTimer("rule_paths"):
-        rc = L.gr_rule_adj_build(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(g.rowptr_h), _p(g.src_h),
-                                 _p(g.rel_h), _p(g.fact_h), Nt, F, _p(adj.rowptr), _p(adj.len), _p(adj.nbr),
-                                 _p(adj.lab), _p(ws), nbytes, _stream())
-    _lib.check(rc)
-    STATS.launches += 2
+    ws, nbytes = _workspace(dev, "gr_rule_adj_workspace_bytes", F)
+    _launch("gr_rule_adj_build", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(g.rowptr_h), _p(g.src_h),
+            _p(g.rel_h), _p(g.fact_h), Nt, F, _p(adj.rowptr), _p(adj.len), _p(adj.nbr), _p(adj.lab), _p(ws), nbytes,
+            launches=2, op="rule_paths")
     return adj
 
 
@@ -1000,7 +928,7 @@ def rule_walks(adj, start, rule_off, rule_len, rule_lab):
     Host numpy int32 inputs: start[J] (node id, -1 = not in the graph), rule_off[J] / rule_len[J] into rule_lab
     (label ids, -1 = absent label).  Returns (paths, counts, elem_off): paths = int32 device tensor holding, for job j,
     counts[j] rows of rule_len[j] + 1 node ids from elem_off[j] on (host int64 arrays)."""
-    with _OpTimer("rule_paths"):
+    with _Timer("rule_paths"):
         return _rule_walks(adj, start, rule_off, rule_len, rule_lab)
 
 
@@ -1018,23 +946,21 @@ def _rule_walks(adj, start, rule_off, rule_len, rule_lab):
     res_begin = torch.zeros(max(J, 1), **i32)
     res_count = torch.zeros(max(J, 1), **i32)
     levels_node, levels_parent = [node], [torch.full_like(node, -1)]
-    L = _L()
     for level in range(int(rule_len.max()) + 1 if J else 0):
         n = node.numel()
         seg = torch.empty(max(n, 1), **i32)
         off = torch.empty(n + 1, dtype=torch.int64, device=dev)
-        nbytes = L.gr_rule_level_workspace_bytes(n)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _lib.check(L.gr_rule_level_count(_p(adj.rowptr), _p(adj.len), _p(adj.lab), _p(d_off), _p(d_len), _p(d_lab),
-                                         J, level, _p(node), _p(job), n, _p(seg), _p(off), _p(res_begin),
-                                         _p(res_count), _p(ws), nbytes, _stream()))
+        ws, nbytes = _workspace(dev, "gr_rule_level_workspace_bytes", n)
+        _launch("gr_rule_level_count", _p(adj.rowptr), _p(adj.len), _p(adj.lab), _p(d_off), _p(d_len), _p(d_lab),
+                J, level, _p(node), _p(job), n, _p(seg), _p(off), _p(res_begin), _p(res_count), _p(ws), nbytes,
+                launches=0)
         if level == rule_len.max():
             break
         total = int(off[n].item())              # the one read-back per level: the next level is allocated exactly
         fits = total <= 0x7fffffff              # a level that int32 cannot index is refused by gr_rule_level_emit
         nxt = [torch.empty(max(total if fits else 0, 1), **i32) for _ in range(3)]
-        _lib.check(L.gr_rule_level_emit(_p(adj.nbr), _p(job), _p(seg), _p(off), n, total, _p(nxt[0]), _p(nxt[1]),
-                                        _p(nxt[2]), _stream()))
+        _launch("gr_rule_level_emit", _p(adj.nbr), _p(job), _p(seg), _p(off), n, total, _p(nxt[0]), _p(nxt[1]),
+                _p(nxt[2]), launches=0)
         node, job = nxt[0][:total], nxt[2][:total]
         levels_node.append(node)
         levels_parent.append(nxt[1][:total])
@@ -1049,8 +975,8 @@ def _rule_walks(adj, start, rule_off, rule_len, rule_lab):
         lv_node = torch.tensor([t.data_ptr() for t in levels_node], dtype=torch.int64, device=dev)
         lv_parent = torch.tensor([t.data_ptr() for t in levels_parent], dtype=torch.int64, device=dev)
         d_path_off, d_elem_off = torch.from_numpy(path_off).to(dev), torch.from_numpy(elem_off).to(dev)
-        _lib.check(L.gr_rule_paths_write(_p(lv_node), _p(lv_parent), _p(d_len), _p(res_begin), _p(d_path_off),
-                                         _p(d_elem_off), J, int(path_off[-1]), _p(paths), _stream()))
+        _launch("gr_rule_paths_write", _p(lv_node), _p(lv_parent), _p(d_len), _p(res_begin), _p(d_path_off),
+                _p(d_elem_off), J, int(path_off[-1]), _p(paths), launches=0)
     return paths[: int(elem_off[-1])], counts, elem_off[:J]
 
 
@@ -1123,15 +1049,10 @@ def graft_stage(e2f, f2e, kb_fact_rel, B, N, R1, live=None):
     dev = kb_fact_rel.device
     gg = GraftGraph(B, N, max_fact, F0, dev)
     gg.kb_fact_rel = kb_fact_rel
-    L = _L()
-    nbytes = L.gr_graft_stage_workspace_bytes(B, max_fact)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    with _OpTimer("csr_build"):
-        rc = L.gr_graft_stage(_p(e2f[0]), _p(e2f[1]), _p(e2f[2]), F0, _p(f2e[0]), _p(f2e[1]), _p(f2e[2]), F1,
-                              _p(kb_fact_rel), B, N, max_fact, R1, _p(gg.heads), _p(gg.rels), _p(gg.tails),
-                              _p(gg.slot_of), _p(gg.nfacts), _p(gg.status), _p(live), _p(ws), nbytes, _stream())
-    _lib.check(rc)
-    STATS.launches += 5
+    ws, nbytes = _workspace(dev, "gr_graft_stage_workspace_bytes", B, max_fact)
+    _launch("gr_graft_stage", _p(e2f[0]), _p(e2f[1]), _p(e2f[2]), F0, _p(f2e[0]), _p(f2e[1]), _p(f2e[2]), F1,
+            _p(kb_fact_rel), B, N, max_fact, R1, _p(gg.heads), _p(gg.rels), _p(gg.tails),
+            _p(gg.slot_of), _p(gg.nfacts), _p(gg.status), _p(live), _p(ws), nbytes, launches=5, op="csr_build")
     gg.graph = csr_build(gg.heads[:F0], gg.rels[:F0], gg.tails[:F0], B, N, R1, nfacts=gg.nfacts)
     return gg
 
@@ -1150,12 +1071,9 @@ def graft_attention(gg, qh, qmask, rel, out_w=False):
     Wt = torch.empty(max(S, 1), dtype=torch.float32, device=dev)
     E = torch.empty(B * gg.N, dtype=torch.float32, device=dev)
     g = gg.graph
-    with _OpTimer("graft_attention"):
-        rc = _L().gr_graft_attention(_p(qh), _p(qmask), Q, _p(rel), rel.stride(0), rel.shape[0], _p(gg.kb_fact_rel),
-                                     B, gg.max_fact, D, _p(g.rowptr_h), _p(g.fact_h), _p(gg.slot_of), gg.N, _p(W),
-                                     _p(Wt), _p(E), _p(gg.status), _stream())
-    _lib.check(rc)
-    STATS.launches += 3 if S > 0 else 1
+    _launch("gr_graft_attention", _p(qh), _p(qmask), Q, _p(rel), rel.stride(0), rel.shape[0], _p(gg.kb_fact_rel),
+            B, gg.max_fact, D, _p(g.rowptr_h), _p(g.fact_h), _p(gg.slot_of), gg.N, _p(W), _p(Wt), _p(E),
+            _p(gg.status), launches=3 if S > 0 else 1, op="graft_attention")
     return (W[:S] if out_w else None), Wt[:S], E
 
 
@@ -1178,15 +1096,12 @@ def graft_aggregate(gg, Wt, E, prior, self_tab, head_tab, lam, q2e=None, sum_out
     if q2e is not None:
         q2e = _cuda(q2e, torch.float32, "q2e").contiguous()
     hi, lo = planes if planes is not None else (None, None)
-    with _AggTimer(("graft", 1)):
-        rc = _L().gr_graft_aggregate(_p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(gg.slot_of),
-                                     _p(Wt), _p(E), _p(prior), _p(self_tab), self_tab.stride(0), _p(head_tab),
-                                     head_tab.stride(0), _p(q2e), float(lam), _p(sum_out),
-                                     sum_out.stride(0) if sum_out is not None else 0, _p(hi), _p(lo),
-                                     hi.stride(0) if hi is not None else 0, col_sum, col_indeg, col_q2e,
-                                     _p(indeg_out), _p(prior_next), B, N, D, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_graft_aggregate", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(gg.slot_of),
+            _p(Wt), _p(E), _p(prior), _p(self_tab), self_tab.stride(0), _p(head_tab),
+            head_tab.stride(0), _p(q2e), float(lam), _p(sum_out),
+            sum_out.stride(0) if sum_out is not None else 0, _p(hi), _p(lo),
+            hi.stride(0) if hi is not None else 0, col_sum, col_indeg, col_q2e,
+            _p(indeg_out), _p(prior_next), B, N, D, agg=("graft", 1))
     return prior_next
 
 
@@ -1206,9 +1121,14 @@ def graft_dropout_mask(seed, p, S, D):
     seed, p = _seed_p(seed, p)
     dev = seed.device if seed is not None else torch.device("cuda")
     mask = torch.empty(max(S, 1), D, dtype=torch.uint8, device=dev)
-    _lib.check(_L().gr_graft_dropout_mask(_p(seed), p, S, D, _p(mask), _stream()))
-    STATS.launches += 1 if S > 0 else 0
+    _launch("gr_graft_dropout_mask", _p(seed), p, S, D, _p(mask), launches=1 if S > 0 else 0)
     return mask[:S]
+
+
+def fact_train_ok(D):
+    """True when the TypeLayer and GraftNet training kernels (gr_type_layer_backward, gr_graft_aggregate_train /
+    _backward, gr_graft_attention_backward) admit width D: D <= 512."""
+    return D <= 512
 
 
 def graft_aggregate_train(gg, s, self_tab, head_tab, seed=None, p=0.0, sum_out=None):
@@ -1229,12 +1149,9 @@ def graft_aggregate_train(gg, s, self_tab, head_tab, seed=None, p=0.0, sum_out=N
     assert sum_out.stride(1) == 1
     if s.numel() == 0:               # no staged facts (every question's subgraph empty): every row sums nothing
         return sum_out.zero_()
-    with _AggTimer(("graft_train", 1)):
-        rc = _call_io(_L(), "gr_graft_aggregate_train", io, _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t),
-                      _p(gg.slot_of), _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab), head_tab.stride(0),
-                      _p(seed), p, _p(sum_out), sum_out.stride(0), gg.B, gg.N, D, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_graft_aggregate_train", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(g.fact_t), _p(gg.slot_of), _p(s),
+            _p(self_tab), self_tab.stride(0), _p(head_tab), head_tab.stride(0), _p(seed), p, _p(sum_out),
+            sum_out.stride(0), gg.B, gg.N, D, io=io, agg=("graft_train", 1))
     return sum_out
 
 
@@ -1254,29 +1171,17 @@ def graft_aggregate_backward(gg, s, self_tab, head_tab, grad_sum, grad_s, grad_s
     seed, p = _seed_p(seed, p)
     if s.numel() == 0:               # no staged facts: nothing to add
         return
+    args = (_p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h), _p(gg.slot_of), _p(s), _p(self_tab),
+            self_tab.stride(0), _p(head_tab), head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0),
+            _p(grad_s), _p(grad_self), grad_self.stride(0), _p(grad_head), grad_head.stride(0), gg.B, gg.N, D)
     if deterministic:
         R1 = self_tab.shape[0]
         rix_ptr, rix_fact = gg.fact_relation_index(R1)
-        L = _L()
-        nbytes = L.gr_graft_aggregate_backward_det_workspace_bytes(gg.cap, D)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=s.device)
-        with _OpTimer("aggregation_bwd_det"):
-            rc = _call_io(
-                L, "gr_graft_aggregate_backward_det", io, _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(g.fact_h),
-                _p(gg.slot_of), _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab), head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0),
-                _p(grad_s), _p(grad_self), grad_self.stride(0), _p(grad_head), grad_head.stride(0), gg.B, gg.N, D,
-                _p(gg.heads), _p(gg.rels), _p(gg.tails), _p(rix_ptr), _p(rix_fact), R1, gg.cap, _p(ws), nbytes,
-                _stream())
-        _lib.check(rc)
-        STATS.launches += 3
+        ws, nbytes = _workspace(s.device, "gr_graft_aggregate_backward_det_workspace_bytes", gg.cap, D)
+        _launch("gr_graft_aggregate_backward_det", *args, _p(gg.heads), _p(gg.rels), _p(gg.tails), _p(rix_ptr),
+                _p(rix_fact), R1, gg.cap, _p(ws), nbytes, io=io, launches=3, op="aggregation_bwd_det")
         return
-    with _OpTimer("aggregation_bwd"):
-        rc = _call_io(_L(), "gr_graft_aggregate_backward", io, _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h),
-                      _p(g.fact_h), _p(gg.slot_of), _p(s), _p(self_tab), self_tab.stride(0), _p(head_tab),
-                      head_tab.stride(0), _p(seed), p, _p(grad_sum), grad_sum.stride(0), _p(grad_s), _p(grad_self),
-                      grad_self.stride(0), _p(grad_head), grad_head.stride(0), gg.B, gg.N, D, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_graft_aggregate_backward", *args, io=io, op="aggregation_bwd")
 
 
 def graft_attention_backward(gg, qh, qmask, rel, grad_W, grad_qh, grad_rel, deterministic=False):
@@ -1294,23 +1199,14 @@ def graft_attention_backward(gg, qh, qmask, rel, grad_W, grad_qh, grad_rel, dete
             return
         R1 = rel.shape[0]
         rix_ptr, rix_slot = gg.slot_relation_index(R1)
-        L = _L()
-        nbytes = L.gr_graft_attention_backward_det_workspace_bytes(B, gg.max_fact, Q, D)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=qh.device)
-        with _OpTimer("graft_attention_bwd_det"):
-            rc = L.gr_graft_attention_backward_det(_p(qh), _p(qmask), Q, _p(rel), rel.stride(0), R1,
-                                                   _p(gg.kb_fact_rel), B, gg.max_fact, D, _p(grad_W), _p(grad_qh),
-                                                   _p(grad_rel), grad_rel.stride(0), _p(rix_ptr), _p(rix_slot),
-                                                   _p(ws), nbytes, _stream())
-        _lib.check(rc)
-        STATS.launches += 4
+        ws, nbytes = _workspace(qh.device, "gr_graft_attention_backward_det_workspace_bytes", B, gg.max_fact, Q, D)
+        _launch("gr_graft_attention_backward_det", _p(qh), _p(qmask), Q, _p(rel), rel.stride(0), R1,
+                _p(gg.kb_fact_rel), B, gg.max_fact, D, _p(grad_W), _p(grad_qh), _p(grad_rel), grad_rel.stride(0),
+                _p(rix_ptr), _p(rix_slot), _p(ws), nbytes, launches=4, op="graft_attention_bwd_det")
         return
-    with _OpTimer("graft_attention_bwd"):
-        rc = _L().gr_graft_attention_backward(_p(qh), _p(qmask), Q, _p(rel), rel.stride(0), rel.shape[0],
-                                              _p(gg.kb_fact_rel), B, gg.max_fact, D, _p(grad_W), _p(grad_qh),
-                                              _p(grad_rel), grad_rel.stride(0), _stream())
-    _lib.check(rc)
-    STATS.launches += 1 if gg.max_fact > 0 else 0
+    _launch("gr_graft_attention_backward", _p(qh), _p(qmask), Q, _p(rel), rel.stride(0), rel.shape[0],
+            _p(gg.kb_fact_rel), B, gg.max_fact, D, _p(grad_W), _p(grad_qh), _p(grad_rel), grad_rel.stride(0),
+            launches=1 if gg.max_fact > 0 else 0, op="graft_attention_bwd")
 
 
 def type_layer_backward(g, grad_out, out, grad_table, w_t=None, w_h=None, deterministic=False):
@@ -1324,20 +1220,12 @@ def type_layer_backward(g, grad_out, out, grad_table, w_t=None, w_h=None, determ
         assert grad_table.shape[0] >= g.R1
         ptr_t, slot_t, row_t = csr_relation_index(g, "fwd")
         ptr_h, slot_h, row_h = csr_relation_index(g, "inv")
-        L = _L()
-        nbytes = L.gr_type_layer_backward_det_workspace_bytes(g.F, D)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
-        with _OpTimer("type_layer_bwd_det"):
-            rc = _call_io(L, "gr_type_layer_backward_det", io, _p(g.rel_t), _p(w_t), _p(ptr_t), _p(slot_t), _p(row_t),
-                          _p(g.rel_h), _p(w_h), _p(ptr_h), _p(slot_h), _p(row_h), _p(grad_out), grad_out.stride(0),
-                          _p(out), out.stride(0), _p(grad_table), grad_table.stride(0), g.R1, D, g.F, _p(ws), nbytes,
-                          _stream())
-        _lib.check(rc)
-        STATS.launches += 4 if g.F > 0 else 0
+        ws, nbytes = _workspace(out.device, "gr_type_layer_backward_det_workspace_bytes", g.F, D)
+        _launch("gr_type_layer_backward_det", _p(g.rel_t), _p(w_t), _p(ptr_t), _p(slot_t), _p(row_t),
+                _p(g.rel_h), _p(w_h), _p(ptr_h), _p(slot_h), _p(row_h), _p(grad_out), grad_out.stride(0),
+                _p(out), out.stride(0), _p(grad_table), grad_table.stride(0), g.R1, D, g.F, _p(ws), nbytes, io=io,
+                launches=4 if g.F > 0 else 0, op="type_layer_bwd_det")
         return
-    with _OpTimer("type_layer_bwd"):
-        rc = _call_io(_L(), "gr_type_layer_backward", io, _p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h),
-                      _p(g.rel_h), _p(w_h), _p(grad_out), grad_out.stride(0), _p(out), out.stride(0), _p(grad_table),
-                      grad_table.stride(0), g.B, g.N, D, g.F, _stream())
-    _lib.check(rc)
-    STATS.launches += 1
+    _launch("gr_type_layer_backward", _p(g.rowptr_t), _p(g.rel_t), _p(w_t), _p(g.rowptr_h), _p(g.rel_h), _p(w_h),
+            _p(grad_out), grad_out.stride(0), _p(out), out.stride(0), _p(grad_table), grad_table.stride(0),
+            g.B, g.N, D, g.F, io=io, op="type_layer_bwd")

@@ -1,12 +1,14 @@
 """CPU: every training entry point refuses bad arguments with a fixed (status, gr_last_error()) pair, whichever of
-its fp32, `_ex`, `_det` and `_det_ex` forms is called.  Every call below is refused before any CUDA call, so the
+its fp32, `_ex`, `_det` and `_det_ex` forms is called, and admits exactly the shapes the matching rule of ops
+admits.  Every call below is refused before any CUDA call, so the
 pointers are placeholders that are never dereferenced."""
+import ctypes
 import os
 import re
 
 import pytest
 
-from gnn_rag_b200 import _lib
+from gnn_rag_b200 import _lib, ops
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PTR = 0x1000          # a non-null device pointer: never dereferenced, every call is refused first
@@ -237,3 +239,82 @@ def test_entry_point_refuses(name, good, over, rc, msg, arg_name, ws_name):
         expected = "%s: invalid argument: %s" % (arg_name, msg)
     assert need > 0 or "workspace_bytes" not in PARAMS[name]
     assert call(name, args) == (rc, expected)
+
+
+# ---- the shape rules of ops against the entry points that enforce them ----------------------------------------------
+# For each bound of a rule: the largest shape it admits and the first it refuses.  The entry point must refuse the
+# second with its shape message.  It refuses the first as well, but later, by a check it runs after the shape check
+# (a null output, a stride, a workspace), so that no call reaches CUDA.
+
+UNSUPPORTED = -4
+
+
+def _host_ptrs(n):
+    """The host array of n weight pointers that the question-side entry points read before their shape check."""
+    return (ctypes.c_void_p * n)(*[PTR] * n)
+
+
+def _agg_bwd(D, I):
+    # grad_col0 = 1 puts the last segment one column past the row: the stride check comes after the shape check
+    args = dict(AGG_BWD, D=D, I=I, seg_stride=max(D, 1), grad_row_stride=I * D, grad_col0=1)
+    err = "gr_aggregate_backward_ex: invalid argument: "
+    return "gr_aggregate_backward", args, (INVALID, err + _STRIDE), (INVALID, err + _SIZES)
+
+
+def _type_bwd(D):
+    args = dict(TYPE_BWD, D=D, ld_grad=D, ld_out=D, ld_gtable=D, grad_table=None)
+    err = "gr_type_layer_backward_ex: invalid argument: "
+    return "gr_type_layer_backward", args, (INVALID, err + "null pointer"), (INVALID, err + _TSIZES)
+
+
+def _instructions(Q, D, I):
+    args = dict(pad_id=0, Wq_host=_host_ptrs(I), bq_host=_host_ptrs(I), out=None, attn_out=None, B=2, Q=Q, D=D, I=I,
+                stream=None)
+    err = "gr_instructions: invalid argument: "
+    refused = "bad shape (num_ins <= 8)" if I > 8 else "question length x entity_dim too large for shared memory"
+    return "gr_instructions", args, (INVALID, err + "null pointer"), (INVALID, err + refused)
+
+
+def _query_reform(D, I):
+    args = dict(ldh=D, Wr_host=_host_ptrs(I), Wg_host=_host_ptrs(I), ins_out=None, seed_out=None, B=2, N=3, D=D, I=I,
+                stream=None)
+    err = "gr_query_reform: invalid argument: "
+    refused = "bad shape (D <= 1024, num_ins <= 8)" if D > 1024 or I > 8 else \
+        "num_ins x entity_dim too large for shared memory"
+    return "gr_query_reform", args, (INVALID, err + "null pointer"), (INVALID, err + refused)
+
+
+def _linear_tc(N, K):
+    M = 16
+    args = dict(lda=K, ldw=K, bias=None, ldc=N, M=M, N=N, K=K, flags=0, workspace_bytes=0, stream=None)
+    need = _lib.load().gr_linear_tc_workspace_bytes(M, N, K)
+    return ("gr_linear_tc", args, (WORKSPACE, "gr_linear_tc: workspace too small (0 < %d)" % need),
+            (UNSUPPORTED, "gr_linear_tc: unsupported shape M=%d N=%d K=%d (need 8 <= N <= 256, K >= 8)" % (M, N, K)))
+
+
+# (ops rule, entry point case, largest admitted shape, first refused shape)
+RULE_BOUNDS = [
+    ("aggregate_backward_ok", _agg_bwd, (256, 4), (257, 4)),
+    ("aggregate_backward_ok", _agg_bwd, (1, 4), (0, 4)),
+    ("aggregate_backward_ok", _agg_bwd, (256, 4), (256, 5)),
+    ("aggregate_backward_ok", _agg_bwd, (256, 1), (256, 0)),
+    ("fact_train_ok", _type_bwd, (512,), (513,)),
+    ("instructions_ok", _instructions, (20, 50, 8), (20, 50, 9)),
+    ("instructions_ok", _instructions, (244, 200, 2), (245, 200, 2)),      # (Q D + 9 D + 2 Q) floats <= 200 KB
+    ("query_reform_ok", _query_reform, (1024, 1), (1025, 1)),
+    ("query_reform_ok", _query_reform, (8, 8), (8, 9)),
+    ("query_reform_ok", _query_reform, (768, 3), (769, 3)),              # 16 D floats <= 48 KB
+    ("tc_linear_ok", _linear_tc, (8, 8), (7, 8)),
+    ("tc_linear_ok", _linear_tc, (256, 8), (257, 8)),
+    ("tc_linear_ok", _linear_tc, (8, 8), (8, 7)),
+]
+
+
+@pytest.mark.parametrize("rule,case,admitted,refused", RULE_BOUNDS,
+                         ids=["%s-%s" % (r[0], "x".join(map(str, r[3]))) for r in RULE_BOUNDS])
+def test_ops_shape_rule_is_the_entry_points(rule, case, admitted, refused):
+    ok = getattr(ops, rule)
+    name, args, past_shape_check, _ = case(*admitted)
+    assert ok(*admitted) and call(name, args) == past_shape_check
+    name, args, _, shape_refusal = case(*refused)
+    assert not ok(*refused) and call(name, args) == shape_refusal

@@ -297,13 +297,13 @@ def test_query_reform_backward_at_the_widest_admitted_width(I):
 
 
 @pytest.mark.parametrize("D,I,N", [(50, 3, 500), (200, 2, 1025), (1024, 1, 300)])
-def test_query_reform_bf16_h_is_the_fp32_kernel_on_the_upcast_h(D, I, N):
+def test_query_reform_bf16_h_equals_the_fp32_kernel_on_the_upcast_h(D, I, N):
     """GR_IO_BF16: forward and backward equal the fp32 calls on h.float(); the bf16 grad_h holds the fp32 result
     rounded to nearest even (pre-filled bf16 rows widened, the seed term added, rounded once)."""
     L = QS._Reform(D + I, 4, N, D, I)
     h16 = L.h.to(BF)
-    out16 = ops.query_reform_train(L.seed, h16, L.ins, L.Wr, L.Wg, L.B, N)
-    out32 = ops.query_reform_train(L.seed, h16.float(), L.ins, L.Wr, L.Wg, L.B, N)
+    out16 = ops.query_reform(L.seed, h16, L.ins, L.Wr, L.Wg, L.B, N)
+    out32 = ops.query_reform(L.seed, h16.float(), L.ins, L.Wr, L.Wg, L.B, N)
     _bits_equal(out16, out32)
     Gout = torch.randn(L.B, I, D, device=DEV)
     pre16 = torch.randn(L.B * N, D, device=DEV).to(BF)
@@ -315,10 +315,16 @@ def test_query_reform_bf16_h_is_the_fp32_kernel_on_the_upcast_h(D, I, N):
     _bits_equal(g16, g32.to(BF))
 
 
-def test_query_reform_train_fp32_equals_gr_query_reform():
+def test_query_reform_fp32_equals_gr_query_reform_ex_with_io_0():
+    """The fp32 wrapper and gr_query_reform_ex with io = 0 give the bits of gr_query_reform."""
     L = QS._Reform(7, 4, 1025, 130, 3, ldh_pad=3)
     out, _ = L.run()
-    _bits_equal(ops.query_reform_train(L.seed, L.h, L.ins, L.Wr, L.Wg, L.B, L.N), out)
+    _bits_equal(ops.query_reform(L.seed, L.h, L.ins, L.Wr, L.Wg, L.B, L.N), out)
+    ex = _nan(L.B, L.I, L.D)
+    _lib.check(_lib.load().gr_query_reform_ex(_p(L.seed), _p(L.h), L.h.stride(0), _p(L.ins), ops._ptr_array(L.Wr),
+                                              ops._ptr_array(L.Wg), _p(ex), None, L.B, L.N, L.D, L.I, 0,
+                                              ops._stream()))
+    _bits_equal(ex, out)
 
 
 # --------------------------------------------------------------------------------------------------------------

@@ -818,7 +818,9 @@ extern "C" int gr_aggregate_dual_abs(const int32_t* rowptr_t, const int32_t* src
   using namespace gr;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   GR_CHECK_ARG(rowptr_t && rowptr_h && prior && pn_fwd && pn_inv && ins && out_hi, "null pointer");
-  GR_CHECK_ARG(out_lo || tile_counter, "hi-only output (bf16 activation storage) needs the persistent kernel");
+  // only the persistent kernels have a hi-only form; agg_abs_kernel (no tile counter, or agg_abs_ws 0) always stores lo
+  GR_CHECK_ARG(out_lo || (tile_counter && g_opt_agg_abs_ws != 0),
+               "hi-only output (bf16 activation storage) needs a persistent kernel (a tile counter and agg_abs_ws != 0)");
   GR_CHECK_ARG(F == 0 || (src_t && rel_t && src_h && rel_h), "null edge arrays");
   GR_CHECK_ARG(B > 0 && N >= kRows && I > 0, "B, I must be positive and N >= 64");
   GR_CHECK_ARG(D == 200 && seg_pitch == 208, "this build specialises D = 200, seg_pitch = 208 (use gr_aggregate_dual)");

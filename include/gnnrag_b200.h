@@ -204,7 +204,10 @@ int gr_aggregate_dual_abs(const int32_t* rowptr_t, const int32_t* src_t, const i
  * warp prepares the next tile of rows while the consumer warps aggregate the current one; dynamic tile scheduler);
  * NULL -> one CTA per 64-row tile.  gr_set_option("agg_abs_ws", v) picks the persistent variant: 1 = 8 consumer warps /
  * 64-row tiles, 2 (default) = 9 consumer warps / 72-row tiles, 3 = gather through TMA tile::gather4 copies into
- * shared-memory rings (bit-identical results; slower at cfg2, kept as the measured alternative, DESIGN.md 4.1). */
+ * shared-memory rings (bit-identical results; slower at cfg2, kept as the measured alternative, DESIGN.md 4.1);
+ * 0 = one CTA per 64-row tile even when a tile counter is given.
+ * out_lo NULL (bf16 activation storage: the hi plane only) is accepted only by the persistent kernels 1 and 2, so it
+ * needs a tile counter and agg_abs_ws != 0 (GR_ERR_INVALID_ARG otherwise); with agg_abs_ws 3 it runs variant 2. */
 
 /* One dense-prior ReaRev layer as ONE kernel (csrc/fused_layer.cu): the aggregation of both directions and all
  * instructions (reason_layer / reason_layer_inv, reasongnn.py:61-116) is produced straight into the shared-memory

@@ -241,6 +241,32 @@ def test_entry_point_refuses(name, good, over, rc, msg, arg_name, ws_name):
     assert call(name, args) == (rc, expected)
 
 
+# ---- gr_aggregate_dual_abs: the hi-only output needs a persistent kernel ---------------------------------------------
+# Only the persistent kernels (agg_abs_ws 1 and 2; 3 falls back to 2) have a form that writes the hi plane alone; the
+# one-CTA-per-tile kernel (no tile counter, or agg_abs_ws 0) always stores the lo plane.  An admitted call is refused
+# later in the same entry point by a misaligned padded table, before any CUDA call.
+
+DUAL_ABS = dict(w_t=None, w_h=None, table_rows=3, out_lo=None, ld_planes=2 * 2 * 208, out_col0=0, seg_pitch=208,
+                B=2, N=64, D=200, I=2, F=4, stream=None)
+_DUAL_ABS_ERR = "gr_aggregate_dual_abs: invalid argument: "
+_HI_ONLY = "hi-only output (bf16 activation storage) needs a persistent kernel (a tile counter and agg_abs_ws != 0)"
+
+
+@pytest.mark.parametrize("mode,counter,refused", [(0, True, True), (1, True, False), (2, True, False),
+                                                  (3, True, False), (2, False, True)])
+def test_aggregate_dual_abs_hi_only_needs_a_persistent_kernel(mode, counter, refused):
+    args = dict(DUAL_ABS, pn_fwd=PTR + 8, tile_counter=PTR if counter else None)
+    ops.set_option("agg_abs_ws", mode)
+    try:
+        got = call("gr_aggregate_dual_abs", args)
+    finally:
+        ops.set_option("agg_abs_ws", 2)
+    want = _HI_ONLY if refused else "misaligned planes / padded tables"
+    assert got == (INVALID, _DUAL_ABS_ERR + want)
+    args["out_lo"] = PTR                                  # both planes: every mode and the counter-less kernel admit it
+    assert call("gr_aggregate_dual_abs", args) == (INVALID, _DUAL_ABS_ERR + "misaligned planes / padded tables")
+
+
 # ---- the shape rules of ops against the entry points that enforce them ----------------------------------------------
 # For each bound of a rule: the largest shape it admits and the first it refuses.  The entry point must refuse the
 # second with its shape message.  It refuses the first as well, but later, by a check it runs after the shape check

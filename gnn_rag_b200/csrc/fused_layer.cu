@@ -22,14 +22,19 @@
 // direction and turn {table offset, source node} into {table offset, c_f} there (weighted graphs: fused_coef_kernel), so
 // no per-edge index arithmetic runs inside the fused kernel.
 //
+// The pair can walk K in this kernel's order (gr_linear_tc_planes with GR_LINEAR_K_GROUPED, same W planes:
+// plan_grouped_k / grouped_w_split below) and then returns this kernel's bits; at accumulator widths above 128 columns
+// it is the faster of the two (see the end of this comment) and ops.dense_layer runs it.  This kernel is the
+// reference it is held to, and the dense layer of the widths it can issue as one instruction.
+//
 // Warp roles (512 threads, one CTA per SM, clusters of 2 share W by TMA multicast):
 //   warp 0      TMA producer: W k-blocks into a 3-stage ring, the H block of every group into its operand slot (the
 //               next tile's h blocks are L2-prefetched a tile ahead)
 //   warps 2, 3  stagers: bulk copies of the tile's ELL entries + quad offsets, relu(+-ins)/2 of its <= 2 questions
 //               -> double-buffered tile descriptor
-//   warps 4-11  two consumer warpgroups, 64 tile rows each: wgmma.mma_async (one full-width m64n{NP}k16 per product
-//               and k-step, 3 products) with the fp32 accumulator in registers, then the epilogue: bias + relu + score
-//               dot -> fp32 h / bf16 planes via TMA stores
+//   warps 4-11  two consumer warpgroups, 64 tile rows each: wgmma.mma_async (3 products per k-step: one m64n{NP}k16
+//               each up to NP = 128, 32-column instructions above, see "Registers" below) with the fp32 accumulator in
+//               registers, then the epilogue: bias + relu + score dot -> fp32 h / bf16 planes via TMA stores
 //   warps 12-15 aggregation: warp a owns tile rows 32a .. 32a+31 = eight quads; a quarter-warp owns a row, lane = 4
 //               columns of the 32-column group, so one warp-wide 16-byte load gathers one in-edge of each row of the
 //               quad (one 128-byte table line per row); 8 such loads in flight per lane, no predicates (slots past a
@@ -42,7 +47,8 @@
 // Registers: ptxas places a wgmma accumulator operand within the 128 registers per thread of the launch, so an
 // m64n208k16 (130 needed) does not compile here: accumulators wider than 128 columns are issued as 32-column
 // instructions, one straight-line batch per k-block.
-// Performance on one H100 SXM at 400 W, cfg2: 1.03 ms per dense layer (the unfused pair: 0.24 + 0.59 ms).
+// Performance on one H100 80GB HBM3 at 700 W, cfg2 (scripts/dense_layer_probe.py): 1.02 ms per dense layer; the pair
+// in this kernel's K order 0.23 + 0.49 ms, in segment order 0.23 + 0.34 ms.
 #include <algorithm>
 #include <cstddef>
 
@@ -799,10 +805,8 @@ FusedPlan plan_fused(int64_t Nq, int64_t D, int64_t pitch, int I, int64_t N_out)
   FusedPlan f{};
   f.n_pad = (int)((N_out + 15) / 16 * 16);
   f.np = f.n_pad <= 64 ? 64 : f.n_pad <= 128 ? 128 : f.n_pad <= 208 ? 208 : 224;
-  f.G = (int)((pitch + BK - 1) / BK);
-  f.ksteps_last = (int)((pitch - (int64_t)(f.G - 1) * BK) / MMA_K);
-  f.kp = (int64_t)f.G * (2 * I + 1) * BK;
-  f.w_plane_bytes = align_up((size_t)N_out * f.kp * 2, 256);
+  const GroupedK k = plan_grouped_k(pitch, I, N_out);
+  f.G = k.G; f.ksteps_last = k.ksteps_last; f.kp = k.kp; f.w_plane_bytes = k.w_plane_bytes;
   f.smem_bytes = I == 2 ? fused_smem_bytes<2>(f.np) : fused_smem_bytes<1>(f.np);
   f.ok = (I == 1 || I == 2) && Nq >= BM && D >= 8 && D <= pitch && pitch % 16 == 0 && (pitch + BK - 1) / BK * BK <= kXCols &&
          N_out >= 8 && f.n_pad <= 224 && f.smem_bytes <= 227 * 1024 && get_encode_fn() != nullptr;
@@ -832,6 +836,28 @@ int launch_fused_np(const CUtensorMap* const (&m)[7], int I, int cs, const Fused
 }
 
 }  // namespace
+
+namespace tc {
+
+GroupedK plan_grouped_k(int64_t pitch, int I, int64_t N_out) {
+  GroupedK k{};
+  k.G = (int)((pitch + BK - 1) / BK);
+  k.ksteps_last = (int)((pitch - (int64_t)(k.G - 1) * BK) / MMA_K);
+  k.kp = (int64_t)k.G * (2 * I + 1) * BK;
+  k.w_plane_bytes = align_up((size_t)N_out * k.kp * 2, 256);
+  return k;
+}
+
+int grouped_w_split(const float* W, int64_t ldw, int64_t N_out, int D, int I, const GroupedK& k, __nv_bfloat16* hi,
+                    __nv_bfloat16* lo, cudaStream_t stream) {
+  const int64_t work = N_out * k.kp;
+  const int grid = (int)std::min<int64_t>(ceil_div(work, 256), 32LL * sm_count());
+  fused_w_split_kernel<<<grid, 256, 0, stream>>>(W, ldw, (int)N_out, D, I, k.G, hi, lo);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+}  // namespace tc
 }  // namespace gr
 
 extern "C" int gr_fused_profile_read(unsigned long long* out, int n) {
@@ -920,10 +946,7 @@ extern "C" int gr_fused_layer(const int32_t* rowptr_t, const int32_t* src_t, con
   __nv_bfloat16* w_hi = reinterpret_cast<__nv_bfloat16*>(ws);
   __nv_bfloat16* w_lo = reinterpret_cast<__nv_bfloat16*>(ws + f.w_plane_bytes);
   if (!(flags & GR_LINEAR_W_PRESPLIT)) {
-    const int64_t work = N_out * f.kp;
-    const int grid = (int)std::min<int64_t>(ceil_div(work, 256), 32LL * sm_count());
-    fused_w_split_kernel<<<grid, 256, 0, stream>>>(W, ldw, (int)N_out, D, I, f.G, w_hi, w_lo);
-    GR_CHECK_LAUNCH();
+    if (int rc = grouped_w_split(W, ldw, N_out, D, I, plan_grouped_k(seg_pitch, I, N_out), w_hi, w_lo, stream)) return rc;
   }
   FParams p{};
   p.dir[0] = FDir{rowptr_t, src_t, rel_t, w_t, reinterpret_cast<const char*>(pn_fwd)};

@@ -11,15 +11,16 @@
 // full/empty mbarriers); warpgroups 1 and 2 = consumers, 64 rows each: one full-width wgmma.mma_async m64n{NP}k16
 // from shared memory per product and K step (NP = n_pad rounded up to an instantiated width: 64, 128, 208 or 256),
 // fp32 accumulator in registers, then the epilogue (bias + relu + score dot,
-// fp32 and bf16 hi/lo plane outputs, staged TMA stores or direct stores).  Clusters of 2 CTAs share the W tiles by
-// TMA multicast.
+// fp32 and bf16 hi/lo plane outputs, staged TMA stores or direct stores).  With tc_cluster = 2, clusters of 2 CTAs
+// share the W tiles by TMA multicast (single-CTA clusters measured faster and are the default).  GR_LINEAR_K_GROUPED
+// walks a segmented K in the fused layer kernel's k-block order (GroupedK, wgmma.cuh) and so returns its bits.
 //
 // Roofline: tensor-pipe work 3 * 2*M*N*K flop; HBM traffic ~ 2 planes * M*K*2 B = M*K*4 B (same as fp32 A).
 #include "wgmma.cuh"
 
 namespace gr {
 
-int g_tc_cluster = 2;      // gr_set_option("tc_cluster", 1|2): CTAs per cluster sharing W tiles by TMA multicast
+int g_tc_cluster = 1;      // gr_set_option("tc_cluster", 1|2): 2 = CTA pairs share the W tiles by TMA multicast
 int g_tc_bk = 32;          // gr_set_option("tc_bk", 32|64): k-block width (64B / 128B swizzle)
 int g_tc_tma_store = 1;    // gr_set_option("tc_tma_store", 0|1): staged TMA-store epilogue vs direct per-row stores
 
@@ -103,6 +104,9 @@ struct TcParams {
   int M, N, K, n_pad, n16, stages, num_tiles;   // n_pad = round16(N): the epilogue skips the columns beyond it
   uint32_t flags;
   int tma_store;            // 1: epilogue stages 64x16 chunks in smem and writes them with TMA stores
+  // GR_LINEAR_K_GROUPED (the GROUPED instantiations; kg_T = 0 otherwise): T segments of kg_pitch columns walked in kg_G
+  // column groups (GroupedK, wgmma.cuh); the k-blocks from kg_half on are one k-step
+  int kg_T, kg_G, kg_pitch, kg_half;
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -110,8 +114,10 @@ struct TcParams {
 // consumers: each issues wgmma for its 64 rows of the tile, holds the accumulator in registers and runs the epilogue.
 // The producer runs up to `stages` k-blocks ahead, so the next tile's loads overlap this tile's epilogue.
 // ---------------------------------------------------------------------------------------------------
-// NP: accumulator width (W tile rows); CS: CTAs per cluster sharing W tiles by multicast; BK: k-block width
-template <int NP, int CS, int BK>
+// NP: accumulator width (W tile rows); CS: CTAs per cluster sharing W tiles by multicast; BK: k-block width;
+// GROUPED: k-block kb = g*T + t reads A at column seg(t)*pitch + 32g and W at column 32 kb -- the k-block sequence, and
+// so the per-element accumulation order, of fused_layer_kernel
+template <int NP, int CS, int BK, bool GROUPED>
 __global__ void __launch_bounds__(kThreads, 1)
 linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                  const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
@@ -138,7 +144,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   }
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nkb = (p.K + BK - 1) / BK;
+  const int nkb = GROUPED ? p.kg_G * p.kg_T : (p.K + BK - 1) / BK;
   const int crank = CS > 1 ? (int)cluster_ctarank() : 0;
   const int ncluster = gridDim.x / CS, cid = blockIdx.x / CS;
   const int ngroups = (p.num_tiles + CS - 1) / CS;       // tile groups: CS consecutive 128-row tiles
@@ -168,8 +174,14 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
           mbar_wait(&empty_bar[s], phase ^ 1);
           uint8_t* st = smem + (size_t)s * stage_bytes;
           mbar_expect_tx(&full_bar[s], (uint32_t)stage_bytes);
-          tma_load_2d(st, &map_a_hi, &full_bar[s], kb * BK, m0);
-          if (!single) tma_load_2d(st + a_bytes, &map_a_lo, &full_bar[s], kb * BK, m0);
+          int a_col = kb * BK;
+          if constexpr (GROUPED) {
+            const int g = kb / p.kg_T, t = kb - g * p.kg_T, ni = p.kg_T >> 1;
+            const int seg = t == 0 ? 0 : 1 + 2 * ((t - 1) % ni) + (t - 1) / ni;
+            a_col = seg * p.kg_pitch + g * BK;
+          }
+          tma_load_2d(st, &map_a_hi, &full_bar[s], a_col, m0);
+          if (!single) tma_load_2d(st + a_bytes, &map_a_lo, &full_bar[s], a_col, m0);
           if (CS == 1) {
             tma_load_2d(st + w_off, &map_w_hi, &full_bar[s], kb * BK, 0);
             if (!single) tma_load_2d(st + w_off + w_bytes, &map_w_lo, &full_bar[s], kb * BK, 0);
@@ -209,8 +221,15 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
         const uint32_t a_row = (uint32_t)(cw * WG_M * BK * 2);
         const uint64_t da_hi = make_smem_desc<BK>(sa + a_row), da_lo = make_smem_desc<BK>(sa + a_bytes + a_row);
         const uint64_t dw_hi = make_smem_desc<BK>(sa + w_off), dw_lo = make_smem_desc<BK>(sa + w_off + w_bytes);
-        if (single) mma_kblock<NP, BK, BK / MMA_K, true>(acc, da_hi, da_lo, dw_hi, dw_lo);
-        else mma_kblock<NP, BK, BK / MMA_K, false>(acc, da_hi, da_lo, dw_hi, dw_lo);
+        if constexpr (GROUPED) {
+          // the last column group of a 16-column-padded segment holds one k-step: its own straight-line batch
+          if (kb >= p.kg_half) mma_kblock<NP, BK, 1, false>(acc, da_hi, da_lo, dw_hi, dw_lo);
+          else mma_kblock<NP, BK, BK / MMA_K, false>(acc, da_hi, da_lo, dw_hi, dw_lo);
+        } else if (single) {
+          mma_kblock<NP, BK, BK / MMA_K, true>(acc, da_hi, da_lo, dw_hi, dw_lo);
+        } else {
+          mma_kblock<NP, BK, BK / MMA_K, false>(acc, da_hi, da_lo, dw_hi, dw_lo);
+        }
         wgmma_wait<1>();                                 // the previous k-block's products are done: free its slot
         if (prev >= 0 && lane == 0) release_slot<CS>(&empty_bar[prev]);
         prev = s;
@@ -315,19 +334,23 @@ int split_launch(const float* A, int64_t lda, int64_t M, int64_t K, __nv_bfloat1
   return GR_OK;
 }
 
-template <int NP, int CS, int BK>
+template <int NP, int CS, int BK, bool GROUPED = false>
 int launch_tc_cs(const CUtensorMap& m_a_hi, const CUtensorMap& m_a_lo, const CUtensorMap& m_w_hi,
                  const CUtensorMap& m_w_lo, const CUtensorMap& m_c, const CUtensorMap& m_c_hi,
                  const CUtensorMap& m_c_lo, const TcPlan& t, const TcParams& p, cudaStream_t stream) {
   const int ngroups = (p.num_tiles + CS - 1) / CS;
   const int nclusters = std::max(1, std::min(ngroups, sm_count() / CS));
-  return launch_cluster<linear_tc_kernel<NP, CS, BK>>("gr_linear_tc", kLaunchRegs, CS, nclusters * CS, kThreads,
-                                                      t.smem_bytes, stream, m_a_hi, m_a_lo, m_w_hi, m_w_lo, m_c,
-                                                      m_c_hi, m_c_lo, p);
+  return launch_cluster<linear_tc_kernel<NP, CS, BK, GROUPED>>("gr_linear_tc", kLaunchRegs, CS, nclusters * CS, kThreads,
+                                                               t.smem_bytes, stream, m_a_hi, m_a_lo, m_w_hi, m_w_lo,
+                                                               m_c, m_c_hi, m_c_lo, p);
 }
 
 template <int NP>
 int launch_tc_np(const CUtensorMap* const (&m)[7], int cs, const TcPlan& t, const TcParams& p, cudaStream_t stream) {
+  if (p.kg_T) {
+    if (cs == 2) return launch_tc_cs<NP, 2, 32, true>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], t, p, stream);
+    return launch_tc_cs<NP, 1, 32, true>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], t, p, stream);
+  }
   if (t.bk == 64) {
     if (cs == 2) return launch_tc_cs<NP, 2, 64>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], t, p, stream);
     return launch_tc_cs<NP, 1, 64>(*m[0], *m[1], *m[2], *m[3], *m[4], *m[5], *m[6], t, p, stream);
@@ -344,9 +367,10 @@ int launch_tc(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int64_t lda1
   // cluster multicast of W needs 8-row-aligned W slices and at least two tiles
   int cs = (g_tc_cluster >= 2 && (t.np / 2) % 8 == 0 && p.num_tiles >= 2) ? 2 : 1;
   CUtensorMap m_a_hi, m_a_lo, m_w_hi, m_w_lo;
+  const int64_t w_cols = p.kg_T ? ldw16 : p.K;           // grouped order: dense planes of kg_G * kg_T * 32 columns
   if (!make_tmap(&m_a_hi, a_hi, p.M, p.K, lda16, BM, t.bk) || !make_tmap(&m_a_lo, a_lo, p.M, p.K, lda16, BM, t.bk) ||
-      !make_tmap(&m_w_hi, w_hi, p.N, p.K, ldw16, t.np / cs, t.bk) ||
-      !make_tmap(&m_w_lo, w_lo, p.N, p.K, ldw16, t.np / cs, t.bk)) {
+      !make_tmap(&m_w_hi, w_hi, p.N, w_cols, ldw16, t.np / cs, t.bk) ||
+      !make_tmap(&m_w_lo, w_lo, p.N, w_cols, ldw16, t.np / cs, t.bk)) {
     set_error("gr_linear_tc: cuTensorMapEncodeTiled failed (pointers must be 16-byte aligned, row strides "
               "multiples of 8 elements)");
     return GR_ERR_CUDA;
@@ -442,7 +466,16 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
   GR_CHECK_ARG(A_hi && (A_lo || (flags & GR_LINEAR_BF16_SINGLE)) && W && workspace, "null pointer");
   GR_CHECK_ARG(C || C_hi, "no output requested");
   GR_CHECK_ARG(M > 0 && N > 0 && K > 0, "M, N, K must be positive");
-  const bool segmented = k_seg > 0 && k_seg_pitch > k_seg;
+  const bool grouped = (flags & GR_LINEAR_K_GROUPED) != 0;
+  if (grouped) {
+    GR_CHECK_ARG(k_seg > 0 && k_seg_pitch >= k_seg && k_seg_pitch % 16 == 0,
+                 "GR_LINEAR_K_GROUPED needs segmented K: k_seg > 0 and k_seg_pitch >= k_seg, a multiple of 16");
+    GR_CHECK_ARG(K % k_seg_pitch == 0 && (K / k_seg_pitch) % 2 == 1,
+                 "GR_LINEAR_K_GROUPED needs an odd number of segments (2 I + 1)");
+    GR_CHECK_ARG(g_tc_bk != 64, "GR_LINEAR_K_GROUPED needs 32-column k-blocks (tc_bk = 32)");
+    GR_CHECK_ARG(!(flags & GR_LINEAR_BF16_SINGLE), "GR_LINEAR_K_GROUPED does not combine with GR_LINEAR_BF16_SINGLE");
+  }
+  const bool segmented = grouped || (k_seg > 0 && k_seg_pitch > k_seg);
   GR_CHECK_ARG(lda16 >= K && lda16 % 8 == 0, "lda16 must be >= K and a multiple of 8");
   GR_CHECK_ARG(!segmented || K % k_seg_pitch == 0, "K must be a multiple of k_seg_pitch");
   GR_CHECK_ARG(ldw >= (segmented ? K / k_seg_pitch * k_seg : K), "ldw smaller than the weight row length");
@@ -456,16 +489,22 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
               (long long)K);
     return GR_ERR_UNSUPPORTED;
   }
-  if (workspace_bytes < t.w_only_bytes || (reinterpret_cast<uintptr_t>(workspace) & 255) != 0) {
+  // grouped order: the W planes gr_fused_layer keeps (same layout, same size: one workspace serves both)
+  const int num_ins = grouped ? (int)(K / k_seg_pitch / 2) : 0;
+  const GroupedK gk = grouped ? plan_grouped_k(k_seg_pitch, num_ins, N) : GroupedK{};
+  const size_t w_plane_bytes = grouped ? gk.w_plane_bytes : t.w_plane_bytes;
+  if (workspace_bytes < 2 * w_plane_bytes || (reinterpret_cast<uintptr_t>(workspace) & 255) != 0) {
     set_error("gr_linear_tc_planes: workspace too small or not 256-byte aligned");
     return GR_ERR_WORKSPACE;
   }
   char* ws = reinterpret_cast<char*>(workspace);
   __nv_bfloat16* w_hi = reinterpret_cast<__nv_bfloat16*>(ws);
-  __nv_bfloat16* w_lo = reinterpret_cast<__nv_bfloat16*>(ws + t.w_plane_bytes);
+  __nv_bfloat16* w_lo = reinterpret_cast<__nv_bfloat16*>(ws + w_plane_bytes);
   int rc = GR_OK;
   if (flags & GR_LINEAR_W_PRESPLIT) {
     // the caller kept the workspace of an earlier call with the same W / N / K / k_seg / k_seg_pitch
+  } else if (grouped) {
+    rc = grouped_w_split(W, ldw, N, (int)k_seg, num_ins, gk, w_hi, w_lo, stream);
   } else if (segmented) {
     int64_t work = N * K;
     int grid = (int)std::min<int64_t>(ceil_div(work, 256), 32LL * sm_count());
@@ -480,6 +519,11 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
   p.c_hi = reinterpret_cast<__nv_bfloat16*>(C_hi); p.c_lo = reinterpret_cast<__nv_bfloat16*>(C_lo);
   p.ldc16 = ldc16; p.w_score = w_score; p.dots = dots;
   p.M = (int)M; p.N = (int)N; p.K = (int)K; p.flags = flags;
+  if (grouped) {
+    p.kg_T = 2 * num_ins + 1; p.kg_G = gk.G; p.kg_pitch = (int)k_seg_pitch;
+    p.kg_half = gk.ksteps_last == 1 ? (gk.G - 1) * p.kg_T : gk.G * p.kg_T;
+  }
   return launch_tc(reinterpret_cast<const __nv_bfloat16*>(A_hi),
-                   reinterpret_cast<const __nv_bfloat16*>(A_lo ? A_lo : A_hi), lda16, w_hi, w_lo, t.kp, t, p, stream);
+                   reinterpret_cast<const __nv_bfloat16*>(A_lo ? A_lo : A_hi), lda16, w_hi, w_lo,
+                   grouped ? gk.kp : t.kp, t, p, stream);
 }

@@ -20,6 +20,23 @@ constexpr int BM = 128;          // rows per CTA tile: two consumer warpgroups o
 constexpr int WG_M = 64;         // rows per consumer warpgroup (wgmma M)
 constexpr int MMA_K = 16;
 
+// Grouped K order of a dense ReaRev layer.  The layer input is T = 2I + 1 segments [h | nb_0-> | nb_0<- | nb_1-> | ...]
+// of `pitch` columns each.  In grouped order K is walked in G = ceil(pitch / 32) column groups; group g holds the
+// 32-column block g of every segment: k-block g*T + t is columns 32g .. 32g+31 of segment seg(t), seg(0) = 0 (h) and
+// seg(t) = 1 + 2*((t-1) % I) + (t-1) / I (direction 0 for every instruction, then direction 1).  The W planes of this
+// order are [N, G*T*32] bf16 hi/lo, k-block kb at columns 32 kb, zero beyond D inside each block.  When the last group
+// of a segment holds 16 columns (ksteps_last == 1) its k-blocks are ONE k-step.  gr_fused_layer and
+// gr_linear_tc_planes (GR_LINEAR_K_GROUPED) share this plan, these planes and therefore the fp32 accumulation order
+// of every output element.  Defined in fused_layer.cu.
+struct GroupedK {
+  int G, ksteps_last;
+  int64_t kp;                    // columns of the W planes: G * T * 32
+  size_t w_plane_bytes;
+};
+GroupedK plan_grouped_k(int64_t pitch, int I, int64_t N_out);
+int grouped_w_split(const float* W, int64_t ldw, int64_t N_out, int D, int I, const GroupedK& k, __nv_bfloat16* hi,
+                    __nv_bfloat16* lo, cudaStream_t stream);
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,

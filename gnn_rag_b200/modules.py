@@ -428,11 +428,11 @@ class ReasonGNNLayer(_GraphLayerBase):
         e2e = getattr(self, "e2e_linear" + str(step))
         if (self.use_planes and pn is not None and ops.AGG_ABS and ops.FUSED_LAYER and not ops.ACT_BF16
                 and self.B * self.N >= ops.FUSED_MIN_ROWS and ops.fused_layer_supported(self.N, D, self.Dp, self.num_ins, D)):
-            # aggregation produced straight into the GEMM's operand stages: the neighbour segments never reach HBM
+            # the dense layer in grouped K order: one fused kernel, or the aggregation kernel + the full-width GEMM
             sw, sb = self.score_func.weight.view(-1), self.score_func.bias
-            ops.fused_layer(g, current_dist, pn[0], pn[1], relational_ins, self.cur_planes(), self.Dp, e2e.weight,
+            ops.dense_layer(g, current_dist, pn[0], pn[1], relational_ins, self.cur_planes(), self.Dp, e2e.weight,
                             e2e.bias, out=self.h32 if need_h else None, out_planes=tuple(self.P[1 - self.cur]),
-                            w_score=sw, dots=self.dots, relu=True, w_t=wt, w_h=wh)
+                            w_score=sw, dots=self.dots, w_t=wt, w_h=wh)
             self.h32_valid = bool(need_h)
             self.cur = 1 - self.cur
             dist = ops.masked_softmax(self.dots, sb, self.local_entity_mask, self.B, self.N)

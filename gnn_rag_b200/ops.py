@@ -17,6 +17,7 @@ LINEAR_RELU = 1
 LINEAR_EXACT_FP32 = 2
 LINEAR_W_PRESPLIT = 4
 LINEAR_BF16_SINGLE = 8
+LINEAR_K_GROUPED = 16
 
 # bf16 ACTIVATION STORAGE (BASELINE configs[2], "bf16"): the layer-input matrix keeps its hi plane only -- the aggregation
 # kernel skips the lo plane (half the output bytes) and the e2e GEMM runs ONE bf16 product instead of three.  Tables,
@@ -404,7 +405,11 @@ def aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, out_col0, seg_pitc
             out_col0, seg_pitch, B, g.N, D, I, g.F, _p(_TILE_COUNTER[dev]), launches=(I + 3) // 4, agg=("dual", I))
 
 
-FUSED_LAYER = True      # dense-prior ReaRev layers: aggregation fused into the e2e GEMM (csrc/fused_layer.cu)
+FUSED_LAYER = True      # dense-prior ReaRev layers run in grouped K order (the k-block order of csrc/fused_layer.cu)
+# Which kernels run such a layer (ops.dense_layer).  gr_fused_layer issues an accumulator wider than 128 columns as
+# 32-column wgmma instructions; for those widths (D = 200: 208 columns) the aggregation kernel followed by the full-width
+# GEMM in the same K order gives the same bits faster (scripts/dense_layer_probe.py).  False: gr_fused_layer at every width.
+DENSE_WIDE_AS_PAIR = True
 FUSED_MIN_ROWS = 132 * 128   # below one 128-row tile per SM the fused kernel's serial per-tile chain (35 dependent k-blocks)
                              # loses to the two wide kernels
 
@@ -452,6 +457,22 @@ def fused_layer(g, prior, pn_fwd, pn_inv, ins, h_planes, seg_pitch, W, bias, out
             launches=2 if (w_t is not None or w_h is not None) else 1,     # weighted graphs: + the coefficient pass
             op="fused_layer")
     return out
+
+
+def dense_layer(g, prior, pn_fwd, pn_inv, ins, planes, seg_pitch, W, bias, out=None, out_planes=None, w_score=None,
+                dots=None, w_t=None, w_h=None):
+    """One dense-prior ReaRev layer in grouped K order: ``relu(e2e([h | nb...]))`` with the score dot.  ``planes`` =
+    (hi, lo) layer-input planes [M, >= (2I+1) * seg_pitch] whose first segment holds h.  Accumulators of more than 128
+    columns run as :func:`aggregate_dual_abs` into the neighbour segments of ``planes`` + :func:`linear_tc_planes` in
+    grouped order, the others as :func:`fused_layer`; the outputs are the same bits either way."""
+    I, n_out = ins.shape[1], W.shape[0]
+    if DENSE_WIDE_AS_PAIR and (n_out + 15) // 16 * 16 > 128:
+        aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, seg_pitch, seg_pitch, w_t, w_h)
+        return linear_tc_planes(planes[0], planes[1], (2 * I + 1) * seg_pitch, W, bias, out=out, out_planes=out_planes,
+                                w_score=w_score, dots=dots, relu=True, k_seg=ins.shape[2], k_seg_pitch=seg_pitch,
+                                k_grouped=True)
+    return fused_layer(g, prior, pn_fwd, pn_inv, ins, planes, seg_pitch, W, bias, out=out, out_planes=out_planes,
+                       w_score=w_score, dots=dots, relu=True, w_t=w_t, w_h=w_h)
 
 
 def type_layer(g, table, out, w_t=None, w_h=None, planes=None):
@@ -542,13 +563,15 @@ def live_weight_workspaces():
 
 
 def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=None, dots=None, relu=True,
-                     k_seg=0, k_seg_pitch=0, single_ok=False):
+                     k_seg=0, k_seg_pitch=0, single_ok=False, k_grouped=False):
     """wgmma split-bf16 GEMM whose A operand already lives in bf16 hi/lo planes [M, >=K] (shapes:
     :func:`tc_planes_ok`).
     ``single_ok``: this call may run as ONE bf16 product when ``ACT_BF16`` is on (the node-update GEMMs; the small
     relation-table GEMMs always keep the three-product fp32-class path).
     Writes any of: fp32 ``out`` [M,N]; ``out_planes`` (hi, lo) [M, >=N] (next layer's h columns);
     ``dots`` [2*M] = the two column-half partial sums of out @ w_score.
+    ``k_grouped``: walk the K segments column group by column group (GR_LINEAR_K_GROUPED): the accumulation order, the
+    W planes and the cached workspace of :func:`fused_layer`; always the three-product path.
     N > 256 (cfg5: entity_dim 400) is tiled over the output columns: one launch per slice of W rows."""
     N = W.shape[0]
     if N > TC_MAX_N:
@@ -562,7 +585,7 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
                              out=None if out is None else out[:, n0:n1],
                              out_planes=None if out_planes is None else (out_planes[0][:, n0:n1], out_planes[1][:, n0:n1]),
                              w_score=None if w_score is None else w_score[n0:n1], dots=d, relu=relu, k_seg=k_seg,
-                             k_seg_pitch=k_seg_pitch, single_ok=single_ok)
+                             k_seg_pitch=k_seg_pitch, single_ok=single_ok, k_grouped=k_grouped)
             if dots is not None and n0 > 0:
                 part = d if part is None else part + d
         if part is not None:
@@ -575,11 +598,15 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
     else:
         assert W.shape[1] == K
     assert W.stride(1) == 1
-    nbytes = _L().gr_linear_tc_planes_workspace_bytes(N, K)
-    ws, presplit = _weight_ws(W, N, K, k_seg, k_seg_pitch, nbytes)
+    if k_grouped:                   # fused_layer's W planes, under fused_layer's cache key
+        nbytes = _L().gr_fused_layer_workspace_bytes(k_seg, k_seg_pitch, K // k_seg_pitch // 2, N)
+        ws, presplit = _weight_ws(W, N, W.shape[1], "fused", k_seg_pitch, nbytes)
+    else:
+        nbytes = _L().gr_linear_tc_planes_workspace_bytes(N, K)
+        ws, presplit = _weight_ws(W, N, K, k_seg, k_seg_pitch, nbytes)
     chi, clo = out_planes if out_planes is not None else (None, None)
     flags = (LINEAR_RELU if relu else 0) | (LINEAR_W_PRESPLIT if presplit else 0) | \
-        (LINEAR_BF16_SINGLE if (ACT_BF16 and single_ok) else 0)
+        (LINEAR_K_GROUPED if k_grouped else LINEAR_BF16_SINGLE if (ACT_BF16 and single_ok) else 0)
     _launch("gr_linear_tc_planes", _p(a_hi), _p(a_lo), a_hi.stride(0), _p(W), W.stride(0), _p(bias),
             _p(out), out.stride(0) if out is not None else 0,
             _p(chi), _p(clo), chi.stride(0) if chi is not None else 0,

@@ -51,9 +51,18 @@ typedef enum gr_status {
                                   * For inference with fixed weights (weight pre-formatting, done once per weight
                                   * version by the caller). */
 
+#define GR_LINEAR_K_GROUPED 16u /* gr_linear_tc_planes: walk the T = K / k_seg_pitch segments of A column group by
+                                  * column group, k-block g*T + t = columns 32g.. of segment seg(t) -- the k-block
+                                  * order of gr_fused_layer, so that every output element sees the same sequence of
+                                  * fp32 accumulations and the outputs equal gr_fused_layer's bit for bit.  Needs
+                                  * k_seg > 0, k_seg_pitch >= k_seg and a multiple of 16, T odd (2 I + 1) and "tc_bk"
+                                  * 32; not with GR_LINEAR_BF16_SINGLE.  The workspace is the one of gr_fused_layer
+                                  * (gr_fused_layer_workspace_bytes(k_seg, k_seg_pitch, I, N)): same W planes, so
+                                  * GR_LINEAR_W_PRESPLIT carries over between the two entry points. */
+
 int gr_abi_version(void);
 const char* gr_last_error(void);
-/* runtime switches: "agg_tma" (0|1: stage CSR slices with bulk TMA copies), "tc_cluster" (1|2: CTAs per cluster
+/* runtime switches: "agg_tma" (0|1: stage CSR slices with bulk TMA copies), "tc_cluster" (1|2, default 1: CTAs per cluster
  * that share the W tiles of the wgmma GEMM through TMA multicast), "tc_bk" (32|64: k-block width of the wgmma GEMM),
  * "tc_tma_store" (0|1: TMA-store epilogue of the wgmma GEMM where the outputs are 16-byte aligned), "agg_abs_ws"
  * (0|1|2|3: build of the |v| aggregation kernel, see gr_aggregate_dual_abs), "fused_debug" (bits: timing decomposition
@@ -223,7 +232,8 @@ int gr_aggregate_dual_abs(const int32_t* rowptr_t, const int32_t* src_t, const i
  *                  (dots[m] = <out[m], w_score>, dots[B*N + m] = 0: the layout gr_masked_softmax takes)
  * Supported (gr_fused_layer_supported): I <= 2, N >= 128, seg_pitch % 16 == 0, seg_pitch <= 224, N_out <= 256 and the
  * operand stages must fit shared memory (D = N_out = 200 does).  The A operand is bit-identical to the unfused pair;
- * the tensor core accumulates the k-blocks in a different order (fp32 rounding). */
+ * the tensor core accumulates the k-blocks in another order than the pair's default (fp32 rounding), and in the same
+ * order as the pair with GR_LINEAR_K_GROUPED, whose outputs equal this kernel's bit for bit. */
 /* Diagnostic: per-CTA wait-cycle counters of the last gr_fused_layer launch made with gr_set_option("fused_debug", 32)
  * (16 uint64 per CTA, slot meaning in csrc/fused_layer.cu). */
 int gr_fused_profile_read(unsigned long long* out, int n);

@@ -24,7 +24,8 @@
 //     lanes that own real columns (3 wavefronts instead of 4); edges are taken two at a time with an unpadded
 //     single-edge tail.
 //   * output: the split-bf16 planes of the e2e GEMM's A operand, segment pitch SEGP (32-byte sectors, see
-//     aggregate.cu); columns D..SEGP-1 receive exact zeros (staged ins are zero there).
+//     aggregate.cu); columns D..SEGP-1 receive exact zeros (staged ins are zero there).  With GR_AGG_K_ORDER (template
+//     flag KO of every kernel) the same values go to the K-order layout of the dense layer's GEMM (ko_lane).
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -133,12 +134,32 @@ struct LaneIns {
   }
 };
 
+// K-order layout (GR_AGG_K_ORDER, KO): this lane's columns relative to the neighbour region.  Chunk 0 (columns lane*4 ..)
+// of slot u lies at c0 + 32 u; chunk 1 (128 + lane*4 ..) at c1 + s1 u: s1 = 32 inside the full 32-column groups, 16 in
+// the tail.  A lane's 4 columns never cross a 32-column group, so each store stays one 8-byte piece.
+struct KoLane {
+  int c0, c1, s1;
+};
+template <int SEGP>
+__device__ __forceinline__ KoLane ko_lane(int lane, int I) {
+  constexpr int GF = SEGP / 32;
+  static_assert(SEGP % 16 == 0 && SEGP - 32 * GF <= 16, "a 16-column tail at most");
+  const int k0 = lane * 4, k1 = 128 + lane * 4;
+  KoLane l;
+  l.c0 = (k0 >> 5) * 64 * I + (k0 & 31);
+  if (k1 < 32 * GF) { l.c1 = (k1 >> 5) * 64 * I + (k1 & 31); l.s1 = 32; }
+  else { l.c1 = GF * 64 * I + (k1 - 32 * GF); l.s1 = 16; }
+  return l;
+}
+
 // One (destination row, direction) unit: gather + accumulate the row's in-edges, then emit the NI instruction
 // segments.  rc: staged {table byte offset, coefficient} of the tile's edge slice; [beg, end) the row's range in it.
-template <int NI, int DT, int SEGP, bool LO = true>
+// KO: hrow / lrow point at the row's neighbour region and seg_d is the slot of the unit's first instruction
+template <int NI, int DT, int SEGP, bool LO = true, bool KO = false>
 __device__ __forceinline__ void row_unit(const int2* __restrict__ rc, int beg, int end, int ebase, const PnDir& dd,
                                          const float* __restrict__ prior, const char* tb, const LaneIns<NI>& x,
-                                         __nv_bfloat16* hrow, __nv_bfloat16* lrow, int seg_d, bool ld1, bool wr1) {
+                                         __nv_bfloat16* hrow, __nv_bfloat16* lrow, int seg_d, bool ld1, bool wr1,
+                                         KoLane ko = KoLane{}) {
   float4 S0 = zero4(), S1 = S0, Q0 = S0, Q1 = S0;
   float4 v01 = zero4(), v11 = zero4();                     // lanes without chunk-1 columns never overwrite these
   const int fast_end = min(end, kEdgeCap);
@@ -174,9 +195,15 @@ __device__ __forceinline__ void row_unit(const int2* __restrict__ rc, int beg, i
   const float4 U1 = addsub4(Q1, S1, 1.f), V1 = addsub4(Q1, S1, -1.f);
 #pragma unroll
   for (int j = 0; j < NI; ++j) {
-    const int seg = seg_d + j * 2 * SEGP;
-    emit4<LO>(hrow + seg, lrow + seg, true, x.xp[j][0], x.xn[j][0], U0, V0);
-    emit4<LO>(hrow + seg + 128, lrow + seg + 128, wr1, x.xp[j][1], x.xn[j][1], U1, V1);
+    if constexpr (KO) {
+      const int o0 = ko.c0 + 32 * (seg_d + j), o1 = ko.c1 + ko.s1 * (seg_d + j);
+      emit4<LO>(hrow + o0, lrow + o0, true, x.xp[j][0], x.xn[j][0], U0, V0);
+      emit4<LO>(hrow + o1, lrow + o1, wr1, x.xp[j][1], x.xn[j][1], U1, V1);
+    } else {
+      const int seg = seg_d + j * 2 * SEGP;
+      emit4<LO>(hrow + seg, lrow + seg, true, x.xp[j][0], x.xn[j][0], U0, V0);
+      emit4<LO>(hrow + seg + 128, lrow + seg + 128, wr1, x.xp[j][1], x.xn[j][1], U1, V1);
+    }
   }
 }
 
@@ -199,7 +226,7 @@ __device__ __forceinline__ void stage_ins(float (*x)[NI][2][kPnCols], const PnPa
 // ---------------------------------------------------------------------------------------------------------
 // One CTA per 64-row tile (used when the caller passes no tile counter)
 // ---------------------------------------------------------------------------------------------------------
-template <int NI, int DT, int SEGP>
+template <int NI, int DT, int SEGP, bool KO = false>
 __global__ void __launch_bounds__(kThreads, 2) agg_abs_kernel(const PnParams p) {
   static_assert(DT % 4 == 0 && DT > 128 && DT <= kPnCols, "two column chunks of 128");
   __shared__ int32_t s_rowptr[2][kRows + 1];
@@ -254,8 +281,12 @@ __global__ void __launch_bounds__(kThreads, 2) agg_abs_kernel(const PnParams p) 
   const char* tb[2];
 #pragma unroll
   for (int d = 0; d < 2; ++d) tb[d] = reinterpret_cast<const char*>(p.dir[d].pn) + lane * 16;
-  __nv_bfloat16* const hi_lane = p.out_hi + r0 * p.ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
-  __nv_bfloat16* const lo_lane = p.out_lo + r0 * p.ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
+  // KO: the row's neighbour region, the lane's columns come from ko
+  __nv_bfloat16* const hi_lane = KO ? p.out_hi + r0 * p.ld + p.out_col0
+                          : p.out_hi + r0 * p.ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
+  __nv_bfloat16* const lo_lane = KO ? p.out_lo + r0 * p.ld + p.out_col0
+                          : p.out_lo + r0 * p.ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
+  const KoLane ko = KO ? ko_lane<SEGP>(lane, p.I) : KoLane{};
   const int lr_switch = N - rem0;                            // first tile row of question b0 + 1 (N >= kRows)
   LaneIns<NI> x;
   int cur_q = -1;
@@ -274,17 +305,20 @@ __global__ void __launch_bounds__(kThreads, 2) agg_abs_kernel(const PnParams p) 
       if (!s_any[d][lr]) {
 #pragma unroll
         for (int j = 0; j < NI; ++j) {
-          const int seg = d * SEGP + j * 2 * SEGP;
+          const int u = d * p.I + p.j0 + j;
+          const int seg = KO ? ko.c0 + 32 * u : d * SEGP + j * 2 * SEGP;
+          const int seg1 = KO ? ko.c1 + ko.s1 * u : seg + 128;
           *reinterpret_cast<uint2*>(hrow + seg) = make_uint2(0u, 0u);
           *reinterpret_cast<uint2*>(lrow + seg) = make_uint2(0u, 0u);
           if (wr1) {
-            *reinterpret_cast<uint2*>(hrow + seg + 128) = make_uint2(0u, 0u);
-            *reinterpret_cast<uint2*>(lrow + seg + 128) = make_uint2(0u, 0u);
+            *reinterpret_cast<uint2*>(hrow + seg1) = make_uint2(0u, 0u);
+            *reinterpret_cast<uint2*>(lrow + seg1) = make_uint2(0u, 0u);
           }
         }
         continue;
       }
-      row_unit<NI, DT, SEGP>(s_rc[d], beg, end, ebase, p.dir[d], p.prior, tb[d], x, hrow, lrow, d * SEGP, ld1, wr1);
+      row_unit<NI, DT, SEGP, true, KO>(s_rc[d], beg, end, ebase, p.dir[d], p.prior, tb[d], x, hrow, lrow,
+                                       KO ? d * p.I + p.j0 : d * SEGP, ld1, wr1, ko);
     }
   }
 }
@@ -401,7 +435,7 @@ __device__ __forceinline__ void produce_tile_rows(Buf& bf, const PnParams& p, in
 // against 131 us for 8 + 1 / 64 rows).  More warps do not help: 11 + 1 at 80 registers 143 us, 19 + 1 in one CTA
 // 164 us, 7 + 1 x 3 CTAs 148 us (profiles/r2_agg_modes.txt).
 // ---------------------------------------------------------------------------------------------------------
-template <int NI, int DT, int SEGP, int KW, int ROWS, int MINB, bool LO>
+template <int NI, int DT, int SEGP, int KW, int ROWS, int MINB, bool LO, bool KO = false>
 __global__ void __launch_bounds__((KW + 1) * 32, MINB) agg_abs_wsg_kernel(const PnParams p, int ntiles) {
   using Buf = HBuf<NI, ROWS>;
   extern __shared__ __align__(16) unsigned char ws_smem[];
@@ -439,6 +473,7 @@ __global__ void __launch_bounds__((KW + 1) * 32, MINB) agg_abs_wsg_kernel(const 
   const char* tb[2];
 #pragma unroll
   for (int d = 0; d < 2; ++d) tb[d] = reinterpret_cast<const char*>(p.dir[d].pn) + lane * 16;
+  const KoLane ko = KO ? ko_lane<SEGP>(lane, p.I) : KoLane{};
   LaneIns<NI> x;
   for (int it = 0;; ++it) {
     Buf& bf = bufs[it & 1];
@@ -449,8 +484,10 @@ __global__ void __launch_bounds__((KW + 1) * 32, MINB) agg_abs_wsg_kernel(const 
     const int nrows = (int)min((int64_t)ROWS, p.Nt - r0);
     const int b0 = (int)(r0 / N);
     const int lr_switch = N - (int)(r0 - (int64_t)b0 * N);
-    __nv_bfloat16* const hi_lane = p.out_hi + r0 * p.ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
-    __nv_bfloat16* const lo_lane = p.out_lo + r0 * p.ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
+    __nv_bfloat16* const hi_lane = KO ? p.out_hi + r0 * p.ld + p.out_col0
+                          : p.out_hi + r0 * p.ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
+    __nv_bfloat16* const lo_lane = KO ? p.out_lo + r0 * p.ld + p.out_col0
+                          : p.out_lo + r0 * p.ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
     int cur_q = -1;
     for (int lr = warp; lr < nrows; lr += KW) {
       const int q = lr >= lr_switch ? 1 : 0;
@@ -464,8 +501,8 @@ __global__ void __launch_bounds__((KW + 1) * 32, MINB) agg_abs_wsg_kernel(const 
       for (int d = 0; d < 2; ++d) {
         const int ebase = bf.rowptr[d][0];
         const int beg = bf.rowptr[d][lr] - ebase, end = bf.rowptr[d][lr + 1] - ebase;
-        row_unit<NI, DT, SEGP, LO>(bf.rc[d], beg, end, ebase, p.dir[d], p.prior, tb[d], x, hrow, lrow, d * SEGP, ld1,
-                                   wr1);
+        row_unit<NI, DT, SEGP, LO, KO>(bf.rc[d], beg, end, ebase, p.dir[d], p.prior, tb[d], x, hrow, lrow,
+                                       KO ? d * p.I + p.j0 : d * SEGP, ld1, wr1, ko);
       }
     }
     mbar_arrive(&s_empty[it & 1]);
@@ -524,7 +561,7 @@ struct alignas(16) G5Buf {
 // unit takes one or two groups (its first <= 8 staged edges), its mbarrier is the one of its first group, and a flat
 // prefetch cursor keeps issuing ahead (across the tile boundary) while groups are free: 2-3 units in flight.
 // ---------------------------------------------------------------------------------------------------------
-template <int NI, int DT, int SEGP, int KW, int RPW>
+template <int NI, int DT, int SEGP, int KW, int RPW, bool KO = false>
 __global__ void __launch_bounds__((KW + 2) * 32, 1)
 agg_abs_g5_kernel(const PnParams p, int ntiles) {
   static_assert(DT % 4 == 0 && DT > 128 && DT <= kPnCols, "two column chunks of 128");
@@ -595,6 +632,7 @@ agg_abs_g5_kernel(const PnParams p, int ntiles) {
   // =============================== consumer warps ===============================
   const bool ld1 = 128 + lane * 4 < DT;
   const bool wr1 = 128 + lane * 4 < SEGP;
+  const KoLane ko = KO ? ko_lane<SEGP>(lane, p.I) : KoLane{};
   const uint32_t ring_s = smem_u32(ring_all) + (uint32_t)warp * 4u * kGroup;   // this warp's four groups
   const uint32_t ring_lane = ring_s + lane * 16;
   uint64_t* const bars = s_bar[warp];
@@ -616,8 +654,10 @@ agg_abs_g5_kernel(const PnParams p, int ntiles) {
     const int b0 = (int)(r0 / N);
     const int lr_switch = N - (int)(r0 - (int64_t)b0 * N);
     const int64_t ld = p.ld;
-    __nv_bfloat16* hrow = p.out_hi + (r0 + warp) * ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
-    __nv_bfloat16* lrow = p.out_lo + (r0 + warp) * ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
+    __nv_bfloat16* hrow = KO ? p.out_hi + (r0 + warp) * ld + p.out_col0
+                          : p.out_hi + (r0 + warp) * ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
+    __nv_bfloat16* lrow = KO ? p.out_lo + (r0 + warp) * ld + p.out_col0
+                          : p.out_lo + (r0 + warp) * ld + p.out_col0 + lane * 4 + (int64_t)p.j0 * 2 * SEGP;
     if (pit < it) { pit = it; plr = warp; pd = 0; pnrows = nrows; }
     int cur_q = -1;
     for (int lr = warp; lr < nrows; lr += KW, hrow += KW * ld, lrow += KW * ld) {
@@ -717,9 +757,11 @@ agg_abs_g5_kernel(const PnParams p, int ntiles) {
         const float4 U1 = addsub4(Q1, S1, 1.f), V1 = addsub4(Q1, S1, -1.f);
 #pragma unroll
         for (int j = 0; j < NI; ++j) {
-          const int seg = d * SEGP + j * 2 * SEGP;
+          const int u = d * p.I + p.j0 + j;
+          const int seg = KO ? ko.c0 + 32 * u : d * SEGP + j * 2 * SEGP;
+          const int seg1 = KO ? ko.c1 + ko.s1 * u : seg + 128;
           emit4(hrow + seg, lrow + seg, true, x.xp[j][0], x.xn[j][0], U0, V0);
-          emit4(hrow + seg + 128, lrow + seg + 128, wr1, x.xp[j][1], x.xn[j][1], U1, V1);
+          emit4(hrow + seg1, lrow + seg1, wr1, x.xp[j][1], x.xn[j][1], U1, V1);
         }
       }
     }
@@ -741,9 +783,9 @@ __global__ void pad_table_kernel(const float* __restrict__ table, int64_t ldt, i
 }
 
 
-template <int NI, int KW, int ROWS, int MINB, bool LO>
+template <int NI, int KW, int ROWS, int MINB, bool LO, bool KO>
 int launch_wsg_lo(const PnParams& p, cudaStream_t stream) {
-  constexpr auto kern = agg_abs_wsg_kernel<NI, 200, 208, KW, ROWS, MINB, LO>;
+  constexpr auto kern = agg_abs_wsg_kernel<NI, 200, 208, KW, ROWS, MINB, LO, KO>;
   const size_t smem = 2 * sizeof(HBuf<NI, ROWS>);
   if (int rc = opt_in_smem<kern>(__func__, (int)smem)) return rc;
   GR_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), stream));
@@ -754,15 +796,17 @@ int launch_wsg_lo(const PnParams& p, cudaStream_t stream) {
   return GR_OK;
 }
 
-template <int NI, int KW, int ROWS, int MINB>
+template <int NI, int KW, int ROWS, int MINB, bool KO>
 int launch_wsg(const PnParams& p, cudaStream_t stream) {
-  // out_lo == NULL: bf16 activation storage (hi plane only)
-  return p.out_lo ? launch_wsg_lo<NI, KW, ROWS, MINB, true>(p, stream) : launch_wsg_lo<NI, KW, ROWS, MINB, false>(p, stream);
+  // out_lo == NULL: bf16 activation storage (hi plane only; the K-order layout always has both planes)
+  if constexpr (KO) return launch_wsg_lo<NI, KW, ROWS, MINB, true, true>(p, stream);
+  return p.out_lo ? launch_wsg_lo<NI, KW, ROWS, MINB, true, false>(p, stream)
+                  : launch_wsg_lo<NI, KW, ROWS, MINB, false, false>(p, stream);
 }
 
-template <int NI, int KW, int RPW>
+template <int NI, int KW, int RPW, bool KO>
 int launch_g4(const PnParams& p, cudaStream_t stream) {
-  constexpr auto kern = agg_abs_g5_kernel<NI, 200, 208, KW, RPW>;
+  constexpr auto kern = agg_abs_g5_kernel<NI, 200, 208, KW, RPW, KO>;
   const size_t smem = 128 + (size_t)KW * 16 * 200 * 4 + 2 * sizeof(G5Buf<NI, KW * RPW>);
   if (int rc = opt_in_smem<kern>(__func__, (int)smem)) return rc;
   GR_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), stream));
@@ -774,18 +818,19 @@ int launch_g4(const PnParams& p, cudaStream_t stream) {
 }
 
 // agg_abs_ws: 0 one CTA per 64-row tile | 1 persistent, 8 + 1 warps, 64-row tiles (the round-1 shape) |
-//             2 persistent, 9 + 1 warps, 72-row tiles (default) | 3 gather4 kernel (NI == 2 and table_rows given)
-template <int NI>
+//             2 persistent, 9 + 1 warps, 72-row tiles (default) | 3 gather4 kernel (NI == 2 and table_rows given).
+// KO: the neighbour segments in the K-order layout (GR_AGG_K_ORDER), every variant
+template <int NI, bool KO>
 int launch_pn(const PnParams& p, cudaStream_t stream) {
   if (p.tile_counter && g_opt_agg_abs_ws) {
     if constexpr (NI == 2) {
-      if (g_opt_agg_abs_ws == 3 && p.table_rows > 0 && p.out_lo) return launch_g4<2, 14, 4>(p, stream);
+      if (g_opt_agg_abs_ws == 3 && p.table_rows > 0 && p.out_lo) return launch_g4<2, 14, 4, KO>(p, stream);
     }
-    if (g_opt_agg_abs_ws == 1 || p.N < 72) return launch_wsg<NI, 8, 64, 2>(p, stream);   // a tile spans <= 2 questions
-    return launch_wsg<NI, 9, 72, 2>(p, stream);
+    if (g_opt_agg_abs_ws == 1 || p.N < 72) return launch_wsg<NI, 8, 64, 2, KO>(p, stream);   // a tile spans <= 2 questions
+    return launch_wsg<NI, 9, 72, 2, KO>(p, stream);
   }
   const unsigned grid = (unsigned)ceil_div(p.Nt, kRows);
-  agg_abs_kernel<NI, 200, 208><<<grid, kThreads, 0, stream>>>(p);
+  agg_abs_kernel<NI, 200, 208, KO><<<grid, kThreads, 0, stream>>>(p);
   GR_CHECK_LAUNCH();
   return GR_OK;
 }
@@ -809,24 +854,31 @@ extern "C" int gr_aggregate_dual_abs_supported(int N, int D, int64_t seg_pitch, 
   return (D == 200 && seg_pitch == 208 && N >= gr::kRows && R1 > 0 && R1 < (1 << 21)) ? 1 : 0;
 }
 
-extern "C" int gr_aggregate_dual_abs(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
-                                    const float* w_t, const int32_t* rowptr_h, const int32_t* src_h,
-                                    const int32_t* rel_h, const float* w_h, const float* prior,
-                                    const float* pn_fwd, const float* pn_inv, int64_t table_rows, const float* ins, void* out_hi,
-                                    void* out_lo, int64_t ld_planes, int64_t out_col0, int64_t seg_pitch, int B,
-                                    int N, int D, int I, int64_t F, int32_t* tile_counter, void* stream_) {
-  using namespace gr;
+namespace gr {
+namespace {
+// both entry points; errors are reported as `fn`
+int aggregate_dual_abs(const char* fn, const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                       const float* w_t, const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h,
+                       const float* w_h, const float* prior, const float* pn_fwd, const float* pn_inv,
+                       int64_t table_rows, const float* ins, void* out_hi, void* out_lo, int64_t ld_planes,
+                       int64_t out_col0, int64_t seg_pitch, int B, int N, int D, int I, int64_t F,
+                       int32_t* tile_counter, uint32_t flags, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(rowptr_t && rowptr_h && prior && pn_fwd && pn_inv && ins && out_hi, "null pointer");
+  GR_CHECK_ARG_AS(fn, rowptr_t && rowptr_h && prior && pn_fwd && pn_inv && ins && out_hi, "null pointer");
+  GR_CHECK_ARG_AS(fn, (flags & ~GR_AGG_K_ORDER) == 0, "unknown flags");
+  const bool ko = (flags & GR_AGG_K_ORDER) != 0;
+  GR_CHECK_ARG_AS(fn, !ko || out_lo, "GR_AGG_K_ORDER needs both planes (no hi-only output: the dense layer keeps fp32-class A)");
+  // the dense layer runs I <= 2; wider K-order builds would spill (as the segment-layout ones of 3 and 4 instructions do)
+  GR_CHECK_ARG_AS(fn, !ko || I <= 2, "GR_AGG_K_ORDER is built for I <= 2");
   // only the persistent kernels have a hi-only form; agg_abs_kernel (no tile counter, or agg_abs_ws 0) always stores lo
-  GR_CHECK_ARG(out_lo || (tile_counter && g_opt_agg_abs_ws != 0),
+  GR_CHECK_ARG_AS(fn, out_lo || (tile_counter && g_opt_agg_abs_ws != 0),
                "hi-only output (bf16 activation storage) needs a persistent kernel (a tile counter and agg_abs_ws != 0)");
-  GR_CHECK_ARG(F == 0 || (src_t && rel_t && src_h && rel_h), "null edge arrays");
-  GR_CHECK_ARG(B > 0 && N >= kRows && I > 0, "B, I must be positive and N >= 64");
-  GR_CHECK_ARG(D == 200 && seg_pitch == 208, "this build specialises D = 200, seg_pitch = 208 (use gr_aggregate_dual)");
-  GR_CHECK_ARG(ld_planes % 4 == 0 && out_col0 % 4 == 0 && ld_planes >= out_col0 + 2 * (int64_t)I * seg_pitch,
+  GR_CHECK_ARG_AS(fn, F == 0 || (src_t && rel_t && src_h && rel_h), "null edge arrays");
+  GR_CHECK_ARG_AS(fn, B > 0 && N >= kRows && I > 0, "B, I must be positive and N >= 64");
+  GR_CHECK_ARG_AS(fn, D == 200 && seg_pitch == 208, "this build specialises D = 200, seg_pitch = 208 (use gr_aggregate_dual)");
+  GR_CHECK_ARG_AS(fn, ld_planes % 4 == 0 && out_col0 % 4 == 0 && ld_planes >= out_col0 + 2 * (int64_t)I * seg_pitch,
                "plane row pitch / column offset must be multiples of 4 and cover all segments");
-  GR_CHECK_ARG((reinterpret_cast<uintptr_t>(out_hi) & 7) == 0 && (reinterpret_cast<uintptr_t>(out_lo) & 7) == 0 &&   /* NULL ok */
+  GR_CHECK_ARG_AS(fn, (reinterpret_cast<uintptr_t>(out_hi) & 7) == 0 && (reinterpret_cast<uintptr_t>(out_lo) & 7) == 0 &&   /* NULL ok */
                    (reinterpret_cast<uintptr_t>(pn_fwd) & 15) == 0 && (reinterpret_cast<uintptr_t>(pn_inv) & 15) == 0,
                "misaligned planes / padded tables");
   PnParams p{};
@@ -840,9 +892,36 @@ extern "C" int gr_aggregate_dual_abs(const int32_t* rowptr_t, const int32_t* src
   for (int j0 = 0; j0 < I; j0 += 4) {
     p.j0 = j0;
     const int ni = I - j0 < 4 ? I - j0 : 4;
-    int rc = ni == 1 ? launch_pn<1>(p, stream) : ni == 2 ? launch_pn<2>(p, stream)
-             : ni == 3 ? launch_pn<3>(p, stream) : launch_pn<4>(p, stream);
+    int rc = ko ? (ni == 1 ? launch_pn<1, true>(p, stream) : launch_pn<2, true>(p, stream))
+                : (ni == 1 ? launch_pn<1, false>(p, stream) : ni == 2 ? launch_pn<2, false>(p, stream)
+                   : ni == 3 ? launch_pn<3, false>(p, stream) : launch_pn<4, false>(p, stream));
     if (rc != GR_OK) return rc;
   }
   return GR_OK;
+}
+
+}  // namespace
+}  // namespace gr
+
+extern "C" int gr_aggregate_dual_abs_ex(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                                        const float* w_t, const int32_t* rowptr_h, const int32_t* src_h,
+                                        const int32_t* rel_h, const float* w_h, const float* prior,
+                                        const float* pn_fwd, const float* pn_inv, int64_t table_rows, const float* ins,
+                                        void* out_hi, void* out_lo, int64_t ld_planes, int64_t out_col0,
+                                        int64_t seg_pitch, int B, int N, int D, int I, int64_t F,
+                                        int32_t* tile_counter, uint32_t flags, void* stream_) {
+  return gr::aggregate_dual_abs(__func__, rowptr_t, src_t, rel_t, w_t, rowptr_h, src_h, rel_h, w_h, prior, pn_fwd,
+                                pn_inv, table_rows, ins, out_hi, out_lo, ld_planes, out_col0, seg_pitch, B, N, D, I, F,
+                                tile_counter, flags, stream_);
+}
+
+extern "C" int gr_aggregate_dual_abs(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t,
+                                    const float* w_t, const int32_t* rowptr_h, const int32_t* src_h,
+                                    const int32_t* rel_h, const float* w_h, const float* prior,
+                                    const float* pn_fwd, const float* pn_inv, int64_t table_rows, const float* ins, void* out_hi,
+                                    void* out_lo, int64_t ld_planes, int64_t out_col0, int64_t seg_pitch, int B,
+                                    int N, int D, int I, int64_t F, int32_t* tile_counter, void* stream_) {
+  return gr::aggregate_dual_abs(__func__, rowptr_t, src_t, rel_t, w_t, rowptr_h, src_h, rel_h, w_h, prior, pn_fwd,
+                                pn_inv, table_rows, ins, out_hi, out_lo, ld_planes, out_col0, seg_pitch, B, N, D, I, F,
+                                tile_counter, 0u, stream_);
 }

@@ -153,16 +153,21 @@ constexpr size_t fused_smem_bytes(int np) {
          2 * sizeof(ETile<NI>) + 64 * 8 + 2 * 256 * 4;
 }
 
-// W [N, (2I+1)*D] fp32 -> hi/lo planes [N, G*T*32] in the kernel's K order (see the header comment)
-__global__ void fused_w_split_kernel(const float* __restrict__ W, int64_t ldw, int N, int D, int I, int G,
+// W [N, (2I+1)*D] fp32 -> hi/lo planes [N, nkb*32] in the kernel's K order (see the header comment); nkb < G*T: the
+// packed walk of GroupedK (wgmma.cuh), whose last I k-blocks hold the last group of two neighbour slots each
+__global__ void fused_w_split_kernel(const float* __restrict__ W, int64_t ldw, int N, int D, int I, int G, int nkb,
                                      __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
   const int T = 2 * I + 1;
-  const int64_t Kp = (int64_t)G * T * BK;
+  const int64_t Kp = (int64_t)nkb * BK;
   const int64_t total = (int64_t)N * Kp;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t n = i / Kp;
     const int k = (int)(i - n * Kp);
-    const int blk = k / BK, c = k % BK;
+    int blk = k / BK, c = k % BK;
+    if (nkb != G * T && blk > (G - 1) * T) {                 // packed tail block i: slots 2i | 2i + 1 of the last group
+      blk = (G - 1) * T + 1 + 2 * (blk - (G - 1) * T - 1) + c / 16;
+      c %= 16;
+    }
     const int g = blk / T, t = blk % T;
     // t == 0: the h segment;  t >= 1: Y(dir = (t-1) / I, j = (t-1) % I) -> segment 1 + 2j + dir
     const int seg = t == 0 ? 0 : 1 + 2 * ((t - 1) % I) + (t - 1) / I;
@@ -839,11 +844,12 @@ int launch_fused_np(const CUtensorMap* const (&m)[7], int I, int cs, const Fused
 
 namespace tc {
 
-GroupedK plan_grouped_k(int64_t pitch, int I, int64_t N_out) {
+GroupedK plan_grouped_k(int64_t pitch, int I, int64_t N_out, bool packed) {
   GroupedK k{};
   k.G = (int)((pitch + BK - 1) / BK);
   k.ksteps_last = (int)((pitch - (int64_t)(k.G - 1) * BK) / MMA_K);
-  k.kp = (int64_t)k.G * (2 * I + 1) * BK;
+  k.nkb = packed && k.ksteps_last == 1 ? (k.G - 1) * (2 * I + 1) + 1 + I : k.G * (2 * I + 1);
+  k.kp = (int64_t)k.nkb * BK;
   k.w_plane_bytes = align_up((size_t)N_out * k.kp * 2, 256);
   return k;
 }
@@ -852,7 +858,7 @@ int grouped_w_split(const float* W, int64_t ldw, int64_t N_out, int D, int I, co
                     __nv_bfloat16* lo, cudaStream_t stream) {
   const int64_t work = N_out * k.kp;
   const int grid = (int)std::min<int64_t>(ceil_div(work, 256), 32LL * sm_count());
-  fused_w_split_kernel<<<grid, 256, 0, stream>>>(W, ldw, (int)N_out, D, I, k.G, hi, lo);
+  fused_w_split_kernel<<<grid, 256, 0, stream>>>(W, ldw, (int)N_out, D, I, k.G, k.nkb, hi, lo);
   GR_CHECK_LAUNCH();
   return GR_OK;
 }

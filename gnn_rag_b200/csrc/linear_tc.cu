@@ -13,7 +13,8 @@
 // fp32 accumulator in registers, then the epilogue (bias + relu + score dot,
 // fp32 and bf16 hi/lo plane outputs, staged TMA stores or direct stores).  With tc_cluster = 2, clusters of 2 CTAs
 // share the W tiles by TMA multicast (single-CTA clusters measured faster and are the default).  GR_LINEAR_K_GROUPED
-// walks a segmented K in the fused layer kernel's k-block order (GroupedK, wgmma.cuh) and so returns its bits.
+// walks a segmented K in the fused layer kernel's k-block order (GroupedK, wgmma.cuh) and so returns its bits, from the
+// segment layout or (GR_LINEAR_K_ORDER_PLANES) from the K-order layout gr_aggregate_dual_abs_ex writes.
 //
 // Roofline: tensor-pipe work 3 * 2*M*N*K flop; HBM traffic ~ 2 planes * M*K*2 B = M*K*4 B (same as fp32 A).
 #include "wgmma.cuh"
@@ -105,8 +106,10 @@ struct TcParams {
   uint32_t flags;
   int tma_store;            // 1: epilogue stages 64x16 chunks in smem and writes them with TMA stores
   // GR_LINEAR_K_GROUPED (the GROUPED instantiations; kg_T = 0 otherwise): T segments of kg_pitch columns walked in kg_G
-  // column groups (GroupedK, wgmma.cuh); the k-blocks from kg_half on are one k-step
-  int kg_T, kg_G, kg_pitch, kg_half;
+  // column groups (GroupedK, wgmma.cuh), kg_nkb k-blocks of which kg_one0 .. kg_one1 - 1 are one k-step.  kg_nb0 > 0
+  // (GR_LINEAR_K_ORDER_PLANES): the 2I neighbour segments lie in the K-order layout from column kg_nb0 on, kg_G counts
+  // the full 32-column groups only and a 16-column last group follows as the h tail and I packed neighbour k-blocks
+  int kg_T, kg_G, kg_pitch, kg_nkb, kg_one0, kg_one1, kg_nb0;
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -116,7 +119,8 @@ struct TcParams {
 // ---------------------------------------------------------------------------------------------------
 // NP: accumulator width (W tile rows); CS: CTAs per cluster sharing W tiles by multicast; BK: k-block width;
 // GROUPED: k-block kb = g*T + t reads A at column seg(t)*pitch + 32g and W at column 32 kb -- the k-block sequence, and
-// so the per-element accumulation order, of fused_layer_kernel
+// so the per-element accumulation order, of fused_layer_kernel.  With kg_nb0 > 0 the same k16 steps come from the K-order
+// layout: h boxes at column 32g, the neighbour boxes one after another from kg_nb0 (every box 64-byte aligned)
 template <int NP, int CS, int BK, bool GROUPED>
 __global__ void __launch_bounds__(kThreads, 1)
 linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
@@ -144,7 +148,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   }
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nkb = GROUPED ? p.kg_G * p.kg_T : (p.K + BK - 1) / BK;
+  const int nkb = GROUPED ? p.kg_nkb : (p.K + BK - 1) / BK;
   const int crank = CS > 1 ? (int)cluster_ctarank() : 0;
   const int ncluster = gridDim.x / CS, cid = blockIdx.x / CS;
   const int ngroups = (p.num_tiles + CS - 1) / CS;       // tile groups: CS consecutive 128-row tiles
@@ -176,9 +180,16 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
           mbar_expect_tx(&full_bar[s], (uint32_t)stage_bytes);
           int a_col = kb * BK;
           if constexpr (GROUPED) {
-            const int g = kb / p.kg_T, t = kb - g * p.kg_T, ni = p.kg_T >> 1;
-            const int seg = t == 0 ? 0 : 1 + 2 * ((t - 1) % ni) + (t - 1) / ni;
-            a_col = seg * p.kg_pitch + g * BK;
+            if (p.kg_nb0 == 0) {
+              const int g = kb / p.kg_T, t = kb - g * p.kg_T, ni = p.kg_T >> 1;
+              const int seg = t == 0 ? 0 : 1 + 2 * ((t - 1) % ni) + (t - 1) / ni;
+              a_col = seg * p.kg_pitch + g * BK;
+            } else {
+              // K-order layout: group g (g = kg_G: the tail) is its h box, then its neighbour boxes, which continue the
+              // ones of the groups before: kb - g - 1 neighbour boxes precede them
+              const int g = min(kb / p.kg_T, p.kg_G), t = kb - g * p.kg_T;
+              a_col = t == 0 ? g * BK : p.kg_nb0 + (kb - g - 1) * BK;
+            }
           }
           tma_load_2d(st, &map_a_hi, &full_bar[s], a_col, m0);
           if (!single) tma_load_2d(st + a_bytes, &map_a_lo, &full_bar[s], a_col, m0);
@@ -222,8 +233,8 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
         const uint64_t da_hi = make_smem_desc<BK>(sa + a_row), da_lo = make_smem_desc<BK>(sa + a_bytes + a_row);
         const uint64_t dw_hi = make_smem_desc<BK>(sa + w_off), dw_lo = make_smem_desc<BK>(sa + w_off + w_bytes);
         if constexpr (GROUPED) {
-          // the last column group of a 16-column-padded segment holds one k-step: its own straight-line batch
-          if (kb >= p.kg_half) mma_kblock<NP, BK, 1, false>(acc, da_hi, da_lo, dw_hi, dw_lo);
+          // a 16-column h block (segment layout: every block of the last group) is one k-step: its own straight-line batch
+          if (kb >= p.kg_one0 && kb < p.kg_one1) mma_kblock<NP, BK, 1, false>(acc, da_hi, da_lo, dw_hi, dw_lo);
           else mma_kblock<NP, BK, BK / MMA_K, false>(acc, da_hi, da_lo, dw_hi, dw_lo);
         } else if (single) {
           mma_kblock<NP, BK, BK / MMA_K, true>(acc, da_hi, da_lo, dw_hi, dw_lo);
@@ -367,8 +378,10 @@ int launch_tc(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int64_t lda1
   // cluster multicast of W needs 8-row-aligned W slices and at least two tiles
   int cs = (g_tc_cluster >= 2 && (t.np / 2) % 8 == 0 && p.num_tiles >= 2) ? 2 : 1;
   CUtensorMap m_a_hi, m_a_lo, m_w_hi, m_w_lo;
-  const int64_t w_cols = p.kg_T ? ldw16 : p.K;           // grouped order: dense planes of kg_G * kg_T * 32 columns
-  if (!make_tmap(&m_a_hi, a_hi, p.M, p.K, lda16, BM, t.bk) || !make_tmap(&m_a_lo, a_lo, p.M, p.K, lda16, BM, t.bk) ||
+  const int64_t w_cols = p.kg_T ? ldw16 : p.K;           // grouped order: dense planes of kg_nkb * 32 columns
+  // K-order layout: the A map reaches the end of the neighbour region (past K), or the last tail box would be zero filled
+  const int64_t a_cols = p.kg_nb0 ? p.kg_nb0 + (int64_t)(p.kg_T - 1) * p.kg_pitch : p.K;
+  if (!make_tmap(&m_a_hi, a_hi, p.M, a_cols, lda16, BM, t.bk) || !make_tmap(&m_a_lo, a_lo, p.M, a_cols, lda16, BM, t.bk) ||
       !make_tmap(&m_w_hi, w_hi, p.N, w_cols, ldw16, t.np / cs, t.bk) ||
       !make_tmap(&m_w_lo, w_lo, p.N, w_cols, ldw16, t.np / cs, t.bk)) {
     set_error("gr_linear_tc: cuTensorMapEncodeTiled failed (pointers must be 16-byte aligned, row strides "
@@ -467,6 +480,8 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
   GR_CHECK_ARG(C || C_hi, "no output requested");
   GR_CHECK_ARG(M > 0 && N > 0 && K > 0, "M, N, K must be positive");
   const bool grouped = (flags & GR_LINEAR_K_GROUPED) != 0;
+  const bool korder = (flags & GR_LINEAR_K_ORDER_PLANES) != 0;
+  GR_CHECK_ARG(!korder || grouped, "GR_LINEAR_K_ORDER_PLANES modifies GR_LINEAR_K_GROUPED and needs it");
   if (grouped) {
     GR_CHECK_ARG(k_seg > 0 && k_seg_pitch >= k_seg && k_seg_pitch % 16 == 0,
                  "GR_LINEAR_K_GROUPED needs segmented K: k_seg > 0 and k_seg_pitch >= k_seg, a multiple of 16");
@@ -489,9 +504,14 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
               (long long)K);
     return GR_ERR_UNSUPPORTED;
   }
-  // grouped order: the W planes gr_fused_layer keeps (same layout, same size: one workspace serves both)
+  // grouped order: the W planes gr_fused_layer keeps (same layout, same size: one workspace serves both); over K-order
+  // planes the packed form of them, no larger
   const int num_ins = grouped ? (int)(K / k_seg_pitch / 2) : 0;
-  const GroupedK gk = grouped ? plan_grouped_k(k_seg_pitch, num_ins, N) : GroupedK{};
+  const GroupedK gk = grouped ? plan_grouped_k(k_seg_pitch, num_ins, N, korder) : GroupedK{};
+  const int64_t nb0 = (k_seg_pitch + 31) / 32 * 32;      // K-order layout: first column of the neighbour region
+  GR_CHECK_ARG(!korder || lda16 >= nb0 + 2 * num_ins * k_seg_pitch,
+               "GR_LINEAR_K_ORDER_PLANES: lda16 must cover the neighbour region (round32(k_seg_pitch) + (K - k_seg_pitch) "
+               "columns)");
   const size_t w_plane_bytes = grouped ? gk.w_plane_bytes : t.w_plane_bytes;
   if (workspace_bytes < 2 * w_plane_bytes || (reinterpret_cast<uintptr_t>(workspace) & 255) != 0) {
     set_error("gr_linear_tc_planes: workspace too small or not 256-byte aligned");
@@ -520,8 +540,15 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
   p.ldc16 = ldc16; p.w_score = w_score; p.dots = dots;
   p.M = (int)M; p.N = (int)N; p.K = (int)K; p.flags = flags;
   if (grouped) {
-    p.kg_T = 2 * num_ins + 1; p.kg_G = gk.G; p.kg_pitch = (int)k_seg_pitch;
-    p.kg_half = gk.ksteps_last == 1 ? (gk.G - 1) * p.kg_T : gk.G * p.kg_T;
+    p.kg_T = 2 * num_ins + 1; p.kg_pitch = (int)k_seg_pitch; p.kg_nkb = gk.nkb;
+    const bool tail = gk.ksteps_last == 1;
+    if (!korder) {
+      p.kg_G = gk.G;
+      p.kg_one0 = tail ? (gk.G - 1) * p.kg_T : gk.nkb; p.kg_one1 = gk.nkb;
+    } else {
+      p.kg_G = tail ? gk.G - 1 : gk.G; p.kg_nb0 = (int)nb0;
+      p.kg_one0 = tail ? p.kg_G * p.kg_T : gk.nkb; p.kg_one1 = tail ? p.kg_one0 + 1 : gk.nkb;
+    }
   }
   return launch_tc(reinterpret_cast<const __nv_bfloat16*>(A_hi),
                    reinterpret_cast<const __nv_bfloat16*>(A_lo ? A_lo : A_hi), lda16, w_hi, w_lo,

@@ -28,12 +28,17 @@ constexpr int MMA_K = 16;
 // of a segment holds 16 columns (ksteps_last == 1) its k-blocks are ONE k-step.  gr_fused_layer and
 // gr_linear_tc_planes (GR_LINEAR_K_GROUPED) share this plan, these planes and therefore the fp32 accumulation order
 // of every output element.  Defined in fused_layer.cu.
+//
+// Packed (GR_LINEAR_K_ORDER_PLANES, the A operand in the K-order layout of gr_aggregate_dual_abs_ex): the same k16 steps
+// in the same order, with a 16-column last group packed as the h tail (one k-step, W block = 16 columns + 16 zeros)
+// followed by I k-blocks of two k-steps, block i = the last group of neighbour slots 2i and 2i+1 (16 columns each).
+// (G-1)*T + 1 + I k-blocks instead of G*T; without a 16-column last group the packed planes are the grouped ones.
 struct GroupedK {
-  int G, ksteps_last;
-  int64_t kp;                    // columns of the W planes: G * T * 32
+  int G, ksteps_last, nkb;       // nkb: k-blocks of the walk
+  int64_t kp;                    // columns of the W planes: nkb * 32
   size_t w_plane_bytes;
 };
-GroupedK plan_grouped_k(int64_t pitch, int I, int64_t N_out);
+GroupedK plan_grouped_k(int64_t pitch, int I, int64_t N_out, bool packed = false);
 int grouped_w_split(const float* W, int64_t ldw, int64_t N_out, int D, int I, const GroupedK& k, __nv_bfloat16* hi,
                     __nv_bfloat16* lo, cudaStream_t stream);
 

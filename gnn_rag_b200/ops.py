@@ -18,6 +18,8 @@ LINEAR_EXACT_FP32 = 2
 LINEAR_W_PRESPLIT = 4
 LINEAR_BF16_SINGLE = 8
 LINEAR_K_GROUPED = 16
+LINEAR_K_ORDER_PLANES = 32
+AGG_K_ORDER = 1
 
 # bf16 ACTIVATION STORAGE (BASELINE configs[2], "bf16"): the layer-input matrix keeps its hi plane only -- the aggregation
 # kernel skips the lo plane (half the output bytes) and the e2e GEMM runs ONE bf16 product instead of three.  Tables,
@@ -387,8 +389,15 @@ def aggregate_dual_abs_supported(N, D, seg_pitch, R1):
 _TILE_COUNTER = {}
 
 
-def aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, out_col0, seg_pitch, w_t=None, w_h=None):
-    """Both directions of one ReaRev layer into the split-bf16 planes, |v|-accumulating kernel (reasongnn.py:150-161)."""
+def k_order_nb0(seg_pitch):
+    """First column of the neighbour region of the K-order layout (:func:`aggregate_dual_abs` with ``k_order``)."""
+    return (seg_pitch + 31) // 32 * 32
+
+
+def aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, out_col0, seg_pitch, w_t=None, w_h=None, k_order=False):
+    """Both directions of one ReaRev layer into the split-bf16 planes, |v|-accumulating kernel (reasongnn.py:150-161).
+    ``k_order``: the 2I neighbour segments go to the K-order layout from ``out_col0`` on (GR_AGG_K_ORDER), the A operand
+    :func:`linear_tc_planes` reads with ``k_order``."""
     prior = _cuda(prior, torch.float32, "prior").contiguous()
     ins = _cuda(ins, torch.float32, "ins").contiguous()
     B, I, D = ins.shape
@@ -399,10 +408,11 @@ def aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, out_col0, seg_pitc
     dev = prior.device
     if dev not in _TILE_COUNTER:
         _TILE_COUNTER[dev] = torch.zeros(1, dtype=torch.int32, device=dev)
-    _launch("gr_aggregate_dual_abs", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
+    _launch("gr_aggregate_dual_abs_ex", _p(g.rowptr_t), _p(g.src_t), _p(g.rel_t), _p(w_t),
             _p(g.rowptr_h), _p(g.src_h), _p(g.rel_h), _p(w_h),
             _p(prior), _p(pn_fwd), _p(pn_inv), pn_fwd.shape[0], _p(ins), _p(hi), _p(lo), hi.stride(0),
-            out_col0, seg_pitch, B, g.N, D, I, g.F, _p(_TILE_COUNTER[dev]), launches=(I + 3) // 4, agg=("dual", I))
+            out_col0, seg_pitch, B, g.N, D, I, g.F, _p(_TILE_COUNTER[dev]), AGG_K_ORDER if k_order else 0,
+            launches=(I + 3) // 4, agg=("dual", I))
 
 
 FUSED_LAYER = True      # dense-prior ReaRev layers run in grouped K order (the k-block order of csrc/fused_layer.cu)
@@ -462,15 +472,17 @@ def fused_layer(g, prior, pn_fwd, pn_inv, ins, h_planes, seg_pitch, W, bias, out
 def dense_layer(g, prior, pn_fwd, pn_inv, ins, planes, seg_pitch, W, bias, out=None, out_planes=None, w_score=None,
                 dots=None, w_t=None, w_h=None):
     """One dense-prior ReaRev layer in grouped K order: ``relu(e2e([h | nb...]))`` with the score dot.  ``planes`` =
-    (hi, lo) layer-input planes [M, >= (2I+1) * seg_pitch] whose first segment holds h.  Accumulators of more than 128
-    columns run as :func:`aggregate_dual_abs` into the neighbour segments of ``planes`` + :func:`linear_tc_planes` in
-    grouped order, the others as :func:`fused_layer`; the outputs are the same bits either way."""
+    (hi, lo) layer-input planes [M, >= k_order_nb0(seg_pitch) + 2I * seg_pitch] whose first segment holds h.
+    Accumulators of more than 128 columns run as :func:`aggregate_dual_abs` into the K-order neighbour region of
+    ``planes`` + :func:`linear_tc_planes` walking it in grouped order, the others as :func:`fused_layer`; the outputs
+    are the same bits either way."""
     I, n_out = ins.shape[1], W.shape[0]
     if DENSE_WIDE_AS_PAIR and (n_out + 15) // 16 * 16 > 128:
-        aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, seg_pitch, seg_pitch, w_t, w_h)
+        aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, k_order_nb0(seg_pitch), seg_pitch, w_t, w_h,
+                           k_order=True)
         return linear_tc_planes(planes[0], planes[1], (2 * I + 1) * seg_pitch, W, bias, out=out, out_planes=out_planes,
                                 w_score=w_score, dots=dots, relu=True, k_seg=ins.shape[2], k_seg_pitch=seg_pitch,
-                                k_grouped=True)
+                                k_grouped=True, k_order=True)
     return fused_layer(g, prior, pn_fwd, pn_inv, ins, planes, seg_pitch, W, bias, out=out, out_planes=out_planes,
                        w_score=w_score, dots=dots, relu=True, w_t=w_t, w_h=w_h)
 
@@ -563,7 +575,7 @@ def live_weight_workspaces():
 
 
 def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=None, dots=None, relu=True,
-                     k_seg=0, k_seg_pitch=0, single_ok=False, k_grouped=False):
+                     k_seg=0, k_seg_pitch=0, single_ok=False, k_grouped=False, k_order=False):
     """wgmma split-bf16 GEMM whose A operand already lives in bf16 hi/lo planes [M, >=K] (shapes:
     :func:`tc_planes_ok`).
     ``single_ok``: this call may run as ONE bf16 product when ``ACT_BF16`` is on (the node-update GEMMs; the small
@@ -572,6 +584,8 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
     ``dots`` [2*M] = the two column-half partial sums of out @ w_score.
     ``k_grouped``: walk the K segments column group by column group (GR_LINEAR_K_GROUPED): the accumulation order, the
     W planes and the cached workspace of :func:`fused_layer`; always the three-product path.
+    ``k_order`` (with ``k_grouped``): the neighbour segments lie in the K-order layout of :func:`aggregate_dual_abs`
+    (GR_LINEAR_K_ORDER_PLANES): the same k16 steps from aligned boxes, W packed to match under a cache key of its own.
     N > 256 (cfg5: entity_dim 400) is tiled over the output columns: one launch per slice of W rows."""
     N = W.shape[0]
     if N > TC_MAX_N:
@@ -585,7 +599,7 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
                              out=None if out is None else out[:, n0:n1],
                              out_planes=None if out_planes is None else (out_planes[0][:, n0:n1], out_planes[1][:, n0:n1]),
                              w_score=None if w_score is None else w_score[n0:n1], dots=d, relu=relu, k_seg=k_seg,
-                             k_seg_pitch=k_seg_pitch, single_ok=single_ok, k_grouped=k_grouped)
+                             k_seg_pitch=k_seg_pitch, single_ok=single_ok, k_grouped=k_grouped, k_order=k_order)
             if dots is not None and n0 > 0:
                 part = d if part is None else part + d
         if part is not None:
@@ -598,15 +612,17 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
     else:
         assert W.shape[1] == K
     assert W.stride(1) == 1
-    if k_grouped:                   # fused_layer's W planes, under fused_layer's cache key
+    assert k_grouped or not k_order
+    if k_grouped:                   # fused_layer's W planes, under fused_layer's cache key (packed: a key of its own)
         nbytes = _L().gr_fused_layer_workspace_bytes(k_seg, k_seg_pitch, K // k_seg_pitch // 2, N)
-        ws, presplit = _weight_ws(W, N, W.shape[1], "fused", k_seg_pitch, nbytes)
+        ws, presplit = _weight_ws(W, N, W.shape[1], "korder" if k_order else "fused", k_seg_pitch, nbytes)
     else:
         nbytes = _L().gr_linear_tc_planes_workspace_bytes(N, K)
         ws, presplit = _weight_ws(W, N, K, k_seg, k_seg_pitch, nbytes)
     chi, clo = out_planes if out_planes is not None else (None, None)
     flags = (LINEAR_RELU if relu else 0) | (LINEAR_W_PRESPLIT if presplit else 0) | \
-        (LINEAR_K_GROUPED if k_grouped else LINEAR_BF16_SINGLE if (ACT_BF16 and single_ok) else 0)
+        (LINEAR_K_GROUPED if k_grouped else LINEAR_BF16_SINGLE if (ACT_BF16 and single_ok) else 0) | \
+        (LINEAR_K_ORDER_PLANES if k_order else 0)
     _launch("gr_linear_tc_planes", _p(a_hi), _p(a_lo), a_hi.stride(0), _p(W), W.stride(0), _p(bias),
             _p(out), out.stride(0) if out is not None else 0,
             _p(chi), _p(clo), chi.stride(0) if chi is not None else 0,

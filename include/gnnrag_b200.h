@@ -59,6 +59,15 @@ typedef enum gr_status {
                                   * 32; not with GR_LINEAR_BF16_SINGLE.  The workspace is the one of gr_fused_layer
                                   * (gr_fused_layer_workspace_bytes(k_seg, k_seg_pitch, I, N)): same W planes, so
                                   * GR_LINEAR_W_PRESPLIT carries over between the two entry points. */
+#define GR_LINEAR_K_ORDER_PLANES 32u /* with GR_LINEAR_K_GROUPED: the 2I neighbour segments of A are not at
+                                  * k_seg_pitch * (1 + s) but in the K-order layout gr_aggregate_dual_abs_ex writes
+                                  * (GR_AGG_K_ORDER), from column NB0 = round32(k_seg_pitch) on; the h segment stays at
+                                  * column 0.  The k-blocks are aligned 64-byte boxes: per 32-column group the h box
+                                  * and 2I consecutive neighbour boxes, then for a 16-column last group the h tail (one
+                                  * k-step) and I boxes of two neighbour slots each.  The k16 steps, and so the output
+                                  * bits, are those of GR_LINEAR_K_GROUPED.  lda16 must reach NB0 + (K - k_seg_pitch).
+                                  * The W planes are packed to match: another format than gr_fused_layer's (keep a
+                                  * separate workspace; gr_fused_layer_workspace_bytes is large enough). */
 
 int gr_abi_version(void);
 const char* gr_last_error(void);
@@ -208,6 +217,21 @@ int gr_aggregate_dual_abs(const int32_t* rowptr_t, const int32_t* src_t, const i
                          const float* prior, const float* pn_fwd, const float* pn_inv, int64_t table_rows,
                          const float* ins, void* out_hi, void* out_lo, int64_t ld_planes, int64_t out_col0,
                          int64_t seg_pitch, int B, int N, int D, int I, int64_t F, int32_t* tile_counter, void* stream);
+/* gr_aggregate_dual_abs_ex: the same with a flags word before the stream (0 = gr_aggregate_dual_abs).
+ * GR_AGG_K_ORDER writes the 2I neighbour segments in the K-order layout that gr_linear_tc_planes reads with
+ * GR_LINEAR_K_ORDER_PLANES: slot u = d*I + j (direction d, instruction j; the K order of gr_fused_layer), Gf =
+ * seg_pitch / 32 full column groups, and column c of slot u at
+ *     out_col0 + (c >> 5) * 64 I + 32 u + (c & 31)           c < 32 Gf
+ *     out_col0 + Gf * 64 I + 16 u + (c - 32 Gf)              c >= 32 Gf (the 16-column tail)
+ * so the region spans 2 I seg_pitch columns, like the segment layout.  The dense layer calls it with out_col0 =
+ * round32(seg_pitch); columns outside the region are not touched.  Needs both planes (out_lo != NULL) and I <= 2. */
+#define GR_AGG_K_ORDER 1u
+int gr_aggregate_dual_abs_ex(const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rel_t, const float* w_t,
+                             const int32_t* rowptr_h, const int32_t* src_h, const int32_t* rel_h, const float* w_h,
+                             const float* prior, const float* pn_fwd, const float* pn_inv, int64_t table_rows,
+                             const float* ins, void* out_hi, void* out_lo, int64_t ld_planes, int64_t out_col0,
+                             int64_t seg_pitch, int B, int N, int D, int I, int64_t F, int32_t* tile_counter,
+                             uint32_t flags, void* stream);
 /* table_rows: rows (R1) of each padded table.
  * tile_counter: 4 bytes of device scratch (zeroed by the call) -> the persistent, warp-specialised kernel (a staging
  * warp prepares the next tile of rows while the consumer warps aggregate the current one; dynamic tile scheduler);

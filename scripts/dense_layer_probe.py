@@ -1,6 +1,8 @@
-"""Per-layer time of the three ways to run one dense-prior ReaRev layer, alternated in one process:
+"""Per-layer time of the four ways to run one dense-prior ReaRev layer, alternated in one process:
      fused          gr_fused_layer (aggregation inside the GEMM kernel)
-     pair grouped   gr_aggregate_dual_abs + gr_linear_tc_planes in grouped K order (the fused kernel's bits)
+     pair k-order   gr_aggregate_dual_abs_ex (GR_AGG_K_ORDER) + gr_linear_tc_planes in grouped K order over the K-order
+                    layout (GR_LINEAR_K_ORDER_PLANES): the fused kernel's bits, what ops.dense_layer runs
+     pair grouped   gr_aggregate_dual_abs + gr_linear_tc_planes in grouped K order over the segment layout (same bits)
      pair segment   gr_aggregate_dual_abs + gr_linear_tc_planes in segment order (other fp32 rounding)
    at the cfg2 layer shape (B = 64) and at the per-GPU shape of cfg4 (B = 128), with tc_cluster 1 and 2 for the GEMMs,
    and the grouped-order against the segment-order GEMM alone at the d50 width.  CUDA events around every launch, a
@@ -79,12 +81,12 @@ def layer_shape(cfg):
     def fused():
         ops.fused_layer(g, prior, pf, pi, ins, cur, P, W, bias, out_planes=nxt, w_score=wsc, dots=dots, relu=True)
 
-    def agg():
-        ops.aggregate_dual_abs(g, prior, pf, pi, ins, cur, P, P)
+    def agg(k_order=False):
+        ops.aggregate_dual_abs(g, prior, pf, pi, ins, cur, ops.k_order_nb0(P) if k_order else P, P, k_order=k_order)
 
-    def gemm(grouped):
+    def gemm(grouped, k_order=False):
         ops.linear_tc_planes(cur[0], cur[1], T * P, W, bias, out_planes=nxt, w_score=wsc, dots=dots, relu=True,
-                             k_seg=D, k_seg_pitch=P, k_grouped=grouped)
+                             k_seg=D, k_seg_pitch=P, k_grouped=grouped, k_order=k_order)
 
     flop = 3 * 2.0 * M * P * T * P
     edges = 2 * g.F
@@ -96,15 +98,19 @@ def layer_shape(cfg):
     print("%s layer shape: M = %d rows, D = %d, I = %d, %d in-edges (both directions)" % (cfg, M, D, I, edges))
     for cs in (1, 2):
         ops.set_option("tc_cluster", cs)
-        ts = alternate({"fused": fused, "agg": agg, "gemm grouped": lambda: gemm(True),
-                        "gemm segment": lambda: gemm(False)})
+        ts = alternate({"fused": fused, "agg": agg, "agg k-order": lambda: agg(True), "gemm grouped": lambda: gemm(True),
+                        "gemm segment": lambda: gemm(False), "gemm k-order": lambda: gemm(True, True)})
         print(" tc_cluster = %d (the GEMMs; the fused kernel always pairs CTAs)" % cs)
         report("fused (gr_fused_layer)", ts["fused"], flop, hbm_fused)
+        report("pair, K-order layout", [a + b for a, b in zip(ts["agg k-order"], ts["gemm k-order"])], flop, hbm_pair)
         report("pair, grouped K order", [a + b for a, b in zip(ts["agg"], ts["gemm grouped"])], flop, hbm_pair)
         report("pair, segment K order", [a + b for a, b in zip(ts["agg"], ts["gemm segment"])], flop, hbm_pair)
-        report("  gr_aggregate_dual_abs alone", ts["agg"], 0.0, csr + 2 * R1 * 1024 + (T - 1) * plane_bytes)
+        agg_bytes = csr + 2 * R1 * 1024 + (T - 1) * plane_bytes
+        report("  gr_aggregate_dual_abs alone", ts["agg"], 0.0, agg_bytes)
+        report("  gr_aggregate_dual_abs K-order", ts["agg k-order"], 0.0, agg_bytes)
         report("  GEMM grouped alone", ts["gemm grouped"], flop, (T + 1) * plane_bytes)
         report("  GEMM segment alone", ts["gemm segment"], flop, (T + 1) * plane_bytes)
+        report("  GEMM K-order alone", ts["gemm k-order"], flop, (T + 1) * plane_bytes)
     ops.set_option("tc_cluster", 1)
 
 

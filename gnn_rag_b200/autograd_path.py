@@ -63,6 +63,38 @@ class _Facts:
             if weight_rel_list is None:
                 raise ValueError("norm_rel needs kb_adj_mat's weight_rel_list")
             self.wr = torch.as_tensor(np.asarray(weight_rel_list, dtype=np.float32), device=device)
+        self.live = None          # every slot is a fact (cf. _LiveFacts)
+
+
+class _LiveFacts:
+    """Fact arrays of a :class:`LiveBatch`: fixed-capacity buffers whose first ``nfacts`` slots are facts.  ``live``
+    marks those slots; the padding slots read node 0 (ids are clamped into the batch, as gr_csr_build clamps them) and
+    the users of ``live`` zero what they contribute.  Only the per-fact torch work that the kernels do not cover reads
+    these (NSM's reason_kb mask); the aggregations see live facts through the CSR."""
+
+    def __init__(self, heads, tails, weight_list, nfacts, Nt):
+        self.live = torch.arange(heads.numel(), device=heads.device) < nfacts
+        self.heads, self.tails = (torch.where(self.live, a.long().clamp(0, Nt - 1), 0) for a in (heads, tails))
+        self.rels = self.bids = self.wr = None
+        self.w = weight_list
+
+
+class LiveBatch:
+    """A training batch already on the device in fixed-capacity buffers (graphed.GraphedTrainStep): the [B, N] and
+    [B, Q] tensors and the CSR of a :class:`batching.DeviceBatch` built with ``nfacts``, plus the raw fact buffers for
+    :class:`_LiveFacts`.  ``model(batch, training=True)``'s forward takes it in place of the ``get_batch`` tuple."""
+
+    def __init__(self, db, heads, tails, weight_list, nfacts):
+        self.db = db
+        self._raw = (heads, tails, weight_list, nfacts)
+        self._facts = None
+
+    @property
+    def facts(self):
+        if self._facts is None:
+            heads, tails, w, nfacts = self._raw
+            self._facts = _LiveFacts(heads, tails, w, nfacts, self.db.B * self.db.N)
+        return self._facts
 
 
 def _scatter_rows(values, dst, rows):
@@ -180,6 +212,8 @@ def _batch_graph(model, batch, device):
     tensors, or ``USE_KERNELS`` off)."""
     if not (USE_KERNELS and device.type == "cuda"):
         return None
+    if isinstance(batch, LiveBatch):
+        return batch.db.graph
     from . import batching
     return batching.stage_batch(batch, device, model.num_relation + 1, model.normalized_gnn, model.norm_rel).graph
 
@@ -398,9 +432,13 @@ def eval_metric(model, pred_dist, answer_dist, seed_dist, local_entity):
 
 
 def _stage(model, batch):
-    local_entity, query_entities, kb_adj_mat, q_input, seed_dist, _tb, answer_dist = batch[:7]
+    """(local_entity, query_entities, facts, q_input, seed_dist, answer_dist) on the model's device."""
     dev = model.word_embedding.weight.device
     _require_cuda(dev)
+    if isinstance(batch, LiveBatch):
+        db = batch.db
+        return db.local_entity, db.query_entities, batch.facts, db.q_input, db.seed_dist, db.answer_dist
+    local_entity, query_entities, kb_adj_mat, q_input, seed_dist, _tb, answer_dist = batch[:7]
 
     def t(x, dtype):
         x = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
@@ -410,9 +448,22 @@ def _stage(model, batch):
             t(seed_dist, torch.float32), t(answer_dist, torch.float32))
 
 
+def _tp_list(model, pred_dist, staged):
+    local_entity, _qe, _facts, _qi, seed_dist, answer_dist = staged
+    h1, f1 = eval_metric(model, pred_dist.detach(), answer_dist, seed_dist, local_entity)
+    return [h1.tolist(), f1.tolist()]
+
+
 def rearev_forward(model, batch):
     """ReaRev forward with autograd (rearev.py:163-243) -> (loss, pred, pred_dist, [h1, f1])."""
-    local_entity, query_entities, facts, q_input, seed_dist, answer_dist = _stage(model, batch)
+    staged = _stage(model, batch)
+    loss, pred, pred_dist = rearev_core(model, batch, staged)
+    return loss, pred, pred_dist, _tp_list(model, pred_dist, staged)
+
+
+def rearev_core(model, batch, staged):
+    """The differentiable part of :func:`rearev_forward` over the inputs of :func:`_stage` -> (loss, pred, pred_dist)."""
+    local_entity, query_entities, facts, q_input, seed_dist, answer_dist = staged
     B, N = local_entity.shape
     Nt, D, I = B * N, model.entity_dim, model.num_ins
     layer = model.reasoning
@@ -465,14 +516,20 @@ def rearev_forward(model, batch):
     pred_dist = dist_history[-1]
     loss = _loss(model, pred_dist, answer_dist)
     pred = torch.max(pred_dist, dim=1)[1]
-    h1, f1 = eval_metric(model, pred_dist.detach(), answer_dist, seed_dist, local_entity)
     model.dist_history = dist_history
-    return loss, pred, pred_dist, [h1.tolist(), f1.tolist()]
+    return loss, pred, pred_dist
 
 
 def nsm_forward(model, batch):
     """NSM forward with autograd (nsm.py:179-254, forward reasoning only)."""
-    local_entity, _qe, facts, q_input, seed_dist, answer_dist = _stage(model, batch)
+    staged = _stage(model, batch)
+    loss, pred, pred_dist = nsm_core(model, batch, staged)
+    return loss, pred, pred_dist, _tp_list(model, pred_dist, staged)
+
+
+def nsm_core(model, batch, staged):
+    """The differentiable part of :func:`nsm_forward` over the inputs of :func:`_stage` -> (loss, pred, pred_dist)."""
+    local_entity, _qe, facts, q_input, seed_dist, answer_dist = staged
     B, N = local_entity.shape
     Nt, D = B * N, model.entity_dim
     layer = model.reasoning
@@ -498,6 +555,8 @@ def nsm_forward(model, batch):
             prior = pf[facts.heads]
             if facts.w is not None:
                 prior = prior * facts.w * facts.w
+            if facts.live is not None:                                     # padding slots of a LiveBatch
+                prior = torch.where(facts.live, prior, 0.0)
             possible = torch.zeros(Nt, device=h.device).index_add_(0, facts.tails, prior)
             m = mask * (possible > 1e-10).float().view(B, N)
         score = layer.score_func(drop(h)).view(B, N) + (1 - m) * VERY_NEG_NUMBER
@@ -506,9 +565,8 @@ def nsm_forward(model, batch):
     pred_dist = dist_history[-1]
     loss = _loss(model, pred_dist, answer_dist)
     pred = torch.max(pred_dist, dim=1)[1]
-    h1, f1 = eval_metric(model, pred_dist.detach(), answer_dist, seed_dist, local_entity)
     model.dist_history = dist_history
-    return loss, pred, pred_dist, [h1.tolist(), f1.tolist()]
+    return loss, pred, pred_dist
 
 
 def _graft_facts(graft, kb_fact_rel, B, N, dev):

@@ -8,6 +8,7 @@
 // (key = (~bits(p)) << 32 | local_index: ascending key == descending p, ascending index on ties), and the
 // same sequential float64 running sum.  Integer/bit work end to end: bit-exact w.r.t. the reference
 // given the same probabilities.
+#include <limits.h>
 #include <math.h>
 
 #include "common.cuh"
@@ -153,8 +154,128 @@ rank_kernel(const float* __restrict__ dist, const int64_t* __restrict__ local_en
     cand_idx[(int64_t)b * N + i] = i < total ? (int32_t)(keys[i] & 0xFFFFFFFFull) : 0;
 }
 
+// ---- train-time metrics (get_eval_metric, base_model.py:236-298) ------------------------------------------------------
+// One CTA per question.  hit@1: answer_dist > 1e-10 at the top-1 of pred_dist (torch.argmax: NaN counts as the maximum,
+// ties go to the first index).  F1 (questions with hit@1 only): the candidates are the first cand_count[b] entries of
+// cand_idx (gr_rank_candidates); the answers are the non-seed, non-pad nodes with answer mass, kept as a LIST of entity
+// ids (duplicates count in the recall denominator); a candidate is correct when its entity id is among them (np.isin).
+// The F1 is evaluated in float64 with the host's operations and rounded once to fp32, so it is bit-equal.
+constexpr int kMetricThreads = 256;
+constexpr int kSmemAnswers = 2048;    // answer ids kept in shared memory; more are matched from global memory
+
+__device__ __forceinline__ bool argmax_before(float v, int i, float bv, int bi) {
+  const bool vn = v != v, bn = bv != bv;
+  if (vn != bn) return vn;
+  if (!vn && v != bv) return v > bv;
+  return i < bi;
+}
+
+__device__ __forceinline__ bool is_answer(const float* ad, const float* sd, const int64_t* le, int64_t pad_id, int n) {
+  return ad[n] > 0.f && !(sd[n] > 0.f) && le[n] != pad_id;
+}
+
+__global__ void __launch_bounds__(kMetricThreads)
+train_metrics_kernel(const float* __restrict__ pred_dist, const float* __restrict__ answer_dist,
+                     const float* __restrict__ seed_dist, const int64_t* __restrict__ local_entity, int64_t pad_id,
+                     const int32_t* __restrict__ cand_idx, const int32_t* __restrict__ cand_count,
+                     float* __restrict__ h1, float* __restrict__ f1, int N) {
+  constexpr int nw = kMetricThreads / 32;
+  __shared__ float s_v[nw];
+  __shared__ int s_i[nw];
+  __shared__ int64_t s_ans[kSmemAnswers];
+  __shared__ int s_hit, s_n_ans, s_correct;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const float* p = pred_dist + (int64_t)b * N;
+  const float* ad = answer_dist + (int64_t)b * N;
+  const float* sd = seed_dist + (int64_t)b * N;
+  const int64_t* le = local_entity + (int64_t)b * N;
+  // 1. top-1 and hit@1
+  float bv = -INFINITY;
+  int bi = INT_MAX;
+  for (int n = tid; n < N; n += kMetricThreads) {
+    const float v = p[n];
+    if (argmax_before(v, n, bv, bi)) { bv = v; bi = n; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_down_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_down_sync(0xffffffffu, bi, o);
+    if (argmax_before(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+  }
+  if (lane == 0) { s_v[wid] = bv; s_i[wid] = bi; }
+  __syncthreads();
+  if (tid == 0) {
+    for (int w = 1; w < nw; ++w)
+      if (argmax_before(s_v[w], s_i[w], bv, bi)) { bv = s_v[w]; bi = s_i[w]; }
+    s_hit = ad[bi] > 1e-10f;           // (answer_dist > 1e-10) of an fp32 tensor compares in fp32
+    s_n_ans = 0;
+    s_correct = 0;
+    h1[b] = s_hit ? 1.f : 0.f;
+  }
+  __syncthreads();
+  if (!s_hit) {
+    if (tid == 0) f1[b] = 0.f;
+    return;
+  }
+  // 2. the answer list
+  for (int n = tid; n < N; n += kMetricThreads) {
+    if (is_answer(ad, sd, le, pad_id, n)) {
+      const int pos = atomicAdd(&s_n_ans, 1);
+      if (pos < kSmemAnswers) s_ans[pos] = le[n];
+    }
+  }
+  __syncthreads();
+  const int n_ans = s_n_ans;
+  const int c = min(max(cand_count[b], 0), N);
+  // 3. candidates whose entity id is an answer id
+  int correct = 0;
+  for (int i = tid; i < c; i += kMetricThreads) {
+    const int ix = cand_idx[(int64_t)b * N + i];
+    if ((unsigned)ix >= (unsigned)N) continue;
+    const int64_t e = le[ix];
+    bool found = false;
+    if (n_ans <= kSmemAnswers) {
+      for (int k = 0; k < n_ans && !found; ++k) found = s_ans[k] == e;
+    } else {
+      for (int n = 0; n < N && !found; ++n) found = le[n] == e && is_answer(ad, sd, le, pad_id, n);
+    }
+    correct += found;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) correct += __shfl_down_sync(0xffffffffu, correct, o);
+  if (lane == 0 && correct) atomicAdd(&s_correct, correct);
+  __syncthreads();
+  if (tid == 0) {
+    const int k = s_correct;
+    double v;
+    if (n_ans == 0) {
+      v = c == 0 ? 1.0 : 0.0;
+    } else if (c == 0 || k == 0) {
+      v = 0.0;
+    } else {                           // 2 / (1/p + 1/r) with p = k / c, r = k / n_ans, each op rounded as on the host
+      const double pr = __ddiv_rn((double)k, (double)c), rc = __ddiv_rn((double)k, (double)n_ans);
+      v = __ddiv_rn(2.0, __dadd_rn(__ddiv_rn(1.0, pr), __ddiv_rn(1.0, rc)));
+    }
+    f1[b] = __double2float_rn(v);
+  }
+}
+
 }  // namespace
 }  // namespace gr
+
+extern "C" int gr_train_metrics(const float* pred_dist, const float* answer_dist, const float* seed_dist,
+                                const int64_t* local_entity, int64_t pad_id, const int32_t* cand_idx,
+                                const int32_t* cand_count, float* h1, float* f1, int B, int N, void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(pred_dist && answer_dist && seed_dist && local_entity && cand_idx && cand_count && h1 && f1,
+               "null pointer");
+  GR_CHECK_ARG(B > 0 && N > 0, "B and N must be positive");
+  train_metrics_kernel<<<B, kMetricThreads, 0, stream>>>(pred_dist, answer_dist, seed_dist, local_entity, pad_id,
+                                                         cand_idx, cand_count, h1, f1, N);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
 
 extern "C" size_t gr_rank_workspace_bytes(int B, int N) {
   if (B <= 0 || N <= 0) return 0;

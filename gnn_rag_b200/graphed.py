@@ -22,13 +22,17 @@ Models.  The input side is a per-model layout chosen from the model class: :clas
 ``GraftSingleDataLoader.get_batch`` (GraftNet: two more fact lists at their own bucketed capacity with live counts for
 ``gr_graft_stage``, and ``kb_fact_rel``).  The LRU, the pipeline and the streams are shared.  The status words of the
 step (one per CSR build / staging) travel back with the results and are checked on the host after the step.
+
+Training: :class:`GraphedTrainStep` captures ``model(batch, training=True)`` + ``loss.backward()`` + the train-time
+metrics (gr_train_metrics) of ReaRev and NSM over the same input side; see its docstring and DESIGN §4.11.
 """
 import collections
+import contextlib
 
 import numpy as np
 import torch
 
-from . import batching, ops
+from . import autograd_path, batching, ops
 from .modules import live_plane_buffers
 
 
@@ -481,3 +485,194 @@ class GraphedStep:
         idx_h, probs_h, ents_h = idx.cpu().numpy(), probs.cpu().numpy(), ents.cpu().numpy()
         res = [Retrieved(idx_h[b, :c], ents_h[b, :c], probs_h[b, :c]) for b, c in enumerate(counts_h.tolist())]
         return res, counts_h.size * 4 + idx_h.size * 8 + probs_h.size * 4 + ents_h.size * 8
+
+
+# ---- training ------------------------------------------------------------------------------------------------------
+
+class TrainStepOutput(tuple):
+    """``(loss, pred, pred_dist, h1, f1)`` of one :meth:`GraphedTrainStep.step`, all device tensors (views of the
+    graph's static outputs, valid until the next step).  ``status`` is the device int32[1] status word of the batch's
+    CSR build; :meth:`check` reads it back and raises when the fact list held ids outside the batch."""
+
+    def __new__(cls, loss, pred, pred_dist, h1, f1, status):
+        out = super().__new__(cls, (loss, pred, pred_dist, h1, f1))
+        out.status = status
+        return out
+
+    def check(self):
+        _KbLayout.raise_for(self.status.tolist())
+
+
+def _release_autograd_history(model):
+    """Drop the tensors with autograd history that a training forward leaves on the model's modules (``dist_history``,
+    the question encoder's states).  While a previous step's graph is alive, the next forward reuses its AccumulateGrad
+    nodes, which stay bound to the stream they were made on; one bound to the default stream cannot join a capture."""
+    def has_history(v):
+        if isinstance(v, (list, tuple)):
+            return any(has_history(t) for t in v)
+        return isinstance(v, torch.Tensor) and v.grad_fn is not None
+    for mod in model.modules():
+        for k, v in list(vars(mod).items()):
+            if has_history(v):
+                setattr(mod, k, None)
+
+
+def _autocast_dtype():
+    return torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else None
+
+
+class GraphedTrainStep:
+    """``model(batch, training=True)`` + ``loss.backward()`` + the train-time hit@1 / F1 as one CUDA graph per batch
+    shape, for ReaRev and NSM.
+
+    :meth:`step` copies the ``get_batch`` 7-tuple into static buffers (the input side of :class:`GraphedStep`: facts
+    at the front of a ``fact_capacity`` bucket, the live count in ``nfacts``), replays the graph and re-attaches the
+    graph's gradient tensors to ``p.grad`` of every trainable parameter.  After a step ``p.grad`` holds this batch's
+    gradient, overwritten rather than accumulated (as ``zero_grad(); loss.backward()``), so
+    ``optimizer.zero_grad(set_to_none=True)`` between steps is fine.  Clipping and ``optimizer.step()`` stay with
+    the caller; they update the parameters in place, and the graph reads every weight from the parameter's storage
+    when it replays.
+
+    A graph is keyed on the batch shape (B, N, fact capacity, Q, index dtype) and on the state the forward reads when
+    it is captured: ``model.training``, every dropout probability in effect, the autocast dtype, torch's
+    deterministic-algorithms flag, the cuDNN / TF32 switches, which parameters are trainable and the ``data_ptr`` of
+    every parameter (``p.data = ...`` recaptures; in-place updates do not).  Captured graphs are kept in an LRU of
+    ``max_graphs`` entries.  Padding slots past ``nfacts`` contribute nothing: the kernels read live facts through
+    the CSR and the torch-side per-fact work masks them (autograd_path.LiveBatch).  Dropout masks come from torch's
+    CUDA generator, which a graph advances on every replay, so each replay draws fresh masks.  After the first
+    capture of a key a step does no host synchronisation.
+
+    Every kernel path of the eager forward must be available (the aggregation, instruction, query-reform and, with
+    ``encode_type``, TypeLayer kernels); otherwise, and for GraftNet or a CPU model, the constructor or the step raises
+    ``ValueError``."""
+
+    def __init__(self, model, max_graphs=8):
+        from .models import GraftNet, ReaRev
+        if isinstance(model, GraftNet):
+            raise ValueError("GraphedTrainStep covers ReaRev and NSM; GraftNet's training forward reads its live graft "
+                             "fact count on the host and is not captured")
+        self.model = model
+        self._params = list(model.parameters())
+        if not self._params or self._params[0].device.type != "cuda":
+            raise ValueError("GraphedTrainStep needs a model on a CUDA device (model.cuda()); there is no CPU path")
+        self.device = self._params[0].device
+        self.max_graphs = max_graphs
+        self._rearev = isinstance(model, ReaRev)
+        self._core = autograd_path.rearev_core if self._rearev else autograd_path.nsm_core
+        self._cache = collections.OrderedDict()
+        self._layout = _KbLayout(self)
+
+    @staticmethod
+    def tp_list(h1, f1):
+        """The ``tp_list`` of ``model(batch, training=True)``: [h1.tolist(), f1.tolist()] (one device read)."""
+        return [h1.tolist(), f1.tolist()]
+
+    # -- capture key and refusals ----------------------------------------------------------------------------------
+    def key(self, batch):
+        """The capture key of ``batch`` under the current model and torch state (see the class docstring)."""
+        m = self.model
+        if len(self._params) != sum(1 for _ in m.parameters()):
+            raise ValueError("the model's parameters changed after GraphedTrainStep was built: build a new one")
+        drops = tuple(float(d.p) if d.training else 0.0 for d in m.modules() if isinstance(d, torch.nn.Dropout))
+        backends = (torch.backends.cudnn.enabled, torch.backends.cudnn.allow_tf32,
+                    torch.backends.cuda.matmul.allow_tf32)
+        rel_text = tuple(t.data_ptr() for t in (getattr(m, "rel_features", None), getattr(m, "rel_features_inv", None))
+                         if isinstance(t, torch.Tensor))
+        return self._layout.key(batch) + (
+            m.training, drops, _autocast_dtype(), torch.are_deterministic_algorithms_enabled(), backends,
+            tuple(p.requires_grad for p in self._params), tuple(p.data_ptr() for p in self._params), rel_text)
+
+    def refusal(self, Q):
+        """Why the eager forward would leave the kernels for questions of Q tokens (a message), or None."""
+        m = self.model
+        dev, D = self.device, m.entity_dim
+        I = m.num_ins if self._rearev else 1
+        if not autograd_path.USE_KERNELS:
+            return "autograd_path.USE_KERNELS is off: the training forward would run its torch restatement"
+        if not ops.aggregate_backward_ok(D, I):
+            return ("_kernel_graph is None: entity_dim %d with %d instruction(s) is outside the aggregation backward "
+                    "kernel (%s)" % (D, I, ops.aggregate_backward_ok.__doc__.split(": ", 1)[1].rstrip(".")))
+        if not autograd_path._instruction_kernels(dev, Q, D, m.instruction.num_ins):
+            return ("_instruction_kernels is false: %d question tokens, entity_dim %d and %d instructions are outside "
+                    "gr_instructions" % (Q, D, m.instruction.num_ins))
+        if self._rearev and not autograd_path._reform_kernels(dev, D, I):
+            return "_reform_kernels is false: entity_dim %d with %d instructions is outside gr_query_reform" % (D, I)
+        if m.encode_type and not autograd_path._fact_kernels(dev, D):
+            return "the TypeLayer kernel does not admit entity_dim %d (ops.fact_train_ok)" % D
+        return None
+
+    # -- capture ---------------------------------------------------------------------------------------------------
+    def _run(self, st, ac):
+        """forward + backward + metrics over the static buffers ``st`` -> (loss, pred, pred_dist, h1, f1, status)."""
+        m = self.model
+        tup = (st.local_entity, st.query_entities,
+               (st.heads, st.rels, st.tails, None, None, st.weight_list, st.weight_rel_list),
+               st.q_input, st.seed_dist, None, st.answer_dist)
+        # Autocast casts every weight once per forward and reuses the copy (its cast cache), so the gradients of a
+        # weight's uses are summed in the low-precision dtype, as in the eager step.  The cache is emptied before the
+        # forward (an entry made outside the capture would freeze that weight into the graph) and after it (the
+        # graph's copies must not serve eager code).
+        with torch.autocast("cuda", dtype=ac) if ac is not None else contextlib.nullcontext():
+            torch.clear_autocast_cache()
+            db = batching.stage_batch(tup, self.device, m.num_relation + 1, m.normalized_gnn, m.norm_rel,
+                                      nfacts=st.nfacts)
+            live = autograd_path.LiveBatch(db, st.heads, st.tails, st.weight_list, st.nfacts)
+            loss, pred, pred_dist = self._core(m, live, autograd_path._stage(m, live))
+            torch.clear_autocast_cache()
+        loss.backward()
+        pred_dist = pred_dist.detach()
+        cand_idx, cand_count, _ = ops.rank_candidates(pred_dist, db.local_entity, (db.seed_dist > 0).float(),
+                                                      m.num_entity, m.eps)
+        h1, f1 = ops.train_metrics(pred_dist, db.answer_dist, db.seed_dist, db.local_entity, cand_idx, cand_count,
+                                   m.num_entity)
+        return loss.detach(), pred, pred_dist, h1, f1, db.graph.status
+
+    def _entry(self, batch):
+        key = self.key(batch)
+        ent = self._cache.get(key)
+        if ent is not None:
+            self._cache.move_to_end(key)
+            return ent
+        why = self.refusal(key[3])
+        if why is not None:
+            raise ValueError("GraphedTrainStep: " + why)
+        while len(self._cache) >= self.max_graphs:          # LRU eviction: the graph, its buffers and its gradients
+            _k, old = self._cache.popitem(last=False)
+            torch.cuda.synchronize()
+            del old
+        ac = _autocast_dtype()
+        st = self._layout.static_inputs(key[:5])
+        self._layout.fill(st, batch)
+        params = [p for p in self._params if p.requires_grad]
+        torch.cuda.synchronize()
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):            # warm-up on a side stream (lazy init, allocator, cuDNN plans)
+            for _ in range(2):
+                _release_autograd_history(self.model)
+                for p in params:
+                    p.grad = None
+                self._run(st, ac)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        _release_autograd_history(self.model)
+        for p in params:                         # the captured backward allocates (not accumulates) every gradient
+            p.grad = None
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            outs = self._run(st, ac)
+        ent = _Captured()
+        ent.st, ent.g, ent.outs = st, g, outs
+        ent.params, ent.grads = params, [p.grad for p in params]
+        self._cache[key] = ent
+        return ent
+
+    def step(self, batch):
+        """One training step on ``batch`` (the 7-tuple of ``get_batch``, host numpy or pinned) ->
+        :class:`TrainStepOutput` ``(loss, pred, pred_dist, h1, f1)``; ``p.grad`` holds this batch's gradients."""
+        ent = self._entry(batch)
+        self._layout.fill(ent.st, batch)
+        ent.g.replay()
+        for p, g in zip(ent.params, ent.grads):
+            p.grad = g
+        return TrainStepOutput(*ent.outs)

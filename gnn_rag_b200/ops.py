@@ -925,6 +925,36 @@ def rank_candidates(dist, local_entity, query_entities, pad_id, eps):
     return cand_idx, cand_count, cand_total
 
 
+def train_metrics_ok(B, N):
+    """True when gr_train_metrics admits B questions of N nodes: B > 0 and N > 0."""
+    return B > 0 and N > 0
+
+
+def train_metrics(pred_dist, answer_dist, seed_dist, local_entity, cand_idx, cand_count, pad_id):
+    """-> (h1, f1) fp32 [B] on the device: the train-time hit@1 and F1 of autograd_path.eval_metric
+    (gr_train_metrics), with the candidates of :func:`rank_candidates` run on query_entities = (seed_dist > 0)."""
+    f32 = lambda t, n: _cuda(t, torch.float32, n).contiguous()   # noqa: E731
+    pred_dist, answer_dist, seed_dist = f32(pred_dist, "pred_dist"), f32(answer_dist, "answer_dist"), \
+        f32(seed_dist, "seed_dist")
+    local_entity = _cuda(local_entity, torch.int64, "local_entity").contiguous()
+    cand_idx = _cuda(cand_idx, torch.int32, "cand_idx").contiguous()
+    cand_count = _cuda(cand_count, torch.int32, "cand_count").contiguous()
+    B, N = pred_dist.shape
+    if not train_metrics_ok(B, N):
+        raise RuntimeError("train_metrics: need B > 0 and N > 0, got B=%d N=%d" % (B, N))
+    for name, t in (("answer_dist", answer_dist), ("seed_dist", seed_dist), ("local_entity", local_entity),
+                    ("cand_idx", cand_idx)):
+        if t.shape != (B, N):
+            raise RuntimeError("train_metrics: %s must be [%d, %d], got %s" % (name, B, N, list(t.shape)))
+    if cand_count.shape != (B,):
+        raise RuntimeError("train_metrics: cand_count must be [%d], got %s" % (B, list(cand_count.shape)))
+    h1 = torch.empty(B, dtype=torch.float32, device=pred_dist.device)
+    f1 = torch.empty(B, dtype=torch.float32, device=pred_dist.device)
+    _launch("gr_train_metrics", _p(pred_dist), _p(answer_dist), _p(seed_dist), _p(local_entity), int(pad_id),
+            _p(cand_idx), _p(cand_count), _p(h1), _p(f1), B, N, op="loss_rank")
+    return h1, f1
+
+
 def shortest_path_nodes(g, source_idx, source_cnt, target_idx, target_cnt, return_distances=False):
     """source_idx int32[B,S], target_idx int32[B,T] local indices (+counts) ->
     (on_path uint8[B,N], pair_dist int32[B,S,T]); with ``return_distances`` also the BFS distance arrays the kernel

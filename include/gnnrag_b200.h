@@ -652,6 +652,20 @@ int gr_rank_candidates(const float* dist, const int64_t* local_entity, const flo
                        int32_t* cand_total, int B, int N, void* workspace, size_t workspace_bytes,
                        void* stream);
 
+/* Train-time metrics, get_eval_metric (gnn/models/base_model.py:236-298), per question, no host involvement:
+ *   h1[b] = 1 when answer_dist > 1e-10 (fp32 compare) at the top-1 of pred_dist (torch.argmax: first maximal index,
+ *           NaN counts as maximal), else 0;
+ *   f1[b] = for h1 = 1: F1 of the retrieval = the first cand_count[b] local indices of cand_idx (gr_rank_candidates
+ *           with query_entities = (seed_dist > 0)) against the answers = nodes with answer_dist > 0, seed_dist <= 0 and
+ *           local_entity != pad_id, matched by ENTITY ID (np.isin; a repeated id counts once per answer node in the
+ *           recall denominator and once per candidate in the count of correct ones).  No answers: 1 if no candidates
+ *           else 0; no candidates or none correct: 0.  Evaluated in float64 and rounded once to fp32.  0 for h1 = 0.
+ *   pred_dist, answer_dist, seed_dist: fp32 [B, N]; local_entity: int64 [B, N]; cand_idx: int32 [B, N];
+ *   cand_count: int32 [B]; h1, f1: fp32 [B].  Refused: null pointers, B or N not positive. */
+int gr_train_metrics(const float* pred_dist, const float* answer_dist, const float* seed_dist,
+                     const int64_t* local_entity, int64_t pad_id, const int32_t* cand_idx, const int32_t* cand_count,
+                     float* h1, float* f1, int B, int N, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Shortest-path node sets (SURVEY.md 8f row 1): nodes lying on any shortest path between any seed and
  * any retrieved candidate in the UNDIRECTED subgraph -- build_graph + get_truth_paths,

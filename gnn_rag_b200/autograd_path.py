@@ -54,15 +54,19 @@ class _Facts:
         if bids is None:
             raise ValueError("training needs the batch_ids array of kb_adj_mat (dataset_load.py:521)")
         self.bids = idx(bids)
+        def weights(w):       # host lists / float64 arrays, or the fp32 tensors of a loader.DeviceSplit batch
+            if isinstance(w, torch.Tensor):
+                return w.to(device=device, dtype=torch.float32)
+            return torch.as_tensor(np.asarray(w, dtype=np.float32), device=device)
         self.w = self.wr = None
         if normalized_gnn:
             if weight_list is None:
                 raise ValueError("normalized_gnn needs kb_adj_mat's weight_list")
-            self.w = torch.as_tensor(np.asarray(weight_list, dtype=np.float32), device=device)
+            self.w = weights(weight_list)
         if norm_rel:
             if weight_rel_list is None:
                 raise ValueError("norm_rel needs kb_adj_mat's weight_rel_list")
-            self.wr = torch.as_tensor(np.asarray(weight_rel_list, dtype=np.float32), device=device)
+            self.wr = weights(weight_rel_list)
         self.live = None          # every slot is a fact (cf. _LiveFacts)
 
 

@@ -1,0 +1,320 @@
+// Device-resident split (loader.DeviceSplit): a split's per-question fact segments are uploaded once, and each batch is
+// assembled on the device from B question ids.
+//
+//   gr_split_assemble        the kb_adj_mat fact arrays of SingleDataLoader._build_fact_mat (gnn/dataset_load.py:473-527)
+//                            in stored fact order with the self-loops appended per question (loader.build_fact_mat with
+//                            shuffle=False): row bias b*N, batch ids, fact ids, one pass.
+//   gr_split_assemble_graft  both graft lists of GraftSingleDataLoader._build_fact_mat_maxfacts
+//                            (gnn/dataset_load_graft.py:70-102) in stored order, and the kb_fact_rel rows.
+//   gr_fact_weights          weight_list = 1/outdeg(head) and weight_rel_list = 1/count(head, rel) (:507-516).
+//
+// Assembly: grid (X, B) with X = CTAs per question (a function of B alone).  Every CTA of question b adds up the fact
+// counts of questions 0..b-1 itself (B ids, read from the resident offsets) to find where its question starts, so no
+// host round trip and no second launch is needed; the host sizes the outputs from its own copy of the counts.
+// Out-of-range question ids count as empty questions and set status bit 1; outputs that would run past the capacity
+// the host passed are not written and set status bit 2.
+//
+// Weights: integer counting only.  outdeg(head) by atomicAdd on an int counter per row; count(head, rel) by an open-
+// addressing hash table over the (head, rel) keys of the batch (linear probing, load <= 1/2) with an int counter per
+// key.  The counts are exact whatever order the atomics land in, and each weight is 1.0 / count in float64 rounded
+// once to fp32: bit-equal to fp32 of the host's float64 weights.
+#include <limits.h>
+
+#include <algorithm>
+
+#include "common.cuh"
+
+namespace gr {
+namespace {
+
+constexpr int kSplitThreads = 256;
+constexpr int kWeightThreads = 256;
+constexpr unsigned long long kEmptyKey = ~0ull;
+
+static int ctas_per_question(int B) {
+  // enough CTAs to cover the SMs twice over at small B, one per question at large B
+  return (int)std::max<int64_t>(1, std::min<int64_t>(64, ceil_div(2 * (int64_t)sm_count(), B)));
+}
+
+__device__ __forceinline__ bool valid_id(int64_t id, int64_t num_q) { return id >= 0 && id < num_q; }
+
+// sum over the block of one int64 per thread (result valid in every thread)
+__device__ __forceinline__ int64_t block_sum(int64_t v, int64_t* s_red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if (lane_id() == 0) s_red[warp_id()] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int64_t t = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_red[w];
+    s_red[32] = t;
+  }
+  __syncthreads();
+  return s_red[32];
+}
+
+template <typename IdxT>
+__global__ void __launch_bounds__(kSplitThreads)
+split_assemble_kernel(const int64_t* __restrict__ q_off, const int32_t* __restrict__ q_heads,
+                      const int32_t* __restrict__ q_rels, const int32_t* __restrict__ q_tails,
+                      const int32_t* __restrict__ q_ents, int64_t num_q, const int64_t* __restrict__ ids, int64_t N,
+                      int64_t self_rel, int use_self_loop, int64_t F, IdxT* __restrict__ heads, IdxT* __restrict__ rels,
+                      IdxT* __restrict__ tails, IdxT* __restrict__ bids, IdxT* __restrict__ fids,
+                      int32_t* __restrict__ status) {
+  __shared__ int64_t s_red[33];
+  const int b = blockIdx.y;
+  auto total = [&](int64_t id) -> int64_t {
+    if (!valid_id(id, num_q)) return 0;
+    return q_off[id + 1] - q_off[id] + (use_self_loop ? (int64_t)q_ents[id] : 0);
+  };
+  int64_t before = 0;
+  for (int j = threadIdx.x; j < b; j += blockDim.x) before += total(ids[j]);
+  const int64_t pos = block_sum(before, s_red);
+  const int64_t id = ids[b];
+  const bool ok = valid_id(id, num_q);
+  const int64_t base = ok ? q_off[id] : 0;
+  const int64_t nf = ok ? q_off[id + 1] - base : 0;
+  const int64_t tot = total(id);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    if (!ok) atomicOr(status, 1);
+    if (pos + tot > F) atomicOr(status, 2);
+  }
+  const int64_t bias = (int64_t)b * N;
+  const int64_t end = min(tot, F - pos);
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < end; k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t o = pos + k;
+    int64_t h, r, t;
+    if (k < nf) {
+      h = bias + q_heads[base + k];
+      r = q_rels[base + k];
+      t = bias + q_tails[base + k];
+    } else {                                   // the self-loops of the question's entities (dataset_load.py:498-505)
+      h = t = bias + (k - nf);
+      r = self_rel;
+    }
+    heads[o] = (IdxT)h;
+    rels[o] = (IdxT)r;
+    tails[o] = (IdxT)t;
+    bids[o] = (IdxT)b;
+    fids[o] = (IdxT)o;
+  }
+}
+
+template <typename IdxT>
+__global__ void __launch_bounds__(kSplitThreads)
+split_assemble_graft_kernel(const int64_t* __restrict__ g_off, const int32_t* __restrict__ g_e2f_f,
+                            const int32_t* __restrict__ g_e2f_e, const int32_t* __restrict__ g_f2e_e,
+                            const int32_t* __restrict__ g_f2e_f, const int64_t* __restrict__ r_off,
+                            const int32_t* __restrict__ r_vals, int64_t num_q, const int64_t* __restrict__ ids,
+                            int64_t max_facts, int64_t rel_pad, int64_t G, IdxT* __restrict__ e2f_b,
+                            IdxT* __restrict__ e2f_f, IdxT* __restrict__ e2f_e, float* __restrict__ e2f_v,
+                            IdxT* __restrict__ f2e_b, IdxT* __restrict__ f2e_e, IdxT* __restrict__ f2e_f,
+                            float* __restrict__ f2e_v, int64_t* __restrict__ kb_fact_rel,
+                            int32_t* __restrict__ status) {
+  __shared__ int64_t s_red[33];
+  const int b = blockIdx.y;
+  auto count = [&](int64_t id) -> int64_t { return valid_id(id, num_q) ? g_off[id + 1] - g_off[id] : 0; };
+  int64_t before = 0;
+  for (int j = threadIdx.x; j < b; j += blockDim.x) before += count(ids[j]);
+  const int64_t pos = block_sum(before, s_red);
+  const int64_t id = ids[b];
+  const bool ok = valid_id(id, num_q);
+  const int64_t base = ok ? g_off[id] : 0, n = count(id);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    if (!ok) atomicOr(status, 1);
+    if (pos + n > G) atomicOr(status, 2);
+  }
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x, k0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t end = min(n, G - pos);
+  for (int64_t k = k0; k < end; k += stride) {
+    const int64_t o = pos + k;
+    e2f_b[o] = (IdxT)b;
+    e2f_f[o] = (IdxT)g_e2f_f[base + k];
+    e2f_e[o] = (IdxT)g_e2f_e[base + k];
+    e2f_v[o] = 1.0f;
+    f2e_b[o] = (IdxT)b;
+    f2e_e[o] = (IdxT)g_f2e_e[base + k];
+    f2e_f[o] = (IdxT)g_f2e_f[base + k];
+    f2e_v[o] = 1.0f;
+  }
+  // the kb_fact_rel row: the stored prefix of the question's row, then the pad relation
+  const int64_t rbase = ok ? r_off[id] : 0, rlen = ok ? min(r_off[id + 1] - rbase, max_facts) : 0;
+  int64_t* row = kb_fact_rel + (int64_t)b * max_facts;
+  for (int64_t j = k0; j < max_facts; j += stride) row[j] = j < rlen ? (int64_t)r_vals[rbase + j] : rel_pad;
+}
+
+__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {   // splitmix64 finaliser
+  x ^= x >> 30;
+  x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27;
+  x *= 0x94d049bb133111ebull;
+  x ^= x >> 31;
+  return x;
+}
+
+__device__ __forceinline__ int64_t ld_index(const void* p, int64_t i, int idx_bytes) {
+  return idx_bytes == 8 ? reinterpret_cast<const int64_t*>(p)[i] : (int64_t)reinterpret_cast<const int32_t*>(p)[i];
+}
+
+// pass 1: outdeg(head) and the (head, rel) counts; the hash slot of every fact is kept for pass 2
+__global__ void __launch_bounds__(kWeightThreads)
+fact_count_kernel(const void* __restrict__ heads, const void* __restrict__ rels, int idx_bytes, int64_t F, int64_t Nt,
+                  unsigned long long* __restrict__ keys, uint32_t* __restrict__ counts, uint64_t table_mask,
+                  uint32_t* __restrict__ deg, uint32_t* __restrict__ slot_of, int32_t* __restrict__ status) {
+  for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t h = ld_index(heads, f, idx_bytes), r = ld_index(rels, f, idx_bytes);
+    if (h < 0 || h >= Nt || r < 0 || r > INT_MAX) {
+      atomicOr(status, 1);
+      slot_of[f] = 0xFFFFFFFFu;
+      continue;
+    }
+    atomicAdd(&deg[h], 1u);
+    const unsigned long long key = ((unsigned long long)h << 32) | (unsigned long long)r;
+    uint64_t s = mix64(key) & table_mask;
+    while (true) {
+      const unsigned long long prev = atomicCAS(&keys[s], kEmptyKey, key);
+      if (prev == kEmptyKey || prev == key) break;
+      s = (s + 1) & table_mask;
+    }
+    atomicAdd(&counts[s], 1u);
+    slot_of[f] = (uint32_t)s;
+  }
+}
+
+// pass 2: weight = 1 / count, in float64, rounded once to fp32 (0 for a fact refused in pass 1)
+__global__ void __launch_bounds__(kWeightThreads)
+fact_weight_kernel(const void* __restrict__ heads, int idx_bytes, int64_t F, const uint32_t* __restrict__ counts,
+                   const uint32_t* __restrict__ deg, const uint32_t* __restrict__ slot_of, float* __restrict__ w,
+                   float* __restrict__ wr) {
+  for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
+    const uint32_t s = slot_of[f];
+    if (s == 0xFFFFFFFFu) {
+      if (w) w[f] = 0.f;
+      if (wr) wr[f] = 0.f;
+      continue;
+    }
+    if (w) w[f] = __double2float_rn(__ddiv_rn(1.0, (double)deg[ld_index(heads, f, idx_bytes)]));
+    if (wr) wr[f] = __double2float_rn(__ddiv_rn(1.0, (double)counts[s]));
+  }
+}
+
+// hash table entries for F facts: the power of two >= 2F (at least 1024)
+static uint64_t weight_table_size(int64_t F) {
+  uint64_t t = 1024;
+  while (t < 2 * (uint64_t)F) t <<= 1;
+  return t;
+}
+
+struct WeightWorkspace {
+  size_t keys, counts, deg, slot, total;
+};
+
+static WeightWorkspace weight_workspace(int64_t F, int64_t Nt) {
+  WeightWorkspace w;
+  const uint64_t T = weight_table_size(F);
+  w.keys = 0;
+  w.counts = align_up(T * sizeof(unsigned long long), 256);
+  w.deg = w.counts + align_up(T * sizeof(uint32_t), 256);
+  w.slot = w.deg + align_up((size_t)Nt * sizeof(uint32_t), 256);
+  w.total = w.slot + align_up((size_t)std::max<int64_t>(F, 1) * sizeof(uint32_t), 256);
+  return w;
+}
+
+}  // namespace
+}  // namespace gr
+
+extern "C" int gr_split_assemble(const int64_t* q_off, const int32_t* q_heads, const int32_t* q_rels,
+                                 const int32_t* q_tails, const int32_t* q_ents, int64_t num_q, const int64_t* ids,
+                                 int B, int64_t N, int64_t self_rel, int use_self_loop, int idx_bytes, int64_t F,
+                                 void* heads, void* rels, void* tails, void* batch_ids, void* fact_ids,
+                                 int32_t* status, void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(q_off && ids && status, "null pointer");
+  GR_CHECK_ARG(num_q >= 0 && B > 0 && N > 0 && F >= 0, "need num_q >= 0, B > 0, N > 0 and F >= 0");
+  GR_CHECK_ARG(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+  GR_CHECK_ARG(idx_bytes == 8 || ((int64_t)B * N <= INT_MAX && F <= INT_MAX && self_rel <= INT_MAX),
+               "the batch overflows int32 indices");
+  GR_CHECK_ARG(self_rel >= 0, "self_rel must be non-negative");
+  GR_CHECK_ARG(F == 0 || (heads && rels && tails && batch_ids && fact_ids), "null output arrays");
+  GR_CHECK_ARG(q_heads && q_rels && q_tails && q_ents, "null resident arrays");
+  const dim3 grid(ctas_per_question(B), B);
+  if (idx_bytes == 8)
+    split_assemble_kernel<int64_t><<<grid, kSplitThreads, 0, stream>>>(
+        q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, N, self_rel, use_self_loop, F, (int64_t*)heads,
+        (int64_t*)rels, (int64_t*)tails, (int64_t*)batch_ids, (int64_t*)fact_ids, status);
+  else
+    split_assemble_kernel<int32_t><<<grid, kSplitThreads, 0, stream>>>(
+        q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, N, self_rel, use_self_loop, F, (int32_t*)heads,
+        (int32_t*)rels, (int32_t*)tails, (int32_t*)batch_ids, (int32_t*)fact_ids, status);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+extern "C" int gr_split_assemble_graft(const int64_t* g_off, const int32_t* g_e2f_f, const int32_t* g_e2f_e,
+                                       const int32_t* g_f2e_e, const int32_t* g_f2e_f, const int64_t* r_off,
+                                       const int32_t* r_vals, int64_t num_q, const int64_t* ids, int B,
+                                       int64_t max_facts, int64_t rel_pad, int idx_bytes, int64_t G, void* e2f_b,
+                                       void* e2f_f, void* e2f_e, float* e2f_v, void* f2e_b, void* f2e_e, void* f2e_f,
+                                       float* f2e_v, int64_t* kb_fact_rel, int32_t* status, void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(g_off && r_off && ids && status, "null pointer");
+  GR_CHECK_ARG(g_e2f_f && g_e2f_e && g_f2e_e && g_f2e_f && r_vals, "null resident arrays");
+  GR_CHECK_ARG(num_q >= 0 && B > 0 && max_facts >= 0 && G >= 0, "need num_q >= 0, B > 0, max_facts >= 0 and G >= 0");
+  GR_CHECK_ARG(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+  GR_CHECK_ARG(idx_bytes == 8 || (G <= INT_MAX && max_facts <= INT_MAX), "the batch overflows int32 indices");
+  GR_CHECK_ARG(G == 0 || (e2f_b && e2f_f && e2f_e && e2f_v && f2e_b && f2e_e && f2e_f && f2e_v),
+               "null output arrays");
+  GR_CHECK_ARG(max_facts == 0 || kb_fact_rel, "null kb_fact_rel");
+  const dim3 grid(ctas_per_question(B), B);
+  if (idx_bytes == 8)
+    split_assemble_graft_kernel<int64_t><<<grid, kSplitThreads, 0, stream>>>(
+        g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q, ids, max_facts, rel_pad, G,
+        (int64_t*)e2f_b, (int64_t*)e2f_f, (int64_t*)e2f_e, e2f_v, (int64_t*)f2e_b, (int64_t*)f2e_e, (int64_t*)f2e_f,
+        f2e_v, kb_fact_rel, status);
+  else
+    split_assemble_graft_kernel<int32_t><<<grid, kSplitThreads, 0, stream>>>(
+        g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q, ids, max_facts, rel_pad, G,
+        (int32_t*)e2f_b, (int32_t*)e2f_f, (int32_t*)e2f_e, e2f_v, (int32_t*)f2e_b, (int32_t*)f2e_e, (int32_t*)f2e_f,
+        f2e_v, kb_fact_rel, status);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+extern "C" size_t gr_fact_weights_workspace_bytes(int64_t F, int64_t Nt) {
+  if (F < 0 || Nt <= 0) return 0;
+  return gr::weight_workspace(F, Nt).total;
+}
+
+extern "C" int gr_fact_weights(const void* heads, const void* rels, int idx_bytes, int64_t F, int64_t Nt,
+                               float* weight, float* weight_rel, int32_t* status, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(heads && rels && status, "null pointer");
+  GR_CHECK_ARG(weight || weight_rel, "no output requested");
+  GR_CHECK_ARG(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+  GR_CHECK_ARG(F >= 0 && Nt > 0 && Nt <= UINT_MAX, "need F >= 0 and 0 < Nt <= 2^32 - 1");
+  GR_CHECK_ARG(F <= (int64_t)INT_MAX, "F must fit int32 (hash slots are 32-bit)");
+  const WeightWorkspace ws = weight_workspace(F, Nt);
+  int rc = check_workspace(__func__, workspace, workspace_bytes, ws.total);
+  if (rc != GR_OK) return rc;
+  if (F == 0) return GR_OK;
+  char* base = static_cast<char*>(workspace);
+  const uint64_t T = weight_table_size(F);
+  auto* keys = reinterpret_cast<unsigned long long*>(base + ws.keys);
+  auto* counts = reinterpret_cast<uint32_t*>(base + ws.counts);
+  auto* deg = reinterpret_cast<uint32_t*>(base + ws.deg);
+  auto* slot_of = reinterpret_cast<uint32_t*>(base + ws.slot);
+  GR_CHECK_CUDA(cudaMemsetAsync(keys, 0xFF, T * sizeof(unsigned long long), stream));
+  GR_CHECK_CUDA(cudaMemsetAsync(counts, 0, ws.slot - ws.counts, stream));        // counts and deg
+  const int grid = (int)std::min<int64_t>(ceil_div(F, kWeightThreads), 8LL * sm_count());
+  fact_count_kernel<<<grid, kWeightThreads, 0, stream>>>(heads, rels, idx_bytes, F, Nt, keys, counts, T - 1, deg,
+                                                         slot_of, status);
+  GR_CHECK_LAUNCH();
+  fact_weight_kernel<<<grid, kWeightThreads, 0, stream>>>(heads, idx_bytes, F, counts, deg, slot_of, weight,
+                                                          weight_rel);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}

@@ -46,7 +46,7 @@ class _Captured:
 
 class Ticket:
     """One in-flight step of the submit/collect pipeline."""
-    __slots__ = ("slot", "done", "ent", "local_entity_host", "B", "N")
+    __slots__ = ("slot", "done", "ent", "local_entity_host", "cand_ent_host", "B", "N")
 
 
 def fact_capacity(F):
@@ -410,7 +410,11 @@ class GraphedStep:
             cs.wait_event(pipe.land_free[slot])
         land = pipe.land[slot]
         src = batch
-        if self._layout.needs_staging(batch):
+        le = batch[0]
+        on_device = isinstance(le, torch.Tensor) and le.is_cuda     # a loader.DeviceSplit batch
+        if on_device:
+            cs.wait_stream(cur)                      # the batch was assembled on the current stream
+        elif self._layout.needs_staging(batch):
             if pipe.h2d_done[slot] is not None:
                 pipe.h2d_done[slot].synchronize()    # the previous DMA out of this staging set has finished
             src = self._layout.stage_host(pipe.stage[slot], batch)
@@ -434,6 +438,13 @@ class GraphedStep:
         od["loss"].copy_(loss, non_blocking=True)
         for i, w in enumerate(self._layout.status_words(db)):
             od["status"][i:i + 1].copy_(w, non_blocking=True)
+        ents = None
+        if on_device:                                # the candidates' entity ids, gathered here instead of on the host
+            if getattr(pipe, "ents", None) is None:
+                pipe.ents = [(torch.empty_like(db.local_entity),
+                              torch.empty(db.local_entity.shape, dtype=torch.int64, pin_memory=True)) for _ in range(2)]
+            ents = pipe.ents[slot]
+            torch.gather(db.local_entity, 1, cand_idx.long(), out=ents[0])
         out_ready = torch.cuda.Event()
         out_ready.record(cur)
         ds = self._d2h_stream
@@ -441,14 +452,19 @@ class GraphedStep:
         with torch.cuda.stream(ds):
             for k, v in od.items():
                 pipe.out_host[slot][k].copy_(v, non_blocking=True)
+            if ents is not None:
+                ents[1].copy_(ents[0], non_blocking=True)
             pipe.done[slot] = torch.cuda.Event()
             pipe.done[slot].record(ds)
         db.h2d_bytes = self._h2d_bytes
         self.model.last_batch = db
         t = Ticket()
         t.slot, t.done, t.ent = slot, pipe.done[slot], ent
-        le = batch[0]
-        t.local_entity_host = le.cpu().numpy() if isinstance(le, torch.Tensor) else np.asarray(le)
+        if on_device:
+            t.local_entity_host, t.cand_ent_host = None, ents[1]
+        else:
+            t.local_entity_host = le.cpu().numpy() if isinstance(le, torch.Tensor) else np.asarray(le)
+            t.cand_ent_host = None
         t.B, t.N = db.B, db.N
         return t
 
@@ -463,11 +479,15 @@ class GraphedStep:
         idx_h, dist_h = h["cand_idx"].numpy(), h["pred_dist"].numpy()
         counts = h["cand_count"].numpy()
         le = ticket.local_entity_host
+        ents = None if ticket.cand_ent_host is None else ticket.cand_ent_host.numpy()
         res = []
         for b, c in enumerate(counts.tolist()):
             ix = idx_h[b, :c].astype(np.int64)
-            res.append(Retrieved(ix, le[b, ix].astype(np.int64), dist_h[b, ix]))
+            ent = le[b, ix].astype(np.int64) if ents is None else ents[b, :c].astype(np.int64)
+            res.append(Retrieved(ix, ent, dist_h[b, ix]))
         nbytes = sum(v.numel() * v.element_size() for v in h.values())
+        if ents is not None:
+            nbytes += ents.nbytes
         return res, nbytes, float(h["loss"]), h["pred"].numpy().copy()
 
     def retrieve(self, out):

@@ -30,8 +30,14 @@ the per-question triple taken from the loader's own ``create_kb_adj_mats_facts``
 
     loader.install_graft(GraftSingleDataLoader)    # monkeypatches _build_fact_mat_maxfacts
 
-Pure numpy on the host; nothing here touches the GPU.
+Everything above is pure numpy on the host.  :class:`DeviceSplit` goes one step further: it uploads a whole split
+once and assembles each batch on the GPU from its question ids (csrc/split.cu), so per batch only B ids cross PCIe:
+
+    split = loader.DeviceSplit(valid_data, torch.device("cuda"))
+    evaluator.evaluate(split, test_batch_size=20)          # get_batch returns the loader's tuple, built from CUDA tensors
 """
+import time
+
 import numpy as np
 
 
@@ -220,3 +226,212 @@ def install_graft(loader):
     else:
         loader._build_fact_mat_maxfacts = types.MethodType(build_fact_mat_maxfacts, loader)
     return orig
+
+
+_INT32_MAX = 2 ** 31 - 1
+
+
+class DeviceSplit:
+    """A split resident in device memory: ``get_batch`` assembles each batch on the GPU from its question ids.
+
+    ``DeviceSplit(data_loader, device, weights="arrays", index_dtype=torch.int32)`` wraps a ``SingleDataLoader`` or a
+    ``GraftSingleDataLoader`` (recognised by its ``create_kb_adj_mats_facts``) and uploads, once: the per-question
+    fact segments (int32 local ids with int64 offsets), the entity counts, the [num_q, N] tables
+    (``candidate_entities``, ``query_entities``, ``seed_distribution``, ``answer_dists``) and ``query_texts``; for
+    GraftNet also both graft lists per question and the stored prefix of every ``kb_fact_rels`` row.
+
+    ``get_batch(iteration, batch_size, fact_dropout, q_type=None, test=False)`` has the loader's signature and returns
+    its tuple layout (7-tuple, or GraftNet's 9-tuple; ``answer_lists`` appended with ``test=True``, still the loader's
+    host object array) built from CUDA tensors: ``local_entity`` int64 [B, N], ``query_entities`` / ``seed_dist`` /
+    ``answer_dist`` fp32 [B, N], ``q_input`` int64 [B, Q], ``kb_adj_mat`` with its five index arrays in
+    ``index_dtype`` and fp32 weights (``None`` with ``weights="none"``); GraftNet's graft lists in ``index_dtype``
+    with fp32 1.0 values and ``kb_fact_rel`` int64 [B, max_facts].  The facts are in stored order with the self-loops
+    appended per question, exactly :func:`build_fact_mat` with ``shuffle=False`` (and the graft lists
+    :func:`build_fact_mat_maxfacts` under the identity permutation); the weights are bit-equal to fp32 of the host's
+    float64 ones.  The question ids come from ``data_loader.batches`` as in the loader, so ``reset_batches`` works,
+    and ``sample_ids`` is set on the loader.  The fact count of a batch comes from a host copy of the per-question
+    counts, so assembling a batch never waits on the device.
+
+    Refused (``ValueError``): fact dropout, ``data_eff``, a ``q_type`` other than ``"seq"``, and a batch whose facts
+    would overflow int32 indices.  ``reset_batches``, ``num_data``, ``max_local_entity`` and ``get_quest`` pass
+    through to the loader, so ``Evaluator.evaluate(split)`` and a ``train_epoch``-shaped loop run unchanged."""
+
+    def __init__(self, data_loader, device, weights="arrays", index_dtype=None):
+        import torch
+        index_dtype = torch.int32 if index_dtype is None else index_dtype
+        if weights not in ("arrays", "none"):
+            raise ValueError("DeviceSplit: weights must be 'arrays' or 'none', got %r" % (weights,))
+        if index_dtype not in (torch.int32, torch.int64):
+            raise ValueError("DeviceSplit: index_dtype must be torch.int32 or torch.int64, got %s" % (index_dtype,))
+        if getattr(data_loader, "data_eff", False):
+            raise ValueError("DeviceSplit: data_eff loaders build their facts per batch; the split needs stored "
+                             "kb_adj_mats (data_eff off)")
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("DeviceSplit: the split lives on a CUDA device, got %s" % dev)
+        self.loader, self.device, self.weights, self.index_dtype = data_loader, dev, weights, index_dtype
+        self.graft = hasattr(data_loader, "create_kb_adj_mats_facts")
+        L = data_loader
+        N = int(L.max_local_entity)
+        self.N, self.self_rel, self.use_self_loop = N, int(L.num_kb_relation) - 1, bool(L.use_self_loop)
+        had_flat = getattr(L, "_gr_flat", None) is not None
+        fl = L._gr_flat if had_flat else preconvert(L)
+        num_q = len(fl["ents"])
+        self.num_q = num_q
+        for name in ("heads", "tails"):
+            a = fl[name]
+            if a.size and (a.min() < 0 or a.max() >= N):
+                raise ValueError("DeviceSplit: kb_adj_mats %s hold local ids outside [0, %d)" % (name, N))
+        if fl["rels"].size and (fl["rels"].min() < 0 or fl["rels"].max() > _INT32_MAX):
+            raise ValueError("DeviceSplit: kb_adj_mats hold relation ids outside [0, 2^31)")
+        if fl["ents"].size and fl["ents"].max() > N:
+            raise ValueError("DeviceSplit: a question has more entities than max_local_entity = %d" % N)
+        nf = np.diff(fl["off"])
+        self._count = nf + (fl["ents"] if self.use_self_loop else 0)       # host copy: facts per question
+
+        t0 = time.perf_counter()
+        self._res = {}
+        self._put("q_off", fl["off"], np.int64)
+        for name in ("heads", "rels", "tails"):
+            self._put("q_" + name, fl[name], np.int32)
+        self._put("q_ents", fl["ents"], np.int32)
+        self._put("local_entity", L.candidate_entities, np.int64)
+        for name, src in (("query_entities", L.query_entities), ("seed_dist", L.seed_distribution),
+                          ("answer_dist", L.answer_dists)):
+            self._put(name, src, np.float32)
+        self._put("q_input", L.query_texts, np.int64)
+        if self.graft:
+            self._upload_graft(L, num_q)
+        torch.cuda.synchronize(dev)
+        self.build_seconds = time.perf_counter() - t0        # the upload; preconvert and the graft parse come before
+        if not had_flat:
+            del L._gr_flat                                    # flattened here for the upload only
+        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+
+    def _put(self, name, a, dtype):
+        import torch
+        a = np.ascontiguousarray(np.asarray(a).astype(dtype, copy=False))
+        if a.size == 0:                 # a null pointer is refused: keep one element behind an empty array
+            a = np.zeros(1, dtype=dtype)
+        self._res[name] = torch.from_numpy(a).to(self.device)
+
+    def _upload_graft(self, L, num_q):
+        parts = [[] for _ in range(4)]
+        cnt = np.zeros(num_q, dtype=np.int64)
+        for q in range(num_q):
+            ((m00, m01, v0), (m10, m11, v1)), _rel = L.create_kb_adj_mats_facts(q)
+            if len(v0) != len(v1):
+                raise ValueError("DeviceSplit: question %d has graft lists of different lengths" % q)
+            if np.any(np.asarray(v0) != 1.0) or np.any(np.asarray(v1) != 1.0):
+                raise ValueError("DeviceSplit: question %d has graft values other than 1.0" % q)
+            cnt[q] = len(v0)
+            for lst, a in zip(parts, (m00, m01, m10, m11)):
+                lst.append(np.asarray(a, dtype=np.int64).ravel())
+        flat = [np.concatenate(p) if p else np.zeros(0, dtype=np.int64) for p in parts]
+        for a in flat:
+            if a.size and (a.min() < 0 or a.max() > _INT32_MAX):
+                raise ValueError("DeviceSplit: graft lists hold ids outside [0, 2^31)")
+        off = np.zeros(num_q + 1, dtype=np.int64)
+        np.cumsum(cnt, out=off[1:])
+        self._graft_count = cnt
+        self._put("g_off", off, np.int64)
+        for name, a in zip(("g_e2f_f", "g_e2f_e", "g_f2e_e", "g_f2e_f"), flat):
+            self._put(name, a, np.int32)
+        # kb_fact_rels rows (what get_batch reads): keep each row up to its last entry that is not the pad relation
+        kfr = np.asarray(L.kb_fact_rels)
+        self.max_facts, self.rel_pad = int(kfr.shape[1]), int(L.num_kb_relation)
+        live = kfr != self.rel_pad
+        rlen = np.where(live.any(axis=1), kfr.shape[1] - np.argmax(live[:, ::-1], axis=1), 0).astype(np.int64)
+        if kfr.size and (kfr.min() < 0 or kfr.max() > _INT32_MAX):
+            raise ValueError("DeviceSplit: kb_fact_rels hold relation ids outside [0, 2^31)")
+        roff = np.zeros(num_q + 1, dtype=np.int64)
+        np.cumsum(rlen, out=roff[1:])
+        vals = np.concatenate([kfr[q, :rlen[q]] for q in range(num_q)]) if num_q else np.zeros(0, dtype=np.int64)
+        self._put("r_off", roff, np.int64)
+        self._put("r_vals", vals, np.int32)
+
+    # -- what Evaluator.evaluate and train_epoch read from their loader ------------------------------------------------
+    @property
+    def num_data(self):
+        return self.loader.num_data
+
+    @property
+    def max_local_entity(self):
+        return self.loader.max_local_entity
+
+    def reset_batches(self, is_sequential=True):
+        return self.loader.reset_batches(is_sequential=is_sequential)
+
+    def get_quest(self, training=False):
+        return self.loader.get_quest(training)
+
+    @property
+    def resident_bytes(self):
+        """Device bytes the split holds."""
+        return int(sum(t.numel() * t.element_size() for t in self._res.values()))
+
+    def check(self):
+        """Raise when the last batch's assembly flagged an id out of range or an overflow (reads the device)."""
+        s = int(self.status.item())
+        if s:
+            raise RuntimeError("DeviceSplit: batch assembly status %d (1: question id out of range, 2: more facts than "
+                               "the batch's capacity)" % s)
+
+    # -- one batch ---------------------------------------------------------------------------------------------------
+    def get_batch(self, iteration, batch_size, fact_dropout, q_type=None, test=False):
+        import torch
+        from . import ops
+        L, r, dev = self.loader, self._res, self.device
+        if fact_dropout != 0:
+            raise ValueError("DeviceSplit.get_batch: fact_dropout must be 0 (facts come in stored order), got %r"
+                             % (fact_dropout,))
+        if q_type is None:
+            q_type = getattr(L, "q_type", "seq")
+        if q_type != "seq":
+            raise ValueError("DeviceSplit.get_batch: q_type must be 'seq', got %r" % (q_type,))
+        start = batch_size * iteration
+        end = min(batch_size * (iteration + 1), L.num_data)
+        sample_ids = L.batches[start:end]
+        L.sample_ids = sample_ids                                  # get_quest / deal_q_type read it
+        ids = np.asarray(sample_ids, dtype=np.int64).reshape(-1)
+        if ids.size and (ids.min() < 0 or ids.max() >= self.num_q):
+            raise ValueError("DeviceSplit.get_batch: question ids outside [0, %d)" % self.num_q)
+        B, N = len(ids), self.N
+        F = int(self._count[ids].sum())
+        idt = self.index_dtype
+        if idt == torch.int32 and (B * N > _INT32_MAX or F > _INT32_MAX):
+            raise ValueError("DeviceSplit.get_batch: the batch overflows int32 indices (B*N = %d, %d facts); use "
+                             "index_dtype=torch.int64" % (B * N, F))
+        ids_dev = torch.from_numpy(ids).to(dev, non_blocking=True)
+        rows = lambda name: torch.index_select(r[name], 0, ids_dev)      # noqa: E731
+        le, qe, sd, ad, qi = (rows(n) for n in ("local_entity", "query_entities", "seed_dist", "answer_dist",
+                                                 "q_input"))
+        if B:
+            heads, rels, tails, bids, fids, self.status = ops.split_assemble(
+                r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids_dev, N, F, self.self_rel,
+                self.use_self_loop, idt)
+        else:
+            heads, rels, tails, bids, fids = (torch.empty(0, dtype=idt, device=dev) for _ in range(5))
+        w = wr = None
+        if self.weights == "arrays":
+            if F:
+                w, wr, _st = ops.fact_weights(heads, rels, max(B * N, 1))
+            else:
+                w, wr = (torch.empty(0, dtype=torch.float32, device=dev) for _ in range(2))
+        kb = (heads, rels, tails, bids, fids, w, wr)
+        tail = (L.answer_lists[sample_ids],) if test else ()
+        if not self.graft:
+            return (le, qe, kb, qi, sd, None, ad) + tail
+        G = int(self._graft_count[ids].sum())
+        if idt == torch.int32 and G > _INT32_MAX:
+            raise ValueError("DeviceSplit.get_batch: the graft lists overflow int32 indices (%d entries)" % G)
+        if B:
+            graft, kfr, gst = ops.split_assemble_graft(
+                r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"], ids_dev,
+                self.max_facts, self.rel_pad, G, idt)
+            self.status = self.status | gst
+        else:
+            e = lambda dt: torch.empty(0, dtype=dt, device=dev)       # noqa: E731
+            graft = ((e(idt), e(idt), e(idt), e(torch.float32)), (e(idt), e(idt), e(idt), e(torch.float32)))
+            kfr = torch.empty(0, self.max_facts, dtype=torch.int64, device=dev)
+        return (le, qe, kb, graft, qi, kfr, sd, None, ad) + tail

@@ -955,6 +955,105 @@ def train_metrics(pred_dist, answer_dist, seed_dist, local_entity, cand_idx, can
     return h1, f1
 
 
+_INT32_MAX = 2 ** 31 - 1
+_INDEX_BYTES = {torch.int32: 4, torch.int64: 8}
+
+
+def split_assemble_ok(B, N, F, index_dtype):
+    """True when gr_split_assemble admits a batch of B questions of N nodes and F facts: B > 0, N > 0, F >= 0, an
+    int32 or int64 index dtype, and with int32 B*N and F within the int32 range."""
+    if index_dtype not in _INDEX_BYTES or B <= 0 or N <= 0 or F < 0:
+        return False
+    return index_dtype == torch.int64 or (B * N <= _INT32_MAX and F <= _INT32_MAX)
+
+
+def split_assemble(q_off, q_heads, q_rels, q_tails, q_ents, ids, N, F, self_rel, use_self_loop, index_dtype):
+    """-> (heads, rels, tails, batch_ids, fact_ids, status): the fact arrays of the questions ``ids`` (int64 [B] on the
+    device) of a resident split (gr_split_assemble), each [F] in ``index_dtype``; ``status`` int32[1] on the device
+    (bit 1: an id out of range, bit 2: more facts than F).  q_off int64 [num_q+1]; q_heads/q_rels/q_tails int32 (local
+    ids, by question); q_ents int32 [num_q]."""
+    q_off = _cuda(q_off, torch.int64, "q_off").contiguous()
+    q_heads, q_rels, q_tails, q_ents = (_cuda(t, torch.int32, n).contiguous() for t, n in
+                                        ((q_heads, "q_heads"), (q_rels, "q_rels"), (q_tails, "q_tails"),
+                                         (q_ents, "q_ents")))
+    ids = _cuda(ids, torch.int64, "ids").contiguous()
+    B, num_q = ids.numel(), q_ents.numel()
+    if not split_assemble_ok(B, N, F, index_dtype):
+        raise RuntimeError("split_assemble: need B > 0, N > 0, F >= 0 and an int32 / int64 index dtype whose range "
+                           "holds B*N and F, got B=%d N=%d F=%d %s" % (B, N, F, index_dtype))
+    dev = ids.device
+    out = [torch.empty(F, dtype=index_dtype, device=dev) for _ in range(5)]
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    _launch("gr_split_assemble", _p(q_off), _p(q_heads), _p(q_rels), _p(q_tails), _p(q_ents), num_q, _p(ids), B,
+            int(N), int(self_rel), int(bool(use_self_loop)), _INDEX_BYTES[index_dtype], int(F),
+            *(_p(t) if F else None for t in out), _p(status), op="split_assemble")
+    return (*out, status)
+
+
+def split_assemble_graft_ok(B, max_facts, G, index_dtype):
+    """True when gr_split_assemble_graft admits B questions, rows of max_facts and G graft entries: B > 0,
+    max_facts >= 0, G >= 0, an int32 or int64 index dtype, and with int32 G and max_facts within the int32 range."""
+    if index_dtype not in _INDEX_BYTES or B <= 0 or max_facts < 0 or G < 0:
+        return False
+    return index_dtype == torch.int64 or (G <= _INT32_MAX and max_facts <= _INT32_MAX)
+
+
+def split_assemble_graft(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, ids, max_facts, rel_pad, G,
+                         index_dtype):
+    """-> ((e2f_b, e2f_f, e2f_e, e2f_v), (f2e_b, f2e_e, f2e_f, f2e_v)), kb_fact_rel, status: the graft lists ([G], the
+    index entries in ``index_dtype``, the values fp32 1.0) and kb_fact_rel int64 [B, max_facts] of the questions
+    ``ids`` of a resident split (gr_split_assemble_graft); ``status`` as :func:`split_assemble`."""
+    g_off, r_off = _cuda(g_off, torch.int64, "g_off").contiguous(), _cuda(r_off, torch.int64, "r_off").contiguous()
+    lists = [_cuda(t, torch.int32, n).contiguous() for t, n in
+             ((g_e2f_f, "g_e2f_f"), (g_e2f_e, "g_e2f_e"), (g_f2e_e, "g_f2e_e"), (g_f2e_f, "g_f2e_f"),
+              (r_vals, "r_vals"))]
+    ids = _cuda(ids, torch.int64, "ids").contiguous()
+    B, num_q = ids.numel(), g_off.numel() - 1
+    if not split_assemble_graft_ok(B, max_facts, G, index_dtype):
+        raise RuntimeError("split_assemble_graft: need B > 0, max_facts >= 0, G >= 0 and an int32 / int64 index dtype "
+                           "whose range holds G and max_facts, got B=%d max_facts=%d G=%d %s"
+                           % (B, max_facts, G, index_dtype))
+    dev = ids.device
+    idx = [torch.empty(G, dtype=index_dtype, device=dev) for _ in range(6)]
+    vals = [torch.empty(G, dtype=torch.float32, device=dev) for _ in range(2)]
+    kfr = torch.empty(B, max_facts, dtype=torch.int64, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    p = (lambda t: _p(t) if t.numel() else None)     # noqa: E731
+    _launch("gr_split_assemble_graft", _p(g_off), *(_p(t) for t in lists[:4]), _p(r_off), _p(lists[4]), num_q,
+            _p(ids), B, int(max_facts), int(rel_pad), _INDEX_BYTES[index_dtype], int(G),
+            p(idx[0]), p(idx[1]), p(idx[2]), p(vals[0]), p(idx[3]), p(idx[4]), p(idx[5]), p(vals[1]), p(kfr),
+            _p(status), op="split_assemble")
+    return ((idx[0], idx[1], idx[2], vals[0]), (idx[3], idx[4], idx[5], vals[1])), kfr, status
+
+
+def fact_weights_ok(F, Nt):
+    """True when gr_fact_weights admits F facts over Nt node rows: 0 <= F <= 2^31 - 1 and 0 < Nt < 2^32."""
+    return 0 <= F <= _INT32_MAX and 0 < Nt < 2 ** 32
+
+
+def fact_weights(heads, rels, Nt, weight=True, weight_rel=True):
+    """-> (weight_list, weight_rel_list, status): fp32 [F] 1/outdeg(head) and 1/count(head, rel) of a fact list
+    (gr_fact_weights), each bit-equal to fp32 of the host's float64 value; None for an output not asked for.
+    heads/rels: int32 or int64 [F] on the device, heads global rows in [0, Nt)."""
+    heads, rels = _cuda(heads, name="heads").contiguous(), _cuda(rels, name="rels").contiguous()
+    if heads.dtype not in _INDEX_BYTES or rels.dtype != heads.dtype:
+        raise RuntimeError("fact_weights: heads and rels must share dtype int32 or int64")
+    F = heads.numel()
+    if not fact_weights_ok(F, Nt) or not (weight or weight_rel):
+        raise RuntimeError("fact_weights: need 0 <= F <= 2^31 - 1, 0 < Nt < 2^32 and an output, got F=%d Nt=%d"
+                           % (F, Nt))
+    dev = heads.device
+    w = torch.empty(F, dtype=torch.float32, device=dev) if weight else None
+    wr = torch.empty(F, dtype=torch.float32, device=dev) if weight_rel else None
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    if F == 0:
+        return w, wr, status
+    ws, nbytes = _workspace(dev, "gr_fact_weights_workspace_bytes", F, Nt)
+    _launch("gr_fact_weights", _p(heads), _p(rels), _INDEX_BYTES[heads.dtype], F, int(Nt), _p(w), _p(wr),
+            _p(status), _p(ws), nbytes, launches=2, op="split_assemble")
+    return w, wr, status
+
+
 def shortest_path_nodes(g, source_idx, source_cnt, target_idx, target_cnt, return_distances=False):
     """source_idx int32[B,S], target_idx int32[B,T] local indices (+counts) ->
     (on_path uint8[B,N], pair_dist int32[B,S,T]); with ``return_distances`` also the BFS distance arrays the kernel

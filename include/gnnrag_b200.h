@@ -667,6 +667,45 @@ int gr_train_metrics(const float* pred_dist, const float* answer_dist, const flo
                      float* h1, float* f1, int B, int N, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Device-resident split (loader.DeviceSplit, csrc/split.cu): a split's per-question facts are uploaded once and
+ * every batch is assembled on the device from B question ids (the int64 device array `ids`, B > 0).
+ * A question id outside [0, num_q) counts as an empty question and sets bit 1 of `status` (int32[1], OR-ed); a batch
+ * whose entries would run past the capacity passed (F, G) is cut there and sets bit 2.  Nothing is read or written
+ * outside the arrays.  Index outputs are int64 (idx_bytes = 8) or int32 (idx_bytes = 4; refused when B*N, the
+ * capacity or self_rel exceed INT_MAX).  Launch shape: (CTAs per question, B), a function of B alone.
+ *
+ * gr_split_assemble: the kb_adj_mat arrays of SingleDataLoader._build_fact_mat (gnn/dataset_load.py:473-527) in
+ * STORED fact order (loader.build_fact_mat with shuffle=False): question b = ids[b] contributes its facts
+ * q_heads/q_rels/q_tails[q_off[id] .. q_off[id+1]) (int32 local ids) with heads/tails + b*N, then, with use_self_loop,
+ * one self-loop (b*N + k, self_rel, b*N + k) for each k < q_ents[id]; batch_ids = b, fact_ids = position.
+ * q_off: int64 [num_q+1]; q_ents: int32 [num_q]; outputs: [F], F = the batch's fact count computed by the caller. */
+int gr_split_assemble(const int64_t* q_off, const int32_t* q_heads, const int32_t* q_rels, const int32_t* q_tails,
+                      const int32_t* q_ents, int64_t num_q, const int64_t* ids, int B, int64_t N, int64_t self_rel,
+                      int use_self_loop, int idx_bytes, int64_t F, void* heads, void* rels, void* tails,
+                      void* batch_ids, void* fact_ids, int32_t* status, void* stream);
+
+/* gr_split_assemble_graft: the graft lists of GraftSingleDataLoader._build_fact_mat_maxfacts
+ * (gnn/dataset_load_graft.py:70-102) in stored order: question b = ids[b] contributes entries g_off[id] .. g_off[id+1]
+ * to e2f = (b, g_e2f_f, g_e2f_e, 1.0) and f2e = (b, g_f2e_e, g_f2e_f, 1.0); the lists have G entries.  kb_fact_rel
+ * int64 [B, max_facts]: row b = r_vals[r_off[id] .. r_off[id+1]) (at most max_facts entries), then rel_pad. */
+int gr_split_assemble_graft(const int64_t* g_off, const int32_t* g_e2f_f, const int32_t* g_e2f_e,
+                            const int32_t* g_f2e_e, const int32_t* g_f2e_f, const int64_t* r_off,
+                            const int32_t* r_vals, int64_t num_q, const int64_t* ids, int B, int64_t max_facts,
+                            int64_t rel_pad, int idx_bytes, int64_t G, void* e2f_b, void* e2f_f, void* e2f_e,
+                            float* e2f_v, void* f2e_b, void* f2e_e, void* f2e_f, float* f2e_v, int64_t* kb_fact_rel,
+                            int32_t* status, void* stream);
+
+/* gr_fact_weights: weight_list / weight_rel_list of _build_fact_mat (gnn/dataset_load.py:507-516) for F facts with
+ * global head rows in [0, Nt): weight[f] = 1 / #facts with head[f], weight_rel[f] = 1 / #facts with (head[f], rel[f]),
+ * each 1.0 / count in float64 rounded once to fp32 (bit-equal to fp32 of the host's float64 values).  Integer
+ * counting only (no float atomics).  Either output may be null (not both).  A fact whose head is outside [0, Nt) or
+ * whose relation is negative sets status bit 1, is left out of the counts and gets weight 0.  F <= INT_MAX.
+ * Workspace: gr_fact_weights_workspace_bytes(F, Nt). */
+size_t gr_fact_weights_workspace_bytes(int64_t F, int64_t Nt);
+int gr_fact_weights(const void* heads, const void* rels, int idx_bytes, int64_t F, int64_t Nt, float* weight,
+                    float* weight_rel, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Shortest-path node sets (SURVEY.md 8f row 1): nodes lying on any shortest path between any seed and
  * any retrieved candidate in the UNDIRECTED subgraph -- build_graph + get_truth_paths,
  * llm/src/utils/graph_utils.py:10-21,49-75.  Uses both CSRs of a question batch; one CTA per question.

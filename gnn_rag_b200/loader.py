@@ -35,6 +35,12 @@ once and assembles each batch on the GPU from its question ids (csrc/split.cu), 
 
     split = loader.DeviceSplit(valid_data, torch.device("cuda"))
     evaluator.evaluate(split, test_batch_size=20)          # get_batch returns the loader's tuple, built from CUDA tensors
+
+With ``shuffle=True`` it also draws the reference's fact dropout on the device, so ``train_epoch`` with
+``fact_drop > 0`` trains from a resident split:
+
+    train = loader.DeviceSplit(train_data, torch.device("cuda"), shuffle=True)
+    batch = train.get_batch(iteration, batch_size, fact_dropout=args['fact_drop'])
 """
 import time
 
@@ -231,6 +237,12 @@ def install_graft(loader):
 _INT32_MAX = 2 ** 31 - 1
 
 
+def kept_counts(n, fact_dropout):
+    """Facts kept per question under fact dropout: ``int(np.floor(n * (1 - fact_dropout)))`` of the reference
+    (gnn/dataset_load.py:488, gnn/dataset_load_graft.py:88) for every count in ``n``, in float64 as there.  int64."""
+    return np.floor(np.asarray(n, dtype=np.int64) * (1 - float(fact_dropout))).astype(np.int64)
+
+
 class DeviceSplit:
     """A split resident in device memory: ``get_batch`` assembles each batch on the GPU from its question ids.
 
@@ -252,11 +264,22 @@ class DeviceSplit:
     and ``sample_ids`` is set on the loader.  The fact count of a batch comes from a host copy of the per-question
     counts, so assembling a batch never waits on the device.
 
-    Refused (``ValueError``): fact dropout, ``data_eff``, a ``q_type`` other than ``"seq"``, and a batch whose facts
-    would overflow int32 indices.  ``reset_batches``, ``num_data``, ``max_local_entity`` and ``get_quest`` pass
-    through to the loader, so ``Evaluator.evaluate(split)`` and a ``train_epoch``-shaped loop run unchanged."""
+    Refused (``ValueError``): fact dropout without ``shuffle`` (with it, one outside [0, 1]), ``data_eff``, a
+    ``q_type`` other than ``"seq"``, and a batch whose facts would overflow int32 indices.  ``reset_batches``, ``num_data``, ``max_local_entity`` and ``get_quest`` pass
+    through to the loader, so ``Evaluator.evaluate(split)`` and a ``train_epoch``-shaped loop run unchanged.
 
-    def __init__(self, data_loader, device, weights="arrays", index_dtype=None):
+    ``shuffle=True`` samples facts as the reference's training batches do (:func:`build_fact_mat` with
+    ``shuffle=True``, :func:`build_fact_mat_maxfacts`): ``get_batch(it, B, p)`` takes any ``p`` in [0, 1], and each
+    question keeps :func:`kept_counts` of its facts, the first of a uniform random permutation, in permutation order,
+    with its self-loops after them in entity order.  GraftNet's graft lists keep the same number of their entries
+    from a second, independent permutation; ``kb_fact_rel`` rows stay as stored.  The permutations are drawn on the
+    device (csrc/split.cu, gr_split_fact_order) from one seed per call taken from torch's CUDA generator, so
+    ``torch.manual_seed`` makes a run reproducible and no call waits on the device.  ``np.random`` is not touched:
+    the sampled facts differ from the host loader's for the same numpy seed.  The last batch's orders are kept in
+    ``last_order``: ``kb`` / ``graft`` device int32 arrays of stored indices per question, in batch order, and
+    ``kb_offsets`` / ``graft_offsets`` numpy int64 [B+1] where each question's run starts."""
+
+    def __init__(self, data_loader, device, weights="arrays", index_dtype=None, shuffle=False):
         import torch
         index_dtype = torch.int32 if index_dtype is None else index_dtype
         if weights not in ("arrays", "none"):
@@ -270,6 +293,7 @@ class DeviceSplit:
         if dev.type != "cuda":
             raise ValueError("DeviceSplit: the split lives on a CUDA device, got %s" % dev)
         self.loader, self.device, self.weights, self.index_dtype = data_loader, dev, weights, index_dtype
+        self.shuffle, self.last_order = bool(shuffle), None
         self.graft = hasattr(data_loader, "create_kb_adj_mats_facts")
         L = data_loader
         N = int(L.max_local_entity)
@@ -287,7 +311,10 @@ class DeviceSplit:
         if fl["ents"].size and fl["ents"].max() > N:
             raise ValueError("DeviceSplit: a question has more entities than max_local_entity = %d" % N)
         nf = np.diff(fl["off"])
-        self._count = nf + (fl["ents"] if self.use_self_loop else 0)       # host copy: facts per question
+        # host copies per question: stored facts, self-loops, and both together
+        self._stored = nf
+        self._ents = fl["ents"] if self.use_self_loop else np.zeros_like(nf)
+        self._count = nf + self._ents
 
         t0 = time.perf_counter()
         self._res = {}
@@ -382,9 +409,11 @@ class DeviceSplit:
         import torch
         from . import ops
         L, r, dev = self.loader, self._res, self.device
-        if fact_dropout != 0:
+        if not self.shuffle and fact_dropout != 0:
             raise ValueError("DeviceSplit.get_batch: fact_dropout must be 0 (facts come in stored order), got %r"
                              % (fact_dropout,))
+        if self.shuffle and not 0 <= fact_dropout <= 1:
+            raise ValueError("DeviceSplit.get_batch: fact_dropout must be in [0, 1], got %r" % (fact_dropout,))
         if q_type is None:
             q_type = getattr(L, "q_type", "seq")
         if q_type != "seq":
@@ -397,16 +426,35 @@ class DeviceSplit:
         if ids.size and (ids.min() < 0 or ids.max() >= self.num_q):
             raise ValueError("DeviceSplit.get_batch: question ids outside [0, %d)" % self.num_q)
         B, N = len(ids), self.N
-        F = int(self._count[ids].sum())
+        if self.shuffle:
+            kept = kept_counts(self._stored[ids], fact_dropout)
+            F = int(kept.sum() + self._ents[ids].sum())
+        else:
+            F = int(self._count[ids].sum())
         idt = self.index_dtype
         if idt == torch.int32 and (B * N > _INT32_MAX or F > _INT32_MAX):
             raise ValueError("DeviceSplit.get_batch: the batch overflows int32 indices (B*N = %d, %d facts); use "
                              "index_dtype=torch.int64" % (B * N, F))
-        ids_dev = torch.from_numpy(ids).to(dev, non_blocking=True)
+        if self.shuffle:
+            kept_g = kept_counts(self._graft_count[ids], fact_dropout) if self.graft else kept[:0]
+            # one upload: the ids, then the kept counts of the kb facts and of the graft lists
+            up = torch.from_numpy(np.concatenate([ids, kept, kept_g])).to(dev, non_blocking=True)
+            ids_dev, kept_dev, kept_g_dev = up[:B], up[B:2 * B], up[2 * B:]
+            seed = torch.randint(0, 2 ** 62, (1,), device=dev)
+        else:
+            ids_dev = torch.from_numpy(ids).to(dev, non_blocking=True)
         rows = lambda name: torch.index_select(r[name], 0, ids_dev)      # noqa: E731
         le, qe, sd, ad, qi = (rows(n) for n in ("local_entity", "query_entities", "seed_dist", "answer_dist",
                                                  "q_input"))
-        if B:
+        if B and self.shuffle:
+            K = int(kept.sum())
+            order, ost = ops.split_fact_order(r["q_off"], ids_dev, kept_dev, seed, 0, int(self._stored[ids].sum()), K)
+            heads, rels, tails, bids, fids, self.status = ops.split_assemble_ordered(
+                r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids_dev, kept_dev, order, N, F,
+                self.self_rel, self.use_self_loop, idt)
+            self.status = self.status | ost
+            self.last_order = dict(kb=order, kb_offsets=np.concatenate([[0], np.cumsum(kept)]))
+        elif B:
             heads, rels, tails, bids, fids, self.status = ops.split_assemble(
                 r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids_dev, N, F, self.self_rel,
                 self.use_self_loop, idt)
@@ -422,10 +470,18 @@ class DeviceSplit:
         tail = (L.answer_lists[sample_ids],) if test else ()
         if not self.graft:
             return (le, qe, kb, qi, sd, None, ad) + tail
-        G = int(self._graft_count[ids].sum())
+        G = int(kept_g.sum()) if self.shuffle else int(self._graft_count[ids].sum())
         if idt == torch.int32 and G > _INT32_MAX:
             raise ValueError("DeviceSplit.get_batch: the graft lists overflow int32 indices (%d entries)" % G)
-        if B:
+        if B and self.shuffle:
+            gorder, ost = ops.split_fact_order(r["g_off"], ids_dev, kept_g_dev, seed, 1,
+                                               int(self._graft_count[ids].sum()), G)
+            graft, kfr, gst = ops.split_assemble_graft_ordered(
+                r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"], ids_dev,
+                kept_g_dev, gorder, self.max_facts, self.rel_pad, G, idt)
+            self.status = self.status | gst | ost
+            self.last_order.update(graft=gorder, graft_offsets=np.concatenate([[0], np.cumsum(kept_g)]))
+        elif B:
             graft, kfr, gst = ops.split_assemble_graft(
                 r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"], ids_dev,
                 self.max_facts, self.rel_pad, G, idt)

@@ -1026,6 +1026,86 @@ def split_assemble_graft(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_val
     return ((idx[0], idx[1], idx[2], vals[0]), (idx[3], idx[4], idx[5], vals[1])), kfr, status
 
 
+def split_fact_order_ok(B, n_total, K):
+    """True when gr_split_fact_order admits B questions holding n_total stored facts with K kept in all: B > 0,
+    n_total >= 0 and 0 <= K <= 2^31 - 1."""
+    return B > 0 and n_total >= 0 and 0 <= K <= _INT32_MAX
+
+
+def split_fact_order(off, ids, kept, seed, perm, n_total, K):
+    """-> (order, status): order int32 [K], per question of ``ids`` in batch order the stored indices of the first
+    ``kept[b]`` facts of the question's permutation drawn from ``seed`` (gr_split_fact_order); ``status`` as
+    :func:`split_assemble`.  off int64 [num_q+1] (q_off or g_off); ids, kept int64 [B]; seed int64 [1], all on the
+    device; perm 0 (kb facts) or 1 (graft lists); n_total >= the stored facts of the B questions."""
+    off = _cuda(off, torch.int64, "off").contiguous()
+    ids, kept = _cuda(ids, torch.int64, "ids").contiguous(), _cuda(kept, torch.int64, "kept").contiguous()
+    seed = _cuda(seed, torch.int64, "seed").contiguous()
+    B, num_q = ids.numel(), off.numel() - 1
+    if not split_fact_order_ok(B, n_total, K) or kept.numel() != B or seed.numel() != 1:
+        raise RuntimeError("split_fact_order: need B > 0, kept [B], one seed, n_total >= 0 and 0 <= K <= 2^31 - 1, "
+                           "got B=%d kept %s n_total=%d K=%d" % (B, list(kept.shape), n_total, K))
+    dev = ids.device
+    order = torch.empty(K, dtype=torch.int32, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    ws, nbytes = _workspace(dev, "gr_split_fact_order_workspace_bytes", int(n_total))
+    _launch("gr_split_fact_order", _p(off), num_q, _p(ids), _p(kept), B, _p(seed), int(perm), int(n_total), int(K),
+            _p(order) if K else None, _p(status), _p(ws), nbytes, op="split_assemble")
+    return order, status
+
+
+def split_assemble_ordered(q_off, q_heads, q_rels, q_tails, q_ents, ids, kept, order, N, F, self_rel, use_self_loop,
+                           index_dtype):
+    """:func:`split_assemble` with question b contributing the facts at the stored indices of its ``kept[b]`` entries
+    of ``order`` (:func:`split_fact_order`), then its self-loops (gr_split_assemble_ordered).  Shape rule:
+    :func:`split_assemble_ok`."""
+    q_off = _cuda(q_off, torch.int64, "q_off").contiguous()
+    q_heads, q_rels, q_tails, q_ents = (_cuda(t, torch.int32, n).contiguous() for t, n in
+                                        ((q_heads, "q_heads"), (q_rels, "q_rels"), (q_tails, "q_tails"),
+                                         (q_ents, "q_ents")))
+    ids, kept = _cuda(ids, torch.int64, "ids").contiguous(), _cuda(kept, torch.int64, "kept").contiguous()
+    order = _cuda(order, torch.int32, "order").contiguous()
+    B, num_q, K = ids.numel(), q_ents.numel(), order.numel()
+    if not split_assemble_ok(B, N, F, index_dtype) or kept.numel() != B:
+        raise RuntimeError("split_assemble_ordered: need B > 0, kept [B], N > 0, F >= 0 and an int32 / int64 index "
+                           "dtype whose range holds B*N and F, got B=%d N=%d F=%d %s" % (B, N, F, index_dtype))
+    dev = ids.device
+    out = [torch.empty(F, dtype=index_dtype, device=dev) for _ in range(5)]
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    _launch("gr_split_assemble_ordered", _p(q_off), _p(q_heads), _p(q_rels), _p(q_tails), _p(q_ents), num_q, _p(ids),
+            _p(kept), _p(order) if K else None, K, B, int(N), int(self_rel), int(bool(use_self_loop)),
+            _INDEX_BYTES[index_dtype], int(F), *(_p(t) if F else None for t in out), _p(status), op="split_assemble")
+    return (*out, status)
+
+
+def split_assemble_graft_ordered(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, ids, kept, order,
+                                 max_facts, rel_pad, G, index_dtype):
+    """:func:`split_assemble_graft` with both graft lists taking question b's entries at its ``kept[b]`` positions of
+    ``order`` (gr_split_assemble_graft_ordered); the kb_fact_rel rows are the stored ones.  Shape rule:
+    :func:`split_assemble_graft_ok`."""
+    g_off, r_off = _cuda(g_off, torch.int64, "g_off").contiguous(), _cuda(r_off, torch.int64, "r_off").contiguous()
+    lists = [_cuda(t, torch.int32, n).contiguous() for t, n in
+             ((g_e2f_f, "g_e2f_f"), (g_e2f_e, "g_e2f_e"), (g_f2e_e, "g_f2e_e"), (g_f2e_f, "g_f2e_f"),
+              (r_vals, "r_vals"))]
+    ids, kept = _cuda(ids, torch.int64, "ids").contiguous(), _cuda(kept, torch.int64, "kept").contiguous()
+    order = _cuda(order, torch.int32, "order").contiguous()
+    B, num_q, K = ids.numel(), g_off.numel() - 1, order.numel()
+    if not split_assemble_graft_ok(B, max_facts, G, index_dtype) or kept.numel() != B:
+        raise RuntimeError("split_assemble_graft_ordered: need B > 0, kept [B], max_facts >= 0, G >= 0 and an int32 / "
+                           "int64 index dtype whose range holds G and max_facts, got B=%d max_facts=%d G=%d %s"
+                           % (B, max_facts, G, index_dtype))
+    dev = ids.device
+    idx = [torch.empty(G, dtype=index_dtype, device=dev) for _ in range(6)]
+    vals = [torch.empty(G, dtype=torch.float32, device=dev) for _ in range(2)]
+    kfr = torch.empty(B, max_facts, dtype=torch.int64, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    p = (lambda t: _p(t) if t.numel() else None)     # noqa: E731
+    _launch("gr_split_assemble_graft_ordered", _p(g_off), *(_p(t) for t in lists[:4]), _p(r_off), _p(lists[4]),
+            num_q, _p(ids), _p(kept), p(order), K, B, int(max_facts), int(rel_pad), _INDEX_BYTES[index_dtype], int(G),
+            p(idx[0]), p(idx[1]), p(idx[2]), p(vals[0]), p(idx[3]), p(idx[4]), p(idx[5]), p(vals[1]), p(kfr),
+            _p(status), op="split_assemble")
+    return ((idx[0], idx[1], idx[2], vals[0]), (idx[3], idx[4], idx[5], vals[1])), kfr, status
+
+
 def fact_weights_ok(F, Nt):
     """True when gr_fact_weights admits F facts over Nt node rows: 0 <= F <= 2^31 - 1 and 0 < Nt < 2^32."""
     return 0 <= F <= _INT32_MAX and 0 < Nt < 2 ** 32

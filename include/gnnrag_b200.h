@@ -705,6 +705,43 @@ size_t gr_fact_weights_workspace_bytes(int64_t F, int64_t Nt);
 int gr_fact_weights(const void* heads, const void* rels, int idx_bytes, int64_t F, int64_t Nt, float* weight,
                     float* weight_rel, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Fact dropout on a resident split (loader.DeviceSplit with shuffle=True): the reference keeps the first
+ * floor(n (1 - p)) facts of a fresh np.random.permutation of each question's n stored facts.  `kept` (int64 [B], from
+ * the host) holds those counts; a count is clamped to [0, n] (n = 0 for an id out of range).
+ *
+ * gr_split_fact_order: order (int32 [K]) = per question b, in batch order, the stored indices (0 .. n-1) of the first
+ * kept[b] facts of the permutation that sorts the question's facts by (key, index) ascending, where fact i's key is
+ * the 64-bit value whose high word is philox4x32_10_x0(*seed, i lo, i hi, b, perm) and whose low word is
+ * philox4x32_10_x0(*seed, i lo, i hi, b, perm | 2).  perm = 0 for the kb facts, 1 for the graft lists.  off is the
+ * question offsets (q_off or g_off, int64 [num_q+1]); seed is one int64 on the device.  Deterministic for a seed.
+ * n_total >= the sum of the stored counts of the B questions sizes the workspace
+ * (gr_split_fact_order_workspace_bytes(n_total)).  A question whose kept prefix would run past K, or that holds more
+ * than INT_MAX facts, is not written and sets status bit 2.  One CTA per question, any question size. */
+size_t gr_split_fact_order_workspace_bytes(int64_t n_total);
+int gr_split_fact_order(const int64_t* off, int64_t num_q, const int64_t* ids, const int64_t* kept, int B,
+                        const int64_t* seed, int perm, int64_t n_total, int64_t K, int32_t* order, int32_t* status,
+                        void* workspace, size_t workspace_bytes, void* stream);
+
+/* gr_split_assemble_ordered: gr_split_assemble with question b contributing the facts order[o_b .. o_b + kept[b])
+ * (stored indices; o_b = the kept counts before b) instead of all of its facts, then its self-loops.  F = the sum of
+ * kept[b] (+ q_ents with use_self_loop).  An order entry outside [0, n) sets status bit 1 and its fact is not
+ * written; reading past K sets bit 2. */
+int gr_split_assemble_ordered(const int64_t* q_off, const int32_t* q_heads, const int32_t* q_rels,
+                              const int32_t* q_tails, const int32_t* q_ents, int64_t num_q, const int64_t* ids,
+                              const int64_t* kept, const int32_t* order, int64_t K, int B, int64_t N,
+                              int64_t self_rel, int use_self_loop, int idx_bytes, int64_t F, void* heads, void* rels,
+                              void* tails, void* batch_ids, void* fact_ids, int32_t* status, void* stream);
+
+/* gr_split_assemble_graft_ordered: gr_split_assemble_graft with both graft lists taking question b's entries at the
+ * positions order[o_b .. o_b + kept[b]) (G = the sum of kept[b]); the kb_fact_rel rows are the stored ones. */
+int gr_split_assemble_graft_ordered(const int64_t* g_off, const int32_t* g_e2f_f, const int32_t* g_e2f_e,
+                                    const int32_t* g_f2e_e, const int32_t* g_f2e_f, const int64_t* r_off,
+                                    const int32_t* r_vals, int64_t num_q, const int64_t* ids, const int64_t* kept,
+                                    const int32_t* order, int64_t K, int B, int64_t max_facts, int64_t rel_pad,
+                                    int idx_bytes, int64_t G, void* e2f_b, void* e2f_f, void* e2f_e, float* e2f_v,
+                                    void* f2e_b, void* f2e_e, void* f2e_f, float* f2e_v, int64_t* kb_fact_rel,
+                                    int32_t* status, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Shortest-path node sets (SURVEY.md 8f row 1): nodes lying on any shortest path between any seed and
  * any retrieved candidate in the UNDIRECTED subgraph -- build_graph + get_truth_paths,

@@ -1,0 +1,154 @@
+"""Training rate with fact dropout, the batch sampled and assembled on the host vs on the device
+(loader.DeviceSplit(shuffle=True)), and the device time of gr_split_fact_order.
+
+A train_epoch-shaped loop (gnn/train_model.py:219) over a synthetic WebQSP-shape split (scripts/device_split_probe.py:
+N = 2000 nodes, E = 6000 stored facts per question, self-loops on): per batch ``get_batch(it, B, 0.1)``, the step,
+``loss.item()`` as train_epoch logs it, clip_grad_norm_ and Adam.step().
+
+  host    the loader's get_batch with loader.install(shuffle=True, weights="arrays", index_dtype=np.int32)
+          (GraftNet: plus loader.install_graft), so np.random.permutation per question as in the reference
+  device  DeviceSplit(loader, weights="arrays", shuffle=True).get_batch
+
+Shapes: ReaRev and NSM at the reference's training shape (B 8, entity_dim 50) through graphed.GraphedTrainStep;
+GraftNet (B 8, entity_dim 50) eager, as GraphedTrainStep refuses it; and cfg2 (ReaRev, B 64, entity_dim 200) through
+GraphedTrainStep.  A pass runs the whole split; the questions/s of a mode is the median over ``--runs`` passes, host
+and device alternating, after one warm-up pass of each (graph captures).  Then gr_split_fact_order alone, between CUDA
+events over ``--launches`` launches: B = 64 questions of 6 000 facts, and one question of 50 000 facts.  The GPU's
+name and power limit are read in the same run.  One JSON line per measurement.
+
+    python scripts/split_shuffle_probe.py [--questions 640] [--runs 3] [--out split_shuffle_probe.json]
+"""
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+
+import gnn_rag_b200 as G                                        # noqa: E402
+from gnn_rag_b200 import graphed, loader, ops, synthetic as S  # noqa: E402
+from device_split_probe import NE, NR, NW, SyntheticSplit, gpu_info  # noqa: E402
+
+SHAPES = {   # name -> model, batch size, model arguments, graphed
+    "rearev_d50": ("ReaRev", 8, dict(entity_dim=50, num_ins=3, num_iter=2, num_gnn=3), True),
+    "nsm_d50": ("NSM", 8, dict(entity_dim=50), True),
+    "graftnet_d50": ("GraftNet", 8, dict(entity_dim=50), False),
+    "cfg2": ("ReaRev", 64, dict(entity_dim=200, num_ins=2, num_iter=3, num_gnn=3), True),
+}
+FACT_DROP = 0.1
+
+
+def train_pass(data, step_fn, B):
+    """One epoch over the split, train_epoch-shaped; -> seconds."""
+    nb = (data.num_data + B - 1) // B
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for it in range(nb):
+        step_fn(data.get_batch(it, B, FACT_DROP))
+    torch.cuda.synchronize()
+    return time.perf_counter() - t0
+
+
+def make_step(name, m, use_graph):
+    params = [p for p in m.parameters() if p.requires_grad]
+    opt = torch.optim.Adam(params, lr=1e-4)
+    gstep = graphed.GraphedTrainStep(m) if use_graph else None
+
+    def step(batch):
+        opt.zero_grad(set_to_none=True)
+        if gstep is not None:
+            loss, _pred, _pd, h1, f1 = gstep.step(batch)
+            gstep.tp_list(h1, f1)
+        else:
+            loss, _pred, _pd, _tp = m(batch, training=True)
+            loss.backward()
+        loss.item()
+        torch.nn.utils.clip_grad_norm_(params, 1.0)
+        opt.step()
+    return step
+
+
+def order_kernel_ms(dev, B, E, launches):
+    """Device milliseconds per gr_split_fact_order launch over B questions of E stored facts at FACT_DROP."""
+    counts = np.full(B, E, dtype=np.int64)
+    off = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)])).to(dev)
+    ids = torch.arange(B, dtype=torch.int64, device=dev)
+    kept_h = loader.kept_counts(counts, FACT_DROP)
+    kept = torch.from_numpy(kept_h).to(dev)
+    seed = torch.randint(0, 2 ** 62, (1,), device=dev)
+    K, n_total = int(kept_h.sum()), int(counts.sum())
+    for _ in range(3):
+        ops.split_fact_order(off, ids, kept, seed, 0, n_total, K)
+    torch.cuda.synchronize()
+    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    s.record()
+    for _ in range(launches):
+        ops.split_fact_order(off, ids, kept, seed, 0, n_total, K)
+    e.record()
+    e.synchronize()
+    return s.elapsed_time(e) / launches
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--questions", type=int, default=640)
+    ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--shapes", default=",".join(SHAPES))
+    ap.add_argument("--launches", type=int, default=50)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("split_shuffle_probe needs a CUDA device")
+    info = gpu_info()
+    dev = torch.device("cuda")
+    results = []
+    splits = {}
+    for shape in a.shapes.split(","):
+        name, B, over, use_graph = SHAPES[shape]
+        graft = name == "GraftNet"
+        if graft not in splits:
+            L = SyntheticSplit(a.questions, graft=graft)
+            loader.install(L, weights="arrays", index_dtype=np.int32, shuffle=True)
+            if graft:
+                loader.install_graft(L)
+            splits[graft] = (L, loader.DeviceSplit(L, dev, weights="arrays", index_dtype=torch.int32, shuffle=True))
+        L, split = splits[graft]
+        args = S.model_args(name, use_cuda=True, **over)
+        torch.manual_seed(0)
+        m = {"ReaRev": G.ReaRev, "NSM": G.NSM, "GraftNet": G.GraftNet}[name](dict(args), NE, NR, NW).cuda().train()
+        step = make_step(name, m, use_graph)
+        modes = {"host": L, "device": split}
+        for data in modes.values():                   # warm-up: captures, caches
+            train_pass(data, step, B)
+        secs = {k: [] for k in modes}
+        for _ in range(a.runs):
+            for k, data in modes.items():
+                secs[k].append(train_pass(data, step, B))
+        qps = {k: a.questions / float(np.median(v)) for k, v in secs.items()}
+        res = dict(shape=shape, model=name, B=B, D=over["entity_dim"], graphed=use_graph, fact_drop=FACT_DROP,
+                   N=L.max_local_entity, E=6000, questions=a.questions, host_qps=round(qps["host"], 1),
+                   device_qps=round(qps["device"], 1), speedup=round(qps["device"] / qps["host"], 2),
+                   host_s=[round(x, 4) for x in secs["host"]], device_s=[round(x, 4) for x in secs["device"]],
+                   gpu=info)
+        results.append(res)
+        print(json.dumps(res), flush=True)
+        del step, m
+        torch.cuda.empty_cache()
+    for B, E in ((64, 6000), (1, 50000)):
+        res = dict(kernel="gr_split_fact_order", B=B, E=E, fact_drop=FACT_DROP,
+                   ms=round(order_kernel_ms(dev, B, E, a.launches), 4), launches=a.launches, gpu=info)
+        results.append(res)
+        print(json.dumps(res), flush=True)
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(results, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()

@@ -981,6 +981,8 @@ extern "C" int gr_fused_layer(const int32_t* rowptr_t, const int32_t* src_t, con
   }
   memset(&m_c, 0, sizeof(m_c)); memset(&m_c_hi, 0, sizeof(m_c_hi)); memset(&m_c_lo, 0, sizeof(m_c_lo));
   bool ok = true;
+  // TMA stores only: with N_out % 4 != 0 they write past column N_out to the end of its 16-byte unit (gr_linear_tc_planes
+  // takes direct stores there).  The model's C is a contiguous h32 [M, N_out], whose pitch refuses such a map.
   if (C) ok = make_out_tmap(&m_c, C, M, N_out, ldc, 4);
   const int64_t n16 = std::min<int64_t>((N_out + 15) / 16 * 16, ldc16);
   if (ok && C_hi) ok = make_out_tmap(&m_c_hi, C_hi, M, n16, ldc16, 2) && make_out_tmap(&m_c_lo, C_lo, M, n16, ldc16, 2);

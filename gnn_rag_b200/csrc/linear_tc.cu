@@ -394,7 +394,10 @@ int launch_tc(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int64_t lda1
   CUtensorMap m_c, m_c_hi, m_c_lo;
   memset(&m_c, 0, sizeof(m_c)); memset(&m_c_hi, 0, sizeof(m_c_hi)); memset(&m_c_lo, 0, sizeof(m_c_lo));
   bool ok = g_tc_tma_store != 0;
-  if (ok && p.C) ok = make_out_tmap(&m_c, p.C, p.M, p.N, p.ldc, 4);
+  // with N % 4 != 0 the TMA-store epilogue wrote past column N of an fp32 column view whose pitch is 16-byte aligned
+  // (observed on an H100: N = 50 wrote columns 50 and 51, the rest of the last 16-byte unit), so such an output takes
+  // the direct stores
+  if (ok && p.C) ok = p.N % 4 == 0 && make_out_tmap(&m_c, p.C, p.M, p.N, p.ldc, 4);
   if (ok && p.c_hi) ok = make_out_tmap(&m_c_hi, p.c_hi, p.M, p.n16, p.ldc16, 2) &&
                          make_out_tmap(&m_c_lo, p.c_lo, p.M, p.n16, p.ldc16, 2);
   p.tma_store = ok ? 1 : 0;

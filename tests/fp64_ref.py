@@ -112,6 +112,67 @@ def rearev_layer_scale(h, prior, tf, ti, ins, W, b, facts, w):
     return pre + b.abs() if b is not None else pre
 
 
+def nsm_layer(h, prior, table, ins, W, b, w_score, facts, w):
+    """One NSM step, forward direction, one instruction (nsm_gnn.py:54-77, 87-112): y = relu(W [h | nb] + b) with
+    nb[n] = sum_{e -> n} w_e^2 p[head_e] relu(P[r_e] * ins[b_e]), the score dot y . w_score (no score bias) and the
+    ``possible`` mask reason_kb multiplies into the answer mask.  ins [B, D]; returns (y, s, possible)."""
+    x = torch.cat([h, aggregate(table, ins.unsqueeze(1), prior, *facts, w, "fwd")], dim=1)
+    y = torch.relu(x @ W.t() + b)
+    return y, y @ w_score, possible(prior, facts, w, h.shape[0])[0]
+
+
+def nsm_layer_scale(h, prior, table, ins, W, b, facts, w):
+    """|W| [|h| | aggregate_abs] + |b|: the per-element scale of :func:`nsm_layer`'s pre-activation."""
+    x = torch.cat([h.abs(), aggregate_abs(table, ins.unsqueeze(1), prior, *facts, w, "fwd")], dim=1)
+    return x @ W.abs().t() + b.abs()
+
+
+def _graft_layer(h, d, q, fact_rel, W_tilde, E, e2f, f2e, lin, score_w, lam, fact_scale, act):
+    B, N = d.shape
+    Mf, D = W_tilde.shape[1], h.shape[1]
+    eb, ef, en = (_i(a) for a in e2f)
+    fb, fn, ff = (_i(a) for a in f2e)
+    eslot, enode = eb * Mf + ef, eb * N + en
+    fslot, fnode = fb * Mf + ff, fb * N + fn
+
+    def linear(x, name):
+        W, b = lin[name]
+        return x @ W.t() + b
+
+    head = linear(h, "kb_head")
+    e2f_emb = act(linear(fact_rel.reshape(B * Mf, D), "kb_self")
+                  + torch.zeros(B * Mf, D, dtype=h.dtype).index_add_(0, eslot, head[enode]))          # :118-121
+    norm = W_tilde.reshape(-1) * torch.zeros(B * Mf, dtype=h.dtype).index_add_(0, eslot, (d.reshape(-1) / E.reshape(-1))[enode])
+    e2f_emb = e2f_emb * norm.unsqueeze(1)                                                              # :122-124
+    tail = linear(e2f_emb, "kb_tail")                     # the bias enters once per (fact, tail) pair
+    f2e_emb = act(linear(h, "kb_self") + torch.zeros(B * N, D, dtype=h.dtype).index_add_(0, fnode, tail[fslot]))
+    nd = lam * torch.zeros(B * N, dtype=h.dtype).index_add_(0, fnode, norm[fslot]) + (1 - lam) * d.reshape(-1)
+    node_b = torch.arange(B * N) // N
+    x = torch.cat([h, linear(q, "q2e")[node_b], fact_scale * f2e_emb], dim=1)                          # :136-137
+    query = torch.zeros(B, D, dtype=h.dtype).index_add_(0, node_b, nd.unsqueeze(1) * linear(x, "e2q"))
+    y = act(linear(x, "e2e"))
+    return y, y @ score_w, nd.view(B, N), query
+
+
+def graft_layer(h, d, q, fact_rel, W_tilde, E, e2f, f2e, lin, score_w, lam, fact_scale):
+    """One GraftNet layer (graft_gnn.py:111-153) as per-fact gathers and ``index_add``.  h [B*N, D] node embeddings,
+    d [B, N] PageRank prior, q [B, D] query (query_node_emb at layer 0), fact_rel [B, M, D] = rel[kb_fact_rel],
+    W_tilde [B, M] fact attention, E [B, N] its clamped per-head sum; e2f = (b, fact slot, head) and
+    f2e = (b, tail, fact slot) index lists; lin: name -> (W, b) for q2e, e2q, e2e, kb_head, kb_tail, kb_self;
+    score_w [D].  Returns (h' = relu(e2e(x)), its score dot (no score bias), the next prior d' [B, N], query_emb
+    [B, D] = sum_n d'[n] e2q(x[n]))."""
+    return _graft_layer(h, d, q, fact_rel, W_tilde, E, e2f, f2e, lin, score_w, lam, fact_scale, torch.relu)
+
+
+def graft_layer_scale(h, d, q, fact_rel, W_tilde, E, e2f, f2e, lin, score_w, lam, fact_scale):
+    """:func:`graft_layer` on |inputs| and |weights| with the relus dropped: an elementwise envelope of every
+    pre-activation and output, the magnitude each rounding error along the layer is relative to.  An error of at
+    most e times its envelope in any intermediate stays within e times the envelope of each result."""
+    absl = {k: (W.abs(), b.abs()) for k, (W, b) in lin.items()}
+    return _graft_layer(h.abs(), d.abs(), q.abs(), fact_rel.abs(), W_tilde.abs(), E.abs(), e2f, f2e, absl,
+                        score_w.abs(), lam, abs(fact_scale), lambda t: t)
+
+
 def possible(prior, facts, w, Nt):
     """sum_{e -> n} w_e^2 p[head_e] > 1e-10 per tail row n (nsm_gnn.py:101-103), as float 0/1."""
     heads, _rels, tails = facts

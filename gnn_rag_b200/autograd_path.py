@@ -384,13 +384,17 @@ def _retrieved_sets_host(pred_dist, local_entity, seeds, num_entity, eps):
     """Candidate cut of f1_and_hits (base_model.py:216-234) with torch ops on the tensors' own device: used when the
     training tensors do not live on a GPU (the CUDA path uses the ranking kernel)."""
     B, N = pred_dist.shape
-    keep = (seeds == 0) & (local_entity != num_entity) & (pred_dist >= (1 - eps) / N)
-    p = torch.where(keep, pred_dist, torch.full_like(pred_dist, -1.0))
+    # p < (1 - eps) / N in float64, as the reference compares Python floats: against the fp32 tensor torch would round
+    # the bound to fp32 and keep a p just below it
+    ignore_prob = (1 - eps) / N
+    keep = (seeds == 0) & (local_entity != num_entity) & ~(pred_dist.double() < ignore_prob)
+    p = torch.where(keep, pred_dist, torch.full_like(pred_dist, float("-inf")))
     order = torch.sort(p, dim=1, descending=True, stable=True)[1]
-    ps = torch.gather(p, 1, order)
-    csum = torch.cumsum(torch.where(ps >= 0, ps, torch.zeros_like(ps)).double(), dim=1)
+    kept = torch.gather(keep, 1, order)
+    ps = torch.gather(pred_dist, 1, order)
+    csum = torch.cumsum(torch.where(kept, ps, torch.zeros_like(ps)).double(), dim=1)
     total = keep.sum(1)
-    crossed = (csum > eps) & (ps >= 0)
+    crossed = (csum > eps) & kept
     first = torch.where(crossed.any(1), crossed.float().argmax(1) + 1, total)
     count = torch.minimum(first, total)
     return order, count

@@ -5,9 +5,13 @@
 // (:25-50) sorts with python's STABLE sorted(..., reverse=True) (equal probabilities keep local-index
 // order) and keeps the prefix up to and including the item where the running float64 sum exceeds eps.
 // Here: one CTA per question, order-preserving compaction, a 64-bit key sort
-// (key = (~bits(p)) << 32 | local_index: ascending key == descending p, ascending index on ties), and the
+// (key = desc_key(p) << 32 | local_index: ascending key == descending p, ascending index on ties), and the
 // same sequential float64 running sum.  Integer/bit work end to end: bit-exact w.r.t. the reference
 // given the same probabilities.
+// Input domain: any fp32 p but NaN.  -0.0 ranks level with +0.0 and negative values rank below every other, as in
+// python's sorted; they survive the (1-eps)/N cut only when eps >= 1 (e.g. eps = 1 to retrieve every candidate), and
+// then the order is the whole output.  NaN is outside the contract: python's sorted has no order for NaN keys that
+// could be restated.
 #include <limits.h>
 #include <math.h>
 
@@ -41,6 +45,18 @@ __device__ void bitonic_sort_u64(unsigned long long* a, int n) {
       __syncthreads();
     }
   }
+}
+
+// 32-bit sort key of p: ascending key == descending p.  The standard order-preserving map of a float's bits (-0.0 made
+// +0.0 first; a negative value gets all bits flipped, any other the sign bit set), inverted for descending order.
+__device__ __forceinline__ unsigned desc_key(float p) {
+  unsigned u = __float_as_uint(p);
+  if (u == 0x80000000u) u = 0u;
+  return ~((u & 0x80000000u) ? ~u : (u | 0x80000000u));
+}
+
+__device__ __forceinline__ float key_value(unsigned k) {   // inverse of desc_key (-0.0 comes back as +0.0)
+  return __uint_as_float((k & 0x80000000u) ? k : ~(k | 0x80000000u));
 }
 
 __global__ void __launch_bounds__(kRankThreads)
@@ -84,8 +100,7 @@ rank_kernel(const float* __restrict__ dist, const int64_t* __restrict__ local_en
     __syncthreads();
     if (keep) {
       int pos = s_woff[wid] + __popc(bal & ((1u << lane) - 1));
-      unsigned hi = 0xFFFFFFFFu - __float_as_uint(pv);
-      gkeys[pos] = ((unsigned long long)hi << 32) | (unsigned)n;
+      gkeys[pos] = ((unsigned long long)desc_key(pv) << 32) | (unsigned)n;
     }
     __syncthreads();
   }
@@ -105,7 +120,8 @@ rank_kernel(const float* __restrict__ dist, const int64_t* __restrict__ local_en
   //    The reference adds sequentially in python floats (fp64).  Every surviving p_k is an fp32 value
   //    >= ignore_prob, so with exact_ok (host: 24 + ceil(log2(1/ignore_prob)) + 1 <= 53) every partial sum of
   //    any subset is exactly representable in fp64: the fp64 sum is ORDER-INDEPENDENT and a parallel scan is
-  //    bit-identical to the sequential loop.  Otherwise fall back to the sequential loop.
+  //    bit-identical to the sequential loop.  Otherwise fall back to the sequential loop.  exact_ok implies eps < 1,
+  //    so ignore_prob > 0 and no zero or negative p is ever kept on this path: the argument holds as stated.
   if (exact_ok && !s_bad) {
     __shared__ double s_wsum[kRankThreads / 32];
     __shared__ double s_carry;
@@ -115,7 +131,7 @@ rank_kernel(const float* __restrict__ dist, const int64_t* __restrict__ local_en
     for (int base = 0; base < total && s_first == total; base += kRankThreads) {
       const int i = base + tid;
       double v = 0.0;
-      if (i < total) v = (double)__uint_as_float(0xFFFFFFFFu - (unsigned)(keys[i] >> 32));
+      if (i < total) v = (double)key_value((unsigned)(keys[i] >> 32));
       double x = v;                                   // inclusive warp scan
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
@@ -140,9 +156,7 @@ rank_kernel(const float* __restrict__ dist, const int64_t* __restrict__ local_en
     double tp = 0.0;
     int cnt = 0;
     for (int i = 0; i < total; ++i) {
-      unsigned hi = (unsigned)(keys[i] >> 32);
-      float pv = __uint_as_float(0xFFFFFFFFu - hi);
-      tp += (double)pv;
+      tp += (double)key_value((unsigned)(keys[i] >> 32));
       cnt = i + 1;
       if (tp > eps) break;
     }

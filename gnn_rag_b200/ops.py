@@ -909,8 +909,20 @@ def kl_loss_pred(dist, teacher):
     return loss, pred
 
 
+def rank_candidates_ok(B, N):
+    """True when gr_rank_candidates admits B questions of N nodes: B > 0 and N > 0."""
+    return B > 0 and N > 0
+
+
 def rank_candidates(dist, local_entity, query_entities, pad_id, eps):
-    """-> (cand_idx int32[B,N], cand_count int32[B], cand_total int32[B]) on device."""
+    """-> (cand_idx int32[B,N], cand_count int32[B], cand_total int32[B]) on device.  dist, local_entity and
+    query_entities are all [B, N]: the kernel reads N entries of each per question."""
+    if dist.dim() != 2 or not rank_candidates_ok(*dist.shape):
+        raise RuntimeError("rank_candidates: dist must be [B, N] with B > 0 and N > 0, got %s" % list(dist.shape))
+    for name, t in (("local_entity", local_entity), ("query_entities", query_entities)):
+        if t.shape != dist.shape:
+            raise RuntimeError("rank_candidates: %s must be %s like dist, got %s"
+                               % (name, list(dist.shape), list(t.shape)))
     dist = _cuda(dist, torch.float32, "dist").contiguous()
     local_entity = _cuda(local_entity, torch.int64, "local_entity").contiguous()
     query_entities = _cuda(query_entities, torch.float32, "query_entities").contiguous()

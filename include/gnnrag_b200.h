@@ -638,11 +638,12 @@ int gr_seed_retrieve(const float* seed_info, const float* h, int64_t ldh, float*
 
 /* ------------------------------------------------------------------------------------------------
  * Candidate ranking = the retrieved answer-node set, Evaluator.evaluate + f1_and_hits
- * (gnn/evaluate.py:156, 188-209, 25-50).  Per question: drop seeds (query_entities == 1), pads
- * (local_entity == pad_id) and p < (1-eps)/N (compared in double); stable sort by p descending
- * (ties keep local-index order); keep the prefix up to and including the item at which the
- * sequential float64 running sum exceeds eps.
- *   cand_idx:  int32[B, N]  local indices in retrieval order (first cand_count[b] valid)
+ * (gnn/evaluate.py:156, 188-209, 25-50).  Per question: drop seeds (query_entities truncated to an
+ * integer == 1), pads (local_entity == pad_id) and p < (1-eps)/N (compared in double); stable sort by
+ * p descending (ties keep local-index order, -0.0 ties with +0.0, negative p last); keep the prefix up
+ * to and including the item at which the sequential float64 running sum exceeds eps.  Any eps; p may
+ * be any fp32 value but NaN.
+ *   cand_idx:  int32[B, N]  local indices in retrieval order (first cand_count[b] valid, 0 past cand_total[b])
  *   cand_count:int32[B]; cand_total:int32[B] = number of candidates before the eps cut.
  * Workspace: gr_rank_workspace_bytes(B, N).
  */

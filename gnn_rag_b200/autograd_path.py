@@ -659,6 +659,39 @@ def _graft_kernel_batch(model, batch, dev):
     return db
 
 
+def graft_live_stage(db):
+    """The inputs of :func:`graftnet_core` for a graft batch staged from fixed-capacity buffers
+    (graphed.GraphedGraftTrainStep): the (slot, head, tail) index vectors over the whole capacity of ``db.graft``,
+    with its first ``nfacts`` entries live.  ``GraftGraph``'s buffers are written only in their live front, so each
+    padding entry is replaced by a spare index before anything gathers through it: slot B*max_fact and node B*N, one
+    past the end.  The core gathers 0 there and drops what is summed there, so a padding entry contributes nothing
+    and shares no sum with a live one: torch's deterministic index_add groups the terms of one row, and how it adds
+    them up depends on how many there are."""
+    gg = db.graft
+    live = torch.arange(gg.cap, device=gg.nfacts.device) < gg.nfacts
+    Nt = db.B * db.N
+    facts = tuple(torch.where(live, a[: gg.cap].long(), spare)
+                  for a, spare in ((gg.slot_of, gg.B * gg.max_fact), (gg.heads, Nt), (gg.tails, Nt)))
+    return db.local_entity, db.q_input, db.seed_dist, db.answer_dist, gg.kb_fact_rel, db, facts
+
+
+def _stage_graft(model, batch):
+    """(local_entity, q_input, seed_dist, answer_dist, kb_fact_rel, db, None) of a ``get_batch`` tuple on the model's
+    device; ``db`` is the staged graft batch of the kernel path (None otherwise), whose malformed fact lists raise."""
+    (local_entity, _qe, _kb, _graft, q_input, kb_fact_rel, seed_dist, _tb, answer_dist) = batch[:9]
+    dev = model.word_embedding.weight.device
+    _require_cuda(dev)
+
+    def t(x, dtype):
+        x = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
+        return x.to(device=dev, dtype=dtype)
+    local_entity, q_input = t(local_entity, torch.int64), t(q_input, torch.int64)
+    seed_dist, answer_dist = t(seed_dist, torch.float32), t(answer_dist, torch.float32)
+    kb_fact_rel = t(kb_fact_rel, torch.int64)
+    db = _graft_kernel_batch(model, batch, dev) if _fact_kernels(dev, model.entity_dim) else None
+    return local_entity, q_input, seed_dist, answer_dist, kb_fact_rel, db, None
+
+
 def graftnet_forward(model, batch):
     """GraftNet forward with autograd (graftnet.py:135-183, graft_gnn.py:64-153) -> (loss, pred, pred_dist, [h1, f1]).
 
@@ -670,23 +703,34 @@ def graftnet_forward(model, batch):
     seed per layer from torch's CUDA generator).
     Otherwise (CPU under ``HOST_CHECK``, or ``USE_KERNELS`` off): per-fact messages are gathered and reduced with
     ``index_add_``; dropout sits where the reference applies it."""
-    (local_entity, query_entities, kb_adj_mat, graft, q_input, kb_fact_rel, seed_dist, _tb,
-     answer_dist) = batch[:9]
-    dev = model.word_embedding.weight.device
-    _require_cuda(dev)
+    staged = _stage_graft(model, batch)
+    loss, pred, pred_dist = graftnet_core(model, batch, staged)
+    local_entity, _qi, seed_dist, answer_dist = staged[:4]
+    h1, f1 = eval_metric(model, pred_dist.detach(), answer_dist, seed_dist, local_entity)
+    return loss, pred, pred_dist, [h1.tolist(), f1.tolist()]
 
-    def t(x, dtype):
-        x = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
-        return x.to(device=dev, dtype=dtype)
-    local_entity, q_input = t(local_entity, torch.int64), t(q_input, torch.int64)
-    seed_dist, answer_dist = t(seed_dist, torch.float32), t(answer_dist, torch.float32)
-    kb_fact_rel = t(kb_fact_rel, torch.int64)
+
+def graftnet_core(model, batch, staged):
+    """The differentiable part of :func:`graftnet_forward` -> (loss, pred, pred_dist).  ``staged``: the inputs of
+    :func:`_stage_graft` (the live graft fact count is then read on the host and the per-fact vectors have that length)
+    or of :func:`graft_live_stage` (capacity-length vectors whose padding entries hold the spare indices)."""
+    (_le, _qe, kb_adj_mat, graft) = batch[:4]
+    local_entity, q_input, seed_dist, answer_dist, kb_fact_rel, db, live_facts = staged
+    dev = local_entity.device
     B, N = local_entity.shape
     Nt, D = B * N, model.entity_dim
     layer = model.reasoning
     drop = layer.linear_drop_train
-    kernels = _fact_kernels(dev, D)
-    db = _graft_kernel_batch(model, batch, dev) if kernels else None
+    kernels = db is not None
+    spare = live_facts is not None
+
+    def pad(v):               # v and, past its end, the 0 the spare index gathers
+        return F.pad(v, (0, 1)) if spare else v
+
+    def node_sums(idx, v):    # per-node sums; the spare row's is dropped
+        if spare:
+            return torch.zeros(Nt + 1, device=dev).index_add(0, idx, v)[:Nt]
+        return torch.zeros(Nt, device=dev).index_add(0, idx, v)
     rel = model.get_rel_feature_train()
     if model.encode_type and kernels:
         h = _type_layer(model.type_layer, None, rel, Nt, db.graph)
@@ -699,8 +743,11 @@ def graftnet_forward(model, batch):
     qh, qnode, qmask = enc.query_hidden_emb, enc.query_node_emb, enc.query_mask_train
     if kernels:
         gg = db.graft
-        nf = int(gg.nfacts.item())
-        slot, head, tail = (t[:nf].long() for t in (gg.slot_of, gg.heads, gg.tails))
+        if spare:
+            slot, head, tail = live_facts
+        else:
+            nf = int(gg.nfacts.item())
+            slot, head, tail = (t[:nf].long() for t in (gg.slot_of, gg.heads, gg.tails))
         W = _GraftAttentionFn.apply(qh, rel, qmask.float(), gg)                  # [B, max_fact]
     else:
         slot, head, tail = _graft_facts(graft, kb_fact_rel, B, N, dev)
@@ -710,19 +757,20 @@ def graftnet_forward(model, batch):
         sim = torch.bmm(qh, fact_emb.transpose(1, 2)) / div
         sim = F.softmax(sim + (1 - qmask.unsqueeze(2)) * VERY_NEG_NUMBER, dim=1)  # [B, Q, max_fact]
         W = torch.sum(torch.bmm(sim.transpose(1, 2), qh) * fact_emb, dim=2) / div
-    W_tilde = torch.exp(W - torch.max(W, dim=1, keepdim=True)[0]).reshape(-1)[slot]
-    E = torch.clamp(torch.zeros(Nt, device=dev).index_add(0, head, W_tilde), min=1e-10)
+    W_tilde = pad(torch.exp(W - torch.max(W, dim=1, keepdim=True)[0]).reshape(-1))[slot]
+    E = torch.clamp(node_sums(head, W_tilde), min=1e-10)
     mask = (local_entity != model.num_entity).float()
-    fact_rel = kb_fact_rel.reshape(-1)[slot]
     d = seed_dist.reshape(-1)
     query = qnode                                                                 # [B, 1, D]
     dist_history, pagerank = [seed_dist], [seed_dist]
     lam = layer.pagerank_lambda
     if kernels:
-        indeg = torch.zeros(Nt, device=dev).index_add_(0, tail, torch.ones_like(W_tilde)).unsqueeze(1)
+        indeg = node_sums(tail, torch.ones_like(W_tilde)).unsqueeze(1)
+    else:
+        fact_rel = kb_fact_rel.reshape(-1)[slot]
     for i in range(model.num_layer):
         q2e = layer.lin("q2e_linear", i)(drop(query)).expand(B, N, D).reshape(Nt, D)
-        s = W_tilde * (d / E)[head]
+        s = W_tilde * pad(d / E)[head]
         if kernels:
             kt = layer.lin("kb_tail_linear", i)
             p = float(drop.p) if drop.training else 0.0
@@ -735,7 +783,7 @@ def graftnet_forward(model, batch):
             v = v * s.unsqueeze(1)
             f2e = F.relu(layer.lin("kb_self_linear", i)(h) + torch.zeros(Nt, D, device=dev).index_add(
                 0, tail, layer.lin("kb_tail_linear", i)(drop(v)).float()))
-        d = lam * torch.zeros(Nt, device=dev).index_add(0, tail, s) + (1 - lam) * d
+        d = lam * node_sums(tail, s) + (1 - lam) * d
         x = torch.cat([h, q2e, layer.fact_scale * f2e], dim=1)
         query = torch.bmm(d.view(B, 1, N), layer.lin("e2q_linear", i)(drop(x)).view(B, N, D))
         h = F.relu(layer.lin("e2e_linear", i)(drop(x)))
@@ -746,6 +794,5 @@ def graftnet_forward(model, batch):
     case_valid = (torch.sum(answer_dist, dim=1, keepdim=True) > 0).float()
     loss = model.calc_loss_label(logit, answer_dist, case_valid)
     pred = torch.max(pred_dist, dim=1)[1]
-    h1, f1 = eval_metric(model, pred_dist.detach(), answer_dist, seed_dist, local_entity)
     model.dist_history, model.pagerank_history = dist_history, pagerank
-    return loss, pred, pred_dist, [h1.tolist(), f1.tolist()]
+    return loss, pred, pred_dist

@@ -24,7 +24,8 @@ Models.  The input side is a per-model layout chosen from the model class: :clas
 step (one per CSR build / staging) travel back with the results and are checked on the host after the step.
 
 Training: :class:`GraphedTrainStep` captures ``model(batch, training=True)`` + ``loss.backward()`` + the train-time
-metrics (gr_train_metrics) of ReaRev and NSM over the same input side; see its docstring and DESIGN §4.11.
+metrics (gr_train_metrics) of ReaRev and NSM over the same input side, and :class:`GraphedGraftTrainStep` those of
+GraftNet over :class:`_GraftLayout` (the graft fact count stays on the device); see their docstrings and DESIGN §4.11.
 """
 import collections
 import contextlib
@@ -253,14 +254,18 @@ class _GraftLayout(_KbLayout):
                           .reshape(stage.kb_fact_rel.shape))
         return (le, qe, kb2, (e2f + (None,), f2e + (None,)), qi, kfr, sd, None, ad)
 
+    @staticmethod
+    def batch_of(st):
+        """The 9-tuple over the static buffers ``st``."""
+        return (st.local_entity, st.query_entities,
+                (st.heads, st.rels, st.tails, None, None, st.weight_list, st.weight_rel_list),
+                ((st.e2f_b, st.e2f_f, st.e2f_e, None), (st.f2e_b, st.f2e_e, st.f2e_f, None)),
+                st.q_input, st.kb_fact_rel, st.seed_dist, None, st.answer_dist)
+
     def run(self, st):
         m = self.step.model
-        tup = (st.local_entity, st.query_entities,
-               (st.heads, st.rels, st.tails, None, None, st.weight_list, st.weight_rel_list),
-               ((st.e2f_b, st.e2f_f, st.e2f_e, None), (st.f2e_b, st.f2e_e, st.f2e_f, None)),
-               st.q_input, st.kb_fact_rel, st.seed_dist, None, st.answer_dist)
-        db = batching.stage_graft_batch(tup, self.step.device, m.num_relation + 1, m.normalized_gnn, m.norm_rel,
-                                        nfacts=st.nfacts, graft_live=st.graft_live)
+        db = batching.stage_graft_batch(self.batch_of(st), self.step.device, m.num_relation + 1, m.normalized_gnn,
+                                        m.norm_rel, nfacts=st.nfacts, graft_live=st.graft_live)
         with torch.no_grad():        # the status words are read by GraphedStep after the step, not inside the capture
             loss, pred, pred_dist, _ = m._forward_infer(db, check_status=False)
         return db, loss, pred, pred_dist
@@ -511,16 +516,17 @@ class GraphedStep:
 
 class TrainStepOutput(tuple):
     """``(loss, pred, pred_dist, h1, f1)`` of one :meth:`GraphedTrainStep.step`, all device tensors (views of the
-    graph's static outputs, valid until the next step).  ``status`` is the device int32[1] status word of the batch's
-    CSR build; :meth:`check` reads it back and raises when the fact list held ids outside the batch."""
+    graph's static outputs, valid until the next step).  ``status`` holds the device int32 status words of the batch's
+    staging (ReaRev, NSM: the CSR build's; GraftNet: also the graft staging's); :meth:`check` reads them back and
+    raises, with the messages of the input layout that produced them, when a fact list was malformed."""
 
-    def __new__(cls, loss, pred, pred_dist, h1, f1, status):
+    def __new__(cls, loss, pred, pred_dist, h1, f1, status, raise_for=_KbLayout.raise_for):
         out = super().__new__(cls, (loss, pred, pred_dist, h1, f1))
-        out.status = status
+        out.status, out._raise_for = status, raise_for
         return out
 
     def check(self):
-        _KbLayout.raise_for(self.status.tolist())
+        self._raise_for(self.status.tolist())
 
 
 def _release_autograd_history(model):
@@ -569,18 +575,21 @@ class GraphedTrainStep:
     def __init__(self, model, max_graphs=8):
         from .models import GraftNet, ReaRev
         if isinstance(model, GraftNet):
-            raise ValueError("GraphedTrainStep covers ReaRev and NSM; GraftNet's training forward reads its live graft "
-                             "fact count on the host and is not captured")
+            raise ValueError("GraphedTrainStep covers ReaRev and NSM; GraftNet trains in GraphedGraftTrainStep")
+        self._setup(model, max_graphs, _KbLayout)
+        self._rearev = isinstance(model, ReaRev)
+        self._core = autograd_path.rearev_core if self._rearev else autograd_path.nsm_core
+
+    def _setup(self, model, max_graphs, layout):
         self.model = model
         self._params = list(model.parameters())
         if not self._params or self._params[0].device.type != "cuda":
-            raise ValueError("GraphedTrainStep needs a model on a CUDA device (model.cuda()); there is no CPU path")
+            raise ValueError("%s needs a model on a CUDA device (model.cuda()); there is no CPU path"
+                             % type(self).__name__)
         self.device = self._params[0].device
         self.max_graphs = max_graphs
-        self._rearev = isinstance(model, ReaRev)
-        self._core = autograd_path.rearev_core if self._rearev else autograd_path.nsm_core
         self._cache = collections.OrderedDict()
-        self._layout = _KbLayout(self)
+        self._layout = layout(self)
 
     @staticmethod
     def tp_list(h1, f1):
@@ -622,22 +631,28 @@ class GraphedTrainStep:
         return None
 
     # -- capture ---------------------------------------------------------------------------------------------------
-    def _run(self, st, ac):
-        """forward + backward + metrics over the static buffers ``st`` -> (loss, pred, pred_dist, h1, f1, status)."""
+    def _forward(self, st):
+        """The model's training forward over the static buffers ``st`` -> (db, loss, pred, pred_dist)."""
         m = self.model
         tup = (st.local_entity, st.query_entities,
                (st.heads, st.rels, st.tails, None, None, st.weight_list, st.weight_rel_list),
                st.q_input, st.seed_dist, None, st.answer_dist)
+        db = batching.stage_batch(tup, self.device, m.num_relation + 1, m.normalized_gnn, m.norm_rel,
+                                  nfacts=st.nfacts)
+        live = autograd_path.LiveBatch(db, st.heads, st.tails, st.weight_list, st.nfacts)
+        loss, pred, pred_dist = self._core(m, live, autograd_path._stage(m, live))
+        return db, loss, pred, pred_dist
+
+    def _run(self, st, ac):
+        """forward + backward + metrics over the static buffers ``st`` -> (loss, pred, pred_dist, h1, f1, status)."""
+        m = self.model
         # Autocast casts every weight once per forward and reuses the copy (its cast cache), so the gradients of a
         # weight's uses are summed in the low-precision dtype, as in the eager step.  The cache is emptied before the
         # forward (an entry made outside the capture would freeze that weight into the graph) and after it (the
         # graph's copies must not serve eager code).
         with torch.autocast("cuda", dtype=ac) if ac is not None else contextlib.nullcontext():
             torch.clear_autocast_cache()
-            db = batching.stage_batch(tup, self.device, m.num_relation + 1, m.normalized_gnn, m.norm_rel,
-                                      nfacts=st.nfacts)
-            live = autograd_path.LiveBatch(db, st.heads, st.tails, st.weight_list, st.nfacts)
-            loss, pred, pred_dist = self._core(m, live, autograd_path._stage(m, live))
+            db, loss, pred, pred_dist = self._forward(st)
             torch.clear_autocast_cache()
         loss.backward()
         pred_dist = pred_dist.detach()
@@ -645,7 +660,8 @@ class GraphedTrainStep:
                                                       m.num_entity, m.eps)
         h1, f1 = ops.train_metrics(pred_dist, db.answer_dist, db.seed_dist, db.local_entity, cand_idx, cand_count,
                                    m.num_entity)
-        return loss.detach(), pred, pred_dist, h1, f1, db.graph.status
+        words = self._layout.status_words(db)
+        return loss.detach(), pred, pred_dist, h1, f1, words[0] if len(words) == 1 else torch.cat(words)
 
     def _entry(self, batch):
         key = self.key(batch)
@@ -661,7 +677,7 @@ class GraphedTrainStep:
             torch.cuda.synchronize()
             del old
         ac = _autocast_dtype()
-        st = self._layout.static_inputs(key[:5])
+        st = self._layout.static_inputs(key)
         self._layout.fill(st, batch)
         params = [p for p in self._params if p.requires_grad]
         torch.cuda.synchronize()
@@ -695,4 +711,56 @@ class GraphedTrainStep:
         ent.g.replay()
         for p, g in zip(ent.params, ent.grads):
             p.grad = g
-        return TrainStepOutput(*ent.outs)
+        return TrainStepOutput(*ent.outs, raise_for=self._layout.raise_for)
+
+
+class GraphedGraftTrainStep(GraphedTrainStep):
+    """:class:`GraphedTrainStep` for GraftNet: ``model(batch, training=True)`` + ``loss.backward()`` + the train-time
+    hit@1 / F1 as one CUDA graph per batch shape, with the same :meth:`step`, :meth:`tp_list`, LRU and gradients.
+
+    :meth:`step` takes the 9/10-tuple of ``GraftSingleDataLoader.get_batch`` (host numpy, pinned tensors or a
+    ``loader.DeviceSplit`` batch) and copies it into the static buffers of :class:`_GraftLayout`: kb facts at a
+    ``fact_capacity`` bucket with their live count in ``nfacts``, both graft lists at their own bucket with their live
+    counts in ``graft_live``, ``kb_fact_rel``.  In the graph gr_graft_stage stages the live graft facts and writes
+    their count on the device, and the forward runs ``autograd_path.graftnet_core`` over capacity-length per-fact
+    vectors (``autograd_path.graft_live_stage``), so nothing reads a count on the host.  The three status words (kb CSR,
+    graft staging, graft CSR) come back in the output; ``out.check()`` raises ``GraftGraph``'s messages.
+
+    The capture key is :class:`GraphedTrainStep`'s plus the graft capacity, ``max_fact``, and the two Python scalars
+    the forward bakes into the graph: ``pagerank_lambda`` and ``fact_scale``.  A CPU model, ``USE_KERNELS`` off or an
+    ``entity_dim`` the GraftNet training kernels do not admit (``ops.fact_train_ok``) raises ``ValueError``, as does a
+    batch that is not a graft tuple."""
+
+    def __init__(self, model, max_graphs=8):
+        from .models import GraftNet
+        if not isinstance(model, GraftNet):
+            raise ValueError("GraphedGraftTrainStep covers GraftNet; ReaRev and NSM train in GraphedTrainStep")
+        self._setup(model, max_graphs, _GraftLayout)
+
+    def key(self, batch):
+        if len(batch) not in (9, 10):
+            raise ValueError("GraphedGraftTrainStep takes the 9/10-tuple of GraftSingleDataLoader.get_batch, not a "
+                             "%d-tuple" % len(batch))
+        layer = self.model.reasoning
+        return super().key(batch) + (float(layer.pagerank_lambda), float(layer.fact_scale))
+
+    def refusal(self, Q):
+        """Why the eager forward would leave the kernels (a message), or None.  GraftNet's forward takes the kernel
+        path or the per-fact torch ops as a whole (``autograd_path._fact_kernels``); its question encoder has no
+        kernel path in training, so Q does not matter."""
+        D = self.model.entity_dim
+        if not autograd_path.USE_KERNELS:
+            return "autograd_path.USE_KERNELS is off: the training forward would run its torch restatement"
+        if not autograd_path._fact_kernels(self.device, D):
+            return ("_fact_kernels is false: entity_dim %d is outside the GraftNet training kernels (%s)"
+                    % (D, ops.fact_train_ok.__doc__.split(": ", 1)[1].rstrip(".")))
+        return None
+
+    def _forward(self, st):
+        m = self.model
+        tup = _GraftLayout.batch_of(st)
+        # the training forward stages without normalized_gnn (GraftNet does not read the kb weights)
+        db = batching.stage_graft_batch(tup, self.device, m.num_relation + 1, False, m.norm_rel, nfacts=st.nfacts,
+                                        graft_live=st.graft_live)
+        loss, pred, pred_dist = autograd_path.graftnet_core(m, tup, autograd_path.graft_live_stage(db))
+        return db, loss, pred, pred_dist

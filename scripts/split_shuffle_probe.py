@@ -10,8 +10,8 @@ N = 2000 nodes, E = 6000 stored facts per question, self-loops on): per batch ``
   device  DeviceSplit(loader, weights="arrays", shuffle=True).get_batch
 
 Shapes: ReaRev and NSM at the reference's training shape (B 8, entity_dim 50) through graphed.GraphedTrainStep;
-GraftNet (B 8, entity_dim 50) eager, as GraphedTrainStep refuses it; and cfg2 (ReaRev, B 64, entity_dim 200) through
-GraphedTrainStep.  A pass runs the whole split; the questions/s of a mode is the median over ``--runs`` passes, host
+GraftNet (B 8, entity_dim 50) eager (graftnet_d50) and through graphed.GraphedGraftTrainStep (graftnet_d50_graphed);
+and cfg2 (ReaRev, B 64, entity_dim 200) through GraphedTrainStep.  A pass runs the whole split; the questions/s of a mode is the median over ``--runs`` passes, host
 and device alternating, after one warm-up pass of each (graph captures).  Then gr_split_fact_order alone, between CUDA
 events over ``--launches`` launches: B = 64 questions of 6 000 facts, and one question of 50 000 facts.  The GPU's
 name and power limit are read in the same run.  One JSON line per measurement.
@@ -38,6 +38,7 @@ SHAPES = {   # name -> model, batch size, model arguments, graphed
     "rearev_d50": ("ReaRev", 8, dict(entity_dim=50, num_ins=3, num_iter=2, num_gnn=3), True),
     "nsm_d50": ("NSM", 8, dict(entity_dim=50), True),
     "graftnet_d50": ("GraftNet", 8, dict(entity_dim=50), False),
+    "graftnet_d50_graphed": ("GraftNet", 8, dict(entity_dim=50), True),
     "cfg2": ("ReaRev", 64, dict(entity_dim=200, num_ins=2, num_iter=3, num_gnn=3), True),
 }
 FACT_DROP = 0.1
@@ -57,7 +58,8 @@ def train_pass(data, step_fn, B):
 def make_step(name, m, use_graph):
     params = [p for p in m.parameters() if p.requires_grad]
     opt = torch.optim.Adam(params, lr=1e-4)
-    gstep = graphed.GraphedTrainStep(m) if use_graph else None
+    cls = graphed.GraphedGraftTrainStep if name == "GraftNet" else graphed.GraphedTrainStep
+    gstep = cls(m) if use_graph else None
 
     def step(batch):
         opt.zero_grad(set_to_none=True)

@@ -1,10 +1,13 @@
-"""Milliseconds per training step, eager against graphed (graphed.GraphedTrainStep), at the reference's training shape.
+"""Milliseconds per training step, eager against graphed (graphed.GraphedTrainStep, GraphedGraftTrainStep), at the
+reference's training shape.
 
     python scripts/train_graph_probe.py [--steps 50] [--warmup 10] [--runs 5] [--out train_graph_probe.json]
 
-Shapes: d50 = B 8, entity_dim 50, num_ins 3, num_iter 2, num_gnn 3, lstm (gnn/scripts/rearev_cwq.sh); cfg2 = B 64,
-entity_dim 200, num_ins 2, num_iter 3, num_gnn 3.  Both on WebQSP-shape synthetic subgraphs (N 2000, 6000 facts per
-question), dropout 0.2 / 0.3 as in the reference's defaults.  One step = forward + backward + the train-time hit@1 / F1
+Shapes: d50 = ReaRev B 8, entity_dim 50, num_ins 3, num_iter 2, num_gnn 3, lstm (gnn/scripts/rearev_cwq.sh); cfg2 =
+ReaRev B 64, entity_dim 200, num_ins 2, num_iter 3, num_gnn 3; graftnet_d50 = GraftNet B 8, entity_dim 50, num_layer 3,
+lstm (the reference's GraftNet training shape); graftnet_cfg2 = GraftNet B 64, entity_dim 200, num_layer 3.  All on
+WebQSP-shape synthetic subgraphs (N 2000, 6000 facts per question; GraftNet: the same facts as graft tuples), dropout
+0.2 / 0.3 as in the reference's defaults.  One step = forward + backward + the train-time hit@1 / F1
 as host lists (the tp_list train_epoch keeps), with or without the caller's clip_grad_norm_ + Adam.step().  A run
 times ``--steps`` steps between two CUDA events after ``--warmup`` steps; each mode runs ``--runs`` times, alternating
 eager and graphed, and the median and the spread are reported.  The GPU's name, SM clock and power limit are read in
@@ -26,6 +29,8 @@ from gnn_rag_b200 import graphed, synthetic as S
 SHAPES = {
     "d50": dict(B=8, D=50, I=3, T=2, K=3),
     "cfg2": dict(B=64, D=200, I=2, T=3, K=3),
+    "graftnet_d50": dict(model="GraftNet", B=8, D=50, L=3),
+    "graftnet_cfg2": dict(model="GraftNet", B=64, D=200, L=3),
 }
 
 
@@ -40,12 +45,19 @@ def gpu_info():
 
 
 def build(c):
-    args = S.model_args("ReaRev", entity_dim=c["D"], num_ins=c["I"], num_iter=c["T"], num_gnn=c["K"], use_cuda=True)
+    """-> (model, two batches, the graphed step)."""
     torch.manual_seed(0)
-    m = G.ReaRev(dict(args), S.WEBQSP_NUM_ENTITY, S.WEBQSP_NUM_RELATION, S.WEBQSP_NUM_WORD).cuda().train()
+    sizes = (S.WEBQSP_NUM_ENTITY, S.WEBQSP_NUM_RELATION, S.WEBQSP_NUM_WORD)
+    if c.get("model") == "GraftNet":
+        args = S.model_args("GraftNet", entity_dim=c["D"], num_layer=c["L"], use_cuda=True)
+        m = G.GraftNet(dict(args), *sizes).cuda().train()
+        batches = [S.make_graft_batch(s, B=c["B"], N=2000, E=6000) for s in (1, 2)]
+        return m, batches, graphed.GraphedGraftTrainStep(m)
+    args = S.model_args("ReaRev", entity_dim=c["D"], num_ins=c["I"], num_iter=c["T"], num_gnn=c["K"], use_cuda=True)
+    m = G.ReaRev(dict(args), *sizes).cuda().train()
     batches = [S.make_batch(s, B=c["B"], N=2000, E=6000, with_weights=False)[:7] for s in (1, 2)]
     # the graphed step's buckets: both batches in one capacity bucket, so one graph serves the timed loop
-    return m, batches
+    return m, batches, graphed.GraphedTrainStep(m)
 
 
 def time_mode(step_fn, batches, steps, warmup):
@@ -66,7 +78,7 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--runs", type=int, default=5)
-    ap.add_argument("--shapes", default="d50,cfg2")
+    ap.add_argument("--shapes", default=",".join(SHAPES))
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -74,10 +86,9 @@ def main():
     res = dict(gpu=gpu_info(), steps=a.steps, warmup=a.warmup, runs=a.runs, results={})
     for name in a.shapes.split(","):
         c = SHAPES[name]
-        m, batches = build(c)
+        m, batches, gstep = build(c)
         params = [p for p in m.parameters() if p.requires_grad]
         opt = torch.optim.Adam(params, lr=1e-4)
-        gstep = graphed.GraphedTrainStep(m)
 
         def eager(b):
             loss, _pred, _pd, tp = m(b, training=True)

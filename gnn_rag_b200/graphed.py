@@ -25,15 +25,18 @@ step (one per CSR build / staging) travel back with the results and are checked 
 
 Training: :class:`GraphedTrainStep` captures ``model(batch, training=True)`` + ``loss.backward()`` + the train-time
 metrics (gr_train_metrics) of ReaRev and NSM over the same input side, and :class:`GraphedGraftTrainStep` those of
-GraftNet over :class:`_GraftLayout` (the graft fact count stays on the device); see their docstrings and DESIGN §4.11.
+GraftNet over :class:`_GraftLayout` (the graft fact count stays on the device).  Given a ``torch.optim.Adam``, both
+also capture the gradient clipping and the optimizer step (:class:`optim.ClipAdam`); see their docstrings and DESIGN
+§4.11.
 """
 import collections
 import contextlib
+import gc
 
 import numpy as np
 import torch
 
-from . import autograd_path, batching, ops
+from . import autograd_path, batching, ops, optim
 from .modules import live_plane_buffers
 
 
@@ -518,11 +521,12 @@ class TrainStepOutput(tuple):
     """``(loss, pred, pred_dist, h1, f1)`` of one :meth:`GraphedTrainStep.step`, all device tensors (views of the
     graph's static outputs, valid until the next step).  ``status`` holds the device int32 status words of the batch's
     staging (ReaRev, NSM: the CSR build's; GraftNet: also the graft staging's); :meth:`check` reads them back and
-    raises, with the messages of the input layout that produced them, when a fact list was malformed."""
+    raises, with the messages of the input layout that produced them, when a fact list was malformed.  ``grad_norm``:
+    the total gradient norm before clipping (device fp32 scalar) of a step with ``max_norm``, else None."""
 
-    def __new__(cls, loss, pred, pred_dist, h1, f1, status, raise_for=_KbLayout.raise_for):
+    def __new__(cls, loss, pred, pred_dist, h1, f1, status, raise_for=_KbLayout.raise_for, grad_norm=None):
         out = super().__new__(cls, (loss, pred, pred_dist, h1, f1))
-        out.status, out._raise_for = status, raise_for
+        out.status, out._raise_for, out.grad_norm = status, raise_for, grad_norm
         return out
 
     def check(self):
@@ -555,14 +559,26 @@ class GraphedTrainStep:
     at the front of a ``fact_capacity`` bucket, the live count in ``nfacts``), replays the graph and re-attaches the
     graph's gradient tensors to ``p.grad`` of every trainable parameter.  After a step ``p.grad`` holds this batch's
     gradient, overwritten rather than accumulated (as ``zero_grad(); loss.backward()``), so
-    ``optimizer.zero_grad(set_to_none=True)`` between steps is fine.  Clipping and ``optimizer.step()`` stay with
-    the caller; they update the parameters in place, and the graph reads every weight from the parameter's storage
-    when it replays.
+    ``optimizer.zero_grad(set_to_none=True)`` between steps is fine.  Without ``optimizer``, clipping and
+    ``optimizer.step()`` stay with the caller; they update the parameters in place, and the graph reads every weight
+    from the parameter's storage when it replays.
+
+    With a ``torch.optim.Adam`` as ``optimizer``, the graph goes on after the metrics with
+    ``clip_grad_norm_(params, max_norm)`` (when ``max_norm`` is given) and ``optimizer.step()`` as two kernels
+    (:class:`optim.ClipAdam`), bit-equal to torch's foreach Adam given the norm they compute, which the output returns
+    as ``grad_norm``.  ``params`` are the parameters the captured backward gives a gradient; the optimizer updates
+    those it holds, as ``Adam.step()`` skips ``grad is None``.  The optimizer state stays torch's (missing state is
+    created before the capture, the CPU ``step`` tensors advance on the host), so ``state_dict()``, checkpoints and
+    eager steps in between keep working, and ``p.grad`` holds the clipped gradient afterwards.  ``lr`` and the other
+    hyperparameters are read on every step, so a scheduler needs no new capture.  :func:`optim.check_optimizer`
+    lists what is refused (``ValueError``).
 
     A graph is keyed on the batch shape (B, N, fact capacity, Q, index dtype) and on the state the forward reads when
     it is captured: ``model.training``, every dropout probability in effect, the autocast dtype, torch's
     deterministic-algorithms flag, the cuDNN / TF32 switches, which parameters are trainable and the ``data_ptr`` of
-    every parameter (``p.data = ...`` recaptures; in-place updates do not).  Captured graphs are kept in an LRU of
+    every parameter (``p.data = ...`` recaptures; in-place updates do not); with an optimizer also ``max_norm``,
+    whether any group has a weight decay and the ``data_ptr`` of every optimizer state tensor (so
+    ``optimizer.load_state_dict`` recaptures).  Captured graphs are kept in an LRU of
     ``max_graphs`` entries.  Padding slots past ``nfacts`` contribute nothing: the kernels read live facts through
     the CSR and the torch-side per-fact work masks them (autograd_path.LiveBatch).  Dropout masks come from torch's
     CUDA generator, which a graph advances on every replay, so each replay draws fresh masks.  After the first
@@ -572,20 +588,24 @@ class GraphedTrainStep:
     ``encode_type``, TypeLayer kernels); otherwise, and for GraftNet or a CPU model, the constructor or the step raises
     ``ValueError``."""
 
-    def __init__(self, model, max_graphs=8):
+    optimizer = max_norm = None          # without an optimizer the graph ends at the gradients
+
+    def __init__(self, model, max_graphs=8, optimizer=None, max_norm=None):
         from .models import GraftNet, ReaRev
         if isinstance(model, GraftNet):
             raise ValueError("GraphedTrainStep covers ReaRev and NSM; GraftNet trains in GraphedGraftTrainStep")
-        self._setup(model, max_graphs, _KbLayout)
+        self._setup(model, max_graphs, _KbLayout, optimizer, max_norm)
         self._rearev = isinstance(model, ReaRev)
         self._core = autograd_path.rearev_core if self._rearev else autograd_path.nsm_core
 
-    def _setup(self, model, max_graphs, layout):
+    def _setup(self, model, max_graphs, layout, optimizer, max_norm):
         self.model = model
         self._params = list(model.parameters())
         if not self._params or self._params[0].device.type != "cuda":
             raise ValueError("%s needs a model on a CUDA device (model.cuda()); there is no CPU path"
                              % type(self).__name__)
+        optim.check_optimizer(optimizer, self._params, max_norm)
+        self.optimizer, self.max_norm = optimizer, None if max_norm is None else float(max_norm)
         self.device = self._params[0].device
         self.max_graphs = max_graphs
         self._cache = collections.OrderedDict()
@@ -607,9 +627,12 @@ class GraphedTrainStep:
                     torch.backends.cuda.matmul.allow_tf32)
         rel_text = tuple(t.data_ptr() for t in (getattr(m, "rel_features", None), getattr(m, "rel_features_inv", None))
                          if isinstance(t, torch.Tensor))
+        opt = self.optimizer
+        fused = () if opt is None else (self.max_norm, any(g["weight_decay"] != 0 for g in opt.param_groups),
+                                        optim.state_key(opt))
         return self._layout.key(batch) + (
             m.training, drops, _autocast_dtype(), torch.are_deterministic_algorithms_enabled(), backends,
-            tuple(p.requires_grad for p in self._params), tuple(p.data_ptr() for p in self._params), rel_text)
+            tuple(p.requires_grad for p in self._params), tuple(p.data_ptr() for p in self._params), rel_text) + fused
 
     def refusal(self, Q):
         """Why the eager forward would leave the kernels for questions of Q tokens (a message), or None."""
@@ -691,32 +714,56 @@ class GraphedTrainStep:
                 self._run(st, ac)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
+        fused = None
+        if self.optimizer is not None:
+            # the warm-up's gradients show which parameters the backward reaches; their missing Adam state is made
+            # now, so the key the next step computes (it holds the state's data_ptrs) is the one stored below
+            fused = optim.ClipAdam(self.optimizer, params, [p.grad for p in params], self.max_norm)
+            key = self.key(batch)
         _release_autograd_history(self.model)
         for p in params:                         # the captured backward allocates (not accumulates) every gradient
             p.grad = None
         g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            outs = self._run(st, ac)
+        # no cyclic garbage collection during the capture: collecting a dropped step's graph there (its exec graph
+        # and private pool are released) is a CUDA call that invalidates the capture
+        gc_on = gc.isenabled()
+        gc.disable()
+        try:
+            with torch.cuda.graph(g):
+                outs = self._run(st, ac)
+                if fused is not None:
+                    fused.launch()
+        finally:
+            if gc_on:
+                gc.enable()
         ent = _Captured()
         ent.st, ent.g, ent.outs = st, g, outs
         ent.params, ent.grads = params, [p.grad for p in params]
+        ent.fused = fused
+        if fused is not None:                    # the kernels read and clip the captured backward's gradients
+            fused.bind([p.grad for p in fused.params])
         self._cache[key] = ent
         return ent
 
     def step(self, batch):
         """One training step on ``batch`` (the 7-tuple of ``get_batch``, host numpy or pinned) ->
-        :class:`TrainStepOutput` ``(loss, pred, pred_dist, h1, f1)``; ``p.grad`` holds this batch's gradients."""
+        :class:`TrainStepOutput` ``(loss, pred, pred_dist, h1, f1)``; ``p.grad`` holds this batch's gradients (clipped,
+        and the parameters updated, with an optimizer)."""
         ent = self._entry(batch)
         self._layout.fill(ent.st, batch)
+        if ent.fused is not None:
+            ent.fused.prepare()
         ent.g.replay()
         for p, g in zip(ent.params, ent.grads):
             p.grad = g
-        return TrainStepOutput(*ent.outs, raise_for=self._layout.raise_for)
+        return TrainStepOutput(*ent.outs, raise_for=self._layout.raise_for,
+                               grad_norm=None if ent.fused is None else ent.fused.grad_norm)
 
 
 class GraphedGraftTrainStep(GraphedTrainStep):
     """:class:`GraphedTrainStep` for GraftNet: ``model(batch, training=True)`` + ``loss.backward()`` + the train-time
-    hit@1 / F1 as one CUDA graph per batch shape, with the same :meth:`step`, :meth:`tp_list`, LRU and gradients.
+    hit@1 / F1 as one CUDA graph per batch shape, with the same :meth:`step`, :meth:`tp_list`, LRU, gradients and
+    optional clip + Adam step (``optimizer``, ``max_norm``).
 
     :meth:`step` takes the 9/10-tuple of ``GraftSingleDataLoader.get_batch`` (host numpy, pinned tensors or a
     ``loader.DeviceSplit`` batch) and copies it into the static buffers of :class:`_GraftLayout`: kb facts at a
@@ -731,11 +778,11 @@ class GraphedGraftTrainStep(GraphedTrainStep):
     ``entity_dim`` the GraftNet training kernels do not admit (``ops.fact_train_ok``) raises ``ValueError``, as does a
     batch that is not a graft tuple."""
 
-    def __init__(self, model, max_graphs=8):
+    def __init__(self, model, max_graphs=8, optimizer=None, max_norm=None):
         from .models import GraftNet
         if not isinstance(model, GraftNet):
             raise ValueError("GraphedGraftTrainStep covers GraftNet; ReaRev and NSM train in GraphedTrainStep")
-        self._setup(model, max_graphs, _GraftLayout)
+        self._setup(model, max_graphs, _GraftLayout, optimizer, max_norm)
 
     def key(self, batch):
         if len(batch) not in (9, 10):

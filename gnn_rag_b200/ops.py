@@ -967,6 +967,37 @@ def train_metrics(pred_dist, answer_dist, seed_dist, local_entity, cand_idx, can
     return h1, f1
 
 
+ADAM_ALIGNED16 = 1          # GR_ADAM_ALIGNED16: a tensor-table row whose pointers are all 16-byte aligned
+ADAM_WEIGHT_DECAY = 1       # GR_ADAM_WEIGHT_DECAY: some row of the table has weight_decay != 0
+
+
+@functools.lru_cache(maxsize=None)
+def adam_chunk_elems():
+    """Elements per chunk of :func:`clip_adam` (gr_adam_chunk_elems): a tensor of n elements takes ceil(n / E)."""
+    return int(_L().gr_adam_chunk_elems())
+
+
+def clip_adam(table, scalars, chunks, slots=None, max_norm=0.0, grad_norm=None, weight_decay=False):
+    """clip_grad_norm_ + Adam.step() over a tensor list (gr_grad_sumsq, then gr_clip_adam; csrc/optim.cu).
+
+    ``table`` int64 [T, 6], ``scalars`` fp32 [T, 8] and ``chunks`` int32 [C, 2] are device tensors laid out as the
+    header says; ``slots`` float64 [C] turns clipping to ``max_norm`` on, and ``grad_norm`` (fp32, one element) then
+    receives the total norm.  ``weight_decay``: some row has weight_decay != 0.  Nothing here waits on the host, so a
+    CUDA graph can capture the two launches."""
+    table = _cuda(table, torch.int64, "table")
+    scalars = _cuda(scalars, torch.float32, "scalars")
+    chunks = _cuda(chunks, torch.int32, "chunks")
+    slots = _cuda(slots, torch.float64, "slots")
+    grad_norm = _cuda(grad_norm, torch.float32, "grad_norm")
+    T, C = table.shape[0], chunks.shape[0]
+    assert table.shape == (T, 6) and scalars.shape == (T, 8) and chunks.shape == (C, 2)
+    if slots is not None:
+        assert slots.numel() >= C
+        _launch("gr_grad_sumsq", _p(table), _p(chunks), C, _p(slots), op="optimizer")
+    _launch("gr_clip_adam", _p(table), _p(scalars), _p(chunks), C, _p(slots), float(max_norm), _p(grad_norm),
+            ADAM_WEIGHT_DECAY if weight_decay else 0, op="optimizer")
+
+
 _INT32_MAX = 2 ** 31 - 1
 _INDEX_BYTES = {torch.int32: 4, torch.int64: 8}
 

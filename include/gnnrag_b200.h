@@ -668,6 +668,36 @@ int gr_train_metrics(const float* pred_dist, const float* answer_dist, const flo
                      float* h1, float* f1, int B, int N, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Gradient clipping + Adam over fp32 tensor lists (csrc/optim.cu): torch.nn.utils.clip_grad_norm_(params, max_norm)
+ * followed by torch.optim.Adam.step() (gnn/train_model.py:91-92, 221-230), bit for bit as torch's default CUDA path,
+ * torch.optim.adam._multi_tensor_adam (foreach, not capturable, no amsgrad / maximize / decoupled weight decay).
+ * Deterministic, no atomics.
+ *
+ * table: int64 [T][6], one row per tensor: {param, grad, exp_avg, exp_avg_sq, numel, flags} (device pointers as
+ *   integers; exp_avg = 0: the row is clipped but not updated; flags: GR_ADAM_ALIGNED16 when every pointer of the row
+ *   is 16-byte aligned).  Tensors are contiguous fp32; numel may be 0.
+ * scalars: fp32 [T][8], per tensor, each rounded from the float64 value torch computes on the host:
+ *   {1 - beta1, beta2, 1 - beta2, eps, weight_decay, step_size = -(lr / (1 - beta1^t)), (1 - beta2^t) ** 0.5, 0}.
+ * chunks: int32 [C][2] = {tensor row, chunk index k}: the elements [k E, min((k + 1) E, numel)) of that tensor,
+ *   E = gr_adam_chunk_elems().  One CTA per chunk.
+ * gr_grad_sumsq: slots[c] (float64 [C]) = sum of grad^2 over chunk c.
+ * gr_clip_adam: with slots (clipping): total = sqrt of the sum of slots[0 .. C) in one fixed order, in float64, rounded
+ *   once to fp32 and written to grad_norm[0] (fp32, may be NULL); coef = min(fp32(1 / (total + 1e-6)) * max_norm, 1)
+ *   in fp32 (clip_grads_with_norm_: a NaN total gives NaN, an infinite one 0); grad *= coef, written back.  Then
+ *   for every row with exp_avg: g = grad (+ weight_decay * param when weight_decay != 0, not written back);
+ *   exp_avg.lerp_(g, 1 - beta1) (ATen/native/Lerp.h); exp_avg_sq = exp_avg_sq * beta2, then + (1 - beta2) g g
+ *   (addcmul); param += step_size * (exp_avg / (sqrt(exp_avg_sq) / bc2_sqrt + eps)) (addcdiv); one fp32 rounding
+ *   per foreach op.  slots = NULL: no clipping (max_norm and grad_norm unused; grad_norm must be NULL).
+ *   flags: GR_ADAM_WEIGHT_DECAY when any row has weight_decay != 0 (without it the weight decay is not read).
+ */
+#define GR_ADAM_ALIGNED16 1
+#define GR_ADAM_WEIGHT_DECAY 1u
+int gr_adam_chunk_elems(void);
+int gr_grad_sumsq(const int64_t* table, const int32_t* chunks, int C, double* slots, void* stream);
+int gr_clip_adam(const int64_t* table, const float* scalars, const int32_t* chunks, int C, const double* slots,
+                 double max_norm, float* grad_norm, uint32_t flags, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Device-resident split (loader.DeviceSplit, csrc/split.cu): a split's per-question facts are uploaded once and
  * every batch is assembled on the device from B question ids (the int64 device array `ids`, B > 0).
  * A question id outside [0, num_q) counts as an empty question and sets bit 1 of `status` (int32[1], OR-ed); a batch

@@ -8,6 +8,8 @@ N = 2000 nodes, E = 6000 stored facts per question, self-loops on): per batch ``
   host    the loader's get_batch with loader.install(shuffle=True, weights="arrays", index_dtype=np.int32)
           (GraftNet: plus loader.install_graft), so np.random.permutation per question as in the reference
   device  DeviceSplit(loader, weights="arrays", shuffle=True).get_batch
+  device_fused  the device batches through a graphed step that also runs clip_grad_norm_ and Adam.step() in its graph
+          (``optimizer=``, ``max_norm=``; optim.ClipAdam); graphed shapes only
 
 Shapes: ReaRev and NSM at the reference's training shape (B 8, entity_dim 50) through graphed.GraphedTrainStep;
 GraftNet (B 8, entity_dim 50) eager (graftnet_d50) and through graphed.GraphedGraftTrainStep (graftnet_d50_graphed);
@@ -55,10 +57,18 @@ def train_pass(data, step_fn, B):
     return time.perf_counter() - t0
 
 
-def make_step(name, m, use_graph):
+def make_step(name, m, use_graph, fused=False):
     params = [p for p in m.parameters() if p.requires_grad]
     opt = torch.optim.Adam(params, lr=1e-4)
     cls = graphed.GraphedGraftTrainStep if name == "GraftNet" else graphed.GraphedTrainStep
+    if fused:
+        fstep = cls(m, optimizer=opt, max_norm=1.0)
+
+        def step_fused(batch):
+            loss, _pred, _pd, h1, f1 = fstep.step(batch)
+            fstep.tp_list(h1, f1)
+            loss.item()
+        return step_fused
     gstep = cls(m) if use_graph else None
 
     def step(batch):
@@ -124,22 +134,28 @@ def main():
         torch.manual_seed(0)
         m = {"ReaRev": G.ReaRev, "NSM": G.NSM, "GraftNet": G.GraftNet}[name](dict(args), NE, NR, NW).cuda().train()
         step = make_step(name, m, use_graph)
-        modes = {"host": L, "device": split}
-        for data in modes.values():                   # warm-up: captures, caches
-            train_pass(data, step, B)
+        modes = {"host": (L, step), "device": (split, step)}
+        if use_graph:
+            modes["device_fused"] = (split, make_step(name, m, use_graph, fused=True))
+        for data, fn in modes.values():               # warm-up: captures, caches
+            train_pass(data, fn, B)
         secs = {k: [] for k in modes}
         for _ in range(a.runs):
-            for k, data in modes.items():
-                secs[k].append(train_pass(data, step, B))
+            for k, (data, fn) in modes.items():
+                secs[k].append(train_pass(data, fn, B))
         qps = {k: a.questions / float(np.median(v)) for k, v in secs.items()}
         res = dict(shape=shape, model=name, B=B, D=over["entity_dim"], graphed=use_graph, fact_drop=FACT_DROP,
                    N=L.max_local_entity, E=6000, questions=a.questions, host_qps=round(qps["host"], 1),
                    device_qps=round(qps["device"], 1), speedup=round(qps["device"] / qps["host"], 2),
                    host_s=[round(x, 4) for x in secs["host"]], device_s=[round(x, 4) for x in secs["device"]],
                    gpu=info)
+        if use_graph:
+            res.update(device_fused_qps=round(qps["device_fused"], 1),
+                       device_fused_s=[round(x, 4) for x in secs["device_fused"]],
+                       fused_speedup=round(qps["device_fused"] / qps["device"], 2))
         results.append(res)
         print(json.dumps(res), flush=True)
-        del step, m
+        del step, modes, m
         torch.cuda.empty_cache()
     for B, E in ((64, 6000), (1, 50000)):
         res = dict(kernel="gr_split_fact_order", B=B, E=E, fact_drop=FACT_DROP,

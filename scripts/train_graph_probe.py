@@ -8,10 +8,13 @@ ReaRev B 64, entity_dim 200, num_ins 2, num_iter 3, num_gnn 3; graftnet_d50 = Gr
 lstm (the reference's GraftNet training shape); graftnet_cfg2 = GraftNet B 64, entity_dim 200, num_layer 3.  All on
 WebQSP-shape synthetic subgraphs (N 2000, 6000 facts per question; GraftNet: the same facts as graft tuples), dropout
 0.2 / 0.3 as in the reference's defaults.  One step = forward + backward + the train-time hit@1 / F1
-as host lists (the tp_list train_epoch keeps), with or without the caller's clip_grad_norm_ + Adam.step().  A run
+as host lists (the tp_list train_epoch keeps), with or without the caller's clip_grad_norm_ + Adam.step(), and
+"graphed+fused" with both in the graph (``optimizer=``, ``max_norm=``: optim.ClipAdam).  A run
 times ``--steps`` steps between two CUDA events after ``--warmup`` steps; each mode runs ``--runs`` times, alternating
 eager and graphed, and the median and the spread are reported.  The GPU's name, SM clock and power limit are read in
-the same run and printed beside the numbers."""
+the same run and printed beside the numbers.  Last, the two clip + Adam kernels alone (gr_grad_sumsq + gr_clip_adam)
+between CUDA events over ``--launches`` launches, with the bytes they move (sumsq reads each gradient; the update
+reads and writes gradient, parameter and both moments)."""
 import argparse
 import json
 import os
@@ -44,6 +47,26 @@ def gpu_info():
         return {"name": torch.cuda.get_device_name(), "error": str(e)}
 
 
+def step_class(c):
+    return graphed.GraphedGraftTrainStep if c.get("model") == "GraftNet" else graphed.GraphedTrainStep
+
+
+def kernel_time(fused, launches):
+    """(microseconds per gr_grad_sumsq + gr_clip_adam pair, bytes they move) of ``fused`` (an optim.ClipAdam)."""
+    adam = set(fused._adam_rows)
+    nbytes = sum(p.numel() * 4 * (1 + (8 if r in adam else 2)) for r, p in enumerate(fused.params))
+    for _ in range(3):
+        fused.launch()
+    torch.cuda.synchronize()
+    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    s.record()
+    for _ in range(launches):
+        fused.launch()
+    e.record()
+    e.synchronize()
+    return s.elapsed_time(e) * 1e3 / launches, nbytes
+
+
 def build(c):
     """-> (model, two batches, the graphed step)."""
     torch.manual_seed(0)
@@ -52,12 +75,12 @@ def build(c):
         args = S.model_args("GraftNet", entity_dim=c["D"], num_layer=c["L"], use_cuda=True)
         m = G.GraftNet(dict(args), *sizes).cuda().train()
         batches = [S.make_graft_batch(s, B=c["B"], N=2000, E=6000) for s in (1, 2)]
-        return m, batches, graphed.GraphedGraftTrainStep(m)
+        return m, batches, step_class(c)(m)
     args = S.model_args("ReaRev", entity_dim=c["D"], num_ins=c["I"], num_iter=c["T"], num_gnn=c["K"], use_cuda=True)
     m = G.ReaRev(dict(args), *sizes).cuda().train()
     batches = [S.make_batch(s, B=c["B"], N=2000, E=6000, with_weights=False)[:7] for s in (1, 2)]
     # the graphed step's buckets: both batches in one capacity bucket, so one graph serves the timed loop
-    return m, batches, graphed.GraphedTrainStep(m)
+    return m, batches, step_class(c)(m)
 
 
 def time_mode(step_fn, batches, steps, warmup):
@@ -79,6 +102,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--shapes", default=",".join(SHAPES))
+    ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -89,6 +113,7 @@ def main():
         m, batches, gstep = build(c)
         params = [p for p in m.parameters() if p.requires_grad]
         opt = torch.optim.Adam(params, lr=1e-4)
+        fstep = step_class(c)(m, optimizer=opt, max_norm=1.0)
 
         def eager(b):
             loss, _pred, _pd, tp = m(b, training=True)
@@ -98,6 +123,10 @@ def main():
         def graph(b):
             _loss, _pred, _pd, h1, f1 = gstep.step(b)
             return gstep.tp_list(h1, f1)
+
+        def fused(b):
+            _loss, _pred, _pd, h1, f1 = fstep.step(b)
+            return fstep.tp_list(h1, f1)
 
         def with_opt(fn):
             def run(b):
@@ -115,7 +144,7 @@ def main():
             return run
 
         modes = {"eager": plain(eager), "graphed": plain(graph), "eager+clip+adam": with_opt(eager),
-                 "graphed+clip+adam": with_opt(graph)}
+                 "graphed+clip+adam": with_opt(graph), "graphed+fused": fused}
         times = {k: [] for k in modes}
         for _ in range(a.runs):
             for k, fn in modes.items():           # alternating, so drift hits every mode alike
@@ -125,9 +154,15 @@ def main():
         out["graphs"] = len(gstep._cache)
         out["speedup"] = out["eager"]["median_ms"] / out["graphed"]["median_ms"]
         out["speedup_with_opt"] = out["eager+clip+adam"]["median_ms"] / out["graphed+clip+adam"]["median_ms"]
+        out["tail_eager_ms"] = out["graphed+clip+adam"]["median_ms"] - out["graphed"]["median_ms"]
+        out["tail_fused_ms"] = out["graphed+fused"]["median_ms"] - out["graphed"]["median_ms"]
+        f = next(iter(fstep._cache.values())).fused
+        us, nbytes = kernel_time(f, a.launches)
+        out["clip_adam_kernels"] = dict(us=us, bytes=nbytes, gb_per_s=nbytes / us * 1e-3, tensors=len(f.params),
+                                        elements=sum(p.numel() for p in f.params))
         res["results"][name] = dict(shape=c, **out)
         print(name, json.dumps(res["results"][name]))
-        del gstep, m, opt
+        del gstep, fstep, m, opt
         torch.cuda.empty_cache()
     print(json.dumps(res))
     if a.out:

@@ -7,6 +7,8 @@
 //   gr_split_assemble_graft  both graft lists of GraftSingleDataLoader._build_fact_mat_maxfacts
 //                            (gnn/dataset_load_graft.py:70-102) in stored order, and the kb_fact_rel rows.
 //   gr_fact_weights          weight_list = 1/outdeg(head) and weight_rel_list = 1/count(head, rel) (:507-516).
+//   gr_fact_weights_live     the same over the live prefix of capacity-length fact buffers, its length read on the
+//                            device (the batch a captured training epoch assembles in place).
 //
 // Assembly: grid (X, B) with X = CTAs per question (a function of B alone).  Every CTA of question b adds up the fact
 // counts of questions 0..b-1 itself (B ids, read from the resident offsets) to find where its question starts, so no
@@ -168,11 +170,18 @@ __device__ __forceinline__ int64_t ld_index(const void* p, int64_t i, int idx_by
   return idx_bytes == 8 ? reinterpret_cast<const int64_t*>(p)[i] : (int64_t)reinterpret_cast<const int32_t*>(p)[i];
 }
 
+// live facts of F slots: all of them, or the first min(F, max(*live, 0)) (as gr_csr_build reads nfacts)
+__device__ __forceinline__ int64_t live_prefix(int64_t F, const int32_t* live) {
+  return live ? min(F, (int64_t)max(*live, 0)) : F;
+}
+
 // pass 1: outdeg(head) and the (head, rel) counts; the hash slot of every fact is kept for pass 2
 __global__ void __launch_bounds__(kWeightThreads)
 fact_count_kernel(const void* __restrict__ heads, const void* __restrict__ rels, int idx_bytes, int64_t F, int64_t Nt,
                   unsigned long long* __restrict__ keys, uint32_t* __restrict__ counts, uint64_t table_mask,
-                  uint32_t* __restrict__ deg, uint32_t* __restrict__ slot_of, int32_t* __restrict__ status) {
+                  uint32_t* __restrict__ deg, uint32_t* __restrict__ slot_of, int32_t* __restrict__ status,
+                  const int32_t* __restrict__ live) {
+  F = live_prefix(F, live);
   for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
     const int64_t h = ld_index(heads, f, idx_bytes), r = ld_index(rels, f, idx_bytes);
     if (h < 0 || h >= Nt || r < 0 || r > INT_MAX) {
@@ -197,7 +206,8 @@ fact_count_kernel(const void* __restrict__ heads, const void* __restrict__ rels,
 __global__ void __launch_bounds__(kWeightThreads)
 fact_weight_kernel(const void* __restrict__ heads, int idx_bytes, int64_t F, const uint32_t* __restrict__ counts,
                    const uint32_t* __restrict__ deg, const uint32_t* __restrict__ slot_of, float* __restrict__ w,
-                   float* __restrict__ wr) {
+                   float* __restrict__ wr, const int32_t* __restrict__ live) {
+  F = live_prefix(F, live);
   for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
     const uint32_t s = slot_of[f];
     if (s == 0xFFFFFFFFu) {
@@ -548,18 +558,21 @@ extern "C" size_t gr_fact_weights_workspace_bytes(int64_t F, int64_t Nt) {
   return gr::weight_workspace(F, Nt).total;
 }
 
-extern "C" int gr_fact_weights(const void* heads, const void* rels, int idx_bytes, int64_t F, int64_t Nt,
-                               float* weight, float* weight_rel, int32_t* status, void* workspace,
-                               size_t workspace_bytes, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(heads && rels && status, "null pointer");
-  GR_CHECK_ARG(weight || weight_rel, "no output requested");
-  GR_CHECK_ARG(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
-  GR_CHECK_ARG(F >= 0 && Nt > 0 && Nt <= UINT_MAX, "need F >= 0 and 0 < Nt <= 2^32 - 1");
-  GR_CHECK_ARG(F <= (int64_t)INT_MAX, "F must fit int32 (hash slots are 32-bit)");
+namespace gr {
+namespace {
+
+// gr_fact_weights (live = null) and gr_fact_weights_live: the table, the grid and the memsets are sized by the F slots,
+// the kernels count and weigh the live prefix only, so the prefix is bit-equal to gr_fact_weights over it
+int fact_weights_launch(const char* fn, const void* heads, const void* rels, int idx_bytes, int64_t F,
+                        const int32_t* live, int64_t Nt, float* weight, float* weight_rel, int32_t* status,
+                        void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  GR_CHECK_ARG_AS(fn, heads && rels && status, "null pointer");
+  GR_CHECK_ARG_AS(fn, weight || weight_rel, "no output requested");
+  GR_CHECK_ARG_AS(fn, idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+  GR_CHECK_ARG_AS(fn, F >= 0 && Nt > 0 && Nt <= UINT_MAX, "need F >= 0 and 0 < Nt <= 2^32 - 1");
+  GR_CHECK_ARG_AS(fn, F <= (int64_t)INT_MAX, "F must fit int32 (hash slots are 32-bit)");
   const WeightWorkspace ws = weight_workspace(F, Nt);
-  int rc = check_workspace(__func__, workspace, workspace_bytes, ws.total);
+  int rc = check_workspace(fn, workspace, workspace_bytes, ws.total);
   if (rc != GR_OK) return rc;
   if (F == 0) return GR_OK;
   char* base = static_cast<char*>(workspace);
@@ -568,16 +581,34 @@ extern "C" int gr_fact_weights(const void* heads, const void* rels, int idx_byte
   auto* counts = reinterpret_cast<uint32_t*>(base + ws.counts);
   auto* deg = reinterpret_cast<uint32_t*>(base + ws.deg);
   auto* slot_of = reinterpret_cast<uint32_t*>(base + ws.slot);
-  GR_CHECK_CUDA(cudaMemsetAsync(keys, 0xFF, T * sizeof(unsigned long long), stream));
-  GR_CHECK_CUDA(cudaMemsetAsync(counts, 0, ws.slot - ws.counts, stream));        // counts and deg
+  GR_CHECK_CUDA_AS(fn, cudaMemsetAsync(keys, 0xFF, T * sizeof(unsigned long long), stream));
+  GR_CHECK_CUDA_AS(fn, cudaMemsetAsync(counts, 0, ws.slot - ws.counts, stream));        // counts and deg
   const int grid = (int)std::min<int64_t>(ceil_div(F, kWeightThreads), 8LL * sm_count());
   fact_count_kernel<<<grid, kWeightThreads, 0, stream>>>(heads, rels, idx_bytes, F, Nt, keys, counts, T - 1, deg,
-                                                         slot_of, status);
-  GR_CHECK_LAUNCH();
+                                                         slot_of, status, live);
+  GR_CHECK_LAUNCH_AS(fn);
   fact_weight_kernel<<<grid, kWeightThreads, 0, stream>>>(heads, idx_bytes, F, counts, deg, slot_of, weight,
-                                                          weight_rel);
-  GR_CHECK_LAUNCH();
+                                                          weight_rel, live);
+  GR_CHECK_LAUNCH_AS(fn);
   return GR_OK;
+}
+
+}  // namespace
+}  // namespace gr
+
+extern "C" int gr_fact_weights(const void* heads, const void* rels, int idx_bytes, int64_t F, int64_t Nt,
+                               float* weight, float* weight_rel, int32_t* status, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+  return gr::fact_weights_launch(__func__, heads, rels, idx_bytes, F, nullptr, Nt, weight, weight_rel, status,
+                                 workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int gr_fact_weights_live(const void* heads, const void* rels, int idx_bytes, int64_t capacity,
+                                    const int32_t* nfacts, int64_t Nt, float* weight, float* weight_rel,
+                                    int32_t* status, void* workspace, size_t workspace_bytes, void* stream_) {
+  GR_CHECK_ARG(nfacts, "null nfacts");
+  return gr::fact_weights_launch(__func__, heads, rels, idx_bytes, capacity, nfacts, Nt, weight, weight_rel, status,
+                                 workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" size_t gr_split_fact_order_workspace_bytes(int64_t n_total) {

@@ -27,7 +27,9 @@ Training: :class:`GraphedTrainStep` captures ``model(batch, training=True)`` + `
 metrics (gr_train_metrics) of ReaRev and NSM over the same input side, and :class:`GraphedGraftTrainStep` those of
 GraftNet over :class:`_GraftLayout` (the graft fact count stays on the device).  Given a ``torch.optim.Adam``, both
 also capture the gradient clipping and the optimizer step (:class:`optim.ClipAdam`); see their docstrings and DESIGN
-§4.11.
+§4.11.  :meth:`GraphedTrainStep.train_epoch` runs a whole ReaRev / NSM epoch over a ``loader.DeviceSplit``: each step's
+graph also assembles its batch from a device cursor into the epoch's question order and records the step's loss and
+metrics on the device (csrc/epoch.cu), so the host only replays graphs and reads the device once per epoch.
 """
 import collections
 import contextlib
@@ -51,6 +53,9 @@ class _Captured:
 class Ticket:
     """One in-flight step of the submit/collect pipeline."""
     __slots__ = ("slot", "done", "ent", "local_entity_host", "cand_ent_host", "B", "N")
+
+
+_INT32_MAX = 2 ** 31 - 1
 
 
 def fact_capacity(F):
@@ -533,6 +538,95 @@ class TrainStepOutput(tuple):
         self._raise_for(self.status.tolist())
 
 
+class EpochPlan:
+    """The host arithmetic of one epoch over a resident split (:func:`epoch_plan`): per step ``B`` (questions),
+    ``F`` (live facts: kept facts + self-loops), ``K`` (kept facts) and ``capacity`` (``fact_capacity(F)``), int64
+    numpy arrays of ``steps`` entries, and ``starts``, the step's first position in the order."""
+    __slots__ = ("steps", "B", "F", "K", "capacity", "starts")
+
+
+def epoch_plan(order, stored, ents, batch_size, fact_dropout=0.0):
+    """Per-step counts of an epoch that takes the questions ``order`` (ids, in batch order) ``batch_size`` at a time,
+    the last batch short when ``len(order) % batch_size != 0``: what ``DeviceSplit.get_batch(it, batch_size,
+    fact_dropout)`` computes on the host for each step, from the split's per-question stored fact counts ``stored``
+    and self-loop counts ``ents`` (zeros without ``use_self_loop``).  A question keeps ``loader.kept_counts`` of its
+    stored facts.  An id outside [0, len(stored)) counts as an empty question, as the device assembly counts it."""
+    from .loader import kept_counts
+    order = np.asarray(order, dtype=np.int64).reshape(-1)
+    stored, ents = np.asarray(stored, dtype=np.int64), np.asarray(ents, dtype=np.int64)
+    n, bs = order.size, int(batch_size)
+    plan = EpochPlan()
+    plan.steps = (n + bs - 1) // bs
+    plan.starts = np.arange(0, n, bs, dtype=np.int64)
+    ok = (order >= 0) & (order < stored.size)
+    q = np.where(ok, order, 0)
+    k = np.where(ok, kept_counts(stored[q] if stored.size else np.zeros(n, np.int64), fact_dropout), 0)
+    e = np.where(ok, ents[q] if ents.size else 0, 0)
+    if n:
+        plan.K = np.add.reduceat(k, plan.starts).astype(np.int64)
+        plan.F = plan.K + np.add.reduceat(e, plan.starts).astype(np.int64)
+    else:
+        plan.K = plan.F = np.zeros(0, dtype=np.int64)
+    plan.B = np.minimum(bs, n - plan.starts).astype(np.int64)
+    plan.capacity = np.array([fact_capacity(f) for f in plan.F.tolist()], dtype=np.int64)
+    return plan
+
+
+class EpochRun:
+    """One epoch started by :meth:`GraphedTrainStep.start_epoch`: device tensors, valid once the current stream reaches
+    them.  ``losses`` / ``grad_norms`` fp32 [steps] (``grad_norms`` None without ``max_norm``), ``h1`` / ``f1`` fp32
+    [num_data] in batch order, ``seeds`` int64 [steps] (the fact-order seed of each step; None without ``shuffle``),
+    ``status`` int32 [2]: the OR of every step's batch-assembly status word and of its CSR build's.
+    :meth:`result` reads them back in one copy; :meth:`check` raises for a nonzero status."""
+
+    def __init__(self, losses, grad_norms, h1, f1, seeds, status):
+        self.losses, self.grad_norms, self.h1, self.f1, self.seeds, self.status = \
+            losses, grad_norms, h1, f1, seeds, status
+        self._words = None
+
+    def result(self):
+        """-> ``(np.mean(losses), [0, 0], h1_list_all, f1_list_all)`` as the reference's ``train_epoch`` returns them
+        (Python floats in the lists), read back in one device-to-host copy."""
+        n, m = self.losses.numel(), self.h1.numel()
+        host = torch.cat([self.losses, self.h1, self.f1, self.status.view(torch.float32)]).cpu()
+        self._words = host[n + 2 * m:].view(torch.int32).tolist()
+        return np.mean(host[:n].tolist()), [0, 0], host[n:n + m].tolist(), host[n + m:n + 2 * m].tolist()
+
+    def check(self):
+        """Raise ``DeviceSplit.check``'s message when an assembly flagged an id out of range or an overflow, else
+        ``TrainStepOutput.check``'s when a CSR build flagged ids outside the batch (reads the status unless
+        :meth:`result` has)."""
+        from .loader import DeviceSplit
+        split_word, csr_word = self._words if self._words is not None else self.status.tolist()
+        DeviceSplit.raise_status(split_word)
+        if csr_word:
+            _KbLayout.raise_for([csr_word])
+
+
+class _EpochBuffers:
+    """The device state the epoch graphs of one (split, batch size) read and write: the cursor, the question order,
+    the kept-count table, the records and the per-step Adam scalars.  Fixed addresses: the graphs hold them."""
+
+    def __init__(self, split, batch_size, max_norm):
+        dev = split.device
+        self.split, self.batch_size = split, int(batch_size)
+        self.num_data = int(split.num_data)
+        self.steps = (self.num_data + self.batch_size - 1) // self.batch_size
+        i64, f32 = dict(dtype=torch.int64, device=dev), dict(dtype=torch.float32, device=dev)
+        self.cursor = torch.zeros(1, **i64)
+        self.order = torch.zeros(self.num_data, **i64)
+        self.kept_table = torch.zeros(max(split.num_q, 1), **i64) if split.shuffle else None
+        self.losses = torch.zeros(self.steps, **f32)
+        self.grad_norms = torch.zeros(self.steps, **f32) if max_norm is not None else None
+        self.seeds = torch.zeros(self.steps, **i64) if split.shuffle else None
+        self.h1 = torch.zeros(self.num_data, **f32)
+        self.f1 = torch.zeros(self.num_data, **f32)
+        self.status = torch.zeros(2, dtype=torch.int32, device=dev)
+        self.adam = None                 # fp32 [steps, T, 8], made at the first capture (T is known then)
+        # the fact-order workspace of any batch: the stored facts of the batch_size largest questions
+        self.n_total = int(np.sort(split._stored)[-self.batch_size:].sum()) if split._stored.size else 0
+
+
 def _release_autograd_history(model):
     """Drop the tensors with autograd history that a training forward leaves on the model's modules (``dist_history``,
     the question encoder's states).  While a previous step's graph is alive, the next forward reuses its AccumulateGrad
@@ -610,6 +704,7 @@ class GraphedTrainStep:
         self.max_graphs = max_graphs
         self._cache = collections.OrderedDict()
         self._layout = layout(self)
+        self._epochs = {}
 
     @staticmethod
     def tp_list(h1, f1):
@@ -619,6 +714,10 @@ class GraphedTrainStep:
     # -- capture key and refusals ----------------------------------------------------------------------------------
     def key(self, batch):
         """The capture key of ``batch`` under the current model and torch state (see the class docstring)."""
+        return self._layout.key(batch) + self._state_key()
+
+    def _state_key(self):
+        """The part of the capture key that is not the batch shape: the model, torch and optimizer state."""
         m = self.model
         if len(self._params) != sum(1 for _ in m.parameters()):
             raise ValueError("the model's parameters changed after GraphedTrainStep was built: build a new one")
@@ -630,7 +729,7 @@ class GraphedTrainStep:
         opt = self.optimizer
         fused = () if opt is None else (self.max_norm, any(g["weight_decay"] != 0 for g in opt.param_groups),
                                         optim.state_key(opt))
-        return self._layout.key(batch) + (
+        return (
             m.training, drops, _autocast_dtype(), torch.are_deterministic_algorithms_enabled(), backends,
             tuple(p.requires_grad for p in self._params), tuple(p.data_ptr() for p in self._params), rel_text) + fused
 
@@ -758,6 +857,207 @@ class GraphedTrainStep:
             p.grad = g
         return TrainStepOutput(*ent.outs, raise_for=self._layout.raise_for,
                                grad_norm=None if ent.fused is None else ent.fused.grad_norm)
+
+
+    # -- a whole epoch -----------------------------------------------------------------------------------------------
+    def train_epoch(self, split, batch_size, fact_dropout):
+        """The reference's ``Trainer_KBQA.train_epoch`` around the model, over the resident split ``split``: one
+        :meth:`start_epoch`, one read.  -> ``(np.mean(losses), [0, 0], h1_list_all, f1_list_all)``.  Raises
+        :meth:`EpochRun.check`'s errors after the epoch when a batch was malformed."""
+        run = self.start_epoch(split, batch_size, fact_dropout)
+        out = run.result()
+        run.check()
+        return out
+
+    def _epoch_refusal(self, split, batch_size, fact_dropout):
+        from .loader import DeviceSplit, same_device
+        if self.optimizer is None:
+            return "an epoch steps the optimizer in its graphs: build the step with optimizer="
+        if isinstance(self._layout, _GraftLayout):
+            return "train_epoch covers ReaRev and NSM; GraftNet's epoch runs step by step (GraphedGraftTrainStep.step)"
+        if not isinstance(split, DeviceSplit):
+            return "train_epoch takes a loader.DeviceSplit, got %s" % type(split).__name__
+        if split.graft:
+            return "train_epoch takes a ReaRev / NSM split; this DeviceSplit holds GraftNet's graft lists"
+        if not same_device(split.device, self.device):
+            return "the split lives on %s, the model on %s" % (split.device, self.device)
+        if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or batch_size <= 0:
+            return "batch_size must be a positive int, got %r" % (batch_size,)
+        if not split.shuffle and fact_dropout != 0:
+            return "fact_dropout must be 0 (facts come in stored order), got %r" % (fact_dropout,)
+        if split.shuffle and not 0 <= fact_dropout <= 1:
+            return "fact_dropout must be in [0, 1], got %r" % (fact_dropout,)
+        if getattr(split.loader, "q_type", "seq") != "seq":
+            return "q_type must be 'seq', got %r" % (split.loader.q_type,)
+        m = self.model
+        if (m.normalized_gnn or m.norm_rel) and split.weights != "arrays":
+            return "normalized_gnn / norm_rel need fact weights: the split was built with weights='none'"
+        return None
+
+    def start_epoch(self, split, batch_size, fact_dropout):
+        """Start one training epoch over ``split`` (a ``loader.DeviceSplit``) and return its :class:`EpochRun` without
+        waiting for the device.
+
+        As the reference's ``train_epoch``: ``model.train()``, ``split.reset_batches(is_sequential=False)`` (the
+        loader's ``np.random`` order), then every batch of ``batch_size`` questions in order, the last one short when
+        ``num_data % batch_size != 0``, each assembled as ``split.get_batch(it, batch_size, fact_dropout)`` does,
+        trained and stepped.  Each step is one graph replay: the graph assembles the batch on the device from a
+        cursor into the epoch's question order (gr_epoch_step_begin, ``DeviceSplit.assemble`` at the bucket's
+        capacity, the fact-order seed drawn from torch's CUDA generator with ``shuffle``), runs the step of
+        :meth:`step` with the step's Adam scalars (all uploaded at the start of the epoch), then records loss,
+        gradient norm, seed, hit@1 and F1 at the cursor and advances it (gr_epoch_step_record).  The host picks each
+        step's graph from :func:`epoch_plan`; the graphs the epoch needs and does not hold yet are captured before the
+        first replay (the LRU grows to hold them all), without moving the records, the parameters or torch's generator.
+
+        Afterwards ``p.grad``, the parameters and the Adam state are those of the loop ``get_batch`` + :meth:`step`,
+        the CPU ``step`` tensors advanced by the number of steps, and ``split.loader.sample_ids`` is the last batch's.
+        Refused (``ValueError``): a step without ``optimizer``, GraftNet, anything but a CUDA ``DeviceSplit`` of a kb
+        loader on the model's device, ``batch_size <= 0``, a ``fact_dropout`` ``get_batch`` refuses, and fact weights
+        (``normalized_gnn`` / ``norm_rel``) over a ``weights="none"`` split."""
+        why = self._epoch_refusal(split, batch_size, fact_dropout)
+        if why is not None:
+            raise ValueError("train_epoch: " + why)
+        self.model.train()
+        split.reset_batches(is_sequential=False)
+        L = split.loader
+        order = np.asarray(L.batches[:L.num_data], dtype=np.int64).reshape(-1)
+        plan = epoch_plan(order, split._stored, split._ents, batch_size, fact_dropout if split.shuffle else 0.0)
+        if split.index_dtype == torch.int32 and plan.steps and (
+                int(plan.B.max()) * split.N > _INT32_MAX or int(plan.F.max()) > _INT32_MAX):
+            raise ValueError("train_epoch: a batch overflows int32 indices; use index_dtype=torch.int64")
+        ep = self._epoch_buffers(split, batch_size)
+        ep.order.copy_(torch.from_numpy(order), non_blocking=True)
+        if ep.kept_table is not None:
+            from .loader import kept_counts
+            ep.kept_table[:split.num_q].copy_(torch.from_numpy(kept_counts(split._stored, fact_dropout)),
+                                              non_blocking=True)
+        entries = self._epoch_entries(ep, plan)
+        fused = entries[0].fused if entries else None
+        if fused is not None and plan.steps:
+            ep.adam.copy_(torch.from_numpy(fused.epoch_scalars(plan.steps)), non_blocking=True)
+        ep.cursor.zero_()
+        ep.status.zero_()
+        for ent in entries:
+            ent.g.replay()
+        if entries:
+            last = entries[-1]
+            for p, g in zip(last.params, last.grads):
+                p.grad = g
+            if fused is not None:
+                fused.advance(plan.steps)
+            s0 = int(plan.starts[-1])
+            L.sample_ids = L.batches[s0:min(s0 + int(batch_size), L.num_data)]
+        return EpochRun(ep.losses.clone(), None if ep.grad_norms is None else ep.grad_norms.clone(), ep.h1.clone(),
+                        ep.f1.clone(), None if ep.seeds is None else ep.seeds.clone(), ep.status.clone())
+
+    def _epoch_buffers(self, split, batch_size):
+        k = (id(split), int(batch_size))
+        ep = self._epochs.get(k)
+        if ep is None or ep.split is not split or ep.num_data != split.num_data:
+            ep = self._epochs[k] = _EpochBuffers(split, batch_size, self.max_norm)
+        return ep
+
+    def _epoch_key(self, ep, B, cap):
+        split = ep.split
+        shape = (B, split.N, cap, int(split._res["q_input"].shape[1]), split.index_dtype)
+        return shape + self._state_key() + ("epoch", id(ep))
+
+    def _epoch_entries(self, ep, plan):
+        """The graph of every step of ``plan`` (a list), capturing the missing ones first."""
+        shapes = {}
+        for s, (B, cap) in enumerate(zip(plan.B.tolist(), plan.capacity.tolist())):
+            shapes.setdefault((B, cap), s)
+        self.max_graphs = max(self.max_graphs, len(shapes))
+        for (B, cap), s in shapes.items():
+            key = self._epoch_key(ep, B, cap)
+            if key in self._cache:
+                self._cache.move_to_end(key)
+            else:
+                self._epoch_capture(ep, B, cap, s)
+        # a capture may create Adam state, which the keys hold: resolve them once all graphs exist
+        ents = {shape: self._cache[self._epoch_key(ep, *shape)] for shape in shapes}
+        layouts = {ent.fused.layout() for ent in ents.values() if ent.fused is not None}
+        if len(layouts) > 1:
+            raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
+        return [ents[shape] for shape in zip(plan.B.tolist(), plan.capacity.tolist())]
+
+    def _epoch_body(self, ep, st, cursor, ac):
+        """One step of the epoch over the static buffers ``st``: the head kernel, the batch assembly into ``st`` and
+        the captured step of :meth:`_run` -> (outs of _run, seed or None, the assembly status word)."""
+        split = ep.split
+        r = split._res
+        cap = st.heads.numel()
+        ops.epoch_step_begin(cursor, ep.order, ep.batch_size, ep.kept_table, r["q_off"], r["q_ents"],
+                             split.use_self_loop, cap, st.ids, st.rows, st.kept, st.nfacts, st.kept_total, st.status)
+        seed = torch.randint(0, 2 ** 62, (1,), device=self.device) if split.shuffle else None
+        _rows, _kb, _order, asm = split.assemble(st.ids, st.kept, seed, cap, cap, ep.n_total, rows=st.rows, out=st,
+                                                 nfacts=st.nfacts)
+        return self._run(st, ac), seed, st.status | asm
+
+    def _epoch_capture(self, ep, B, cap, s0):
+        """Capture the epoch graph of batches of B questions at fact capacity ``cap``; ``s0``: a step of the epoch with
+        that shape, the one the warm-up assembles."""
+        key = self._epoch_key(ep, B, cap)
+        split = ep.split
+        why = self.refusal(key[3])
+        if why is not None:
+            raise ValueError("GraphedTrainStep: " + why)
+        while len(self._cache) >= self.max_graphs:
+            _k, old = self._cache.popitem(last=False)
+            torch.cuda.synchronize()
+            del old
+        ac = _autocast_dtype()
+        st = self._layout.static_inputs(key)
+        dev = self.device
+        st.ids, st.rows, st.kept = (torch.zeros(B, dtype=torch.int64, device=dev) for _ in range(3))
+        st.kept_total = torch.zeros(1, dtype=torch.int64, device=dev)
+        st.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        params = [p for p in self._params if p.requires_grad]
+        torch.cuda.synchronize()
+        rng = torch.cuda.get_rng_state(dev)
+        warm_cursor = torch.full((1,), s0, dtype=torch.int64, device=dev)    # the real cursor does not move
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                _release_autograd_history(self.model)
+                for p in params:
+                    p.grad = None
+                self._epoch_body(ep, st, warm_cursor, ac)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        torch.cuda.set_rng_state(rng, dev)
+        fused = optim.ClipAdam(self.optimizer, params, [p.grad for p in params], self.max_norm)
+        T = fused._scalars.shape[0]
+        if ep.adam is None:
+            ep.adam = torch.zeros(ep.steps, T, 8, dtype=torch.float32, device=dev)
+        elif ep.adam.shape[1] != T:
+            raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
+        key = self._epoch_key(ep, B, cap)
+        _release_autograd_history(self.model)
+        for p in params:
+            p.grad = None
+        g = torch.cuda.CUDAGraph()
+        gc_on = gc.isenabled()
+        gc.disable()
+        try:
+            with torch.cuda.graph(g):
+                outs, seed, split_word = self._epoch_body(ep, st, ep.cursor, ac)
+                torch.index_select(ep.adam, 0, ep.cursor, out=fused._scalars.view(1, T, 8))
+                fused.launch()
+                loss, _pred, _pd, h1, f1, csr = outs
+                ops.epoch_step_record(ep.cursor, ep.batch_size, ep.num_data, loss.float(), fused.grad_norm, seed, h1,
+                                      f1, split_word, csr, ep.losses, ep.grad_norms, ep.seeds, ep.h1, ep.f1, ep.status)
+        finally:
+            if gc_on:
+                gc.enable()
+        ent = _Captured()
+        ent.st, ent.g, ent.outs, ent.epoch = st, g, outs, ep
+        ent.params, ent.grads = params, [p.grad for p in params]
+        ent.fused = fused
+        fused.bind([p.grad for p in fused.params])
+        self._cache[key] = ent
+        return ent
 
 
 class GraphedGraftTrainStep(GraphedTrainStep):

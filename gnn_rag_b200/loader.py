@@ -237,6 +237,15 @@ def install_graft(loader):
 _INT32_MAX = 2 ** 31 - 1
 
 
+def same_device(a, b):
+    """True when torch devices ``a`` and ``b`` are the same CUDA device (``cuda`` is the current one)."""
+    import torch
+
+    def index(d):
+        return d.index if d.index is not None else torch.cuda.current_device()
+    return a.type == b.type == "cuda" and index(a) == index(b)
+
+
 def kept_counts(n, fact_dropout):
     """Facts kept per question under fact dropout: ``int(np.floor(n * (1 - fact_dropout)))`` of the reference
     (gnn/dataset_load.py:488, gnn/dataset_load_graft.py:88) for every count in ``n``, in float64 as there.  int64."""
@@ -399,13 +408,63 @@ class DeviceSplit:
 
     def check(self):
         """Raise when the last batch's assembly flagged an id out of range or an overflow (reads the device)."""
-        s = int(self.status.item())
+        self.raise_status(int(self.status.item()))
+
+    @staticmethod
+    def raise_status(s):
+        """Raise for a nonzero assembly status word ``s`` (an int read from the device)."""
         if s:
             raise RuntimeError("DeviceSplit: batch assembly status %d (1: question id out of range, 2: more facts than "
                                "the batch's capacity)" % s)
 
     # -- one batch ---------------------------------------------------------------------------------------------------
-    def get_batch(self, iteration, batch_size, fact_dropout, q_type=None, test=False):
+    def assemble(self, ids, kept, seed, F, K, n_total, rows=None, out=None, nfacts=None):
+        """The device part of :meth:`get_batch` for the kb side of B > 0 questions: the row gathers, the fact order
+        (with ``shuffle``), the fact assembly and the fact weights (``weights="arrays"``).
+
+        ``ids`` / ``kept`` int64 [B] and ``seed`` int64 [1] on the device (``kept`` and ``seed`` only read with
+        ``shuffle``); ``rows``: the ids the row tables are gathered at (default ``ids``).  ``F``: the capacity of the
+        fact arrays, ``K`` of the order, ``n_total`` >= the stored facts of the B questions (host ints).  ``out``: an
+        object whose ``local_entity``, ``query_entities``, ``seed_dist``, ``answer_dist``, ``q_input``, ``heads``,
+        ``rels``, ``tails``, ``weight_list`` and ``weight_rel_list`` are written in place (a weight that is None is not
+        computed), with ``nfacts`` (int32[1] on the device) the live count of the F slots; without it new tensors of F
+        facts.  Launch shapes and sizes come from these arguments alone, so a CUDA graph can capture the call.
+        -> (le, qe, sd, ad, qi), (heads, rels, tails, batch_ids, fact_ids, w, wr), order (None without shuffle), status
+        int32[1]."""
+        import torch
+        from . import ops
+        r, N, idt = self._res, self.N, self.index_dtype
+        B = ids.numel()
+        rows = ids if rows is None else rows
+        names = ("local_entity", "query_entities", "seed_dist", "answer_dist", "q_input")
+        gathered = tuple(torch.index_select(r[n], 0, rows, out=None if out is None else getattr(out, n)) for n in names)
+        fo = None if out is None else (out.heads, out.rels, out.tails, None, None)
+        if self.shuffle:
+            order, ost = ops.split_fact_order(r["q_off"], ids, kept, seed, 0, n_total, K)
+            *kb, status = ops.split_assemble_ordered(
+                r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, kept, order, N, F,
+                self.self_rel, self.use_self_loop, idt, out=fo)
+            status = status | ost
+        else:
+            order = None
+            *kb, status = ops.split_assemble(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, N,
+                                             F, self.self_rel, self.use_self_loop, idt, out=fo)
+        w = wr = None
+        if self.weights == "arrays":
+            if out is not None:
+                w, wr = out.weight_list, out.weight_rel_list
+                if w is not None or wr is not None:
+                    ops.fact_weights_live(kb[0], kb[1], nfacts, max(B * N, 1), w, wr)
+            elif F:
+                w, wr, _st = ops.fact_weights(kb[0], kb[1], max(B * N, 1))
+            else:
+                w, wr = (torch.empty(0, dtype=torch.float32, device=self.device) for _ in range(2))
+        return gathered, (*kb, w, wr), order, status
+
+    def get_batch(self, iteration, batch_size, fact_dropout, q_type=None, test=False, seed=None):
+        """The loader's ``get_batch`` from the resident split (see the class docstring).  ``seed``: with ``shuffle``,
+        the fact-order seed to use (int64 [1] on the device, e.g. a seed an epoch recorded) instead of one drawn from
+        torch's CUDA generator."""
         import torch
         from . import ops
         L, r, dev = self.loader, self._res, self.device
@@ -435,38 +494,32 @@ class DeviceSplit:
         if idt == torch.int32 and (B * N > _INT32_MAX or F > _INT32_MAX):
             raise ValueError("DeviceSplit.get_batch: the batch overflows int32 indices (B*N = %d, %d facts); use "
                              "index_dtype=torch.int64" % (B * N, F))
+        kept_dev = None
         if self.shuffle:
             kept_g = kept_counts(self._graft_count[ids], fact_dropout) if self.graft else kept[:0]
             # one upload: the ids, then the kept counts of the kb facts and of the graft lists
             up = torch.from_numpy(np.concatenate([ids, kept, kept_g])).to(dev, non_blocking=True)
             ids_dev, kept_dev, kept_g_dev = up[:B], up[B:2 * B], up[2 * B:]
-            seed = torch.randint(0, 2 ** 62, (1,), device=dev)
+            if seed is None:
+                seed = torch.randint(0, 2 ** 62, (1,), device=dev)
+            elif not (isinstance(seed, torch.Tensor) and same_device(seed.device, dev) and seed.dtype == torch.int64
+                      and seed.numel() == 1):
+                raise ValueError("DeviceSplit.get_batch: seed must be one int64 on %s" % dev)
+            seed = seed.reshape(1)
         else:
             ids_dev = torch.from_numpy(ids).to(dev, non_blocking=True)
-        rows = lambda name: torch.index_select(r[name], 0, ids_dev)      # noqa: E731
-        le, qe, sd, ad, qi = (rows(n) for n in ("local_entity", "query_entities", "seed_dist", "answer_dist",
-                                                 "q_input"))
-        if B and self.shuffle:
-            K = int(kept.sum())
-            order, ost = ops.split_fact_order(r["q_off"], ids_dev, kept_dev, seed, 0, int(self._stored[ids].sum()), K)
-            heads, rels, tails, bids, fids, self.status = ops.split_assemble_ordered(
-                r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids_dev, kept_dev, order, N, F,
-                self.self_rel, self.use_self_loop, idt)
-            self.status = self.status | ost
-            self.last_order = dict(kb=order, kb_offsets=np.concatenate([[0], np.cumsum(kept)]))
-        elif B:
-            heads, rels, tails, bids, fids, self.status = ops.split_assemble(
-                r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids_dev, N, F, self.self_rel,
-                self.use_self_loop, idt)
+        if B:
+            K = int(kept.sum()) if self.shuffle else 0
+            n_total = int(self._stored[ids].sum()) if self.shuffle else 0
+            (le, qe, sd, ad, qi), kb, order, self.status = self.assemble(ids_dev, kept_dev, seed, F, K, n_total)
+            if self.shuffle:
+                self.last_order = dict(kb=order, kb_offsets=np.concatenate([[0], np.cumsum(kept)]))
         else:
-            heads, rels, tails, bids, fids = (torch.empty(0, dtype=idt, device=dev) for _ in range(5))
-        w = wr = None
-        if self.weights == "arrays":
-            if F:
-                w, wr, _st = ops.fact_weights(heads, rels, max(B * N, 1))
-            else:
-                w, wr = (torch.empty(0, dtype=torch.float32, device=dev) for _ in range(2))
-        kb = (heads, rels, tails, bids, fids, w, wr)
+            le, qe, sd, ad, qi = (torch.index_select(r[n], 0, ids_dev) for n in (
+                "local_entity", "query_entities", "seed_dist", "answer_dist", "q_input"))
+            kb = tuple(torch.empty(0, dtype=idt, device=dev) for _ in range(5))
+            kb += (None, None) if self.weights != "arrays" else \
+                tuple(torch.empty(0, dtype=torch.float32, device=dev) for _ in range(2))
         tail = (L.answer_lists[sample_ids],) if test else ()
         if not self.graft:
             return (le, qe, kb, qi, sd, None, ad) + tail

@@ -1010,11 +1010,23 @@ def split_assemble_ok(B, N, F, index_dtype):
     return index_dtype == torch.int64 or (B * N <= _INT32_MAX and F <= _INT32_MAX)
 
 
-def split_assemble(q_off, q_heads, q_rels, q_tails, q_ents, ids, N, F, self_rel, use_self_loop, index_dtype):
+def _split_out(out, F, index_dtype, dev):
+    """The five [F] index outputs of a split assembly: the tensors of ``out`` (None entries are made here)."""
+    out = [None] * 5 if out is None else list(out)
+    for i, t in enumerate(out):
+        if t is None:
+            out[i] = torch.empty(F, dtype=index_dtype, device=dev)
+        elif not (t.is_cuda and t.dtype == index_dtype and t.is_contiguous() and t.numel() == F):
+            raise RuntimeError("split assembly: out[%d] must be a contiguous %s [%d] CUDA tensor" % (i, index_dtype, F))
+    return out
+
+
+def split_assemble(q_off, q_heads, q_rels, q_tails, q_ents, ids, N, F, self_rel, use_self_loop, index_dtype, out=None):
     """-> (heads, rels, tails, batch_ids, fact_ids, status): the fact arrays of the questions ``ids`` (int64 [B] on the
     device) of a resident split (gr_split_assemble), each [F] in ``index_dtype``; ``status`` int32[1] on the device
     (bit 1: an id out of range, bit 2: more facts than F).  q_off int64 [num_q+1]; q_heads/q_rels/q_tails int32 (local
-    ids, by question); q_ents int32 [num_q]."""
+    ids, by question); q_ents int32 [num_q].  ``out``: optional five [F] tensors (None entries allocated) written in
+    place of new ones."""
     q_off = _cuda(q_off, torch.int64, "q_off").contiguous()
     q_heads, q_rels, q_tails, q_ents = (_cuda(t, torch.int32, n).contiguous() for t, n in
                                         ((q_heads, "q_heads"), (q_rels, "q_rels"), (q_tails, "q_tails"),
@@ -1025,7 +1037,7 @@ def split_assemble(q_off, q_heads, q_rels, q_tails, q_ents, ids, N, F, self_rel,
         raise RuntimeError("split_assemble: need B > 0, N > 0, F >= 0 and an int32 / int64 index dtype whose range "
                            "holds B*N and F, got B=%d N=%d F=%d %s" % (B, N, F, index_dtype))
     dev = ids.device
-    out = [torch.empty(F, dtype=index_dtype, device=dev) for _ in range(5)]
+    out = _split_out(out, F, index_dtype, dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
     _launch("gr_split_assemble", _p(q_off), _p(q_heads), _p(q_rels), _p(q_tails), _p(q_ents), num_q, _p(ids), B,
             int(N), int(self_rel), int(bool(use_self_loop)), _INDEX_BYTES[index_dtype], int(F),
@@ -1097,10 +1109,10 @@ def split_fact_order(off, ids, kept, seed, perm, n_total, K):
 
 
 def split_assemble_ordered(q_off, q_heads, q_rels, q_tails, q_ents, ids, kept, order, N, F, self_rel, use_self_loop,
-                           index_dtype):
+                           index_dtype, out=None):
     """:func:`split_assemble` with question b contributing the facts at the stored indices of its ``kept[b]`` entries
     of ``order`` (:func:`split_fact_order`), then its self-loops (gr_split_assemble_ordered).  Shape rule:
-    :func:`split_assemble_ok`."""
+    :func:`split_assemble_ok`; ``out`` as there."""
     q_off = _cuda(q_off, torch.int64, "q_off").contiguous()
     q_heads, q_rels, q_tails, q_ents = (_cuda(t, torch.int32, n).contiguous() for t, n in
                                         ((q_heads, "q_heads"), (q_rels, "q_rels"), (q_tails, "q_tails"),
@@ -1112,7 +1124,7 @@ def split_assemble_ordered(q_off, q_heads, q_rels, q_tails, q_ents, ids, kept, o
         raise RuntimeError("split_assemble_ordered: need B > 0, kept [B], N > 0, F >= 0 and an int32 / int64 index "
                            "dtype whose range holds B*N and F, got B=%d N=%d F=%d %s" % (B, N, F, index_dtype))
     dev = ids.device
-    out = [torch.empty(F, dtype=index_dtype, device=dev) for _ in range(5)]
+    out = _split_out(out, F, index_dtype, dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
     _launch("gr_split_assemble_ordered", _p(q_off), _p(q_heads), _p(q_rels), _p(q_tails), _p(q_ents), num_q, _p(ids),
             _p(kept), _p(order) if K else None, K, B, int(N), int(self_rel), int(bool(use_self_loop)),
@@ -1175,6 +1187,76 @@ def fact_weights(heads, rels, Nt, weight=True, weight_rel=True):
     _launch("gr_fact_weights", _p(heads), _p(rels), _INDEX_BYTES[heads.dtype], F, int(Nt), _p(w), _p(wr),
             _p(status), _p(ws), nbytes, launches=2, op="split_assemble")
     return w, wr, status
+
+
+def fact_weights_live(heads, rels, nfacts, Nt, weight=None, weight_rel=None):
+    """1/outdeg(head) into ``weight`` and 1/count(head, rel) into ``weight_rel`` (fp32, the capacity of ``heads``; either
+    may be None, not both) over the live prefix of capacity-length fact buffers, ``nfacts`` (int32[1] on the device)
+    long (gr_fact_weights_live): bit-equal there to :func:`fact_weights` of the prefix; entries past it are not
+    written.  -> status int32[1] (as :func:`fact_weights`).  Shape rule: :func:`fact_weights_ok` of the capacity."""
+    heads, rels = _cuda(heads, name="heads").contiguous(), _cuda(rels, name="rels").contiguous()
+    nfacts = _cuda(nfacts, torch.int32, "nfacts")
+    if heads.dtype not in _INDEX_BYTES or rels.dtype != heads.dtype:
+        raise RuntimeError("fact_weights_live: heads and rels must share dtype int32 or int64")
+    cap = heads.numel()
+    for name, t in (("weight", weight), ("weight_rel", weight_rel)):
+        if t is not None and not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == cap):
+            raise RuntimeError("fact_weights_live: %s must be a contiguous fp32 [%d] CUDA tensor" % (name, cap))
+    if not fact_weights_ok(cap, Nt) or (weight is None and weight_rel is None) or nfacts.numel() != 1:
+        raise RuntimeError("fact_weights_live: need 0 <= capacity <= 2^31 - 1, 0 < Nt < 2^32, one nfacts and an "
+                           "output, got capacity=%d Nt=%d" % (cap, Nt))
+    status = torch.zeros(1, dtype=torch.int32, device=heads.device)
+    if cap == 0:
+        return status
+    ws, nbytes = _workspace(heads.device, "gr_fact_weights_workspace_bytes", cap, Nt)
+    _launch("gr_fact_weights_live", _p(heads), _p(rels), _INDEX_BYTES[heads.dtype], cap, _p(nfacts), int(Nt),
+            _p(weight), _p(weight_rel), _p(status), _p(ws), nbytes, launches=2, op="split_assemble")
+    return status
+
+
+def epoch_step_begin(cursor, order, batch_size, kept_table, q_off, q_ents, use_self_loop, capacity, ids, rows, kept,
+                     nfacts, kept_total, status):
+    """The head of a graphed epoch step (gr_epoch_step_begin): from the device ``cursor`` (int64[1]) and the epoch's
+    ``order`` (int64 [num_data]), the step's ``ids`` / ``rows`` / ``kept`` (int64 [B], B their length), ``nfacts``
+    (int32[1]), ``kept_total`` (int64[1]) and ``status`` (int32[1]), all written in place.  ``kept_table``: int64
+    [num_q] kept counts, or None for every stored fact."""
+    B = ids.numel()
+    for name, t, dt, n in (("cursor", cursor, torch.int64, 1), ("order", order, torch.int64, None),
+                           ("kept_table", kept_table, torch.int64, None), ("q_off", q_off, torch.int64, None),
+                           ("q_ents", q_ents, torch.int32, None), ("ids", ids, torch.int64, B),
+                           ("rows", rows, torch.int64, B), ("kept", kept, torch.int64, B),
+                           ("nfacts", nfacts, torch.int32, 1), ("kept_total", kept_total, torch.int64, 1),
+                           ("status", status, torch.int32, 1)):
+        if t is not None and (not t.is_contiguous() or (n is not None and t.numel() != n)):
+            raise RuntimeError("epoch_step_begin: %s must be contiguous%s" % (name, "" if n is None else " [%d]" % n))
+        _cuda(t, dt, name)
+    _launch("gr_epoch_step_begin", _p(cursor), _p(order), order.numel(), int(batch_size), B, _p(kept_table),
+            _p(q_off), _p(q_ents), q_ents.numel(), int(bool(use_self_loop)), int(capacity), _p(ids), _p(rows),
+            _p(kept), _p(nfacts), _p(kept_total), _p(status), op="split_assemble")
+
+
+def epoch_step_record(cursor, batch_size, num_data, loss, grad_norm, seed, h1, f1, split_status, csr_status, losses,
+                      grad_norms, seeds, h1_all, f1_all, epoch_status):
+    """The tail of a graphed epoch step (gr_epoch_step_record): the step's fp32 ``loss``, ``grad_norm`` and int64
+    ``seed`` (each one element; the last two optional, with their records ``grad_norms`` / ``seeds``) stored at the
+    cursor, ``h1`` / ``f1`` (fp32 [B]) at its batch's positions of ``h1_all`` / ``f1_all`` (fp32 [num_data]), the int32
+    status words OR-ed into ``epoch_status`` (int32[2]), the cursor advanced.  ``losses`` holds one entry per step."""
+    for name, t, dt in (("cursor", cursor, torch.int64), ("loss", loss, torch.float32),
+                        ("grad_norm", grad_norm, torch.float32), ("seed", seed, torch.int64),
+                        ("h1", h1, torch.float32), ("f1", f1, torch.float32), ("split_status", split_status, torch.int32),
+                        ("csr_status", csr_status, torch.int32), ("losses", losses, torch.float32),
+                        ("grad_norms", grad_norms, torch.float32), ("seeds", seeds, torch.int64),
+                        ("h1_all", h1_all, torch.float32), ("f1_all", f1_all, torch.float32),
+                        ("epoch_status", epoch_status, torch.int32)):
+        if t is not None and not t.is_contiguous():
+            raise RuntimeError("epoch_step_record: %s must be contiguous" % name)
+        _cuda(t, dt, name)
+    B, steps = h1.numel(), losses.numel()
+    if f1.numel() != B or h1_all.numel() != num_data or f1_all.numel() != num_data or epoch_status.numel() != 2:
+        raise RuntimeError("epoch_step_record: need h1, f1 [B], h1_all, f1_all [num_data] and epoch_status [2]")
+    _launch("gr_epoch_step_record", _p(cursor), steps, int(batch_size), B, int(num_data), _p(loss), _p(grad_norm),
+            _p(seed), _p(h1), _p(f1), _p(split_status), _p(csr_status), _p(losses), _p(grad_norms), _p(seeds),
+            _p(h1_all), _p(f1_all), _p(epoch_status), op="optimizer")
 
 
 def shortest_path_nodes(g, source_idx, source_cnt, target_idx, target_cnt, return_distances=False):

@@ -155,11 +155,8 @@ class ClipAdam:
     def prepare(self):
         """Advance the ``step`` of every updated parameter (``torch._foreach_add_``, as Adam does for CPU steps) and
         upload this step's scalars (a pageable H2D copy on the current stream: no host synchronisation)."""
+        self._check_groups()
         groups = self.opt.param_groups
-        if any(isinstance(g["lr"], torch.Tensor) for g in groups):
-            raise ValueError("the fused Adam step takes a float lr, not a tensor")
-        if _any_weight_decay(self.opt) != self._wd:
-            raise ValueError("a group's weight_decay moved between zero and non-zero: build a new ClipAdam")
         if self._steps:
             torch._foreach_add_(self._steps, torch.tensor(1.0, device="cpu"), alpha=1.0)
         memo = {}
@@ -173,6 +170,44 @@ class ClipAdam:
             self._host[r] = row
         self._scalars.copy_(torch.from_numpy(self._host.copy()), non_blocking=True)
         self.opt._opt_called = True          # an LR scheduler's check that the optimizer stepped before it
+
+    def _check_groups(self):
+        groups = self.opt.param_groups
+        if any(isinstance(g["lr"], torch.Tensor) for g in groups):
+            raise ValueError("the fused Adam step takes a float lr, not a tensor")
+        if _any_weight_decay(self.opt) != self._wd:
+            raise ValueError("a group's weight_decay moved between zero and non-zero: build a new ClipAdam")
+
+    def layout(self):
+        """What the scalar rows depend on besides the hyperparameters: the updated rows, their groups and ``step``
+        tensors.  Two objects with the same layout take the same :meth:`epoch_scalars`."""
+        return self._scalars.shape[0], tuple(self._adam_rows), tuple(self._groups), tuple(id(s) for s in self._steps)
+
+    def epoch_scalars(self, steps):
+        """The scalar rows of the next ``steps`` :meth:`prepare` calls, fp32 [steps, T, 8], without advancing anything:
+        the same float64 host arithmetic per step, with the current ``lr`` and hyperparameters."""
+        self._check_groups()
+        groups = self.opt.param_groups
+        out = np.zeros((steps, self._scalars.shape[0], 8), dtype=np.float32)
+        memo = {}
+        for r, gi, step in zip(self._adam_rows, self._groups, self._steps):
+            t0 = step.item()
+            rows = memo.get((gi, t0))
+            if rows is None:
+                g = groups[gi]
+                beta1, beta2 = g["betas"]
+                rows = memo[(gi, t0)] = np.stack(
+                    [adam_scalars(g["lr"], beta1, beta2, g["eps"], g["weight_decay"], t0 + s + 1) for s in range(steps)]
+                ) if steps else np.zeros((0, 8), dtype=np.float32)
+            out[:, r] = rows
+        return out
+
+    def advance(self, steps):
+        """Advance the ``step`` of every updated parameter by ``steps`` at once, as ``steps`` calls of :meth:`prepare`
+        do (the counts are integers, exact in the step tensors' dtype up to 2^24)."""
+        if self._steps and steps:
+            torch._foreach_add_(self._steps, torch.tensor(float(steps), device="cpu"), alpha=1.0)
+        self.opt._opt_called = True
 
     def launch(self):
         """Enqueue gr_grad_sumsq (with max_norm) and gr_clip_adam on the current stream."""

@@ -736,6 +736,14 @@ size_t gr_fact_weights_workspace_bytes(int64_t F, int64_t Nt);
 int gr_fact_weights(const void* heads, const void* rels, int idx_bytes, int64_t F, int64_t Nt, float* weight,
                     float* weight_rel, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
+/* gr_fact_weights_live: gr_fact_weights over the live prefix of capacity-length fact buffers, the live count read
+ * from the device: F = min(capacity, max(*nfacts, 0)) (nfacts: int32[1], as gr_csr_build reads it).  Slots
+ * [F, capacity) (a previous batch's facts) are neither counted nor flagged, and their weights are not written; the
+ * live prefix is bit-equal to gr_fact_weights over F facts.  Workspace: gr_fact_weights_workspace_bytes(capacity, Nt). */
+int gr_fact_weights_live(const void* heads, const void* rels, int idx_bytes, int64_t capacity, const int32_t* nfacts,
+                         int64_t Nt, float* weight, float* weight_rel, int32_t* status, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 /* Fact dropout on a resident split (loader.DeviceSplit with shuffle=True): the reference keeps the first
  * floor(n (1 - p)) facts of a fresh np.random.permutation of each question's n stored facts.  `kept` (int64 [B], from
  * the host) holds those counts; a count is clamped to [0, n] (n = 0 for an id out of range).
@@ -772,6 +780,31 @@ int gr_split_assemble_graft_ordered(const int64_t* g_off, const int32_t* g_e2f_f
                                     int idx_bytes, int64_t G, void* e2f_b, void* e2f_f, void* e2f_e, float* e2f_v,
                                     void* f2e_b, void* f2e_e, void* f2e_f, float* f2e_v, int64_t* kb_fact_rel,
                                     int32_t* status, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Step bookkeeping of a training epoch replayed as CUDA graphs (csrc/epoch.cu, graphed.GraphedTrainStep.start_epoch).
+ * cursor: int64[1] on the device, the step index c; step c covers positions [c * batch_size, min((c + 1) * batch_size,
+ * num_data)) of order (int64 [num_data], the epoch's question ids); B is that step's batch size.  One CTA each, no
+ * atomics.
+ *
+ * gr_epoch_step_begin: for j < B, id = order[c * batch_size + j] (-1 past num_data); an id outside [0, num_q) sets
+ *   status bit 1 and counts as an empty question.  ids[j] = id (for the gr_split_* kernels), rows[j] = id or 0 when
+ *   out of range (for row gathers), kept[j] = kept_table[id] clamped to [0, n] (n = the stored facts, q_off[id + 1] -
+ *   q_off[id]; kept_table NULL: n).  kept_total[0] = sum of kept; nfacts[0] = min(sum of kept + q_ents (with
+ *   use_self_loop), capacity); a sum past capacity sets status bit 2.  status[0] is written, not OR-ed.
+ * gr_epoch_step_record: with c in [0, steps): losses[c] = *loss, grad_norms[c] = *grad_norm and seeds[c] = *seed (both
+ *   optional, each with its record array), h1_all / f1_all[c * batch_size + j] = h1 / f1[j] for j < B (positions
+ *   below num_data).  epoch_status[0] |= *split_status, epoch_status[1] |= *csr_status; a cursor outside [0, steps)
+ *   records nothing and sets bit 2 of epoch_status[0].  Then cursor = c + 1. */
+int gr_epoch_step_begin(const int64_t* cursor, const int64_t* order, int64_t num_data, int64_t batch_size, int B,
+                        const int64_t* kept_table, const int64_t* q_off, const int32_t* q_ents, int64_t num_q,
+                        int use_self_loop, int64_t capacity, int64_t* ids, int64_t* rows, int64_t* kept,
+                        int32_t* nfacts, int64_t* kept_total, int32_t* status, void* stream);
+int gr_epoch_step_record(int64_t* cursor, int64_t steps, int64_t batch_size, int B, int64_t num_data,
+                         const float* loss, const float* grad_norm, const int64_t* seed, const float* h1,
+                         const float* f1, const int32_t* split_status, const int32_t* csr_status, float* losses,
+                         float* grad_norms, int64_t* seeds, float* h1_all, float* f1_all, int32_t* epoch_status,
+                         void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Shortest-path node sets (SURVEY.md 8f row 1): nodes lying on any shortest path between any seed and

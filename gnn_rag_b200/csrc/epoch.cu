@@ -5,6 +5,8 @@
 //
 //   gr_epoch_step_begin   at the head of the graph: the step's question ids, gather rows and kept counts, the live
 //                         fact count (`nfacts` of the CSR build) and the live kept total, from the cursor.
+//   gr_epoch_graft_begin  right after it, for GraftNet: the step's graft kept counts and the live graft count
+//                         (`live` of gr_graft_stage), from the ids gr_epoch_step_begin wrote.
 //   gr_epoch_step_record  at the tail: loss, gradient norm, fact-order seed, hit@1 and F1 stored at the cursor, the
 //                         step's status words OR-ed into the epoch's, the cursor advanced.
 //
@@ -69,6 +71,29 @@ epoch_step_begin_kernel(const int64_t* __restrict__ cursor, const int64_t* __res
 }
 
 __global__ void __launch_bounds__(kEpochThreads)
+epoch_graft_begin_kernel(const int64_t* __restrict__ ids, int B, const int64_t* __restrict__ kept_table,
+                         const int64_t* __restrict__ g_off, int64_t num_q, int64_t capacity,
+                         int64_t* __restrict__ kept_g, int32_t* __restrict__ graft_live, int32_t* __restrict__ status) {
+  __shared__ int64_t s_red[33];
+  int64_t sum_g = 0;
+  for (int j = threadIdx.x; j < B; j += blockDim.x) {
+    const int64_t id = ids[j];
+    const bool ok = id >= 0 && id < num_q;
+    const int64_t n = ok ? g_off[id + 1] - g_off[id] : 0;
+    const int64_t k = kept_table && ok ? min(max(kept_table[id], (int64_t)0), n) : n;
+    kept_g[j] = k;
+    sum_g += k;
+  }
+  sum_g = epoch_block_sum(sum_g, s_red);
+  if (threadIdx.x == 0) {
+    const int32_t live = (int32_t)min(sum_g, capacity);
+    graft_live[0] = live;
+    graft_live[1] = live;
+    *status = sum_g > capacity ? 2 : 0;
+  }
+}
+
+__global__ void __launch_bounds__(kEpochThreads)
 epoch_step_record_kernel(int64_t* __restrict__ cursor, int64_t steps, int64_t batch_size, int B, int64_t num_data,
                          const float* __restrict__ loss, const float* __restrict__ grad_norm,
                          const int64_t* __restrict__ seed, const float* __restrict__ h1, const float* __restrict__ f1,
@@ -117,6 +142,21 @@ extern "C" int gr_epoch_step_begin(const int64_t* cursor, const int64_t* order, 
   epoch_step_begin_kernel<<<1, kEpochThreads, 0, stream>>>(cursor, order, num_data, batch_size, B, kept_table, q_off,
                                                            q_ents, num_q, use_self_loop, capacity, ids, rows, kept,
                                                            nfacts, kept_total, status);
+  GR_CHECK_LAUNCH();
+  return GR_OK;
+}
+
+extern "C" int gr_epoch_graft_begin(const int64_t* ids, int B, const int64_t* kept_table, const int64_t* g_off,
+                                    int64_t num_q, int64_t capacity, int64_t* kept_g, int32_t* graft_live,
+                                    int32_t* status, void* stream_) {
+  using namespace gr;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  GR_CHECK_ARG(ids && g_off, "null pointer");
+  GR_CHECK_ARG(kept_g && graft_live && status, "null output");
+  GR_CHECK_ARG(B > 0 && num_q >= 0, "need B > 0 and num_q >= 0");
+  GR_CHECK_ARG(capacity >= 0 && capacity <= INT_MAX, "capacity must be in [0, INT_MAX]");
+  epoch_graft_begin_kernel<<<1, kEpochThreads, 0, stream>>>(ids, B, kept_table, g_off, num_q, capacity, kept_g,
+                                                            graft_live, status);
   GR_CHECK_LAUNCH();
   return GR_OK;
 }

@@ -27,9 +27,10 @@ Training: :class:`GraphedTrainStep` captures ``model(batch, training=True)`` + `
 metrics (gr_train_metrics) of ReaRev and NSM over the same input side, and :class:`GraphedGraftTrainStep` those of
 GraftNet over :class:`_GraftLayout` (the graft fact count stays on the device).  Given a ``torch.optim.Adam``, both
 also capture the gradient clipping and the optimizer step (:class:`optim.ClipAdam`); see their docstrings and DESIGN
-§4.11.  :meth:`GraphedTrainStep.train_epoch` runs a whole ReaRev / NSM epoch over a ``loader.DeviceSplit``: each step's
-graph also assembles its batch from a device cursor into the epoch's question order and records the step's loss and
-metrics on the device (csrc/epoch.cu), so the host only replays graphs and reads the device once per epoch.
+§4.11.  :meth:`GraphedTrainStep.train_epoch` runs a whole ReaRev / NSM epoch over a ``loader.DeviceSplit``, and
+:meth:`GraphedGraftTrainStep.train_epoch` a GraftNet one: each step's graph also assembles its batch (GraftNet: with
+its graft lists) from a device cursor into the epoch's question order and records the step's loss and metrics on the
+device (csrc/epoch.cu), so the host only replays graphs and reads the device once per epoch.
 """
 import collections
 import contextlib
@@ -541,16 +542,18 @@ class TrainStepOutput(tuple):
 class EpochPlan:
     """The host arithmetic of one epoch over a resident split (:func:`epoch_plan`): per step ``B`` (questions),
     ``F`` (live facts: kept facts + self-loops), ``K`` (kept facts) and ``capacity`` (``fact_capacity(F)``), int64
-    numpy arrays of ``steps`` entries, and ``starts``, the step's first position in the order."""
-    __slots__ = ("steps", "B", "F", "K", "capacity", "starts")
+    numpy arrays of ``steps`` entries, and ``starts``, the step's first position in the order.  With graft counts
+    also ``G`` (kept graft entries) and ``graft_capacity`` (``fact_capacity(G)``), else None."""
+    __slots__ = ("steps", "B", "F", "K", "capacity", "starts", "G", "graft_capacity")
 
 
-def epoch_plan(order, stored, ents, batch_size, fact_dropout=0.0):
+def epoch_plan(order, stored, ents, batch_size, fact_dropout=0.0, graft=None):
     """Per-step counts of an epoch that takes the questions ``order`` (ids, in batch order) ``batch_size`` at a time,
     the last batch short when ``len(order) % batch_size != 0``: what ``DeviceSplit.get_batch(it, batch_size,
     fact_dropout)`` computes on the host for each step, from the split's per-question stored fact counts ``stored``
-    and self-loop counts ``ents`` (zeros without ``use_self_loop``).  A question keeps ``loader.kept_counts`` of its
-    stored facts.  An id outside [0, len(stored)) counts as an empty question, as the device assembly counts it."""
+    and self-loop counts ``ents`` (zeros without ``use_self_loop``), and for GraftNet its stored graft entries per
+    question ``graft``.  A question keeps ``loader.kept_counts`` of its stored facts and of its graft entries.  An id
+    outside [0, len(stored)) counts as an empty question, as the device assembly counts it."""
     from .loader import kept_counts
     order = np.asarray(order, dtype=np.int64).reshape(-1)
     stored, ents = np.asarray(stored, dtype=np.int64), np.asarray(ents, dtype=np.int64)
@@ -560,15 +563,21 @@ def epoch_plan(order, stored, ents, batch_size, fact_dropout=0.0):
     plan.starts = np.arange(0, n, bs, dtype=np.int64)
     ok = (order >= 0) & (order < stored.size)
     q = np.where(ok, order, 0)
-    k = np.where(ok, kept_counts(stored[q] if stored.size else np.zeros(n, np.int64), fact_dropout), 0)
-    e = np.where(ok, ents[q] if ents.size else 0, 0)
-    if n:
-        plan.K = np.add.reduceat(k, plan.starts).astype(np.int64)
-        plan.F = plan.K + np.add.reduceat(e, plan.starts).astype(np.int64)
-    else:
-        plan.K = plan.F = np.zeros(0, dtype=np.int64)
+
+    def per_step(counts, keep):
+        """The sums over each step of ``counts`` per question of the order (their kept counts with ``keep``)."""
+        counts = np.asarray(counts, dtype=np.int64)
+        c = counts[q] if counts.size else np.zeros(n, np.int64)
+        c = np.where(ok, kept_counts(c, fact_dropout) if keep else c, 0)
+        return np.add.reduceat(c, plan.starts).astype(np.int64) if n else np.zeros(0, dtype=np.int64)
+    plan.K = per_step(stored, True)
+    plan.F = plan.K + per_step(ents, False)
     plan.B = np.minimum(bs, n - plan.starts).astype(np.int64)
     plan.capacity = np.array([fact_capacity(f) for f in plan.F.tolist()], dtype=np.int64)
+    plan.G = plan.graft_capacity = None
+    if graft is not None:
+        plan.G = per_step(graft, True)
+        plan.graft_capacity = np.array([fact_capacity(g) for g in plan.G.tolist()], dtype=np.int64)
     return plan
 
 
@@ -576,7 +585,8 @@ class EpochRun:
     """One epoch started by :meth:`GraphedTrainStep.start_epoch`: device tensors, valid once the current stream reaches
     them.  ``losses`` / ``grad_norms`` fp32 [steps] (``grad_norms`` None without ``max_norm``), ``h1`` / ``f1`` fp32
     [num_data] in batch order, ``seeds`` int64 [steps] (the fact-order seed of each step; None without ``shuffle``),
-    ``status`` int32 [2]: the OR of every step's batch-assembly status word and of its CSR build's.
+    ``status`` int32 [2]: the OR of every step's batch-assembly status word and of its CSR build's; for GraftNet int32
+    [3]: the assembly word (kb and graft sides), the CSR word (kb and graft CSR builds) and the graft staging word.
     :meth:`result` reads them back in one copy; :meth:`check` raises for a nonzero status."""
 
     def __init__(self, losses, grad_norms, h1, f1, seeds, status):
@@ -593,19 +603,22 @@ class EpochRun:
         return np.mean(host[:n].tolist()), [0, 0], host[n:n + m].tolist(), host[n + m:n + 2 * m].tolist()
 
     def check(self):
-        """Raise ``DeviceSplit.check``'s message when an assembly flagged an id out of range or an overflow, else
-        ``TrainStepOutput.check``'s when a CSR build flagged ids outside the batch (reads the status unless
-        :meth:`result` has)."""
+        """Raise ``DeviceSplit.check``'s message when an assembly flagged an id out of range or an overflow, else (for
+        GraftNet) ``GraftGraph``'s when the graft staging rejected a list, else ``TrainStepOutput.check``'s when a CSR
+        build flagged ids outside the batch (reads the status unless :meth:`result` has)."""
         from .loader import DeviceSplit
-        split_word, csr_word = self._words if self._words is not None else self.status.tolist()
-        DeviceSplit.raise_status(split_word)
-        if csr_word:
-            _KbLayout.raise_for([csr_word])
+        words = self._words if self._words is not None else self.status.tolist()
+        DeviceSplit.raise_status(words[0])
+        if len(words) > 2:
+            ops.GraftGraph.raise_status(words[2])
+        if words[1]:
+            _KbLayout.raise_for([words[1]])
 
 
 class _EpochBuffers:
     """The device state the epoch graphs of one (split, batch size) read and write: the cursor, the question order,
-    the kept-count table, the records and the per-step Adam scalars.  Fixed addresses: the graphs hold them."""
+    the kept-count tables (GraftNet: also the graft entries'), the records and the per-step Adam scalars.  Fixed
+    addresses: the graphs hold them."""
 
     def __init__(self, split, batch_size, max_norm):
         dev = split.device
@@ -621,10 +634,17 @@ class _EpochBuffers:
         self.seeds = torch.zeros(self.steps, **i64) if split.shuffle else None
         self.h1 = torch.zeros(self.num_data, **f32)
         self.f1 = torch.zeros(self.num_data, **f32)
-        self.status = torch.zeros(2, dtype=torch.int32, device=dev)
+        self.status = torch.zeros(3 if split.graft else 2, dtype=torch.int32, device=dev)
         self.adam = None                 # fp32 [steps, T, 8], made at the first capture (T is known then)
-        # the fact-order workspace of any batch: the stored facts of the batch_size largest questions
-        self.n_total = int(np.sort(split._stored)[-self.batch_size:].sum()) if split._stored.size else 0
+
+        def largest(counts):             # the stored entries of the batch_size largest questions
+            return int(np.sort(counts)[-self.batch_size:].sum()) if counts.size else 0
+        # the fact-order workspaces of any batch
+        self.n_total = largest(split._stored)
+        self.graft_kept_table = self.graft_n_total = None
+        if split.graft:
+            self.graft_kept_table = torch.zeros(max(split.num_q, 1), **i64) if split.shuffle else None
+            self.graft_n_total = largest(split._graft_count)
 
 
 def _release_autograd_history(model):
@@ -873,11 +893,13 @@ class GraphedTrainStep:
         from .loader import DeviceSplit, same_device
         if self.optimizer is None:
             return "an epoch steps the optimizer in its graphs: build the step with optimizer="
-        if isinstance(self._layout, _GraftLayout):
-            return "train_epoch covers ReaRev and NSM; GraftNet's epoch runs step by step (GraphedGraftTrainStep.step)"
         if not isinstance(split, DeviceSplit):
             return "train_epoch takes a loader.DeviceSplit, got %s" % type(split).__name__
-        if split.graft:
+        graft_step = isinstance(self._layout, _GraftLayout)
+        if graft_step and not split.graft:
+            return ("GraphedGraftTrainStep.train_epoch takes a GraftNet split; this DeviceSplit holds no graft lists "
+                    "(GraphedTrainStep.train_epoch covers ReaRev and NSM)")
+        if split.graft and not graft_step:
             return "train_epoch takes a ReaRev / NSM split; this DeviceSplit holds GraftNet's graft lists"
         if not same_device(split.device, self.device):
             return "the split lives on %s, the model on %s" % (split.device, self.device)
@@ -911,9 +933,10 @@ class GraphedTrainStep:
 
         Afterwards ``p.grad``, the parameters and the Adam state are those of the loop ``get_batch`` + :meth:`step`,
         the CPU ``step`` tensors advanced by the number of steps, and ``split.loader.sample_ids`` is the last batch's.
-        Refused (``ValueError``): a step without ``optimizer``, GraftNet, anything but a CUDA ``DeviceSplit`` of a kb
-        loader on the model's device, ``batch_size <= 0``, a ``fact_dropout`` ``get_batch`` refuses, and fact weights
-        (``normalized_gnn`` / ``norm_rel``) over a ``weights="none"`` split."""
+        Refused (``ValueError``): a step without ``optimizer``, anything but a CUDA ``DeviceSplit`` of a kb loader on
+        the model's device (GraftNet's epoch is :meth:`GraphedGraftTrainStep.start_epoch`), ``batch_size <= 0``, a
+        ``fact_dropout`` ``get_batch`` refuses, and fact weights (``normalized_gnn`` / ``norm_rel``) over a
+        ``weights="none"`` split."""
         why = self._epoch_refusal(split, batch_size, fact_dropout)
         if why is not None:
             raise ValueError("train_epoch: " + why)
@@ -921,7 +944,8 @@ class GraphedTrainStep:
         split.reset_batches(is_sequential=False)
         L = split.loader
         order = np.asarray(L.batches[:L.num_data], dtype=np.int64).reshape(-1)
-        plan = epoch_plan(order, split._stored, split._ents, batch_size, fact_dropout if split.shuffle else 0.0)
+        p = fact_dropout if split.shuffle else 0.0
+        plan = epoch_plan(order, split._stored, split._ents, batch_size, p, split._graft_count if split.graft else None)
         if split.index_dtype == torch.int32 and plan.steps and (
                 int(plan.B.max()) * split.N > _INT32_MAX or int(plan.F.max()) > _INT32_MAX):
             raise ValueError("train_epoch: a batch overflows int32 indices; use index_dtype=torch.int64")
@@ -931,6 +955,9 @@ class GraphedTrainStep:
             from .loader import kept_counts
             ep.kept_table[:split.num_q].copy_(torch.from_numpy(kept_counts(split._stored, fact_dropout)),
                                               non_blocking=True)
+            if ep.graft_kept_table is not None:
+                ep.graft_kept_table[:split.num_q].copy_(
+                    torch.from_numpy(kept_counts(split._graft_count, fact_dropout)), non_blocking=True)
         entries = self._epoch_entries(ep, plan)
         fused = entries[0].fused if entries else None
         if fused is not None and plan.steps:
@@ -962,42 +989,71 @@ class GraphedTrainStep:
         shape = (B, split.N, cap, int(split._res["q_input"].shape[1]), split.index_dtype)
         return shape + self._state_key() + ("epoch", id(ep))
 
+    @staticmethod
+    def _epoch_shapes(plan):
+        """The graph shape of every step of ``plan``: (B, fact capacity)."""
+        return list(zip(plan.B.tolist(), plan.capacity.tolist()))
+
     def _epoch_entries(self, ep, plan):
         """The graph of every step of ``plan`` (a list), capturing the missing ones first."""
+        steps = self._epoch_shapes(plan)
         shapes = {}
-        for s, (B, cap) in enumerate(zip(plan.B.tolist(), plan.capacity.tolist())):
-            shapes.setdefault((B, cap), s)
+        for s, shape in enumerate(steps):
+            shapes.setdefault(shape, s)
         self.max_graphs = max(self.max_graphs, len(shapes))
-        for (B, cap), s in shapes.items():
-            key = self._epoch_key(ep, B, cap)
+        for shape, s in shapes.items():
+            key = self._epoch_key(ep, *shape)
             if key in self._cache:
                 self._cache.move_to_end(key)
             else:
-                self._epoch_capture(ep, B, cap, s)
+                self._epoch_capture(ep, shape, s)
         # a capture may create Adam state, which the keys hold: resolve them once all graphs exist
         ents = {shape: self._cache[self._epoch_key(ep, *shape)] for shape in shapes}
         layouts = {ent.fused.layout() for ent in ents.values() if ent.fused is not None}
         if len(layouts) > 1:
             raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
-        return [ents[shape] for shape in zip(plan.B.tolist(), plan.capacity.tolist())]
+        return [ents[shape] for shape in steps]
 
-    def _epoch_body(self, ep, st, cursor, ac):
-        """One step of the epoch over the static buffers ``st``: the head kernel, the batch assembly into ``st`` and
-        the captured step of :meth:`_run` -> (outs of _run, seed or None, the assembly status word)."""
+    def _epoch_static(self, key):
+        """The static buffers of an epoch graph: the layout's, plus the head's outputs."""
+        st = self._layout.static_inputs(key)
+        B, dev = key[0], self.device
+        st.ids, st.rows, st.kept = (torch.zeros(B, dtype=torch.int64, device=dev) for _ in range(3))
+        st.kept_total = torch.zeros(1, dtype=torch.int64, device=dev)
+        st.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        return st
+
+    def _epoch_begin(self, ep, st, cursor):
+        """The head kernel of an epoch step: the step's ids, rows and counts into ``st``."""
         split = ep.split
         r = split._res
-        cap = st.heads.numel()
         ops.epoch_step_begin(cursor, ep.order, ep.batch_size, ep.kept_table, r["q_off"], r["q_ents"],
-                             split.use_self_loop, cap, st.ids, st.rows, st.kept, st.nfacts, st.kept_total, st.status)
+                             split.use_self_loop, st.heads.numel(), st.ids, st.rows, st.kept, st.nfacts, st.kept_total,
+                             st.status)
+
+    def _epoch_head(self, ep, st, cursor):
+        """The head kernels, the fact-order seed and the kb half of the batch assembly into ``st`` -> (seed or None,
+        the assembly status word)."""
+        split = ep.split
+        cap = st.heads.numel()
+        self._epoch_begin(ep, st, cursor)
         seed = torch.randint(0, 2 ** 62, (1,), device=self.device) if split.shuffle else None
         _rows, _kb, _order, asm = split.assemble(st.ids, st.kept, seed, cap, cap, ep.n_total, rows=st.rows, out=st,
                                                  nfacts=st.nfacts)
-        return self._run(st, ac), seed, st.status | asm
+        return seed, st.status | asm
 
-    def _epoch_capture(self, ep, B, cap, s0):
-        """Capture the epoch graph of batches of B questions at fact capacity ``cap``; ``s0``: a step of the epoch with
-        that shape, the one the warm-up assembles."""
-        key = self._epoch_key(ep, B, cap)
+    def _epoch_body(self, ep, st, cursor, ac):
+        """One step of the epoch over the static buffers ``st``: the head kernel, the batch assembly into ``st`` and
+        the captured step of :meth:`_run` -> (outs of _run, seed or None, the step's words of ``EpochRun.status``:
+        assembly, CSR)."""
+        seed, asm = self._epoch_head(ep, st, cursor)
+        outs = self._run(st, ac)
+        return outs, seed, [asm, outs[5]]
+
+    def _epoch_capture(self, ep, shape, s0):
+        """Capture the epoch graph of ``shape`` (:meth:`_epoch_shapes`: B questions, the fact capacity and, for
+        GraftNet, the graft capacity); ``s0``: a step of the epoch with that shape, the one the warm-up assembles."""
+        key = self._epoch_key(ep, *shape)
         split = ep.split
         why = self.refusal(key[3])
         if why is not None:
@@ -1007,11 +1063,8 @@ class GraphedTrainStep:
             torch.cuda.synchronize()
             del old
         ac = _autocast_dtype()
-        st = self._layout.static_inputs(key)
+        st = self._epoch_static(key)
         dev = self.device
-        st.ids, st.rows, st.kept = (torch.zeros(B, dtype=torch.int64, device=dev) for _ in range(3))
-        st.kept_total = torch.zeros(1, dtype=torch.int64, device=dev)
-        st.status = torch.zeros(1, dtype=torch.int32, device=dev)
         params = [p for p in self._params if p.requires_grad]
         torch.cuda.synchronize()
         rng = torch.cuda.get_rng_state(dev)
@@ -1033,7 +1086,7 @@ class GraphedTrainStep:
             ep.adam = torch.zeros(ep.steps, T, 8, dtype=torch.float32, device=dev)
         elif ep.adam.shape[1] != T:
             raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
-        key = self._epoch_key(ep, B, cap)
+        key = self._epoch_key(ep, *shape)
         _release_autograd_history(self.model)
         for p in params:
             p.grad = None
@@ -1042,12 +1095,15 @@ class GraphedTrainStep:
         gc.disable()
         try:
             with torch.cuda.graph(g):
-                outs, seed, split_word = self._epoch_body(ep, st, ep.cursor, ac)
+                outs, seed, words = self._epoch_body(ep, st, ep.cursor, ac)
                 torch.index_select(ep.adam, 0, ep.cursor, out=fused._scalars.view(1, T, 8))
                 fused.launch()
-                loss, _pred, _pd, h1, f1, csr = outs
+                loss, _pred, _pd, h1, f1, _words = outs
+                if len(words) > 2:               # GraftNet's graft staging word
+                    ep.status[2:].bitwise_or_(words[2])
                 ops.epoch_step_record(ep.cursor, ep.batch_size, ep.num_data, loss.float(), fused.grad_norm, seed, h1,
-                                      f1, split_word, csr, ep.losses, ep.grad_norms, ep.seeds, ep.h1, ep.f1, ep.status)
+                                      f1, words[0], words[1], ep.losses, ep.grad_norms, ep.seeds, ep.h1, ep.f1,
+                                      ep.status[:2])
         finally:
             if gc_on:
                 gc.enable()
@@ -1102,6 +1158,76 @@ class GraphedGraftTrainStep(GraphedTrainStep):
             return ("_fact_kernels is false: entity_dim %d is outside the GraftNet training kernels (%s)"
                     % (D, ops.fact_train_ok.__doc__.split(": ", 1)[1].rstrip(".")))
         return None
+
+    # -- a whole epoch -----------------------------------------------------------------------------------------------
+    def train_epoch(self, split, batch_size, fact_dropout):
+        """The reference's ``Trainer_KBQA.train_epoch`` around GraftNet, over the resident GraftNet split ``split``:
+        one :meth:`start_epoch`, one read.  -> ``(np.mean(losses), [0, 0], h1_list_all, f1_list_all)``.  Raises
+        :meth:`EpochRun.check`'s errors after the epoch when a batch was malformed."""
+        return super().train_epoch(split, batch_size, fact_dropout)
+
+    def start_epoch(self, split, batch_size, fact_dropout):
+        """Start one GraftNet training epoch over ``split`` (a ``loader.DeviceSplit`` of a GraftNet loader) and return
+        its :class:`EpochRun` without waiting for the device.
+
+        As the reference's ``train_epoch``: ``model.train()``, ``split.reset_batches(is_sequential=False)`` (the
+        loader's ``np.random`` order), then every batch of ``batch_size`` questions in order, the last one short when
+        ``num_data % batch_size != 0``, each assembled as ``split.get_batch(it, batch_size, fact_dropout)`` does,
+        trained and stepped.  Each step is one graph replay: the graph assembles the batch on the device from a
+        cursor into the epoch's question order (gr_epoch_step_begin and gr_epoch_graft_begin, then
+        ``DeviceSplit.assemble`` at the bucket's fact capacity and ``DeviceSplit.assemble_graft`` at its graft
+        capacity, both fact orders drawn from one seed taken from torch's CUDA generator with ``shuffle``), runs the
+        step of :meth:`step` with the step's Adam scalars (all uploaded at the start of the epoch), then records loss,
+        gradient norm, seed, hit@1 and F1 at the cursor and advances it (gr_epoch_step_record).  The host picks each
+        step's graph, one per (B, fact capacity, graft capacity), from :func:`epoch_plan`; the graphs the epoch needs
+        and does not hold yet are captured before the first replay (the LRU grows to hold them all), without moving
+        the records, the parameters or torch's generator.  ``EpochRun.status`` has three words: assembly, CSR and
+        graft staging.
+
+        Afterwards ``p.grad``, the parameters and the Adam state are those of the loop ``get_batch`` + :meth:`step`,
+        the CPU ``step`` tensors advanced by the number of steps, and ``split.loader.sample_ids`` is the last batch's.
+        Refused (``ValueError``): a step without ``optimizer``, anything but a CUDA ``DeviceSplit`` of a GraftNet loader
+        on the model's device, ``batch_size <= 0``, a ``fact_dropout`` ``get_batch`` refuses, and fact weights
+        (``norm_rel``) over a ``weights="none"`` split."""
+        return super().start_epoch(split, batch_size, fact_dropout)
+
+    def _epoch_key(self, ep, B, cap, gcap):
+        split = ep.split
+        layer = self.model.reasoning
+        shape = (B, split.N, cap, int(split._res["q_input"].shape[1]), split.index_dtype, gcap, split.max_facts)
+        return (shape + self._state_key() + (float(layer.pagerank_lambda), float(layer.fact_scale))
+                + ("epoch", id(ep)))
+
+    @staticmethod
+    def _epoch_shapes(plan):
+        """The graph shape of every step of ``plan``: (B, fact capacity, graft capacity)."""
+        return list(zip(plan.B.tolist(), plan.capacity.tolist(), plan.graft_capacity.tolist()))
+
+    def _epoch_static(self, key):
+        st = super()._epoch_static(key)
+        B, gcap, dev = key[0], key[5], self.device
+        st.kept_g = torch.zeros(B, dtype=torch.int64, device=dev)
+        st.graft_status = torch.zeros(1, dtype=torch.int32, device=dev)
+        # the graft assembly writes the lists' values (all 1.0); GraftNet's training forward never reads them
+        st.e2f_v, st.f2e_v = (torch.zeros(gcap, dtype=torch.float32, device=dev) for _ in range(2))
+        return st
+
+    def _epoch_begin(self, ep, st, cursor):
+        super()._epoch_begin(ep, st, cursor)
+        ops.epoch_graft_begin(st.ids, ep.graft_kept_table, ep.split._res["g_off"], st.e2f_b.numel(), st.kept_g,
+                              st.graft_live, st.graft_status)
+
+    def _epoch_body(self, ep, st, cursor, ac):
+        """:meth:`GraphedTrainStep._epoch_body` with the graft half of the head (gr_epoch_graft_begin) and of the
+        assembly (the graft lists at their capacity and ``kb_fact_rel``) -> words: assembly, CSR, graft staging."""
+        split = ep.split
+        gcap = st.e2f_b.numel()
+        seed, asm = self._epoch_head(ep, st, cursor)
+        out = ((st.e2f_b, st.e2f_f, st.e2f_e, st.e2f_v), (st.f2e_b, st.f2e_e, st.f2e_f, st.f2e_v), st.kb_fact_rel)
+        _graft, _kfr, _order, gasm = split.assemble_graft(st.ids, st.kept_g, seed, gcap, ep.graft_n_total, out=out)
+        outs = self._run(st, ac)
+        csr, staging, graft_csr = outs[5][0:1], outs[5][1:2], outs[5][2:3]
+        return outs, seed, [asm | st.graft_status | gasm, csr | graft_csr, staging]
 
     def _forward(self, st):
         m = self.model

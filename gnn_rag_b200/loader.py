@@ -461,12 +461,35 @@ class DeviceSplit:
                 w, wr = (torch.empty(0, dtype=torch.float32, device=self.device) for _ in range(2))
         return gathered, (*kb, w, wr), order, status
 
+    def assemble_graft(self, ids, kept_g, seed, G, n_total, out=None):
+        """The device part of :meth:`get_batch` for GraftNet's graft side of B > 0 questions: the graft order (with
+        ``shuffle``, from the same ``seed`` as the kb facts' order, as a second permutation) and the assembly of both
+        graft lists and of ``kb_fact_rel``.
+
+        ``ids`` / ``kept_g`` int64 [B] and ``seed`` int64 [1] on the device (``kept_g``, the graft entries each
+        question keeps, and ``seed`` only read with ``shuffle``).  ``G``: the length of the lists and of the order,
+        ``n_total`` >= the stored graft entries of the B questions (host ints).  ``out``: ``((e2f_b, e2f_f, e2f_e,
+        e2f_v), (f2e_b, f2e_e, f2e_f, f2e_v), kb_fact_rel)`` written in place (G their capacity, the index dtype
+        theirs: the live entries at the front, a batch past G cut there and flagged); without it new tensors of G
+        entries in ``index_dtype``.  Launch shapes and sizes come from these arguments alone, so a CUDA graph can
+        capture the call.  -> (graft lists, kb_fact_rel, order (None without shuffle), status int32[1])."""
+        from . import ops
+        r = self._res
+        lists = (r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"])
+        idt = None if out is not None else self.index_dtype
+        if self.shuffle:
+            order, ost = ops.split_fact_order(r["g_off"], ids, kept_g, seed, 1, n_total, G)
+            graft, kfr, status = ops.split_assemble_graft_ordered(*lists, ids, kept_g, order, self.max_facts,
+                                                                  self.rel_pad, G, idt, out=out)
+            return graft, kfr, order, status | ost
+        graft, kfr, status = ops.split_assemble_graft(*lists, ids, self.max_facts, self.rel_pad, G, idt, out=out)
+        return graft, kfr, None, status
+
     def get_batch(self, iteration, batch_size, fact_dropout, q_type=None, test=False, seed=None):
         """The loader's ``get_batch`` from the resident split (see the class docstring).  ``seed``: with ``shuffle``,
         the fact-order seed to use (int64 [1] on the device, e.g. a seed an epoch recorded) instead of one drawn from
         torch's CUDA generator."""
         import torch
-        from . import ops
         L, r, dev = self.loader, self._res, self.device
         if not self.shuffle and fact_dropout != 0:
             raise ValueError("DeviceSplit.get_batch: fact_dropout must be 0 (facts come in stored order), got %r"
@@ -526,19 +549,12 @@ class DeviceSplit:
         G = int(kept_g.sum()) if self.shuffle else int(self._graft_count[ids].sum())
         if idt == torch.int32 and G > _INT32_MAX:
             raise ValueError("DeviceSplit.get_batch: the graft lists overflow int32 indices (%d entries)" % G)
-        if B and self.shuffle:
-            gorder, ost = ops.split_fact_order(r["g_off"], ids_dev, kept_g_dev, seed, 1,
-                                               int(self._graft_count[ids].sum()), G)
-            graft, kfr, gst = ops.split_assemble_graft_ordered(
-                r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"], ids_dev,
-                kept_g_dev, gorder, self.max_facts, self.rel_pad, G, idt)
-            self.status = self.status | gst | ost
-            self.last_order.update(graft=gorder, graft_offsets=np.concatenate([[0], np.cumsum(kept_g)]))
-        elif B:
-            graft, kfr, gst = ops.split_assemble_graft(
-                r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"], ids_dev,
-                self.max_facts, self.rel_pad, G, idt)
+        if B:
+            graft, kfr, gorder, gst = self.assemble_graft(ids_dev, kept_g_dev if self.shuffle else None, seed, G,
+                                                          int(self._graft_count[ids].sum()))
             self.status = self.status | gst
+            if self.shuffle:
+                self.last_order.update(graft=gorder, graft_offsets=np.concatenate([[0], np.cumsum(kept_g)]))
         else:
             e = lambda dt: torch.empty(0, dtype=dt, device=dev)       # noqa: E731
             graft = ((e(idt), e(idt), e(idt), e(torch.float32)), (e(idt), e(idt), e(idt), e(torch.float32)))

@@ -1053,25 +1053,60 @@ def split_assemble_graft_ok(B, max_facts, G, index_dtype):
     return index_dtype == torch.int64 or (G <= _INT32_MAX and max_facts <= _INT32_MAX)
 
 
+def _graft_out(fn, out, B, max_facts, G, index_dtype, dev):
+    """(the six [G] index lists, the two fp32 [G] value lists, kb_fact_rel int64 [B, max_facts]) of a graft assembly:
+    the tensors of ``out`` = ((e2f_b, e2f_f, e2f_e, e2f_v), (f2e_b, f2e_e, f2e_f, f2e_v), kb_fact_rel), checked, or
+    new ones without it."""
+    if out is None:
+        idx = [torch.empty(G, dtype=index_dtype, device=dev) for _ in range(6)]
+        vals = [torch.empty(G, dtype=torch.float32, device=dev) for _ in range(2)]
+        return idx, vals, torch.empty(B, max_facts, dtype=torch.int64, device=dev)
+    (e2f, f2e), kfr = out[:2], out[2]
+    idx, vals = [*e2f[:3], *f2e[:3]], [e2f[3], f2e[3]]
+    for i, t in enumerate(idx):
+        if not (t.is_cuda and t.dtype == index_dtype and t.is_contiguous() and t.numel() == G):
+            raise RuntimeError("%s: out index list %d must be a contiguous %s [%d] CUDA tensor"
+                               % (fn, i, index_dtype, G))
+    for i, t in enumerate(vals):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == G):
+            raise RuntimeError("%s: out value list %d must be a contiguous fp32 [%d] CUDA tensor" % (fn, i, G))
+    if not (kfr.is_cuda and kfr.dtype == torch.int64 and kfr.is_contiguous() and tuple(kfr.shape) == (B, max_facts)):
+        raise RuntimeError("%s: out kb_fact_rel must be a contiguous int64 [%d, %d] CUDA tensor" % (fn, B, max_facts))
+    return idx, vals, kfr
+
+
+def _graft_index_dtype(fn, out, index_dtype):
+    """The index dtype of a graft assembly: ``out``'s (its six index lists share one), else ``index_dtype``."""
+    if out is None:
+        return index_dtype
+    dts = {t.dtype for t in (*out[0][:3], *out[1][:3])}
+    if len(dts) != 1 or (index_dtype is not None and dts != {index_dtype}):
+        raise RuntimeError("%s: the out index lists must share one dtype%s, got %s"
+                           % (fn, "" if index_dtype is None else " (%s)" % index_dtype, sorted(map(str, dts))))
+    return dts.pop()
+
+
 def split_assemble_graft(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, ids, max_facts, rel_pad, G,
-                         index_dtype):
+                         index_dtype=None, out=None):
     """-> ((e2f_b, e2f_f, e2f_e, e2f_v), (f2e_b, f2e_e, f2e_f, f2e_v)), kb_fact_rel, status: the graft lists ([G], the
     index entries in ``index_dtype``, the values fp32 1.0) and kb_fact_rel int64 [B, max_facts] of the questions
-    ``ids`` of a resident split (gr_split_assemble_graft); ``status`` as :func:`split_assemble`."""
+    ``ids`` of a resident split (gr_split_assemble_graft); ``status`` as :func:`split_assemble`.  ``out``: optional
+    tensors in the layout returned, ``((e2f_b, e2f_f, e2f_e, e2f_v), (f2e_b, f2e_e, f2e_f, f2e_v), kb_fact_rel)``,
+    written in place of new ones; the index dtype is then theirs, and G their length (a capacity: the batch's entries
+    fill the front, and entries past G are not written and set status bit 2)."""
     g_off, r_off = _cuda(g_off, torch.int64, "g_off").contiguous(), _cuda(r_off, torch.int64, "r_off").contiguous()
     lists = [_cuda(t, torch.int32, n).contiguous() for t, n in
              ((g_e2f_f, "g_e2f_f"), (g_e2f_e, "g_e2f_e"), (g_f2e_e, "g_f2e_e"), (g_f2e_f, "g_f2e_f"),
               (r_vals, "r_vals"))]
     ids = _cuda(ids, torch.int64, "ids").contiguous()
     B, num_q = ids.numel(), g_off.numel() - 1
+    index_dtype = _graft_index_dtype("split_assemble_graft", out, index_dtype)
     if not split_assemble_graft_ok(B, max_facts, G, index_dtype):
         raise RuntimeError("split_assemble_graft: need B > 0, max_facts >= 0, G >= 0 and an int32 / int64 index dtype "
                            "whose range holds G and max_facts, got B=%d max_facts=%d G=%d %s"
                            % (B, max_facts, G, index_dtype))
     dev = ids.device
-    idx = [torch.empty(G, dtype=index_dtype, device=dev) for _ in range(6)]
-    vals = [torch.empty(G, dtype=torch.float32, device=dev) for _ in range(2)]
-    kfr = torch.empty(B, max_facts, dtype=torch.int64, device=dev)
+    idx, vals, kfr = _graft_out("split_assemble_graft", out, B, max_facts, G, index_dtype, dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
     p = (lambda t: _p(t) if t.numel() else None)     # noqa: E731
     _launch("gr_split_assemble_graft", _p(g_off), *(_p(t) for t in lists[:4]), _p(r_off), _p(lists[4]), num_q,
@@ -1133,10 +1168,10 @@ def split_assemble_ordered(q_off, q_heads, q_rels, q_tails, q_ents, ids, kept, o
 
 
 def split_assemble_graft_ordered(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, ids, kept, order,
-                                 max_facts, rel_pad, G, index_dtype):
+                                 max_facts, rel_pad, G, index_dtype=None, out=None):
     """:func:`split_assemble_graft` with both graft lists taking question b's entries at its ``kept[b]`` positions of
     ``order`` (gr_split_assemble_graft_ordered); the kb_fact_rel rows are the stored ones.  Shape rule:
-    :func:`split_assemble_graft_ok`."""
+    :func:`split_assemble_graft_ok`; ``out`` as there."""
     g_off, r_off = _cuda(g_off, torch.int64, "g_off").contiguous(), _cuda(r_off, torch.int64, "r_off").contiguous()
     lists = [_cuda(t, torch.int32, n).contiguous() for t, n in
              ((g_e2f_f, "g_e2f_f"), (g_e2f_e, "g_e2f_e"), (g_f2e_e, "g_f2e_e"), (g_f2e_f, "g_f2e_f"),
@@ -1144,14 +1179,13 @@ def split_assemble_graft_ordered(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_of
     ids, kept = _cuda(ids, torch.int64, "ids").contiguous(), _cuda(kept, torch.int64, "kept").contiguous()
     order = _cuda(order, torch.int32, "order").contiguous()
     B, num_q, K = ids.numel(), g_off.numel() - 1, order.numel()
+    index_dtype = _graft_index_dtype("split_assemble_graft_ordered", out, index_dtype)
     if not split_assemble_graft_ok(B, max_facts, G, index_dtype) or kept.numel() != B:
         raise RuntimeError("split_assemble_graft_ordered: need B > 0, kept [B], max_facts >= 0, G >= 0 and an int32 / "
                            "int64 index dtype whose range holds G and max_facts, got B=%d max_facts=%d G=%d %s"
                            % (B, max_facts, G, index_dtype))
     dev = ids.device
-    idx = [torch.empty(G, dtype=index_dtype, device=dev) for _ in range(6)]
-    vals = [torch.empty(G, dtype=torch.float32, device=dev) for _ in range(2)]
-    kfr = torch.empty(B, max_facts, dtype=torch.int64, device=dev)
+    idx, vals, kfr = _graft_out("split_assemble_graft_ordered", out, B, max_facts, G, index_dtype, dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
     p = (lambda t: _p(t) if t.numel() else None)     # noqa: E731
     _launch("gr_split_assemble_graft_ordered", _p(g_off), *(_p(t) for t in lists[:4]), _p(r_off), _p(lists[4]),
@@ -1233,6 +1267,23 @@ def epoch_step_begin(cursor, order, batch_size, kept_table, q_off, q_ents, use_s
     _launch("gr_epoch_step_begin", _p(cursor), _p(order), order.numel(), int(batch_size), B, _p(kept_table),
             _p(q_off), _p(q_ents), q_ents.numel(), int(bool(use_self_loop)), int(capacity), _p(ids), _p(rows),
             _p(kept), _p(nfacts), _p(kept_total), _p(status), op="split_assemble")
+
+
+def epoch_graft_begin(ids, kept_table, g_off, capacity, kept_g, graft_live, status):
+    """GraftNet's half of the head of a graphed epoch step (gr_epoch_graft_begin), after :func:`epoch_step_begin` and
+    from the ``ids`` (int64 [B]) it wrote: the graft kept counts ``kept_g`` (int64 [B]), ``graft_live`` (int32[2], both
+    the live graft count clamped to ``capacity``) and ``status`` (int32[1]; bit 2: more entries than ``capacity``),
+    all written in place.  ``kept_table``: int64 [num_q] kept counts, or None for every stored entry; ``g_off`` int64
+    [num_q+1]."""
+    B = ids.numel()
+    for name, t, dt, n in (("ids", ids, torch.int64, B), ("kept_table", kept_table, torch.int64, None),
+                           ("g_off", g_off, torch.int64, None), ("kept_g", kept_g, torch.int64, B),
+                           ("graft_live", graft_live, torch.int32, 2), ("status", status, torch.int32, 1)):
+        if t is not None and (not t.is_contiguous() or (n is not None and t.numel() != n)):
+            raise RuntimeError("epoch_graft_begin: %s must be contiguous%s" % (name, "" if n is None else " [%d]" % n))
+        _cuda(t, dt, name)
+    _launch("gr_epoch_graft_begin", _p(ids), B, _p(kept_table), _p(g_off), g_off.numel() - 1, int(capacity),
+            _p(kept_g), _p(graft_live), _p(status), op="split_assemble")
 
 
 def epoch_step_record(cursor, batch_size, num_data, loss, grad_norm, seed, h1, f1, split_status, csr_status, losses,

@@ -792,6 +792,11 @@ int gr_split_assemble_graft_ordered(const int64_t* g_off, const int32_t* g_e2f_f
  *   out of range (for row gathers), kept[j] = kept_table[id] clamped to [0, n] (n = the stored facts, q_off[id + 1] -
  *   q_off[id]; kept_table NULL: n).  kept_total[0] = sum of kept; nfacts[0] = min(sum of kept + q_ents (with
  *   use_self_loop), capacity); a sum past capacity sets status bit 2.  status[0] is written, not OR-ed.
+ * gr_epoch_graft_begin: GraftNet's half of the head, after gr_epoch_step_begin, from the ids it wrote (int64 [B]): for
+ *   j < B, kept_g[j] = kept_table[ids[j]] clamped to [0, n] (n = the stored graft entries, g_off[id + 1] - g_off[id];
+ *   kept_table NULL: n; an id outside [0, num_q) counts as an empty question, n = 0).  graft_live[0] = graft_live[1]
+ *   = min(G, capacity) with G the sum of kept_g (the `live` gr_graft_stage reads); status[0] = 2 when G > capacity,
+ *   else 0 (written, not OR-ed).  g_off: int64 [num_q+1]; kept_table: int64 [num_q] or NULL.
  * gr_epoch_step_record: with c in [0, steps): losses[c] = *loss, grad_norms[c] = *grad_norm and seeds[c] = *seed (both
  *   optional, each with its record array), h1_all / f1_all[c * batch_size + j] = h1 / f1[j] for j < B (positions
  *   below num_data).  epoch_status[0] |= *split_status, epoch_status[1] |= *csr_status; a cursor outside [0, steps)
@@ -800,6 +805,8 @@ int gr_epoch_step_begin(const int64_t* cursor, const int64_t* order, int64_t num
                         const int64_t* kept_table, const int64_t* q_off, const int32_t* q_ents, int64_t num_q,
                         int use_self_loop, int64_t capacity, int64_t* ids, int64_t* rows, int64_t* kept,
                         int32_t* nfacts, int64_t* kept_total, int32_t* status, void* stream);
+int gr_epoch_graft_begin(const int64_t* ids, int B, const int64_t* kept_table, const int64_t* g_off, int64_t num_q,
+                         int64_t capacity, int64_t* kept_g, int32_t* graft_live, int32_t* status, void* stream);
 int gr_epoch_step_record(int64_t* cursor, int64_t steps, int64_t batch_size, int B, int64_t num_data,
                          const float* loss, const float* grad_norm, const int64_t* seed, const float* h1,
                          const float* f1, const int32_t* split_status, const int32_t* csr_status, float* losses,

@@ -10,16 +10,19 @@ N = 2000 nodes, E = 6000 stored facts per question, self-loops on): per batch ``
   device  DeviceSplit(loader, weights="arrays", shuffle=True).get_batch
   device_fused  the device batches through a graphed step that also runs clip_grad_norm_ and Adam.step() in its graph
           (``optimizer=``, ``max_norm=``; optim.ClipAdam); graphed shapes only
-  device_epoch  the whole epoch as one GraphedTrainStep.train_epoch call: the batch assembly in the step graphs too,
-          one graph replay per step and one read at the end of the epoch; ReaRev / NSM graphed shapes only.  Its
-          number of graphs and the peak device memory after its untimed epoch are reported next to device_fused's.
+  device_epoch  the whole epoch as one GraphedTrainStep.train_epoch call (GraftNet: GraphedGraftTrainStep's): the
+          batch assembly in the step graphs too, one graph replay per step and one read at the end of the epoch;
+          graphed shapes only.  Its number of graphs and the peak device memory after its untimed epoch are reported
+          next to device_fused's.
 
 Shapes: ReaRev and NSM at the reference's training shape (B 8, entity_dim 50) through graphed.GraphedTrainStep;
 GraftNet (B 8, entity_dim 50) eager (graftnet_d50) and through graphed.GraphedGraftTrainStep (graftnet_d50_graphed);
 cfg2 (ReaRev, B 64, entity_dim 200) through GraphedTrainStep; and rearev_d50_varied, ReaRev at B 8 over a split whose
-questions hold 500..12 000 stored facts, so that an epoch's batches fall into many fact-capacity buckets (graphs).  A pass runs the whole split; the questions/s of a mode is the median over ``--runs`` passes, host
-and device alternating, after one warm-up pass of each (graph captures).  Then gr_split_fact_order alone, between CUDA
-events over ``--launches`` launches: B = 64 questions of 6 000 facts, and one question of 50 000 facts.  The GPU's
+questions hold 500..12 000 stored facts, so that an epoch's batches fall into many fact-capacity buckets (graphs).
+``buckets`` counts the distinct fact capacities of an epoch in stored order (GraftNet: also ``graft_buckets``, the
+distinct (fact, graft) capacity pairs, one epoch graph each).  A pass runs the whole split; the questions/s of a mode
+is the median over ``--runs`` passes, host and device alternating, after one warm-up pass of each (graph captures).
+Then gr_split_fact_order alone, between CUDA events over ``--launches`` launches: B = 64 questions of 6 000 facts, and one question of 50 000 facts.  The GPU's
 name and power limit are read in the same run.  One JSON line per measurement.
 
     python scripts/split_shuffle_probe.py [--questions 640] [--runs 3] [--modes host,device,device_fused,device_epoch]
@@ -66,7 +69,7 @@ def train_pass(data, step_fn, B):
 
 
 def epoch_pass(data, gts, B):
-    """One epoch as GraphedTrainStep.train_epoch; -> seconds."""
+    """One epoch as GraphedTrainStep.train_epoch (GraftNet: GraphedGraftTrainStep's); -> seconds."""
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     gts.train_epoch(data, B, FACT_DROP)
@@ -167,10 +170,10 @@ def main():
         modes = {"host": (L, step, train_pass), "device": (split, step, train_pass)}
         if use_graph:
             modes["device_fused"] = (split, make_step(name, m, use_graph, fused=True), train_pass)
-            if not graft:
-                ep = graphed.GraphedTrainStep(m, optimizer=torch.optim.Adam(
-                    [p for p in m.parameters() if p.requires_grad], lr=1e-4), max_norm=1.0, max_graphs=MAX_GRAPHS)
-                modes["device_epoch"] = (split, ep, epoch_pass)
+            cls = graphed.GraphedGraftTrainStep if graft else graphed.GraphedTrainStep
+            ep = cls(m, optimizer=torch.optim.Adam([p for p in m.parameters() if p.requires_grad], lr=1e-4),
+                     max_norm=1.0, max_graphs=MAX_GRAPHS)
+            modes["device_epoch"] = (split, ep, epoch_pass)
         modes = {k: v for k, v in modes.items() if k in want}
         graphs, peak = {}, {}
         for k, (data, fn, run) in modes.items():      # warm-up: captures, caches
@@ -186,10 +189,13 @@ def main():
             for k, (data, fn, run) in modes.items():
                 secs[k].append(run(data, fn, B))
         qps = {k: a.questions / float(np.median(v)) for k, v in secs.items()}
-        plan = graphed.epoch_plan(np.arange(a.questions), split._stored, split._ents, B, FACT_DROP)
+        plan = graphed.epoch_plan(np.arange(a.questions), split._stored, split._ents, B, FACT_DROP,
+                                  split._graft_count if graft else None)
         res = dict(shape=shape, model=name, B=B, D=over["entity_dim"], graphed=use_graph, fact_drop=FACT_DROP,
                    N=L.max_local_entity, E="500..12000" if varied else 6000, questions=a.questions,
                    buckets=len(set(plan.capacity.tolist())), gpu=info)
+        if graft:
+            res["graft_buckets"] = len(set(zip(plan.capacity.tolist(), plan.graft_capacity.tolist())))
         for k in modes:
             res[k + "_qps"] = round(qps[k], 1)
             res[k + "_s"] = [round(x, 4) for x in secs[k]]

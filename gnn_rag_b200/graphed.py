@@ -20,8 +20,9 @@ batch i, so the end-to-end rate is bounded by the device time of the step, not b
 Models.  The input side is a per-model layout chosen from the model class: :class:`_KbLayout` for the 7-tuple of
 ``SingleDataLoader.get_batch`` (ReaRev, NSM) and :class:`_GraftLayout` for the 9/10-tuple of
 ``GraftSingleDataLoader.get_batch`` (GraftNet: two more fact lists at their own bucketed capacity with live counts for
-``gr_graft_stage``, and ``kb_fact_rel``).  The LRU, the pipeline and the streams are shared.  The status words of the
-step (one per CSR build / staging) travel back with the results and are checked on the host after the step.
+``gr_graft_stage``, and ``kb_fact_rel``).  The layout also holds the rest of what differs by model in the training
+steps below.  The LRU, the capture routine, the pipeline and the streams are shared.  The status words of the step
+(one per CSR build / staging) travel back with the results and are checked on the host after the step.
 
 Training: :class:`GraphedTrainStep` captures ``model(batch, training=True)`` + ``loss.backward()`` + the train-time
 metrics (gr_train_metrics) of ReaRev and NSM over the same input side, and :class:`GraphedGraftTrainStep` those of
@@ -89,25 +90,55 @@ def _stage_copy(dst, src, n=None):
 
 
 class _KbLayout:
-    """Input side of the 7-tuple of ``SingleDataLoader.get_batch`` (ReaRev, NSM)."""
+    """What the graphed steps do differently per model family, for ReaRev and NSM: the input side of the 7-tuple of
+    ``SingleDataLoader.get_batch``, the serving and training forwards, the training refusals and key scalars, and the
+    model's part of an epoch graph."""
 
     def __init__(self, step):
+        from .models import ReaRev
         self.step = step
         m = step.model
         self.weights = bool(m.normalized_gnn), bool(m.norm_rel)
+        self.rearev = isinstance(m, ReaRev)
 
     @staticmethod
     def kb_view(batch):
         """(local_entity, query_entities, kb_adj_mat, q_input, seed_dist, true_batch_id, answer_dist)."""
         return batch[:7]
 
+    @staticmethod
+    def _shape_key(B, N, cap, Q, idx_dtype):
+        return (B, N, cap, Q, idx_dtype)
+
     def key(self, batch):
+        """The shape part of the capture key of ``batch``: (B, N, fact capacity, Q, index dtype)."""
         le, _qe, kb, qi = self.kb_view(batch)[:4]
         B, N = le.shape
-        cap = fact_capacity(int(kb[0].shape[0]))
-        Q = int(qi.shape[1])
         idx_dtype = torch.int32 if str(kb[0].dtype).endswith("int32") else torch.int64
-        return (B, N, cap, Q, idx_dtype)
+        return self._shape_key(B, N, fact_capacity(int(kb[0].shape[0])), int(qi.shape[1]), idx_dtype)
+
+    def model_key(self):
+        """The Python scalars of the model that its training forward bakes into a graph (none for ReaRev / NSM)."""
+        return ()
+
+    def refusal(self, Q):
+        """Why the eager training forward would leave the kernels for questions of Q tokens (a message), or None."""
+        m = self.step.model
+        dev, D = self.step.device, m.entity_dim
+        I = m.num_ins if self.rearev else 1
+        if not autograd_path.USE_KERNELS:
+            return "autograd_path.USE_KERNELS is off: the training forward would run its torch restatement"
+        if not ops.aggregate_backward_ok(D, I):
+            return ("_kernel_graph is None: entity_dim %d with %d instruction(s) is outside the aggregation backward "
+                    "kernel (%s)" % (D, I, ops.aggregate_backward_ok.__doc__.split(": ", 1)[1].rstrip(".")))
+        if not autograd_path._instruction_kernels(dev, Q, D, m.instruction.num_ins):
+            return ("_instruction_kernels is false: %d question tokens, entity_dim %d and %d instructions are outside "
+                    "gr_instructions" % (Q, D, m.instruction.num_ins))
+        if self.rearev and not autograd_path._reform_kernels(dev, D, I):
+            return "_reform_kernels is false: entity_dim %d with %d instructions is outside gr_query_reform" % (D, I)
+        if m.encode_type and not autograd_path._fact_kernels(dev, D):
+            return "the TypeLayer kernel does not admit entity_dim %d (ops.fact_train_ok)" % D
+        return None
 
     def static_inputs(self, key):
         B, N, cap, Q, idx_dtype = key[:5]
@@ -125,15 +156,6 @@ class _KbLayout:
         st.weight_list = torch.ones(cap, dtype=torch.float32, device=dev) if self.weights[0] else None
         st.weight_rel_list = torch.ones(cap, dtype=torch.float32, device=dev) if self.weights[1] else None
         return st
-
-    def names(self):
-        names = ["local_entity", "query_entities", "seed_dist", "answer_dist", "q_input", "heads", "rels", "tails",
-                 "nfacts"]
-        if self.weights[0]:
-            names.append("weight_list")
-        if self.weights[1]:
-            names.append("weight_rel_list")
-        return names
 
     def fill(self, st, batch):
         """Host batch -> the buffers of ``st`` (facts to the front of the capacity, live count to ``nfacts``);
@@ -179,15 +201,31 @@ class _KbLayout:
         return (put(stage.local_entity, le), put(stage.query_entities, qe), kb2, put(stage.q_input, qi),
                 put(stage.seed_dist, sd), None, put(stage.answer_dist, ad))
 
-    def run(self, st):
-        """The model part of the captured step -> (db, loss, pred, pred_dist)."""
+    @staticmethod
+    def batch_of(st):
+        """The 7-tuple over the static buffers ``st``."""
+        return (st.local_entity, st.query_entities,
+                (st.heads, st.rels, st.tails, None, None, st.weight_list, st.weight_rel_list),
+                st.q_input, st.seed_dist, None, st.answer_dist)
+
+    def _stage(self, st):
         m = self.step.model
-        tup = (st.local_entity, st.query_entities,
-               (st.heads, st.rels, st.tails, None, None, st.weight_list, st.weight_rel_list),
-               st.q_input, st.seed_dist, None, st.answer_dist)
-        db = batching.stage_batch(tup, self.step.device, m.num_relation + 1, m.normalized_gnn, m.norm_rel,
-                                  nfacts=st.nfacts)
-        loss, pred, pred_dist, _ = m(db)
+        return batching.stage_batch(self.batch_of(st), self.step.device, m.num_relation + 1, m.normalized_gnn,
+                                    m.norm_rel, nfacts=st.nfacts)
+
+    def run(self, st):
+        """The model part of the captured serving step -> (db, loss, pred, pred_dist)."""
+        db = self._stage(st)
+        loss, pred, pred_dist, _ = self.step.model(db)
+        return db, loss, pred, pred_dist
+
+    def train_forward(self, st):
+        """The model's training forward over the static buffers ``st`` -> (db, loss, pred, pred_dist)."""
+        m = self.step.model
+        db = self._stage(st)
+        live = autograd_path.LiveBatch(db, st.heads, st.tails, st.weight_list, st.nfacts)
+        core = autograd_path.rearev_core if self.rearev else autograd_path.nsm_core
+        loss, pred, pred_dist = core(m, live, autograd_path._stage(m, live))
         return db, loss, pred, pred_dist
 
     @staticmethod
@@ -203,6 +241,44 @@ class _KbLayout:
 
     def check(self, db):
         self.raise_for(torch.cat(self.status_words(db)).tolist())
+
+    # -- the model's part of a training epoch (GraphedTrainStep.start_epoch) ------------------------------------------
+    def epoch_refusal(self, split):
+        """Why ``split`` (a ``loader.DeviceSplit``) does not hold this model family's batches (a message), or None."""
+        if split.graft:
+            return "train_epoch takes a ReaRev / NSM split; this DeviceSplit holds GraftNet's graft lists"
+        return None
+
+    @staticmethod
+    def epoch_shapes(plan):
+        """The graph shape of every step of ``plan``: (B, fact capacity)."""
+        return list(zip(plan.B.tolist(), plan.capacity.tolist()))
+
+    def epoch_key(self, split, shape):
+        """The shape part of the capture key of an epoch step of ``shape`` (:meth:`epoch_shapes`) over ``split``."""
+        return self._shape_key(shape[0], split.N, shape[1], int(split._res["q_input"].shape[1]), split.index_dtype)
+
+    def epoch_inputs(self, key):
+        """The static buffers of an epoch graph: :meth:`static_inputs`, plus the head's outputs."""
+        st = self.static_inputs(key)
+        B, dev = key[0], self.step.device
+        st.ids, st.rows, st.kept = (torch.zeros(B, dtype=torch.int64, device=dev) for _ in range(3))
+        st.kept_total = torch.zeros(1, dtype=torch.int64, device=dev)
+        st.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        return st
+
+    def epoch_begin(self, ep, st):
+        """The model's head kernels after gr_epoch_step_begin (none for ReaRev / NSM)."""
+
+    def epoch_assemble(self, ep, st, seed):
+        """The model's part of the batch assembly after the kb facts' -> its status word (None for ReaRev / NSM)."""
+        return None
+
+    @staticmethod
+    def epoch_words(st, asm, model_asm, status):
+        """The step's words of ``EpochRun.status`` from the assembly word, :meth:`epoch_assemble`'s and the status
+        word of :meth:`GraphedTrainStep._run`: assembly, CSR."""
+        return [asm, status]
 
 
 class _GraftLayout(_KbLayout):
@@ -223,6 +299,23 @@ class _GraftLayout(_KbLayout):
         max_fact = int(kfr.shape[-1]) if len(kfr.shape) == 2 else int(kfr.shape[0]) // len(batch[0])
         return super().key(batch) + (gcap, max_fact)
 
+    def model_key(self):
+        """``pagerank_lambda`` and ``fact_scale``: Python scalars the training forward bakes into a graph."""
+        layer = self.step.model.reasoning
+        return float(layer.pagerank_lambda), float(layer.fact_scale)
+
+    def refusal(self, Q):
+        """Why the eager training forward would leave the kernels (a message), or None.  GraftNet's forward takes the
+        kernel path or the per-fact torch ops as a whole (``autograd_path._fact_kernels``); its question encoder has no
+        kernel path in training, so Q does not matter."""
+        D = self.step.model.entity_dim
+        if not autograd_path.USE_KERNELS:
+            return "autograd_path.USE_KERNELS is off: the training forward would run its torch restatement"
+        if not autograd_path._fact_kernels(self.step.device, D):
+            return ("_fact_kernels is false: entity_dim %d is outside the GraftNet training kernels (%s)"
+                    % (D, ops.fact_train_ok.__doc__.split(": ", 1)[1].rstrip(".")))
+        return None
+
     def static_inputs(self, key):
         st = super().static_inputs(key)
         B, gcap, max_fact = key[0], key[5], key[6]
@@ -232,9 +325,6 @@ class _GraftLayout(_KbLayout):
         st.graft_live = torch.zeros(2, dtype=torch.int32, device=dev)
         st.kb_fact_rel = torch.zeros(B, max_fact, dtype=torch.int64, device=dev)
         return st
-
-    def names(self):
-        return super().names() + self.LIST_NAMES + ["graft_live", "kb_fact_rel"]
 
     def fill(self, st, batch):
         nbytes = super().fill(st, batch)
@@ -279,6 +369,15 @@ class _GraftLayout(_KbLayout):
             loss, pred, pred_dist, _ = m._forward_infer(db, check_status=False)
         return db, loss, pred, pred_dist
 
+    def train_forward(self, st):
+        m = self.step.model
+        tup = self.batch_of(st)
+        # the training forward stages without normalized_gnn (GraftNet does not read the kb weights)
+        db = batching.stage_graft_batch(tup, self.step.device, m.num_relation + 1, False, m.norm_rel, nfacts=st.nfacts,
+                                        graft_live=st.graft_live)
+        loss, pred, pred_dist = autograd_path.graftnet_core(m, tup, autograd_path.graft_live_stage(db))
+        return db, loss, pred, pred_dist
+
     @staticmethod
     def status_words(db):
         return [db.graph.status, db.graft.status, db.graft.graph.status]
@@ -290,10 +389,97 @@ class _GraftLayout(_KbLayout):
         if graft_csr or kb:
             _KbLayout.raise_for([graft_csr | kb])
 
+    def epoch_refusal(self, split):
+        if not split.graft:
+            return ("GraphedGraftTrainStep.train_epoch takes a GraftNet split; this DeviceSplit holds no graft lists "
+                    "(GraphedTrainStep.train_epoch covers ReaRev and NSM)")
+        return None
+
+    @staticmethod
+    def epoch_shapes(plan):
+        """The graph shape of every step of ``plan``: (B, fact capacity, graft capacity)."""
+        return list(zip(plan.B.tolist(), plan.capacity.tolist(), plan.graft_capacity.tolist()))
+
+    def epoch_key(self, split, shape):
+        return super().epoch_key(split, shape) + (shape[2], split.max_facts)
+
+    def epoch_inputs(self, key):
+        st = super().epoch_inputs(key)
+        B, gcap, dev = key[0], key[5], self.step.device
+        st.kept_g = torch.zeros(B, dtype=torch.int64, device=dev)
+        st.graft_status = torch.zeros(1, dtype=torch.int32, device=dev)
+        # the graft assembly writes the lists' values (all 1.0); GraftNet's training forward never reads them
+        st.e2f_v, st.f2e_v = (torch.zeros(gcap, dtype=torch.float32, device=dev) for _ in range(2))
+        return st
+
+    def epoch_begin(self, ep, st):
+        """gr_epoch_graft_begin: the graft kept counts and ``graft_live`` of the step's ids."""
+        ops.epoch_graft_begin(st.ids, ep.graft_kept_table, ep.split._res["g_off"], st.e2f_b.numel(), st.kept_g,
+                              st.graft_live, st.graft_status)
+
+    def epoch_assemble(self, ep, st, seed):
+        """The graft lists at their capacity and ``kb_fact_rel``, in the fact order of ``seed``."""
+        out = ((st.e2f_b, st.e2f_f, st.e2f_e, st.e2f_v), (st.f2e_b, st.f2e_e, st.f2e_f, st.f2e_v), st.kb_fact_rel)
+        _graft, _kfr, _order, gasm = ep.split.assemble_graft(st.ids, st.kept_g, seed, st.e2f_b.numel(),
+                                                            ep.graft_n_total, out=out)
+        return gasm
+
+    @staticmethod
+    def epoch_words(st, asm, model_asm, status):
+        """-> assembly (kb, graft head and graft assembly), CSR (kb and graft CSR builds), graft staging."""
+        csr, staging, graft_csr = status[0:1], status[1:2], status[2:3]
+        return [asm | st.graft_status | model_asm, csr | graft_csr, staging]
+
 
 def _layout_for(model):
     from .models import GraftNet
     return _GraftLayout if isinstance(model, GraftNet) else _KbLayout
+
+
+# ---- capture ---------------------------------------------------------------------------------------------------------
+
+def _evict(cache, max_graphs):
+    """LRU eviction down to room for one more entry: its graph and every buffer it holds are released."""
+    while len(cache) >= max_graphs:
+        _k, old = cache.popitem(last=False)
+        torch.cuda.synchronize()
+        del old
+
+
+def _warm_up(fn):
+    """Run ``fn`` twice on a side stream (lazy init, allocator, caches, cuDNN plans), the device idle around it."""
+    torch.cuda.synchronize()
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        for _ in range(2):
+            fn()
+    torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.synchronize()
+
+
+def _capture(fn):
+    """Capture ``fn`` into a CUDA graph -> (graph, what ``fn`` returned)."""
+    g = torch.cuda.CUDAGraph()
+    # no cyclic garbage collection during the capture: collecting a dropped step's graph there (its exec graph and
+    # private pool are released) is a CUDA call that invalidates the capture
+    gc_on = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(g):
+            outs = fn()
+    finally:
+        if gc_on:
+            gc.enable()
+    return g, outs
+
+
+def _buffers_like(st, make):
+    """A buffer set holding ``make(t)`` for every tensor ``t`` of ``st`` (None stays None)."""
+    out = _Captured()
+    for name, t in vars(st).items():
+        setattr(out, name, None if t is None else make(t))
+    return out
 
 
 class GraphedStep:
@@ -327,23 +513,11 @@ class GraphedStep:
         if ent is not None:
             self._cache.move_to_end(key)
             return ent
-        while len(self._cache) >= self.max_graphs:          # LRU eviction: graph, static + landing + pinned buffers
-            _k, old = self._cache.popitem(last=False)
-            torch.cuda.synchronize()
-            del old
+        _evict(self._cache, self.max_graphs)
         st = self._layout.static_inputs(shape_key)
         self._fill(st, batch)
-        torch.cuda.synchronize()
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):            # warm-up on a side stream (lazy init, allocator, caches)
-            for _ in range(2):
-                self._run(st)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            outs = self._run(st)
+        _warm_up(lambda: self._run(st))
+        g, outs = _capture(lambda: self._run(st))
         ent = _Captured()
         ent.st, ent.g, ent.outs = st, g, outs
         ent.pipe = None
@@ -376,38 +550,22 @@ class GraphedStep:
                 self._copy_stream = torch.cuda.Stream()
                 self._d2h_stream = torch.cuda.Stream()
             db, loss, pred, pred_dist, cand_idx, cand_count, _ = ent.outs
+            nwords = len(self._layout.status_words(db))
             pipe = _Captured()
-            pipe.land, pipe.out_dev, pipe.out_host = [], [], []
-            pipe.land_free, pipe.done = [], []
-            for _ in range(2):
-                land = _Captured()
-                for name in self._layout.names():
-                    setattr(land, name, torch.empty_like(getattr(ent.st, name)))
-                land.weight_list = getattr(land, "weight_list", None)
-                land.weight_rel_list = getattr(land, "weight_rel_list", None)
-                pipe.land.append(land)
-                od = dict(cand_idx=torch.empty_like(cand_idx), pred_dist=torch.empty_like(pred_dist),
-                          cand_count=torch.empty_like(cand_count), pred=torch.empty_like(pred),
-                          loss=torch.empty_like(loss),
-                          status=torch.empty(len(self._layout.status_words(db)), dtype=torch.int32,
-                                             device=self.device))
-                pipe.out_dev.append(od)
-                pipe.out_host.append({k: torch.empty(v.shape, dtype=v.dtype, pin_memory=True)
-                                      for k, v in od.items()})
-                pipe.land_free.append(None)
-                pipe.done.append(None)
-                # pinned host staging of the inputs: pageable loader output (numpy, int64 / float64) is cast and copied
-                # here by the host (memcpy speed), the DMA to the landing set then runs asynchronously
-                stage = _Captured()
-                for name in self._layout.names():
-                    t = getattr(ent.st, name)
-                    setattr(stage, name, torch.empty(t.shape, dtype=t.dtype, pin_memory=True))
-                stage.weight_list = getattr(stage, "weight_list", None)
-                stage.weight_rel_list = getattr(stage, "weight_rel_list", None)
-                pipe.stage = getattr(pipe, "stage", [])
-                pipe.stage.append(stage)
-                pipe.h2d_done = getattr(pipe, "h2d_done", [])
-                pipe.h2d_done.append(None)
+            pipe.land = [_buffers_like(ent.st, torch.empty_like) for _ in range(2)]
+            # pinned host staging of the inputs: pageable loader output (numpy, int64 / float64) is cast and copied
+            # here by the host (memcpy speed), the DMA to the landing set then runs asynchronously
+            pipe.stage = [_buffers_like(ent.st, lambda t: torch.empty(t.shape, dtype=t.dtype, pin_memory=True))
+                          for _ in range(2)]
+            pipe.out_dev = [dict(cand_idx=torch.empty_like(cand_idx), pred_dist=torch.empty_like(pred_dist),
+                                 cand_count=torch.empty_like(cand_count), pred=torch.empty_like(pred),
+                                 loss=torch.empty_like(loss),
+                                 status=torch.empty(nwords, dtype=torch.int32, device=self.device))
+                            for _ in range(2)]
+            pipe.out_host = [{k: torch.empty(v.shape, dtype=v.dtype, pin_memory=True) for k, v in od.items()}
+                             for od in pipe.out_dev]
+            pipe.land_free, pipe.done, pipe.h2d_done = [None, None], [None, None], [None, None]
+            pipe.ents = None                         # device and pinned candidate entity ids, for DeviceSplit batches
             ent.pipe = pipe
         return ent.pipe
 
@@ -438,8 +596,9 @@ class GraphedStep:
             h2d_done.record(cs)
         pipe.h2d_done[slot] = h2d_done
         cur.wait_event(h2d_done)
-        for name in self._layout.names():            # landing set -> the graph's static inputs (D2D, ~10 us)
-            getattr(ent.st, name).copy_(getattr(land, name), non_blocking=True)
+        for name, t in vars(land).items():           # landing set -> the graph's static inputs (D2D, ~10 us)
+            if t is not None:
+                getattr(ent.st, name).copy_(t, non_blocking=True)
         pipe.land_free[slot] = torch.cuda.Event()
         pipe.land_free[slot].record(cur)
         ent.g.replay()
@@ -454,7 +613,7 @@ class GraphedStep:
             od["status"][i:i + 1].copy_(w, non_blocking=True)
         ents = None
         if on_device:                                # the candidates' entity ids, gathered here instead of on the host
-            if getattr(pipe, "ents", None) is None:
+            if pipe.ents is None:
                 pipe.ents = [(torch.empty_like(db.local_entity),
                               torch.empty(db.local_entity.shape, dtype=torch.int64, pin_memory=True)) for _ in range(2)]
             ents = pipe.ents[slot]
@@ -647,10 +806,11 @@ class _EpochBuffers:
             self.graft_n_total = largest(split._graft_count)
 
 
-def _release_autograd_history(model):
+def _release_autograd_history(model, params):
     """Drop the tensors with autograd history that a training forward leaves on the model's modules (``dist_history``,
-    the question encoder's states).  While a previous step's graph is alive, the next forward reuses its AccumulateGrad
-    nodes, which stay bound to the stream they were made on; one bound to the default stream cannot join a capture."""
+    the question encoder's states), and the gradients of ``params``, so the next backward allocates them rather than
+    accumulating.  While a previous step's graph is alive, the next forward reuses its AccumulateGrad nodes, which stay
+    bound to the stream they were made on; one bound to the default stream cannot join a capture."""
     def has_history(v):
         if isinstance(v, (list, tuple)):
             return any(has_history(t) for t in v)
@@ -659,6 +819,8 @@ def _release_autograd_history(model):
         for k, v in list(vars(mod).items()):
             if has_history(v):
                 setattr(mod, k, None)
+    for p in params:
+        p.grad = None
 
 
 def _autocast_dtype():
@@ -705,12 +867,10 @@ class GraphedTrainStep:
     optimizer = max_norm = None          # without an optimizer the graph ends at the gradients
 
     def __init__(self, model, max_graphs=8, optimizer=None, max_norm=None):
-        from .models import GraftNet, ReaRev
+        from .models import GraftNet
         if isinstance(model, GraftNet):
             raise ValueError("GraphedTrainStep covers ReaRev and NSM; GraftNet trains in GraphedGraftTrainStep")
         self._setup(model, max_graphs, _KbLayout, optimizer, max_norm)
-        self._rearev = isinstance(model, ReaRev)
-        self._core = autograd_path.rearev_core if self._rearev else autograd_path.nsm_core
 
     def _setup(self, model, max_graphs, layout, optimizer, max_norm):
         self.model = model
@@ -734,7 +894,7 @@ class GraphedTrainStep:
     # -- capture key and refusals ----------------------------------------------------------------------------------
     def key(self, batch):
         """The capture key of ``batch`` under the current model and torch state (see the class docstring)."""
-        return self._layout.key(batch) + self._state_key()
+        return self._layout.key(batch) + self._state_key() + self._layout.model_key()
 
     def _state_key(self):
         """The part of the capture key that is not the batch shape: the model, torch and optimizer state."""
@@ -755,36 +915,9 @@ class GraphedTrainStep:
 
     def refusal(self, Q):
         """Why the eager forward would leave the kernels for questions of Q tokens (a message), or None."""
-        m = self.model
-        dev, D = self.device, m.entity_dim
-        I = m.num_ins if self._rearev else 1
-        if not autograd_path.USE_KERNELS:
-            return "autograd_path.USE_KERNELS is off: the training forward would run its torch restatement"
-        if not ops.aggregate_backward_ok(D, I):
-            return ("_kernel_graph is None: entity_dim %d with %d instruction(s) is outside the aggregation backward "
-                    "kernel (%s)" % (D, I, ops.aggregate_backward_ok.__doc__.split(": ", 1)[1].rstrip(".")))
-        if not autograd_path._instruction_kernels(dev, Q, D, m.instruction.num_ins):
-            return ("_instruction_kernels is false: %d question tokens, entity_dim %d and %d instructions are outside "
-                    "gr_instructions" % (Q, D, m.instruction.num_ins))
-        if self._rearev and not autograd_path._reform_kernels(dev, D, I):
-            return "_reform_kernels is false: entity_dim %d with %d instructions is outside gr_query_reform" % (D, I)
-        if m.encode_type and not autograd_path._fact_kernels(dev, D):
-            return "the TypeLayer kernel does not admit entity_dim %d (ops.fact_train_ok)" % D
-        return None
+        return self._layout.refusal(Q)
 
     # -- capture ---------------------------------------------------------------------------------------------------
-    def _forward(self, st):
-        """The model's training forward over the static buffers ``st`` -> (db, loss, pred, pred_dist)."""
-        m = self.model
-        tup = (st.local_entity, st.query_entities,
-               (st.heads, st.rels, st.tails, None, None, st.weight_list, st.weight_rel_list),
-               st.q_input, st.seed_dist, None, st.answer_dist)
-        db = batching.stage_batch(tup, self.device, m.num_relation + 1, m.normalized_gnn, m.norm_rel,
-                                  nfacts=st.nfacts)
-        live = autograd_path.LiveBatch(db, st.heads, st.tails, st.weight_list, st.nfacts)
-        loss, pred, pred_dist = self._core(m, live, autograd_path._stage(m, live))
-        return db, loss, pred, pred_dist
-
     def _run(self, st, ac):
         """forward + backward + metrics over the static buffers ``st`` -> (loss, pred, pred_dist, h1, f1, status)."""
         m = self.model
@@ -794,7 +927,7 @@ class GraphedTrainStep:
         # graph's copies must not serve eager code).
         with torch.autocast("cuda", dtype=ac) if ac is not None else contextlib.nullcontext():
             torch.clear_autocast_cache()
-            db, loss, pred, pred_dist = self._forward(st)
+            db, loss, pred, pred_dist = self._layout.train_forward(st)
             torch.clear_autocast_cache()
         loss.backward()
         pred_dist = pred_dist.detach()
@@ -814,49 +947,37 @@ class GraphedTrainStep:
         why = self.refusal(key[3])
         if why is not None:
             raise ValueError("GraphedTrainStep: " + why)
-        while len(self._cache) >= self.max_graphs:          # LRU eviction: the graph, its buffers and its gradients
-            _k, old = self._cache.popitem(last=False)
-            torch.cuda.synchronize()
-            del old
+        _evict(self._cache, self.max_graphs)
         ac = _autocast_dtype()
         st = self._layout.static_inputs(key)
         self._layout.fill(st, batch)
         params = [p for p in self._params if p.requires_grad]
-        torch.cuda.synchronize()
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):            # warm-up on a side stream (lazy init, allocator, cuDNN plans)
-            for _ in range(2):
-                _release_autograd_history(self.model)
-                for p in params:
-                    p.grad = None
-                self._run(st, ac)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
+
+        def warm():
+            _release_autograd_history(self.model, params)
+            self._run(st, ac)
+        _warm_up(warm)
         fused = None
         if self.optimizer is not None:
             # the warm-up's gradients show which parameters the backward reaches; their missing Adam state is made
             # now, so the key the next step computes (it holds the state's data_ptrs) is the one stored below
             fused = optim.ClipAdam(self.optimizer, params, [p.grad for p in params], self.max_norm)
             key = self.key(batch)
-        _release_autograd_history(self.model)
-        for p in params:                         # the captured backward allocates (not accumulates) every gradient
-            p.grad = None
-        g = torch.cuda.CUDAGraph()
-        # no cyclic garbage collection during the capture: collecting a dropped step's graph there (its exec graph
-        # and private pool are released) is a CUDA call that invalidates the capture
-        gc_on = gc.isenabled()
-        gc.disable()
-        try:
-            with torch.cuda.graph(g):
-                outs = self._run(st, ac)
-                if fused is not None:
-                    fused.launch()
-        finally:
-            if gc_on:
-                gc.enable()
+        _release_autograd_history(self.model, params)    # the captured backward allocates every gradient
+
+        def captured():
+            outs = self._run(st, ac)
+            if fused is not None:
+                fused.launch()
+            return outs
+        g, outs = _capture(captured)
+        return self._store(key, st, g, outs, params, fused)
+
+    def _store(self, key, st, g, outs, params, fused, epoch=None):
+        """Cache a captured training graph under ``key`` with everything its replays read and write (``epoch``: the
+        epoch buffers of an epoch graph)."""
         ent = _Captured()
-        ent.st, ent.g, ent.outs = st, g, outs
+        ent.st, ent.g, ent.outs, ent.epoch = st, g, outs, epoch
         ent.params, ent.grads = params, [p.grad for p in params]
         ent.fused = fused
         if fused is not None:                    # the kernels read and clip the captured backward's gradients
@@ -878,12 +999,12 @@ class GraphedTrainStep:
         return TrainStepOutput(*ent.outs, raise_for=self._layout.raise_for,
                                grad_norm=None if ent.fused is None else ent.fused.grad_norm)
 
-
     # -- a whole epoch -----------------------------------------------------------------------------------------------
     def train_epoch(self, split, batch_size, fact_dropout):
-        """The reference's ``Trainer_KBQA.train_epoch`` around the model, over the resident split ``split``: one
-        :meth:`start_epoch`, one read.  -> ``(np.mean(losses), [0, 0], h1_list_all, f1_list_all)``.  Raises
-        :meth:`EpochRun.check`'s errors after the epoch when a batch was malformed."""
+        """The reference's ``Trainer_KBQA.train_epoch`` around the model, over the resident split ``split`` (for
+        :class:`GraphedGraftTrainStep` a GraftNet split): one :meth:`start_epoch`, one read.  -> ``(np.mean(losses),
+        [0, 0], h1_list_all, f1_list_all)``.  Raises :meth:`EpochRun.check`'s errors after the epoch when a batch was
+        malformed."""
         run = self.start_epoch(split, batch_size, fact_dropout)
         out = run.result()
         run.check()
@@ -895,12 +1016,9 @@ class GraphedTrainStep:
             return "an epoch steps the optimizer in its graphs: build the step with optimizer="
         if not isinstance(split, DeviceSplit):
             return "train_epoch takes a loader.DeviceSplit, got %s" % type(split).__name__
-        graft_step = isinstance(self._layout, _GraftLayout)
-        if graft_step and not split.graft:
-            return ("GraphedGraftTrainStep.train_epoch takes a GraftNet split; this DeviceSplit holds no graft lists "
-                    "(GraphedTrainStep.train_epoch covers ReaRev and NSM)")
-        if split.graft and not graft_step:
-            return "train_epoch takes a ReaRev / NSM split; this DeviceSplit holds GraftNet's graft lists"
+        why = self._layout.epoch_refusal(split)
+        if why is not None:
+            return why
         if not same_device(split.device, self.device):
             return "the split lives on %s, the model on %s" % (split.device, self.device)
         if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or batch_size <= 0:
@@ -924,19 +1042,22 @@ class GraphedTrainStep:
         loader's ``np.random`` order), then every batch of ``batch_size`` questions in order, the last one short when
         ``num_data % batch_size != 0``, each assembled as ``split.get_batch(it, batch_size, fact_dropout)`` does,
         trained and stepped.  Each step is one graph replay: the graph assembles the batch on the device from a
-        cursor into the epoch's question order (gr_epoch_step_begin, ``DeviceSplit.assemble`` at the bucket's
-        capacity, the fact-order seed drawn from torch's CUDA generator with ``shuffle``), runs the step of
-        :meth:`step` with the step's Adam scalars (all uploaded at the start of the epoch), then records loss,
-        gradient norm, seed, hit@1 and F1 at the cursor and advances it (gr_epoch_step_record).  The host picks each
-        step's graph from :func:`epoch_plan`; the graphs the epoch needs and does not hold yet are captured before the
-        first replay (the LRU grows to hold them all), without moving the records, the parameters or torch's generator.
+        cursor into the epoch's question order (gr_epoch_step_begin, ``DeviceSplit.assemble`` at the bucket's fact
+        capacity, the fact-order seed drawn from torch's CUDA generator with ``shuffle``; for GraftNet also
+        gr_epoch_graft_begin after the first kernel and ``DeviceSplit.assemble_graft`` at the bucket's graft capacity,
+        both fact orders drawn from the one seed), runs the step of :meth:`step` with the step's Adam scalars (all
+        uploaded at the start of the epoch), then records loss, gradient norm, seed, hit@1 and F1 at the cursor and
+        advances it (gr_epoch_step_record).  The host picks each step's graph, one per (B, fact capacity) and for
+        GraftNet per graft capacity too, from :func:`epoch_plan`; the graphs the epoch needs and does not hold yet are
+        captured before the first replay (the LRU grows to hold them all), without moving the records, the parameters
+        or torch's generator.  A GraftNet ``EpochRun.status`` has three words: assembly, CSR and graft staging.
 
         Afterwards ``p.grad``, the parameters and the Adam state are those of the loop ``get_batch`` + :meth:`step`,
         the CPU ``step`` tensors advanced by the number of steps, and ``split.loader.sample_ids`` is the last batch's.
-        Refused (``ValueError``): a step without ``optimizer``, anything but a CUDA ``DeviceSplit`` of a kb loader on
-        the model's device (GraftNet's epoch is :meth:`GraphedGraftTrainStep.start_epoch`), ``batch_size <= 0``, a
-        ``fact_dropout`` ``get_batch`` refuses, and fact weights (``normalized_gnn`` / ``norm_rel``) over a
-        ``weights="none"`` split."""
+        Refused (``ValueError``): a step without ``optimizer``, anything but a CUDA ``DeviceSplit`` on the model's
+        device of the step's model family (a kb loader for ReaRev / NSM, a GraftNet loader for
+        :class:`GraphedGraftTrainStep`), ``batch_size <= 0``, a ``fact_dropout`` ``get_batch`` refuses, and fact
+        weights (``normalized_gnn`` / ``norm_rel``) over a ``weights="none"`` split."""
         why = self._epoch_refusal(split, batch_size, fact_dropout)
         if why is not None:
             raise ValueError("train_epoch: " + why)
@@ -984,101 +1105,65 @@ class GraphedTrainStep:
             ep = self._epochs[k] = _EpochBuffers(split, batch_size, self.max_norm)
         return ep
 
-    def _epoch_key(self, ep, B, cap):
-        split = ep.split
-        shape = (B, split.N, cap, int(split._res["q_input"].shape[1]), split.index_dtype)
-        return shape + self._state_key() + ("epoch", id(ep))
-
-    @staticmethod
-    def _epoch_shapes(plan):
-        """The graph shape of every step of ``plan``: (B, fact capacity)."""
-        return list(zip(plan.B.tolist(), plan.capacity.tolist()))
+    def _epoch_key(self, ep, shape):
+        return (self._layout.epoch_key(ep.split, shape) + self._state_key() + self._layout.model_key()
+                + ("epoch", id(ep)))
 
     def _epoch_entries(self, ep, plan):
         """The graph of every step of ``plan`` (a list), capturing the missing ones first."""
-        steps = self._epoch_shapes(plan)
+        steps = self._layout.epoch_shapes(plan)
         shapes = {}
         for s, shape in enumerate(steps):
             shapes.setdefault(shape, s)
         self.max_graphs = max(self.max_graphs, len(shapes))
         for shape, s in shapes.items():
-            key = self._epoch_key(ep, *shape)
+            key = self._epoch_key(ep, shape)
             if key in self._cache:
                 self._cache.move_to_end(key)
             else:
                 self._epoch_capture(ep, shape, s)
         # a capture may create Adam state, which the keys hold: resolve them once all graphs exist
-        ents = {shape: self._cache[self._epoch_key(ep, *shape)] for shape in shapes}
+        ents = {shape: self._cache[self._epoch_key(ep, shape)] for shape in shapes}
         layouts = {ent.fused.layout() for ent in ents.values() if ent.fused is not None}
         if len(layouts) > 1:
             raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
         return [ents[shape] for shape in steps]
 
-    def _epoch_static(self, key):
-        """The static buffers of an epoch graph: the layout's, plus the head's outputs."""
-        st = self._layout.static_inputs(key)
-        B, dev = key[0], self.device
-        st.ids, st.rows, st.kept = (torch.zeros(B, dtype=torch.int64, device=dev) for _ in range(3))
-        st.kept_total = torch.zeros(1, dtype=torch.int64, device=dev)
-        st.status = torch.zeros(1, dtype=torch.int32, device=dev)
-        return st
-
-    def _epoch_begin(self, ep, st, cursor):
-        """The head kernel of an epoch step: the step's ids, rows and counts into ``st``."""
-        split = ep.split
-        r = split._res
+    def _epoch_body(self, ep, st, cursor, ac):
+        """One step of the epoch over the static buffers ``st``: the head kernels, the batch assembly into ``st`` and
+        the captured step of :meth:`_run` -> (outs of _run, seed or None, the step's words of ``EpochRun.status``)."""
+        split, layout = ep.split, self._layout
+        r, cap = split._res, st.heads.numel()
         ops.epoch_step_begin(cursor, ep.order, ep.batch_size, ep.kept_table, r["q_off"], r["q_ents"],
-                             split.use_self_loop, st.heads.numel(), st.ids, st.rows, st.kept, st.nfacts, st.kept_total,
-                             st.status)
-
-    def _epoch_head(self, ep, st, cursor):
-        """The head kernels, the fact-order seed and the kb half of the batch assembly into ``st`` -> (seed or None,
-        the assembly status word)."""
-        split = ep.split
-        cap = st.heads.numel()
-        self._epoch_begin(ep, st, cursor)
+                             split.use_self_loop, cap, st.ids, st.rows, st.kept, st.nfacts, st.kept_total, st.status)
+        layout.epoch_begin(ep, st)
         seed = torch.randint(0, 2 ** 62, (1,), device=self.device) if split.shuffle else None
         _rows, _kb, _order, asm = split.assemble(st.ids, st.kept, seed, cap, cap, ep.n_total, rows=st.rows, out=st,
                                                  nfacts=st.nfacts)
-        return seed, st.status | asm
-
-    def _epoch_body(self, ep, st, cursor, ac):
-        """One step of the epoch over the static buffers ``st``: the head kernel, the batch assembly into ``st`` and
-        the captured step of :meth:`_run` -> (outs of _run, seed or None, the step's words of ``EpochRun.status``:
-        assembly, CSR)."""
-        seed, asm = self._epoch_head(ep, st, cursor)
+        asm = st.status | asm
+        model_asm = layout.epoch_assemble(ep, st, seed)
         outs = self._run(st, ac)
-        return outs, seed, [asm, outs[5]]
+        return outs, seed, layout.epoch_words(st, asm, model_asm, outs[5])
 
     def _epoch_capture(self, ep, shape, s0):
-        """Capture the epoch graph of ``shape`` (:meth:`_epoch_shapes`: B questions, the fact capacity and, for
-        GraftNet, the graft capacity); ``s0``: a step of the epoch with that shape, the one the warm-up assembles."""
-        key = self._epoch_key(ep, *shape)
-        split = ep.split
+        """Capture the epoch graph of ``shape`` (``_KbLayout.epoch_shapes``); ``s0``: a step of the epoch with that
+        shape, the one the warm-up assembles."""
+        key = self._epoch_key(ep, shape)
         why = self.refusal(key[3])
         if why is not None:
             raise ValueError("GraphedTrainStep: " + why)
-        while len(self._cache) >= self.max_graphs:
-            _k, old = self._cache.popitem(last=False)
-            torch.cuda.synchronize()
-            del old
+        _evict(self._cache, self.max_graphs)
         ac = _autocast_dtype()
-        st = self._epoch_static(key)
+        st = self._layout.epoch_inputs(key)
         dev = self.device
         params = [p for p in self._params if p.requires_grad]
-        torch.cuda.synchronize()
         rng = torch.cuda.get_rng_state(dev)
         warm_cursor = torch.full((1,), s0, dtype=torch.int64, device=dev)    # the real cursor does not move
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                _release_autograd_history(self.model)
-                for p in params:
-                    p.grad = None
-                self._epoch_body(ep, st, warm_cursor, ac)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
+
+        def warm():
+            _release_autograd_history(self.model, params)
+            self._epoch_body(ep, st, warm_cursor, ac)
+        _warm_up(warm)
         torch.cuda.set_rng_state(rng, dev)
         fused = optim.ClipAdam(self.optimizer, params, [p.grad for p in params], self.max_norm)
         T = fused._scalars.shape[0]
@@ -1086,34 +1171,21 @@ class GraphedTrainStep:
             ep.adam = torch.zeros(ep.steps, T, 8, dtype=torch.float32, device=dev)
         elif ep.adam.shape[1] != T:
             raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
-        key = self._epoch_key(ep, *shape)
-        _release_autograd_history(self.model)
-        for p in params:
-            p.grad = None
-        g = torch.cuda.CUDAGraph()
-        gc_on = gc.isenabled()
-        gc.disable()
-        try:
-            with torch.cuda.graph(g):
-                outs, seed, words = self._epoch_body(ep, st, ep.cursor, ac)
-                torch.index_select(ep.adam, 0, ep.cursor, out=fused._scalars.view(1, T, 8))
-                fused.launch()
-                loss, _pred, _pd, h1, f1, _words = outs
-                if len(words) > 2:               # GraftNet's graft staging word
-                    ep.status[2:].bitwise_or_(words[2])
-                ops.epoch_step_record(ep.cursor, ep.batch_size, ep.num_data, loss.float(), fused.grad_norm, seed, h1,
-                                      f1, words[0], words[1], ep.losses, ep.grad_norms, ep.seeds, ep.h1, ep.f1,
-                                      ep.status[:2])
-        finally:
-            if gc_on:
-                gc.enable()
-        ent = _Captured()
-        ent.st, ent.g, ent.outs, ent.epoch = st, g, outs, ep
-        ent.params, ent.grads = params, [p.grad for p in params]
-        ent.fused = fused
-        fused.bind([p.grad for p in fused.params])
-        self._cache[key] = ent
-        return ent
+        key = self._epoch_key(ep, shape)
+        _release_autograd_history(self.model, params)
+
+        def captured():
+            outs, seed, words = self._epoch_body(ep, st, ep.cursor, ac)
+            torch.index_select(ep.adam, 0, ep.cursor, out=fused._scalars.view(1, T, 8))
+            fused.launch()
+            loss, _pred, _pd, h1, f1, _words = outs
+            for i in range(2, len(words)):       # gr_epoch_step_record ORs the first two words (assembly, CSR)
+                ep.status[i:i + 1].bitwise_or_(words[i])
+            ops.epoch_step_record(ep.cursor, ep.batch_size, ep.num_data, loss.float(), fused.grad_norm, seed, h1, f1,
+                                  words[0], words[1], ep.losses, ep.grad_norms, ep.seeds, ep.h1, ep.f1, ep.status[:2])
+            return outs
+        g, outs = _capture(captured)
+        return self._store(key, st, g, outs, params, fused, ep)
 
 
 class GraphedGraftTrainStep(GraphedTrainStep):
@@ -1144,96 +1216,4 @@ class GraphedGraftTrainStep(GraphedTrainStep):
         if len(batch) not in (9, 10):
             raise ValueError("GraphedGraftTrainStep takes the 9/10-tuple of GraftSingleDataLoader.get_batch, not a "
                              "%d-tuple" % len(batch))
-        layer = self.model.reasoning
-        return super().key(batch) + (float(layer.pagerank_lambda), float(layer.fact_scale))
-
-    def refusal(self, Q):
-        """Why the eager forward would leave the kernels (a message), or None.  GraftNet's forward takes the kernel
-        path or the per-fact torch ops as a whole (``autograd_path._fact_kernels``); its question encoder has no
-        kernel path in training, so Q does not matter."""
-        D = self.model.entity_dim
-        if not autograd_path.USE_KERNELS:
-            return "autograd_path.USE_KERNELS is off: the training forward would run its torch restatement"
-        if not autograd_path._fact_kernels(self.device, D):
-            return ("_fact_kernels is false: entity_dim %d is outside the GraftNet training kernels (%s)"
-                    % (D, ops.fact_train_ok.__doc__.split(": ", 1)[1].rstrip(".")))
-        return None
-
-    # -- a whole epoch -----------------------------------------------------------------------------------------------
-    def train_epoch(self, split, batch_size, fact_dropout):
-        """The reference's ``Trainer_KBQA.train_epoch`` around GraftNet, over the resident GraftNet split ``split``:
-        one :meth:`start_epoch`, one read.  -> ``(np.mean(losses), [0, 0], h1_list_all, f1_list_all)``.  Raises
-        :meth:`EpochRun.check`'s errors after the epoch when a batch was malformed."""
-        return super().train_epoch(split, batch_size, fact_dropout)
-
-    def start_epoch(self, split, batch_size, fact_dropout):
-        """Start one GraftNet training epoch over ``split`` (a ``loader.DeviceSplit`` of a GraftNet loader) and return
-        its :class:`EpochRun` without waiting for the device.
-
-        As the reference's ``train_epoch``: ``model.train()``, ``split.reset_batches(is_sequential=False)`` (the
-        loader's ``np.random`` order), then every batch of ``batch_size`` questions in order, the last one short when
-        ``num_data % batch_size != 0``, each assembled as ``split.get_batch(it, batch_size, fact_dropout)`` does,
-        trained and stepped.  Each step is one graph replay: the graph assembles the batch on the device from a
-        cursor into the epoch's question order (gr_epoch_step_begin and gr_epoch_graft_begin, then
-        ``DeviceSplit.assemble`` at the bucket's fact capacity and ``DeviceSplit.assemble_graft`` at its graft
-        capacity, both fact orders drawn from one seed taken from torch's CUDA generator with ``shuffle``), runs the
-        step of :meth:`step` with the step's Adam scalars (all uploaded at the start of the epoch), then records loss,
-        gradient norm, seed, hit@1 and F1 at the cursor and advances it (gr_epoch_step_record).  The host picks each
-        step's graph, one per (B, fact capacity, graft capacity), from :func:`epoch_plan`; the graphs the epoch needs
-        and does not hold yet are captured before the first replay (the LRU grows to hold them all), without moving
-        the records, the parameters or torch's generator.  ``EpochRun.status`` has three words: assembly, CSR and
-        graft staging.
-
-        Afterwards ``p.grad``, the parameters and the Adam state are those of the loop ``get_batch`` + :meth:`step`,
-        the CPU ``step`` tensors advanced by the number of steps, and ``split.loader.sample_ids`` is the last batch's.
-        Refused (``ValueError``): a step without ``optimizer``, anything but a CUDA ``DeviceSplit`` of a GraftNet loader
-        on the model's device, ``batch_size <= 0``, a ``fact_dropout`` ``get_batch`` refuses, and fact weights
-        (``norm_rel``) over a ``weights="none"`` split."""
-        return super().start_epoch(split, batch_size, fact_dropout)
-
-    def _epoch_key(self, ep, B, cap, gcap):
-        split = ep.split
-        layer = self.model.reasoning
-        shape = (B, split.N, cap, int(split._res["q_input"].shape[1]), split.index_dtype, gcap, split.max_facts)
-        return (shape + self._state_key() + (float(layer.pagerank_lambda), float(layer.fact_scale))
-                + ("epoch", id(ep)))
-
-    @staticmethod
-    def _epoch_shapes(plan):
-        """The graph shape of every step of ``plan``: (B, fact capacity, graft capacity)."""
-        return list(zip(plan.B.tolist(), plan.capacity.tolist(), plan.graft_capacity.tolist()))
-
-    def _epoch_static(self, key):
-        st = super()._epoch_static(key)
-        B, gcap, dev = key[0], key[5], self.device
-        st.kept_g = torch.zeros(B, dtype=torch.int64, device=dev)
-        st.graft_status = torch.zeros(1, dtype=torch.int32, device=dev)
-        # the graft assembly writes the lists' values (all 1.0); GraftNet's training forward never reads them
-        st.e2f_v, st.f2e_v = (torch.zeros(gcap, dtype=torch.float32, device=dev) for _ in range(2))
-        return st
-
-    def _epoch_begin(self, ep, st, cursor):
-        super()._epoch_begin(ep, st, cursor)
-        ops.epoch_graft_begin(st.ids, ep.graft_kept_table, ep.split._res["g_off"], st.e2f_b.numel(), st.kept_g,
-                              st.graft_live, st.graft_status)
-
-    def _epoch_body(self, ep, st, cursor, ac):
-        """:meth:`GraphedTrainStep._epoch_body` with the graft half of the head (gr_epoch_graft_begin) and of the
-        assembly (the graft lists at their capacity and ``kb_fact_rel``) -> words: assembly, CSR, graft staging."""
-        split = ep.split
-        gcap = st.e2f_b.numel()
-        seed, asm = self._epoch_head(ep, st, cursor)
-        out = ((st.e2f_b, st.e2f_f, st.e2f_e, st.e2f_v), (st.f2e_b, st.f2e_e, st.f2e_f, st.f2e_v), st.kb_fact_rel)
-        _graft, _kfr, _order, gasm = split.assemble_graft(st.ids, st.kept_g, seed, gcap, ep.graft_n_total, out=out)
-        outs = self._run(st, ac)
-        csr, staging, graft_csr = outs[5][0:1], outs[5][1:2], outs[5][2:3]
-        return outs, seed, [asm | st.graft_status | gasm, csr | graft_csr, staging]
-
-    def _forward(self, st):
-        m = self.model
-        tup = _GraftLayout.batch_of(st)
-        # the training forward stages without normalized_gnn (GraftNet does not read the kb weights)
-        db = batching.stage_graft_batch(tup, self.device, m.num_relation + 1, False, m.norm_rel, nfacts=st.nfacts,
-                                        graft_live=st.graft_live)
-        loss, pred, pred_dist = autograd_path.graftnet_core(m, tup, autograd_path.graft_live_stage(db))
-        return db, loss, pred, pred_dist
+        return super().key(batch)

@@ -65,10 +65,9 @@ def test_refuses_graftnet_and_cpu_models():
 def _unbuilt_step(model, device="cpu"):
     """A GraphedTrainStep over a CPU model, built past the constructor's device refusal: its key and refusal logic run
     on the host and capture nothing."""
-    from gnn_rag_b200.models import ReaRev
     st = object.__new__(graphed.GraphedTrainStep)
     st.model, st._params, st.device = model, list(model.parameters()), torch.device(device)
-    st.max_graphs, st._rearev, st._cache = 8, isinstance(model, ReaRev), {}
+    st.max_graphs, st._cache = 8, {}
     st._layout = graphed._KbLayout(st)
     return st
 

@@ -6,6 +6,8 @@
 //                            shuffle=False): row bias b*N, batch ids, fact ids, one pass.
 //   gr_split_assemble_graft  both graft lists of GraftSingleDataLoader._build_fact_mat_maxfacts
 //                            (gnn/dataset_load_graft.py:70-102) in stored order, and the kb_fact_rel rows.
+//   gr_split_assemble_ordered / gr_split_assemble_graft_ordered   the same two with fact dropout (below): a question's
+//                            facts are its kept count of a fact order, gathered through it.
 //   gr_fact_weights          weight_list = 1/outdeg(head) and weight_rel_list = 1/count(head, rel) (:507-516).
 //   gr_fact_weights_live     the same over the live prefix of capacity-length fact buffers, its length read on the
 //                            device (the batch a captured training epoch assembles in place).
@@ -14,7 +16,12 @@
 // counts of questions 0..b-1 itself (B ids, read from the resident offsets) to find where its question starts, so no
 // host round trip and no second launch is needed; the host sizes the outputs from its own copy of the counts.
 // Out-of-range question ids count as empty questions and set status bit 1; outputs that would run past the capacity
-// the host passed are not written and set status bit 2.
+// the host passed are not written and set status bit 2.  One kernel per list serves both entry points of that list.
+// Stored order reads every stored fact, fact k at k, after one block sum; ordered (kOrdered) the counts are kept[b]
+// clamped to the stored ones and fact k is read at order[k], which adds the order's offsets (a second block sum for
+// the kb facts), the bound K on the order and bit 1 for an entry that is not a stored index.  kOrdered is a template
+// parameter, so the stored-order instance compiles to the stored-order code alone; the launcher picks it from `kept`,
+// never from `order`: with every fact dropped, K = 0 and the order pointer is null.
 //
 // Weights: integer counting only.  outdeg(head) by atomicAdd on an int counter per row; count(head, rel) by an open-
 // addressing hash table over the (head, rel) keys of the batch (linear probing, load <= 1/2) with an int counter per
@@ -31,7 +38,6 @@
 //                            workspace; only the buckets that hold kept ranks are scattered and sorted, each in shared
 //                            memory, or in the workspace when it overflows.  The sort is by a total order, so the
 //                            result does not depend on the order the scatter's atomics land in.
-//   gr_split_assemble_ordered / gr_split_assemble_graft_ordered   the assembly above, gathering through that order.
 #include <limits.h>
 
 #include <algorithm>
@@ -67,43 +73,57 @@ __device__ __forceinline__ int64_t block_sum(int64_t v, int64_t* s_red) {
   return s_red[32];
 }
 
-template <typename IdxT>
+// per question: its facts (in stored order, or kOrdered: at the stored indices in its run of `order`), then the
+// self-loops of its entities
+template <typename IdxT, bool kOrdered>
 __global__ void __launch_bounds__(kSplitThreads)
 split_assemble_kernel(const int64_t* __restrict__ q_off, const int32_t* __restrict__ q_heads,
                       const int32_t* __restrict__ q_rels, const int32_t* __restrict__ q_tails,
-                      const int32_t* __restrict__ q_ents, int64_t num_q, const int64_t* __restrict__ ids, int64_t N,
+                      const int32_t* __restrict__ q_ents, int64_t num_q, const int64_t* __restrict__ ids,
+                      const int64_t* __restrict__ kept, const int32_t* __restrict__ order, int64_t K, int64_t N,
                       int64_t self_rel, int use_self_loop, int64_t F, IdxT* __restrict__ heads, IdxT* __restrict__ rels,
                       IdxT* __restrict__ tails, IdxT* __restrict__ bids, IdxT* __restrict__ fids,
                       int32_t* __restrict__ status) {
   __shared__ int64_t s_red[33];
   const int b = blockIdx.y;
-  auto total = [&](int64_t id) -> int64_t {
-    if (!valid_id(id, num_q)) return 0;
-    return q_off[id + 1] - q_off[id] + (use_self_loop ? (int64_t)q_ents[id] : 0);
-  };
-  int64_t before = 0;
-  for (int j = threadIdx.x; j < b; j += blockDim.x) before += total(ids[j]);
+  auto stored = [&](int64_t id) -> int64_t { return valid_id(id, num_q) ? q_off[id + 1] - q_off[id] : 0; };
+  auto facts = [&](int j, int64_t n) -> int64_t { return kOrdered ? min(max(kept[j], (int64_t)0), n) : n; };
+  auto ents = [&](int64_t id) -> int64_t { return use_self_loop && valid_id(id, num_q) ? (int64_t)q_ents[id] : 0; };
+  int64_t before = 0, obefore = 0;
+  for (int j = threadIdx.x; j < b; j += blockDim.x) {
+    const int64_t idj = ids[j], kj = facts(j, stored(idj));
+    obefore += kj;
+    before += kj + ents(idj);
+  }
   const int64_t pos = block_sum(before, s_red);
+  const int64_t opos = kOrdered ? block_sum(obefore, s_red) : 0;
   const int64_t id = ids[b];
   const bool ok = valid_id(id, num_q);
-  const int64_t base = ok ? q_off[id] : 0;
-  const int64_t nf = ok ? q_off[id + 1] - base : 0;
-  const int64_t tot = total(id);
+  const int64_t base = ok ? q_off[id] : 0, nf = stored(id), k = facts(b, nf), tot = k + ents(id);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     if (!ok) atomicOr(status, 1);
-    if (pos + tot > F) atomicOr(status, 2);
+    if (pos + tot > F || (kOrdered && opos + k > K)) atomicOr(status, 2);
   }
   const int64_t bias = (int64_t)b * N;
   const int64_t end = min(tot, F - pos);
-  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < end; k += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t o = pos + k;
+  for (int64_t kk = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; kk < end; kk += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t o = pos + kk;
     int64_t h, r, t;
-    if (k < nf) {
-      h = bias + q_heads[base + k];
-      r = q_rels[base + k];
-      t = bias + q_tails[base + k];
+    if (kk < k) {
+      int64_t s = kk;
+      if (kOrdered) {
+        if (opos + kk >= K) continue;          // past the order array (flagged above)
+        s = order[opos + kk];
+        if (s < 0 || s >= nf) {                // not a stored index of this question: not read, not written
+          atomicOr(status, 1);
+          continue;
+        }
+      }
+      h = bias + q_heads[base + s];
+      r = q_rels[base + s];
+      t = bias + q_tails[base + s];
     } else {                                   // the self-loops of the question's entities (dataset_load.py:498-505)
-      h = t = bias + (k - nf);
+      h = t = bias + (kk - k);
       r = self_rel;
     }
     heads[o] = (IdxT)h;
@@ -114,12 +134,15 @@ split_assemble_kernel(const int64_t* __restrict__ q_off, const int32_t* __restri
   }
 }
 
-template <typename IdxT>
+// both graft lists (in stored order, or kOrdered: at the positions in `order`, the lists and the order sharing one
+// layout) and the kb_fact_rel rows, stored either way
+template <typename IdxT, bool kOrdered>
 __global__ void __launch_bounds__(kSplitThreads)
 split_assemble_graft_kernel(const int64_t* __restrict__ g_off, const int32_t* __restrict__ g_e2f_f,
                             const int32_t* __restrict__ g_e2f_e, const int32_t* __restrict__ g_f2e_e,
                             const int32_t* __restrict__ g_f2e_f, const int64_t* __restrict__ r_off,
                             const int32_t* __restrict__ r_vals, int64_t num_q, const int64_t* __restrict__ ids,
+                            const int64_t* __restrict__ kept, const int32_t* __restrict__ order, int64_t K,
                             int64_t max_facts, int64_t rel_pad, int64_t G, IdxT* __restrict__ e2f_b,
                             IdxT* __restrict__ e2f_f, IdxT* __restrict__ e2f_e, float* __restrict__ e2f_v,
                             IdxT* __restrict__ f2e_b, IdxT* __restrict__ f2e_e, IdxT* __restrict__ f2e_f,
@@ -127,28 +150,38 @@ split_assemble_graft_kernel(const int64_t* __restrict__ g_off, const int32_t* __
                             int32_t* __restrict__ status) {
   __shared__ int64_t s_red[33];
   const int b = blockIdx.y;
-  auto count = [&](int64_t id) -> int64_t { return valid_id(id, num_q) ? g_off[id + 1] - g_off[id] : 0; };
+  auto stored = [&](int64_t id) -> int64_t { return valid_id(id, num_q) ? g_off[id + 1] - g_off[id] : 0; };
+  auto entries = [&](int j, int64_t n) -> int64_t { return kOrdered ? min(max(kept[j], (int64_t)0), n) : n; };
   int64_t before = 0;
-  for (int j = threadIdx.x; j < b; j += blockDim.x) before += count(ids[j]);
+  for (int j = threadIdx.x; j < b; j += blockDim.x) before += entries(j, stored(ids[j]));
   const int64_t pos = block_sum(before, s_red);
   const int64_t id = ids[b];
   const bool ok = valid_id(id, num_q);
-  const int64_t base = ok ? g_off[id] : 0, n = count(id);
+  const int64_t base = ok ? g_off[id] : 0, n = stored(id), k = entries(b, n);
+  const int64_t cap = kOrdered ? min(G, K) : G;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     if (!ok) atomicOr(status, 1);
-    if (pos + n > G) atomicOr(status, 2);
+    if (pos + k > cap) atomicOr(status, 2);
   }
   const int64_t stride = (int64_t)gridDim.x * blockDim.x, k0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t end = min(n, G - pos);
-  for (int64_t k = k0; k < end; k += stride) {
-    const int64_t o = pos + k;
+  const int64_t end = min(k, cap - pos);
+  for (int64_t kk = k0; kk < end; kk += stride) {
+    const int64_t o = pos + kk;
+    int64_t s = kk;
+    if (kOrdered) {
+      s = order[o];
+      if (s < 0 || s >= n) {
+        atomicOr(status, 1);
+        continue;
+      }
+    }
     e2f_b[o] = (IdxT)b;
-    e2f_f[o] = (IdxT)g_e2f_f[base + k];
-    e2f_e[o] = (IdxT)g_e2f_e[base + k];
+    e2f_f[o] = (IdxT)g_e2f_f[base + s];
+    e2f_e[o] = (IdxT)g_e2f_e[base + s];
     e2f_v[o] = 1.0f;
     f2e_b[o] = (IdxT)b;
-    f2e_e[o] = (IdxT)g_f2e_e[base + k];
-    f2e_f[o] = (IdxT)g_f2e_f[base + k];
+    f2e_e[o] = (IdxT)g_f2e_e[base + s];
+    f2e_f[o] = (IdxT)g_f2e_f[base + s];
     f2e_v[o] = 1.0f;
   }
   // the kb_fact_rel row: the stored prefix of the question's row, then the pad relation
@@ -359,112 +392,6 @@ split_fact_order_kernel(const int64_t* __restrict__ off, int64_t num_q, const in
   }
 }
 
-// per question: the kept facts in `order` (stored indices), then the self-loops
-template <typename IdxT>
-__global__ void __launch_bounds__(kSplitThreads)
-split_assemble_ordered_kernel(const int64_t* __restrict__ q_off, const int32_t* __restrict__ q_heads,
-                              const int32_t* __restrict__ q_rels, const int32_t* __restrict__ q_tails,
-                              const int32_t* __restrict__ q_ents, int64_t num_q, const int64_t* __restrict__ ids,
-                              const int64_t* __restrict__ kept, const int32_t* __restrict__ order, int64_t K,
-                              int64_t N, int64_t self_rel, int use_self_loop, int64_t F, IdxT* __restrict__ heads,
-                              IdxT* __restrict__ rels, IdxT* __restrict__ tails, IdxT* __restrict__ bids,
-                              IdxT* __restrict__ fids, int32_t* __restrict__ status) {
-  __shared__ int64_t s_red[33];
-  const int b = blockIdx.y;
-  auto stored = [&](int64_t id) -> int64_t { return valid_id(id, num_q) ? q_off[id + 1] - q_off[id] : 0; };
-  auto keep = [&](int j) -> int64_t { return min(max(kept[j], (int64_t)0), stored(ids[j])); };
-  auto ents = [&](int64_t id) -> int64_t { return use_self_loop && valid_id(id, num_q) ? (int64_t)q_ents[id] : 0; };
-  int64_t before = 0, obefore = 0;
-  for (int j = threadIdx.x; j < b; j += blockDim.x) {
-    const int64_t kj = keep(j);
-    obefore += kj;
-    before += kj + ents(ids[j]);
-  }
-  const int64_t pos = block_sum(before, s_red);
-  const int64_t opos = block_sum(obefore, s_red);
-  const int64_t id = ids[b];
-  const bool ok = valid_id(id, num_q);
-  const int64_t base = ok ? q_off[id] : 0, nf = stored(id), k = keep(b), tot = k + ents(id);
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    if (!ok) atomicOr(status, 1);
-    if (pos + tot > F || opos + k > K) atomicOr(status, 2);
-  }
-  const int64_t bias = (int64_t)b * N;
-  const int64_t end = min(tot, F - pos);
-  for (int64_t kk = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; kk < end; kk += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t o = pos + kk;
-    int64_t h, r, t;
-    if (kk < k) {
-      if (opos + kk >= K) continue;            // past the order array (flagged above)
-      const int64_t s = order[opos + kk];
-      if (s < 0 || s >= nf) {                  // not a stored index of this question: not read, not written
-        atomicOr(status, 1);
-        continue;
-      }
-      h = bias + q_heads[base + s];
-      r = q_rels[base + s];
-      t = bias + q_tails[base + s];
-    } else {
-      h = t = bias + (kk - k);
-      r = self_rel;
-    }
-    heads[o] = (IdxT)h;
-    rels[o] = (IdxT)r;
-    tails[o] = (IdxT)t;
-    bids[o] = (IdxT)b;
-    fids[o] = (IdxT)o;
-  }
-}
-
-// both graft lists at the positions in `order`; kb_fact_rel rows as split_assemble_graft_kernel
-template <typename IdxT>
-__global__ void __launch_bounds__(kSplitThreads)
-split_assemble_graft_ordered_kernel(const int64_t* __restrict__ g_off, const int32_t* __restrict__ g_e2f_f,
-                                    const int32_t* __restrict__ g_e2f_e, const int32_t* __restrict__ g_f2e_e,
-                                    const int32_t* __restrict__ g_f2e_f, const int64_t* __restrict__ r_off,
-                                    const int32_t* __restrict__ r_vals, int64_t num_q, const int64_t* __restrict__ ids,
-                                    const int64_t* __restrict__ kept, const int32_t* __restrict__ order, int64_t K,
-                                    int64_t max_facts, int64_t rel_pad, int64_t G, IdxT* __restrict__ e2f_b,
-                                    IdxT* __restrict__ e2f_f, IdxT* __restrict__ e2f_e, float* __restrict__ e2f_v,
-                                    IdxT* __restrict__ f2e_b, IdxT* __restrict__ f2e_e, IdxT* __restrict__ f2e_f,
-                                    float* __restrict__ f2e_v, int64_t* __restrict__ kb_fact_rel,
-                                    int32_t* __restrict__ status) {
-  __shared__ int64_t s_red[33];
-  const int b = blockIdx.y;
-  auto stored = [&](int64_t id) -> int64_t { return valid_id(id, num_q) ? g_off[id + 1] - g_off[id] : 0; };
-  auto keep = [&](int j) -> int64_t { return min(max(kept[j], (int64_t)0), stored(ids[j])); };
-  int64_t before = 0;
-  for (int j = threadIdx.x; j < b; j += blockDim.x) before += keep(j);
-  const int64_t pos = block_sum(before, s_red);      // the lists and the order share one layout
-  const int64_t id = ids[b];
-  const bool ok = valid_id(id, num_q);
-  const int64_t base = ok ? g_off[id] : 0, n = stored(id), k = keep(b);
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    if (!ok) atomicOr(status, 1);
-    if (pos + k > G || pos + k > K) atomicOr(status, 2);
-  }
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x, k0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t end = min(k, min(G, K) - pos);
-  for (int64_t kk = k0; kk < end; kk += stride) {
-    const int64_t o = pos + kk, s = order[o];
-    if (s < 0 || s >= n) {
-      atomicOr(status, 1);
-      continue;
-    }
-    e2f_b[o] = (IdxT)b;
-    e2f_f[o] = (IdxT)g_e2f_f[base + s];
-    e2f_e[o] = (IdxT)g_e2f_e[base + s];
-    e2f_v[o] = 1.0f;
-    f2e_b[o] = (IdxT)b;
-    f2e_e[o] = (IdxT)g_f2e_e[base + s];
-    f2e_f[o] = (IdxT)g_f2e_f[base + s];
-    f2e_v[o] = 1.0f;
-  }
-  const int64_t rbase = ok ? r_off[id] : 0, rlen = ok ? min(r_off[id + 1] - rbase, max_facts) : 0;
-  int64_t* row = kb_fact_rel + (int64_t)b * max_facts;
-  for (int64_t j = k0; j < max_facts; j += stride) row[j] = j < rlen ? (int64_t)r_vals[rbase + j] : rel_pad;
-}
-
 static size_t order_workspace_key_bytes(int64_t n_total) {
   return align_up((size_t)std::max<int64_t>(n_total, 1) * sizeof(unsigned long long), 256);
 }
@@ -491,6 +418,70 @@ static WeightWorkspace weight_workspace(int64_t F, int64_t Nt) {
   return w;
 }
 
+// gr_split_assemble (kept and order null, K = 0: stored order) and gr_split_assemble_ordered: one validation and one
+// launch, the messages reported as the calling entry point `fn`.  The ordered entry point refuses a null `kept` itself.
+int split_assemble_launch(const char* fn, const int64_t* q_off, const int32_t* q_heads, const int32_t* q_rels,
+                          const int32_t* q_tails, const int32_t* q_ents, int64_t num_q, const int64_t* ids,
+                          const int64_t* kept, const int32_t* order, int64_t K, int B, int64_t N, int64_t self_rel,
+                          int use_self_loop, int idx_bytes, int64_t F, void* heads, void* rels, void* tails,
+                          void* batch_ids, void* fact_ids, int32_t* status, cudaStream_t stream) {
+  GR_CHECK_ARG_AS(fn, q_off && ids && status, "null pointer");
+  GR_CHECK_ARG_AS(fn, num_q >= 0 && B > 0 && N > 0 && F >= 0 && K >= 0,
+                  kept ? "need num_q >= 0, B > 0, N > 0, F >= 0 and K >= 0"
+                       : "need num_q >= 0, B > 0, N > 0 and F >= 0");
+  GR_CHECK_ARG_AS(fn, idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+  GR_CHECK_ARG_AS(fn, idx_bytes == 8 || ((int64_t)B * N <= INT_MAX && F <= INT_MAX && self_rel <= INT_MAX),
+                  "the batch overflows int32 indices");
+  GR_CHECK_ARG_AS(fn, self_rel >= 0, "self_rel must be non-negative");
+  GR_CHECK_ARG_AS(fn, F == 0 || (heads && rels && tails && batch_ids && fact_ids), "null output arrays");
+  GR_CHECK_ARG_AS(fn, K == 0 || order, "null order");
+  GR_CHECK_ARG_AS(fn, q_heads && q_rels && q_tails && q_ents, "null resident arrays");
+  const dim3 grid(ctas_per_question(B), B);
+  auto go = [&](auto t) {
+    using IdxT = typename decltype(t)::type;
+    const auto kernel = kept ? split_assemble_kernel<IdxT, true> : split_assemble_kernel<IdxT, false>;
+    kernel<<<grid, kSplitThreads, 0, stream>>>(q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, kept, order, K, N,
+                                               self_rel, use_self_loop, F, (IdxT*)heads, (IdxT*)rels, (IdxT*)tails,
+                                               (IdxT*)batch_ids, (IdxT*)fact_ids, status);
+  };
+  idx_bytes == 8 ? go(type_tag<int64_t>{}) : go(type_tag<int32_t>{});
+  GR_CHECK_LAUNCH_AS(fn);
+  return GR_OK;
+}
+
+// gr_split_assemble_graft and gr_split_assemble_graft_ordered, as split_assemble_launch
+int split_assemble_graft_launch(const char* fn, const int64_t* g_off, const int32_t* g_e2f_f, const int32_t* g_e2f_e,
+                                const int32_t* g_f2e_e, const int32_t* g_f2e_f, const int64_t* r_off,
+                                const int32_t* r_vals, int64_t num_q, const int64_t* ids, const int64_t* kept,
+                                const int32_t* order, int64_t K, int B, int64_t max_facts, int64_t rel_pad,
+                                int idx_bytes, int64_t G, void* e2f_b, void* e2f_f, void* e2f_e, float* e2f_v,
+                                void* f2e_b, void* f2e_e, void* f2e_f, float* f2e_v, int64_t* kb_fact_rel,
+                                int32_t* status, cudaStream_t stream) {
+  GR_CHECK_ARG_AS(fn, g_off && r_off && ids && status, "null pointer");
+  GR_CHECK_ARG_AS(fn, g_e2f_f && g_e2f_e && g_f2e_e && g_f2e_f && r_vals, "null resident arrays");
+  GR_CHECK_ARG_AS(fn, num_q >= 0 && B > 0 && max_facts >= 0 && G >= 0 && K >= 0,
+                  kept ? "need num_q >= 0, B > 0, max_facts >= 0, G >= 0 and K >= 0"
+                       : "need num_q >= 0, B > 0, max_facts >= 0 and G >= 0");
+  GR_CHECK_ARG_AS(fn, idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+  GR_CHECK_ARG_AS(fn, idx_bytes == 8 || (G <= INT_MAX && max_facts <= INT_MAX), "the batch overflows int32 indices");
+  GR_CHECK_ARG_AS(fn, G == 0 || (e2f_b && e2f_f && e2f_e && e2f_v && f2e_b && f2e_e && f2e_f && f2e_v),
+                  "null output arrays");
+  GR_CHECK_ARG_AS(fn, K == 0 || order, "null order");
+  GR_CHECK_ARG_AS(fn, max_facts == 0 || kb_fact_rel, "null kb_fact_rel");
+  const dim3 grid(ctas_per_question(B), B);
+  auto go = [&](auto t) {
+    using IdxT = typename decltype(t)::type;
+    const auto kernel = kept ? split_assemble_graft_kernel<IdxT, true> : split_assemble_graft_kernel<IdxT, false>;
+    kernel<<<grid, kSplitThreads, 0, stream>>>(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q, ids,
+                                               kept, order, K, max_facts, rel_pad, G, (IdxT*)e2f_b, (IdxT*)e2f_f,
+                                               (IdxT*)e2f_e, e2f_v, (IdxT*)f2e_b, (IdxT*)f2e_e, (IdxT*)f2e_f, f2e_v,
+                                               kb_fact_rel, status);
+  };
+  idx_bytes == 8 ? go(type_tag<int64_t>{}) : go(type_tag<int32_t>{});
+  GR_CHECK_LAUNCH_AS(fn);
+  return GR_OK;
+}
+
 }  // namespace
 }  // namespace gr
 
@@ -499,27 +490,9 @@ extern "C" int gr_split_assemble(const int64_t* q_off, const int32_t* q_heads, c
                                  int B, int64_t N, int64_t self_rel, int use_self_loop, int idx_bytes, int64_t F,
                                  void* heads, void* rels, void* tails, void* batch_ids, void* fact_ids,
                                  int32_t* status, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(q_off && ids && status, "null pointer");
-  GR_CHECK_ARG(num_q >= 0 && B > 0 && N > 0 && F >= 0, "need num_q >= 0, B > 0, N > 0 and F >= 0");
-  GR_CHECK_ARG(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
-  GR_CHECK_ARG(idx_bytes == 8 || ((int64_t)B * N <= INT_MAX && F <= INT_MAX && self_rel <= INT_MAX),
-               "the batch overflows int32 indices");
-  GR_CHECK_ARG(self_rel >= 0, "self_rel must be non-negative");
-  GR_CHECK_ARG(F == 0 || (heads && rels && tails && batch_ids && fact_ids), "null output arrays");
-  GR_CHECK_ARG(q_heads && q_rels && q_tails && q_ents, "null resident arrays");
-  const dim3 grid(ctas_per_question(B), B);
-  if (idx_bytes == 8)
-    split_assemble_kernel<int64_t><<<grid, kSplitThreads, 0, stream>>>(
-        q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, N, self_rel, use_self_loop, F, (int64_t*)heads,
-        (int64_t*)rels, (int64_t*)tails, (int64_t*)batch_ids, (int64_t*)fact_ids, status);
-  else
-    split_assemble_kernel<int32_t><<<grid, kSplitThreads, 0, stream>>>(
-        q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, N, self_rel, use_self_loop, F, (int32_t*)heads,
-        (int32_t*)rels, (int32_t*)tails, (int32_t*)batch_ids, (int32_t*)fact_ids, status);
-  GR_CHECK_LAUNCH();
-  return GR_OK;
+  return gr::split_assemble_launch(__func__, q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, nullptr, nullptr, 0,
+                                   B, N, self_rel, use_self_loop, idx_bytes, F, heads, rels, tails, batch_ids,
+                                   fact_ids, status, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int gr_split_assemble_graft(const int64_t* g_off, const int32_t* g_e2f_f, const int32_t* g_e2f_e,
@@ -528,29 +501,10 @@ extern "C" int gr_split_assemble_graft(const int64_t* g_off, const int32_t* g_e2
                                        int64_t max_facts, int64_t rel_pad, int idx_bytes, int64_t G, void* e2f_b,
                                        void* e2f_f, void* e2f_e, float* e2f_v, void* f2e_b, void* f2e_e, void* f2e_f,
                                        float* f2e_v, int64_t* kb_fact_rel, int32_t* status, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(g_off && r_off && ids && status, "null pointer");
-  GR_CHECK_ARG(g_e2f_f && g_e2f_e && g_f2e_e && g_f2e_f && r_vals, "null resident arrays");
-  GR_CHECK_ARG(num_q >= 0 && B > 0 && max_facts >= 0 && G >= 0, "need num_q >= 0, B > 0, max_facts >= 0 and G >= 0");
-  GR_CHECK_ARG(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
-  GR_CHECK_ARG(idx_bytes == 8 || (G <= INT_MAX && max_facts <= INT_MAX), "the batch overflows int32 indices");
-  GR_CHECK_ARG(G == 0 || (e2f_b && e2f_f && e2f_e && e2f_v && f2e_b && f2e_e && f2e_f && f2e_v),
-               "null output arrays");
-  GR_CHECK_ARG(max_facts == 0 || kb_fact_rel, "null kb_fact_rel");
-  const dim3 grid(ctas_per_question(B), B);
-  if (idx_bytes == 8)
-    split_assemble_graft_kernel<int64_t><<<grid, kSplitThreads, 0, stream>>>(
-        g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q, ids, max_facts, rel_pad, G,
-        (int64_t*)e2f_b, (int64_t*)e2f_f, (int64_t*)e2f_e, e2f_v, (int64_t*)f2e_b, (int64_t*)f2e_e, (int64_t*)f2e_f,
-        f2e_v, kb_fact_rel, status);
-  else
-    split_assemble_graft_kernel<int32_t><<<grid, kSplitThreads, 0, stream>>>(
-        g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q, ids, max_facts, rel_pad, G,
-        (int32_t*)e2f_b, (int32_t*)e2f_f, (int32_t*)e2f_e, e2f_v, (int32_t*)f2e_b, (int32_t*)f2e_e, (int32_t*)f2e_f,
-        f2e_v, kb_fact_rel, status);
-  GR_CHECK_LAUNCH();
-  return GR_OK;
+  return gr::split_assemble_graft_launch(__func__, g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q,
+                                         ids, nullptr, nullptr, 0, B, max_facts, rel_pad, idx_bytes, G, e2f_b, e2f_f,
+                                         e2f_e, e2f_v, f2e_b, f2e_e, f2e_f, f2e_v, kb_fact_rel, status,
+                                         reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" size_t gr_fact_weights_workspace_bytes(int64_t F, int64_t Nt) {
@@ -645,28 +599,10 @@ extern "C" int gr_split_assemble_ordered(const int64_t* q_off, const int32_t* q_
                                          int B, int64_t N, int64_t self_rel, int use_self_loop, int idx_bytes,
                                          int64_t F, void* heads, void* rels, void* tails, void* batch_ids,
                                          void* fact_ids, int32_t* status, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(q_off && ids && kept && status, "null pointer");
-  GR_CHECK_ARG(num_q >= 0 && B > 0 && N > 0 && F >= 0 && K >= 0, "need num_q >= 0, B > 0, N > 0, F >= 0 and K >= 0");
-  GR_CHECK_ARG(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
-  GR_CHECK_ARG(idx_bytes == 8 || ((int64_t)B * N <= INT_MAX && F <= INT_MAX && self_rel <= INT_MAX),
-               "the batch overflows int32 indices");
-  GR_CHECK_ARG(self_rel >= 0, "self_rel must be non-negative");
-  GR_CHECK_ARG(F == 0 || (heads && rels && tails && batch_ids && fact_ids), "null output arrays");
-  GR_CHECK_ARG(K == 0 || order, "null order");
-  GR_CHECK_ARG(q_heads && q_rels && q_tails && q_ents, "null resident arrays");
-  const dim3 grid(ctas_per_question(B), B);
-  if (idx_bytes == 8)
-    split_assemble_ordered_kernel<int64_t><<<grid, kSplitThreads, 0, stream>>>(
-        q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, kept, order, K, N, self_rel, use_self_loop, F,
-        (int64_t*)heads, (int64_t*)rels, (int64_t*)tails, (int64_t*)batch_ids, (int64_t*)fact_ids, status);
-  else
-    split_assemble_ordered_kernel<int32_t><<<grid, kSplitThreads, 0, stream>>>(
-        q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, kept, order, K, N, self_rel, use_self_loop, F,
-        (int32_t*)heads, (int32_t*)rels, (int32_t*)tails, (int32_t*)batch_ids, (int32_t*)fact_ids, status);
-  GR_CHECK_LAUNCH();
-  return GR_OK;
+  GR_CHECK_ARG(kept, "null pointer");
+  return gr::split_assemble_launch(__func__, q_off, q_heads, q_rels, q_tails, q_ents, num_q, ids, kept, order, K, B,
+                                   N, self_rel, use_self_loop, idx_bytes, F, heads, rels, tails, batch_ids, fact_ids,
+                                   status, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int gr_split_assemble_graft_ordered(const int64_t* g_off, const int32_t* g_e2f_f, const int32_t* g_e2f_e,
@@ -677,29 +613,9 @@ extern "C" int gr_split_assemble_graft_ordered(const int64_t* g_off, const int32
                                                void* e2f_b, void* e2f_f, void* e2f_e, float* e2f_v, void* f2e_b,
                                                void* f2e_e, void* f2e_f, float* f2e_v, int64_t* kb_fact_rel,
                                                int32_t* status, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(g_off && r_off && ids && kept && status, "null pointer");
-  GR_CHECK_ARG(g_e2f_f && g_e2f_e && g_f2e_e && g_f2e_f && r_vals, "null resident arrays");
-  GR_CHECK_ARG(num_q >= 0 && B > 0 && max_facts >= 0 && G >= 0 && K >= 0,
-               "need num_q >= 0, B > 0, max_facts >= 0, G >= 0 and K >= 0");
-  GR_CHECK_ARG(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
-  GR_CHECK_ARG(idx_bytes == 8 || (G <= INT_MAX && max_facts <= INT_MAX), "the batch overflows int32 indices");
-  GR_CHECK_ARG(G == 0 || (e2f_b && e2f_f && e2f_e && e2f_v && f2e_b && f2e_e && f2e_f && f2e_v),
-               "null output arrays");
-  GR_CHECK_ARG(K == 0 || order, "null order");
-  GR_CHECK_ARG(max_facts == 0 || kb_fact_rel, "null kb_fact_rel");
-  const dim3 grid(ctas_per_question(B), B);
-  if (idx_bytes == 8)
-    split_assemble_graft_ordered_kernel<int64_t><<<grid, kSplitThreads, 0, stream>>>(
-        g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q, ids, kept, order, K, max_facts, rel_pad, G,
-        (int64_t*)e2f_b, (int64_t*)e2f_f, (int64_t*)e2f_e, e2f_v, (int64_t*)f2e_b, (int64_t*)f2e_e, (int64_t*)f2e_f,
-        f2e_v, kb_fact_rel, status);
-  else
-    split_assemble_graft_ordered_kernel<int32_t><<<grid, kSplitThreads, 0, stream>>>(
-        g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q, ids, kept, order, K, max_facts, rel_pad, G,
-        (int32_t*)e2f_b, (int32_t*)e2f_f, (int32_t*)e2f_e, e2f_v, (int32_t*)f2e_b, (int32_t*)f2e_e, (int32_t*)f2e_f,
-        f2e_v, kb_fact_rel, status);
-  GR_CHECK_LAUNCH();
-  return GR_OK;
+  GR_CHECK_ARG(kept, "null pointer");
+  return gr::split_assemble_graft_launch(__func__, g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, num_q,
+                                         ids, kept, order, K, B, max_facts, rel_pad, idx_bytes, G, e2f_b, e2f_f,
+                                         e2f_e, e2f_v, f2e_b, f2e_e, f2e_f, f2e_v, kb_fact_rel, status,
+                                         reinterpret_cast<cudaStream_t>(stream_));
 }

@@ -439,16 +439,14 @@ class DeviceSplit:
         names = ("local_entity", "query_entities", "seed_dist", "answer_dist", "q_input")
         gathered = tuple(torch.index_select(r[n], 0, rows, out=None if out is None else getattr(out, n)) for n in names)
         fo = None if out is None else (out.heads, out.rels, out.tails, None, None)
+        order = ost = None
         if self.shuffle:
             order, ost = ops.split_fact_order(r["q_off"], ids, kept, seed, 0, n_total, K)
-            *kb, status = ops.split_assemble_ordered(
-                r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, kept, order, N, F,
-                self.self_rel, self.use_self_loop, idt, out=fo)
+        *kb, status = ops.split_assemble(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, N, F,
+                                         self.self_rel, self.use_self_loop, idt, out=fo,
+                                         kept=kept if self.shuffle else None, order=order)
+        if ost is not None:
             status = status | ost
-        else:
-            order = None
-            *kb, status = ops.split_assemble(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, N,
-                                             F, self.self_rel, self.use_self_loop, idt, out=fo)
         w = wr = None
         if self.weights == "arrays":
             if out is not None:
@@ -477,13 +475,14 @@ class DeviceSplit:
         r = self._res
         lists = (r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"])
         idt = None if out is not None else self.index_dtype
+        order = ost = None
         if self.shuffle:
             order, ost = ops.split_fact_order(r["g_off"], ids, kept_g, seed, 1, n_total, G)
-            graft, kfr, status = ops.split_assemble_graft_ordered(*lists, ids, kept_g, order, self.max_facts,
-                                                                  self.rel_pad, G, idt, out=out)
-            return graft, kfr, order, status | ost
-        graft, kfr, status = ops.split_assemble_graft(*lists, ids, self.max_facts, self.rel_pad, G, idt, out=out)
-        return graft, kfr, None, status
+        graft, kfr, status = ops.split_assemble_graft(*lists, ids, self.max_facts, self.rel_pad, G, idt, out=out,
+                                                      kept=kept_g if self.shuffle else None, order=order)
+        if ost is not None:
+            status = status | ost
+        return graft, kfr, order, status
 
     def get_batch(self, iteration, batch_size, fact_dropout, q_type=None, test=False, seed=None):
         """The loader's ``get_batch`` from the resident split (see the class docstring).  ``seed``: with ``shuffle``,

@@ -1021,27 +1021,44 @@ def _split_out(out, F, index_dtype, dev):
     return out
 
 
-def split_assemble(q_off, q_heads, q_rels, q_tails, q_ents, ids, N, F, self_rel, use_self_loop, index_dtype, out=None):
+def _split_order(fn, kept, order, B):
+    """(kept, order) of an assembly through a fact order, checked: both or neither; kept int64 [B], order int32."""
+    if (kept is None) != (order is None):
+        raise RuntimeError("%s: kept and order come together, got only %s" % (fn, "order" if kept is None else "kept"))
+    if kept is None:
+        return None, None
+    kept = _cuda(kept, torch.int64, "kept").contiguous()
+    if kept.numel() != B:
+        raise RuntimeError("%s: need kept [B], got B=%d kept %s" % (fn, B, list(kept.shape)))
+    return kept, _cuda(order, torch.int32, "order").contiguous()
+
+
+def split_assemble(q_off, q_heads, q_rels, q_tails, q_ents, ids, N, F, self_rel, use_self_loop, index_dtype, out=None,
+                   kept=None, order=None):
     """-> (heads, rels, tails, batch_ids, fact_ids, status): the fact arrays of the questions ``ids`` (int64 [B] on the
     device) of a resident split (gr_split_assemble), each [F] in ``index_dtype``; ``status`` int32[1] on the device
     (bit 1: an id out of range, bit 2: more facts than F).  q_off int64 [num_q+1]; q_heads/q_rels/q_tails int32 (local
     ids, by question); q_ents int32 [num_q].  ``out``: optional five [F] tensors (None entries allocated) written in
-    place of new ones."""
+    place of new ones.  ``kept`` (int64 [B]) and ``order`` (int32, :func:`split_fact_order`), given together: question
+    b contributes the facts at the stored indices of its ``kept[b]`` entries of ``order``, then its self-loops
+    (gr_split_assemble_ordered; an order entry that is not a stored index of its question also sets bit 1)."""
     q_off = _cuda(q_off, torch.int64, "q_off").contiguous()
     q_heads, q_rels, q_tails, q_ents = (_cuda(t, torch.int32, n).contiguous() for t, n in
                                         ((q_heads, "q_heads"), (q_rels, "q_rels"), (q_tails, "q_tails"),
                                          (q_ents, "q_ents")))
     ids = _cuda(ids, torch.int64, "ids").contiguous()
     B, num_q = ids.numel(), q_ents.numel()
+    kept, order = _split_order("split_assemble", kept, order, B)
     if not split_assemble_ok(B, N, F, index_dtype):
         raise RuntimeError("split_assemble: need B > 0, N > 0, F >= 0 and an int32 / int64 index dtype whose range "
                            "holds B*N and F, got B=%d N=%d F=%d %s" % (B, N, F, index_dtype))
     dev = ids.device
     out = _split_out(out, F, index_dtype, dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
-    _launch("gr_split_assemble", _p(q_off), _p(q_heads), _p(q_rels), _p(q_tails), _p(q_ents), num_q, _p(ids), B,
-            int(N), int(self_rel), int(bool(use_self_loop)), _INDEX_BYTES[index_dtype], int(F),
-            *(_p(t) if F else None for t in out), _p(status), op="split_assemble")
+    through = () if kept is None else (_p(kept), _p(order) if order.numel() else None, order.numel())
+    _launch("gr_split_assemble" if kept is None else "gr_split_assemble_ordered", _p(q_off), _p(q_heads), _p(q_rels),
+            _p(q_tails), _p(q_ents), num_q, _p(ids), *through, B, int(N), int(self_rel), int(bool(use_self_loop)),
+            _INDEX_BYTES[index_dtype], int(F), *(_p(t) if F else None for t in out), _p(status), op="split_assemble")
     return (*out, status)
 
 
@@ -1053,7 +1070,7 @@ def split_assemble_graft_ok(B, max_facts, G, index_dtype):
     return index_dtype == torch.int64 or (G <= _INT32_MAX and max_facts <= _INT32_MAX)
 
 
-def _graft_out(fn, out, B, max_facts, G, index_dtype, dev):
+def _graft_out(out, B, max_facts, G, index_dtype, dev):
     """(the six [G] index lists, the two fp32 [G] value lists, kb_fact_rel int64 [B, max_facts]) of a graft assembly:
     the tensors of ``out`` = ((e2f_b, e2f_f, e2f_e, e2f_v), (f2e_b, f2e_e, f2e_f, f2e_v), kb_fact_rel), checked, or
     new ones without it."""
@@ -1065,54 +1082,60 @@ def _graft_out(fn, out, B, max_facts, G, index_dtype, dev):
     idx, vals = [*e2f[:3], *f2e[:3]], [e2f[3], f2e[3]]
     for i, t in enumerate(idx):
         if not (t.is_cuda and t.dtype == index_dtype and t.is_contiguous() and t.numel() == G):
-            raise RuntimeError("%s: out index list %d must be a contiguous %s [%d] CUDA tensor"
-                               % (fn, i, index_dtype, G))
+            raise RuntimeError("split_assemble_graft: out index list %d must be a contiguous %s [%d] CUDA tensor"
+                               % (i, index_dtype, G))
     for i, t in enumerate(vals):
         if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == G):
-            raise RuntimeError("%s: out value list %d must be a contiguous fp32 [%d] CUDA tensor" % (fn, i, G))
+            raise RuntimeError("split_assemble_graft: out value list %d must be a contiguous fp32 [%d] CUDA tensor"
+                               % (i, G))
     if not (kfr.is_cuda and kfr.dtype == torch.int64 and kfr.is_contiguous() and tuple(kfr.shape) == (B, max_facts)):
-        raise RuntimeError("%s: out kb_fact_rel must be a contiguous int64 [%d, %d] CUDA tensor" % (fn, B, max_facts))
+        raise RuntimeError("split_assemble_graft: out kb_fact_rel must be a contiguous int64 [%d, %d] CUDA tensor"
+                           % (B, max_facts))
     return idx, vals, kfr
 
 
-def _graft_index_dtype(fn, out, index_dtype):
+def _graft_index_dtype(out, index_dtype):
     """The index dtype of a graft assembly: ``out``'s (its six index lists share one), else ``index_dtype``."""
     if out is None:
         return index_dtype
     dts = {t.dtype for t in (*out[0][:3], *out[1][:3])}
     if len(dts) != 1 or (index_dtype is not None and dts != {index_dtype}):
-        raise RuntimeError("%s: the out index lists must share one dtype%s, got %s"
-                           % (fn, "" if index_dtype is None else " (%s)" % index_dtype, sorted(map(str, dts))))
+        raise RuntimeError("split_assemble_graft: the out index lists must share one dtype%s, got %s"
+                           % ("" if index_dtype is None else " (%s)" % index_dtype, sorted(map(str, dts))))
     return dts.pop()
 
 
 def split_assemble_graft(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, ids, max_facts, rel_pad, G,
-                         index_dtype=None, out=None):
+                         index_dtype=None, out=None, kept=None, order=None):
     """-> ((e2f_b, e2f_f, e2f_e, e2f_v), (f2e_b, f2e_e, f2e_f, f2e_v)), kb_fact_rel, status: the graft lists ([G], the
     index entries in ``index_dtype``, the values fp32 1.0) and kb_fact_rel int64 [B, max_facts] of the questions
     ``ids`` of a resident split (gr_split_assemble_graft); ``status`` as :func:`split_assemble`.  ``out``: optional
     tensors in the layout returned, ``((e2f_b, e2f_f, e2f_e, e2f_v), (f2e_b, f2e_e, f2e_f, f2e_v), kb_fact_rel)``,
     written in place of new ones; the index dtype is then theirs, and G their length (a capacity: the batch's entries
-    fill the front, and entries past G are not written and set status bit 2)."""
+    fill the front, and entries past G are not written and set status bit 2).  ``kept`` / ``order`` as in
+    :func:`split_assemble`: both graft lists take question b's entries at its ``kept[b]`` positions of ``order``
+    (gr_split_assemble_graft_ordered); the kb_fact_rel rows are the stored ones."""
     g_off, r_off = _cuda(g_off, torch.int64, "g_off").contiguous(), _cuda(r_off, torch.int64, "r_off").contiguous()
     lists = [_cuda(t, torch.int32, n).contiguous() for t, n in
              ((g_e2f_f, "g_e2f_f"), (g_e2f_e, "g_e2f_e"), (g_f2e_e, "g_f2e_e"), (g_f2e_f, "g_f2e_f"),
               (r_vals, "r_vals"))]
     ids = _cuda(ids, torch.int64, "ids").contiguous()
     B, num_q = ids.numel(), g_off.numel() - 1
-    index_dtype = _graft_index_dtype("split_assemble_graft", out, index_dtype)
+    kept, order = _split_order("split_assemble_graft", kept, order, B)
+    index_dtype = _graft_index_dtype(out, index_dtype)
     if not split_assemble_graft_ok(B, max_facts, G, index_dtype):
         raise RuntimeError("split_assemble_graft: need B > 0, max_facts >= 0, G >= 0 and an int32 / int64 index dtype "
                            "whose range holds G and max_facts, got B=%d max_facts=%d G=%d %s"
                            % (B, max_facts, G, index_dtype))
     dev = ids.device
-    idx, vals, kfr = _graft_out("split_assemble_graft", out, B, max_facts, G, index_dtype, dev)
+    idx, vals, kfr = _graft_out(out, B, max_facts, G, index_dtype, dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
     p = (lambda t: _p(t) if t.numel() else None)     # noqa: E731
-    _launch("gr_split_assemble_graft", _p(g_off), *(_p(t) for t in lists[:4]), _p(r_off), _p(lists[4]), num_q,
-            _p(ids), B, int(max_facts), int(rel_pad), _INDEX_BYTES[index_dtype], int(G),
-            p(idx[0]), p(idx[1]), p(idx[2]), p(vals[0]), p(idx[3]), p(idx[4]), p(idx[5]), p(vals[1]), p(kfr),
-            _p(status), op="split_assemble")
+    through = () if kept is None else (_p(kept), p(order), order.numel())
+    _launch("gr_split_assemble_graft" if kept is None else "gr_split_assemble_graft_ordered", _p(g_off),
+            *(_p(t) for t in lists[:4]), _p(r_off), _p(lists[4]), num_q, _p(ids), *through, B, int(max_facts),
+            int(rel_pad), _INDEX_BYTES[index_dtype], int(G), p(idx[0]), p(idx[1]), p(idx[2]), p(vals[0]), p(idx[3]),
+            p(idx[4]), p(idx[5]), p(vals[1]), p(kfr), _p(status), op="split_assemble")
     return ((idx[0], idx[1], idx[2], vals[0]), (idx[3], idx[4], idx[5], vals[1])), kfr, status
 
 
@@ -1141,58 +1164,6 @@ def split_fact_order(off, ids, kept, seed, perm, n_total, K):
     _launch("gr_split_fact_order", _p(off), num_q, _p(ids), _p(kept), B, _p(seed), int(perm), int(n_total), int(K),
             _p(order) if K else None, _p(status), _p(ws), nbytes, op="split_assemble")
     return order, status
-
-
-def split_assemble_ordered(q_off, q_heads, q_rels, q_tails, q_ents, ids, kept, order, N, F, self_rel, use_self_loop,
-                           index_dtype, out=None):
-    """:func:`split_assemble` with question b contributing the facts at the stored indices of its ``kept[b]`` entries
-    of ``order`` (:func:`split_fact_order`), then its self-loops (gr_split_assemble_ordered).  Shape rule:
-    :func:`split_assemble_ok`; ``out`` as there."""
-    q_off = _cuda(q_off, torch.int64, "q_off").contiguous()
-    q_heads, q_rels, q_tails, q_ents = (_cuda(t, torch.int32, n).contiguous() for t, n in
-                                        ((q_heads, "q_heads"), (q_rels, "q_rels"), (q_tails, "q_tails"),
-                                         (q_ents, "q_ents")))
-    ids, kept = _cuda(ids, torch.int64, "ids").contiguous(), _cuda(kept, torch.int64, "kept").contiguous()
-    order = _cuda(order, torch.int32, "order").contiguous()
-    B, num_q, K = ids.numel(), q_ents.numel(), order.numel()
-    if not split_assemble_ok(B, N, F, index_dtype) or kept.numel() != B:
-        raise RuntimeError("split_assemble_ordered: need B > 0, kept [B], N > 0, F >= 0 and an int32 / int64 index "
-                           "dtype whose range holds B*N and F, got B=%d N=%d F=%d %s" % (B, N, F, index_dtype))
-    dev = ids.device
-    out = _split_out(out, F, index_dtype, dev)
-    status = torch.zeros(1, dtype=torch.int32, device=dev)
-    _launch("gr_split_assemble_ordered", _p(q_off), _p(q_heads), _p(q_rels), _p(q_tails), _p(q_ents), num_q, _p(ids),
-            _p(kept), _p(order) if K else None, K, B, int(N), int(self_rel), int(bool(use_self_loop)),
-            _INDEX_BYTES[index_dtype], int(F), *(_p(t) if F else None for t in out), _p(status), op="split_assemble")
-    return (*out, status)
-
-
-def split_assemble_graft_ordered(g_off, g_e2f_f, g_e2f_e, g_f2e_e, g_f2e_f, r_off, r_vals, ids, kept, order,
-                                 max_facts, rel_pad, G, index_dtype=None, out=None):
-    """:func:`split_assemble_graft` with both graft lists taking question b's entries at its ``kept[b]`` positions of
-    ``order`` (gr_split_assemble_graft_ordered); the kb_fact_rel rows are the stored ones.  Shape rule:
-    :func:`split_assemble_graft_ok`; ``out`` as there."""
-    g_off, r_off = _cuda(g_off, torch.int64, "g_off").contiguous(), _cuda(r_off, torch.int64, "r_off").contiguous()
-    lists = [_cuda(t, torch.int32, n).contiguous() for t, n in
-             ((g_e2f_f, "g_e2f_f"), (g_e2f_e, "g_e2f_e"), (g_f2e_e, "g_f2e_e"), (g_f2e_f, "g_f2e_f"),
-              (r_vals, "r_vals"))]
-    ids, kept = _cuda(ids, torch.int64, "ids").contiguous(), _cuda(kept, torch.int64, "kept").contiguous()
-    order = _cuda(order, torch.int32, "order").contiguous()
-    B, num_q, K = ids.numel(), g_off.numel() - 1, order.numel()
-    index_dtype = _graft_index_dtype("split_assemble_graft_ordered", out, index_dtype)
-    if not split_assemble_graft_ok(B, max_facts, G, index_dtype) or kept.numel() != B:
-        raise RuntimeError("split_assemble_graft_ordered: need B > 0, kept [B], max_facts >= 0, G >= 0 and an int32 / "
-                           "int64 index dtype whose range holds G and max_facts, got B=%d max_facts=%d G=%d %s"
-                           % (B, max_facts, G, index_dtype))
-    dev = ids.device
-    idx, vals, kfr = _graft_out("split_assemble_graft_ordered", out, B, max_facts, G, index_dtype, dev)
-    status = torch.zeros(1, dtype=torch.int32, device=dev)
-    p = (lambda t: _p(t) if t.numel() else None)     # noqa: E731
-    _launch("gr_split_assemble_graft_ordered", _p(g_off), *(_p(t) for t in lists[:4]), _p(r_off), _p(lists[4]),
-            num_q, _p(ids), _p(kept), p(order), K, B, int(max_facts), int(rel_pad), _INDEX_BYTES[index_dtype], int(G),
-            p(idx[0]), p(idx[1]), p(idx[2]), p(vals[0]), p(idx[3]), p(idx[4]), p(idx[5]), p(vals[1]), p(kfr),
-            _p(status), op="split_assemble")
-    return ((idx[0], idx[1], idx[2], vals[0]), (idx[3], idx[4], idx[5], vals[1])), kfr, status
 
 
 def fact_weights_ok(F, Nt):

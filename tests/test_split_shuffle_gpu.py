@@ -390,7 +390,7 @@ def test_get_batch_and_submit_do_not_synchronise(name):
 
 # ---- status word -------------------------------------------------------------------------------------------------------
 
-def test_ordered_path_status_word():
+def test_ordered_assembly_status_word():
     L = SplitLoader(seed=3, num_questions=4, max_local_entity=12, facts_lo=5, facts_hi=30)
     split = loader.DeviceSplit(L, dev, shuffle=True)
     r, st = split._res, split._stored
@@ -403,8 +403,8 @@ def test_ordered_path_status_word():
         K_ = int(sum(min(k, st[i]) for i, k in zip(bad, kept) if 0 <= i < 4)) if K is None else K
         order, ost = ops.split_fact_order(r["q_off"], ids, kept_t, seed, 0, int(st[good].sum()), K_)
         F_ = K_ + int(split._ents[good].sum()) if F is None else F
-        out = ops.split_assemble_ordered(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids,
-                                         kept_t, order, 12, F_, NR_SELF, True, torch.int32)
+        out = ops.split_assemble(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, 12, F_,
+                                 NR_SELF, True, torch.int32, kept=kept_t, order=order)
         return int(ost.item()), int(out[5].item())
 
     NR_SELF = split.self_rel
@@ -418,8 +418,8 @@ def test_ordered_path_status_word():
     ids = torch.tensor([0, 1], dtype=torch.int64, device=dev)
     kept = torch.tensor([2, 2], dtype=torch.int64, device=dev)
     order = torch.tensor([0, 1, 0, int(st[1])], dtype=torch.int32, device=dev)
-    out = ops.split_assemble_ordered(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, kept,
-                                     order, 12, 4 + int(split._ents[[0, 1]].sum()), NR_SELF, True, torch.int32)
+    out = ops.split_assemble(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, 12,
+                             4 + int(split._ents[[0, 1]].sum()), NR_SELF, True, torch.int32, kept=kept, order=order)
     assert int(out[5].item()) == 1
     G_ = GraftSplitLoader(seed=5, num_questions=3, max_local_entity=9, facts_lo=5)
     gs = loader.DeviceSplit(G_, dev, shuffle=True)
@@ -427,11 +427,74 @@ def test_ordered_path_status_word():
     ids = torch.tensor([0, 3], dtype=torch.int64, device=dev)
     kept = torch.tensor([2, 2], dtype=torch.int64, device=dev)
     gorder, ost = ops.split_fact_order(r["g_off"], ids, kept, seed, 1, int(gs._graft_count[0]), 2)
-    _g, kfr, gst = ops.split_assemble_graft_ordered(r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"],
-                                                    r["g_f2e_f"], r["r_off"], r["r_vals"], ids, kept, gorder,
-                                                    gs.max_facts, gs.rel_pad, 2, torch.int32)
+    _g, kfr, gst = ops.split_assemble_graft(r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"],
+                                            r["r_off"], r["r_vals"], ids, gs.max_facts, gs.rel_pad, 2, torch.int32,
+                                            kept=kept, order=gorder)
     assert int(ost.item()) == 1 and int(gst.item()) == 1 and bool((kfr[1] == gs.rel_pad).all())
-    _g, _kfr, gst = ops.split_assemble_graft_ordered(r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"],
-                                                     r["g_f2e_f"], r["r_off"], r["r_vals"], ids[:1], kept[:1], gorder,
-                                                     gs.max_facts, gs.rel_pad, 1, torch.int32)
+    _g, _kfr, gst = ops.split_assemble_graft(r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"],
+                                             r["r_off"], r["r_vals"], ids[:1], gs.max_facts, gs.rel_pad, 1,
+                                             torch.int32, kept=kept[:1], order=gorder)
     assert int(gst.item()) == 2
+
+
+# ---- one kernel per list: stored order is the ordered path through the identity order ----------------------------------
+
+@pytest.mark.parametrize("cut,bad", [(0, False), (3, False), (0, True)])
+@pytest.mark.parametrize("index_dtype", [torch.int32, torch.int64])
+def test_stored_order_equals_the_identity_order(index_dtype, cut, bad):
+    """The stored-order assembly and the ordered one at kept = the stored counts through the identity order write the
+    same bits and the same status word, kb facts and graft lists: at the exact capacity, at a capacity ``cut`` short
+    (bit 2) and with an out-of-range id (bit 1).  Outputs start as a sentinel, so unwritten entries compare too."""
+    L = GraftSplitLoader(seed=8, num_questions=5, max_local_entity=16, facts_lo=3, facts_hi=40,
+                         index_dtype=IDX[index_dtype])
+    split = loader.DeviceSplit(L, dev, index_dtype=index_dtype)
+    r = split._res
+    ids_h = np.array([3, 0, 5, 2] if bad else [3, 0, 4, 2])
+    ids, good = torch.tensor(ids_h, device=dev), ids_h[ids_h < 5]
+
+    def identity(stored):
+        n = np.array([stored[i] if i < 5 else 0 for i in ids_h], dtype=np.int64)
+        order = np.concatenate([np.arange(k) for k in n]).astype(np.int32)
+        return dict(kept=torch.tensor(n, device=dev), order=torch.tensor(order, device=dev))
+
+    def bits(ts):
+        return [t.cpu().numpy().view(np.uint8) for t in ts]
+
+    want = (1 if bad else 0) | (2 if cut else 0)
+    F = int(split._count[good].sum()) - cut
+    kb = []
+    for extra in ({}, identity(split._stored)):
+        out = [torch.full((F,), -7, dtype=index_dtype, device=dev) for _ in range(5)]
+        *arrays, st = ops.split_assemble(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids,
+                                         split.N, F, split.self_rel, split.use_self_loop, index_dtype, out=out,
+                                         **extra)
+        kb.append((bits(arrays), int(st.item())))
+    G = int(split._graft_count[good].sum()) - cut
+    lists = (r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"])
+    graft = []
+    for extra in ({}, identity(split._graft_count)):
+        out = tuple(tuple(torch.full((G,), -7, dtype=dt, device=dev) for dt in (index_dtype,) * 3 + (torch.float32,))
+                    for _ in range(2)) + (torch.full((len(ids_h), split.max_facts), -7, device=dev),)
+        (e2f, f2e), kfr, st = ops.split_assemble_graft(*lists, ids, split.max_facts, split.rel_pad, G, out=out,
+                                                       **extra)
+        graft.append((bits((*e2f, *f2e, kfr)), int(st.item())))
+    for name, (stored, ordered) in (("kb", kb), ("graft", graft)):
+        assert stored[1] == ordered[1] == want, name
+        for i, (a, b) in enumerate(zip(stored[0], ordered[0])):
+            np.testing.assert_array_equal(a, b, err_msg="%s[%d]" % (name, i))
+
+
+def test_kept_and_order_come_together():
+    L = GraftSplitLoader(seed=5, num_questions=3, max_local_entity=9, facts_lo=5)
+    split = loader.DeviceSplit(L, dev, shuffle=True)
+    r = split._res
+    ids = torch.tensor([0, 1], dtype=torch.int64, device=dev)
+    kept = torch.tensor([2, 2], dtype=torch.int64, device=dev)
+    order = torch.tensor([0, 1, 0, 1], dtype=torch.int32, device=dev)
+    lists = (r["g_off"], r["g_e2f_f"], r["g_e2f_e"], r["g_f2e_e"], r["g_f2e_f"], r["r_off"], r["r_vals"])
+    for half, only in ((dict(kept=kept), "kept"), (dict(order=order), "order")):
+        with pytest.raises(RuntimeError, match="split_assemble: kept and order come together, got only " + only):
+            ops.split_assemble(r["q_off"], r["q_heads"], r["q_rels"], r["q_tails"], r["q_ents"], ids, split.N, 8,
+                               split.self_rel, True, torch.int32, **half)
+        with pytest.raises(RuntimeError, match="split_assemble_graft: kept and order come together, got only " + only):
+            ops.split_assemble_graft(*lists, ids, split.max_facts, split.rel_pad, 4, torch.int32, **half)

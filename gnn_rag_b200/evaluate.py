@@ -67,9 +67,15 @@ def f1_and_hits(answers, retrieved_ids):
 
 
 class Evaluator:
-    """Drop-in for ``gnn/evaluate.py:Evaluator`` (constructor :70-104, ``write_info`` :106-138, ``evaluate`` :140-240)."""
+    """Drop-in for ``gnn/evaluate.py:Evaluator`` (constructor :70-104, ``write_info`` :106-138, ``evaluate`` :140-240).
 
-    def __init__(self, args, model, entity2id, relation2id, device):
+    ``step``: optionally a ``graphed.GraphedStep`` of ``model`` that ranks with this evaluator's pad id
+    (``len(entity2id)``) and ``eps``.  With it, :meth:`evaluate` over a ``loader.DeviceSplit`` runs the whole split as
+    one evaluation epoch (``GraphedStep.start_eval``: batch assembly, forward, ranking and metrics in CUDA graphs) and
+    builds the ``.info`` rows from its records on the host; it returns the same values and writes the same file as
+    the per-batch loop, which still serves host loaders and evaluators without a step."""
+
+    def __init__(self, args, model, entity2id, relation2id, device, step=None):
         self.model, self.args, self.eps = model, args, args["eps"]
         self.model_name = args["model_name"]
         self.id2entity = {idx: ent for ent, idx in entity2id.items()}
@@ -88,6 +94,16 @@ class Evaluator:
         self.id2relation = id2relation
         self.device = device
         self.file_write = None
+        if step is not None:
+            from .graphed import GraphedStep
+            if not isinstance(step, GraphedStep) or step.model is not model:
+                raise ValueError("Evaluator: step must be a graphed.GraphedStep of this model")
+            if step.num_entity != len(self.id2entity):
+                raise ValueError("Evaluator: the step ranks with pad id %d, the evaluator with %d (len(entity2id))"
+                                 % (step.num_entity, len(self.id2entity)))
+            if step.eps != self.eps:
+                raise ValueError("Evaluator: the step ranks with eps %r, the evaluator with %r" % (step.eps, self.eps))
+        self.step = step
 
     def _name(self, ent):
         return self.id2entity[ent] if self.entity2name is None else self.entity2name[self.id2entity[ent]]
@@ -110,7 +126,25 @@ class Evaluator:
                     obj[j]["action"] = str(act[i])
         return obj_list
 
+    def _open_info(self):
+        if self.file_write is None:
+            path = os.path.join(self.args["checkpoint_dir"], "{}_test.info".format(self.args["experiment_name"]))
+            self.file_write = open(path, "w")
+
+    def _row(self, obj, answers, p, r, f1, hit, em, cand):
+        obj["answers"] = [self._name(a) for a in answers]
+        obj["precison"] = p
+        obj["recall"] = r
+        obj["f1"] = f1
+        obj["hit"] = hit
+        obj["em"] = em
+        obj["cand"] = [(self._name(c), pr) for c, pr in cand.pairs()]
+        self.file_write.write(json.dumps(obj) + "\n")
+
     def evaluate(self, valid_data, test_batch_size=20, write_info=False):
+        from .loader import DeviceSplit
+        if self.step is not None and isinstance(valid_data, DeviceSplit):
+            return self._evaluate_epoch(valid_data, test_batch_size)
         write_info = True                                          # the reference forces it (gnn/evaluate.py:141)
         self.model.eval()
         self.count = 0
@@ -118,9 +152,8 @@ class Evaluator:
         f1s, hits, ems, precisions, recalls = [], [], [], [], []
         valid_data.reset_batches(is_sequential=True)
         num_epoch = math.ceil(valid_data.num_data / test_batch_size)
-        if write_info and self.file_write is None:
-            path = os.path.join(self.args["checkpoint_dir"], "{}_test.info".format(self.args["experiment_name"]))
-            self.file_write = open(path, "w")
+        if write_info:
+            self._open_info()
         case_ct = {}
         num_entity = len(self.id2entity)
         for it in range(num_epoch):
@@ -139,15 +172,7 @@ class Evaluator:
                 answers = list(answer_lists[b])
                 p, r, f1, hit, em, case = f1_and_hits(answers, ret.ent.tolist())
                 if write_info:
-                    obj = obj_list[b]
-                    obj["answers"] = [self._name(a) for a in answers]
-                    obj["precison"] = p
-                    obj["recall"] = r
-                    obj["f1"] = f1
-                    obj["hit"] = hit
-                    obj["em"] = em
-                    obj["cand"] = [(self._name(c), pr) for c, pr in ret.pairs()]
-                    self.file_write.write(json.dumps(obj) + "\n")
+                    self._row(obj_list[b], answers, p, r, f1, hit, em, ret)
                 case_ct[case] = case_ct.get(case, 0) + 1
                 f1s.append(f1); hits.append(hit); ems.append(em); precisions.append(p); recalls.append(r)
         self.case_ct = case_ct
@@ -155,6 +180,30 @@ class Evaluator:
             self.file_write.close()
             self.file_write = None
         return float(np.mean(f1s)), float(np.mean(hits)), float(np.mean(ems))
+
+    def _evaluate_epoch(self, split, test_batch_size):
+        """:meth:`evaluate` over the resident split ``split`` as one evaluation epoch of ``self.step``: the metrics and
+        candidates come from the device records, the ``.info`` rows are built here batch by batch (``get_quest``
+        after setting the loader's ``sample_ids``, as ``get_batch`` sets them)."""
+        self.model.eval()
+        self.count = 0
+        prec, rec, f1, hit, em, cases, retrieved = self.step.evaluate_split(split, test_batch_size)
+        self._open_info()
+        L = split.loader
+        prec, rec, f1l, hitl, eml, cases_l = (a.tolist() for a in (prec, rec, f1, hit, em, cases))
+        case_ct = {}
+        for start in range(0, split.num_data, test_batch_size):
+            L.sample_ids = L.batches[start:min(start + test_batch_size, split.num_data)]
+            obj_list = self.write_info(split, None, self.model.num_iter)    # an eval forward returns tp_list None
+            for b, answers in enumerate(L.answer_lists[L.sample_ids]):
+                i, case = start + b, cases_l[start + b]
+                e = int(eml[i]) if case == 3 else eml[i]          # f1_and_hits: an int in case 3 only
+                self._row(obj_list[b], list(answers), prec[i], rec[i], f1l[i], hitl[i], e, retrieved[i])
+                case_ct[case] = case_ct.get(case, 0) + 1
+        self.case_ct = case_ct
+        self.file_write.close()
+        self.file_write = None
+        return float(np.mean(f1)), float(np.mean(hit)), float(np.mean(em))
 
 
 def merge_candidates(cand1, cand2):

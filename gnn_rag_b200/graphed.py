@@ -494,6 +494,7 @@ class GraphedStep:
         self._d2h_stream = None       # separate: a D2H waiting for graph i must not block the H2D of batch i+1
         self._slot = 0
         self._layout = _layout_for(model)(self)
+        self._evals = {}              # (id(split), batch size) -> _EvalBuffers
 
     # -- the work that gets captured ------------------------------------------------------------------------
     def _run(self, st):
@@ -679,6 +680,151 @@ class GraphedStep:
         res = [Retrieved(idx_h[b, :c], ents_h[b, :c], probs_h[b, :c]) for b, c in enumerate(counts_h.tolist())]
         return res, counts_h.size * 4 + idx_h.size * 8 + probs_h.size * 4 + ents_h.size * 8
 
+    # -- a whole evaluation ------------------------------------------------------------------------------------------
+    def evaluate_split(self, split, batch_size):
+        """One :meth:`start_eval` and one read: -> :meth:`EvalRun.result`.  Raises :meth:`EvalRun.check`'s errors
+        when a batch was malformed."""
+        run = self.start_eval(split, batch_size)
+        out = run.result()
+        run.check()
+        return out
+
+    def _eval_refusal(self, split, batch_size):
+        from .loader import DeviceSplit, same_device
+        if not isinstance(split, DeviceSplit):
+            return "the split must be a loader.DeviceSplit, got %s" % type(split).__name__
+        graft = isinstance(self._layout, _GraftLayout)
+        if split.graft and not graft:
+            return "a ReaRev / NSM model evaluates a kb split; this DeviceSplit holds GraftNet's graft lists"
+        if graft and not split.graft:
+            return "GraftNet evaluates a GraftNet split; this DeviceSplit holds no graft lists"
+        if not same_device(split.device, self.device):
+            return "the split lives on %s, the model on %s" % (split.device, self.device)
+        if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or batch_size <= 0:
+            return "batch_size must be a positive int, got %r" % (batch_size,)
+        if getattr(split.loader, "q_type", "seq") != "seq":
+            return "q_type must be 'seq', got %r" % (split.loader.q_type,)
+        m = self.model
+        if (m.normalized_gnn or m.norm_rel) and split.weights != "arrays":
+            return "normalized_gnn / norm_rel need fact weights: the split was built with weights='none'"
+        return None
+
+    def start_eval(self, split, batch_size):
+        """Start an evaluation of the whole split ``split`` (a ``loader.DeviceSplit``) and return its :class:`EvalRun`
+        without waiting for the device.
+
+        As ``evaluate.Evaluator.evaluate`` over the split: ``model.eval()``, ``split.reset_batches(is_sequential=True)``,
+        then every batch of ``batch_size`` questions in order, the last one short when ``num_data % batch_size != 0``,
+        each assembled as ``split.get_batch(it, batch_size, 0.0)`` assembles it (with ``shuffle``, from a fact-order
+        seed drawn in the graph from torch's CUDA generator and recorded in ``EvalRun.seeds``), run through the
+        serving step of :meth:`__call__` and ranked, and its questions scored against the split's answer lists
+        (``DeviceSplit.answer_table``) as ``evaluate.f1_and_hits`` scores them (gr_eval_step_record).  Each step is
+        one graph replay: gr_epoch_step_begin and the assembly from a device cursor (GraftNet: also
+        gr_epoch_graft_begin and the graft assembly), the forward, the ranking and the records.  The host picks each
+        step's graph, one per (B, fact capacity) and for GraftNet per graft capacity too, from :func:`epoch_plan`;
+        the missing ones are captured before the first replay (the LRU grows to hold them all).  Their key holds the
+        shapes, ``model_key``, ``eps``, the pad id and the ``data_ptr`` of every parameter but not its version: the
+        graphs format the weights they read on each replay (``ops.graph_private_weights``), so they stay valid across
+        in-place ``optimizer.step()`` and ``load_state_dict``.  Once the graphs exist nothing here waits on the device.
+        Afterwards ``split.loader.sample_ids`` is the last batch's.
+
+        Refused (``ValueError``): anything but a CUDA ``DeviceSplit`` on the model's device of the model's family,
+        ``batch_size <= 0``, a ``q_type`` other than ``"seq"``, fact weights (``normalized_gnn`` / ``norm_rel``) over
+        a ``weights="none"`` split, and answers that are not integers."""
+        why = self._eval_refusal(split, batch_size)
+        if why is not None:
+            raise ValueError("start_eval: " + why)
+        answers = split.answer_table()
+        self.model.eval()
+        split.reset_batches(is_sequential=True)
+        L = split.loader
+        order = np.asarray(L.batches[:L.num_data], dtype=np.int64).reshape(-1)
+        plan = epoch_plan(order, split._stored, split._ents, batch_size, 0.0,
+                          split._graft_count if split.graft else None)
+        if split.index_dtype == torch.int32 and plan.steps and (
+                int(plan.B.max()) * split.N > _INT32_MAX or int(plan.F.max()) > _INT32_MAX):
+            raise ValueError("start_eval: a batch overflows int32 indices; use index_dtype=torch.int64")
+        ep = self._eval_buffers(split, batch_size)
+        ep.order.copy_(torch.from_numpy(order), non_blocking=True)
+        entries = self._eval_entries(ep, plan, answers)
+        ep.cursor.zero_()
+        ep.blob.zero_()
+        for ent in entries:
+            ent.g.replay()
+        if plan.steps:
+            s0 = int(plan.starts[-1])
+            L.sample_ids = L.batches[s0:min(s0 + int(batch_size), L.num_data)]
+        return EvalRun(ep.blob.clone(), ep.cand.clone(), None if ep.seeds is None else ep.seeds.clone(), ep.num_data)
+
+    def _eval_buffers(self, split, batch_size):
+        k = (id(split), int(batch_size))
+        ep = self._evals.get(k)
+        if ep is None or ep.split is not split or ep.num_data != split.num_data or ep.pad_id != self.num_entity:
+            ep = self._evals[k] = _EvalBuffers(split, batch_size, self.num_entity)
+        return ep
+
+    def _eval_key(self, ep, shape):
+        m = self.model
+        rel_text = tuple(t.data_ptr() for t in (getattr(m, "rel_features", None), getattr(m, "rel_features_inv", None))
+                         if isinstance(t, torch.Tensor))
+        return (("eval", id(ep)) + self._layout.epoch_key(ep.split, shape) + self._layout.model_key()
+                + (float(self.eps), int(self.num_entity)) + tuple(p.data_ptr() for p in m.parameters()) + rel_text)
+
+    def _eval_entries(self, ep, plan, answers):
+        """The graph of every step of ``plan`` (a list), capturing the missing ones first."""
+        steps = self._layout.epoch_shapes(plan)
+        shapes = {}
+        for s, shape in enumerate(steps):
+            shapes.setdefault(shape, s)
+        self.max_graphs = max(self.max_graphs, len(shapes))
+        ents = {}
+        for shape, s in shapes.items():
+            key = self._eval_key(ep, shape)
+            if key in self._cache:
+                self._cache.move_to_end(key)
+            else:
+                self._eval_capture(ep, shape, s, key, answers)
+            ents[shape] = self._cache[key]
+        return [ents[shape] for shape in steps]
+
+    def _eval_body(self, ep, st, cursor):
+        """One evaluation step over the static buffers ``st``: the assembly and the serving step of :meth:`_run` ->
+        (outs of _run, seed or None, the step's status words: assembly, CSR[, graft staging])."""
+        seed, asm, model_asm = _assemble_step(self._layout, ep, st, cursor, self.device)
+        outs = self._run(st)
+        words = self._layout.epoch_words(st, asm, model_asm, torch.cat(self._layout.status_words(outs[0])))
+        return outs, seed, words
+
+    def _eval_capture(self, ep, shape, s0, key, answers):
+        """Capture the evaluation graph of ``shape`` under ``key``; ``s0``: a step with that shape, the one the
+        warm-up assembles."""
+        _evict(self._cache, self.max_graphs)
+        dev = self.device
+        st = self._layout.epoch_inputs(self._layout.epoch_key(ep.split, shape))
+        rng = torch.cuda.get_rng_state(dev)
+        warm_cursor = torch.full((1,), s0, dtype=torch.int64, device=dev)    # the real cursor does not move
+        with torch.no_grad():
+            _warm_up(lambda: self._eval_body(ep, st, warm_cursor))
+        torch.cuda.set_rng_state(rng, dev)
+        a_off, a_ids = answers
+
+        def captured():
+            outs, seed, words = self._eval_body(ep, st, ep.cursor)
+            db, _loss, _pred, pred_dist, cand_idx, cand_count, _total = outs
+            if len(words) > 2:                   # gr_eval_step_record ORs the first two words (assembly, CSR)
+                ep.status[3:4].bitwise_or_(words[2])
+            ops.eval_step_record(ep.cursor, ep.batch_size, ep.steps, st.ids, db.local_entity, pred_dist, cand_idx,
+                                 cand_count, a_off, a_ids, seed, words[0], words[1], ep.metrics, ep.cases, ep.counts,
+                                 ep.cand_off, ep.cand, ep.cand_total, ep.seeds, ep.status[:3])
+            return outs
+        with torch.no_grad(), ops.graph_private_weights() as private:
+            g, outs = _capture(captured)
+        ent = _Captured()
+        ent.st, ent.g, ent.outs, ent.epoch, ent.pipe = st, g, outs, ep, None
+        ent.weights = private                    # the graph formats the weights into these on every replay
+        ent.planes = live_plane_buffers()        # as GraphedStep._entry: the operand planes the graph relies on
+        self._cache[key] = ent
+
 
 # ---- training ------------------------------------------------------------------------------------------------------
 
@@ -795,15 +941,125 @@ class _EpochBuffers:
         self.f1 = torch.zeros(self.num_data, **f32)
         self.status = torch.zeros(3 if split.graft else 2, dtype=torch.int32, device=dev)
         self.adam = None                 # fp32 [steps, T, 8], made at the first capture (T is known then)
-
-        def largest(counts):             # the stored entries of the batch_size largest questions
-            return int(np.sort(counts)[-self.batch_size:].sum()) if counts.size else 0
         # the fact-order workspaces of any batch
-        self.n_total = largest(split._stored)
+        self.n_total = _largest(split._stored, self.batch_size)
         self.graft_kept_table = self.graft_n_total = None
         if split.graft:
             self.graft_kept_table = torch.zeros(max(split.num_q, 1), **i64) if split.shuffle else None
-            self.graft_n_total = largest(split._graft_count)
+            self.graft_n_total = _largest(split._graft_count, self.batch_size)
+
+
+def _largest(counts, batch_size):
+    """The stored entries of the ``batch_size`` largest questions of ``counts``: a bound on any batch's."""
+    return int(np.sort(counts)[-batch_size:].sum()) if counts.size else 0
+
+
+def _assemble_step(layout, ep, st, cursor, device):
+    """The head of a graphed epoch step over the static buffers ``st`` of ``layout``: gr_epoch_step_begin from the
+    device ``cursor`` into ``ep.order``, the model's head kernels and the batch assembly into ``st`` (the fact-order
+    seed drawn from torch's CUDA generator with ``shuffle``) -> (seed or None, the assembly status word, the model's
+    assembly word or None).  ``ep``: the epoch buffers (:class:`_EpochBuffers`, :class:`_EvalBuffers`)."""
+    split = ep.split
+    r, cap = split._res, st.heads.numel()
+    ops.epoch_step_begin(cursor, ep.order, ep.batch_size, ep.kept_table, r["q_off"], r["q_ents"],
+                         split.use_self_loop, cap, st.ids, st.rows, st.kept, st.nfacts, st.kept_total, st.status)
+    layout.epoch_begin(ep, st)
+    seed = torch.randint(0, 2 ** 62, (1,), device=device) if split.shuffle else None
+    _rows, _kb, _order, asm = split.assemble(st.ids, st.kept, seed, cap, cap, ep.n_total, rows=st.rows, out=st,
+                                             nfacts=st.nfacts)
+    asm = st.status | asm
+    return seed, asm, layout.epoch_assemble(ep, st, seed)
+
+
+class EvalRun:
+    """One evaluation started by :meth:`GraphedStep.start_eval`: device copies of its records, valid once the current
+    stream reaches them.  ``seeds``: int64 [steps], the fact-order seed of each step (None without ``shuffle``).
+    :meth:`result` reads the records back; :meth:`check` raises for a nonzero status."""
+
+    def __init__(self, blob, cand, seeds, num_data):
+        self.blob, self.cand, self.seeds, self.num_data = blob, cand, seeds, num_data
+        self._words = None
+
+    def result(self):
+        """-> ``(precision, recall, f1, hit, em, case, retrieved)`` of every question in batch order: five float64
+        numpy arrays with the values ``evaluate.f1_and_hits`` returns (``em`` as a float), the int8 case (0..3) and
+        one :class:`evaluate.Retrieved` per question.  Reads the device twice at most: the per-question records and
+        the status in one copy, then the candidates in use."""
+        from .evaluate import Retrieved
+        n = self.num_data
+        host = self.blob.cpu().numpy()
+        v = _EvalBuffers.views(host, n)
+        self._words = v["status"].tolist()
+        used = min(int(v["cand_total"][0]), self.cand.shape[0])
+        cand = self.cand[:used].cpu().numpy() if used else np.zeros((0, 2), dtype=np.int64)
+        ent, pair = cand[:, 0], cand[:, 1:].copy().view(np.int32)
+        idx, prob = pair[:, 0].astype(np.int64), pair[:, 1].view(np.float32)
+        retrieved = []
+        for o, c in zip(v["cand_off"].tolist(), v["counts"].tolist()):
+            o, c = (0, 0) if o + c > used else (o, c)          # cut: an overflow, which check() reports
+            retrieved.append(Retrieved(idx[o:o + c], ent[o:o + c], prob[o:o + c]))
+        m = v["metrics"]
+        return m[:, 0].copy(), m[:, 1].copy(), m[:, 2].copy(), m[:, 3].copy(), m[:, 4].copy(), v["cases"].copy(), \
+            retrieved
+
+    def check(self):
+        """Raise ``DeviceSplit.check``'s message when an assembly flagged an id out of range or an overflow, else (for
+        GraftNet) ``GraftGraph``'s when the graft staging rejected a list, else ``GraphedStep``'s when a CSR build
+        flagged ids outside the batch, else when the candidate records overflowed (reads the status unless
+        :meth:`result` has)."""
+        from .loader import DeviceSplit
+        words = self._words
+        if words is None:
+            words = _EvalBuffers.views(self.blob, self.num_data)["status"].tolist()
+        asm, csr, records, staging = words
+        DeviceSplit.raise_status(asm)
+        if staging:
+            ops.GraftGraph.raise_status(staging)
+        if csr:
+            _KbLayout.raise_for([csr])
+        if records:
+            raise RuntimeError("EvalRun: more ranked candidates than the %d candidate records of the split"
+                               % self.cand.shape[0])
+
+
+class _EvalBuffers:
+    """The device state the evaluation graphs of one (split, batch size, pad id) read and write: the cursor, the
+    question order, the records (one byte buffer, so that one copy reads them: float64 [num_data, 5] metrics, int64
+    [num_data] candidate offsets, int64 candidate total, int32 [num_data] candidate counts, int32 [4] status words --
+    assembly, CSR, candidate records, GraftNet's graft staging -- and int8 [num_data] cases) and the candidate records
+    (int64 [capacity, 2], see gr_eval_step_record).  Fixed addresses: the graphs hold them."""
+
+    def __init__(self, split, batch_size, pad_id):
+        dev = split.device
+        self.split, self.batch_size, self.pad_id = split, int(batch_size), int(pad_id)
+        self.num_data = n = int(split.num_data)
+        self.steps = (n + self.batch_size - 1) // self.batch_size
+        self.cursor = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.order = torch.zeros(n, dtype=torch.int64, device=dev)
+        self.kept_table = self.graft_kept_table = None          # every stored fact
+        self.seeds = torch.zeros(self.steps, dtype=torch.int64, device=dev) if split.shuffle else None
+        self.n_total = _largest(split._stored, self.batch_size)
+        self.graft_n_total = _largest(split._graft_count, self.batch_size) if split.graft else None
+        self.blob = torch.zeros(self.nbytes(n), dtype=torch.uint8, device=dev)
+        for name, t in self.views(self.blob, n).items():
+            setattr(self, name, t)
+        from .loader import candidate_capacity
+        self.cand = torch.zeros(max(candidate_capacity(split.loader.candidate_entities, pad_id), 1), 2,
+                                dtype=torch.int64, device=dev)
+
+    @staticmethod
+    def nbytes(n):
+        return 53 * n + 24
+
+    @staticmethod
+    def views(blob, n):
+        """The records of :class:`_EvalBuffers` as views of ``blob`` (a torch uint8 tensor or a numpy uint8 array)."""
+        layout = (("metrics", 0, 40 * n, (n, 5), "float64"), ("cand_off", 40 * n, 8 * n, (n,), "int64"),
+                  ("cand_total", 48 * n, 8, (1,), "int64"), ("counts", 48 * n + 8, 4 * n, (n,), "int32"),
+                  ("status", 52 * n + 8, 16, (4,), "int32"), ("cases", 52 * n + 24, n, (n,), "int8"))
+        if isinstance(blob, torch.Tensor):
+            return {k: blob[o:o + b].view(getattr(torch, dt)).view(shape) for k, o, b, shape, dt in layout}
+        return {k: blob[o:o + b].view(dt).reshape(shape) for k, o, b, shape, dt in layout}
 
 
 def _release_autograd_history(model, params):
@@ -1132,18 +1388,9 @@ class GraphedTrainStep:
     def _epoch_body(self, ep, st, cursor, ac):
         """One step of the epoch over the static buffers ``st``: the head kernels, the batch assembly into ``st`` and
         the captured step of :meth:`_run` -> (outs of _run, seed or None, the step's words of ``EpochRun.status``)."""
-        split, layout = ep.split, self._layout
-        r, cap = split._res, st.heads.numel()
-        ops.epoch_step_begin(cursor, ep.order, ep.batch_size, ep.kept_table, r["q_off"], r["q_ents"],
-                             split.use_self_loop, cap, st.ids, st.rows, st.kept, st.nfacts, st.kept_total, st.status)
-        layout.epoch_begin(ep, st)
-        seed = torch.randint(0, 2 ** 62, (1,), device=self.device) if split.shuffle else None
-        _rows, _kb, _order, asm = split.assemble(st.ids, st.kept, seed, cap, cap, ep.n_total, rows=st.rows, out=st,
-                                                 nfacts=st.nfacts)
-        asm = st.status | asm
-        model_asm = layout.epoch_assemble(ep, st, seed)
+        seed, asm, model_asm = _assemble_step(self._layout, ep, st, cursor, self.device)
         outs = self._run(st, ac)
-        return outs, seed, layout.epoch_words(st, asm, model_asm, outs[5])
+        return outs, seed, self._layout.epoch_words(st, asm, model_asm, outs[5])
 
     def _epoch_capture(self, ep, shape, s0):
         """Capture the epoch graph of ``shape`` (``_KbLayout.epoch_shapes``); ``s0``: a step of the epoch with that

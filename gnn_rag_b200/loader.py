@@ -252,6 +252,32 @@ def kept_counts(n, fact_dropout):
     return np.floor(np.asarray(n, dtype=np.int64) * (1 - float(fact_dropout))).astype(np.int64)
 
 
+def pack_answers(answer_lists):
+    """Per-question answer lists (the loader's ``answer_lists``: global entity ids, possibly outside the subgraph and
+    repeated) -> ``(off, ids)``: int64 [len(answer_lists) + 1] offsets and int64 ids, each question's run sorted
+    ascending with repeats kept, so membership is a binary search and the run's length is ``len(answers)``.  ``ids``
+    keeps one element when there are no answers at all.  Raises ``ValueError`` naming the question when an answer is
+    not an integer or outside int64."""
+    import numbers
+    off = np.zeros(len(answer_lists) + 1, dtype=np.int64)
+    runs = []
+    for q in range(len(answer_lists)):
+        answers = list(answer_lists[q])
+        for a in answers:
+            if not isinstance(a, numbers.Integral) or not -2 ** 63 <= int(a) < 2 ** 63:
+                raise ValueError("DeviceSplit: question %d has an answer that is not an int64 entity id: %r" % (q, a))
+        runs.append(np.sort(np.array([int(a) for a in answers], dtype=np.int64)))
+        off[q + 1] = off[q] + len(answers)
+    ids = np.concatenate(runs) if off[-1] else np.zeros(1, dtype=np.int64)       # a null pointer is refused
+    return off, ids
+
+
+def candidate_capacity(candidate_entities, pad_id):
+    """Candidates an evaluation over a split can retrieve, at most: the entities of its questions'
+    ``candidate_entities`` rows that are not the pad ``pad_id`` (the ranking drops pads and seeds)."""
+    return int(np.count_nonzero(np.asarray(candidate_entities) != pad_id))
+
+
 class DeviceSplit:
     """A split resident in device memory: ``get_batch`` assembles each batch on the GPU from its question ids.
 
@@ -343,6 +369,7 @@ class DeviceSplit:
         if not had_flat:
             del L._gr_flat                                    # flattened here for the upload only
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._answers = None                                  # answer_table(), uploaded by the first evaluation
 
     def _put(self, name, a, dtype):
         import torch
@@ -400,6 +427,14 @@ class DeviceSplit:
 
     def get_quest(self, training=False):
         return self.loader.get_quest(training)
+
+    def answer_table(self):
+        """:func:`pack_answers` of the loader's ``answer_lists`` on the device, uploaded at the first call and kept:
+        ``(a_off, a_ids)`` int64 tensors."""
+        if self._answers is None:
+            import torch
+            self._answers = tuple(torch.from_numpy(a).to(self.device) for a in pack_answers(self.loader.answer_lists))
+        return self._answers
 
     @property
     def resident_bytes(self):

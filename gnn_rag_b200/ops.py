@@ -4,6 +4,7 @@ All ops raise if handed a CPU tensor -- there is no CPU fallback on the product 
 
 Each kernel's shape rule (``*_ok``) sits next to its wrapper: the training path asks it to choose between a kernel and
 its torch restatement, and tests/test_entry_refusals_host.py holds it to the entry point's own refusals."""
+import contextlib
 import ctypes
 import functools
 import weakref
@@ -511,6 +512,22 @@ def split_bf16(A, hi, lo):
 
 WEIGHT_CACHE = True    # keep pre-formatted weights (bf16 hi/lo splits) until their tensor version changes
 _CACHE = {}            # key -> [buffers (tuple of tensors), owner version, weakref(owner tensor)]
+_PRIVATE = None        # inside graph_private_weights: the buffers handed to the capture
+
+
+@contextlib.contextmanager
+def graph_private_weights():
+    """A CUDA graph captured inside this context formats every weight it reads (the split-bf16 workspaces of the wgmma
+    GEMM and the fused layer, :func:`param_planes`) into buffers of its own on every replay, instead of reading the
+    cache's copies formatted at capture time.  Such a graph stays valid across in-place parameter updates
+    (``optimizer.step()``, ``load_state_dict``) at the cost of those formatting kernels per replay.  Yields the list
+    of those buffers: the graph's owner keeps it alive with the graph.  Nothing changes outside a capture."""
+    global _PRIVATE
+    prev, _PRIVATE = _PRIVATE, []
+    try:
+        yield _PRIVATE
+    finally:
+        _PRIVATE = prev
 
 
 def _base(t):
@@ -522,8 +539,13 @@ def _cached(key, owner, fits, make):
     in-place update / load_state_dict re-formats on the next call).  The entry of ``key`` is reused while it belongs
     to the same ``owner`` object and ``fits(buffers)``; ``current`` says whether it still holds owner's ``_version``
     (False: the caller rewrites the buffers).  Otherwise ``make()`` gives new buffers.  While a CUDA graph is being
-    captured nothing is inserted or refreshed: a stale or missing entry gets new buffers the cache does not keep."""
+    captured nothing is inserted or refreshed: a stale or missing entry gets new buffers the cache does not keep.
+    Inside :func:`graph_private_weights` a capture always gets new buffers with ``current`` False."""
     capturing = torch.cuda.is_current_stream_capturing()
+    if capturing and _PRIVATE is not None:
+        buffers = make()
+        _PRIVATE.extend(buffers)
+        return buffers, False
     ent = _CACHE.get(key) if WEIGHT_CACHE else None
     if ent is not None and ent[2]() is owner and fits(ent[0]):
         if ent[1] == owner._version:
@@ -1279,6 +1301,41 @@ def epoch_step_record(cursor, batch_size, num_data, loss, grad_norm, seed, h1, f
     _launch("gr_epoch_step_record", _p(cursor), steps, int(batch_size), B, int(num_data), _p(loss), _p(grad_norm),
             _p(seed), _p(h1), _p(f1), _p(split_status), _p(csr_status), _p(losses), _p(grad_norms), _p(seeds),
             _p(h1_all), _p(f1_all), _p(epoch_status), op="optimizer")
+
+
+def eval_step_record(cursor, batch_size, steps, ids, local_entity, pred_dist, cand_idx, cand_count, a_off, a_ids, seed,
+                     split_status, csr_status, metrics, cases, counts, cand_off, cand, cand_total, seeds, eval_status):
+    """The tail of a graphed evaluation step (gr_eval_step_record): the evaluator's metrics of the step's questions
+    (``ids`` int64 [B]; ``local_entity`` int64, ``pred_dist`` fp32, ``cand_idx`` int32 [B, N] and ``cand_count``
+    int32 [B] of :func:`rank_candidates`) against their answers (``a_off`` int64 [num_a + 1], ``a_ids`` int64, each
+    question's run ascending) stored at the cursor's positions of ``metrics`` (float64 [num_data, 5]), ``cases``
+    (int8), ``counts`` (int32) and ``cand_off`` (int64, all [num_data]); the candidates appended to ``cand`` (int64
+    [capacity, 2]) at ``cand_total`` (int64[1]); ``seed`` (int64[1] or None) at the cursor of ``seeds``; the status
+    words OR-ed into ``eval_status`` (int32[3]); the cursor advanced.  See include/gnnrag_b200.h."""
+    for name, t, dt in (("cursor", cursor, torch.int64), ("ids", ids, torch.int64),
+                        ("local_entity", local_entity, torch.int64), ("pred_dist", pred_dist, torch.float32),
+                        ("cand_idx", cand_idx, torch.int32), ("cand_count", cand_count, torch.int32),
+                        ("a_off", a_off, torch.int64), ("a_ids", a_ids, torch.int64), ("seed", seed, torch.int64),
+                        ("split_status", split_status, torch.int32), ("csr_status", csr_status, torch.int32),
+                        ("metrics", metrics, torch.float64), ("cases", cases, torch.int8),
+                        ("counts", counts, torch.int32), ("cand_off", cand_off, torch.int64),
+                        ("cand", cand, torch.int64), ("cand_total", cand_total, torch.int64),
+                        ("seeds", seeds, torch.int64), ("eval_status", eval_status, torch.int32)):
+        if t is not None and not t.is_contiguous():
+            raise RuntimeError("eval_step_record: %s must be contiguous" % name)
+        _cuda(t, dt, name)
+    B, N = local_entity.shape
+    num_data = cases.numel()
+    if (ids.numel() != B or pred_dist.shape != (B, N) or cand_idx.shape != (B, N) or cand_count.numel() != B
+            or metrics.shape != (num_data, 5) or counts.numel() != num_data or cand_off.numel() != num_data
+            or cand.dim() != 2 or cand.shape[1] != 2 or eval_status.numel() != 3):
+        raise RuntimeError("eval_step_record: need ids, cand_count [B], pred_dist, cand_idx [B, N] like local_entity, "
+                           "metrics [num_data, 5], counts, cand_off [num_data] like cases, cand [capacity, 2] and "
+                           "eval_status [3]")
+    _launch("gr_eval_step_record", _p(cursor), int(steps), int(batch_size), B, num_data, N, _p(ids),
+            _p(local_entity), _p(pred_dist), _p(cand_idx), _p(cand_count), _p(a_off), _p(a_ids), a_off.numel() - 1,
+            _p(seed), _p(split_status), _p(csr_status), _p(metrics), _p(cases), _p(counts), _p(cand_off), _p(cand),
+            cand.shape[0], _p(cand_total), _p(seeds), _p(eval_status), op="loss_rank")
 
 
 def shortest_path_nodes(g, source_idx, source_cnt, target_idx, target_cnt, return_distances=False):

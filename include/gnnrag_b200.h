@@ -813,6 +813,30 @@ int gr_epoch_step_record(int64_t* cursor, int64_t steps, int64_t batch_size, int
                          float* grad_norms, int64_t* seeds, float* h1_all, float* f1_all, int32_t* epoch_status,
                          void* stream);
 
+/* gr_eval_step_record: the tail of an evaluation epoch step (graphed.GraphedStep.start_eval), after
+ * gr_epoch_step_begin, the serving forward and gr_rank_candidates.  With c in [0, steps), for every j < B whose
+ * position p = c * batch_size + j is below num_data: C = cand_count[j] clamped to [0, N], the candidates
+ * e_k = local_entity[j, cand_idx[j, k]] (k < C; cand_idx entries in [0, N)) and the answers of ids[j], the ascending
+ * run a_ids[a_off[id] .. a_off[id + 1]) of length A (A = 0 for an id outside [0, num_a)).  As f1_and_hits
+ * (evaluate.f1_and_hits): correct = #{k : e_k among the answers}, hit = (e_0, or -1 when C = 0, among the answers),
+ * case 0 (A = 0, C = 0), 1 (A = 0), 2 (C = 0) or 3, with p = correct / C, r = correct / A and
+ * f1 = 2 / (1/p + 1/r) (0 when p or r is 0) in IEEE round-to-nearest float64.  Writes metrics[p] = (precision,
+ * recall, f1, hit, em) (float64 [num_data, 5]), cases[p] (int8), counts[p] = C (int32) and cand_off[p] (int64), the
+ * offset of its candidates in the flat records: cand_off of the step's recorded questions is the exclusive scan of
+ * their C in batch order, starting at *cand_total.  Candidate k of position p goes to record cand_off[p] + k of cand
+ * (int64 [capacity, 2]: the entity id, then the int32 pair (local index, fp32 bits of pred_dist[j, local index])) when
+ * all C of them fit below capacity; a question that does not fit is not written and sets bit 1 of eval_status[2].
+ * Then *cand_total = cand_off past the step's last record and seeds[c] = *seed (both optional together).
+ * eval_status[0] |= *split_status, eval_status[1] |= *csr_status; a cursor outside [0, steps) records nothing and sets
+ * bit 2 of eval_status[0].  Then cursor = c + 1.  pred_dist fp32, local_entity int64, cand_idx int32: [B, N]. */
+int gr_eval_step_record(int64_t* cursor, int64_t steps, int64_t batch_size, int B, int64_t num_data, int64_t N,
+                        const int64_t* ids, const int64_t* local_entity, const float* pred_dist,
+                        const int32_t* cand_idx, const int32_t* cand_count, const int64_t* a_off,
+                        const int64_t* a_ids, int64_t num_a, const int64_t* seed, const int32_t* split_status,
+                        const int32_t* csr_status, double* metrics, int8_t* cases, int32_t* counts, int64_t* cand_off,
+                        int64_t* cand, int64_t capacity, int64_t* cand_total, int64_t* seeds, int32_t* eval_status,
+                        void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Shortest-path node sets (SURVEY.md 8f row 1): nodes lying on any shortest path between any seed and
  * any retrieved candidate in the UNDIRECTED subgraph -- build_graph + get_truth_paths,

@@ -161,14 +161,14 @@ def test_linear_tc_planes_cluster_variants(cluster, bk, tma_store):
             assert (ohi[:, N:] == 0).all() and (olo[:, N:] == 0).all()
             dsum = dots.view(2, M).double().sum(0)
             assert (dsum - out.double() @ ws.double()).abs().max().item() < 1e-4 * (scale + 1)
-    finally:
-        ops.set_option("tc_cluster", 2)
+    finally:                                      # the documented defaults (linear_tc.cu)
+        ops.set_option("tc_cluster", 1)
         ops.set_option("tc_bk", 32)
         ops.set_option("tc_tma_store", 1)
 
 
 def test_forward_with_tc_linear_matches_golden():
-    ops.TC_LINEAR = True
+    prev, ops.TC_LINEAR = ops.TC_LINEAR, True
     try:
         for name in ("rearev_sharp_ties", "rearev_small", "rearev_d50_pads", "nsm_reason_kb"):
             g = Golden(name)
@@ -179,7 +179,7 @@ def test_forward_with_tc_linear_matches_golden():
             if name == "rearev_sharp_ties":
                 assert torch.equal(dist[:, 4], dist[:, 5])       # twins still tie exactly
     finally:
-        ops.TC_LINEAR = False
+        ops.TC_LINEAR = prev
 
 
 # ------------------------------------------------------------------ aggregation kernel -------------

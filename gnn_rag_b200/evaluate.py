@@ -72,8 +72,8 @@ class Evaluator:
     ``step``: optionally a ``graphed.GraphedStep`` of ``model`` that ranks with this evaluator's pad id
     (``len(entity2id)``) and ``eps``.  With it, :meth:`evaluate` over a ``loader.DeviceSplit`` runs the whole split as
     one evaluation epoch (``GraphedStep.start_eval``: batch assembly, forward, ranking and metrics in CUDA graphs) and
-    builds the ``.info`` rows from its records on the host; it returns the same values and writes the same file as
-    the per-batch loop, which still serves host loaders and evaluators without a step."""
+    formats the ``.info`` rows from its records on the device (``EvalRun.info``); it returns the same values and
+    writes the same file as the per-batch loop, which still serves host loaders and evaluators without a step."""
 
     def __init__(self, args, model, entity2id, relation2id, device, step=None):
         self.model, self.args, self.eps = model, args, args["eps"]
@@ -104,6 +104,7 @@ class Evaluator:
             if step.eps != self.eps:
                 raise ValueError("Evaluator: the step ranks with eps %r, the evaluator with %r" % (step.eps, self.eps))
         self.step = step
+        self._tables = {}             # id(split) -> InfoTables
 
     def _name(self, ent):
         return self.id2entity[ent] if self.entity2name is None else self.entity2name[self.id2entity[ent]]
@@ -126,10 +127,12 @@ class Evaluator:
                     obj[j]["action"] = str(act[i])
         return obj_list
 
+    def _info_path(self):
+        return os.path.join(self.args["checkpoint_dir"], "{}_test.info".format(self.args["experiment_name"]))
+
     def _open_info(self):
         if self.file_write is None:
-            path = os.path.join(self.args["checkpoint_dir"], "{}_test.info".format(self.args["experiment_name"]))
-            self.file_write = open(path, "w")
+            self.file_write = open(self._info_path(), "w")
 
     def _row(self, obj, answers, p, r, f1, hit, em, cand):
         obj["answers"] = [self._name(a) for a in answers]
@@ -182,28 +185,85 @@ class Evaluator:
         return float(np.mean(f1s)), float(np.mean(hits)), float(np.mean(ems))
 
     def _evaluate_epoch(self, split, test_batch_size):
-        """:meth:`evaluate` over the resident split ``split`` as one evaluation epoch of ``self.step``: the metrics and
-        candidates come from the device records, the ``.info`` rows are built here batch by batch (``get_quest``
-        after setting the loader's ``sample_ids``, as ``get_batch`` sets them)."""
+        """:meth:`evaluate` over the resident split ``split`` as one evaluation epoch of ``self.step``: the means and
+        ``case_ct`` come from the device records, the ``.info`` file from ``EvalRun.info`` with this evaluator's
+        :meth:`info_tables` of the split (a malformed run raises before the file is opened)."""
         self.model.eval()
         self.count = 0
-        prec, rec, f1, hit, em, cases, retrieved = self.step.evaluate_split(split, test_batch_size)
-        self._open_info()
-        L = split.loader
-        prec, rec, f1l, hitl, eml, cases_l = (a.tolist() for a in (prec, rec, f1, hit, em, cases))
+        tables = self.info_tables(split)
+        run = self.step.start_eval(split, test_batch_size)
+        metrics, cases = run.records()
+        data = run.info(tables)
         case_ct = {}
-        for start in range(0, split.num_data, test_batch_size):
-            L.sample_ids = L.batches[start:min(start + test_batch_size, split.num_data)]
-            obj_list = self.write_info(split, None, self.model.num_iter)    # an eval forward returns tp_list None
-            for b, answers in enumerate(L.answer_lists[L.sample_ids]):
-                i, case = start + b, cases_l[start + b]
-                e = int(eml[i]) if case == 3 else eml[i]          # f1_and_hits: an int in case 3 only
-                self._row(obj_list[b], list(answers), prec[i], rec[i], f1l[i], hitl[i], e, retrieved[i])
-                case_ct[case] = case_ct.get(case, 0) + 1
+        for case in cases.tolist():
+            case_ct[case] = case_ct.get(case, 0) + 1
         self.case_ct = case_ct
-        self.file_write.close()
-        self.file_write = None
-        return float(np.mean(f1)), float(np.mean(hit)), float(np.mean(em))
+        with open(self._info_path(), "wb") as f:
+            f.write(data)
+        return float(np.mean(metrics[:, 2])), float(np.mean(metrics[:, 3])), float(np.mean(metrics[:, 4]))
+
+    def info_tables(self, split):
+        """The :class:`InfoTables` of the resident split ``split`` for this evaluator's names, built on the first call
+        and kept: the later evaluations of the split (between training epochs, say) reuse them."""
+        t = self._tables.get(id(split))
+        if t is None or t.split is not split:
+            t = self._tables[id(split)] = InfoTables(self, split)
+        return t
+
+
+class InfoTables:
+    """What the ``.info`` rows of an evaluation epoch (``graphed.EvalRun.info``) take from the host, on the split's
+    device.  ``prefix`` (uint8) with ``prefix_off`` (int64 [num_q + 1]): question q's row up to and including
+    ``"answers": [...], ``, cut from ``json.dumps`` of the dict :meth:`Evaluator.write_info` and the answer names
+    make.  ``names`` (uint8) with ``name_off`` (int64 [num_names + 1]): ``json.dumps`` of the name
+    (``Evaluator._name``) of every entity the split can rank, its ``candidate_entities`` other than the pad id;
+    ``name_slot`` (int32, one per entity id up to the largest of them): the entity's name index, -1 for none."""
+
+    def __init__(self, evaluator, split):
+        import torch
+        self.split = split
+        for name, a in self.host_arrays(evaluator, split.loader, split.num_q).items():
+            setattr(self, name, torch.from_numpy(a).to(split.device))
+
+    @staticmethod
+    def host_arrays(evaluator, data_loader, num_q):
+        """The tables as numpy arrays (a dict of the attribute names) for the first ``num_q`` questions of
+        ``data_loader``; its ``sample_ids`` are restored afterwards."""
+        ev, L = evaluator, data_loader
+        had_ids = hasattr(L, "sample_ids")
+        saved = getattr(L, "sample_ids", None)
+        L.sample_ids = np.arange(num_q)                         # get_quest decodes the questions of sample_ids
+        try:
+            objs = ev.write_info(L, None, ev.model.num_iter)      # an eval forward returns tp_list None
+        finally:
+            if had_ids:
+                L.sample_ids = saved
+            else:
+                del L.sample_ids
+        prefixes = []
+        for obj, answers in zip(objs, L.answer_lists):
+            obj["answers"] = [ev._name(a) for a in answers]
+            prefixes.append(json.dumps(obj)[:-1].encode("ascii") + b", ")
+        ents = np.unique(np.asarray(L.candidate_entities, dtype=np.int64))
+        ents = ents[(ents >= 0) & (ents != len(ev.id2entity))]
+        slot = np.full(int(ents[-1]) + 1 if ents.size else 1, -1, dtype=np.int32)
+        names = []
+        for e in ents.tolist():
+            try:
+                name = ev._name(e)
+            except (KeyError, IndexError):
+                continue
+            slot[e] = len(names)
+            names.append(json.dumps(name).encode("ascii"))
+
+        def flat(chunks):
+            off = np.zeros(len(chunks) + 1, dtype=np.int64)
+            np.cumsum(np.array([len(c) for c in chunks], dtype=np.int64), out=off[1:])
+            return np.frombuffer(b"".join(chunks) or b"\0", dtype=np.uint8).copy(), off
+        out = dict(name_slot=slot)
+        out["prefix"], out["prefix_off"] = flat(prefixes)
+        out["names"], out["name_off"] = flat(names)
+        return out
 
 
 def merge_candidates(cand1, cand2):

@@ -754,7 +754,8 @@ class GraphedStep:
         if plan.steps:
             s0 = int(plan.starts[-1])
             L.sample_ids = L.batches[s0:min(s0 + int(batch_size), L.num_data)]
-        return EvalRun(ep.blob.clone(), ep.cand.clone(), None if ep.seeds is None else ep.seeds.clone(), ep.num_data)
+        return EvalRun(ep.blob.clone(), ep.cand.clone(), None if ep.seeds is None else ep.seeds.clone(), ep.num_data,
+                       ep.order.clone())
 
     def _eval_buffers(self, split, batch_size):
         k = (id(split), int(batch_size))
@@ -973,12 +974,28 @@ def _assemble_step(layout, ep, st, cursor, device):
 
 class EvalRun:
     """One evaluation started by :meth:`GraphedStep.start_eval`: device copies of its records, valid once the current
-    stream reaches them.  ``seeds``: int64 [steps], the fact-order seed of each step (None without ``shuffle``).
-    :meth:`result` reads the records back; :meth:`check` raises for a nonzero status."""
+    stream reaches them.  ``seeds``: int64 [steps], the fact-order seed of each step (None without ``shuffle``);
+    ``order``: int64 [num_data], the question id of each position.  :meth:`result` and :meth:`records` read the
+    records back; :meth:`info` formats the run's ``.info`` rows on the device; :meth:`check` raises for a nonzero
+    status."""
 
-    def __init__(self, blob, cand, seeds, num_data):
-        self.blob, self.cand, self.seeds, self.num_data = blob, cand, seeds, num_data
+    def __init__(self, blob, cand, seeds, num_data, order):
+        self.blob, self.cand, self.seeds, self.num_data, self.order = blob, cand, seeds, num_data, order
         self._words = None
+        self._host = None
+
+    def _read(self):
+        """The per-question records and the status, read back in one copy (once)."""
+        if self._host is None:
+            self._host = _EvalBuffers.views(self.blob.cpu().numpy(), self.num_data)
+            self._words = self._host["status"].tolist()
+        return self._host
+
+    def records(self):
+        """-> ``(metrics, case)``: float64 [num_data, 5] (precision, recall, f1, hit, em as ``evaluate.f1_and_hits``
+        returns them, ``em`` as a float) and the int8 case (0..3) of every question in batch order."""
+        v = self._read()
+        return v["metrics"], v["cases"]
 
     def result(self):
         """-> ``(precision, recall, f1, hit, em, case, retrieved)`` of every question in batch order: five float64
@@ -986,10 +1003,7 @@ class EvalRun:
         one :class:`evaluate.Retrieved` per question.  Reads the device twice at most: the per-question records and
         the status in one copy, then the candidates in use."""
         from .evaluate import Retrieved
-        n = self.num_data
-        host = self.blob.cpu().numpy()
-        v = _EvalBuffers.views(host, n)
-        self._words = v["status"].tolist()
+        v = self._read()
         used = min(int(v["cand_total"][0]), self.cand.shape[0])
         cand = self.cand[:used].cpu().numpy() if used else np.zeros((0, 2), dtype=np.int64)
         ent, pair = cand[:, 0], cand[:, 1:].copy().view(np.int32)
@@ -1002,11 +1016,41 @@ class EvalRun:
         return m[:, 0].copy(), m[:, 1].copy(), m[:, 2].copy(), m[:, 3].copy(), m[:, 4].copy(), v["cases"].copy(), \
             retrieved
 
+    def info(self, tables, file=None):
+        """The ``.info`` rows of the run, byte for byte what ``evaluate.Evaluator`` writes for these questions with
+        ``json.dumps``: one row per question in batch order, formatted on the device from the records
+        (gr_info_rows_size, gr_info_rows_write) with the question prefixes and entity names of ``tables`` (an
+        ``evaluate.InfoTables`` of the split, from ``Evaluator.info_tables``).  Calls :meth:`check` first, so a
+        malformed run raises its message and formats nothing.  Reads the total size back once, then copies the
+        bytes once into pinned memory.  -> the bytes as a uint8 numpy array over that memory, or, with ``file`` (an
+        open binary file), None after one ``file.write`` of them.  Raises ``RuntimeError`` when a candidate record
+        falls outside the records, a question id outside the tables, or a candidate entity has no name."""
+        self.check()
+        n, dev = self.num_data, self.blob.device
+        v = _EvalBuffers.views(self.blob, n)
+        recs = (v["metrics"], v["cases"], v["counts"], v["cand_off"], v["cand_total"])
+        row_off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        summary = torch.empty(2, dtype=torch.int64, device=dev)
+        ops.info_rows_size(*recs, v["status"], self.cand, self.order, tables, row_off, summary)
+        total, flags = summary.tolist()
+        if flags:
+            raise RuntimeError("EvalRun.info: flags %d (2: a candidate record outside the records or a question id "
+                               "outside the tables, 4: a candidate entity without a name)" % flags)
+        out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+        ops.info_rows_write(*recs, self.cand, self.order, tables, row_off, summary, out)
+        host = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+        host.copy_(out[:total])
+        data = host.numpy()
+        if file is None:
+            return data
+        file.write(data)
+        return None
+
     def check(self):
         """Raise ``DeviceSplit.check``'s message when an assembly flagged an id out of range or an overflow, else (for
         GraftNet) ``GraftGraph``'s when the graft staging rejected a list, else ``GraphedStep``'s when a CSR build
         flagged ids outside the batch, else when the candidate records overflowed (reads the status unless
-        :meth:`result` has)."""
+        :meth:`result` or :meth:`records` has)."""
         from .loader import DeviceSplit
         words = self._words
         if words is None:

@@ -1338,6 +1338,63 @@ def eval_step_record(cursor, batch_size, steps, ids, local_entity, pred_dist, ca
             cand.shape[0], _p(cand_total), _p(seeds), _p(eval_status), op="loss_rank")
 
 
+def _info_rows_args(name, metrics, cases, counts, cand_off, cand_total, cand, order, tables):
+    """The checked record and table arguments of the two ``.info`` row entry points."""
+    for arg, t, dt in (("metrics", metrics, torch.float64), ("cases", cases, torch.int8), ("counts", counts, torch.int32),
+                       ("cand_off", cand_off, torch.int64), ("cand_total", cand_total, torch.int64),
+                       ("cand", cand, torch.int64), ("order", order, torch.int64),
+                       ("prefix", tables.prefix, torch.uint8), ("prefix_off", tables.prefix_off, torch.int64),
+                       ("name_slot", tables.name_slot, torch.int32), ("names", tables.names, torch.uint8),
+                       ("name_off", tables.name_off, torch.int64)):
+        if not t.is_contiguous():
+            raise RuntimeError("%s: %s must be contiguous" % (name, arg))
+        _cuda(t, dt, arg)
+    n = cases.numel()
+    if (metrics.shape != (n, 5) or counts.numel() != n or cand_off.numel() != n or order.numel() != n
+            or cand_total.numel() != 1 or cand.dim() != 2 or cand.shape[1] != 2):
+        raise RuntimeError("%s: need metrics [num_data, 5], counts, cand_off, order [num_data] like cases, cand_total "
+                           "[1] and cand [capacity, 2]" % name)
+    return n, (tables.prefix_off.numel() - 1, tables.name_slot.numel(), tables.name_off.numel() - 1)
+
+
+def info_rows_size(metrics, cases, counts, cand_off, cand_total, eval_status, cand, order, tables, row_off, summary):
+    """Sizes of the ``.info`` rows of an evaluation's records (gr_info_rows_size): ``row_off`` (int64 [num_data + 1])
+    receives the rows' byte offsets and ``summary`` (int64[2]) the total and the flags.  The records are
+    gr_eval_step_record's (``metrics`` float64 [num_data, 5], ``cases`` int8, ``counts`` int32, ``cand_off`` int64
+    [num_data], ``cand_total`` int64[1], ``eval_status`` int32[4], ``cand`` int64 [capacity, 2]); ``order``: the
+    question id of each position; ``tables``: an ``evaluate.InfoTables``.  See include/gnnrag_b200.h."""
+    n, (num_q, num_entity, num_names) = _info_rows_args("info_rows_size", metrics, cases, counts, cand_off, cand_total,
+                                                        cand, order, tables)
+    for arg, t, dt in (("eval_status", eval_status, torch.int32), ("row_off", row_off, torch.int64),
+                       ("summary", summary, torch.int64)):
+        if not t.is_contiguous():
+            raise RuntimeError("info_rows_size: %s must be contiguous" % arg)
+        _cuda(t, dt, arg)
+    if eval_status.numel() != 4 or row_off.numel() != n + 1 or summary.numel() != 2:
+        raise RuntimeError("info_rows_size: need eval_status [4], row_off [num_data + 1] and summary [2]")
+    _launch("gr_info_rows_size", _p(metrics), _p(cases), _p(counts), _p(cand_off), _p(cand_total), _p(eval_status), n,
+            _p(cand), cand.shape[0], _p(order), _p(tables.prefix_off), num_q, _p(tables.name_slot), num_entity,
+            _p(tables.name_off), num_names, _p(row_off), _p(summary), launches=2, op="info_rows")
+
+
+def info_rows_write(metrics, cases, counts, cand_off, cand_total, cand, order, tables, row_off, summary, out):
+    """The ``.info`` rows of an evaluation's records into ``out`` (uint8, at least ``summary[0]`` bytes) at the
+    offsets :func:`info_rows_size` wrote into ``row_off`` (gr_info_rows_write); nothing when ``summary`` holds
+    flags.  Same records and tables as :func:`info_rows_size`."""
+    n, (num_q, num_entity, num_names) = _info_rows_args("info_rows_write", metrics, cases, counts, cand_off, cand_total,
+                                                        cand, order, tables)
+    for arg, t, dt in (("row_off", row_off, torch.int64), ("summary", summary, torch.int64), ("out", out, torch.uint8)):
+        if not t.is_contiguous():
+            raise RuntimeError("info_rows_write: %s must be contiguous" % arg)
+        _cuda(t, dt, arg)
+    if row_off.numel() != n + 1 or summary.numel() != 2:
+        raise RuntimeError("info_rows_write: need row_off [num_data + 1] and summary [2]")
+    _launch("gr_info_rows_write", _p(metrics), _p(cases), _p(counts), _p(cand_off), _p(cand_total), n, _p(cand),
+            cand.shape[0], _p(order), _p(tables.prefix), _p(tables.prefix_off), num_q, _p(tables.name_slot),
+            num_entity, _p(tables.names), _p(tables.name_off), num_names, _p(row_off), _p(summary), _p(out),
+            out.numel(), op="info_rows")
+
+
 def shortest_path_nodes(g, source_idx, source_cnt, target_idx, target_cnt, return_distances=False):
     """source_idx int32[B,S], target_idx int32[B,T] local indices (+counts) ->
     (on_path uint8[B,N], pair_dist int32[B,S,T]); with ``return_distances`` also the BFS distance arrays the kernel

@@ -838,6 +838,36 @@ int gr_eval_step_record(int64_t* cursor, int64_t steps, int64_t batch_size, int 
                         void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The `.info` file of an evaluation epoch (csrc/info_rows.cu, graphed.EvalRun.info): one JSONL row per position p of
+ * the run, byte for byte the json.dumps row evaluate.Evaluator writes:
+ *   prefix[q]  "precison": P, "recall": R, "f1": F, "hit": H, "em": E, "cand": [["name", prob], ...]}\n
+ * with q = order[p] (int64 [num_data]).  The records are gr_eval_step_record's: metrics float64 [num_data, 5], cases
+ * int8, counts int32 and cand_off int64 [num_data], cand_total int64[1], eval_status int32[4] (the run's status words)
+ * and cand int64 [capacity, 2].  The numbers are Python reprs of float64 values (shortest round trip, csrc/float_repr.cuh)
+ * -- em an int (0 / 1) in case 3 -- and each prob is the float64 of the candidate record's fp32.  Host-built tables:
+ * prefix (bytes) with prefix_off int64 [num_q + 1], question q's text up to and including `"answers": [...], `;
+ * names (bytes) with name_off int64 [num_names + 1], JSON strings with their quotes; name_slot int32 [num_entity],
+ * the name of each entity id or -1.
+ *
+ * gr_info_rows_size: row_off int64 [num_data + 1] = the rows' byte offsets (row_off[0] = 0) and summary int64[2] =
+ *   (total bytes, flags).  flags: 1 a status word is nonzero; else the OR over the rows of 2 (q outside [0, num_q), or
+ *   candidates outside [0, min(*cand_total, capacity))) and 4 (a candidate entity without a name).  With flags the
+ *   total is 0.  Two launches, no workspace.
+ * gr_info_rows_write: the rows into out (out_bytes >= summary[0]) at row_off; writes nothing when summary[1] != 0 or
+ *   summary[0] > out_bytes.  Same records and tables as the size call. */
+int gr_info_rows_size(const double* metrics, const int8_t* cases, const int32_t* counts, const int64_t* cand_off,
+                      const int64_t* cand_total, const int32_t* eval_status, int64_t num_data, const int64_t* cand,
+                      int64_t capacity, const int64_t* order, const int64_t* prefix_off, int64_t num_q,
+                      const int32_t* name_slot, int64_t num_entity, const int64_t* name_off, int64_t num_names,
+                      int64_t* row_off, int64_t* summary, void* stream);
+int gr_info_rows_write(const double* metrics, const int8_t* cases, const int32_t* counts, const int64_t* cand_off,
+                       const int64_t* cand_total, int64_t num_data, const int64_t* cand, int64_t capacity,
+                       const int64_t* order, const uint8_t* prefix, const int64_t* prefix_off, int64_t num_q,
+                       const int32_t* name_slot, int64_t num_entity, const uint8_t* names, const int64_t* name_off,
+                       int64_t num_names, const int64_t* row_off, const int64_t* summary, uint8_t* out,
+                       int64_t out_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Shortest-path node sets (SURVEY.md 8f row 1): nodes lying on any shortest path between any seed and
  * any retrieved candidate in the UNDIRECTED subgraph -- build_graph + get_truth_paths,
  * llm/src/utils/graph_utils.py:10-21,49-75.  Uses both CSRs of a question batch; one CTA per question.

@@ -7,8 +7,8 @@ A whole ``Evaluator.evaluate(split, test_batch_size=B)`` over a synthetic WebQSP
 
   per_batch         the Evaluator without a step: per batch an eager get_batch, an eager forward, retrieve() and
                     f1_and_hits in Python
-  epoch             Evaluator(step=GraphedStep(model, NE)), warm: one graph replay per step, the rows built from the
-                    device records
+  epoch             Evaluator(step=GraphedStep(model, NE)), warm: one graph replay per step, the rows formatted on
+                    the device from its records (EvalRun.info) and written with one copy and one write
   epoch_after_step  the same right after an in-place Adam step on every parameter (untimed): what an evaluation
                     between training epochs costs; no graph is captured again
   first_epoch_s     the first evaluation of a new GraphedStep, captures included, timed on its own; ``capture_s`` is
@@ -18,7 +18,11 @@ Shapes: ReaRev, NSM and GraftNet at the reference's WebQSP evaluation (B 20, ent
 entity_dim 200).  ``cands_per_q`` is the mean retrieved count: the randomly initialised models' distributions are
 flat, so the eps = 0.95 cut keeps most of a question's 1 000..2 000 entities and the ``.info`` rows are large.  The
 questions/s of a mode is the median over ``--runs`` passes, the modes alternating, after one
-untimed pass of each.  Then one ``torch.profiler`` run per shape over ``--profile-steps`` steps of each path (a split
+untimed pass of each; both paths' files are compared byte for byte.  ``info`` splits the ``.info`` part of a warm
+epoch (median of ``--runs``): gr_info_rows_size and gr_info_rows_write (CUDA events), the device-to-host copy of the
+bytes into pinned memory and the file write (host clock); ``info_bytes`` is the file's size.  The one-time build of the
+evaluator's host tables (``evaluate.InfoTables``: question prefixes and entity names) is timed on its own and printed
+on a line of its own before the shape's.  Then one ``torch.profiler`` run per shape over ``--profile-steps`` steps of each path (a split
 of that many batches): per step, the launches and device time of every kernel, and the kernels the evaluation graph
 launches more often than the per-batch forward (the weight formatting the graphs redo on every replay,
 ``ops.graph_private_weights``).  The GPU's name and power limit are read in the same run.  One JSON line per shape.
@@ -122,6 +126,41 @@ def profile(name, m, B, steps, tmp):
     return summary
 
 
+def info_parts(ev, step, split, B, runs, path):
+    """Median seconds of each part of ``EvalRun.info`` + the file write over ``runs`` warm evaluations."""
+    from gnn_rag_b200 import ops
+    tables = ev.info_tables(split)
+    parts = collections.defaultdict(list)
+    for _ in range(runs):
+        run = step.start_eval(split, B)
+        run.check()
+        n = run.num_data
+        v = graphed._EvalBuffers.views(run.blob, n)
+        recs = (v["metrics"], v["cases"], v["counts"], v["cand_off"], v["cand_total"])
+        row_off = torch.empty(n + 1, dtype=torch.int64, device="cuda")
+        summary = torch.empty(2, dtype=torch.int64, device="cuda")
+        ev0, ev1, ev2, ev3 = (torch.cuda.Event(enable_timing=True) for _ in range(4))
+        ev0.record()
+        ops.info_rows_size(*recs, v["status"], run.cand, run.order, tables, row_off, summary)
+        ev1.record()
+        total = int(summary[0])
+        out = torch.empty(max(total, 1), dtype=torch.uint8, device="cuda")
+        ev2.record()
+        ops.info_rows_write(*recs, run.cand, run.order, tables, row_off, summary, out)
+        ev3.record()
+        host = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+        t_copy, _ = timed(lambda: host.copy_(out[:total]))
+        t0 = time.perf_counter()
+        with open(path, "wb") as f:
+            f.write(host.numpy())
+        parts["write_s"].append(time.perf_counter() - t0)
+        parts["size_kernels_ms"].append(ev0.elapsed_time(ev1))
+        parts["write_kernel_ms"].append(ev2.elapsed_time(ev3))
+        parts["d2h_ms"].append(t_copy * 1e3)
+        parts["bytes"] = [total]
+    return {k: round(float(np.median(x)), 4) for k, x in parts.items()}
+
+
 def main():
     global ENT
     ap = argparse.ArgumentParser()
@@ -154,11 +193,19 @@ def main():
         ev_b = evaluator(name, m, tmp)
         step = graphed.GraphedStep(m, NE)
         ev_e = evaluator(name, m, tmp, step=step)
+        t_tables, _ = timed(lambda: ev_e.info_tables(split))
+        print(json.dumps(dict(shape=shape, info_tables_s=round(t_tables, 3), questions=a.questions, gpu=info)),
+              flush=True)
         first, want = timed(lambda: ev_e.evaluate(split, B))
+        path = os.path.join(tmp, name + "_test.info")
+        with open(path, "rb") as f:
+            want_file = f.read()
         graphs = len(step._cache)
         cands = float(np.mean([len(r) for r in step.evaluate_split(split, B)[6]]))
         got = ev_b.evaluate(split, B)                 # untimed pass of the per-batch path
         assert got == want, (got, want)
+        with open(path, "rb") as f:
+            assert f.read() == want_file
 
         def after_step():
             optimizer_step(m, opt, gen)
@@ -179,9 +226,10 @@ def main():
         for k, v in med.items():
             res[k + "_qps"] = round(a.questions / v, 1)
             res[k + "_s"] = [round(x, 4) for x in secs[k]]
-        res["first_epoch_s"] = round(first, 3)
+        res["first_epoch_s"] = round(first, 3)         # the tables were built before it
         res["capture_s"] = round(first - med["epoch"], 3)
         res["speedup"] = round(med["per_batch"] / med["epoch"], 2)
+        res["info"] = info_parts(ev_e, step, split, B, a.runs, os.path.join(tmp, "parts.info"))
         res["profile"] = profile(name, m, B, a.profile_steps, tmp)
         results.append(res)
         print(json.dumps(res), flush=True)

@@ -36,6 +36,12 @@ def retrieve(pred_dist, db, num_entity, eps):
     -> (list of :class:`Retrieved`, one per question; d2h_bytes)."""
     cand_idx, cand_count, _total = ops.rank_candidates(pred_dist, db.local_entity, db.query_entities,
                                                        num_entity, eps)
+    return read_ranked(pred_dist, db, cand_idx, cand_count)
+
+
+def read_ranked(pred_dist, db, cand_idx, cand_count):
+    """The ordered candidate lists of a ranked batch (``cand_idx`` / ``cand_count`` of ``ops.rank_candidates``),
+    read back to the host, the counts first -> (list of :class:`Retrieved`, one per question; d2h_bytes)."""
     counts_h = cand_count.cpu().numpy()
     maxc = int(counts_h.max()) if counts_h.size else 0
     empty_i, empty_f = np.zeros(0, dtype=np.int64), np.zeros(0, dtype=np.float32)

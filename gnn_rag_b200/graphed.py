@@ -32,6 +32,9 @@ also capture the gradient clipping and the optimizer step (:class:`optim.ClipAda
 :meth:`GraphedGraftTrainStep.train_epoch` a GraftNet one: each step's graph also assembles its batch (GraftNet: with
 its graft lists) from a device cursor into the epoch's question order and records the step's loss and metrics on the
 device (csrc/epoch.cu), so the host only replays graphs and reads the device once per epoch.
+:meth:`GraphedStep.start_eval` evaluates a whole split the same way, through the same epoch driver (``_split_refusal``,
+``_begin_epoch``, ``_epoch_graphs``, ``_warm_up_epoch_step``, ``_epoch_step``, ``_replay_epoch``,
+``_raise_epoch_status``): only the step each graph runs and the records it keeps differ.
 """
 import collections
 import contextlib
@@ -242,11 +245,14 @@ class _KbLayout:
     def check(self, db):
         self.raise_for(torch.cat(self.status_words(db)).tolist())
 
-    # -- the model's part of a training epoch (GraphedTrainStep.start_epoch) ------------------------------------------
-    def epoch_refusal(self, split):
-        """Why ``split`` (a ``loader.DeviceSplit``) does not hold this model family's batches (a message), or None."""
+    # -- the model's part of an epoch (GraphedTrainStep.start_epoch, GraphedStep.start_eval) -------------------------
+    def epoch_refusal(self, split, training):
+        """Why ``split`` (a ``loader.DeviceSplit``) does not hold this model family's batches (a message), or None;
+        worded for the training epoch with ``training``, else for the evaluation epoch."""
         if split.graft:
-            return "train_epoch takes a ReaRev / NSM split; this DeviceSplit holds GraftNet's graft lists"
+            if training:
+                return "train_epoch takes a ReaRev / NSM split; this DeviceSplit holds GraftNet's graft lists"
+            return "a ReaRev / NSM model evaluates a kb split; this DeviceSplit holds GraftNet's graft lists"
         return None
 
     @staticmethod
@@ -389,10 +395,12 @@ class _GraftLayout(_KbLayout):
         if graft_csr or kb:
             _KbLayout.raise_for([graft_csr | kb])
 
-    def epoch_refusal(self, split):
+    def epoch_refusal(self, split, training):
         if not split.graft:
-            return ("GraphedGraftTrainStep.train_epoch takes a GraftNet split; this DeviceSplit holds no graft lists "
-                    "(GraphedTrainStep.train_epoch covers ReaRev and NSM)")
+            if training:
+                return ("GraphedGraftTrainStep.train_epoch takes a GraftNet split; this DeviceSplit holds no graft "
+                        "lists (GraphedTrainStep.train_epoch covers ReaRev and NSM)")
+            return "GraftNet evaluates a GraftNet split; this DeviceSplit holds no graft lists"
         return None
 
     @staticmethod
@@ -666,19 +674,9 @@ class GraphedStep:
 
     def retrieve(self, out):
         """Ordered candidate lists of a :class:`StepOutput` (one D2H), like evaluate.retrieve."""
-        from .evaluate import Retrieved
-        counts_h = out.cand_count.cpu().numpy()
+        from .evaluate import read_ranked
         self._check(out.db)
-        maxc = int(counts_h.max()) if counts_h.size else 0
-        ei, ef = np.zeros(0, dtype=np.int64), np.zeros(0, dtype=np.float32)
-        if maxc == 0:
-            return [Retrieved(ei, ei, ef) for _ in range(out.db.B)], counts_h.size * 4
-        idx = out.cand_idx[:, :maxc].long()
-        probs = torch.gather(out.pred_dist, 1, idx)
-        ents = torch.gather(out.db.local_entity, 1, idx)
-        idx_h, probs_h, ents_h = idx.cpu().numpy(), probs.cpu().numpy(), ents.cpu().numpy()
-        res = [Retrieved(idx_h[b, :c], ents_h[b, :c], probs_h[b, :c]) for b, c in enumerate(counts_h.tolist())]
-        return res, counts_h.size * 4 + idx_h.size * 8 + probs_h.size * 4 + ents_h.size * 8
+        return read_ranked(out.pred_dist, out.db, out.cand_idx, out.cand_count)
 
     # -- a whole evaluation ------------------------------------------------------------------------------------------
     def evaluate_split(self, split, batch_size):
@@ -688,26 +686,6 @@ class GraphedStep:
         out = run.result()
         run.check()
         return out
-
-    def _eval_refusal(self, split, batch_size):
-        from .loader import DeviceSplit, same_device
-        if not isinstance(split, DeviceSplit):
-            return "the split must be a loader.DeviceSplit, got %s" % type(split).__name__
-        graft = isinstance(self._layout, _GraftLayout)
-        if split.graft and not graft:
-            return "a ReaRev / NSM model evaluates a kb split; this DeviceSplit holds GraftNet's graft lists"
-        if graft and not split.graft:
-            return "GraftNet evaluates a GraftNet split; this DeviceSplit holds no graft lists"
-        if not same_device(split.device, self.device):
-            return "the split lives on %s, the model on %s" % (split.device, self.device)
-        if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or batch_size <= 0:
-            return "batch_size must be a positive int, got %r" % (batch_size,)
-        if getattr(split.loader, "q_type", "seq") != "seq":
-            return "q_type must be 'seq', got %r" % (split.loader.q_type,)
-        m = self.model
-        if (m.normalized_gnn or m.norm_rel) and split.weights != "arrays":
-            return "normalized_gnn / norm_rel need fact weights: the split was built with weights='none'"
-        return None
 
     def start_eval(self, split, batch_size):
         """Start an evaluation of the whole split ``split`` (a ``loader.DeviceSplit``) and return its :class:`EvalRun`
@@ -731,86 +709,39 @@ class GraphedStep:
         Refused (``ValueError``): anything but a CUDA ``DeviceSplit`` on the model's device of the model's family,
         ``batch_size <= 0``, a ``q_type`` other than ``"seq"``, fact weights (``normalized_gnn`` / ``norm_rel``) over
         a ``weights="none"`` split, and answers that are not integers."""
-        why = self._eval_refusal(split, batch_size)
+        why = _split_refusal(self, split, batch_size, False)
         if why is not None:
             raise ValueError("start_eval: " + why)
         answers = split.answer_table()
         self.model.eval()
-        split.reset_batches(is_sequential=True)
-        L = split.loader
-        order = np.asarray(L.batches[:L.num_data], dtype=np.int64).reshape(-1)
-        plan = epoch_plan(order, split._stored, split._ents, batch_size, 0.0,
-                          split._graft_count if split.graft else None)
-        if split.index_dtype == torch.int32 and plan.steps and (
-                int(plan.B.max()) * split.N > _INT32_MAX or int(plan.F.max()) > _INT32_MAX):
-            raise ValueError("start_eval: a batch overflows int32 indices; use index_dtype=torch.int64")
-        ep = self._eval_buffers(split, batch_size)
-        ep.order.copy_(torch.from_numpy(order), non_blocking=True)
-        entries = self._eval_entries(ep, plan, answers)
+        ep, plan = _begin_epoch(split, batch_size, False, 0.0, lambda: _buffers_for(
+            self._evals, split, batch_size, lambda ep: ep.pad_id != self.num_entity,
+            lambda: _EvalBuffers(split, batch_size, self.num_entity)))
+        entries = _epoch_graphs(self, plan, lambda shape: self._eval_key(ep, shape),
+                                lambda shape, s0: self._eval_capture(ep, shape, s0, answers))
         ep.cursor.zero_()
         ep.blob.zero_()
-        for ent in entries:
-            ent.g.replay()
-        if plan.steps:
-            s0 = int(plan.starts[-1])
-            L.sample_ids = L.batches[s0:min(s0 + int(batch_size), L.num_data)]
+        _replay_epoch(ep, plan, entries)
         return EvalRun(ep.blob.clone(), ep.cand.clone(), None if ep.seeds is None else ep.seeds.clone(), ep.num_data,
                        ep.order.clone())
 
-    def _eval_buffers(self, split, batch_size):
-        k = (id(split), int(batch_size))
-        ep = self._evals.get(k)
-        if ep is None or ep.split is not split or ep.num_data != split.num_data or ep.pad_id != self.num_entity:
-            ep = self._evals[k] = _EvalBuffers(split, batch_size, self.num_entity)
-        return ep
-
     def _eval_key(self, ep, shape):
-        m = self.model
-        rel_text = tuple(t.data_ptr() for t in (getattr(m, "rel_features", None), getattr(m, "rel_features_inv", None))
-                         if isinstance(t, torch.Tensor))
         return (("eval", id(ep)) + self._layout.epoch_key(ep.split, shape) + self._layout.model_key()
-                + (float(self.eps), int(self.num_entity)) + tuple(p.data_ptr() for p in m.parameters()) + rel_text)
+                + (float(self.eps), int(self.num_entity)) + tuple(p.data_ptr() for p in self.model.parameters())
+                + _rel_text_ptrs(self.model))
 
-    def _eval_entries(self, ep, plan, answers):
-        """The graph of every step of ``plan`` (a list), capturing the missing ones first."""
-        steps = self._layout.epoch_shapes(plan)
-        shapes = {}
-        for s, shape in enumerate(steps):
-            shapes.setdefault(shape, s)
-        self.max_graphs = max(self.max_graphs, len(shapes))
-        ents = {}
-        for shape, s in shapes.items():
-            key = self._eval_key(ep, shape)
-            if key in self._cache:
-                self._cache.move_to_end(key)
-            else:
-                self._eval_capture(ep, shape, s, key, answers)
-            ents[shape] = self._cache[key]
-        return [ents[shape] for shape in steps]
-
-    def _eval_body(self, ep, st, cursor):
-        """One evaluation step over the static buffers ``st``: the assembly and the serving step of :meth:`_run` ->
-        (outs of _run, seed or None, the step's status words: assembly, CSR[, graft staging])."""
-        seed, asm, model_asm = _assemble_step(self._layout, ep, st, cursor, self.device)
-        outs = self._run(st)
-        words = self._layout.epoch_words(st, asm, model_asm, torch.cat(self._layout.status_words(outs[0])))
-        return outs, seed, words
-
-    def _eval_capture(self, ep, shape, s0, key, answers):
-        """Capture the evaluation graph of ``shape`` under ``key``; ``s0``: a step with that shape, the one the
-        warm-up assembles."""
-        _evict(self._cache, self.max_graphs)
-        dev = self.device
-        st = self._layout.epoch_inputs(self._layout.epoch_key(ep.split, shape))
-        rng = torch.cuda.get_rng_state(dev)
-        warm_cursor = torch.full((1,), s0, dtype=torch.int64, device=dev)    # the real cursor does not move
+    def _eval_capture(self, ep, shape, s0, answers):
+        """Capture the evaluation graph of ``shape``; ``s0``: a step with that shape, the one the warm-up assembles."""
+        def body(st, cursor):
+            # the serving step of _run, its status words (CSR[, graft staging, graft CSR]) in one tensor
+            return _epoch_step(self, ep, st, cursor, self._run,
+                               lambda outs: torch.cat(self._layout.status_words(outs[0])))
         with torch.no_grad():
-            _warm_up(lambda: self._eval_body(ep, st, warm_cursor))
-        torch.cuda.set_rng_state(rng, dev)
+            st = _warm_up_epoch_step(self, ep, shape, s0, body)
         a_off, a_ids = answers
 
         def captured():
-            outs, seed, words = self._eval_body(ep, st, ep.cursor)
+            outs, seed, words = body(st, ep.cursor)
             db, _loss, _pred, pred_dist, cand_idx, cand_count, _total = outs
             if len(words) > 2:                   # gr_eval_step_record ORs the first two words (assembly, CSR)
                 ep.status[3:4].bitwise_or_(words[2])
@@ -824,7 +755,7 @@ class GraphedStep:
         ent.st, ent.g, ent.outs, ent.epoch, ent.pipe = st, g, outs, ep, None
         ent.weights = private                    # the graph formats the weights into these on every replay
         ent.planes = live_plane_buffers()        # as GraphedStep._entry: the operand planes the graph relies on
-        self._cache[key] = ent
+        self._cache[self._eval_key(ep, shape)] = ent
 
 
 # ---- training ------------------------------------------------------------------------------------------------------
@@ -912,42 +843,50 @@ class EpochRun:
         """Raise ``DeviceSplit.check``'s message when an assembly flagged an id out of range or an overflow, else (for
         GraftNet) ``GraftGraph``'s when the graft staging rejected a list, else ``TrainStepOutput.check``'s when a CSR
         build flagged ids outside the batch (reads the status unless :meth:`result` has)."""
-        from .loader import DeviceSplit
         words = self._words if self._words is not None else self.status.tolist()
-        DeviceSplit.raise_status(words[0])
-        if len(words) > 2:
-            ops.GraftGraph.raise_status(words[2])
-        if words[1]:
-            _KbLayout.raise_for([words[1]])
+        _raise_epoch_status(words[0], words[1], words[2] if len(words) > 2 else 0)
 
 
-class _EpochBuffers:
-    """The device state the epoch graphs of one (split, batch size) read and write: the cursor, the question order,
-    the kept-count tables (GraftNet: also the graft entries'), the records and the per-step Adam scalars.  Fixed
-    addresses: the graphs hold them."""
+# ---- the epoch driver: what a training epoch and an evaluation epoch share -----------------------------------------
 
-    def __init__(self, split, batch_size, max_norm):
+class _SplitBuffers:
+    """The device state the epoch graphs of one (split, batch size) read: the cursor, the question order, the
+    kept-count tables (None: every stored fact), the fact-order seed records with ``shuffle`` and the sizes of the
+    fact-order workspaces.  Fixed addresses: the graphs hold them."""
+
+    def __init__(self, split, batch_size):
         dev = split.device
         self.split, self.batch_size = split, int(batch_size)
         self.num_data = int(split.num_data)
         self.steps = (self.num_data + self.batch_size - 1) // self.batch_size
-        i64, f32 = dict(dtype=torch.int64, device=dev), dict(dtype=torch.float32, device=dev)
+        i64 = dict(dtype=torch.int64, device=dev)
         self.cursor = torch.zeros(1, **i64)
         self.order = torch.zeros(self.num_data, **i64)
-        self.kept_table = torch.zeros(max(split.num_q, 1), **i64) if split.shuffle else None
+        self.kept_table = self.graft_kept_table = None
+        self.seeds = torch.zeros(self.steps, **i64) if split.shuffle else None
+        # the fact-order workspaces of any batch
+        self.n_total = _largest(split._stored, self.batch_size)
+        self.graft_n_total = _largest(split._graft_count, self.batch_size) if split.graft else None
+
+
+class _EpochBuffers(_SplitBuffers):
+    """:class:`_SplitBuffers` of a training epoch, with the kept-count tables of ``shuffle`` (GraftNet: also the
+    graft entries'), the records and the per-step Adam scalars."""
+
+    def __init__(self, split, batch_size, max_norm):
+        super().__init__(split, batch_size)
+        dev = split.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        if split.shuffle:
+            self.kept_table = torch.zeros(max(split.num_q, 1), dtype=torch.int64, device=dev)
+            if split.graft:
+                self.graft_kept_table = torch.zeros(max(split.num_q, 1), dtype=torch.int64, device=dev)
         self.losses = torch.zeros(self.steps, **f32)
         self.grad_norms = torch.zeros(self.steps, **f32) if max_norm is not None else None
-        self.seeds = torch.zeros(self.steps, **i64) if split.shuffle else None
         self.h1 = torch.zeros(self.num_data, **f32)
         self.f1 = torch.zeros(self.num_data, **f32)
         self.status = torch.zeros(3 if split.graft else 2, dtype=torch.int32, device=dev)
         self.adam = None                 # fp32 [steps, T, 8], made at the first capture (T is known then)
-        # the fact-order workspaces of any batch
-        self.n_total = _largest(split._stored, self.batch_size)
-        self.graft_kept_table = self.graft_n_total = None
-        if split.graft:
-            self.graft_kept_table = torch.zeros(max(split.num_q, 1), **i64) if split.shuffle else None
-            self.graft_n_total = _largest(split._graft_count, self.batch_size)
 
 
 def _largest(counts, batch_size):
@@ -955,21 +894,140 @@ def _largest(counts, batch_size):
     return int(np.sort(counts)[-batch_size:].sum()) if counts.size else 0
 
 
-def _assemble_step(layout, ep, st, cursor, device):
-    """The head of a graphed epoch step over the static buffers ``st`` of ``layout``: gr_epoch_step_begin from the
-    device ``cursor`` into ``ep.order``, the model's head kernels and the batch assembly into ``st`` (the fact-order
-    seed drawn from torch's CUDA generator with ``shuffle``) -> (seed or None, the assembly status word, the model's
-    assembly word or None).  ``ep``: the epoch buffers (:class:`_EpochBuffers`, :class:`_EvalBuffers`)."""
-    split = ep.split
+def _buffers_for(cache, split, batch_size, stale, make):
+    """The buffers ``cache`` holds for (``split``, ``batch_size``), replaced by ``make()`` when there are none, when
+    they belong to another split or question count, or when ``stale(buffers)``."""
+    k = (id(split), int(batch_size))
+    ep = cache.get(k)
+    if ep is None or ep.split is not split or ep.num_data != split.num_data or stale(ep):
+        ep = cache[k] = make()
+    return ep
+
+
+def _rel_text_ptrs(model):
+    """The ``data_ptr`` of the model's relation-text features (``rel_features`` / ``rel_features_inv``) it has."""
+    return tuple(t.data_ptr() for t in (getattr(model, "rel_features", None), getattr(model, "rel_features_inv", None))
+                 if isinstance(t, torch.Tensor))
+
+
+def _split_refusal(step, split, batch_size, training, more=None):
+    """Why ``step`` runs no epoch (training with ``training``, else evaluation) of ``batch_size`` questions over
+    ``split`` (a message), or None.  In this order: anything but a ``loader.DeviceSplit`` of the model's family on its
+    device, a ``batch_size`` that is not a positive int, ``more()`` (the caller's own checks -> a message or None),
+    a ``q_type`` other than ``"seq"``, fact weights (``normalized_gnn`` / ``norm_rel``) over a ``weights="none"``
+    split."""
+    from .loader import DeviceSplit, same_device
+    if not isinstance(split, DeviceSplit):
+        return ("train_epoch takes a loader.DeviceSplit, got %s" if training
+                else "the split must be a loader.DeviceSplit, got %s") % type(split).__name__
+    why = step._layout.epoch_refusal(split, training)
+    if why is not None:
+        return why
+    if not same_device(split.device, step.device):
+        return "the split lives on %s, the model on %s" % (split.device, step.device)
+    if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or batch_size <= 0:
+        return "batch_size must be a positive int, got %r" % (batch_size,)
+    why = None if more is None else more()
+    if why is not None:
+        return why
+    if getattr(split.loader, "q_type", "seq") != "seq":
+        return "q_type must be 'seq', got %r" % (split.loader.q_type,)
+    m = step.model
+    if (m.normalized_gnn or m.norm_rel) and split.weights != "arrays":
+        return "normalized_gnn / norm_rel need fact weights: the split was built with weights='none'"
+    return None
+
+
+def _begin_epoch(split, batch_size, training, fact_dropout, buffers):
+    """The host side of an epoch's start: ``split.reset_batches`` (the loader's ``np.random`` order with
+    ``training``, its stored order without), the :func:`epoch_plan` of that order with ``fact_dropout``, the refusal
+    of a batch that overflows the split's int32 indices, then ``buffers()`` with the order uploaded ->
+    (the buffers, the plan)."""
+    split.reset_batches(is_sequential=not training)
+    L = split.loader
+    order = np.asarray(L.batches[:L.num_data], dtype=np.int64).reshape(-1)
+    plan = epoch_plan(order, split._stored, split._ents, batch_size, fact_dropout,
+                      split._graft_count if split.graft else None)
+    if split.index_dtype == torch.int32 and plan.steps and (
+            int(plan.B.max()) * split.N > _INT32_MAX or int(plan.F.max()) > _INT32_MAX):
+        raise ValueError(("train_epoch: " if training else "start_eval: ")
+                         + "a batch overflows int32 indices; use index_dtype=torch.int64")
+    ep = buffers()
+    ep.order.copy_(torch.from_numpy(order), non_blocking=True)
+    return ep, plan
+
+
+def _epoch_graphs(step, plan, key, capture):
+    """The graph of every step of ``plan`` from ``step``'s LRU (a list), one per step shape
+    (``epoch_shapes``): ``capture(shape, s0)`` captures a missing one under ``key(shape)``, ``s0`` being the first step
+    of that shape.  The LRU grows to hold them all.  The keys are read again once every graph exists: a training
+    capture can create Adam state, which its keys hold."""
+    steps = step._layout.epoch_shapes(plan)
+    shapes = {}
+    for s, shape in enumerate(steps):
+        shapes.setdefault(shape, s)
+    step.max_graphs = max(step.max_graphs, len(shapes))
+    for shape, s in shapes.items():
+        k = key(shape)
+        if k in step._cache:
+            step._cache.move_to_end(k)
+        else:
+            capture(shape, s)
+    ents = {shape: step._cache[key(shape)] for shape in shapes}
+    return [ents[shape] for shape in steps]
+
+
+def _epoch_step(step, ep, st, cursor, run, status):
+    """One step of an epoch graph over the static buffers ``st``: gr_epoch_step_begin from the device ``cursor`` into
+    ``ep.order``, the model's head kernels, the batch assembly into ``st`` (the fact-order seed drawn from torch's
+    CUDA generator with ``shuffle``), then ``outs = run(st)`` -> (outs, seed or None, the step's status words:
+    ``epoch_words`` with ``status(outs)``, the CSR / staging words)."""
+    split, layout = ep.split, step._layout
     r, cap = split._res, st.heads.numel()
     ops.epoch_step_begin(cursor, ep.order, ep.batch_size, ep.kept_table, r["q_off"], r["q_ents"],
                          split.use_self_loop, cap, st.ids, st.rows, st.kept, st.nfacts, st.kept_total, st.status)
     layout.epoch_begin(ep, st)
-    seed = torch.randint(0, 2 ** 62, (1,), device=device) if split.shuffle else None
+    seed = torch.randint(0, 2 ** 62, (1,), device=step.device) if split.shuffle else None
     _rows, _kb, _order, asm = split.assemble(st.ids, st.kept, seed, cap, cap, ep.n_total, rows=st.rows, out=st,
                                              nfacts=st.nfacts)
     asm = st.status | asm
-    return seed, asm, layout.epoch_assemble(ep, st, seed)
+    model_asm = layout.epoch_assemble(ep, st, seed)
+    outs = run(st)
+    return outs, seed, layout.epoch_words(st, asm, model_asm, status(outs))
+
+
+def _warm_up_epoch_step(step, ep, shape, s0, body):
+    """Make room in ``step``'s LRU for the epoch graph of ``shape`` and warm up its step: ``body(st, cursor)`` over
+    new static buffers ``st`` on a cursor at step ``s0`` (the real cursor does not move), torch's CUDA generator
+    left where it was -> ``st``."""
+    _evict(step._cache, step.max_graphs)
+    dev = step.device
+    st = step._layout.epoch_inputs(step._layout.epoch_key(ep.split, shape))
+    rng = torch.cuda.get_rng_state(dev)
+    warm_cursor = torch.full((1,), s0, dtype=torch.int64, device=dev)
+    _warm_up(lambda: body(st, warm_cursor))
+    torch.cuda.set_rng_state(rng, dev)
+    return st
+
+
+def _replay_epoch(ep, plan, entries):
+    """Replay the graph of every step, then set ``sample_ids`` of the split's loader to the last batch's."""
+    for ent in entries:
+        ent.g.replay()
+    if plan.steps:
+        L = ep.split.loader
+        s0 = int(plan.starts[-1])
+        L.sample_ids = L.batches[s0:min(s0 + ep.batch_size, L.num_data)]
+
+
+def _raise_epoch_status(asm, csr, staging):
+    """Raise ``DeviceSplit.check``'s message for a nonzero assembly word, else ``GraftGraph``'s for a nonzero graft
+    staging word, else the CSR build's for a nonzero CSR word."""
+    from .loader import DeviceSplit
+    DeviceSplit.raise_status(asm)
+    ops.GraftGraph.raise_status(staging)
+    if csr:
+        _KbLayout.raise_for([csr])
 
 
 class EvalRun:
@@ -1051,39 +1109,27 @@ class EvalRun:
         GraftNet) ``GraftGraph``'s when the graft staging rejected a list, else ``GraphedStep``'s when a CSR build
         flagged ids outside the batch, else when the candidate records overflowed (reads the status unless
         :meth:`result` or :meth:`records` has)."""
-        from .loader import DeviceSplit
         words = self._words
         if words is None:
             words = _EvalBuffers.views(self.blob, self.num_data)["status"].tolist()
         asm, csr, records, staging = words
-        DeviceSplit.raise_status(asm)
-        if staging:
-            ops.GraftGraph.raise_status(staging)
-        if csr:
-            _KbLayout.raise_for([csr])
+        _raise_epoch_status(asm, csr, staging)
         if records:
             raise RuntimeError("EvalRun: more ranked candidates than the %d candidate records of the split"
                                % self.cand.shape[0])
 
 
-class _EvalBuffers:
-    """The device state the evaluation graphs of one (split, batch size, pad id) read and write: the cursor, the
-    question order, the records (one byte buffer, so that one copy reads them: float64 [num_data, 5] metrics, int64
-    [num_data] candidate offsets, int64 candidate total, int32 [num_data] candidate counts, int32 [4] status words --
-    assembly, CSR, candidate records, GraftNet's graft staging -- and int8 [num_data] cases) and the candidate records
-    (int64 [capacity, 2], see gr_eval_step_record).  Fixed addresses: the graphs hold them."""
+class _EvalBuffers(_SplitBuffers):
+    """:class:`_SplitBuffers` of an evaluation (of one pad id; no kept tables: every stored fact), with the records
+    (one byte buffer, so that one copy reads them: float64 [num_data, 5] metrics, int64 [num_data] candidate offsets,
+    int64 candidate total, int32 [num_data] candidate counts, int32 [4] status words -- assembly, CSR, candidate
+    records, GraftNet's graft staging -- and int8 [num_data] cases) and the candidate records (int64 [capacity, 2],
+    see gr_eval_step_record)."""
 
     def __init__(self, split, batch_size, pad_id):
-        dev = split.device
-        self.split, self.batch_size, self.pad_id = split, int(batch_size), int(pad_id)
-        self.num_data = n = int(split.num_data)
-        self.steps = (n + self.batch_size - 1) // self.batch_size
-        self.cursor = torch.zeros(1, dtype=torch.int64, device=dev)
-        self.order = torch.zeros(n, dtype=torch.int64, device=dev)
-        self.kept_table = self.graft_kept_table = None          # every stored fact
-        self.seeds = torch.zeros(self.steps, dtype=torch.int64, device=dev) if split.shuffle else None
-        self.n_total = _largest(split._stored, self.batch_size)
-        self.graft_n_total = _largest(split._graft_count, self.batch_size) if split.graft else None
+        super().__init__(split, batch_size)
+        dev, n = split.device, self.num_data
+        self.pad_id = int(pad_id)
         self.blob = torch.zeros(self.nbytes(n), dtype=torch.uint8, device=dev)
         for name, t in self.views(self.blob, n).items():
             setattr(self, name, t)
@@ -1204,14 +1250,13 @@ class GraphedTrainStep:
         drops = tuple(float(d.p) if d.training else 0.0 for d in m.modules() if isinstance(d, torch.nn.Dropout))
         backends = (torch.backends.cudnn.enabled, torch.backends.cudnn.allow_tf32,
                     torch.backends.cuda.matmul.allow_tf32)
-        rel_text = tuple(t.data_ptr() for t in (getattr(m, "rel_features", None), getattr(m, "rel_features_inv", None))
-                         if isinstance(t, torch.Tensor))
         opt = self.optimizer
         fused = () if opt is None else (self.max_norm, any(g["weight_decay"] != 0 for g in opt.param_groups),
                                         optim.state_key(opt))
         return (
             m.training, drops, _autocast_dtype(), torch.are_deterministic_algorithms_enabled(), backends,
-            tuple(p.requires_grad for p in self._params), tuple(p.data_ptr() for p in self._params), rel_text) + fused
+            tuple(p.requires_grad for p in self._params), tuple(p.data_ptr() for p in self._params),
+            _rel_text_ptrs(m)) + fused
 
     def refusal(self, Q):
         """Why the eager forward would leave the kernels for questions of Q tokens (a message), or None."""
@@ -1310,30 +1355,6 @@ class GraphedTrainStep:
         run.check()
         return out
 
-    def _epoch_refusal(self, split, batch_size, fact_dropout):
-        from .loader import DeviceSplit, same_device
-        if self.optimizer is None:
-            return "an epoch steps the optimizer in its graphs: build the step with optimizer="
-        if not isinstance(split, DeviceSplit):
-            return "train_epoch takes a loader.DeviceSplit, got %s" % type(split).__name__
-        why = self._layout.epoch_refusal(split)
-        if why is not None:
-            return why
-        if not same_device(split.device, self.device):
-            return "the split lives on %s, the model on %s" % (split.device, self.device)
-        if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or batch_size <= 0:
-            return "batch_size must be a positive int, got %r" % (batch_size,)
-        if not split.shuffle and fact_dropout != 0:
-            return "fact_dropout must be 0 (facts come in stored order), got %r" % (fact_dropout,)
-        if split.shuffle and not 0 <= fact_dropout <= 1:
-            return "fact_dropout must be in [0, 1], got %r" % (fact_dropout,)
-        if getattr(split.loader, "q_type", "seq") != "seq":
-            return "q_type must be 'seq', got %r" % (split.loader.q_type,)
-        m = self.model
-        if (m.normalized_gnn or m.norm_rel) and split.weights != "arrays":
-            return "normalized_gnn / norm_rel need fact weights: the split was built with weights='none'"
-        return None
-
     def start_epoch(self, split, batch_size, fact_dropout):
         """Start one training epoch over ``split`` (a ``loader.DeviceSplit``) and return its :class:`EpochRun` without
         waiting for the device.
@@ -1358,20 +1379,21 @@ class GraphedTrainStep:
         device of the step's model family (a kb loader for ReaRev / NSM, a GraftNet loader for
         :class:`GraphedGraftTrainStep`), ``batch_size <= 0``, a ``fact_dropout`` ``get_batch`` refuses, and fact
         weights (``normalized_gnn`` / ``norm_rel``) over a ``weights="none"`` split."""
-        why = self._epoch_refusal(split, batch_size, fact_dropout)
+        def dropout_refusal():
+            if not split.shuffle and fact_dropout != 0:
+                return "fact_dropout must be 0 (facts come in stored order), got %r" % (fact_dropout,)
+            if split.shuffle and not 0 <= fact_dropout <= 1:
+                return "fact_dropout must be in [0, 1], got %r" % (fact_dropout,)
+            return None
+        if self.optimizer is None:
+            why = "an epoch steps the optimizer in its graphs: build the step with optimizer="
+        else:
+            why = _split_refusal(self, split, batch_size, True, dropout_refusal)
         if why is not None:
             raise ValueError("train_epoch: " + why)
         self.model.train()
-        split.reset_batches(is_sequential=False)
-        L = split.loader
-        order = np.asarray(L.batches[:L.num_data], dtype=np.int64).reshape(-1)
-        p = fact_dropout if split.shuffle else 0.0
-        plan = epoch_plan(order, split._stored, split._ents, batch_size, p, split._graft_count if split.graft else None)
-        if split.index_dtype == torch.int32 and plan.steps and (
-                int(plan.B.max()) * split.N > _INT32_MAX or int(plan.F.max()) > _INT32_MAX):
-            raise ValueError("train_epoch: a batch overflows int32 indices; use index_dtype=torch.int64")
-        ep = self._epoch_buffers(split, batch_size)
-        ep.order.copy_(torch.from_numpy(order), non_blocking=True)
+        ep, plan = _begin_epoch(split, batch_size, True, fact_dropout if split.shuffle else 0.0, lambda: _buffers_for(
+            self._epochs, split, batch_size, lambda ep: False, lambda: _EpochBuffers(split, batch_size, self.max_norm)))
         if ep.kept_table is not None:
             from .loader import kept_counts
             ep.kept_table[:split.num_q].copy_(torch.from_numpy(kept_counts(split._stored, fact_dropout)),
@@ -1379,94 +1401,56 @@ class GraphedTrainStep:
             if ep.graft_kept_table is not None:
                 ep.graft_kept_table[:split.num_q].copy_(
                     torch.from_numpy(kept_counts(split._graft_count, fact_dropout)), non_blocking=True)
-        entries = self._epoch_entries(ep, plan)
+        entries = _epoch_graphs(self, plan, lambda shape: self._epoch_key(ep, shape),
+                                lambda shape, s0: self._epoch_capture(ep, shape, s0))
+        if len({ent.fused.layout() for ent in entries if ent.fused is not None}) > 1:
+            raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
         fused = entries[0].fused if entries else None
         if fused is not None and plan.steps:
             ep.adam.copy_(torch.from_numpy(fused.epoch_scalars(plan.steps)), non_blocking=True)
         ep.cursor.zero_()
         ep.status.zero_()
-        for ent in entries:
-            ent.g.replay()
+        _replay_epoch(ep, plan, entries)
         if entries:
             last = entries[-1]
             for p, g in zip(last.params, last.grads):
                 p.grad = g
             if fused is not None:
                 fused.advance(plan.steps)
-            s0 = int(plan.starts[-1])
-            L.sample_ids = L.batches[s0:min(s0 + int(batch_size), L.num_data)]
         return EpochRun(ep.losses.clone(), None if ep.grad_norms is None else ep.grad_norms.clone(), ep.h1.clone(),
                         ep.f1.clone(), None if ep.seeds is None else ep.seeds.clone(), ep.status.clone())
-
-    def _epoch_buffers(self, split, batch_size):
-        k = (id(split), int(batch_size))
-        ep = self._epochs.get(k)
-        if ep is None or ep.split is not split or ep.num_data != split.num_data:
-            ep = self._epochs[k] = _EpochBuffers(split, batch_size, self.max_norm)
-        return ep
 
     def _epoch_key(self, ep, shape):
         return (self._layout.epoch_key(ep.split, shape) + self._state_key() + self._layout.model_key()
                 + ("epoch", id(ep)))
 
-    def _epoch_entries(self, ep, plan):
-        """The graph of every step of ``plan`` (a list), capturing the missing ones first."""
-        steps = self._layout.epoch_shapes(plan)
-        shapes = {}
-        for s, shape in enumerate(steps):
-            shapes.setdefault(shape, s)
-        self.max_graphs = max(self.max_graphs, len(shapes))
-        for shape, s in shapes.items():
-            key = self._epoch_key(ep, shape)
-            if key in self._cache:
-                self._cache.move_to_end(key)
-            else:
-                self._epoch_capture(ep, shape, s)
-        # a capture may create Adam state, which the keys hold: resolve them once all graphs exist
-        ents = {shape: self._cache[self._epoch_key(ep, shape)] for shape in shapes}
-        layouts = {ent.fused.layout() for ent in ents.values() if ent.fused is not None}
-        if len(layouts) > 1:
-            raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
-        return [ents[shape] for shape in steps]
-
-    def _epoch_body(self, ep, st, cursor, ac):
-        """One step of the epoch over the static buffers ``st``: the head kernels, the batch assembly into ``st`` and
-        the captured step of :meth:`_run` -> (outs of _run, seed or None, the step's words of ``EpochRun.status``)."""
-        seed, asm, model_asm = _assemble_step(self._layout, ep, st, cursor, self.device)
-        outs = self._run(st, ac)
-        return outs, seed, self._layout.epoch_words(st, asm, model_asm, outs[5])
-
     def _epoch_capture(self, ep, shape, s0):
         """Capture the epoch graph of ``shape`` (``_KbLayout.epoch_shapes``); ``s0``: a step of the epoch with that
         shape, the one the warm-up assembles."""
-        key = self._epoch_key(ep, shape)
-        why = self.refusal(key[3])
+        why = self.refusal(self._layout.epoch_key(ep.split, shape)[3])
         if why is not None:
             raise ValueError("GraphedTrainStep: " + why)
-        _evict(self._cache, self.max_graphs)
         ac = _autocast_dtype()
-        st = self._layout.epoch_inputs(key)
-        dev = self.device
         params = [p for p in self._params if p.requires_grad]
-        rng = torch.cuda.get_rng_state(dev)
-        warm_cursor = torch.full((1,), s0, dtype=torch.int64, device=dev)    # the real cursor does not move
 
-        def warm():
+        def body(st, cursor):
+            return _epoch_step(self, ep, st, cursor, lambda st: self._run(st, ac), lambda outs: outs[5])
+
+        def warm(st, cursor):
             _release_autograd_history(self.model, params)
-            self._epoch_body(ep, st, warm_cursor, ac)
-        _warm_up(warm)
-        torch.cuda.set_rng_state(rng, dev)
+            body(st, cursor)
+        st = _warm_up_epoch_step(self, ep, shape, s0, warm)
         fused = optim.ClipAdam(self.optimizer, params, [p.grad for p in params], self.max_norm)
         T = fused._scalars.shape[0]
         if ep.adam is None:
-            ep.adam = torch.zeros(ep.steps, T, 8, dtype=torch.float32, device=dev)
+            ep.adam = torch.zeros(ep.steps, T, 8, dtype=torch.float32, device=self.device)
         elif ep.adam.shape[1] != T:
             raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
         key = self._epoch_key(ep, shape)
         _release_autograd_history(self.model, params)
 
         def captured():
-            outs, seed, words = self._epoch_body(ep, st, ep.cursor, ac)
+            outs, seed, words = body(st, ep.cursor)
             torch.index_select(ep.adam, 0, ep.cursor, out=fused._scalars.view(1, T, 8))
             fused.launch()
             loss, _pred, _pd, h1, f1, _words = outs

@@ -5,7 +5,7 @@ Public surface mirrors the reference (cmavro/GNN-RAG ``gnn/``):
 """
 from .models import NSM, GraftNet, ReaRev  # noqa: F401
 from .evaluate import Evaluator, retrieve  # noqa: F401
-from .graphed import GraphedGraftTrainStep, GraphedStep, GraphedTrainStep  # noqa: F401
+from .graphed import GraphedGraftTrainStep, GraphedStep, GraphedTrainStep, Sweep  # noqa: F401
 
 __all__ = ["ReaRev", "NSM", "GraftNet", "Evaluator", "retrieve", "GraphedStep", "GraphedTrainStep",
-           "GraphedGraftTrainStep"]
+           "GraphedGraftTrainStep", "Sweep"]

@@ -33,8 +33,13 @@ also capture the gradient clipping and the optimizer step (:class:`optim.ClipAda
 its graft lists) from a device cursor into the epoch's question order and records the step's loss and metrics on the
 device (csrc/epoch.cu), so the host only replays graphs and reads the device once per epoch.
 :meth:`GraphedStep.start_eval` evaluates a whole split the same way, through the same epoch driver (``_split_refusal``,
-``_begin_epoch``, ``_epoch_graphs``, ``_warm_up_epoch_step``, ``_epoch_step``, ``_replay_epoch``,
+``_plan_epoch``, ``_epoch_graphs``, ``_warm_up_epoch_step``, ``_epoch_step``, ``_EpochJob``, ``_run_epochs``,
 ``_raise_epoch_status``): only the step each graph runs and the records it keeps differ.
+
+Sweeps: :class:`Sweep` runs the epochs of several independent runs (distinct models on one GPU) side by side, each
+member's graphs replayed on its own stream and drawing from its own CUDA generator and ``np.random.RandomState``, so
+that every member computes the bits it computes alone.  A single epoch is a sweep of one job without a member: the same
+``_run_epochs``.
 """
 import collections
 import contextlib
@@ -466,15 +471,17 @@ def _warm_up(fn):
     torch.cuda.synchronize()
 
 
-def _capture(fn):
-    """Capture ``fn`` into a CUDA graph -> (graph, what ``fn`` returned)."""
+def _capture(fn, stream=None):
+    """Capture ``fn`` into a CUDA graph on ``stream`` (None: torch's capture stream) -> (graph, what ``fn``
+    returned).  Graphs that replay side by side are captured on streams of their own: cuBLAS keeps one workspace per
+    (handle, stream), and a graph keeps the one of its capture stream."""
     g = torch.cuda.CUDAGraph()
     # no cyclic garbage collection during the capture: collecting a dropped step's graph there (its exec graph and
     # private pool are released) is a CUDA call that invalidates the capture
     gc_on = gc.isenabled()
     gc.disable()
     try:
-        with torch.cuda.graph(g):
+        with torch.cuda.graph(g, stream=stream):
             outs = fn()
     finally:
         if gc_on:
@@ -709,28 +716,52 @@ class GraphedStep:
         Refused (``ValueError``): anything but a CUDA ``DeviceSplit`` on the model's device of the model's family,
         ``batch_size <= 0``, a ``q_type`` other than ``"seq"``, fact weights (``normalized_gnn`` / ``norm_rel``) over
         a ``weights="none"`` split, and answers that are not integers."""
-        why = _split_refusal(self, split, batch_size, False)
+        why = self._eval_refusal(split, batch_size)
         if why is not None:
-            raise ValueError("start_eval: " + why)
-        answers = split.answer_table()
-        self.model.eval()
-        ep, plan = _begin_epoch(split, batch_size, False, 0.0, lambda: _buffers_for(
-            self._evals, split, batch_size, lambda ep: ep.pad_id != self.num_entity,
-            lambda: _EvalBuffers(split, batch_size, self.num_entity)))
-        entries = _epoch_graphs(self, plan, lambda shape: self._eval_key(ep, shape),
-                                lambda shape, s0: self._eval_capture(ep, shape, s0, answers))
-        ep.cursor.zero_()
-        ep.blob.zero_()
-        _replay_epoch(ep, plan, entries)
-        return EvalRun(ep.blob.clone(), ep.cand.clone(), None if ep.seeds is None else ep.seeds.clone(), ep.num_data,
-                       ep.order.clone())
+            raise ValueError(why)
+        return _run_epochs([self._eval_job(split, batch_size)])[0]
 
-    def _eval_key(self, ep, shape):
+    def _eval_refusal(self, split, batch_size):
+        """The ``ValueError`` message :meth:`start_eval` refuses ``(split, batch_size)`` with, or None."""
+        why = _split_refusal(self, split, batch_size, False)
+        return None if why is None else "start_eval: " + why
+
+    def _eval_job(self, split, batch_size, member=None):
+        """The :class:`_EpochJob` of :meth:`start_eval` (for the sweep member ``member``)."""
+        job = _EpochJob(split, member)
+
+        def start():
+            job.answers = split.answer_table()
+            job.plan, job.order, job.batches = _plan_epoch(split, batch_size, False, 0.0, job.rng())
+
+        def begin():
+            self.model.eval()
+            job.ep = _buffers_for(self._evals, split, batch_size, lambda ep: ep.pad_id != self.num_entity,
+                                  lambda: _EvalBuffers(split, batch_size, self.num_entity))
+            _upload_order(job.ep, job.order)
+
+        def capture():
+            ep = job.ep
+            entries = _epoch_graphs(self, job.plan, lambda shape: self._eval_key(ep, shape, member),
+                                    lambda shape, s0: self._eval_capture(ep, shape, s0, job.answers, member))
+            ep.cursor.zero_()
+            ep.blob.zero_()
+            return entries
+
+        def finish():
+            ep = job.ep
+            job.set_sample_ids()
+            return EvalRun(ep.blob.clone(), ep.cand.clone(), None if ep.seeds is None else ep.seeds.clone(),
+                           ep.num_data, ep.order.clone())
+        job.start, job.begin, job.capture, job.finish = start, begin, capture, finish
+        return job
+
+    def _eval_key(self, ep, shape, member=None):
         return (("eval", id(ep)) + self._layout.epoch_key(ep.split, shape) + self._layout.model_key()
                 + (float(self.eps), int(self.num_entity)) + tuple(p.data_ptr() for p in self.model.parameters())
-                + _rel_text_ptrs(self.model))
+                + _rel_text_ptrs(self.model) + _member_key(member))
 
-    def _eval_capture(self, ep, shape, s0, answers):
+    def _eval_capture(self, ep, shape, s0, answers, member=None):
         """Capture the evaluation graph of ``shape``; ``s0``: a step with that shape, the one the warm-up assembles."""
         def body(st, cursor):
             # the serving step of _run, its status words (CSR[, graft staging, graft CSR]) in one tensor
@@ -750,12 +781,13 @@ class GraphedStep:
                                  ep.cand_off, ep.cand, ep.cand_total, ep.seeds, ep.status[:3])
             return outs
         with torch.no_grad(), ops.graph_private_weights() as private:
-            g, outs = _capture(captured)
+            g, outs = _capture(captured, _capture_stream(member))
         ent = _Captured()
         ent.st, ent.g, ent.outs, ent.epoch, ent.pipe = st, g, outs, ep, None
         ent.weights = private                    # the graph formats the weights into these on every replay
         ent.planes = live_plane_buffers()        # as GraphedStep._entry: the operand planes the graph relies on
-        self._cache[self._eval_key(ep, shape)] = ent
+        ent.draws = _member_draws(member)        # its generator and scratch (and the id in the key) stay alive
+        self._cache[self._eval_key(ep, shape, member)] = ent
 
 
 # ---- training ------------------------------------------------------------------------------------------------------
@@ -938,12 +970,30 @@ def _split_refusal(step, split, batch_size, training, more=None):
     return None
 
 
-def _begin_epoch(split, batch_size, training, fact_dropout, buffers):
-    """The host side of an epoch's start: ``split.reset_batches`` (the loader's ``np.random`` order with
-    ``training``, its stored order without), the :func:`epoch_plan` of that order with ``fact_dropout``, the refusal
-    of a batch that overflows the split's int32 indices, then ``buffers()`` with the order uploaded ->
-    (the buffers, the plan)."""
-    split.reset_batches(is_sequential=not training)
+@contextlib.contextmanager
+def _numpy_random(rng):
+    """``rng`` (a ``np.random.RandomState``) as the global ``np.random`` stream inside the block: the global state is
+    set to ``rng``'s on entry; on exit ``rng`` takes the state the block left and the global state is put back.
+    ``rng`` None: the global stream itself."""
+    if rng is None:
+        yield
+        return
+    saved = np.random.get_state()
+    np.random.set_state(rng.get_state())
+    try:
+        yield
+    finally:
+        rng.set_state(np.random.get_state())
+        np.random.set_state(saved)
+
+
+def _plan_epoch(split, batch_size, training, fact_dropout, rng=None):
+    """The host side of an epoch's start, before anything reaches the device: ``split.reset_batches`` (the loader's
+    ``np.random`` order with ``training``, its stored order without; a sweep member's ``rng`` stands in for
+    ``np.random`` there), the :func:`epoch_plan` of that order with ``fact_dropout`` and the refusal of a batch that
+    overflows the split's int32 indices -> (the plan, the order as int64, the loader's ``batches``)."""
+    with _numpy_random(rng):
+        split.reset_batches(is_sequential=not training)
     L = split.loader
     order = np.asarray(L.batches[:L.num_data], dtype=np.int64).reshape(-1)
     plan = epoch_plan(order, split._stored, split._ents, batch_size, fact_dropout,
@@ -952,9 +1002,11 @@ def _begin_epoch(split, batch_size, training, fact_dropout, buffers):
             int(plan.B.max()) * split.N > _INT32_MAX or int(plan.F.max()) > _INT32_MAX):
         raise ValueError(("train_epoch: " if training else "start_eval: ")
                          + "a batch overflows int32 indices; use index_dtype=torch.int64")
-    ep = buffers()
+    return plan, order, L.batches
+
+
+def _upload_order(ep, order):
     ep.order.copy_(torch.from_numpy(order), non_blocking=True)
-    return ep, plan
 
 
 def _epoch_graphs(step, plan, key, capture):
@@ -1010,14 +1062,133 @@ def _warm_up_epoch_step(step, ep, shape, s0, body):
     return st
 
 
-def _replay_epoch(ep, plan, entries):
-    """Replay the graph of every step, then set ``sample_ids`` of the split's loader to the last batch's."""
-    for ent in entries:
-        ent.g.replay()
-    if plan.steps:
-        L = ep.split.loader
-        s0 = int(plan.starts[-1])
-        L.sample_ids = L.batches[s0:min(s0 + ep.batch_size, L.num_data)]
+class _EpochJob:
+    """One epoch of one step over ``split``, from its refusal to its run, in the phases :func:`_run_epochs` calls:
+    ``start()`` (host only: the order and the plan, which may still refuse the epoch; sets ``plan``, ``order`` and
+    ``batches``), ``begin()`` (the buffers and the uploads: sets ``ep``), ``capture()`` (the graphs the epoch needs and
+    whatever must precede its first replay -> the graph of every step) and, after the replays, ``finish()`` -> the
+    run.  ``member``: the :class:`Sweep` member it runs for, None for a solo epoch."""
+
+    def __init__(self, split, member):
+        self.split, self.member = split, member
+        self.ep = self.plan = self.order = self.batches = None
+        self.start = self.begin = self.capture = self.finish = None
+
+    def rng(self):
+        return None if self.member is None else self.member.rng
+
+    def set_sample_ids(self):
+        """``sample_ids`` of the split's loader := the epoch's last batch (its ids in the order the epoch drew)."""
+        if self.plan.steps:
+            L, s0 = self.ep.split.loader, int(self.plan.starts[-1])
+            L.sample_ids = self.batches[s0:min(s0 + self.ep.batch_size, L.num_data)]
+
+
+_NO_BATCHES = object()
+
+
+def _start_all(jobs):
+    """Every job's ``start``.  When one refuses, the members' ``RandomState`` objects and their loaders' ``batches``
+    are put back as they were, so a refused sweep leaves nothing drawn (a solo job has no member to put back)."""
+    saved = [(j.member.rng.get_state(), j.split.loader, vars(j.split.loader).get("batches", _NO_BATCHES))
+             for j in jobs if j.member is not None]
+    try:
+        for j in jobs:
+            j.start()
+    except BaseException:
+        for (state, L, batches), j in zip(saved, [j for j in jobs if j.member is not None]):
+            j.member.rng.set_state(state)
+            if batches is _NO_BATCHES:
+                vars(L).pop("batches", None)
+            else:
+                L.batches = batches
+        raise
+
+
+def replay_schedule(steps):
+    """The replay order of epochs of ``steps`` steps each (one count per job): [(job, step)], step s of every job that
+    has one before step s + 1 of any, jobs in their order within a step."""
+    steps = [int(n) for n in steps]
+    return [(k, s) for s in range(max(steps, default=0)) for k, n in enumerate(steps) if s < n]
+
+
+def _run_epochs(jobs):
+    """Run the epochs ``jobs`` (:class:`_EpochJob`, at most one per step) -> their runs.  Every job's ``start`` (the
+    host side, where an epoch can still be refused: :func:`_start_all`), then every job's ``begin``, then every job's
+    ``capture``, so that no capture (and none of its device-wide synchronisations) lands between replays; then the
+    graphs in :func:`replay_schedule` order, each job's on its member's stream (a solo job's on the current stream),
+    then ``finish`` of each job on the current stream, which waits on the members' streams first.  A member's work
+    between the two waits (uploads, replays) goes to its own stream, and nothing waits on the device.  Because of
+    the two waits, the epochs of one call overlap each other but not the work of an earlier or a later call."""
+    _start_all(jobs)
+    cur = torch.cuda.current_stream()
+    streams = [cur if j.member is None else j.member.stream for j in jobs]
+    for s in streams:
+        if s != cur:
+            s.wait_stream(cur)
+    for j, s in zip(jobs, streams):
+        with torch.cuda.stream(s):
+            j.begin()
+    entries = []
+    for j, s in zip(jobs, streams):
+        with torch.cuda.stream(s), _member_scope(j.member):
+            entries.append(j.capture())
+    for k, i in replay_schedule([len(e) for e in entries]):
+        with torch.cuda.stream(streams[k]):
+            entries[k][i].g.replay()
+    for s in streams:
+        if s != cur:
+            cur.wait_stream(s)
+    return [j.finish() for j in jobs]
+
+
+def _member_key(member):
+    """The part of an epoch graph's key that names where it draws its random numbers and keeps its scratch: nothing
+    for torch's default generator and the shared scratch, the sweep member's :class:`_Draws` otherwise."""
+    return () if member is None else ("member", id(member.draws))
+
+
+def _member_draws(member):
+    """What a member's graph holds for as long as it lives: its :class:`_Draws` (None for a solo graph)."""
+    return None if member is None else member.draws
+
+
+def _capture_stream(member):
+    return None if member is None else member.draws.capture_stream
+
+
+def _shared_scratch():
+    """The scratch buffers the forwards keep per shape rather than per model, so that models of one shape share them:
+    (owner, attribute) of each dict -- the reasoning layers' operand planes, the relation-feature planes and the
+    aggregation's tile counter.  A graph writes them on every replay, so graphs that replay side by side need
+    copies of their own (:func:`_member_scope`)."""
+    from . import modules
+    return ((modules._GraphLayerBase, "_plane_cache"), (modules.GraftLayer, "_plane_cache"), (ops.RelFeatures, "_buf"),
+            (ops, "_TILE_COUNTER"))
+
+
+@contextlib.contextmanager
+def _member_scope(member):
+    """A sweep member's captures: its generator as the graph-safe state of torch's default CUDA generator (each graph
+    captured here registers it, so only this member's replays advance it) and its own copies of every
+    :func:`_shared_scratch` dict, so that members replaying side by side never write the same buffer.  Nothing for
+    None."""
+    if member is None:
+        yield
+        return
+    draws = member.draws
+    gen = torch.cuda.default_generators[draws.device.index]
+    shared = _shared_scratch()
+    saved = gen.graphsafe_get_state(), [getattr(owner, name) for owner, name in shared]
+    gen.graphsafe_set_state(draws.generator.graphsafe_get_state())
+    for (owner, name), mine in zip(shared, draws.scratch):
+        setattr(owner, name, mine)
+    try:
+        yield
+    finally:
+        for (owner, name), theirs in zip(shared, saved[1]):
+            setattr(owner, name, theirs)
+        gen.graphsafe_set_state(saved[0])
 
 
 def _raise_epoch_status(asm, csr, staging):
@@ -1379,6 +1550,14 @@ class GraphedTrainStep:
         device of the step's model family (a kb loader for ReaRev / NSM, a GraftNet loader for
         :class:`GraphedGraftTrainStep`), ``batch_size <= 0``, a ``fact_dropout`` ``get_batch`` refuses, and fact
         weights (``normalized_gnn`` / ``norm_rel``) over a ``weights="none"`` split."""
+        why = self._train_refusal(split, batch_size, fact_dropout)
+        if why is not None:
+            raise ValueError(why)
+        return _run_epochs([self._train_job(split, batch_size, fact_dropout)])[0]
+
+    def _train_refusal(self, split, batch_size, fact_dropout):
+        """The ``ValueError`` message :meth:`start_epoch` refuses ``(split, batch_size, fact_dropout)`` with, or
+        None."""
         def dropout_refusal():
             if not split.shuffle and fact_dropout != 0:
                 return "fact_dropout must be 0 (facts come in stored order), got %r" % (fact_dropout,)
@@ -1389,42 +1568,63 @@ class GraphedTrainStep:
             why = "an epoch steps the optimizer in its graphs: build the step with optimizer="
         else:
             why = _split_refusal(self, split, batch_size, True, dropout_refusal)
-        if why is not None:
-            raise ValueError("train_epoch: " + why)
-        self.model.train()
-        ep, plan = _begin_epoch(split, batch_size, True, fact_dropout if split.shuffle else 0.0, lambda: _buffers_for(
-            self._epochs, split, batch_size, lambda ep: False, lambda: _EpochBuffers(split, batch_size, self.max_norm)))
-        if ep.kept_table is not None:
-            from .loader import kept_counts
-            ep.kept_table[:split.num_q].copy_(torch.from_numpy(kept_counts(split._stored, fact_dropout)),
-                                              non_blocking=True)
-            if ep.graft_kept_table is not None:
-                ep.graft_kept_table[:split.num_q].copy_(
-                    torch.from_numpy(kept_counts(split._graft_count, fact_dropout)), non_blocking=True)
-        entries = _epoch_graphs(self, plan, lambda shape: self._epoch_key(ep, shape),
-                                lambda shape, s0: self._epoch_capture(ep, shape, s0))
-        if len({ent.fused.layout() for ent in entries if ent.fused is not None}) > 1:
-            raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
-        fused = entries[0].fused if entries else None
-        if fused is not None and plan.steps:
-            ep.adam.copy_(torch.from_numpy(fused.epoch_scalars(plan.steps)), non_blocking=True)
-        ep.cursor.zero_()
-        ep.status.zero_()
-        _replay_epoch(ep, plan, entries)
-        if entries:
-            last = entries[-1]
-            for p, g in zip(last.params, last.grads):
-                p.grad = g
-            if fused is not None:
-                fused.advance(plan.steps)
-        return EpochRun(ep.losses.clone(), None if ep.grad_norms is None else ep.grad_norms.clone(), ep.h1.clone(),
-                        ep.f1.clone(), None if ep.seeds is None else ep.seeds.clone(), ep.status.clone())
+        return None if why is None else "train_epoch: " + why
 
-    def _epoch_key(self, ep, shape):
+    def _train_job(self, split, batch_size, fact_dropout, member=None):
+        """The :class:`_EpochJob` of :meth:`start_epoch` (for the sweep member ``member``)."""
+        job = _EpochJob(split, member)
+
+        def start():
+            job.plan, job.order, job.batches = _plan_epoch(split, batch_size, True,
+                                                           fact_dropout if split.shuffle else 0.0, job.rng())
+
+        def begin():
+            self.model.train()
+            ep = job.ep = _buffers_for(self._epochs, split, batch_size, lambda ep: False,
+                                       lambda: _EpochBuffers(split, batch_size, self.max_norm))
+            _upload_order(ep, job.order)
+            if ep.kept_table is not None:
+                from .loader import kept_counts
+                ep.kept_table[:split.num_q].copy_(torch.from_numpy(kept_counts(split._stored, fact_dropout)),
+                                                  non_blocking=True)
+                if ep.graft_kept_table is not None:
+                    ep.graft_kept_table[:split.num_q].copy_(
+                        torch.from_numpy(kept_counts(split._graft_count, fact_dropout)), non_blocking=True)
+
+        def capture():
+            ep, plan = job.ep, job.plan
+            entries = _epoch_graphs(self, plan, lambda shape: self._epoch_key(ep, shape, member),
+                                    lambda shape, s0: self._epoch_capture(ep, shape, s0, member))
+            if len({ent.fused.layout() for ent in entries if ent.fused is not None}) > 1:
+                raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
+            fused = entries[0].fused if entries else None
+            if fused is not None and plan.steps:
+                ep.adam.copy_(torch.from_numpy(fused.epoch_scalars(plan.steps)), non_blocking=True)
+            ep.cursor.zero_()
+            ep.status.zero_()
+            job.entries = entries
+            return entries
+
+        def finish():
+            ep, entries = job.ep, job.entries
+            job.set_sample_ids()
+            if entries:
+                last = entries[-1]
+                for p, g in zip(last.params, last.grads):
+                    p.grad = g
+                if entries[0].fused is not None:
+                    entries[0].fused.advance(job.plan.steps)
+            return EpochRun(ep.losses.clone(), None if ep.grad_norms is None else ep.grad_norms.clone(),
+                            ep.h1.clone(), ep.f1.clone(), None if ep.seeds is None else ep.seeds.clone(),
+                            ep.status.clone())
+        job.start, job.begin, job.capture, job.finish = start, begin, capture, finish
+        return job
+
+    def _epoch_key(self, ep, shape, member=None):
         return (self._layout.epoch_key(ep.split, shape) + self._state_key() + self._layout.model_key()
-                + ("epoch", id(ep)))
+                + ("epoch", id(ep)) + _member_key(member))
 
-    def _epoch_capture(self, ep, shape, s0):
+    def _epoch_capture(self, ep, shape, s0, member=None):
         """Capture the epoch graph of ``shape`` (``_KbLayout.epoch_shapes``); ``s0``: a step of the epoch with that
         shape, the one the warm-up assembles."""
         why = self.refusal(self._layout.epoch_key(ep.split, shape)[3])
@@ -1446,7 +1646,7 @@ class GraphedTrainStep:
             ep.adam = torch.zeros(ep.steps, T, 8, dtype=torch.float32, device=self.device)
         elif ep.adam.shape[1] != T:
             raise RuntimeError("train_epoch: the epoch's graphs update different parameter sets")
-        key = self._epoch_key(ep, shape)
+        key = self._epoch_key(ep, shape, member)
         _release_autograd_history(self.model, params)
 
         def captured():
@@ -1459,8 +1659,10 @@ class GraphedTrainStep:
             ops.epoch_step_record(ep.cursor, ep.batch_size, ep.num_data, loss.float(), fused.grad_norm, seed, h1, f1,
                                   words[0], words[1], ep.losses, ep.grad_norms, ep.seeds, ep.h1, ep.f1, ep.status[:2])
             return outs
-        g, outs = _capture(captured)
-        return self._store(key, st, g, outs, params, fused, ep)
+        g, outs = _capture(captured, _capture_stream(member))
+        ent = self._store(key, st, g, outs, params, fused, ep)
+        ent.draws = _member_draws(member)        # its generator and scratch (and the id in the key) stay alive
+        return ent
 
 
 class GraphedGraftTrainStep(GraphedTrainStep):
@@ -1492,3 +1694,181 @@ class GraphedGraftTrainStep(GraphedTrainStep):
             raise ValueError("GraphedGraftTrainStep takes the 9/10-tuple of GraftSingleDataLoader.get_batch, not a "
                              "%d-tuple" % len(batch))
         return super().key(batch)
+
+
+# ---- several runs side by side on one GPU ----------------------------------------------------------------------------
+
+class _Draws:
+    """What a sweep member's graphs hold for as long as they live, and nothing more (no step: a graph cached in a step's
+    LRU must not keep its step alive through a cycle): the member's CUDA generator, its device, its copies of the
+    :func:`_shared_scratch` dicts and the stream its graphs are captured on.  Its ``id`` is part of their keys."""
+
+    def __init__(self, generator, device):
+        self.generator, self.device = generator, device
+        self.scratch = tuple({} for _ in _shared_scratch())
+        self.capture_stream = torch.cuda.Stream(device=device)
+
+
+class _Member:
+    """One run of a :class:`Sweep`: its step, its ``np.random.RandomState`` (``rng``), the stream its uploads and
+    replays go to, its :class:`_Draws` (the CUDA generator, the scratch and the capture stream its graphs keep) and the
+    :class:`GraphedStep` its evaluations run through."""
+
+    def __init__(self, step, generator, rng):
+        self.step, self.rng = step, rng
+        self.draws = _Draws(generator, step.device)
+        self.stream = torch.cuda.Stream(device=step.device)
+        self._eval_step = step if isinstance(step, GraphedStep) else None
+
+    @property
+    def generator(self):
+        return self.draws.generator
+
+    def eval_step(self):
+        """The member's :class:`GraphedStep`: the step itself, or for a training step one over its model (the model's
+        ``num_entity`` and ``eps``), made at the first use."""
+        if self._eval_step is None:
+            m = self.step.model
+            self._eval_step = GraphedStep(m, m.num_entity)
+        return self._eval_step
+
+
+def _check_members(steps):
+    """Refuse (``ValueError``) sweep members that are not graphed steps, that share a model or that are not on one
+    CUDA device."""
+    if not steps:
+        raise ValueError("Sweep: no members")
+    for i, s in enumerate(steps):
+        if not isinstance(s, (GraphedStep, GraphedTrainStep)):
+            raise ValueError("Sweep: member %d is a %s; members are GraphedTrainStep, GraphedGraftTrainStep or "
+                             "GraphedStep objects" % (i, type(s).__name__))
+    seen = {}
+    for i, s in enumerate(steps):
+        j = seen.setdefault(id(s.model), i)
+        if j != i:
+            raise ValueError("Sweep: members %d and %d hold the same model; each run needs a model of its own" % (j, i))
+    devices = [torch.device(s.device) for s in steps]
+    if any(d.type != "cuda" for d in devices):
+        raise ValueError("Sweep: the members' models are on %s; a sweep runs on one CUDA device"
+                         % ", ".join(sorted({str(d) for d in devices})))
+    if len({d.index for d in devices}) > 1:
+        raise ValueError("Sweep: members on different devices (%s); a sweep runs on one CUDA device"
+                         % ", ".join(sorted({str(d) for d in devices})))
+
+
+def _job_refusal(member, job, training):
+    """Why the sweep refuses ``job`` for ``member`` (a message), or None: what :meth:`GraphedTrainStep.start_epoch`
+    (with ``training``) or :meth:`GraphedStep.start_eval` refuses, with their messages, a job that is not their
+    argument tuple, and a training job for a :class:`GraphedStep`.  ``job`` None: the member sits this one out."""
+    if job is None:
+        return None
+    name, arity = ("start_epochs", 3) if training else ("start_evals", 2)
+    if not isinstance(job, (tuple, list)) or len(job) != arity:
+        return "Sweep.%s: a job is %s or None, got %r" % (
+            name, "(split, batch_size, fact_dropout)" if training else "(split, batch_size)", job)
+    if training:
+        if not isinstance(member.step, GraphedTrainStep):
+            return ("Sweep.start_epochs: a GraphedStep member evaluates only; a training member is a "
+                    "GraphedTrainStep / GraphedGraftTrainStep built with optimizer=")
+        return member.step._train_refusal(*job)
+    return member.eval_step()._eval_refusal(*job)
+
+
+class Sweep:
+    """Several independent runs on one GPU, their epochs side by side: each member replays its epoch graphs on a
+    stream of its own, so the small launches of one run fill the SMs the others leave idle.  Each member's results are
+    bit for bit those of the same epochs run alone (:meth:`GraphedTrainStep.start_epoch`,
+    :meth:`GraphedStep.start_eval`) with torch's default CUDA generator at the member's generator state and
+    ``np.random`` at its ``RandomState``, whatever the other members run (DESIGN §4.14).
+
+    ``steps``: the members, each a :class:`GraphedTrainStep` / :class:`GraphedGraftTrainStep` built with
+    ``optimizer=`` or a :class:`GraphedStep` that only evaluates; each over a model of its own, all on one CUDA device.
+    ``generators``: one ``torch.Generator`` per member on that device, else each member gets a generator seeded with
+    one draw from torch's default CUDA generator when the sweep is built.  A member's graphs are captured with its
+    generator as the default generator's graph-safe state, so they draw its fact-order seeds, its dropout masks and
+    GraftNet's dropout seeds from it, and only its own replays advance it.  ``rngs``: one ``np.random.RandomState``
+    per member, else each seeded with one draw from ``np.random`` when the sweep is built; it stands in for
+    ``np.random`` while the member's ``reset_batches`` draws its epoch order, and nowhere else.
+
+    :meth:`start_epochs` and :meth:`start_evals` take one job per member -- the arguments of ``start_epoch`` /
+    ``start_eval``, or None for a member that sits it out -- and return one :class:`EpochRun` / :class:`EvalRun` per
+    member (None for those) without waiting for the device.  Every job is checked first, with the messages of the
+    single-run methods; then every member's host start and uploads, then every capture any member needs, and only
+    then the replays: step s of every member, then step s + 1, members with fewer steps dropping out.  Between
+    epochs, LR schedulers, ``optimizer.state_dict()`` and checkpoints work per member as they do for a single run.
+    Members may share a ``DeviceSplit``: the split holds no scratch its steps write.  A shared split's
+    ``loader.sample_ids`` ends as the last batch of the last member (in member order) that ran over it.  A refused
+    job raises before any member's order is drawn: a refusal found while planning (an int32 overflow, answers that
+    are not integers) puts every member's ``RandomState`` and its loader's ``batches`` back.
+
+    The epochs of one call overlap each other.  Consecutive calls do not overlap: each call's members wait for the
+    caller's stream first, and the caller's stream waits for them at the end, so ``start_evals`` right after
+    ``start_epochs`` runs the evaluations after the training replays.
+
+    Build a sweep once and keep it.  A graph is bound to the generator it was captured with, so each sweep captures
+    its members' graphs anew; they stay in the steps' LRUs (``max_graphs``) and are released by its eviction."""
+
+    def __init__(self, steps, generators=None, rngs=None):
+        steps = list(steps)
+        _check_members(steps)
+        K, dev = len(steps), torch.device(steps[0].device)
+        if generators is None:
+            seeds = torch.randint(0, 2 ** 62, (K,), dtype=torch.int64, device=dev).tolist()
+            generators = [torch.Generator(device=dev) for _ in range(K)]
+            for g, s in zip(generators, seeds):
+                g.manual_seed(s)
+        generators = list(generators)
+        from .loader import same_device
+        if len(generators) != K or any(not isinstance(g, torch.Generator) or not same_device(g.device, dev)
+                                       for g in generators):
+            raise ValueError("Sweep: generators must be %d torch.Generator objects on %s" % (K, dev))
+        if len({id(g) for g in generators}) != K:
+            raise ValueError("Sweep: two members share a generator; each run needs its own")
+        if rngs is None:
+            rngs = [np.random.RandomState(s) for s in np.random.randint(0, 2 ** 31 - 1, size=K).tolist()]
+        rngs = list(rngs)
+        if len(rngs) != K or any(not isinstance(r, np.random.RandomState) for r in rngs):
+            raise ValueError("Sweep: rngs must be %d np.random.RandomState objects" % K)
+        if len({id(r) for r in rngs}) != K:
+            raise ValueError("Sweep: two members share a RandomState; each run needs its own")
+        self.members = [_Member(s, g, r) for s, g, r in zip(steps, generators, rngs)]
+
+    @property
+    def generators(self):
+        return [m.generator for m in self.members]
+
+    @property
+    def rngs(self):
+        return [m.rng for m in self.members]
+
+    def eval_step(self, i):
+        """The :class:`GraphedStep` member ``i`` evaluates through."""
+        return self.members[i].eval_step()
+
+    def start_epochs(self, jobs):
+        """One training epoch per member with a job ``(split, batch_size, fact_dropout)`` -> one :class:`EpochRun`
+        per member (None where the job is None), as :meth:`GraphedTrainStep.start_epoch` returns it."""
+        return self._start(jobs, True)
+
+    def start_evals(self, jobs):
+        """One evaluation per member with a job ``(split, batch_size)`` -> one :class:`EvalRun` per member (None where
+        the job is None), as :meth:`GraphedStep.start_eval` returns it.  A training member evaluates its model
+        through :meth:`eval_step`."""
+        return self._start(jobs, False)
+
+    def _start(self, jobs, training):
+        jobs = list(jobs)
+        if len(jobs) != len(self.members):
+            raise ValueError("Sweep.%s: %d jobs for %d members (None: a member sits this one out)"
+                             % ("start_epochs" if training else "start_evals", len(jobs), len(self.members)))
+        for m, job in zip(self.members, jobs):
+            why = _job_refusal(m, job, training)
+            if why is not None:
+                raise ValueError(why)
+        todo = [(k, m, job) for k, (m, job) in enumerate(zip(self.members, jobs)) if job is not None]
+        made = [m.step._train_job(*job, member=m) if training else m.eval_step()._eval_job(*job, member=m)
+                for _k, m, job in todo]
+        runs = [None] * len(jobs)
+        for (k, _m, _job), run in zip(todo, _run_epochs(made)):
+            runs[k] = run
+        return runs

@@ -694,7 +694,7 @@ class GraphedStep:
         run.check()
         return out
 
-    def start_eval(self, split, batch_size):
+    def start_eval(self, split, batch_size, path_targets=None):
         """Start an evaluation of the whole split ``split`` (a ``loader.DeviceSplit``) and return its :class:`EvalRun`
         without waiting for the device.
 
@@ -713,22 +713,35 @@ class GraphedStep:
         in-place ``optimizer.step()`` and ``load_state_dict``.  Once the graphs exist nothing here waits on the device.
         Afterwards ``split.loader.sample_ids`` is the last batch's.
 
+        ``path_targets``: an int T >= 1 makes each step's graph also compute the retrieved shortest-path node sets of
+        its questions (gr_eval_step_paths, after the ranking): the BFS from each of the question's seeds (its local
+        indices with ``query_entities != 0``, ascending, at most ``DeviceSplit.max_seeds()``) and each of its first
+        ``min(count, T)`` ranked candidates over the step's kb CSR, the on-path nodes compacted into node records sized
+        like the candidate records; :meth:`EvalRun.paths` reads them.  T is part of the graph key; without it the
+        graphs are those of an evaluation without paths.
+
         Refused (``ValueError``): anything but a CUDA ``DeviceSplit`` on the model's device of the model's family,
         ``batch_size <= 0``, a ``q_type`` other than ``"seq"``, fact weights (``normalized_gnn`` / ``norm_rel``) over
-        a ``weights="none"`` split, and answers that are not integers."""
-        why = self._eval_refusal(split, batch_size)
+        a ``weights="none"`` split, then a ``path_targets`` that is not a positive int or whose BFS workspace
+        (B * (max_seeds + T) * N for the largest batch) overflows int32 indexing, and answers that are not
+        integers."""
+        why = self._eval_refusal(split, batch_size, path_targets)
         if why is not None:
             raise ValueError(why)
-        return _run_epochs([self._eval_job(split, batch_size)])[0]
+        return _run_epochs([self._eval_job(split, batch_size, path_targets)])[0]
 
-    def _eval_refusal(self, split, batch_size):
-        """The ``ValueError`` message :meth:`start_eval` refuses ``(split, batch_size)`` with, or None."""
+    def _eval_refusal(self, split, batch_size, path_targets=None):
+        """The ``ValueError`` message :meth:`start_eval` refuses ``(split, batch_size, path_targets)`` with, or
+        None."""
         why = _split_refusal(self, split, batch_size, False)
+        if why is None and path_targets is not None:
+            why = paths_refusal(split, batch_size, path_targets)
         return None if why is None else "start_eval: " + why
 
-    def _eval_job(self, split, batch_size, member=None):
+    def _eval_job(self, split, batch_size, path_targets=None, member=None):
         """The :class:`_EpochJob` of :meth:`start_eval` (for the sweep member ``member``)."""
         job = _EpochJob(split, member)
+        T = None if path_targets is None else int(path_targets)
 
         def start():
             job.answers = split.answer_table()
@@ -739,30 +752,42 @@ class GraphedStep:
             job.ep = _buffers_for(self._evals, split, batch_size, lambda ep: ep.pad_id != self.num_entity,
                                   lambda: _EvalBuffers(split, batch_size, self.num_entity))
             _upload_order(job.ep, job.order)
+            if T is not None and T not in job.ep.paths:
+                job.ep.paths[T] = _EvalPaths(split.device, job.ep.num_data, split.max_seeds(), T, job.ep.capacity)
 
         def capture():
             ep = job.ep
-            entries = _epoch_graphs(self, job.plan, lambda shape: self._eval_key(ep, shape, member),
-                                    lambda shape, s0: self._eval_capture(ep, shape, s0, job.answers, member))
+            entries = _epoch_graphs(self, job.plan, lambda shape: self._eval_key(ep, shape, member, T),
+                                    lambda shape, s0: self._eval_capture(ep, shape, s0, job.answers, member, T))
             ep.cursor.zero_()
             ep.blob.zero_()
+            if T is not None:
+                ep.paths[T].blob.zero_()
             return entries
 
         def finish():
             ep = job.ep
             job.set_sample_ids()
+            paths = None
+            if T is not None:
+                pp = ep.paths[T]
+                c, order = split.seed_counts(), job.order
+                known = (order >= 0) & (order < c.size)          # an id out of range is check()'s to report
+                seeds = np.where(known, c[np.where(known, order, 0)] if c.size else 0, 0)
+                paths = (pp.blob.clone(), pp.S, pp.T, pp.capacity, seeds)
             return EvalRun(ep.blob.clone(), ep.cand.clone(), None if ep.seeds is None else ep.seeds.clone(),
-                           ep.num_data, ep.order.clone())
+                           ep.num_data, ep.order.clone(), paths)
         job.start, job.begin, job.capture, job.finish = start, begin, capture, finish
         return job
 
-    def _eval_key(self, ep, shape, member=None):
+    def _eval_key(self, ep, shape, member=None, T=None):
         return (("eval", id(ep)) + self._layout.epoch_key(ep.split, shape) + self._layout.model_key()
                 + (float(self.eps), int(self.num_entity)) + tuple(p.data_ptr() for p in self.model.parameters())
-                + _rel_text_ptrs(self.model) + _member_key(member))
+                + _rel_text_ptrs(self.model) + _member_key(member) + (() if T is None else ("paths", T)))
 
-    def _eval_capture(self, ep, shape, s0, answers, member=None):
-        """Capture the evaluation graph of ``shape``; ``s0``: a step with that shape, the one the warm-up assembles."""
+    def _eval_capture(self, ep, shape, s0, answers, member=None, T=None):
+        """Capture the evaluation graph of ``shape``; ``s0``: a step with that shape, the one the warm-up assembles;
+        ``T``: the path targets (None: no node sets)."""
         def body(st, cursor):
             # the serving step of _run, its status words (CSR[, graft staging, graft CSR]) in one tensor
             return _epoch_step(self, ep, st, cursor, self._run,
@@ -776,6 +801,11 @@ class GraphedStep:
             db, _loss, _pred, pred_dist, cand_idx, cand_count, _total = outs
             if len(words) > 2:                   # gr_eval_step_record ORs the first two words (assembly, CSR)
                 ep.status[3:4].bitwise_or_(words[2])
+            if T is not None:                    # before gr_eval_step_record, which moves the cursor
+                pp = ep.paths[T]
+                ops.eval_step_paths(ep.cursor, ep.batch_size, ep.steps, ep.num_data, db.graph,
+                                    db.query_entities.contiguous(), cand_idx, cand_count, pp.S, T, pp.node_off,
+                                    pp.node_count, pp.pair_dist, pp.nodes, pp.node_total, ep.status[2:3])
             ops.eval_step_record(ep.cursor, ep.batch_size, ep.steps, st.ids, db.local_entity, pred_dist, cand_idx,
                                  cand_count, a_off, a_ids, seed, words[0], words[1], ep.metrics, ep.cases, ep.counts,
                                  ep.cand_off, ep.cand, ep.cand_total, ep.seeds, ep.status[:3])
@@ -787,7 +817,7 @@ class GraphedStep:
         ent.weights = private                    # the graph formats the weights into these on every replay
         ent.planes = live_plane_buffers()        # as GraphedStep._entry: the operand planes the graph relies on
         ent.draws = _member_draws(member)        # its generator and scratch (and the id in the key) stay alive
-        self._cache[self._eval_key(ep, shape, member)] = ent
+        self._cache[self._eval_key(ep, shape, member, T)] = ent
 
 
 # ---- training ------------------------------------------------------------------------------------------------------
@@ -1205,11 +1235,12 @@ class EvalRun:
     """One evaluation started by :meth:`GraphedStep.start_eval`: device copies of its records, valid once the current
     stream reaches them.  ``seeds``: int64 [steps], the fact-order seed of each step (None without ``shuffle``);
     ``order``: int64 [num_data], the question id of each position.  :meth:`result` and :meth:`records` read the
-    records back; :meth:`info` formats the run's ``.info`` rows on the device; :meth:`check` raises for a nonzero
-    status."""
+    records back; :meth:`info` formats the run's ``.info`` rows on the device; :meth:`paths` reads the shortest-path
+    node sets of a run started with ``path_targets``; :meth:`check` raises for a nonzero status."""
 
-    def __init__(self, blob, cand, seeds, num_data, order):
+    def __init__(self, blob, cand, seeds, num_data, order, paths=None):
         self.blob, self.cand, self.seeds, self.num_data, self.order = blob, cand, seeds, num_data, order
+        self._paths = paths           # (blob, S, T, capacity, seed count of each position) or None
         self._words = None
         self._host = None
 
@@ -1245,6 +1276,20 @@ class EvalRun:
         return m[:, 0].copy(), m[:, 1].copy(), m[:, 2].copy(), m[:, 3].copy(), m[:, 4].copy(), v["cases"].copy(), \
             retrieved
 
+    def paths(self):
+        """-> ``(node_sets, pair_dist)`` of a run started with ``path_targets=T``, one entry per question in batch
+        order: the sorted list of local indices on a shortest path between one of the question's seeds and one of
+        its first ``min(count, T)`` retrieved candidates, as ``evaluate.path_node_sets(db, retrieved, T)`` gives it,
+        and the int32 [n_seeds, n_targets] hop distances of those pairs (-1: unreachable).  Calls :meth:`check`
+        first.  Reads the device once more at most: the node records, after the records :meth:`result` reads."""
+        if self._paths is None:
+            raise ValueError("EvalRun.paths: the evaluation was started without path_targets")
+        counts = self._read()["counts"]
+        self.check()
+        blob, S, T, capacity, seeds = self._paths
+        v = _EvalPaths.views(blob.cpu().numpy(), self.num_data, S, T, capacity)
+        return _EvalPaths.decode(v, np.minimum(seeds, S), np.minimum(counts, T))
+
     def info(self, tables, file=None):
         """The ``.info`` rows of the run, byte for byte what ``evaluate.Evaluator`` writes for these questions with
         ``json.dumps``: one row per question in batch order, formatted on the device from the records
@@ -1278,16 +1323,19 @@ class EvalRun:
     def check(self):
         """Raise ``DeviceSplit.check``'s message when an assembly flagged an id out of range or an overflow, else (for
         GraftNet) ``GraftGraph``'s when the graft staging rejected a list, else ``GraphedStep``'s when a CSR build
-        flagged ids outside the batch, else when the candidate records overflowed (reads the status unless
-        :meth:`result` or :meth:`records` has)."""
+        flagged ids outside the batch, else when the candidate records overflowed, else when the path node records
+        did (reads the status unless :meth:`result` or :meth:`records` has)."""
         words = self._words
         if words is None:
             words = _EvalBuffers.views(self.blob, self.num_data)["status"].tolist()
         asm, csr, records, staging = words
         _raise_epoch_status(asm, csr, staging)
-        if records:
+        if records & 1:
             raise RuntimeError("EvalRun: more ranked candidates than the %d candidate records of the split"
                                % self.cand.shape[0])
+        if records & 2:
+            raise RuntimeError("EvalRun: more shortest-path nodes than the %d node records of the split"
+                               % self._paths[3])
 
 
 class _EvalBuffers(_SplitBuffers):
@@ -1305,8 +1353,9 @@ class _EvalBuffers(_SplitBuffers):
         for name, t in self.views(self.blob, n).items():
             setattr(self, name, t)
         from .loader import candidate_capacity
-        self.cand = torch.zeros(max(candidate_capacity(split.loader.candidate_entities, pad_id), 1), 2,
-                                dtype=torch.int64, device=dev)
+        self.capacity = candidate_capacity(split.loader.candidate_entities, pad_id)
+        self.cand = torch.zeros(max(self.capacity, 1), 2, dtype=torch.int64, device=dev)
+        self.paths = {}               # path targets T -> _EvalPaths
 
     @staticmethod
     def nbytes(n):
@@ -1321,6 +1370,59 @@ class _EvalBuffers(_SplitBuffers):
         if isinstance(blob, torch.Tensor):
             return {k: blob[o:o + b].view(getattr(torch, dt)).view(shape) for k, o, b, shape, dt in layout}
         return {k: blob[o:o + b].view(dt).reshape(shape) for k, o, b, shape, dt in layout}
+
+
+class _EvalPaths:
+    """The shortest-path records of an evaluation with ``path_targets=T`` (gr_eval_step_paths), one byte buffer so that
+    one copy reads them: int64 [num_data] node offsets, the int64 node total, int32 [num_data] node counts, int32
+    [num_data, S, T] pair distances (S: the split's ``max_seeds``) and the int32 [capacity] node records, each
+    question's on-path local indices ascending at its offset."""
+
+    def __init__(self, device, n, S, T, capacity):
+        self.S, self.T, self.capacity = int(S), int(T), int(capacity)
+        self.blob = torch.zeros(self.nbytes(n, S, T, capacity), dtype=torch.uint8, device=device)
+        for name, t in self.views(self.blob, n, S, T, capacity).items():
+            setattr(self, name, t)
+
+    @staticmethod
+    def nbytes(n, S, T, capacity):
+        return 12 * n + 8 + 4 * n * S * T + 4 * capacity
+
+    @staticmethod
+    def views(blob, n, S, T, capacity):
+        """The records of :class:`_EvalPaths` as views of ``blob`` (a torch uint8 tensor or a numpy uint8 array)."""
+        pd = 12 * n + 8
+        layout = (("node_off", 0, 8 * n, (n,), "int64"), ("node_total", 8 * n, 8, (1,), "int64"),
+                  ("node_count", 8 * n + 8, 4 * n, (n,), "int32"), ("pair_dist", pd, 4 * n * S * T, (n, S, T), "int32"),
+                  ("nodes", pd + 4 * n * S * T, 4 * capacity, (capacity,), "int32"))
+        if isinstance(blob, torch.Tensor):
+            return {k: blob[o:o + b].view(getattr(torch, dt)).view(shape) for k, o, b, shape, dt in layout}
+        return {k: blob[o:o + b].view(dt).reshape(shape) for k, o, b, shape, dt in layout}
+
+    @staticmethod
+    def decode(v, n_seeds, n_targets):
+        """Host views ``v`` of the records and the seed / target count of every position -> (node lists, pair
+        distance blocks [n_seeds, n_targets])."""
+        nodes, pair = v["nodes"], v["pair_dist"]
+        sets = [nodes[o:o + c].tolist() for o, c in zip(v["node_off"].tolist(), v["node_count"].tolist())]
+        blocks = [pair[p, :s, :t].copy() for p, (s, t) in enumerate(zip(np.asarray(n_seeds).tolist(),
+                                                                         np.asarray(n_targets).tolist()))]
+        return sets, blocks
+
+
+def paths_refusal(split, batch_size, path_targets):
+    """Why an evaluation of ``split`` in batches of ``batch_size`` refuses ``path_targets`` (a message), or None: a
+    value that is not a positive int, or a BFS workspace (B * (``split.max_seeds()`` + T) * N, B the largest batch)
+    past int32 indexing."""
+    T = path_targets
+    if isinstance(T, bool) or not isinstance(T, (int, np.integer)) or T <= 0:
+        return "path_targets must be a positive int, got %r" % (T,)
+    B = max(min(int(batch_size), int(split.num_data)), 1)
+    cells = B * (split.max_seeds() + int(T)) * int(split.N)
+    if cells > _INT32_MAX:
+        return ("path_targets %d: the BFS workspace of a batch, B * (max_seeds + T) * N = %d * (%d + %d) * %d, "
+                "overflows int32 indexing" % (T, B, split.max_seeds(), T, split.N))
+    return None
 
 
 def _release_autograd_history(model, params):
@@ -1759,13 +1861,19 @@ def _check_members(steps):
 def _job_refusal(member, job, training):
     """Why the sweep refuses ``job`` for ``member`` (a message), or None: what :meth:`GraphedTrainStep.start_epoch`
     (with ``training``) or :meth:`GraphedStep.start_eval` refuses, with their messages, a job that is not their
-    argument tuple, and a training job for a :class:`GraphedStep`.  ``job`` None: the member sits this one out."""
+    argument tuple (an evaluation job of three is one over a ``loader.DeviceSplit``), and a training job for a
+    :class:`GraphedStep`.  ``job`` None: the member sits this one out."""
     if job is None:
         return None
-    name, arity = ("start_epochs", 3) if training else ("start_evals", 2)
-    if not isinstance(job, (tuple, list)) or len(job) != arity:
+    from .loader import DeviceSplit
+    if training:
+        shaped = isinstance(job, (tuple, list)) and len(job) == 3
+    else:                             # (split, batch_size) or (split, batch_size, path_targets) over a DeviceSplit
+        shaped = isinstance(job, (tuple, list)) and (len(job) == 2 or len(job) == 3 and isinstance(job[0], DeviceSplit))
+    if not shaped:
         return "Sweep.%s: a job is %s or None, got %r" % (
-            name, "(split, batch_size, fact_dropout)" if training else "(split, batch_size)", job)
+            "start_epochs" if training else "start_evals",
+            "(split, batch_size, fact_dropout)" if training else "(split, batch_size[, path_targets])", job)
     if training:
         if not isinstance(member.step, GraphedTrainStep):
             return ("Sweep.start_epochs: a GraphedStep member evaluates only; a training member is a "
@@ -1851,8 +1959,8 @@ class Sweep:
         return self._start(jobs, True)
 
     def start_evals(self, jobs):
-        """One evaluation per member with a job ``(split, batch_size)`` -> one :class:`EvalRun` per member (None where
-        the job is None), as :meth:`GraphedStep.start_eval` returns it.  A training member evaluates its model
+        """One evaluation per member with a job ``(split, batch_size)`` or ``(split, batch_size, path_targets)`` -> one
+        :class:`EvalRun` per member (None where the job is None), as :meth:`GraphedStep.start_eval` returns it.  A training member evaluates its model
         through :meth:`eval_step`."""
         return self._start(jobs, False)
 

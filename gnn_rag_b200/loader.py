@@ -278,6 +278,13 @@ def candidate_capacity(candidate_entities, pad_id):
     return int(np.count_nonzero(np.asarray(candidate_entities) != pad_id))
 
 
+def seed_counts(query_entities):
+    """Seeds of each question: its local entities whose ``query_entities`` entry is nonzero in fp32, the table the
+    split uploads (the sources of ``evaluate.path_node_sets``).  int64 [num_q]."""
+    qe = np.asarray(query_entities, dtype=np.float32)
+    return np.count_nonzero(qe != 0, axis=1).astype(np.int64)
+
+
 class DeviceSplit:
     """A split resident in device memory: ``get_batch`` assembles each batch on the GPU from its question ids.
 
@@ -370,6 +377,7 @@ class DeviceSplit:
             del L._gr_flat                                    # flattened here for the upload only
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
         self._answers = None                                  # answer_table(), uploaded by the first evaluation
+        self._seed_counts = None                              # seed_counts(), counted by the first evaluation with paths
 
     def _put(self, name, a, dtype):
         import torch
@@ -435,6 +443,18 @@ class DeviceSplit:
             import torch
             self._answers = tuple(torch.from_numpy(a).to(self.device) for a in pack_answers(self.loader.answer_lists))
         return self._answers
+
+    def seed_counts(self):
+        """:func:`seed_counts` of the loader's ``query_entities``, counted at the first call and kept: int64 [num_q]."""
+        if self._seed_counts is None:
+            self._seed_counts = seed_counts(self.loader.query_entities)
+        return self._seed_counts
+
+    def max_seeds(self):
+        """The largest seed count of any question of the split (0 without questions): the source capacity of the
+        shortest-path node sets of an evaluation (``GraphedStep.start_eval(..., path_targets=T)``)."""
+        c = self.seed_counts()
+        return int(c.max()) if c.size else 0
 
     @property
     def resident_bytes(self):

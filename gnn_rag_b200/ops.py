@@ -1338,6 +1338,37 @@ def eval_step_record(cursor, batch_size, steps, ids, local_entity, pred_dist, ca
             cand.shape[0], _p(cand_total), _p(seeds), _p(eval_status), op="loss_rank")
 
 
+def eval_step_paths(cursor, batch_size, steps, num_data, g, query_entities, cand_idx, cand_count, S, T, node_off,
+                    node_count, pair_dist, nodes, node_total, eval_status):
+    """The shortest-path node sets of a graphed evaluation step (gr_eval_step_paths), before :func:`eval_step_record`
+    moves the cursor: the sources of each question of the step are its local indices with ``query_entities`` (fp32
+    [B, N]) nonzero, ascending, at most ``S``; its targets the first ``min(cand_count, T)`` of ``cand_idx`` (int32
+    [B, N]); the BFS runs over the CsrGraph ``g``.  At the cursor's positions: ``node_off`` (int64 [num_data]),
+    ``node_count`` (int32 [num_data]) and ``pair_dist`` (int32 [num_data, S, T]); the ascending on-path nodes appended
+    to ``nodes`` (int32 [capacity]) at ``node_total`` (int64[1]), or none of the step's with bit 2 of ``eval_status``
+    (int32[1]) set when they do not fit.  See include/gnnrag_b200.h."""
+    for name, t, dt in (("cursor", cursor, torch.int64), ("query_entities", query_entities, torch.float32),
+                        ("cand_idx", cand_idx, torch.int32), ("cand_count", cand_count, torch.int32),
+                        ("node_off", node_off, torch.int64), ("node_count", node_count, torch.int32),
+                        ("pair_dist", pair_dist, torch.int32), ("nodes", nodes, torch.int32),
+                        ("node_total", node_total, torch.int64), ("eval_status", eval_status, torch.int32)):
+        if not t.is_contiguous():
+            raise RuntimeError("eval_step_paths: %s must be contiguous" % name)
+        _cuda(t, dt, name)
+    B, N = query_entities.shape
+    if (cand_idx.shape != (B, N) or cand_count.numel() != B or node_off.numel() != num_data
+            or node_count.numel() != num_data or pair_dist.shape != (num_data, S, T) or node_total.numel() != 1
+            or eval_status.numel() != 1 or (g.B, g.N) != (B, N)):
+        raise RuntimeError("eval_step_paths: need cand_idx [B, N] like query_entities and the graph's B, N, cand_count "
+                           "[B], node_off, node_count [num_data], pair_dist [num_data, S, T], node_total and "
+                           "eval_status [1]")
+    ws, nbytes = _workspace(cursor.device, "gr_eval_paths_workspace_bytes", B, N, int(S), int(T))
+    _launch("gr_eval_step_paths", _p(cursor), int(steps), int(batch_size), B, int(num_data), N, _p(query_entities),
+            _p(cand_idx), _p(cand_count), int(S), int(T), _p(g.rowptr_t), _p(g.src_t), _p(g.rowptr_h), _p(g.src_h),
+            _p(node_off), _p(node_count), _p(pair_dist), _p(nodes), nodes.numel(), _p(node_total), _p(eval_status),
+            _p(ws), nbytes, launches=5, op="paths")
+
+
 def _info_rows_args(name, metrics, cases, counts, cand_off, cand_total, cand, order, tables):
     """The checked record and table arguments of the two ``.info`` row entry points."""
     for arg, t, dt in (("metrics", metrics, torch.float64), ("cases", cases, torch.int8), ("counts", counts, torch.int32),

@@ -870,9 +870,13 @@ int gr_info_rows_write(const double* metrics, const int8_t* cases, const int32_t
 /* ------------------------------------------------------------------------------------------------
  * Shortest-path node sets (SURVEY.md 8f row 1): nodes lying on any shortest path between any seed and
  * any retrieved candidate in the UNDIRECTED subgraph -- build_graph + get_truth_paths,
- * llm/src/utils/graph_utils.py:10-21,49-75.  Uses both CSRs of a question batch; one CTA per question.
- *   sources / targets: float[B*N] indicator arrays (non-zero = member).
- *   on_path: uint8[B*N] output; dist_src: int32[B*N] workspace/output (BFS depth from the sources... see DESIGN.md)
+ * llm/src/utils/graph_utils.py:10-21,49-75.  Uses both CSRs of a question batch.  One CTA per (question, root) runs a
+ * level-synchronous BFS from one of the question's sources or targets; one CTA per question then marks the nodes.
+ *   source_idx int32 [B, max_sources] / target_idx int32 [B, max_targets]: local indices in [0, N), the first
+ *   source_cnt[b] / target_cnt[b] of each row used.  on_path: uint8 [B, N] output, 1 on a shortest path of a connected
+ *   (source, target) pair.  pair_dist: int32 [B, max_sources, max_targets] hop distances, -1 unreachable and past the
+ *   counts.  The workspace keeps the BFS distances int32 [B, max_sources + max_targets, N] (sources first, -1
+ *   unreachable); rows past the counts are not written.
  */
 size_t gr_paths_workspace_bytes(int B, int N, int max_sources, int max_targets);
 int gr_shortest_path_nodes(const int32_t* rowptr_t, const int32_t* src_t,
@@ -881,6 +885,26 @@ int gr_shortest_path_nodes(const int32_t* rowptr_t, const int32_t* src_t,
                            const int32_t* target_idx, const int32_t* target_cnt, int max_targets,
                            uint8_t* on_path, int32_t* pair_dist, int B, int N,
                            void* workspace, size_t workspace_bytes, void* stream);
+
+/* gr_eval_step_paths: the shortest-path node sets of an evaluation epoch step (graphed.GraphedStep.start_eval with
+ * path_targets), after gr_rank_candidates and before gr_eval_step_record, which advances the cursor.  With c = *cursor
+ * in [0, steps), for every j < B whose position p = c * batch_size + j is below num_data: the sources are the local
+ * indices with query_entities[j, v] != 0 in increasing order (the first S of them), the targets the first
+ * min(cand_count[j], T) entries of cand_idx[j] (cand_idx int32 [B, N]); BFS over both CSRs of the step's batch as in
+ * gr_shortest_path_nodes.  Writes pair_dist[p] (int32 [num_data, S, T], -1 unreachable and past the counts),
+ * node_count[p] (int32 [num_data]) = the number of on-path nodes, and node_off[p] (int64 [num_data]): the exclusive
+ * scan of the step's counts in batch order from *node_total.  The nodes of position p, ascending local indices, go
+ * to nodes[node_off[p] ..] (int32 [capacity]) when all of the step's nodes fit below capacity; otherwise the step
+ * writes no node and sets bit 2 of *eval_status.  Then *node_total moves past the step's nodes.  A cursor outside
+ * [0, steps) writes nothing.  No atomics.  Refused: B * (S + T) * N above INT_MAX.  query_entities fp32 [B, N].
+ * Workspace: gr_eval_paths_workspace_bytes(B, N, S, T). */
+size_t gr_eval_paths_workspace_bytes(int B, int64_t N, int S, int T);
+int gr_eval_step_paths(const int64_t* cursor, int64_t steps, int64_t batch_size, int B, int64_t num_data, int64_t N,
+                       const float* query_entities, const int32_t* cand_idx, const int32_t* cand_count, int S, int T,
+                       const int32_t* rowptr_t, const int32_t* src_t, const int32_t* rowptr_h, const int32_t* src_h,
+                       int64_t* node_off, int32_t* node_count, int32_t* pair_dist, int32_t* nodes, int64_t capacity,
+                       int64_t* node_total, int32_t* eval_status, void* workspace, size_t workspace_bytes,
+                       void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Rule-guided reasoning paths (csrc/rule_paths.cu): bfs_with_rule over the undirected graph of build_graph

@@ -97,6 +97,8 @@ struct TcParams {
   const float* bias;
   float* C;                 // fp32 output [M, N] (may be null)
   int64_t ldc;
+  const float* c_rows;      // optional [M]: C receives only the rows m with c_rows[m] != 0 (direct stores), the other
+                            //   rows keep what they held; every other output is written as without it
   __nv_bfloat16* c_hi;      // optional bf16 hi/lo planes of the output (next layer's A operand)
   __nv_bfloat16* c_lo;
   int64_t ldc16;
@@ -250,6 +252,12 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
       if (prev >= 0 && lane == 0) release_slot<CS>(&empty_bar[prev]);
 
       const int64_t row0 = (int64_t)tile * BM + cw * WG_M + r;
+      // C rows r and r + 8 of this thread (all of them without c_rows)
+      bool keep[2] = {true, true};
+      if (p.c_rows) {
+        keep[0] = row0 < p.M && p.c_rows[row0] != 0.f;
+        keep[1] = row0 + 8 < p.M && p.c_rows[row0 + 8] != 0.f;
+      }
       float dot0 = 0.f, dot1 = 0.f;
 #pragma unroll
       for (int q = 0; q < NP / 16; ++q) {
@@ -258,9 +266,10 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
         float v[8];
         epi_values(acc, q, cq, e, v, dot0, dot1);
         if (p.tma_store) {
-          epi_store_tma(v, stg, r, cq, issuer, 1 + cw, &map_c, &map_c_hi, &map_c_lo, p.C != nullptr,
+          // a row-selected C takes the direct stores below: a TMA store writes whole 64-row boxes
+          epi_store_tma(v, stg, r, cq, issuer, 1 + cw, &map_c, &map_c_hi, &map_c_lo, p.C && !p.c_rows,
                         p.c_hi != nullptr, c0, tile * BM + cw * WG_M);
-          continue;
+          if (!p.c_rows) continue;
         }
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
@@ -270,7 +279,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
             const int64_t row = row0 + 8 * hr;
             if (row >= p.M) continue;
             const float x0 = v[4 * b + 2 * hr], x1 = v[4 * b + 2 * hr + 1];
-            if (p.C) {
+            if (p.C && keep[hr]) {
               float* c = p.C + row * p.ldc + col;
               if (vec_c && col + 1 < p.N) {
                 *reinterpret_cast<float2*>(c) = make_float2(x0, x1);
@@ -279,7 +288,7 @@ linear_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
                 if (col + 1 < p.N) c[1] = x1;
               }
             }
-            if (p.c_hi) {
+            if (p.c_hi && !p.tma_store) {
               // the planes also receive the (exactly zero) columns N .. n16
               uint32_t lo;
               const uint32_t hi = split_hi_lo(x0, x1, lo);
@@ -472,39 +481,42 @@ extern "C" int gr_linear_tc(const float* A, int64_t lda, const float* W, int64_t
   return launch_tc(a_hi, a_lo, t.kp, w_hi, w_lo, t.kp, t, p, stream);
 }
 
-extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t lda16, const float* W,
-                                   int64_t ldw, const float* bias, float* C, int64_t ldc, void* C_hi,
-                                   void* C_lo, int64_t ldc16, const float* w_score, float* dots, int64_t M,
-                                   int64_t N, int64_t K, int64_t k_seg, int64_t k_seg_pitch, uint32_t flags,
-                                   void* workspace, size_t workspace_bytes, void* stream_) {
-  using namespace gr;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  GR_CHECK_ARG(A_hi && (A_lo || (flags & GR_LINEAR_BF16_SINGLE)) && W && workspace, "null pointer");
-  GR_CHECK_ARG(C || C_hi, "no output requested");
-  GR_CHECK_ARG(M > 0 && N > 0 && K > 0, "M, N, K must be positive");
+namespace gr {
+namespace {
+
+// gr_linear_tc_planes and gr_linear_tc_planes_rows; errors name the entry point `fn`
+int linear_tc_planes_entry(const char* fn, const void* A_hi, const void* A_lo, int64_t lda16, const float* W,
+                           int64_t ldw, const float* bias, float* C, int64_t ldc, const float* c_rows, void* C_hi,
+                           void* C_lo, int64_t ldc16, const float* w_score, float* dots, int64_t M, int64_t N,
+                           int64_t K, int64_t k_seg, int64_t k_seg_pitch, uint32_t flags, void* workspace,
+                           size_t workspace_bytes, cudaStream_t stream) {
+  GR_CHECK_ARG_AS(fn, A_hi && (A_lo || (flags & GR_LINEAR_BF16_SINGLE)) && W && workspace, "null pointer");
+  GR_CHECK_ARG_AS(fn, C || C_hi, "no output requested");
+  GR_CHECK_ARG_AS(fn, !c_rows || C, "c_rows selects rows of C and needs C");
+  GR_CHECK_ARG_AS(fn, M > 0 && N > 0 && K > 0, "M, N, K must be positive");
   const bool grouped = (flags & GR_LINEAR_K_GROUPED) != 0;
   const bool korder = (flags & GR_LINEAR_K_ORDER_PLANES) != 0;
-  GR_CHECK_ARG(!korder || grouped, "GR_LINEAR_K_ORDER_PLANES modifies GR_LINEAR_K_GROUPED and needs it");
+  GR_CHECK_ARG_AS(fn, !korder || grouped, "GR_LINEAR_K_ORDER_PLANES modifies GR_LINEAR_K_GROUPED and needs it");
   if (grouped) {
-    GR_CHECK_ARG(k_seg > 0 && k_seg_pitch >= k_seg && k_seg_pitch % 16 == 0,
-                 "GR_LINEAR_K_GROUPED needs segmented K: k_seg > 0 and k_seg_pitch >= k_seg, a multiple of 16");
-    GR_CHECK_ARG(K % k_seg_pitch == 0 && (K / k_seg_pitch) % 2 == 1,
-                 "GR_LINEAR_K_GROUPED needs an odd number of segments (2 I + 1)");
-    GR_CHECK_ARG(g_tc_bk != 64, "GR_LINEAR_K_GROUPED needs 32-column k-blocks (tc_bk = 32)");
-    GR_CHECK_ARG(!(flags & GR_LINEAR_BF16_SINGLE), "GR_LINEAR_K_GROUPED does not combine with GR_LINEAR_BF16_SINGLE");
+    GR_CHECK_ARG_AS(fn, k_seg > 0 && k_seg_pitch >= k_seg && k_seg_pitch % 16 == 0,
+                    "GR_LINEAR_K_GROUPED needs segmented K: k_seg > 0 and k_seg_pitch >= k_seg, a multiple of 16");
+    GR_CHECK_ARG_AS(fn, K % k_seg_pitch == 0 && (K / k_seg_pitch) % 2 == 1,
+                    "GR_LINEAR_K_GROUPED needs an odd number of segments (2 I + 1)");
+    GR_CHECK_ARG_AS(fn, g_tc_bk != 64, "GR_LINEAR_K_GROUPED needs 32-column k-blocks (tc_bk = 32)");
+    GR_CHECK_ARG_AS(fn, !(flags & GR_LINEAR_BF16_SINGLE),
+                    "GR_LINEAR_K_GROUPED does not combine with GR_LINEAR_BF16_SINGLE");
   }
   const bool segmented = grouped || (k_seg > 0 && k_seg_pitch > k_seg);
-  GR_CHECK_ARG(lda16 >= K && lda16 % 8 == 0, "lda16 must be >= K and a multiple of 8");
-  GR_CHECK_ARG(!segmented || K % k_seg_pitch == 0, "K must be a multiple of k_seg_pitch");
-  GR_CHECK_ARG(ldw >= (segmented ? K / k_seg_pitch * k_seg : K), "ldw smaller than the weight row length");
-  GR_CHECK_ARG(!C || ldc >= N, "ldc smaller than N");
-  GR_CHECK_ARG(!C_hi || (C_lo && ldc16 >= N), "C_lo missing or ldc16 smaller than N");
-  GR_CHECK_ARG(!dots || w_score, "dots requested without w_score");
-  GR_CHECK_ARG(M < (int64_t)0x7fffffff - BM, "M exceeds int32 range");
+  GR_CHECK_ARG_AS(fn, lda16 >= K && lda16 % 8 == 0, "lda16 must be >= K and a multiple of 8");
+  GR_CHECK_ARG_AS(fn, !segmented || K % k_seg_pitch == 0, "K must be a multiple of k_seg_pitch");
+  GR_CHECK_ARG_AS(fn, ldw >= (segmented ? K / k_seg_pitch * k_seg : K), "ldw smaller than the weight row length");
+  GR_CHECK_ARG_AS(fn, !C || ldc >= N, "ldc smaller than N");
+  GR_CHECK_ARG_AS(fn, !C_hi || (C_lo && ldc16 >= N), "C_lo missing or ldc16 smaller than N");
+  GR_CHECK_ARG_AS(fn, !dots || w_score, "dots requested without w_score");
+  GR_CHECK_ARG_AS(fn, M < (int64_t)0x7fffffff - BM, "M exceeds int32 range");
   TcPlan t = plan_tc(M, N, K, (flags & GR_LINEAR_BF16_SINGLE) != 0);
   if (!t.ok) {
-    set_error("gr_linear_tc_planes: unsupported shape M=%lld N=%lld K=%lld", (long long)M, (long long)N,
-              (long long)K);
+    set_error("%s: unsupported shape M=%lld N=%lld K=%lld", fn, (long long)M, (long long)N, (long long)K);
     return GR_ERR_UNSUPPORTED;
   }
   // grouped order: the W planes gr_fused_layer keeps (same layout, same size: one workspace serves both); over K-order
@@ -512,12 +524,12 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
   const int num_ins = grouped ? (int)(K / k_seg_pitch / 2) : 0;
   const GroupedK gk = grouped ? plan_grouped_k(k_seg_pitch, num_ins, N, korder) : GroupedK{};
   const int64_t nb0 = (k_seg_pitch + 31) / 32 * 32;      // K-order layout: first column of the neighbour region
-  GR_CHECK_ARG(!korder || lda16 >= nb0 + 2 * num_ins * k_seg_pitch,
-               "GR_LINEAR_K_ORDER_PLANES: lda16 must cover the neighbour region (round32(k_seg_pitch) + (K - k_seg_pitch) "
-               "columns)");
+  GR_CHECK_ARG_AS(fn, !korder || lda16 >= nb0 + 2 * num_ins * k_seg_pitch,
+                  "GR_LINEAR_K_ORDER_PLANES: lda16 must cover the neighbour region (round32(k_seg_pitch) + "
+                  "(K - k_seg_pitch) columns)");
   const size_t w_plane_bytes = grouped ? gk.w_plane_bytes : t.w_plane_bytes;
   if (workspace_bytes < 2 * w_plane_bytes || (reinterpret_cast<uintptr_t>(workspace) & 255) != 0) {
-    set_error("gr_linear_tc_planes: workspace too small or not 256-byte aligned");
+    set_error("%s: workspace too small or not 256-byte aligned", fn);
     return GR_ERR_WORKSPACE;
   }
   char* ws = reinterpret_cast<char*>(workspace);
@@ -538,7 +550,7 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
   }
   if (rc != GR_OK) return rc;
   TcParams p{};
-  p.bias = bias; p.C = C; p.ldc = ldc;
+  p.bias = bias; p.C = C; p.ldc = ldc; p.c_rows = c_rows;
   p.c_hi = reinterpret_cast<__nv_bfloat16*>(C_hi); p.c_lo = reinterpret_cast<__nv_bfloat16*>(C_lo);
   p.ldc16 = ldc16; p.w_score = w_score; p.dots = dots;
   p.M = (int)M; p.N = (int)N; p.K = (int)K; p.flags = flags;
@@ -556,4 +568,28 @@ extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t l
   return launch_tc(reinterpret_cast<const __nv_bfloat16*>(A_hi),
                    reinterpret_cast<const __nv_bfloat16*>(A_lo ? A_lo : A_hi), lda16, w_hi, w_lo,
                    grouped ? gk.kp : t.kp, t, p, stream);
+}
+
+}  // namespace
+}  // namespace gr
+
+extern "C" int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t lda16, const float* W,
+                                   int64_t ldw, const float* bias, float* C, int64_t ldc, void* C_hi,
+                                   void* C_lo, int64_t ldc16, const float* w_score, float* dots, int64_t M,
+                                   int64_t N, int64_t K, int64_t k_seg, int64_t k_seg_pitch, uint32_t flags,
+                                   void* workspace, size_t workspace_bytes, void* stream) {
+  return gr::linear_tc_planes_entry(__func__, A_hi, A_lo, lda16, W, ldw, bias, C, ldc, nullptr, C_hi, C_lo, ldc16,
+                                    w_score, dots, M, N, K, k_seg, k_seg_pitch, flags, workspace, workspace_bytes,
+                                    reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int gr_linear_tc_planes_rows(const void* A_hi, const void* A_lo, int64_t lda16, const float* W,
+                                        int64_t ldw, const float* bias, float* C, int64_t ldc, void* C_hi,
+                                        void* C_lo, int64_t ldc16, const float* w_score, float* dots, int64_t M,
+                                        int64_t N, int64_t K, int64_t k_seg, int64_t k_seg_pitch, uint32_t flags,
+                                        void* workspace, size_t workspace_bytes, const float* c_rows,
+                                        void* stream) {
+  return gr::linear_tc_planes_entry(__func__, A_hi, A_lo, lda16, W, ldw, bias, C, ldc, c_rows, C_hi, C_lo, ldc16,
+                                    w_score, dots, M, N, K, k_seg, k_seg_pitch, flags, workspace, workspace_bytes,
+                                    reinterpret_cast<cudaStream_t>(stream));
 }

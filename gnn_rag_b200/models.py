@@ -272,17 +272,24 @@ class ReaRev(BaseModel):
         h = None
         reforms = [getattr(self, "reform" + str(j)).fusion for j in range(I)]
         Wr, Wg = [f.r.weight for f in reforms], [f.g.weight for f in reforms]
-        for _t in range(self.num_iter):                          # rearev.py:206-221
+        seed_rows = db.query_entities.reshape(-1)                # the rows of h the reform reads
+        for t in range(self.num_iter):                           # rearev.py:206-221
+            last_iter = t == self.num_iter - 1
             relation_ins = instructions                          # [B, I, D]
             dist = db.seed_dist                                  # distribution resets to the seed (:208)
             for j in range(self.num_gnn):                        # only the last layer's h feeds the reform
-                # j == 0: the prior is the seed distribution (non-zero on a few nodes) -> sparse-prior path
-                dist, hj = self.reasoning(dist, relation_ins, step=j, need_h=(j == self.num_gnn - 1),
-                                          sparse_prior=(j == 0))
+                last = j == self.num_gnn - 1
+                # j == 0: the prior is the seed distribution (non-zero on a few nodes) -> sparse-prior path.  The last
+                # layer of the last iteration leaves the full fp32 h (layer.h_view) and no planes for a next layer;
+                # the one of an earlier iteration writes fp32 h on the seed rows only
+                dist, hj = self.reasoning(dist, relation_ins, step=j, need_h=last, sparse_prior=(j == 0),
+                                          h_rows=seed_rows if last and not last_iter else None,
+                                          next_layer=not (last and last_iter))
                 h = hj if hj is not None else h
             self.dist_history.append(dist)
-            # all num_ins reforms (seed_retrieve + Fusion) in one launch
-            instructions = ops.query_reform(db.query_entities, h, instructions, Wr, Wg, B, N)
+            if not last_iter:                                    # the last reform's instructions are never read
+                # all num_ins reforms (seed_retrieve + Fusion) in one launch
+                instructions = ops.query_reform(db.query_entities, h, instructions, Wr, Wg, B, N)
         pred_dist = self.dist_history[-1]
         loss, pred = self._loss_and_pred(pred_dist, db.answer_dist)
         return loss, pred, pred_dist, None

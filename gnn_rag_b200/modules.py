@@ -329,17 +329,32 @@ class _GraphLayerBase(nn.Module):
     def cur_planes(self):
         return tuple(self.P[self.cur]) if self.use_planes else None
 
-    def _e2e_and_score(self, e2e, mask, need_h32=True):
+    def _next_planes(self, next_layer):
+        """Output planes of a layer: the next layer's A operand, or None when no layer follows (nothing reads them,
+        and ``cur_planes()`` is stale after such a layer)."""
+        return tuple(self.P[1 - self.cur]) if next_layer else None
+
+    def _h_out(self, need_h, h_rows):
+        """The h a layer returns.  With ``h_rows`` in planes mode it may be ``h32`` written on those rows only
+        (``h32_valid`` False): a seed-row view for the query reform, which reads nothing else.  ``h_view`` never
+        returns such a copy: it rebuilds h from the planes."""
+        if not need_h:
+            return None
+        if h_rows is not None and self.use_planes and not self.h32_valid:
+            return self.h32
+        return self.h_view
+
+    def _e2e_and_score(self, e2e, mask, need_h32=True, next_layer=True):
         """h <- relu(e2e([h, nb...])); dist = softmax(score_func(h) + mask).  ``need_h32``: also write the fp32
-        copy of h (only the instruction update after the last layer of an iteration reads it)."""
+        copy of h (only the instruction update after the last layer of an iteration reads it); ``next_layer``
+        False: no output planes."""
         D = self.entity_dim
         sw, sb = self.score_func.weight.view(-1), self.score_func.bias
         if self.use_planes:
             hi, lo = self.P[self.cur]
-            nhi, nlo = self.P[1 - self.cur]
             ops.linear_tc_planes(hi, lo, self.Kpad, e2e.weight, e2e.bias, out=self.h32 if need_h32 else None,
-                                 out_planes=(nhi, nlo), w_score=sw, dots=self.dots, relu=True, k_seg=D,
-                                 k_seg_pitch=self.Dp, single_ok=True)
+                                 out_planes=self._next_planes(next_layer), w_score=sw, dots=self.dots, relu=True,
+                                 k_seg=D, k_seg_pitch=self.Dp, single_ok=True)
             self.h32_valid = bool(need_h32)
             self.cur = 1 - self.cur
             return ops.masked_softmax(self.dots, sb, mask, self.B, self.N)
@@ -415,10 +430,16 @@ class ReasonGNNLayer(_GraphLayerBase):
         dist = ops.masked_softmax(self.dots, sb, self.local_entity_mask, self.B, self.N)
         return dist, (self.h_view if need_h else None)
 
-    def forward(self, current_dist, relational_ins, step=0, need_h=True, sparse_prior=False):
+    def forward(self, current_dist, relational_ins, step=0, need_h=True, sparse_prior=False, h_rows=None,
+                next_layer=True):
         """One GNN layer (reasongnn.py:134-174): aggregate both directions for every instruction into the
         concat slots, h <- relu(e2e_k([h, nb...])), score, masked softmax.  Returns (dist, h) with h = None when
-        ``need_h`` is False (the caller does not read the embeddings of this layer)."""
+        ``need_h`` is False (the caller does not read the embeddings of this layer).
+        ``h_rows`` (fp32 [B*N], e.g. ``query_entities``): the caller reads only the rows of h with h_rows != 0, and
+        the grouped-order dense layer (:func:`ops.dense_layer`) writes no other row of ``h32`` (:meth:`_h_out`); the
+        other paths write every row.  ``next_layer`` False: no layer runs after this one in the forward, so the
+        dense-prior GEMM writes no operand planes for it; the sparse-prior path writes them all the same."""
+        assert next_layer or (need_h and h_rows is None), "a last layer keeps the full fp32 h"
         D = self.entity_dim
         g = self.graph
         if sparse_prior and self.use_planes and ops.SPARSE_PRIOR_FASTPATH:
@@ -431,12 +452,12 @@ class ReasonGNNLayer(_GraphLayerBase):
             # the dense layer in grouped K order: one fused kernel, or the aggregation kernel + the full-width GEMM
             sw, sb = self.score_func.weight.view(-1), self.score_func.bias
             ops.dense_layer(g, current_dist, pn[0], pn[1], relational_ins, self.cur_planes(), self.Dp, e2e.weight,
-                            e2e.bias, out=self.h32 if need_h else None, out_planes=tuple(self.P[1 - self.cur]),
-                            w_score=sw, dots=self.dots, w_t=wt, w_h=wh)
-            self.h32_valid = bool(need_h)
+                            e2e.bias, out=self.h32 if need_h else None, out_planes=self._next_planes(next_layer),
+                            w_score=sw, dots=self.dots, w_t=wt, w_h=wh, out_rows=h_rows if need_h else None)
+            self.h32_valid = bool(need_h) and h_rows is None
             self.cur = 1 - self.cur
             dist = ops.masked_softmax(self.dots, sb, self.local_entity_mask, self.B, self.N)
-            return dist, (self.h_view if need_h else None)
+            return dist, self._h_out(need_h, h_rows)
         if self.use_planes and pn is not None and ops.AGG_ABS:
             ops.aggregate_dual_abs(g, current_dist, pn[0], pn[1], relational_ins, self.cur_planes(), self.Dp,
                                   self.Dp, wt, wh)
@@ -445,8 +466,8 @@ class ReasonGNNLayer(_GraphLayerBase):
                                planes=self.cur_planes(), seg_pitch=self.Dp)
         else:
             ops.aggregate_dual(g, current_dist, tf, ti, relational_ins, self.X[self.cur], D, wt, wh)
-        dist = self._e2e_and_score(getattr(self, "e2e_linear" + str(step)), self.local_entity_mask, need_h)
-        return dist, (self.h_view if need_h else None)
+        dist = self._e2e_and_score(getattr(self, "e2e_linear" + str(step)), self.local_entity_mask, need_h, next_layer)
+        return dist, self._h_out(need_h, h_rows)
 
 
 class NSMLayer(_GraphLayerBase):

@@ -471,19 +471,20 @@ def fused_layer(g, prior, pn_fwd, pn_inv, ins, h_planes, seg_pitch, W, bias, out
 
 
 def dense_layer(g, prior, pn_fwd, pn_inv, ins, planes, seg_pitch, W, bias, out=None, out_planes=None, w_score=None,
-                dots=None, w_t=None, w_h=None):
+                dots=None, w_t=None, w_h=None, out_rows=None):
     """One dense-prior ReaRev layer in grouped K order: ``relu(e2e([h | nb...]))`` with the score dot.  ``planes`` =
     (hi, lo) layer-input planes [M, >= k_order_nb0(seg_pitch) + 2I * seg_pitch] whose first segment holds h.
     Accumulators of more than 128 columns run as :func:`aggregate_dual_abs` into the K-order neighbour region of
     ``planes`` + :func:`linear_tc_planes` walking it in grouped order, the others as :func:`fused_layer`; the outputs
-    are the same bits either way."""
+    are the same bits either way.  ``out_rows`` (fp32 [M]): only the rows m of ``out`` with out_rows[m] != 0 need be
+    written; the pair writes just those (:func:`linear_tc_planes`), the fused kernel every row."""
     I, n_out = ins.shape[1], W.shape[0]
     if DENSE_WIDE_AS_PAIR and (n_out + 15) // 16 * 16 > 128:
         aggregate_dual_abs(g, prior, pn_fwd, pn_inv, ins, planes, k_order_nb0(seg_pitch), seg_pitch, w_t, w_h,
                            k_order=True)
         return linear_tc_planes(planes[0], planes[1], (2 * I + 1) * seg_pitch, W, bias, out=out, out_planes=out_planes,
                                 w_score=w_score, dots=dots, relu=True, k_seg=ins.shape[2], k_seg_pitch=seg_pitch,
-                                k_grouped=True, k_order=True)
+                                k_grouped=True, k_order=True, **({} if out_rows is None else {"out_rows": out_rows}))
     return fused_layer(g, prior, pn_fwd, pn_inv, ins, planes, seg_pitch, W, bias, out=out, out_planes=out_planes,
                        w_score=w_score, dots=dots, relu=True, w_t=w_t, w_h=w_h)
 
@@ -597,7 +598,7 @@ def live_weight_workspaces():
 
 
 def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=None, dots=None, relu=True,
-                     k_seg=0, k_seg_pitch=0, single_ok=False, k_grouped=False, k_order=False):
+                     k_seg=0, k_seg_pitch=0, single_ok=False, k_grouped=False, k_order=False, out_rows=None):
     """wgmma split-bf16 GEMM whose A operand already lives in bf16 hi/lo planes [M, >=K] (shapes:
     :func:`tc_planes_ok`).
     ``single_ok``: this call may run as ONE bf16 product when ``ACT_BF16`` is on (the node-update GEMMs; the small
@@ -608,6 +609,8 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
     W planes and the cached workspace of :func:`fused_layer`; always the three-product path.
     ``k_order`` (with ``k_grouped``): the neighbour segments lie in the K-order layout of :func:`aggregate_dual_abs`
     (GR_LINEAR_K_ORDER_PLANES): the same k16 steps from aligned boxes, W packed to match under a cache key of its own.
+    ``out_rows``: fp32 [M]; ``out`` then receives only the rows m with out_rows[m] != 0 and keeps its other rows
+    (gr_linear_tc_planes_rows); the other outputs are unchanged by it.
     N > 256 (cfg5: entity_dim 400) is tiled over the output columns: one launch per slice of W rows."""
     N = W.shape[0]
     if N > TC_MAX_N:
@@ -621,7 +624,8 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
                              out=None if out is None else out[:, n0:n1],
                              out_planes=None if out_planes is None else (out_planes[0][:, n0:n1], out_planes[1][:, n0:n1]),
                              w_score=None if w_score is None else w_score[n0:n1], dots=d, relu=relu, k_seg=k_seg,
-                             k_seg_pitch=k_seg_pitch, single_ok=single_ok, k_grouped=k_grouped, k_order=k_order)
+                             k_seg_pitch=k_seg_pitch, single_ok=single_ok, k_grouped=k_grouped, k_order=k_order,
+                             **({} if out_rows is None else {"out_rows": out_rows}))
             if dots is not None and n0 > 0:
                 part = d if part is None else part + d
         if part is not None:
@@ -642,13 +646,17 @@ def linear_tc_planes(a_hi, a_lo, K, W, bias, out=None, out_planes=None, w_score=
         nbytes = _L().gr_linear_tc_planes_workspace_bytes(N, K)
         ws, presplit = _weight_ws(W, N, K, k_seg, k_seg_pitch, nbytes)
     chi, clo = out_planes if out_planes is not None else (None, None)
+    if out_rows is not None:
+        out_rows = _cuda(out_rows, torch.float32, "out_rows")
+        if out is None or not out_rows.is_contiguous() or out_rows.numel() != M:
+            raise ValueError("out_rows must be a contiguous fp32 [M] row predicate of out (M = %d)" % M)
     flags = (LINEAR_RELU if relu else 0) | (LINEAR_W_PRESPLIT if presplit else 0) | \
         (LINEAR_K_GROUPED if k_grouped else LINEAR_BF16_SINGLE if (ACT_BF16 and single_ok) else 0) | \
         (LINEAR_K_ORDER_PLANES if k_order else 0)
-    _launch("gr_linear_tc_planes", _p(a_hi), _p(a_lo), a_hi.stride(0), _p(W), W.stride(0), _p(bias),
+    _launch("gr_linear_tc_planes_rows", _p(a_hi), _p(a_lo), a_hi.stride(0), _p(W), W.stride(0), _p(bias),
             _p(out), out.stride(0) if out is not None else 0,
             _p(chi), _p(clo), chi.stride(0) if chi is not None else 0,
-            _p(w_score), _p(dots), M, N, K, k_seg, k_seg_pitch, flags, _p(ws), nbytes,
+            _p(w_score), _p(dots), M, N, K, k_seg, k_seg_pitch, flags, _p(ws), nbytes, _p(out_rows),
             launches=1 if presplit else 2, op="gemm_tc", info=(M, N, K))
     return out
 

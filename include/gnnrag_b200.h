@@ -145,6 +145,16 @@ int gr_linear_tc_planes(const void* A_hi, const void* A_lo, int64_t lda16, const
                         const float* w_score, float* dots, int64_t M, int64_t N, int64_t K,
                         int64_t k_seg, int64_t k_seg_pitch,
                         uint32_t flags, void* workspace, size_t workspace_bytes, void* stream);
+/* gr_linear_tc_planes with a row predicate on the fp32 output (its arguments, then c_rows): C receives only the rows m with c_rows[m] != 0
+ * (c_rows: float[M], e.g. a question batch's seed weights query_entities [B, N] viewed as [B*N]); the other rows
+ * of C keep what they held.  C_hi / C_lo and dots are written as by gr_linear_tc_planes, bit for bit.  c_rows == NULL
+ * is gr_linear_tc_planes; c_rows without C is refused. */
+int gr_linear_tc_planes_rows(const void* A_hi, const void* A_lo, int64_t lda16, const float* W, int64_t ldw,
+                             const float* bias, float* C, int64_t ldc, void* C_hi, void* C_lo, int64_t ldc16,
+                             const float* w_score, float* dots, int64_t M, int64_t N, int64_t K,
+                             int64_t k_seg, int64_t k_seg_pitch,
+                             uint32_t flags, void* workspace, size_t workspace_bytes, const float* c_rows,
+                             void* stream);
 /* fp32 [M,K] (row stride lda) -> bf16 hi/lo planes (row stride ld_out, multiple of 8). */
 int gr_split_bf16(const float* A, int64_t lda, int64_t M, int64_t K, void* hi, void* lo, int64_t ld_out,
                   void* stream);

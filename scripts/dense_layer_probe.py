@@ -1,5 +1,6 @@
 """Per-layer time of the four ways to run one dense-prior ReaRev layer, alternated in one process:
-     fused          gr_fused_layer (aggregation inside the GEMM kernel)
+     fused          gr_fused_layer (aggregation inside the GEMM kernel), and its mainloop alone: the same launch with
+                    the aggregation warps' work switched off (gr_set_option("fused_debug", 1); results are wrong)
      pair k-order   gr_aggregate_dual_abs_ex (GR_AGG_K_ORDER) + gr_linear_tc_planes in grouped K order over the K-order
                     layout (GR_LINEAR_K_ORDER_PLANES): the fused kernel's bits, what ops.dense_layer runs
      pair grouped   gr_aggregate_dual_abs + gr_linear_tc_planes in grouped K order over the segment layout (same bits)
@@ -81,6 +82,11 @@ def layer_shape(cfg):
     def fused():
         ops.fused_layer(g, prior, pf, pi, ins, cur, P, W, bias, out_planes=nxt, w_score=wsc, dots=dots, relu=True)
 
+    def fused_no_agg():                                        # the mainloop alone: aggregation warps skip their work
+        ops.set_option("fused_debug", 1)
+        fused()
+        ops.set_option("fused_debug", 0)
+
     def agg(k_order=False):
         ops.aggregate_dual_abs(g, prior, pf, pi, ins, cur, ops.k_order_nb0(P) if k_order else P, P, k_order=k_order)
 
@@ -98,10 +104,12 @@ def layer_shape(cfg):
     print("%s layer shape: M = %d rows, D = %d, I = %d, %d in-edges (both directions)" % (cfg, M, D, I, edges))
     for cs in (1, 2):
         ops.set_option("tc_cluster", cs)
-        ts = alternate({"fused": fused, "agg": agg, "agg k-order": lambda: agg(True), "gemm grouped": lambda: gemm(True),
-                        "gemm segment": lambda: gemm(False), "gemm k-order": lambda: gemm(True, True)})
+        ts = alternate({"fused": fused, "fused no agg": fused_no_agg, "agg": agg, "agg k-order": lambda: agg(True),
+                        "gemm grouped": lambda: gemm(True), "gemm segment": lambda: gemm(False),
+                        "gemm k-order": lambda: gemm(True, True)})
         print(" tc_cluster = %d (the GEMMs; the fused kernel always pairs CTAs)" % cs)
         report("fused (gr_fused_layer)", ts["fused"], flop, hbm_fused)
+        report("  fused, aggregation off (fused_debug 1)", ts["fused no agg"], flop, hbm_fused)
         report("pair, K-order layout", [a + b for a, b in zip(ts["agg k-order"], ts["gemm k-order"])], flop, hbm_pair)
         report("pair, grouped K order", [a + b for a, b in zip(ts["agg"], ts["gemm grouped"])], flop, hbm_pair)
         report("pair, segment K order", [a + b for a, b in zip(ts["agg"], ts["gemm segment"])], flop, hbm_pair)

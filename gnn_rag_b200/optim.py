@@ -95,7 +95,8 @@ class ClipAdam:
     model's parameters does); those the optimizer holds are updated, the others only clipped.  ``grads`` are the
     tensors the kernels read and write as ``p.grad``, fixed for the lifetime of the object (a captured backward's
     gradient tensors).  Call :meth:`prepare` before every :meth:`launch` (or replay of a graph that captured it): it
-    advances the CPU ``step`` tensors and uploads that step's scalars.  ``grad_norm`` (device fp32 scalar) holds the
+    advances the CPU ``step`` tensors, uploads that step's scalars and bumps the ``_version`` of every parameter it
+    updates (:meth:`advance` does too, for a whole epoch of replays).  ``grad_norm`` (device fp32 scalar) holds the
     total norm after a launch with ``max_norm``; it is None without."""
 
     def __init__(self, opt, params, grads, max_norm=None):
@@ -123,6 +124,7 @@ class ClipAdam:
                 self._steps.append(st["step"])
             chunks += [(r, k) for k in range((p.numel() + E - 1) // E)]
         self.params = [p for p, _ in rows]
+        self._updated = [self.params[r] for r in self._adam_rows]
         self._wd = _any_weight_decay(opt)
         T, C = len(rows), len(chunks)
         self._table = torch.zeros(T, 6, dtype=torch.int64, device=dev)
@@ -169,7 +171,14 @@ class ClipAdam:
                 row = memo[(gi, t)] = adam_scalars(g["lr"], beta1, beta2, g["eps"], g["weight_decay"], t)
             self._host[r] = row
         self._scalars.copy_(torch.from_numpy(self._host.copy()), non_blocking=True)
+        self._bump_versions()
         self.opt._opt_called = True          # an LR scheduler's check that the optimizer stepped before it
+
+    def _bump_versions(self):
+        """Move the version counter of every parameter this object updates, as an in-place torch op would: the kernels
+        write them through raw pointers, and the weight formats cached per version (``ops._cached``) and the
+        serving graphs keyed on versions (``GraphedStep``) must see the new values."""
+        torch.autograd.graph.increment_version(self._updated)
 
     def _check_groups(self):
         groups = self.opt.param_groups
@@ -207,6 +216,7 @@ class ClipAdam:
         do (the counts are integers, exact in the step tensors' dtype up to 2^24)."""
         if self._steps and steps:
             torch._foreach_add_(self._steps, torch.tensor(float(steps), device="cpu"), alpha=1.0)
+            self._bump_versions()
         self.opt._opt_called = True
 
     def launch(self):

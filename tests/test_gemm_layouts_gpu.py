@@ -25,7 +25,7 @@ import numpy as np
 import pytest
 import torch
 
-from gnn_rag_b200 import batching, modules, ops
+from gnn_rag_b200 import batching, modules, ops, optim
 from gnn_rag_b200 import synthetic as S
 
 import fp64_ref as R
@@ -436,9 +436,10 @@ def test_weight_cache_korder_alternates_with_the_other_layouts():
 
 
 def test_weight_cache_follows_updates():
-    """In-place updates (``mul_`` under no_grad, an optimizer step) are seen by the next call; a per-call weight freed
-    and re-created at the same address gives its new values; a write through ``.data`` is documented not to bump the
-    version, and after clear_weight_cache() the result is right again."""
+    """In-place updates (``mul_`` under no_grad, an optimizer step, the fused clip + Adam step that writes through raw
+    pointers) are seen by the next call; a per-call weight freed and re-created at the same address gives its new
+    values; a write through ``.data`` is documented not to bump the version, and after clear_weight_cache() the result
+    is right again."""
     rs = np.random.RandomState(4)
     M, I, D = 400, 1, 72
     P, T = _r16(D), 2 * I + 1
@@ -465,6 +466,9 @@ def test_weight_cache_follows_updates():
     opt = torch.optim.SGD([W], lr=1.0)
     W.grad = torch.randn_like(W)
     opt.step()
+    worst = max(worst, check(W))
+    W.grad = torch.randn_like(W)
+    optim.ClipAdam(torch.optim.Adam([W], lr=1e-2), [W], [W.grad], max_norm=1.0).step()
     worst = max(worst, check(W))
     ptrs = []
     for k in range(4):

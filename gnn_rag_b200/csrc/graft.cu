@@ -707,7 +707,7 @@ extern "C" int gr_graft_stage(const int64_t* e2f_b, const int64_t* e2f_f, const 
                               const int32_t* live, void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   GR_CHECK_ARG(B > 0 && N > 0 && max_fact >= 0 && R1 > 0 && F_e2f >= 0 && F_f2e >= 0, "bad sizes");
-  GR_CHECK_ARG(nfacts && status && kb_fact_rel, "null pointer");
+  GR_CHECK_ARG(nfacts && status && (max_fact == 0 || kb_fact_rel), "null pointer");   // max_fact == 0: no slots
   GR_CHECK_ARG((int64_t)B * N < 0x7fffffff && (int64_t)B * max_fact < 0x7fffffff, "B*N or B*max_fact exceeds int32");
   GR_CHECK_ARG(F_e2f == 0 || (e2f_b && e2f_f && e2f_e && heads && rels && tails && slot_of), "null pointer");
   GR_CHECK_ARG(F_f2e == 0 || (f2e_b && f2e_e && f2e_f), "null pointer");
@@ -1006,7 +1006,8 @@ extern "C" int gr_graft_attention_backward(const float* qh, const float* qmask, 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   GR_CHECK_ARG(B > 0 && B <= 65535 && D > 0 && D <= 512 && Q > 0 && max_fact >= 0 && R1 > 0 && ldr >= D &&
                    ld_grel >= D, "bad sizes (need 0 < D <= 512, 0 < B <= 65535, Q > 0)");
-  GR_CHECK_ARG(qh && qmask && rel && kb_fact_rel && grad_W && grad_qh && grad_rel, "null pointer");
+  GR_CHECK_ARG(qh && qmask && rel && grad_qh && grad_rel && (max_fact == 0 || (kb_fact_rel && grad_W)),
+               "null pointer");
   if (max_fact == 0) return GR_OK;
   const float div = (float)sqrt((double)D);
   const size_t acc_bytes = (size_t)Q * D * sizeof(float);

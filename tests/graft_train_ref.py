@@ -5,26 +5,15 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from gnn_rag_b200 import autograd_path
+import graft_edges_ref as R
 
-
-def ref_aggregate(self_tab, head_tab, s, st, Nt, mask=None, p=0.0):
-    """sum_out[n] = sum_{f -> n} drop_f(relu(self_tab[r_f] + head_tab[head_f])) * s_f over the staged facts ``st``
-    (heads, tails, rels, slot_of as int64 tensors); ``mask`` [slots, D] is the dropout keep mask."""
-    a = self_tab[st["rels"]] + head_tab[st["heads"]]
-    v = torch.relu(a) * s.unsqueeze(1)
-    if mask is not None:
-        v = v * mask[st["slot_of"]].double() / (1 - p)
-    return torch.zeros(Nt, self_tab.shape[1], dtype=torch.float64).index_add(0, st["tails"], v)
+ref_aggregate = R.train_aggregate
 
 
 def ref_attention(qh, qmask, rel, kfr):
     """W [B, max_fact] of compute_attention (graft_gnn.py:64-87) for every slot, and the softmax a [B, Q, max_fact]."""
-    D = rel.shape[1]
-    fe = rel[torch.as_tensor(kfr)]
-    sim = torch.bmm(qh, fe.transpose(1, 2)) / np.sqrt(D) + (1 - qmask.unsqueeze(2)) * -1e11
-    a = torch.softmax(sim, 1)
-    return (torch.bmm(a.transpose(1, 2), qh) * fe).sum(2) / np.sqrt(D), a
+    at = R.attention(qh, qmask, rel, kfr)
+    return at["W"], at["a"]
 
 
 def graftnet_fp64(m, batch):
@@ -55,22 +44,20 @@ def graftnet_fp64(m, batch):
     enc.encode_question_train(torch.as_tensor(q_input))
     qh, query, qmask = enc.query_hidden_emb.double(), enc.query_node_emb.double(), enc.query_mask_train.double()
     kfr = np.asarray(kfr, dtype=np.int64)
-    slot, head, tail = autograd_path._graft_facts(graft, torch.as_tensor(kfr), B, N, torch.device("cpu"))
+    st = R.stage(graft[0][:3], graft[1][:3], kfr, N)
     W, _a = ref_attention(qh, qmask, rel, kfr)
-    Wt = torch.exp(W - W.max(1, keepdim=True)[0]).reshape(-1)[slot]
-    E = torch.zeros(Nt, dtype=torch.float64).index_add(0, head, Wt).clamp(min=1e-10)
-    st = dict(heads=head, tails=tail, rels=torch.as_tensor(kfr).reshape(-1)[slot], slot_of=slot)
-    indeg = torch.bincount(tail, minlength=Nt).double().unsqueeze(1)
+    Wt = R.w_tilde(W)
+    E = R.e_sum(Wt, st, Nt)[0]
     d = torch.as_tensor(np.asarray(seed_dist, dtype=np.float64)).reshape(-1)
     lam = layer.pagerank_lambda
     pr = []
     for i in range(m.num_layer):
         q2e = L("q2e_linear", i, query).expand(B, N, D).reshape(Nt, D)
-        s = Wt * (d / E)[head]
         kt = layer.lin("kb_tail_linear", i)
-        sum_v = ref_aggregate(L("kb_self_linear", i, rel), L("kb_head_linear", i, h), s, st, Nt)
+        ag = R.aggregate(Wt, E, d, L("kb_self_linear", i, rel), L("kb_head_linear", i, h), st, lam, Nt)
+        sum_v, indeg = ag["sum_out"], ag["indeg"].unsqueeze(1)
         f2e = torch.relu(L("kb_self_linear", i, h) + sum_v @ kt.weight.double().t() + indeg * kt.bias.double())
-        d = lam * torch.zeros(Nt, dtype=torch.float64).index_add(0, tail, s) + (1 - lam) * d
+        d = ag["prior_next"]
         x = torch.cat([h, q2e, layer.fact_scale * f2e], dim=1)
         query = torch.bmm(d.view(B, 1, N), L("e2q_linear", i, x).view(B, N, D))
         h = torch.relu(L("e2e_linear", i, x))
